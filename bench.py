@@ -37,16 +37,16 @@ NQ, TOPK, NPROBES = 10_000, 10, 10
 WORKLOAD = "C1: SIFT-1M-shaped synthetic 1M x 128 f32, IVF_PQ num_partitions=256 num_sub_vectors=16, L2"
 
 # BASELINE.json configs[1..4].  rows = the share ONE GPU holds when the configuration runs as BASELINE.json
-# states it (C3 / C5 "over 8 B200": total / 8; C4 50M x 1536 bf16 = 153.6 GB is also an 8-way shard); every
+# states it (C3 / C5 "over 8 H100": total / 8; C4 50M x 1536 bf16 = 153.6 GB is also an 8-way shard); every
 # rank of a --gpus N run holds one such shard (weak scaling), so --gpus 8 is the configuration at full size.
 CONFIGS = {
-    "C2": dict(desc="C2: synthetic 10M x 768 f32 (OpenAI-ada shape), IVF_PQ 4096/96, L2, single B200",
+    "C2": dict(desc="C2: synthetic 10M x 768 f32 (OpenAI-ada shape), IVF_PQ 4096/96, L2, single H100",
                rows=10_000_000, total=10_000_000, d=768, dtype="f32", kind="pq", K=4096, M=96, metric="l2", ncomp=4096, nprobes=20),
-    "C3": dict(desc="C3: synthetic 100M x 128 f16, IVF_PQ 8192/16, cosine, build sharded over 8 B200 (12.5M rows per GPU)",
+    "C3": dict(desc="C3: synthetic 100M x 128 f16, IVF_PQ 8192/16, cosine, build sharded over 8 H100 (12.5M rows per GPU)",
                rows=12_500_000, total=100_000_000, d=128, dtype="f16", kind="pq", K=8192, M=16, metric="cosine", ncomp=8192, nprobes=20),
     "C4": dict(desc="C4: synthetic 50M x 1536 bf16, IVF_FLAT 4096 partitions (6.25M rows per GPU of 8)",
                rows=6_250_000, total=50_000_000, d=1536, dtype="bf16", kind="flat", K=4096, M=0, metric="l2", ncomp=4096, nprobes=4),
-    "C5": dict(desc="C5: BigANN-style 1B x 128 u8, IVF_PQ 65536/32, 10k-query ADC batches across 8 B200 (125M rows per GPU)",
+    "C5": dict(desc="C5: BigANN-style 1B x 128 u8, IVF_PQ 65536/32, 10k-query ADC batches across 8 H100 (125M rows per GPU)",
                rows=125_000_000, total=1_000_000_000, d=128, dtype="u8", kind="pq", K=65536, M=32, metric="l2", ncomp=65536, nprobes=32),
 }
 
@@ -56,7 +56,7 @@ def peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), float(p.get("bf16_tflops_sustained", p["bf16_tflops"])), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, 1400.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, 989.0, "H100 SXM data sheet (HBM3 GB/s, dense BF16 TFLOP/s at 700 W)"
 
 
 # ------------------------------------------------------------------------------------------------
@@ -307,13 +307,35 @@ KERNEL_BYTES = {
 }
 
 
-def load_ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch from the committed `ncu --set full` summary
-    of the same kernels on the same workload (profiles/ncu_traffic.json, written by profiles/summarize_ncu.py)"""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-    except Exception:
-        return {}
+DUMP_SAMPLE_ROWS = 262144
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, parts, row_base, n):
+    """What the last timed build returned, as .npy files (about 22 MB whatever the row count): the IVF centroids,
+    the PQ codebook and the partition offsets in full, and for a fixed, seeded sample of 262 144 rows each row's
+    partition id and PQ codes.  Rows are addressed by row id, so the files do not depend on the order of rows inside
+    a partition; a sampled row the index does not hold gets partition -1 and codes -1."""
+    off = parts["part_offsets"].astype(np.int64)
+    pos = np.full(n, -1, np.int64)                       # row -> position in the grouped index
+    pos[parts["row_ids"].astype(np.int64) - row_base] = np.arange(len(parts["row_ids"]))
+    part_of_pos = np.repeat(np.arange(len(off) - 1), np.diff(off))
+    sample = np.sort(np.random.default_rng(0).choice(n, min(n, DUMP_SAMPLE_ROWS), replace=False))
+    sp = pos[sample]
+    held = sp >= 0
+    codes = np.full((len(sample), parts["codes"].shape[1]), -1.0, np.float32)
+    codes[held] = parts["codes"][sp[held]]
+    arrays = {"centroids": parts["centroids"].astype(np.float32), "codebook": parts["codebook"].astype(np.float32),
+              "part_offsets": off.astype(np.float64),
+              "sample_rows": sample.astype(np.float64),
+              "sample_partition": np.where(held, part_of_pos[np.maximum(sp, 0)], -1).astype(np.float32),
+              "sample_codes": codes}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_MAX_BYTES:
+        raise SystemExit(f"bench.py: --dump-outputs would write {total} bytes (more than {DUMP_MAX_BYTES})")
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def main():
@@ -326,8 +348,12 @@ def main():
     ap.add_argument("--rows", type=int, default=None, help="rows per GPU (default: the configuration's share)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--only", default="all", choices=["all", "build", "query"],
-                    help="profiling aid (ncu): restrict the run to the resident build or to the query batch")
+                    help="profiling aid: restrict the run to the resident build or to the query batch")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed build returned to DIR/<name>.npy (rank 0; config C1)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.config != "C1" or args.impl != "ours"):
+        ap.error("--dump-outputs is defined for the GPU build of config C1")
     if args.config != "C1":
         if args.steps is None:
             args.steps = 2
@@ -399,14 +425,18 @@ def main():
     lb.launch_count(reset=True)
     t_wall0 = time.time()
     lb.timer_start()
-    stats = None
+    stats = ix = None
     for _ in range(args.steps):
+        if ix is not None:
+            ix.close()
         ix = lb.IvfPqIndex.build(data_dev, "l2", params, row_ids=rid_dev)
         stats = ix.stats
-        ix.close()
     ms_total = lb.timer_stop()
     barrier()
     t_wall1 = time.time()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, ix.export(), row_base, n)
+    ix.close()
     launches = lb.launch_count()
     ms_step = max_over_ranks(ms_total / args.steps)
     clocks = sampler.summary(t_wall0, t_wall1)
@@ -438,7 +468,6 @@ def main():
 
     # ---- kernel breakdown + roofline of the dominant kernel -------------------------------------
     hbm_peak, tensor_peak, peak_src = peaks()
-    traffic = load_ncu_traffic()
     fams = {}
     for fam, (cnt, ms) in sorted(lb.profile.dump().items()):
         fams[fam] = {"launches_per_step": cnt, "ms_per_step": ms, "share": ms / ms_prof}
@@ -447,7 +476,7 @@ def main():
     alg_bytes = KERNEL_BYTES[dom](65536, n)
     achieved = alg_bytes / (per_launch_ms * 1e-3) / 1e9
     roofline = {"kernel": dom, "bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s",
-                "frac": achieved / hbm_peak, "traffic": traffic.get(dom), "peak_source": peak_src,
+                "frac": achieved / hbm_peak, "peak_source": peak_src,
                 "algorithmic_bytes_per_launch": alg_bytes, "avg_launch_ms": per_launch_ms,
                 "note": "dominant kernel of the build step by measured time (CUDA events on the library's stream); "
                         "bytes = SURVEY 8d: the rows' vectors read once (+ ids/codes written for the full pass)"}
@@ -456,8 +485,7 @@ def main():
         pl = fams[fam]["ms_per_step"] / fams[fam]["launches_per_step"]
         ab = KERNEL_BYTES[fam](65536, n)
         roofline_all.append({"kernel": fam, "avg_launch_ms": pl, "algorithmic_bytes_per_launch": ab,
-                             "achieved": ab / (pl * 1e-3) / 1e9, "frac": ab / (pl * 1e-3) / 1e9 / hbm_peak,
-                             "traffic": traffic.get(fam)})
+                             "achieved": ab / (pl * 1e-3) / 1e9, "frac": ab / (pl * 1e-3) / 1e9 / hbm_peak})
 
     if args.only == "build":
         if rank == 0:
@@ -610,7 +638,8 @@ def main():
     # the scan's own ceiling is the shared-memory gather of the lookup tables (the index is L2 resident):
     # one 4-byte LUT read per (row, sub-vector), 32 banks x 4 B per SM and clock
     lookups = NQ * NPROBES * (n / NUM_PARTITIONS) * NUM_SUB_VECTORS
-    smem_peak = 148 * 32 * (clocks["sm_mhz"] or 1965.0) * 1e6       # lookups / s
+    num_sms = torch.cuda.get_device_properties(device).multi_processor_count
+    smem_peak = num_sms * 32 * (clocks["sm_mhz"] or clocks["sm_max_mhz"] or 1980.0) * 1e6       # lookups / s
     scan_launch_ms = scan_ms / max(scan_cnt, 1)
     scan_bytes = NQ * NPROBES * (n / NUM_PARTITIONS) * NUM_SUB_VECTORS + NQ * DIM * 4
     query = {"qps": NQ / (q_ms * 1e-3), "e2e_qps": NQ / (q_e2e_ms * 1e-3), "recall_at_10": recall,
@@ -618,8 +647,7 @@ def main():
              "ms_per_batch": q_ms,
              "roofline": {"kernel": scan_name, "bound": "shared-memory gather (LUT lookups)", "achieved": lookups / (scan_launch_ms * 1e-3) / 1e9,
                           "peak": smem_peak / 1e9, "unit": "Glookup/s", "frac": lookups / (scan_launch_ms * 1e-3) / smem_peak,
-                          "hbm_equivalent_GBps": scan_bytes / (scan_launch_ms * 1e-3) / 1e9, "avg_launch_ms": scan_launch_ms,
-                          "traffic": traffic.get(scan_name)}}
+                          "hbm_equivalent_GBps": scan_bytes / (scan_launch_ms * 1e-3) / 1e9, "avg_launch_ms": scan_launch_ms}}
     sampler.stop()
 
     # ---- CPU baseline (rank 0, N=1 only) ----------------------------------------------------------
@@ -636,7 +664,7 @@ def main():
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": WORKLOAD, "rows_per_gpu": n, "sharding": "row shard per GPU; the k-means loops exchange their packed partial sums once per iteration (one global IVF/PQ model); transform local; search: per-rank lists exchanged + merged in the library",
-                       "cache": "inputs (512 MB) larger than L2 (126 MB)", "k": TOPK, "nprobes": NPROBES},
+                       "cache": "inputs (512 MB) larger than L2 (50 MB)", "k": TOPK, "nprobes": NPROBES},
             "clocks": clocks, "e2e": e2e, "gpu_launches": launches,
             "build_phases_ms": {"ivf_train": stats.ms_ivf_train, "pq_train": stats.ms_pq_train, "transform": stats.ms_transform,
                                 "group": stats.ms_group, "ivf_iters": stats.ivf_iters, "pq_iters_max": stats.pq_iters_max},

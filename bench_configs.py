@@ -139,7 +139,6 @@ def run(args, cfg, B):
             for f, (c, ms) in sorted(lb.profile.dump().items(), key=lambda kv: -kv[1][1])}
     hbm_peak, tensor_peak, peak_src = B.peaks()
     filt = next((f for f in ("transform:tc_filter_general16", "transform:tc_filter_general", "transform:tc_filter") if f in fams), None)
-    traffic = B.load_ncu_traffic().get(f"{args.config}:{filt}") if filt else None
     roofline = None
     if filt:
         flops = 2.0 * n * K * d
@@ -147,9 +146,9 @@ def run(args, cfg, B):
         nl = fams[filt]["launches_per_step"]
         ach = flops / (ms * 1e-3) / 1e12
         roofline = {"kernel": filt, "bound": "tensor", "achieved": ach, "peak": tensor_peak, "unit": "TFLOP/s",
-                    "frac": ach / tensor_peak, "traffic": traffic,
-                    "peak_source": peak_src + " bf16 dense, sustained; " + ("the kernel runs kind::f16 on the native 16-bit rows"
-                                                                            if filt.endswith("16") else "the kernel runs kind::tf32 on f32 rows (half the bf16 rate)"),
+                    "frac": ach / tensor_peak,
+                    "peak_source": peak_src + "; " + ("the kernel runs f16 / bf16 wgmma on the native 16-bit rows"
+                                                      if filt.endswith("16") else "the kernel runs tf32 wgmma on f32 rows (half the bf16 rate)"),
                     "algorithmic_flops_per_launch": flops / nl, "avg_launch_ms": ms / nl, "launches": nl,
                     "hbm_GBps_streaming_x": n * d * esize / (ms * 1e-3) / 1e9}
     top = dict(list(fams.items())[:14])
@@ -272,7 +271,7 @@ def run(args, cfg, B):
             "data": "synthetic",
             "config": {"workload": cfg["desc"], "rows_per_gpu": n, "rows_total": world * n, "config_rows_total": cfg["total"],
                        "d": d, "num_partitions": K, "num_sub_vectors": M, "metric": metric,
-                       "cache": f"inputs ({n * d * esize / 1e9:.1f} GB per GPU) larger than L2 (126 MB)", "k": TOPK, "nprobes": nprobes,
+                       "cache": f"inputs ({n * d * esize / 1e9:.1f} GB per GPU) larger than L2 (50 MB)", "k": TOPK, "nprobes": nprobes,
                        "data_generation_s": t_gen},
             "clocks": clocks, "e2e": e2e, "gpu_launches": launches,
             "build_phases_ms": {"ivf_train": stats.ms_ivf_train, "pq_train": stats.ms_pq_train, "transform": stats.ms_transform,

@@ -1,5 +1,5 @@
 /*
- * lance_b200.h -- C ABI of the B200-native IVF-PQ / IVF-FLAT hot path.
+ * lance_b200.h -- C ABI of the H100-native IVF-PQ / IVF-FLAT hot path.
  *
  * This is the drop-in boundary for lancedb/lance: every entry point replaces one function (or one
  * trait method) of the reference's `lance-index::vector::{kmeans,ivf,pq,flat}` / `lance-linalg`

@@ -1,9 +1,9 @@
-"""lance_b200 -- B200-native IVF-PQ hot path behind lancedb/lance's own operator API.
+"""lance_b200 -- H100-native IVF-PQ hot path behind lancedb/lance's own operator API.
 
 Host-side mirror (Python, test/bench tooling) of the reference's
 `lance-index::vector::{kmeans,ivf,pq,flat}` + `lance-linalg::distance` functions: same names,
 argument meaning and error behaviour; every call goes straight through the C ABI
-(include/lance_b200.h) into hand-written sm_100a kernels.  No CPU fallback exists.
+(include/lance_b200.h) into hand-written sm_90a kernels.  No CPU fallback exists.
 
 Inputs may be numpy arrays (host memory) or `DeviceArray`s (resident in HBM).
 """

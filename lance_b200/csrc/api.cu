@@ -42,7 +42,7 @@ Ctx& ctx() {
     return *g_ctx;
   }
   if (usable_devices() <= 0)
-    fail(LB2_NO_DEVICE, "no CUDA device: lance_b200 has no CPU fallback (needs an sm_100a GPU)");
+    fail(LB2_NO_DEVICE, "no CUDA device: lance_b200 has no CPU fallback (needs an sm_90a GPU)");
   LB2_CUDA(cudaSetDevice(g_requested_device));
   Ctx* c = new Ctx();  // one per (thread, device); lives for the thread's lifetime
   c->device = g_requested_device;
@@ -327,11 +327,10 @@ static void round_model(float* v, size_t count, lb2_dtype dt) {
 // fit the budget), or streamed chunk by chunk through two staging slots during the per-row pass.  f32 views
 // exist for one chunk of rows at a time (zero-copy when the rows already are f32 on the device).
 // What a host-sourced build needs every time, kept per (thread, device) between calls: the copy stream, its
-// event and the device-side landing buffer of the bulk copy.  Measured on a B200 box (tools/e2e_trace.py):
-// re-creating them per build -- above all a fresh 512 MB cudaMallocAsync, which the pool serves by mapping new
-// physical memory whenever its free blocks are fragmented -- cost 0.1 .. 20 ms of HOST time at random before the
-// copy could even start (end-to-end C1 build 20 .. 45 ms per step); with the cache the copy is issued ~0.1 ms
-// after the sample gathers.  Only buffers <= LB2_STAGING_CACHE_MB (default 1024) are retained;
+// event and the device-side landing buffer of the bulk copy.  Re-creating them per build -- above all a fresh
+// 512 MB cudaMallocAsync, which the pool serves by mapping new physical memory whenever its free blocks are
+// fragmented -- costs host time at random before the copy can even start (tools/e2e_trace.py shows it); with
+// the cache the copy is issued right after the sample gathers.  Only buffers <= LB2_STAGING_CACHE_MB (default 1024) are retained;
 // lb2_trim_memory() gives everything back.
 struct StagingCache {
   cudaStream_t copy_stream = nullptr;
@@ -745,7 +744,7 @@ static void index_load_flat_src(lb2_index* ix, const uint32_t* part_ids, Source&
                  (unsigned long long)n, ix->d);
   const int d = ix->d;
   if (!normalize && vdt == src.dtype() && ix->vrow_bytes() % 16 == 0 && (reinterpret_cast<uintptr_t>(nat) & 15) == 0) {
-    // stored type == column type: one pass, no f32 round trip (C4: 2 x 55 GB of bf16 at HBM speed)
+    // stored type == column type: one pass, no f32 round trip (a C4 shard: 2 x 19 GB of bf16 at HBM speed)
     const uint32_t vpr = (uint32_t)(ix->vrow_bytes() / 16);
     LB2_LAUNCH("group_vectors", gather_rows_native_kernel, (unsigned)std::min<uint64_t>(cdiv(kept * vpr, 256), 64ull * ctx().num_sms),
                256, 0, static_cast<const uint4*>(nat), vpr, ms.members.p, kept, reinterpret_cast<uint4*>(ix->vectors.p));
@@ -920,7 +919,7 @@ static void transform_chunk(const float* xf, uint64_t rows, int d, int m, const 
 
 extern "C" {
 
-const char* lb2_version(void) { return "lance_b200 0.1.0 (sm_100a)"; }
+const char* lb2_version(void) { return "lance_b200 0.1.0 (sm_90a)"; }
 
 size_t lb2_last_error(char* buf, size_t len) {
   if (buf && len) {

@@ -87,7 +87,7 @@ struct Ctx {
   std::map<std::string, ProfEntry> prof;
   std::vector<std::pair<std::string, std::pair<cudaEvent_t, cudaEvent_t>>> pending;
   cudaEvent_t t0 = nullptr, t1 = nullptr;
-  int num_sms = 148;
+  int num_sms = 132;
   size_t smem_optin = 0;
   void flush_profile();
 };

@@ -1,11 +1,11 @@
-// tc_assign.cu -- tensor-core FILTER for nearest-centroid assignment (sm_100a: tcgen05 + TMEM + TMA).
+// tc_assign.cu -- tensor-core FILTER for nearest-centroid assignment (sm_90a: wgmma + TMA + mbarrier).
 //
 // Replaces the O(n*K*d) part of  compute_membership_and_dist  (lance-index/src/vector/kmeans.rs:317-369)
 // and  compute_partitions_with_dists (kmeans.rs:1275-1294)  WITHOUT changing a single output bit:
 //
-//   1. tc_filter_kernel: score(x, c) = x.c - (|c|^2 + bias_c)/2 for a 128-row x 256-centroid tile as a
-//      TF32 GEMM (tcgen05.mma kind::tf32, f32 operands straight from TMA-swizzled shared memory,
-//      f32 accumulators in TMEM, double buffered).  The epilogue (tcgen05.ld) keeps the top-3 scores
+//   1. tc_filter_kernel: score(x, c) = x.c - (|c|^2 + bias_c)/2 for a 64-row x 256-centroid tile as a
+//      TF32 GEMM (wgmma.mma_async tf32, f32 operands straight from TMA-swizzled shared memory, f32
+//      accumulators in registers; two consumer warpgroups alternate).  The epilogue keeps the top-3 scores
 //      of every row and classifies the row with a conservative error bound tau:
 //        flag 0: top1 - top2 > tau   -> top1 IS the reference's argmin (no other centroid can win)
 //        flag 1: top1 - top3 > tau   -> the winner is top1 or top2: decide with exact arithmetic
@@ -35,7 +35,7 @@ namespace tc {
 
 struct SmemLayout {
   // offsets from the 1024-aligned base
-  uint32_t b_off, a_off, cnh_off, bar_off, tmem_ptr_off, total;
+  uint32_t b_off, a_off, cnh_off, bar_off, total;
 };
 __host__ __device__ inline SmemLayout smem_layout(int nkc, int stages) {
   SmemLayout L;
@@ -43,9 +43,15 @@ __host__ __device__ inline SmemLayout smem_layout(int nkc, int stages) {
   L.a_off = nkc * B_CHUNK_BYTES;
   L.cnh_off = L.a_off + stages * A_STAGE_BYTES;
   L.bar_off = L.cnh_off + TN * 4;
-  L.tmem_ptr_off = L.bar_off + (2 * MAX_STAGES + 1 + 4) * 8;
-  L.total = L.tmem_ptr_off + 16;
+  L.total = L.bar_off + (2 * MAX_STAGES + 1) * 8;
   return L;
+}
+
+// the classification of a row from its top-3 scores (flag 0: unique, 1: two candidates, 2: undecided)
+__device__ __forceinline__ uint32_t verdict(float m1, float m2, float m3, float tau) {
+  if (m1 - m2 > tau) return 0;
+  if (m1 - m3 > tau) return 1;
+  return 2;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -62,146 +68,105 @@ tc_filter_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
   const SmemLayout L = smem_layout(nkc, stages);
   float* cnh = reinterpret_cast<float*>(smem + L.cnh_off);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem + L.tmem_ptr_off);
   const uint32_t sb = smem_u32(smem);
   auto full_bar = [&](int s) { return smem_u32(&bars[s]); };
   auto empty_bar = [&](int s) { return smem_u32(&bars[MAX_STAGES + s]); };
   const uint32_t b_full = smem_u32(&bars[2 * MAX_STAGES]);
-  auto tfull_bar = [&](int b) { return smem_u32(&bars[2 * MAX_STAGES + 1 + b]); };
-  auto tempty_bar = [&](int b) { return smem_u32(&bars[2 * MAX_STAGES + 3 + b]); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint64_t num_tiles = (n + TM - 1) / TM;
 
   __shared__ float s_cmax2;
   for (int i = threadIdx.x; i < TN; i += NUM_THREADS) cnh[i] = cnh_g[i];
-  if (warp == 3) {  // max_c |c|^2 (the spare warp)
+  if (warp == 3) {  // max_c |c|^2 (a spare producer warp)
     float m = 0.0f;
     for (int i = lane; i < TN; i += 32) m = fmaxf(m, cn2_g[i]);
 #pragma unroll
     for (int off = 16; off >= 1; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
     if (lane == 0) s_cmax2 = m;
   }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 32) {
     for (int s = 0; s < stages; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), 4);  // one arrival per consumer warp
     }
     mbar_init(b_full, 1);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(tfull_bar(b), 1);
-      mbar_init(tempty_bar(b), 4);
-    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_ptr_smem)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===== TMA producer =====
-    if (lane == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
       mbar_expect_tx(b_full, (uint32_t)nkc * B_CHUNK_BYTES);
       for (int kc = 0; kc < nkc; ++kc)
         tma_load_2d(sb + L.b_off + kc * B_CHUNK_BYTES, &map_c, b_full, kc * KC, 0);
       int s = 0;
       uint32_t ph = 0;
-      for (uint64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      for_units_producer(num_tiles, 1, [&](uint64_t tile, int) {
         for (int kc = 0; kc < nkc; ++kc) {
           mbar_wait_relaxed(empty_bar(s), ph ^ 1);
           mbar_expect_tx(full_bar(s), A_STAGE_BYTES);
           tma_load_2d(sb + L.a_off + s * A_STAGE_BYTES, &map_x, full_bar(s), kc * KC, (int)(tile * TM));
           if (++s == stages) { s = 0; ph ^= 1; }
         }
-      }
+      });
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer (one thread) =====
-    if (lane == 0) {
-      mbar_wait(b_full, 0);
-      int s = 0;
-      uint32_t ph = 0;
-      uint32_t it = 0;
-      for (uint64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        const uint32_t buf = it & 1;
-        mbar_wait(tempty_bar(buf), ((it >> 1) & 1) ^ 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t d_tmem = tmem_base + buf * TN;
-        for (int kc = 0; kc < nkc; ++kc) {
-          mbar_wait_relaxed(full_bar(s), ph);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t a_addr = sb + L.a_off + s * A_STAGE_BYTES;
-          const uint32_t b_addr = sb + L.b_off + kc * B_CHUNK_BYTES;
-#pragma unroll
-          for (int k8 = 0; k8 < 4; ++k8)  // 4 x (K = 8 tf32 = 32 bytes) per 128-byte swizzle row
-            umma_tf32(d_tmem, make_desc(a_addr + k8 * 32), make_desc(b_addr + k8 * 32),
-                      (kc | k8) != 0 ? 1u : 0u);
-          umma_commit(empty_bar(s));  // frees the A stage once these MMAs have read it
-          if (++s == stages) { s = 0; ph ^= 1; }
-        }
-        umma_commit(tfull_bar(buf));  // accumulator complete
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue: TMEM -> registers, top-3 per row =====
-    const int q = warp & 3;  // TMEM lane quarter this warp may access
-    const uint32_t group = (warp >> 2) - 1;  // 0 or 1: owns TMEM buffer `group`
+  } else {
+    // ===== consumers: wgmma into registers, top-3 per row =====
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int w = (threadIdx.x >> 7) - 1;
     const float cmax2 = s_cmax2;
-    uint32_t it = 0;
-    for (uint64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const uint32_t buf = it & 1;
-      if (buf != group) continue;
-      mbar_wait(tfull_bar(buf), (it >> 1) & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + buf * TN;
-      float m1 = __int_as_float(0xff800000), m2 = m1, m3 = m1;
-top3_row256(taddr, cnh, m1, m2, m3);
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(tempty_bar(buf));
-      const uint64_t row = tile * TM + q * 32 + lane;
-      if (row < n) {
-        const float tau = tau_scale * (row_norm2[row] + cmax2);
-        uint32_t flag = 2;
-        if (m1 - m2 > tau) flag = 0;
-        else if (m1 - m3 > tau) flag = 1;
-        res[row] = (__float_as_uint(m1) & 0xFFu) | ((__float_as_uint(m2) & 0xFFu) << 12) | (flag << 30);
+    float acc[128];
+    mbar_wait(b_full, 0);
+    for_units_consumer(num_tiles, 1, nkc, w, [&](uint64_t tile, int, uint64_t k, auto pass_turn) {
+      mma_unit<0>(acc, nkc,
+          [&](int kc, uint32_t& a_addr, uint32_t& b_addr) {
+            const uint64_t kk = k + (uint64_t)kc;
+            const int s = (int)(kk % (uint64_t)stages);
+            mbar_wait(full_bar(s), (uint32_t)((kk / (uint64_t)stages) & 1));
+            a_addr = sb + L.a_off + s * A_STAGE_BYTES;
+            b_addr = sb + L.b_off + kc * B_CHUNK_BYTES;
+            return s;
+          },
+          [&](int s) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar(s));
+          });
+      pass_turn();
+      float m[2][3];
+      top3_frag(acc, cnh, m);
+      if ((lane & 3) < 2) {  // lanes 0 / 1 of the quad write rows r0 / r0 + 8
+        const int h = lane & 1;
+        const float m1 = h ? m[1][0] : m[0][0], m2 = h ? m[1][1] : m[0][1], m3 = h ? m[1][2] : m[0][2];
+        const uint64_t row = tile * TM + frag_row(h);
+        if (row < n) {
+          const uint32_t flag = verdict(m1, m2, m3, tau_scale * (row_norm2[row] + cmax2));
+          res[row] = (__float_as_uint(m1) & 0xFFu) | ((__float_as_uint(m2) & 0xFFu) << 12) | (flag << 30);
+        }
       }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
+    });
   }
 }
 
 // ------------------------------------------------------------------------------------------------
 // general shapes: any d % 32 == 0 and any K.  The centroid matrix no longer fits in shared memory,
-// so A (128 rows x 32 floats) AND B (256 centroids x 32 floats) chunks are streamed together through
-// the TMA ring (48 KB per stage), centroid tiles of 256 are visited one after the other with the
-// running top-3 (now with full indices) kept in registers by the epilogue group that owns the row tile.
+// so A (64 rows x 32 floats) AND B (256 centroids x 32 floats) chunks are streamed together through
+// the TMA ring (40 KB per stage), centroid tiles of 256 are visited one after the other with the
+// running top-3 (now with full indices) kept in registers by the warpgroup that owns the row tile.
 // ------------------------------------------------------------------------------------------------
-constexpr int GEN_STAGES = 4;
-constexpr int GEN_STAGE_BYTES = A_STAGE_BYTES + B_CHUNK_BYTES;  // 48 KB
+constexpr int GEN_STAGES = 5;
+constexpr int GEN_STAGE_BYTES = A_STAGE_BYTES + B_CHUNK_BYTES;  // 40 KB
 
 struct GenLayout {
-  uint32_t stage_off, cnh_off, hand_off, bar_off, tmem_ptr_off, total;
+  uint32_t stage_off, bar_off, total;
 };
 __host__ __device__ inline GenLayout gen_layout() {
   GenLayout L;
   L.stage_off = 0;
-  L.cnh_off = GEN_STAGES * GEN_STAGE_BYTES;
-  L.hand_off = L.cnh_off + 2 * TN * 4;
-  L.bar_off = L.hand_off + 2 * 6 * 128 * 4;
-  L.tmem_ptr_off = L.bar_off + (2 * GEN_STAGES + 4) * 8;
-  L.total = L.tmem_ptr_off + 16;
+  L.bar_off = GEN_STAGES * GEN_STAGE_BYTES;
+  L.total = L.bar_off + 2 * GEN_STAGES * 8;
   return L;
 }
 
@@ -240,187 +205,97 @@ tc_filter_general_kernel(const __grid_constant__ CUtensorMap map_x, const __grid
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const GenLayout L = gen_layout();
-  float* cnh_s = reinterpret_cast<float*>(smem + L.cnh_off);  // [2][TN], one slice per epilogue group
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem + L.tmem_ptr_off);
   const uint32_t sb = smem_u32(smem);
   auto full_bar = [&](int s) { return smem_u32(&bars[s]); };
   auto empty_bar = [&](int s) { return smem_u32(&bars[GEN_STAGES + s]); };
-  auto tfull_bar = [&](int b) { return smem_u32(&bars[2 * GEN_STAGES + b]); };
-  auto tempty_bar = [&](int b) { return smem_u32(&bars[2 * GEN_STAGES + 2 + b]); };
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint64_t num_tiles = (n + TM - 1) / TM;
 
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 32) {
     for (int s = 0; s < GEN_STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(tfull_bar(b), 1);
-      mbar_init(tempty_bar(b), 4);
+      mbar_init(empty_bar(s), 4);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_ptr_smem)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr_smem;
 
-  if (warp == 0) {
-    if (lane == 0) {  // ===== TMA producer: A and B chunk of every (row tile, centroid tile, k chunk)
+  if (warp < 4) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x == 0) {  // ===== TMA producer: A and B chunk of every (row tile, centroid tile, k chunk)
       int s = 0;
       uint32_t ph = 0;
-      for (uint64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x)
-        for (int nt = 0; nt < ntiles; ++nt)
-          for (int kc = 0; kc < nkc; ++kc) {
-            mbar_wait_relaxed(empty_bar(s), ph ^ 1);
-            mbar_expect_tx(full_bar(s), GEN_STAGE_BYTES);
-            const uint32_t st = sb + L.stage_off + s * GEN_STAGE_BYTES;
-            tma_load_2d(st, &map_x, full_bar(s), kc * KCE, (int)(tile * TM));
-            tma_load_2d(st + A_STAGE_BYTES, &map_c, full_bar(s), kc * KCE, nt * TN);
-            if (++s == GEN_STAGES) { s = 0; ph ^= 1; }
-          }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {  // ===== MMA issuer
-      int s = 0;
-      uint32_t ph = 0, it = 0;
-      for (uint64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x)
-        for (int nt = 0; nt < ntiles; ++nt, ++it) {
-          const uint32_t buf = it & 1;
-          mbar_wait(tempty_bar(buf), ((it >> 1) & 1) ^ 1);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t d_tmem = tmem_base + buf * TN;
-          for (int kc = 0; kc < nkc; ++kc) {
-            mbar_wait_relaxed(full_bar(s), ph);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint32_t a_addr = sb + L.stage_off + s * GEN_STAGE_BYTES;
-            const uint32_t b_addr = a_addr + A_STAGE_BYTES;
-#pragma unroll
-            for (int k8 = 0; k8 < 4; ++k8)
-              umma_op<OPK>(d_tmem, make_desc(a_addr + k8 * 32), make_desc(b_addr + k8 * 32), (kc | k8) != 0 ? 1u : 0u);
-            umma_commit(empty_bar(s));
-            if (++s == GEN_STAGES) { s = 0; ph ^= 1; }
-          }
-          umma_commit(tfull_bar(buf));
+      for_units_producer(num_tiles, ntiles, [&](uint64_t tile, int nt) {
+        for (int kc = 0; kc < nkc; ++kc) {
+          mbar_wait_relaxed(empty_bar(s), ph ^ 1);
+          mbar_expect_tx(full_bar(s), GEN_STAGE_BYTES);
+          const uint32_t st = sb + L.stage_off + s * GEN_STAGE_BYTES;
+          tma_load_2d(st, &map_x, full_bar(s), kc * KCE, (int)(tile * TM));
+          tma_load_2d(st + A_STAGE_BYTES, &map_c, full_bar(s), kc * KCE, nt * TN);
+          if (++s == GEN_STAGES) { s = 0; ph ^= 1; }
         }
+      });
     }
-  } else if (warp >= 4) {
-    // ===== epilogue: the two groups alternate over the global (row tile, centroid tile) counter so
-    // both stay busy; the group that drains a row tile's LAST centroid tile merges the other group's
-    // partial top-3 (handed over through shared memory) and writes the row's verdict.
-    const int q = warp & 3;
-    const uint32_t group = (warp >> 2) - 1;
-    const int gt = threadIdx.x - 128 - group * 128;  // 0..127 inside the group == row inside the tile
-    float* cn = cnh_s + group * TN;
-    uint32_t* hand = reinterpret_cast<uint32_t*>(smem + L.hand_off);  // [2][6][128]
+  } else {
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int w = (threadIdx.x >> 7) - 1;
     const float cmax2 = *cmax2_ptr;
-    uint32_t mt = 0;
-    if (MODE == 1) {
-      for (uint64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++mt) {
-        const uint32_t it0 = mt * (uint32_t)ntiles;
-        const uint64_t row = tile * TM + q * 32 + lane;
-        const float thr = row < n ? thr_g[row] : __int_as_float(0x7f800000);
-        const uint64_t rc = row < n ? row : 0;
-        for (int nt = 0; nt < ntiles; ++nt) {
-          const uint32_t it = it0 + nt;
-          const uint32_t buf = it & 1;
-          if (buf != group) continue;
-          cn[gt] = cnh_g[(size_t)nt * TN + gt];
-          cn[gt + 128] = cnh_g[(size_t)nt * TN + gt + 128];
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + (int)group) : "memory");
-          mbar_wait(tfull_bar(buf), (it >> 1) & 1);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + buf * TN;
-          cand_row256(taddr, cn, thr, (uint32_t)nt * TN, cand_cnt + rc, cand + rc * CAND_SLOTS);
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(buf));
-          asm volatile("bar.sync %0, 128;" ::"r"(1 + (int)group) : "memory");
+    const float ninf = __int_as_float(0xff800000);
+    float acc[128];
+    float g[2][3];      // running top-3 of the row tile (both fragment rows) over the centroid tiles seen
+    uint32_t gi[2][3];
+    for_units_consumer(num_tiles, ntiles, nkc, w, [&](uint64_t tile, int nt, uint64_t k, auto pass_turn) {
+      mma_unit<OPK>(acc, nkc,
+          [&](int kc, uint32_t& a_addr, uint32_t& b_addr) {
+            const uint64_t kk = k + (uint64_t)kc;
+            const int s = (int)(kk % GEN_STAGES);
+            mbar_wait(full_bar(s), (uint32_t)((kk / GEN_STAGES) & 1));
+            a_addr = sb + L.stage_off + s * GEN_STAGE_BYTES;
+            b_addr = a_addr + A_STAGE_BYTES;
+            return s;
+          },
+          [&](int s) {
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar(s));
+          });
+      pass_turn();
+      const float* cn = cnh_g + (size_t)nt * TN;
+      const uint64_t row0 = tile * TM + frag_row(0), row1 = tile * TM + frag_row(1);
+      if (MODE == 1) {
+        const float thr[2] = {row0 < n ? thr_g[row0] : __int_as_float(0x7f800000),
+                              row1 < n ? thr_g[row1] : __int_as_float(0x7f800000)};
+        const uint64_t rc0 = row0 < n ? row0 : 0, rc1 = row1 < n ? row1 : 0;
+        uint32_t* const cnt[2] = {cand_cnt + rc0, cand_cnt + rc1};
+        uint32_t* const cs[2] = {cand + rc0 * CAND_SLOTS, cand + rc1 * CAND_SLOTS};
+        cand_frag(acc, cn, thr, (uint32_t)nt * TN, cnt, cs);
+        return;
+      }
+      float m[2][3];
+      top3_frag(acc, cn, m);
+      if (nt == 0) {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int j = 0; j < 3; ++j) { g[h][j] = ninf; gi[h][j] = 0; }
+      }
+      const uint32_t base = (uint32_t)nt * TN;
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) top3_insert_idx(m[h][j], base + (__float_as_uint(m[h][j]) & 0xFFu), g[h], gi[h]);
+      if (nt == ntiles - 1 && (lane & 3) < 2) {  // row tile complete: lanes 0 / 1 of the quad write rows r0 / r0 + 8
+        const int h = lane & 1;
+        const uint64_t row = h ? row1 : row0;
+        if (row < n) {
+          const float v0 = h ? g[1][0] : g[0][0], v1 = h ? g[1][1] : g[0][1], v2 = h ? g[1][2] : g[0][2];
+          const uint32_t flag = verdict(v0, v1, v2, tau_scale * (row_norm2[row] + cmax2));
+          res[row] = (h ? gi[1][0] : gi[0][0]) | (flag << 30);
+          res_hi[row] = h ? gi[1][1] : gi[0][1];
+          if (top1_val && flag == 2) top1_val[row] = v0;
         }
       }
-    } else
-    for (uint64_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++mt) {
-      const uint32_t it0 = mt * (uint32_t)ntiles;
-      const float ninf = __int_as_float(0xff800000);
-      float g[3] = {ninf, ninf, ninf};
-      uint32_t gi[3] = {0, 0, 0};
-      float hv[3] = {ninf, ninf, ninf};
-      uint32_t hi[3] = {0, 0, 0};
-      uint32_t* h = hand + (mt & 1) * 6 * 128;
-      const int bar_id = 3 + (int)(mt & 1);
-      for (int nt = 0; nt < ntiles; ++nt) {
-        const uint32_t it = it0 + nt;
-        const uint32_t buf = it & 1;
-        if (buf != group) continue;
-        // this tile's -(|c|^2+bias)/2 slice (the group's own 128 threads, then a group barrier)
-        cn[gt] = cnh_g[(size_t)nt * TN + gt];
-        cn[gt + 128] = cnh_g[(size_t)nt * TN + gt + 128];
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + (int)group) : "memory");
-        mbar_wait(tfull_bar(buf), (it >> 1) & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + buf * TN;
-        float m1 = ninf, m2 = ninf, m3 = ninf;
-        top3_row256(taddr, cn, m1, m2, m3);
-        if (ntiles > 1 && nt == ntiles - 1) {
-          // finisher: take the other group's partial BEFORE releasing this TMEM buffer -- the release is
-          // what lets the pipeline (and with it the other group) run on to the row tile that reuses the
-          // hand-over slot and the named barrier
-          asm volatile("bar.sync %0, 256;" ::"r"(bar_id) : "memory");
-#pragma unroll
-          for (int j = 0; j < 3; ++j) {
-            hv[j] = __uint_as_float(h[j * 128 + gt]);
-            hi[j] = h[(3 + j) * 128 + gt];
-          }
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(tempty_bar(buf));
-        const uint32_t base = (uint32_t)nt * TN;
-        top3_insert_idx(m1, base + (__float_as_uint(m1) & 0xFFu), g, gi);
-        top3_insert_idx(m2, base + (__float_as_uint(m2) & 0xFFu), g, gi);
-        top3_insert_idx(m3, base + (__float_as_uint(m3) & 0xFFu), g, gi);
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + (int)group) : "memory");  // cn is rewritten next tile
-      }
-      const uint32_t fin = (it0 + (uint32_t)ntiles - 1) & 1;
-      if (group != fin) {
-        if (ntiles > 1) {
-#pragma unroll
-          for (int j = 0; j < 3; ++j) {
-            h[j * 128 + gt] = __float_as_uint(g[j]);
-            h[(3 + j) * 128 + gt] = gi[j];
-          }
-          __threadfence_block();
-          asm volatile("bar.arrive %0, 256;" ::"r"(bar_id) : "memory");
-        }
-        continue;
-      }
-      if (ntiles > 1) {
-#pragma unroll
-        for (int j = 0; j < 3; ++j) top3_insert_idx(hv[j], hi[j], g, gi);
-      }
-      const uint64_t row = tile * TM + q * 32 + lane;
-      if (row < n) {
-        const float tau = tau_scale * (row_norm2[row] + cmax2);
-        uint32_t flag = 2;
-        if (g[0] - g[1] > tau) flag = 0;
-        else if (g[0] - g[2] > tau) flag = 1;
-        res[row] = gi[0] | (flag << 30);
-        res_hi[row] = gi[1];
-        if (top1_val && flag == 2) top1_val[row] = g[0];
-      }
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
+    });
   }
 }
 
@@ -587,7 +462,7 @@ rerank_kernel(const float* __restrict__ x, uint64_t n, int d, const float* __res
 }
 
 // ---- refinement of the rows the TF32 filter left undecided ------------------------------------------
-// A second tcgen05 pass over those rows only, with the operands split into TF32-exact pieces
+// A second tensor-core pass over those rows only, with the operands split into TF32-exact pieces
 //     x = xh + xl (+ <= 2^-22 |x|),   c = ch + cl (+ <= 2^-22 |c|),     x.c ~ xh.ch + xh.cl + xl.ch,
 // i.e. the SAME filter kernel run on A' = [xh | xh | xl] (gathered, 3d wide) and B' = [ch | cl | ch]: every
 // product is exact in TF32, what is dropped is <= 1.51 * 2^-22 (|x|^2 + |c|^2), the f32 accumulation over
@@ -932,7 +807,7 @@ bool tc_assign_supported(uint64_t n, int d, int K, int metric, const float* x) {
 // ---- native 16-bit rows ----------------------------------------------------------------------------------------
 // The chunk loops of api.cu announce, next to the f32 view of a chunk, where the same rows lie in their own
 // f16 / bf16 type.  If the model is exactly representable in that type (models trained on such columns are,
-// round_model) the filter passes read the 16-bit rows directly: kind::f16 MMAs at twice the TF32 rate, exact
+// round_model) the filter passes read the 16-bit rows directly: f16 / bf16 wgmma at twice the TF32 rate, exact
 // products, a tau ~10x smaller.  The exact kernels keep reading the f32 view (conversion is exact).
 struct OperandHint {
   const float* f32 = nullptr;

@@ -1,4 +1,4 @@
-// tc_assign.cuh -- internal interface of the tcgen05 filter path (tc_assign.cu)
+// tc_assign.cuh -- internal interface of the tensor-core (wgmma) filter path (tc_assign.cu)
 #pragma once
 #include <stdint.h>
 

@@ -1,6 +1,7 @@
-// tc_common.cuh -- PTX wrappers shared by the tcgen05 kernels (tc_assign.cu, tc_pq.cu):
-// mbarrier, TMA (cp.async.bulk.tensor), UMMA descriptors, tcgen05.mma/commit/ld.
-// Bit layouts follow cute/arch/mma_sm100_desc.hpp (SmemDescriptor, InstrDescriptor).
+// tc_common.cuh -- PTX wrappers shared by the Hopper tensor-core kernels (tc_assign.cu, tc_pq.cu):
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma shared-memory descriptors, wgmma.mma_async, and the
+// reductions of the epilogues over the wgmma accumulator fragment.
+// Descriptor and fragment layouts follow the PTX ISA ("Asynchronous Warpgroup Level Matrix Multiply").
 #pragma once
 #include <cuda.h>
 #include <cudaTypedefs.h>
@@ -12,14 +13,15 @@
 namespace lb2 {
 namespace tc {
 
-constexpr int TM = 128;                  // rows per tile (UMMA M)
-constexpr int TN = 256;                  // centroids per tile (UMMA N)
+constexpr int TM = 64;                   // rows per tile (wgmma M: one consumer warpgroup)
+constexpr int TN = 256;                  // centroids per tile (wgmma N)
 constexpr int KC = 32;                   // f32 per 128-byte swizzle row
-constexpr int A_STAGE_BYTES = TM * 128;  // 16 KB
+constexpr int A_STAGE_BYTES = TM * 128;  // 8 KB
 constexpr int B_CHUNK_BYTES = TN * 128;  // 32 KB
-constexpr int MAX_STAGES = 5;
-constexpr int NUM_THREADS = 384;         // warp0 TMA, warp1 MMA, warp2 TMEM alloc, warps 4-7 / 8-11: two epilogue groups
-                                         // (group g drains TMEM buffer g, so a tcgen05.ld stall of one group is hidden by the other)
+constexpr int MAX_STAGES = 6;
+constexpr int NUM_THREADS = 384;  // warpgroup 0: TMA producer (one thread); warpgroups 1 and 2: consumers taking
+                                  // alternate tiles, so that one warpgroup's epilogue overlaps the other's MMAs
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;  // 128 * 40 + 256 * 232 <= 64 K registers
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
@@ -34,22 +36,9 @@ __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
 // Watchdog: a wait that spins for more than ~4 s of SM clocks is a protocol bug, never a slow kernel.
-// It reports which barrier starved and traps (the launch fails with an error instead of hanging the
-// GPU).  With -DLB2_TC_WATCHDOG_SOFT the first starved wait only raises a flag that makes every
-// later wait fall through, so the kernel ends and the printf buffer reaches the host.
-#ifdef LB2_TC_WATCHDOG_SOFT
-static __device__ int g_wd_abort = 0;
-#endif
-static __device__ __noinline__ void mbar_watchdog_report(uint32_t bar, uint32_t parity) {
-  printf("[lb2 watchdog] block %d thread %d: mbarrier smem+0x%x parity %u starved\n", (int)blockIdx.x,
-         (int)threadIdx.x, bar, parity);
-#ifdef LB2_TC_WATCHDOG_SOFT
-  g_wd_abort = 1;
-  __threadfence();
-#else
-  __trap();
-#endif
-}
+// It traps: the launch fails with an error instead of hanging the GPU.  The path makes no function call
+// (no printf): a call inside the consumer warpgroups would serialize their wgmma pipeline and void their
+// register budget (setmaxnreg).
 __device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -61,32 +50,28 @@ __device__ __forceinline__ bool mbar_try(uint32_t bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// slow path of a wait (kept out of line so the hot loops stay small): called every few thousand failed
-// polls; the first call records the start time, later calls compare against it
-static __device__ __noinline__ bool mbar_watchdog_tick(uint32_t bar, uint32_t parity, long long* t0) {
-#ifdef LB2_TC_WATCHDOG_SOFT
-  if (*(volatile int*)&g_wd_abort) return true;
-#endif
+// slow path of a wait: taken every few thousand failed polls; the first time records the start time, later
+// times compare against it
+__device__ __forceinline__ void mbar_watchdog_tick(long long* t0) {
   const long long now = clock64();
-  if (*t0 == 0) { *t0 = now; return false; }
-  if (now - *t0 > 8000000000ll) { mbar_watchdog_report(bar, parity); return true; }
-  return false;
+  if (*t0 == 0) *t0 = now;
+  else if (now - *t0 > 8000000000ll) __trap();
 }
 __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   long long t0 = 0;
   for (uint32_t spins = 1;; ++spins) {
     if (mbar_try(bar, parity)) return;
-    if ((spins & 0x3FFFu) == 0 && mbar_watchdog_tick(bar, parity, &t0)) return;
+    if ((spins & 0x3FFFu) == 0) mbar_watchdog_tick(&t0);
   }
 }
-// same, for the single-thread producer / issuer roles: back off between polls so that the spin
-// loop does not steal issue slots from the epilogue warps sharing the scheduler
+// same, for the single-thread producer: back off between polls so that the spin loop does not steal
+// issue slots from the consumer warps sharing the scheduler
 __device__ __forceinline__ void mbar_wait_relaxed(uint32_t bar, uint32_t parity) {
   long long t0 = 0;
   for (uint32_t spins = 1;; ++spins) {
     if (mbar_try(bar, parity)) return;
     __nanosleep(40);
-    if ((spins & 0x3FFu) == 0 && mbar_watchdog_tick(bar, parity, &t0)) return;
+    if ((spins & 0x3FFu) == 0) mbar_watchdog_tick(&t0);
   }
 }
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar,
@@ -96,70 +81,99 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
       ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1)
       : "memory");
 }
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp:SmemDescriptor):
-// start>>4 [0,14), LBO>>4 [16,30) (unused for swizzled K-major, 1), SBO>>4 [32,46) = 1024 B (8 rows),
-// version=1 [46,48), layout_type=2 (SWIZZLE_128B) [61,64)
+// K-major, SWIZZLE_128B shared-memory matrix descriptor of wgmma: start>>4 [0,14), LBO>>4 [16,30) (unused for
+// swizzled K-major, 1), SBO>>4 [32,46) = 1024 B (8 rows of 128 B), base offset [49,52) = 0 (every tile starts
+// 1024-aligned), layout type [62,64) = 1 (SWIZZLE_128B).  A K step inside the 128-byte row advances the start.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
+  return (uint64_t)((saddr & 0x3FFFF) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-// instruction descriptor, kind::tf32 (InstrDescriptor): c_format F32=1 [4,6), a/b format TF32=2 [7,10)/[10,13),
-// K-major A and B (bits 15,16 = 0), N>>3 [17,23), M>>4 [24,29)
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
 
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+// ---- wgmma (M64 N256, f32 accumulators in 128 registers per thread) ----------------------------------------
+// d = A (64 x K, shared) * B^T (256 x K, shared) (+ d when scale_d != 0); TF32: K = 8, f16 / bf16: K = 16
+// (32 bytes of a 128-byte swizzled row either way)
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(IDESC), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
-// 16-bit operands (kind::f16): a/b format F16 = 0, BF16 = 1; one instruction covers K = 16 elements (32 B of a
-// 128-byte swizzled row, like K = 8 for TF32), f32 accumulation, twice the TF32 rate
-constexpr uint32_t IDESC_F16 = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-constexpr uint32_t IDESC_BF16 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
+__device__ __forceinline__ void wgmma_f16(float* d, uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_bf16(float* d, uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// ties the accumulator registers to this point: no access to them moves across an asynchronous MMA or its wait
+__device__ __forceinline__ void acc_fence(float* d) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
 // OPK: 0 = f32 operands as TF32, 1 = f16, 2 = bf16
 template <int OPK>
-__device__ __forceinline__ void umma_op(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
-  if (OPK == 0) {
-    umma_tf32(d_tmem, a_desc, b_desc, accumulate);
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(OPK == 1 ? IDESC_F16 : IDESC_BF16), "r"(accumulate)
-        : "memory");
+__device__ __forceinline__ void wgmma_op(float* d, uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  if (OPK == 0) wgmma_tf32(d, a_desc, b_desc, scale_d);
+  else if (OPK == 1) wgmma_f16(d, a_desc, b_desc, scale_d);
+  else wgmma_bf16(d, a_desc, b_desc, scale_d);
+}
+// The MMAs of one unit (a 64-row tile against a 256-centroid tile), chunk by chunk: the four K steps of a 128-byte
+// chunk of A (64 rows) and B (256 rows) are issued as one wgmma group; the unit's first step overwrites d.
+// One group stays in flight: chunk kc is issued before the wait for chunk kc - 1, after which
+// release(stage of kc - 1) hands that stage back to the producer.  stage(kc, a, b) waits for the chunk's operands,
+// sets their shared-memory addresses and returns the stage.  d is final when this returns.
+template <int OPK, class Stage, class Release>
+__device__ __forceinline__ void mma_unit(float* d, int nkc, Stage&& stage, Release&& release) {
+  acc_fence(d);
+  int prev = -1;
+  for (int kc = 0; kc < nkc; ++kc) {
+    uint32_t a_addr, b_addr;
+    const int s = stage(kc, a_addr, b_addr);
+    __syncwarp();  // wgmma is warp-aligned: reconverge after the divergent barrier polls
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      wgmma_op<OPK>(d, make_desc(a_addr + k * 32), make_desc(b_addr + k * 32), (kc != 0 || k != 0) ? 1u : 0u);
+    wgmma_commit();
+    if (prev >= 0) {
+      asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+      release(prev);
+    }
+    prev = s;
   }
+  wgmma_wait_all();
+  acc_fence(d);
+  release(prev);
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
 
-
-// tcgen05.wait::ld that also names the destination registers of the load it completes, so the
-// compiler cannot schedule their consumers above the wait
-__device__ __forceinline__ void tmem_wait_ld(uint32_t* v) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]),
-                 "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15]),
-                 "+r"(v[16]), "+r"(v[17]), "+r"(v[18]), "+r"(v[19]), "+r"(v[20]), "+r"(v[21]), "+r"(v[22]), "+r"(v[23]),
-                 "+r"(v[24]), "+r"(v[25]), "+r"(v[26]), "+r"(v[27]), "+r"(v[28]), "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-               :
-               : "memory");
-}
+// ---- the accumulator fragment ---------------------------------------------------------------------------------
+// Thread t of a warpgroup holds rows r0 = 16 (t / 32) + (t % 32) / 4 and r0 + 8 of the 64-row tile:
+// d[4j + 2h + e] = (row r0 + 8h, column 8j + 2 (t % 4) + e), j < 32.  A row's 256 columns are spread over the
+// four lanes of a quad.
+__device__ __forceinline__ int frag_row(int h) { return 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2) + 8 * h; }
 
 // insert g into the sorted triple (m1 >= m2 >= m3)
 __device__ __forceinline__ void top3_insert(float g, float& m1, float& m2, float& m3) {
@@ -170,117 +184,149 @@ __device__ __forceinline__ void top3_insert(float g, float& m1, float& m2, float
   m3 = fmaxf(m3, t2);
 }
 // ---- top-3 of a 256-column accumulator row by TOURNAMENT ------------------------------------------
-// The epilogue is bound by the half-rate ALU pipe (FMNMX / FMNMX3 / PRMT), so what counts is min/max
-// instructions per column.  Pair the values: the winners (max) go on, and of the losers (min) only the
-// LARGEST can be among the row's top 3 -- a loser is beaten by its own partner, so two losers in the top
-// 3 would need four distinct values ahead of the smaller one.  (All values are distinct: each carries
-// its column index in the low mantissa byte.)  Applying this at every level,
+// The epilogue is bound by min/max instructions per column.  Pair the values: the winners (max) go on, and
+// of the losers (min) only the LARGEST can be among the row's top 3 -- a loser is beaten by its own partner,
+// so two losers in the top 3 would need four distinct values ahead of the smaller one.  (All values are
+// distinct: each carries its column index in the low mantissa byte.)  Applying this at every level,
 //     top3(row) = top3( top3(last-level winners)  U  { largest loser of each level } ),
-// i.e. per level one running FMNMX3 maximum over the losers plus one exact top-3 tracker fed by a single
-// value per 32-column chunk: 83 min/max instructions per chunk instead of 128.
+// i.e. per level one running maximum over the losers plus one exact top-3 tracker fed by a single value per
+// 32-value chunk.
 constexpr int TOUR_LEVELS = 5;
 
-// one 32-column chunk.  C0 is a compile-time constant so that the index OR-ed into the mantissa is an
-// immediate.  T = exact top-3 of the chunk winners so far, L[j] = largest level-j loser so far.
-template <int C0>
-__device__ __forceinline__ void tour_chunk(const uint32_t* v, const float* cn, float* T, float* L) {
-  float g[32];
-#pragma unroll
-  for (int u = 0; u < 32; ++u) {
-    const float f = __uint_as_float(v[u]) + cn[C0 + u];
-    // replace the low mantissa byte by the column index: one PRMT (byte permute) with an immediate
-    g[u] = __uint_as_float(__byte_perm(__float_as_uint(f), (uint32_t)(C0 + u), 0x3214));
-  }
+// one chunk of 32 packed scores g (destroyed).  T = exact top-3 of the chunk winners so far, L[j] = largest
+// level-j loser so far.
+__device__ __forceinline__ void tour_chunk(float* g, float* T, float* L) {
 #pragma unroll
   for (int lvl = 0, cnt = 32; lvl < TOUR_LEVELS; ++lvl, cnt >>= 1) {
-    // cnt values in g[0..cnt) -> cnt/2 winners in g[0..cnt/2), losers folded into L[lvl]
-    float lo[16];
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
       if (i < cnt / 2) {
         const float x = g[2 * i], y = g[2 * i + 1];
         g[i] = fmaxf(x, y);
-        lo[i] = fminf(x, y);
+        L[lvl] = fmaxf(L[lvl], fminf(x, y));
       }
-    }
-    if (cnt / 2 >= 2) {
-#pragma unroll
-      for (int i = 0; i < 16; i += 2)
-        if (i < cnt / 2) L[lvl] = fmaxf(fmaxf(L[lvl], lo[i]), lo[i + 1]);  // -> FMNMX3
-    } else {
-      L[lvl] = fmaxf(L[lvl], lo[0]);
     }
   }
   top3_insert(g[0], T[0], T[1], T[2]);
 }
-
-// top-3 of a 256-column accumulator row; the TMEM loads are software pipelined (the load of chunk
-// c+1 is in flight while chunk c is reduced); fully unrolled over the 8 chunks
-__device__ __forceinline__ void top3_row256(uint32_t taddr, const float* cn, float& m1, float& m2, float& m3) {
-  uint32_t va[32], vb[32];
-  const float ninf = __int_as_float(0xff800000);
-  float T[3] = {ninf, ninf, ninf};
-  float L[TOUR_LEVELS];
-#pragma unroll
-  for (int j = 0; j < TOUR_LEVELS; ++j) L[j] = ninf;
-  tmem_ld32(taddr, va);
-#define LB2_TOP3_STEP(C)                                   \
-  tmem_wait_ld(va);                                        \
-  tmem_ld32(taddr + (C) + 32, vb);                         \
-  tour_chunk<(C)>(va, cn, T, L);                           \
-  tmem_wait_ld(vb);                                        \
-  if ((C) + 64 < TN) tmem_ld32(taddr + (C) + 64, va);      \
-  tour_chunk<(C) + 32>(vb, cn, T, L);
-  LB2_TOP3_STEP(0)
-  LB2_TOP3_STEP(64)
-  LB2_TOP3_STEP(128)
-  LB2_TOP3_STEP(192)
-#undef LB2_TOP3_STEP
-  m1 = T[0]; m2 = T[1]; m3 = T[2];
-#pragma unroll
-  for (int j = 0; j < TOUR_LEVELS; ++j) top3_insert(L[j], m1, m2, m3);
+// score with the column index in the low mantissa byte (one PRMT)
+__device__ __forceinline__ float pack_col(float f, uint32_t col) {
+  return __uint_as_float(__byte_perm(__float_as_uint(f), col, 0x3214));
 }
 
-// ---- candidate pass: every column of a 256-column accumulator row whose score reaches thr -------------------
-// (rows that the top-3 passes could not settle; hits are rare, so the common path is one add + half a 3-input max
-// per column and a single compare per 32-column chunk)
-constexpr int CAND_SLOTS = 16;
-template <int C0>
-__device__ __forceinline__ void cand_chunk(const uint32_t* v, const float* cn, float thr, uint32_t col_base,
-                                           uint32_t* cnt, uint32_t* cand) {
-  float s[32];
+// top-3 of acc + cn[col] for both rows of the thread's fragment; every lane of the quad ends with the row's
+// top-3 of all 256 columns (indices in the low mantissa byte).  cn: 256 floats (shared or global memory).
+__device__ __forceinline__ void top3_frag(const float* acc, const float* cn, float (&m)[2][3]) {
+  const float ninf = __int_as_float(0xff800000);
+  const uint32_t q2 = 2 * (threadIdx.x & 3);
+  float T[2][3], L[2][TOUR_LEVELS];
 #pragma unroll
-  for (int u = 0; u < 32; ++u) s[u] = __uint_as_float(v[u]) + cn[C0 + u];
-  float m = s[0];
+  for (int h = 0; h < 2; ++h) {
+    T[h][0] = T[h][1] = T[h][2] = ninf;
 #pragma unroll
-  for (int u = 1; u < 31; u += 2) m = fmaxf(fmaxf(m, s[u]), s[u + 1]);
-  m = fmaxf(m, s[31]);
-  if (m >= thr) {  // thr = +inf for rows beyond the list; NaN never compares true
+    for (int j = 0; j < TOUR_LEVELS; ++j) L[h][j] = ninf;
+  }
 #pragma unroll
-    for (int u = 0; u < 32; ++u) {
-      if (s[u] >= thr) {
-        const uint32_t slot = atomicAdd(cnt, 1u);
-        if (slot < (uint32_t)CAND_SLOTS) cand[slot] = col_base + (uint32_t)(C0 + u);
+  for (int c = 0; c < 2; ++c) {
+    float g[2][32];
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      const int j = 16 * c + jj;
+      const uint32_t col = 8 * j + q2;
+      const float2 cv = *reinterpret_cast<const float2*>(cn + col);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        g[h][2 * jj] = pack_col(acc[4 * j + 2 * h] + cv.x, col);
+        g[h][2 * jj + 1] = pack_col(acc[4 * j + 2 * h + 1] + cv.y, col + 1);
       }
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) tour_chunk(g[h], T[h], L[h]);
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    m[h][0] = T[h][0]; m[h][1] = T[h][1]; m[h][2] = T[h][2];
+#pragma unroll
+    for (int j = 0; j < TOUR_LEVELS; ++j) top3_insert(L[h][j], m[h][0], m[h][1], m[h][2]);
+#pragma unroll
+    for (int off = 1; off <= 2; off <<= 1) {
+      const float o0 = __shfl_xor_sync(0xffffffffu, m[h][0], off);
+      const float o1 = __shfl_xor_sync(0xffffffffu, m[h][1], off);
+      const float o2 = __shfl_xor_sync(0xffffffffu, m[h][2], off);
+      top3_insert(o0, m[h][0], m[h][1], m[h][2]);
+      top3_insert(o1, m[h][0], m[h][1], m[h][2]);
+      top3_insert(o2, m[h][0], m[h][1], m[h][2]);
     }
   }
 }
-__device__ __forceinline__ void cand_row256(uint32_t taddr, const float* cn, float thr, uint32_t col_base,
-                                            uint32_t* cnt, uint32_t* cand) {
-  uint32_t va[32], vb[32];
-  tmem_ld32(taddr, va);
-#define LB2_CAND_STEP(C)                                   \
-  tmem_wait_ld(va);                                        \
-  tmem_ld32(taddr + (C) + 32, vb);                         \
-  cand_chunk<(C)>(va, cn, thr, col_base, cnt, cand);       \
-  tmem_wait_ld(vb);                                        \
-  if ((C) + 64 < TN) tmem_ld32(taddr + (C) + 64, va);      \
-  cand_chunk<(C) + 32>(vb, cn, thr, col_base, cnt, cand);
-  LB2_CAND_STEP(0)
-  LB2_CAND_STEP(64)
-  LB2_CAND_STEP(128)
-  LB2_CAND_STEP(192)
-#undef LB2_CAND_STEP
+
+// ---- candidate pass: every column of the fragment's rows whose score reaches thr[h] ---------------------------
+// (rows that the top-3 passes could not settle; hits are rare, so the common path is one add and one compare per
+// column; the hits of a row are collected as a bit mask and appended afterwards)
+constexpr int CAND_SLOTS = 16;
+__device__ __forceinline__ void cand_frag(const float* acc, const float* cn, const float (&thr)[2], uint32_t col_base,
+                                          uint32_t* const (&cnt)[2], uint32_t* const (&cand)[2]) {
+  const uint32_t q2 = 2 * (threadIdx.x & 3);
+  uint64_t hit[2] = {0, 0};  // bit 2j + e: column 8j + q2 + e
+#pragma unroll
+  for (int j = 0; j < 32; ++j) {
+    const float2 cv = *reinterpret_cast<const float2*>(cn + 8 * j + q2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {  // thr = +inf for rows beyond the list; NaN never compares true
+      if (acc[4 * j + 2 * h] + cv.x >= thr[h]) hit[h] |= 1ull << (2 * j);
+      if (acc[4 * j + 2 * h + 1] + cv.y >= thr[h]) hit[h] |= 1ull << (2 * j + 1);
+    }
+  }
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    for (uint64_t m = hit[h]; m; m &= m - 1) {
+      const uint32_t b = (uint32_t)(__ffsll((long long)m) - 1);
+      const uint32_t slot = atomicAdd(cnt[h], 1u);
+      if (slot < (uint32_t)CAND_SLOTS) cand[h][slot] = col_base + 8 * (b >> 1) + q2 + (b & 1);
+    }
+  }
+}
+
+// ---- work order of the filter kernels ----------------------------------------------------------------------
+// A unit is one 64-row tile against one 256-centroid tile.  The CTA's row tiles are taken in pairs (one per
+// consumer warpgroup) and, per centroid tile, the two warpgroups take turns: their MMA phases alternate
+// (named barriers 1 and 2), so one warpgroup's epilogue runs while the other's MMAs do.  The turns also keep
+// every stage of the shared TMA ring within one phase of the warpgroup waiting on it: a unit's MMAs start only
+// after every earlier chunk of the ring has been consumed.
+// f(tile, nt) for every unit, in ring order (the producer).
+template <class F>
+__device__ __forceinline__ void for_units_producer(uint64_t num_tiles, int ntiles, F&& f) {
+  for (uint64_t t0 = blockIdx.x; t0 < num_tiles; t0 += 2 * (uint64_t)gridDim.x) {
+    const uint64_t t1 = t0 + gridDim.x;
+    for (int nt = 0; nt < ntiles; ++nt) {
+      f(t0, nt);
+      if (t1 < num_tiles) f(t1, nt);
+    }
+  }
+}
+// f(tile, nt, k, pass_turn) for the units of consumer warpgroup w; k = ring index of the unit's first chunk.
+// The turn is already held when f runs; f passes it on (pass_turn()) once its MMAs are done.
+template <class F>
+__device__ __forceinline__ void for_units_consumer(uint64_t num_tiles, int ntiles, int nkc, int w, F&& f) {
+  uint64_t k = 0;
+  for (uint64_t t0 = blockIdx.x; t0 < num_tiles; t0 += 2 * (uint64_t)gridDim.x) {
+    const uint64_t t1 = t0 + gridDim.x;
+    const bool has1 = t1 < num_tiles;
+    const bool more = t0 + 2 * (uint64_t)gridDim.x < num_tiles;
+    for (int nt = 0; nt < ntiles; ++nt) {
+      for (int o = 0; o < 2; ++o) {
+        if (o == 1 && !has1) continue;
+        if (o == w) {
+          if (o == 1 || (nt > 0 ? has1 : t0 != blockIdx.x)) asm volatile("bar.sync %0, 256;" ::"r"(1 + w) : "memory");
+          const bool pass = o == 0 ? has1 : (nt + 1 < ntiles || more);
+          f(o ? t1 : t0, nt, k, [&] {
+            if (pass) asm volatile("bar.arrive %0, 256;" ::"r"(2 - w) : "memory");
+          });
+        }
+        k += (uint64_t)nkc;
+      }
+    }
+  }
 }
 
 }  // namespace tc

@@ -1,5 +1,5 @@
 // tc_pq.cu -- tensor-core FILTER + in-epilogue exact re-rank for PQ code assignment (8-wide
-// sub-vectors, 256 codewords), sm_100a: tcgen05 kind::tf32 + TMEM + TMA.
+// sub-vectors, 256 codewords), sm_90a: wgmma tf32 + TMA + mbarrier.
 //
 // Replaces the inner loop of  ProductQuantizer::transform_impl  (lance-index/src/vector/pq.rs:116-191:
 // per row, per sub-vector, argmin over the codebook via compute_partition kmeans.rs:1350-1369) and of
@@ -7,9 +7,9 @@
 //
 //   * B operand: the codebook as one K-major matrix Bm[c][m*8+t] = cb[m][c][t] (256 x d f32), resident
 //     in shared memory for the whole kernel (TMA, SWIZZLE_128B).
-//   * A operand: 128-row tiles of the (residual) vectors, TMA-streamed in 32-float chunks (= 4 sub-spaces).
-//   * one tcgen05.mma (M128 N256 K8, tf32) per (tile, sub-space) into a double-buffered TMEM
-//     accumulator; the epilogue keeps the top-3 of  r.c - |c|^2/2  per row and classifies the row
+//   * A operand: 64-row tiles of the (residual) vectors, TMA-streamed in 32-float chunks (= 4 sub-spaces).
+//   * one wgmma (M64 N256 K8, tf32) per (tile, sub-space) into register accumulators, two consumer
+//     warpgroups taking the work items in turns; the epilogue keeps the top-3 of  r.c - |c|^2/2  per row and classifies the row
 //     against tau = 3*2^-10 (|r_m|^2 + max|c_m|^2) exactly like tc_assign.cu;
 //   * flag 0/1 rows are decided IN THE EPILOGUE with reference-order f32 arithmetic on the operands
 //     that are still in shared memory (sequential 8-term sum, l2.rs:69-79; strict-< / lowest index);
@@ -31,10 +31,10 @@ constexpr int STAGES = 4;
 constexpr int MAX_M_RESIDENT = 16;  // d <= 128: the whole codebook matrix stays in shared memory
 constexpr int MAX_M = 256;          // d <= 2048: codebook chunk + its -|c|^2/2 slice streamed per work item
 constexpr int CNH_CHUNK_BYTES = 4 * TN * 4;                                       // 4 sub-spaces
-constexpr int STREAM_STAGE_BYTES = A_STAGE_BYTES + B_CHUNK_BYTES + CNH_CHUNK_BYTES;  // 52 KB
+constexpr int STREAM_STAGE_BYTES = A_STAGE_BYTES + B_CHUNK_BYTES + CNH_CHUNK_BYTES;  // 44 KB
 
-// RESIDENT: [B: nkc x 32 KB][A ring: STAGES x 16 KB][cnh: M x 1 KB]
-// STREAM:   [ring: STAGES x (A 16 KB | B chunk 32 KB | cnh slice 4 KB)]
+// RESIDENT: [B: nkc x 32 KB][A ring: STAGES x 8 KB][cnh: M x 1 KB]
+// STREAM:   [ring: STAGES x (A 8 KB | B chunk 32 KB | cnh slice 4 KB)]
 struct Layout {
   uint32_t b_off, a_off, cnh_off, bar_off, misc_off, total;
   uint32_t stage_bytes;  // distance between two A stages
@@ -54,8 +54,8 @@ __host__ __device__ inline Layout layout(int nkc, int M, bool stream) {
     L.stage_bytes = A_STAGE_BYTES;
     L.bar_off = L.cnh_off + M * TN * 4;
   }
-  L.misc_off = L.bar_off + (2 * STAGES + 1 + 4) * 8;
-  L.total = L.misc_off + 64 + MAX_M;  // tmem pointer, then one "active" byte per sub-space
+  L.misc_off = L.bar_off + (2 * STAGES + 1) * 8;
+  L.total = L.misc_off + MAX_M;  // one "active" byte per sub-space
   return L;
 }
 
@@ -71,6 +71,11 @@ __device__ __forceinline__ const float4* swz(const uint8_t* tile, int r, int u) 
   return reinterpret_cast<const float4*>(tile + (r >> 3) * 1024 + (r & 7) * 128 + ((u ^ (r & 7)) << 4));
 }
 
+// Work items = (64-row tile, 32-float chunk = 4 sub-spaces), finer than whole tiles so that the persistent CTAs
+// (one per SM) stay balanced on short inputs (65 536-row training calls: 1024 tiles).  The two consumer
+// warpgroups take the items with an active sub-space in turns; with an even number of stages every stage
+// always serves the same warpgroup, so a stage is refilled only after its own consumer released it.
+static_assert(STAGES % 2 == 0, "stages alternate between the two consumer warpgroups");
 template <bool TRAIN, bool STREAM>
 __global__ void __launch_bounds__(NUM_THREADS, 1)
 tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_b,
@@ -84,14 +89,11 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
   const int nkc = M / 4;
   const Layout L = layout(nkc, M, STREAM);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
-  uint32_t* tmem_ptr_smem = reinterpret_cast<uint32_t*>(smem + L.misc_off);
-  uint8_t* act_s = smem + L.misc_off + 64;  // [M] 0/1 (M % 4 == 0: read as one word per chunk)
+  uint8_t* act_s = smem + L.misc_off;  // [M] 0/1 (M % 4 == 0: read as one word per chunk)
   const uint32_t sb = smem_u32(smem);
   auto full_bar = [&](int s) { return smem_u32(&bars[s]); };
   auto empty_bar = [&](int s) { return smem_u32(&bars[STAGES + s]); };
   const uint32_t b_full = smem_u32(&bars[2 * STAGES]);
-  auto tfull_bar = [&](int b) { return smem_u32(&bars[2 * STAGES + 1 + b]); };
-  auto tempty_bar = [&](int b) { return smem_u32(&bars[2 * STAGES + 3 + b]); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint64_t num_tiles = (n + TM - 1) / TM;
@@ -106,36 +108,26 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
     act_s[m] = a;
     any_active |= a;
   }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 32) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 9);  // MMA commit + 8 epilogue warps (they re-read the operands)
+      mbar_init(empty_bar(s), 4);  // the 4 warps of the consumer (they re-read the operands after the MMAs)
     }
     mbar_init(b_full, 1);
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(tfull_bar(b), 1);
-      mbar_init(tempty_bar(b), 4);
-    }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 512;" ::"r"(smem_u32(tmem_ptr_smem)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   any_active = __syncthreads_or(any_active);
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_ptr_smem;
+  if (!any_active) return;  // uniform
   // bit j of chunk_mask(kc) = sub-space 4*kc + j still active
   auto chunk_mask = [&](int kc) -> uint32_t {
     const uint32_t w = reinterpret_cast<const uint32_t*>(act_s)[kc];
     return (w | (w >> 7) | (w >> 14) | (w >> 21)) & 0xFu;
   };
-  if (!any_active) goto teardown;  // uniform
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ===== TMA producer =====
-    if (lane == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
       if (!STREAM) {
         mbar_expect_tx(b_full, (uint32_t)nkc * B_CHUNK_BYTES);
         for (int kc = 0; kc < nkc; ++kc)
@@ -143,144 +135,106 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
       }
       int s = 0;
       uint32_t ph = 0;
-      // work item = (row tile, 32-float chunk = 4 sub-spaces): finer than whole tiles so that the
-      // 148 persistent CTAs stay balanced on short inputs (65 536-row training calls: 512 tiles)
       for (uint64_t item = blockIdx.x; item < num_tiles * nkc; item += gridDim.x) {
         const uint64_t tile = item / nkc;
-        {
-          const int kc = (int)(item % nkc);
-          if (chunk_mask(kc) == 0) continue;  // chunk with no active sub-space
-          mbar_wait_relaxed(empty_bar(s), ph ^ 1);
-          mbar_expect_tx(full_bar(s), STREAM ? STREAM_STAGE_BYTES : A_STAGE_BYTES);
-          tma_load_2d(sb + L.a_off + s * L.stage_bytes, &map_r, full_bar(s), kc * KC, (int)(tile * TM));
-          if (STREAM) {
-            tma_load_2d(sb + L.b_off + s * L.stage_bytes, &map_b, full_bar(s), kc * KC, 0);
-            bulk_load_1d(sb + L.cnh_off + s * L.stage_bytes, cnh_g + (size_t)kc * 4 * TN, CNH_CHUNK_BYTES,
-                         full_bar(s));
-          }
-          if (++s == STAGES) { s = 0; ph ^= 1; }
+        const int kc = (int)(item % nkc);
+        if (chunk_mask(kc) == 0) continue;  // chunk with no active sub-space
+        mbar_wait_relaxed(empty_bar(s), ph ^ 1);
+        mbar_expect_tx(full_bar(s), STREAM ? STREAM_STAGE_BYTES : A_STAGE_BYTES);
+        tma_load_2d(sb + L.a_off + s * L.stage_bytes, &map_r, full_bar(s), kc * KC, (int)(tile * TM));
+        if (STREAM) {
+          tma_load_2d(sb + L.b_off + s * L.stage_bytes, &map_b, full_bar(s), kc * KC, 0);
+          bulk_load_1d(sb + L.cnh_off + s * L.stage_bytes, cnh_g + (size_t)kc * 4 * TN, CNH_CHUNK_BYTES,
+                       full_bar(s));
         }
+        if (++s == STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (lane == 0) {
-      if (!STREAM) mbar_wait(b_full, 0);
-      int s = 0;
-      uint32_t ph = 0, it = 0;
-      for (uint64_t item = blockIdx.x; item < num_tiles * nkc; item += gridDim.x) {
-        {
-          const int kc = (int)(item % nkc);
-          const uint32_t cm = chunk_mask(kc);
-          if (cm == 0) continue;
-          mbar_wait_relaxed(full_bar(s), ph);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t a_addr = sb + L.a_off + s * L.stage_bytes;
-          const uint32_t b_addr = sb + L.b_off + (STREAM ? s * L.stage_bytes : kc * B_CHUNK_BYTES);
-          for (int j = 0; j < 4; ++j) {
-            if (!((cm >> j) & 1)) continue;
-            const uint32_t buf = it & 1;
-            mbar_wait(tempty_bar(buf), ((it >> 1) & 1) ^ 1);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            umma_tf32(tmem_base + buf * TN, make_desc(a_addr + j * 32), make_desc(b_addr + j * 32), 0u);
-            umma_commit(tfull_bar(buf));
-            ++it;
-          }
-          umma_commit(empty_bar(s));
-          if (++s == STAGES) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (warp >= 4) {
-    // ===== epilogue =====
-    const int q = warp & 3;
-    const uint32_t group = (warp >> 2) - 1;  // 0 or 1: owns TMEM buffer `group`
-    if (!STREAM) mbar_wait(b_full, 0);  // the codebook tile is re-read by the exact re-rank below
-    int s = 0;
-    uint32_t ph = 0, it = 0;
+  } else {
+    // ===== consumers: one wgmma (K = 8 = one sub-space) per active sub-space, top-3, exact re-rank =====
+    setmaxnreg_inc<CONSUMER_REGS>();
+    const int w = (threadIdx.x >> 7) - 1;
+    if (!STREAM) mbar_wait(b_full, 0);
+    float acc[128];
+    uint32_t k = 0;  // ring index of the items with an active sub-space
     for (uint64_t item = blockIdx.x; item < num_tiles * nkc; item += gridDim.x) {
       const uint64_t tile = item / nkc;
-      const int rl = q * 32 + lane;  // row inside the tile == TMEM lane
-      const uint64_t row = tile * TM + rl;
-      {
-        const int kc = (int)(item % nkc);
-        const uint32_t cm = chunk_mask(kc);
-        if (cm == 0) continue;
-        mbar_wait(full_bar(s), ph);  // operands visible to this thread (re-read below)
-        const uint8_t* atile = smem + L.a_off + s * L.stage_bytes;
-        const uint8_t* bt = smem + L.b_off + (STREAM ? s * L.stage_bytes : kc * B_CHUNK_BYTES);
-        const float* cn4 = reinterpret_cast<const float*>(smem + L.cnh_off + (STREAM ? s * L.stage_bytes : kc * CNH_CHUNK_BYTES));
-        for (int j = 0; j < 4; ++j) {
-          if (!((cm >> j) & 1)) continue;
-          const int m = kc * 4 + j;
-          const uint32_t buf = it & 1;
-          if (buf != group) { ++it; continue; }
-          mbar_wait(tfull_bar(buf), (it >> 1) & 1);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + buf * TN;
-          const float* cn = cn4 + j * TN;
-          float m1 = __int_as_float(0xff800000), m2 = m1, m3 = m1;
-top3_row256(taddr, cn, m1, m2, m3);
-          asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(buf));
-          ++it;
-          if (row < n) {
-            const float tau = 0.0029296875f * (rn2[row * M + m] + cbmax2[m]);
-            uint32_t flag = 2;
-            if (m1 - m2 > tau) flag = 0;
-            else if (m1 - m3 > tau) flag = 1;
-            const uint32_t i1 = __float_as_uint(m1) & 0xFFu, i2 = __float_as_uint(m2) & 0xFFu;
-            uint32_t best_idx = i1;
-            float best_val = 0.0f;
-            bool ok = true;
-            if (flag == 2) {
-              fb_pairs[(size_t)m * n + atomicAdd(fb_count + m, 1u)] = (uint32_t)row;  // per-sub-space list
-            } else if (TRAIN || flag == 1) {
-              // exact, reference-order distance(s) from the operands still in shared memory
-              const float4 r0 = *swz(atile, rl, j * 2), r1 = *swz(atile, rl, j * 2 + 1);
-              const float rv[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-              float bv = __int_as_float(0x7f800000);
-              uint32_t bi = 0xffffffffu;
-              const int ncand = flag == 0 ? 1 : 2;
-              for (int c = 0; c < ncand; ++c) {
-                const uint32_t ci = c == 0 ? i1 : i2;
-                const float4 c0v = *swz(bt, (int)ci, j * 2), c1v = *swz(bt, (int)ci, j * 2 + 1);
-                const float cv[8] = {c0v.x, c0v.y, c0v.z, c0v.w, c1v.x, c1v.y, c1v.z, c1v.w};
-                float sacc = 0.0f;
-#pragma unroll
-                for (int t = 0; t < 8; ++t) sacc = f_add(sacc, sq_diff(rv[t], cv[t]));
-                const float vv = f_add(sacc, 0.0f);
-                if (vv < bv || (vv == bv && ci < bi)) { bv = vv; bi = ci; }
-              }
-              ok = bi != 0xffffffffu;
-              best_idx = ok ? bi : 0u;
-              best_val = bv;
+      const int kc = (int)(item % nkc);
+      const uint32_t cm = chunk_mask(kc);
+      if (cm == 0) continue;
+      const uint32_t mine = (k & 1) == (uint32_t)w;
+      const int s = (int)(k % STAGES);
+      const uint32_t ph = (k / STAGES) & 1;
+      ++k;
+      if (!mine) continue;
+      mbar_wait(full_bar(s), ph);
+      const uint8_t* atile = smem + L.a_off + s * L.stage_bytes;
+      const uint8_t* bt = smem + L.b_off + (STREAM ? s * L.stage_bytes : kc * B_CHUNK_BYTES);
+      const float* cn4 = reinterpret_cast<const float*>(smem + L.cnh_off + (STREAM ? s * L.stage_bytes : kc * CNH_CHUNK_BYTES));
+      const uint32_t a_addr = smem_u32(atile), b_addr = smem_u32(bt);
+      for (int j = 0; j < 4; ++j) {
+        if (!((cm >> j) & 1)) continue;
+        const int m = kc * 4 + j;
+        __syncwarp();
+        acc_fence(acc);
+        wgmma_fence();
+        wgmma_tf32(acc, make_desc(a_addr + j * 32), make_desc(b_addr + j * 32), 0u);
+        wgmma_commit();
+        wgmma_wait_all();
+        acc_fence(acc);
+        float mm[2][3];
+        top3_frag(acc, cn4 + j * TN, mm);
+        const int h = lane & 1;      // lanes 0 / 1 of the quad finish rows r0 / r0 + 8
+        const int rl = frag_row(h);  // row inside the tile
+        const uint64_t row = tile * TM + rl;
+        if ((lane & 3) < 2 && row < n) {
+          const float m1 = h ? mm[1][0] : mm[0][0], m2 = h ? mm[1][1] : mm[0][1], m3 = h ? mm[1][2] : mm[0][2];
+          const float tau = 0.0029296875f * (rn2[row * M + m] + cbmax2[m]);
+          uint32_t flag = 2;
+          if (m1 - m2 > tau) flag = 0;
+          else if (m1 - m3 > tau) flag = 1;
+          const uint32_t i1 = __float_as_uint(m1) & 0xFFu, i2 = __float_as_uint(m2) & 0xFFu;
+          uint32_t best_idx = i1;
+          float best_val = 0.0f;
+          bool ok = true;
+          if (flag == 2) {
+            fb_pairs[(size_t)m * n + atomicAdd(fb_count + m, 1u)] = (uint32_t)row;  // per-sub-space list
+          } else if (TRAIN || flag == 1) {
+            // exact, reference-order distance(s) from the operands still in shared memory
+            const float4 r0 = *swz(atile, rl, j * 2), r1 = *swz(atile, rl, j * 2 + 1);
+            const float rv[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+            float bv = __int_as_float(0x7f800000);
+            uint32_t bi = 0xffffffffu;
+            const int ncand = flag == 0 ? 1 : 2;
+            for (int c = 0; c < ncand; ++c) {
+              const uint32_t ci = c == 0 ? i1 : i2;
+              const float4 c0v = *swz(bt, (int)ci, j * 2), c1v = *swz(bt, (int)ci, j * 2 + 1);
+              const float cv[8] = {c0v.x, c0v.y, c0v.z, c0v.w, c1v.x, c1v.y, c1v.z, c1v.w};
+              float sacc = 0.0f;
+  #pragma unroll
+              for (int t = 0; t < 8; ++t) sacc = f_add(sacc, sq_diff(rv[t], cv[t]));
+              const float vv = f_add(sacc, 0.0f);
+              if (vv < bv || (vv == bv && ci < bi)) { bv = vv; bi = ci; }
             }
-            if (flag != 2) {
-              if (TRAIN) {
-                ids[(uint64_t)m * n + row] = best_idx;
-                dists[(uint64_t)m * n + row] = ok ? best_val : __int_as_float(0x7fc00000);
-                valid[(uint64_t)m * n + row] = ok ? 1 : 0;
-              } else {
-                const bool rv_ok = row_valid ? row_valid[row] != 0 : true;
-                codes[row * (uint64_t)M + m] = (ok && rv_ok) ? (uint8_t)best_idx : (uint8_t)0;
-              }
+            ok = bi != 0xffffffffu;
+            best_idx = ok ? bi : 0u;
+            best_val = bv;
+          }
+          if (flag != 2) {
+            if (TRAIN) {
+              ids[(uint64_t)m * n + row] = best_idx;
+              dists[(uint64_t)m * n + row] = ok ? best_val : __int_as_float(0x7fc00000);
+              valid[(uint64_t)m * n + row] = ok ? 1 : 0;
+            } else {
+              const bool rv_ok = row_valid ? row_valid[row] != 0 : true;
+              codes[row * (uint64_t)M + m] = (ok && rv_ok) ? (uint8_t)best_idx : (uint8_t)0;
             }
           }
         }
         __syncwarp();
-        if (lane == 0) mbar_arrive(empty_bar(s));  // this warp is done re-reading the stage
-        if (++s == STAGES) { s = 0; ph ^= 1; }
       }
+      if (lane == 0) mbar_arrive(empty_bar(s));  // this warp is done with the stage
     }
-  }
-teardown:
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 2) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 512;" ::"r"(tmem_base) : "memory");
   }
 }
 

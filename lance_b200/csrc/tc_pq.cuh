@@ -1,4 +1,4 @@
-// tc_pq.cuh -- internal interface of the tcgen05 PQ code-assignment path (tc_pq.cu)
+// tc_pq.cuh -- internal interface of the tensor-core (wgmma) PQ code-assignment path (tc_pq.cu)
 #pragma once
 #include <stdint.h>
 

@@ -28,7 +28,7 @@ def test_library_exports_every_declared_symbol():
 
 
 def test_version_and_error_buffer():
-    assert b"sm_100a" in _lib.lib().lb2_version()
+    assert b"sm_90a" in _lib.lib().lb2_version()
 
 
 def test_product_never_imports_oracle():

@@ -5,7 +5,7 @@ index packed into the low mantissa byte, top-3 per row, and a row is *unique* wh
 when top1 - top3 > tau, else *undecided* -- with tau = tau_scale (|x|^2 + max|c|^2).  The claim the bit-exactness of
 the whole build rests on: for a unique row the reference's argmin (exact f32 arithmetic in reference order, strict `<`,
 lowest index; lance-linalg/src/kernels.rs:79-111 over l2.rs:57-91) IS top1's column, for a two-candidate row it is one
-of top1 / top2.  The GPU tests check that end to end on a B200; this file checks the ARGUMENT on the CPU, against the
+of top1 / top2.  The GPU tests check that end to end on an H100; this file checks the ARGUMENT on the CPU, against the
 oracle, under every rounding behaviour the hardware could have inside the error budget the kernels assume:
 
   * operands cut to TF32 by truncation or by round-to-nearest-even,

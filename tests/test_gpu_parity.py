@@ -14,7 +14,7 @@ NT = 16
 
 
 def test_device_present_and_native_library_loaded():
-    assert lb.device_count() >= 1, "no GPU: -m gpu tests must run on a B200"
+    assert lb.device_count() >= 1, "no GPU: -m gpu tests must run on an H100"
     lb.set_device(0)
     assert lb.launch_count(reset=True) >= 0
 
@@ -504,7 +504,7 @@ def test_concurrent_host_threads_share_an_index():
         assert all(np.array_equal(a, b) for a, b in zip(p1, p2))
 
 
-# ---- tensor-core filter path (tcgen05) must be bit-identical to the exact path -----------------
+# ---- tensor-core filter path (wgmma) must be bit-identical to the exact path -----------------
 def _both_paths(fn):
     import os
     os.environ.pop("LB2_DISABLE_TC", None)
@@ -614,7 +614,7 @@ def test_tc_candidate_pass_matches_oracle(n, d, k, monkeypatch):
 @pytest.mark.parametrize("n,d,k", [(5000, 128, 512), (3000, 1536, 304)])
 def test_native_16bit_operands_match_oracle(dtype, n, d, k, monkeypatch):
     # f16 / bf16 rows (the model has the same element type, so it is exact in it): the tensor-core passes read the
-    # native rows (kind::f16 MMAs).  Results must equal the oracle on the converted values -- with and without the
+    # native rows (f16 / bf16 wgmma).  Results must equal the oracle on the converted values -- with and without the
     # candidate pass -- and the f32-staged path (LB2_NO_NATIVE16).
     rng = np.random.default_rng(n + d + len(dtype))
     if dtype == "f16":

@@ -1,6 +1,6 @@
 """Numeric model (numpy + the oracle, no GPU) of the NEXT first-pass variant proposed in DESIGN.md section 8 (v):
 integer-valued columns (SIFT, u8: exactly representable in f16) against f32 centroids split into two f16 terms,
-c = ch + cl + r with |r| <= 2^-22 |c|, as ONE kind::f16 GEMM over the operands A' = [x | x], B' = [ch | cl]: every
+c = ch + cl + r with |r| <= 2^-22 |c|, as ONE f16 GEMM over the operands A' = [x | x], B' = [ch | cl]: every
 product is exact, what is lost is r, the f32 accumulation and the index byte.  Prints, for SIFT-shaped data, the share
 of rows each certificate decides (unique + two-candidate) and checks that the certified rows are right.
 usage: python tools/f16_split_model.py [rows] [K]"""
