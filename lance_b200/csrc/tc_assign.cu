@@ -64,7 +64,7 @@ tc_filter_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
                  uint32_t* __restrict__ res, const uint8_t* __restrict__ active, float tau_scale) {
   if (active && !active[0]) return;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   const SmemLayout L = smem_layout(nkc, stages);
   float* cnh = reinterpret_cast<float*>(smem + L.cnh_off);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
@@ -135,15 +135,13 @@ tc_filter_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
             if (lane == 0) mbar_arrive(empty_bar(s));
           });
       pass_turn();
-      float m[2][3];
+      float m[3];
       top3_frag(acc, cnh, m);
       if ((lane & 3) < 2) {  // lanes 0 / 1 of the quad write rows r0 / r0 + 8
-        const int h = lane & 1;
-        const float m1 = h ? m[1][0] : m[0][0], m2 = h ? m[1][1] : m[0][1], m3 = h ? m[1][2] : m[0][2];
-        const uint64_t row = tile * TM + frag_row(h);
+        const uint64_t row = tile * TM + frag_row(lane & 1);
         if (row < n) {
-          const uint32_t flag = verdict(m1, m2, m3, tau_scale * (row_norm2[row] + cmax2));
-          res[row] = (__float_as_uint(m1) & 0xFFu) | ((__float_as_uint(m2) & 0xFFu) << 12) | (flag << 30);
+          const uint32_t flag = verdict(m[0], m[1], m[2], tau_scale * (row_norm2[row] + cmax2));
+          res[row] = (__float_as_uint(m[0]) & 0xFFu) | ((__float_as_uint(m[1]) & 0xFFu) << 12) | (flag << 30);
         }
       }
     });
@@ -203,7 +201,7 @@ tc_filter_general_kernel(const __grid_constant__ CUtensorMap map_x, const __grid
   if (n_dev) n = min(*n_dev, n_cap);  // refinement pass: the row count lives on the device
   if (n == 0) return;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   const GenLayout L = gen_layout();
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
   const uint32_t sb = smem_u32(smem);
@@ -243,8 +241,8 @@ tc_filter_general_kernel(const __grid_constant__ CUtensorMap map_x, const __grid
     const float cmax2 = *cmax2_ptr;
     const float ninf = __int_as_float(0xff800000);
     float acc[128];
-    float g[2][3];      // running top-3 of the row tile (both fragment rows) over the centroid tiles seen
-    uint32_t gi[2][3];
+    float g[3];      // running top-3 of the lane's fragment row over the centroid tiles seen
+    uint32_t gi[3];
     for_units_consumer(num_tiles, ntiles, nkc, w, [&](uint64_t tile, int nt, uint64_t k, auto pass_turn) {
       mma_unit<OPK>(acc, nkc,
           [&](int kc, uint32_t& a_addr, uint32_t& b_addr) {
@@ -271,28 +269,22 @@ tc_filter_general_kernel(const __grid_constant__ CUtensorMap map_x, const __grid
         cand_frag(acc, cn, thr, (uint32_t)nt * TN, cnt, cs);
         return;
       }
-      float m[2][3];
+      float m[3];
       top3_frag(acc, cn, m);
       if (nt == 0) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int j = 0; j < 3; ++j) { g[h][j] = ninf; gi[h][j] = 0; }
+        for (int j = 0; j < 3; ++j) { g[j] = ninf; gi[j] = 0; }
       }
       const uint32_t base = (uint32_t)nt * TN;
 #pragma unroll
-      for (int h = 0; h < 2; ++h)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) top3_insert_idx(m[h][j], base + (__float_as_uint(m[h][j]) & 0xFFu), g[h], gi[h]);
+      for (int j = 0; j < 3; ++j) top3_insert_idx(m[j], base + (__float_as_uint(m[j]) & 0xFFu), g, gi);
       if (nt == ntiles - 1 && (lane & 3) < 2) {  // row tile complete: lanes 0 / 1 of the quad write rows r0 / r0 + 8
-        const int h = lane & 1;
-        const uint64_t row = h ? row1 : row0;
+        const uint64_t row = (lane & 1) ? row1 : row0;
         if (row < n) {
-          const float v0 = h ? g[1][0] : g[0][0], v1 = h ? g[1][1] : g[0][1], v2 = h ? g[1][2] : g[0][2];
-          const uint32_t flag = verdict(v0, v1, v2, tau_scale * (row_norm2[row] + cmax2));
-          res[row] = (h ? gi[1][0] : gi[0][0]) | (flag << 30);
-          res_hi[row] = h ? gi[1][1] : gi[0][1];
-          if (top1_val && flag == 2) top1_val[row] = v0;
+          const uint32_t flag = verdict(g[0], g[1], g[2], tau_scale * (row_norm2[row] + cmax2));
+          res[row] = gi[0] | (flag << 30);
+          res_hi[row] = gi[1];
+          if (top1_val && flag == 2) top1_val[row] = g[0];
         }
       }
     });

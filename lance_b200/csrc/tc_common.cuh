@@ -121,13 +121,34 @@ __device__ __forceinline__ void wgmma_bf16(float* d, uint64_t a_desc, uint64_t b
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
       : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
+// M64 N128 (TF32), 64 registers per thread: half of the columns of the N256 tile, same fragment layout with j < 16
+__device__ __forceinline__ void wgmma_tf32_n128(float* d, uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// wait until at most N committed wgmma groups of this warpgroup are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { wgmma_wait<0>(); }
 // ties the accumulator registers to this point: no access to them moves across an asynchronous MMA or its wait
+template <int N = 128>
 __device__ __forceinline__ void acc_fence(float* d) {
 #pragma unroll
-  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// The 1024-aligned base of the dynamic shared memory (SWIZZLE_128B tiles).  Derived from `raw` by pointer
+// arithmetic, not through an integer, so that the compiler keeps the shared state space of every access through
+// it (LDS, not generic loads).
+__device__ __forceinline__ uint8_t* smem_align1024(uint8_t* raw) {
+  return raw + ((1024u - (smem_u32(raw) & 1023u)) & 1023u);
 }
 // OPK: 0 = f32 operands as TF32, 1 = f16, 2 = bf16
 template <int OPK>
@@ -155,7 +176,7 @@ __device__ __forceinline__ void mma_unit(float* d, int nkc, Stage&& stage, Relea
       wgmma_op<OPK>(d, make_desc(a_addr + k * 32), make_desc(b_addr + k * 32), (kc != 0 || k != 0) ? 1u : 0u);
     wgmma_commit();
     if (prev >= 0) {
-      asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory");
+      wgmma_wait<1>();
       release(prev);
     }
     prev = s;
@@ -175,89 +196,120 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 // four lanes of a quad.
 __device__ __forceinline__ int frag_row(int h) { return 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2) + 8 * h; }
 
-// insert g into the sorted triple (m1 >= m2 >= m3)
-__device__ __forceinline__ void top3_insert(float g, float& m1, float& m2, float& m3) {
-  const float t1 = fminf(m1, g);
-  m1 = fmaxf(m1, g);
-  const float t2 = fminf(m2, t1);
-  m2 = fmaxf(m2, t1);
-  m3 = fmaxf(m3, t2);
-}
 // ---- top-3 of a 256-column accumulator row by TOURNAMENT ------------------------------------------
 // The epilogue is bound by min/max instructions per column.  Pair the values: the winners (max) go on, and
 // of the losers (min) only the LARGEST can be among the row's top 3 -- a loser is beaten by its own partner,
 // so two losers in the top 3 would need four distinct values ahead of the smaller one.  (All values are
 // distinct: each carries its column index in the low mantissa byte.)  Applying this at every level,
-//     top3(row) = top3( top3(last-level winners)  U  { largest loser of each level } ),
-// i.e. per level one running maximum over the losers plus one exact top-3 tracker fed by a single value per
-// 32-value chunk.
-constexpr int TOUR_LEVELS = 5;
+//     top3(row) = { champion }  U  top2( largest loser of each level ),
+// i.e. per level one running maximum over the losers.  The 256 columns come as two 128-column halves (an
+// M64 N128 wgmma each, or the two halves of an N256 fragment); a lane holds 32 values of each half and row:
+// levels 0..4 pair those, level 5 pairs the winners of the two halves.
+constexpr int TOUR_LEVELS = 6;
 
-// one chunk of 32 packed scores g (destroyed).  T = exact top-3 of the chunk winners so far, L[j] = largest
-// level-j loser so far.
-__device__ __forceinline__ void tour_chunk(float* g, float* T, float* L) {
-#pragma unroll
-  for (int lvl = 0, cnt = 32; lvl < TOUR_LEVELS; ++lvl, cnt >>= 1) {
-#pragma unroll
-    for (int i = 0; i < 16; ++i) {
-      if (i < cnt / 2) {
-        const float x = g[2 * i], y = g[2 * i + 1];
-        g[i] = fmaxf(x, y);
-        L[lvl] = fmaxf(L[lvl], fminf(x, y));
-      }
-    }
-  }
-  top3_insert(g[0], T[0], T[1], T[2]);
-}
-// score with the column index in the low mantissa byte (one PRMT)
-__device__ __forceinline__ float pack_col(float f, uint32_t col) {
-  return __uint_as_float(__byte_perm(__float_as_uint(f), col, 0x3214));
+struct Tour {
+  float top[2];              // winner so far of fragment row h
+  float L[2][TOUR_LEVELS];   // largest level-lvl loser so far
+};
+
+// score with its column in the low mantissa byte: byte b of the column word cw (one PRMT, b a constant)
+__device__ __forceinline__ float pack_col(float f, uint32_t cw, int b) {
+  return __uint_as_float(__byte_perm(__float_as_uint(f), cw, 0x3214 + b));
 }
 
-// top-3 of acc + cn[col] for both rows of the thread's fragment; every lane of the quad ends with the row's
-// top-3 of all 256 columns (indices in the low mantissa byte).  cn: 256 floats (shared or global memory).
-__device__ __forceinline__ void top3_frag(const float* acc, const float* cn, float (&m)[2][3]) {
-  const float ninf = __int_as_float(0xff800000);
+// Folds one 128-column half of both fragment rows into the tournament (half 0 starts it, half 1 completes it):
+// score acc + cn[col], packed with its column.  a: the half's 64 accumulators, a[4j + 2h + e] = (row r0 + 8h,
+// column 128 HALF + 8j + 2 (t % 4) + e), j < 16; cn: the 256 values of -|c|^2/2 (shared or global memory).
+template <int HALF>
+__device__ __forceinline__ void top3_half(const float* a, const float* cn, Tour& st) {
   const uint32_t q2 = 2 * (threadIdx.x & 3);
-  float T[2][3], L[2][TOUR_LEVELS];
+  // cw[e][i], byte b: the column of j = 4i + b, 128 HALF + 32i + 8b + q2 + e (< 256: no carry between bytes)
+  uint32_t cw[2][4];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    T[h][0] = T[h][1] = T[h][2] = ninf;
+  for (int e = 0; e < 2; ++e)
 #pragma unroll
-    for (int j = 0; j < TOUR_LEVELS; ++j) L[h][j] = ninf;
+    for (int i = 0; i < 4; ++i) cw[e][i] = (HALF ? 0x98908880u : 0x18100800u) + 0x20202020u * i + 0x01010101u * (q2 + e);
+  float w[2][16];
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {  // level 0: the two columns of a j
+    const float2 cv = *reinterpret_cast<const float2*>(cn + 128 * HALF + 8 * j + q2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float x = pack_col(a[4 * j + 2 * h] + cv.x, cw[0][j >> 2], j & 3);
+      const float y = pack_col(a[4 * j + 2 * h + 1] + cv.y, cw[1][j >> 2], j & 3);
+      w[h][j] = fmaxf(x, y);
+      const float lo = fminf(x, y);
+      st.L[h][0] = (HALF == 0 && j == 0) ? lo : fmaxf(st.L[h][0], lo);
+    }
   }
 #pragma unroll
-  for (int c = 0; c < 2; ++c) {
-    float g[2][32];
+  for (int h = 0; h < 2; ++h) {
 #pragma unroll
-    for (int jj = 0; jj < 16; ++jj) {
-      const int j = 16 * c + jj;
-      const uint32_t col = 8 * j + q2;
-      const float2 cv = *reinterpret_cast<const float2*>(cn + col);
+    for (int lvl = 1, cnt = 16; lvl < 5; ++lvl, cnt >>= 1) {
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        g[h][2 * jj] = pack_col(acc[4 * j + 2 * h] + cv.x, col);
-        g[h][2 * jj + 1] = pack_col(acc[4 * j + 2 * h + 1] + cv.y, col + 1);
+      for (int i = 0; i < 8; ++i) {
+        if (i < cnt / 2) {
+          const float x = w[h][2 * i], y = w[h][2 * i + 1];
+          w[h][i] = fmaxf(x, y);
+          const float lo = fminf(x, y);
+          st.L[h][lvl] = (HALF == 0 && i == 0) ? lo : fmaxf(st.L[h][lvl], lo);
+        }
       }
     }
-#pragma unroll
-    for (int h = 0; h < 2; ++h) tour_chunk(g[h], T[h], L[h]);
-  }
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    m[h][0] = T[h][0]; m[h][1] = T[h][1]; m[h][2] = T[h][2];
-#pragma unroll
-    for (int j = 0; j < TOUR_LEVELS; ++j) top3_insert(L[h][j], m[h][0], m[h][1], m[h][2]);
-#pragma unroll
-    for (int off = 1; off <= 2; off <<= 1) {
-      const float o0 = __shfl_xor_sync(0xffffffffu, m[h][0], off);
-      const float o1 = __shfl_xor_sync(0xffffffffu, m[h][1], off);
-      const float o2 = __shfl_xor_sync(0xffffffffu, m[h][2], off);
-      top3_insert(o0, m[h][0], m[h][1], m[h][2]);
-      top3_insert(o1, m[h][0], m[h][1], m[h][2]);
-      top3_insert(o2, m[h][0], m[h][1], m[h][2]);
+    if (HALF == 0) {
+      st.top[h] = w[h][0];
+    } else {  // level 5
+      st.L[h][5] = fminf(st.top[h], w[h][0]);
+      st.top[h] = fmaxf(st.top[h], w[h][0]);
     }
   }
+}
+
+// top-3 of the union of two sorted triples (a[0] >= a[1] >= a[2]), into a
+__device__ __forceinline__ void top3_merge(float (&a)[3], const float (&b)[3]) {
+  const float x = fminf(a[0], b[0]), y = fmaxf(a[1], b[1]), z = fmaxf(a[2], b[2]);
+  a[0] = fmaxf(a[0], b[0]);
+  a[1] = fmaxf(x, y);
+  a[2] = fmaxf(fminf(x, y), z);
+}
+
+// The finished tournament: m = the top-3 (sorted, column in the low mantissa byte) of all 256 columns of the
+// fragment row r0 + 8 (lane & 1), in every lane of the quad.
+__device__ __forceinline__ void top3_finish(const Tour& st, float (&m)[3]) {
+  float t[2][3];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float a = fmaxf(st.L[h][0], st.L[h][1]), b = fminf(st.L[h][0], st.L[h][1]);
+#pragma unroll
+    for (int lvl = 2; lvl < TOUR_LEVELS; ++lvl) {
+      b = fmaxf(b, fminf(a, st.L[h][lvl]));
+      a = fmaxf(a, st.L[h][lvl]);
+    }
+    t[h][0] = st.top[h];
+    t[h][1] = a;
+    t[h][2] = b;
+  }
+  // lanes 0 / 2 of the quad keep row r0 and lanes 1 / 3 row r0 + 8; each hands the other row to its xor-1
+  // neighbour, then the xor-2 neighbours (same row) merge
+  const bool odd = threadIdx.x & 1;
+  float o[3];
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    m[i] = odd ? t[1][i] : t[0][i];
+    o[i] = __shfl_xor_sync(0xffffffffu, odd ? t[0][i] : t[1][i], 1);
+  }
+  top3_merge(m, o);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) o[i] = __shfl_xor_sync(0xffffffffu, m[i], 2);
+  top3_merge(m, o);
+}
+
+// top-3 of acc + cn[col] over a whole N256 fragment (see top3_finish)
+__device__ __forceinline__ void top3_frag(const float* acc, const float* cn, float (&m)[3]) {
+  Tour st;
+  top3_half<0>(acc, cn, st);
+  top3_half<1>(acc + 64, cn, st);
+  top3_finish(st, m);
 }
 
 // ---- candidate pass: every column of the fragment's rows whose score reaches thr[h] ---------------------------

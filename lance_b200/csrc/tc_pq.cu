@@ -8,8 +8,9 @@
 //   * B operand: the codebook as one K-major matrix Bm[c][m*8+t] = cb[m][c][t] (256 x d f32), resident
 //     in shared memory for the whole kernel (TMA, SWIZZLE_128B).
 //   * A operand: 64-row tiles of the (residual) vectors, TMA-streamed in 32-float chunks (= 4 sub-spaces).
-//   * one wgmma (M64 N256 K8, tf32) per (tile, sub-space) into register accumulators, two consumer
-//     warpgroups taking the work items in turns; the epilogue keeps the top-3 of  r.c - |c|^2/2  per row and classifies the row
+//   * two wgmmas (M64 N128 K8, tf32: one per half of the codebook) per (tile, sub-space) into register
+//     accumulators, two consumer warpgroups taking the work items in turns; the epilogue of one half overlaps
+//     the MMA of the next; it keeps the top-3 of  r.c - |c|^2/2  per row and classifies the row
 //     against tau = 3*2^-10 (|r_m|^2 + max|c_m|^2) exactly like tc_assign.cu;
 //   * flag 0/1 rows are decided IN THE EPILOGUE with reference-order f32 arithmetic on the operands
 //     that are still in shared memory (sequential 8-term sum, l2.rs:69-79; strict-< / lowest index);
@@ -36,7 +37,7 @@ constexpr int STREAM_STAGE_BYTES = A_STAGE_BYTES + B_CHUNK_BYTES + CNH_CHUNK_BYT
 // RESIDENT: [B: nkc x 32 KB][A ring: STAGES x 8 KB][cnh: M x 1 KB]
 // STREAM:   [ring: STAGES x (A 8 KB | B chunk 32 KB | cnh slice 4 KB)]
 struct Layout {
-  uint32_t b_off, a_off, cnh_off, bar_off, misc_off, total;
+  uint32_t b_off, a_off, cnh_off, bar_off, cbm_off, misc_off, total;
   uint32_t stage_bytes;  // distance between two A stages
 };
 __host__ __device__ inline Layout layout(int nkc, int M, bool stream) {
@@ -54,7 +55,9 @@ __host__ __device__ inline Layout layout(int nkc, int M, bool stream) {
     L.stage_bytes = A_STAGE_BYTES;
     L.bar_off = L.cnh_off + M * TN * 4;
   }
-  L.misc_off = L.bar_off + (2 * STAGES + 1) * 8;
+  static_assert((2 * STAGES + 1) * 8 <= 128, "barriers");
+  L.cbm_off = L.bar_off + 128;              // max_c |c|^2 per sub-space
+  L.misc_off = L.cbm_off + MAX_M * 4;
   L.total = L.misc_off + MAX_M;  // one "active" byte per sub-space
   return L;
 }
@@ -85,11 +88,12 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
              uint8_t* __restrict__ valid, uint32_t* __restrict__ fb_pairs,
              uint32_t* __restrict__ fb_count, const uint8_t* __restrict__ active) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smem = smem_align1024(smem_raw);
   const int nkc = M / 4;
   const Layout L = layout(nkc, M, STREAM);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + L.bar_off);
   uint8_t* act_s = smem + L.misc_off;  // [M] 0/1 (M % 4 == 0: read as one word per chunk)
+  float* cbm_s = reinterpret_cast<float*>(smem + L.cbm_off);  // [M]
   const uint32_t sb = smem_u32(smem);
   auto full_bar = [&](int s) { return smem_u32(&bars[s]); };
   auto empty_bar = [&](int s) { return smem_u32(&bars[STAGES + s]); };
@@ -106,6 +110,7 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
   for (int m = threadIdx.x; m < M; m += NUM_THREADS) {
     const uint8_t a = (!active || active[m]) ? 1 : 0;
     act_s[m] = a;
+    cbm_s[m] = cbmax2[m];
     any_active |= a;
   }
   if (threadIdx.x == 32) {
@@ -151,11 +156,16 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
       }
     }
   } else {
-    // ===== consumers: one wgmma (K = 8 = one sub-space) per active sub-space, top-3, exact re-rank =====
+    // ===== consumers: per active sub-space two wgmmas (K = 8, one per 128-codeword half), top-3, exact re-rank =====
+    // Each half is its own wgmma group: the tournament of half 0 runs while half 1 is in flight, and that of
+    // half 1 while the next sub-space's half 0, issued into the registers just read, is.  No MMA is in flight
+    // during the divergent decision code: the compiler would serialize every wgmma of the kernel otherwise.
     setmaxnreg_inc<CONSUMER_REGS>();
     const int w = (threadIdx.x >> 7) - 1;
     if (!STREAM) mbar_wait(b_full, 0);
-    float acc[128];
+    const int h = lane & 1;      // lanes 0 / 1 of the quad finish rows r0 / r0 + 8
+    const int rl = frag_row(h);  // row inside the tile
+    float acc[2][64];
     uint32_t k = 0;  // ring index of the items with an active sub-space
     for (uint64_t item = blockIdx.x; item < num_tiles * nkc; item += gridDim.x) {
       const uint64_t tile = item / nkc;
@@ -167,29 +177,53 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
       const uint32_t ph = (k / STAGES) & 1;
       ++k;
       if (!mine) continue;
+      const uint64_t row = tile * TM + rl;
+      const bool decides = (lane & 3) < 2 && row < n;
+      // |r_m|^2 of the item's four sub-spaces (contiguous, 16-byte aligned: M % 4 == 0), fetched before the MMAs
+      float4 rn4 = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+      if (decides) rn4 = *reinterpret_cast<const float4*>(rn2 + row * M + 4 * kc);
+      const float4 cb4 = *reinterpret_cast<const float4*>(cbm_s + 4 * kc);
       mbar_wait(full_bar(s), ph);
       const uint8_t* atile = smem + L.a_off + s * L.stage_bytes;
       const uint8_t* bt = smem + L.b_off + (STREAM ? s * L.stage_bytes : kc * B_CHUNK_BYTES);
       const float* cn4 = reinterpret_cast<const float*>(smem + L.cnh_off + (STREAM ? s * L.stage_bytes : kc * CNH_CHUNK_BYTES));
       const uint32_t a_addr = smem_u32(atile), b_addr = smem_u32(bt);
-      for (int j = 0; j < 4; ++j) {
-        if (!((cm >> j) & 1)) continue;
-        const int m = kc * 4 + j;
-        __syncwarp();
-        acc_fence(acc);
+      // half `hf` of sub-space j: codewords 128 hf .. 128 hf + 127 are B rows 128 hf.. (128 B each)
+      auto issue = [&](float* d, int j, int hf) {
+        __syncwarp();  // wgmma is warp-aligned: reconverge after the divergent re-rank and barrier polls
+        acc_fence<64>(d);
         wgmma_fence();
-        wgmma_tf32(acc, make_desc(a_addr + j * 32), make_desc(b_addr + j * 32), 0u);
+        wgmma_tf32_n128(d, make_desc(a_addr + j * 32), make_desc(b_addr + hf * (TN / 2) * 128 + j * 32), 0u);
         wgmma_commit();
-        wgmma_wait_all();
-        acc_fence(acc);
-        float mm[2][3];
-        top3_frag(acc, cn4 + j * TN, mm);
-        const int h = lane & 1;      // lanes 0 / 1 of the quad finish rows r0 / r0 + 8
-        const int rl = frag_row(h);  // row inside the tile
-        const uint64_t row = tile * TM + rl;
-        if ((lane & 3) < 2 && row < n) {
-          const float m1 = h ? mm[1][0] : mm[0][0], m2 = h ? mm[1][1] : mm[0][1], m3 = h ? mm[1][2] : mm[0][2];
-          const float tau = 0.0029296875f * (rn2[row * M + m] + cbmax2[m]);
+      };
+      uint32_t rest = cm;
+      int j = __ffs(rest) - 1;
+      rest &= rest - 1;
+      issue(acc[0], j, 0);
+      issue(acc[1], j, 1);
+      for (;;) {
+        const int m = kc * 4 + j;
+        const int jn = rest ? __ffs(rest) - 1 : -1;  // next active sub-space of the item
+        Tour tour;
+        wgmma_wait<1>();
+        acc_fence<64>(acc[0]);
+        top3_half<0>(acc[0], cn4 + j * TN, tour);
+        if (jn >= 0) {
+          issue(acc[0], jn, 0);
+          wgmma_wait<1>();
+        } else {
+          wgmma_wait<0>();
+        }
+        acc_fence<64>(acc[1]);
+        top3_half<1>(acc[1], cn4 + j * TN, tour);
+        float mm[3];
+        top3_finish(tour, mm);
+        wgmma_wait<0>();
+        if (decides) {
+          const float m1 = mm[0], m2 = mm[1], m3 = mm[2];
+          const float rn = j == 0 ? rn4.x : j == 1 ? rn4.y : j == 2 ? rn4.z : rn4.w;
+          const float cbm = j == 0 ? cb4.x : j == 1 ? cb4.y : j == 2 ? cb4.z : cb4.w;
+          const float tau = 0.0029296875f * (rn + cbm);
           uint32_t flag = 2;
           if (m1 - m2 > tau) flag = 0;
           else if (m1 - m3 > tau) flag = 1;
@@ -231,9 +265,14 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
             }
           }
         }
-        __syncwarp();
+        if (jn < 0) break;
+        issue(acc[1], jn, 1);
+        j = jn;
+        rest &= rest - 1;
       }
-      if (lane == 0) mbar_arrive(empty_bar(s));  // this warp is done with the stage
+      // every MMA of the item has completed (wait_group 0 above) and this warp's re-ranks have read the stage
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(s));
     }
   }
 }
