@@ -363,9 +363,12 @@ def flat_topk(dists, row_ids, k, lower_bound=None, upper_bound=None):
     return oi[:cnt[0]], od[:cnt[0]]
 
 
-def ivfpq_transform(centroids, codebook, vectors, distance_type="l2", num_bits=8):
-    """IvfTransformer::transform for IVF_PQ (lance-index/src/vector/ivf.rs:188-236,357)."""
-    centroids, codebook, vectors = _f32(centroids), _f32(codebook), _f32(vectors)
+def ivfpq_transform(centroids, codebook, vectors, distance_type="l2", num_bits=8, bf16=False):
+    """IvfTransformer::transform for IVF_PQ (lance-index/src/vector/ivf.rs:188-236,357).
+    The rows keep their element type; the model has the rows' model type (bf16=True: uint16 bit patterns)."""
+    vectors, dt = _typed(vectors, bf16)
+    centroids = np.ascontiguousarray(centroids, dtype=_model_np(dt))
+    codebook = np.ascontiguousarray(codebook, dtype=_model_np(dt))
     k, d = centroids.shape
     M = codebook.shape[0]
     n = vectors.shape[0]
@@ -374,7 +377,7 @@ def ivfpq_transform(centroids, codebook, vectors, distance_type="l2", num_bits=8
     bp, _k2 = as_ptr(codebook)
     vp, _k3 = as_ptr(vectors)
     check(lib().lb2_ivfpq_transform(cp, C.c_uint32(k), bp, C.c_uint32(M), C.c_uint32(num_bits),
-                                    C.c_uint32(d), C.c_int(F32), C.c_int(_metric(distance_type)), vp,
+                                    C.c_uint32(d), C.c_int(dt), C.c_int(_metric(distance_type)), vp,
                                     C.c_uint64(n), C.c_void_p(part.ctypes.data),
                                     C.c_void_p(codes.ctypes.data), C.c_void_p(valid.ctypes.data)))
     return part, codes, valid.astype(bool)
@@ -400,10 +403,11 @@ class IvfPqIndex:
         self.stats = stats
 
     @classmethod
-    def build(cls, data, distance_type="l2", params=None, row_ids=None):
-        """IvfIndexBuilder::build (builder.rs:236): create_index("IVF_PQ")."""
+    def build(cls, data, distance_type="l2", params=None, row_ids=None, bf16=False):
+        """IvfIndexBuilder::build (builder.rs:236): create_index("IVF_PQ").
+        bf16=True: `data` is a uint16 array holding bfloat16 bit patterns (numpy has no bf16 dtype)."""
         params = params or IvfBuildParams()
-        data, dt = _typed(data)
+        data, dt = _typed(data, bf16)
         n, d = data.shape
         bp = BuildParams()
         lib().lb2_ivfpq_build_params_default(C.byref(bp))
@@ -690,13 +694,16 @@ class IvfFlatIndex(IvfPqIndex):
         return ix
 
     @classmethod
-    def from_parts(cls, centroids, part_ids, vectors, row_ids=None, distance_type="l2"):
-        centroids, vectors = _f32(centroids), _f32(vectors)
+    def from_parts(cls, centroids, part_ids, vectors, row_ids=None, distance_type="l2", bf16=False):
+        """The vectors keep their element type (bf16=True: uint16 bit patterns); the centroids have its model type."""
+        vectors, dt = _typed(vectors, bf16)
+        centroids = np.ascontiguousarray(centroids, dtype=_model_np(dt))
         k, d = centroids.shape
         h = C.c_void_p()
         check(lib().lb2_index_create_flat(C.c_void_p(centroids.ctypes.data), C.c_uint32(k), C.c_uint32(d),
-                                          C.c_int(F32), C.c_int(_metric(distance_type)), C.byref(h)))
+                                          C.c_int(dt), C.c_int(_metric(distance_type)), C.byref(h)))
         ix = cls(h)
+        ix._dt = dt
         part_ids = np.ascontiguousarray(part_ids, dtype=np.uint32)
         rid = None if row_ids is None else np.ascontiguousarray(row_ids, dtype=np.uint64)
         rp, _k = as_ptr(rid)

@@ -390,6 +390,11 @@ class Source {
   }
   Source(const Source&) = delete;
   uint64_t rows_per_chunk() const {  // <= 1 GB of f32 per chunk, 64 Ki .. 1 Mi rows
+    // LB2_CHUNK_ROWS=r replaces the rule (no floor): small inputs then take the multi-chunk paths.  Read on
+    // every call, so that a test can set it for one call.
+    const char* e = getenv("LB2_CHUNK_ROWS");
+    const uint64_t r = e && *e ? strtoull(e, nullptr, 10) : 0;
+    if (r >= 1) return r;
     return std::max<uint64_t>(1ull << 16, std::min<uint64_t>(1ull << 20, (1ull << 28) / (uint64_t)d_));
   }
   // training sample: rows `rows` (ascending) as f32 [rows.size()][d] -- straight out of the caller's memory
@@ -470,6 +475,10 @@ class Source {
     if (dev_native_ || n_ == 0) return;
     const size_t bytes = (size_t)n_ * d_ * es_;
     acquire_cache();  // (a second Source alive on the same thread falls back to private resources)
+    // LB2_MAX_RESIDENT_MB=m: a matrix of more than m MB is streamed (0 = always); read on every call, and
+    // ahead of the warm-cache shortcut below, which would otherwise skip every size test
+    const char* cap_e = getenv("LB2_MAX_RESIDENT_MB");
+    if (cap_e && *cap_e && bytes > ((size_t)strtoull(cap_e, nullptr, 10) << 20)) return;
     StagingCache& sc = g_staging[ctx().device];
     const bool cached_buf = cache_ && bytes <= staging_cache_cap();
     if (!(cached_buf && sc.bytes >= bytes)) {
@@ -575,7 +584,19 @@ class Source {
     }
     LB2_CUDA(cudaEventRecord(slot_free_[slot], ctx().stream));  // everything issued so far is done with the slot
     LB2_CUDA(cudaStreamWaitEvent(copy_stream_, slot_free_[slot], 0));
+    // profiling: one "stage_rows" entry per staged chunk (timed on the copy stream; not a kernel launch)
+    Ctx& c = ctx();
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    if (c.profiling) {
+      LB2_CUDA(cudaEventCreate(&e0));
+      LB2_CUDA(cudaEventCreate(&e1));
+      LB2_CUDA(cudaEventRecord(e0, copy_stream_));
+    }
     LB2_CUDA(cudaMemcpyAsync(dst, static_cast<const uint8_t*>(host_) + off, cnt * es_, cudaMemcpyHostToDevice, copy_stream_));
+    if (e0) {
+      LB2_CUDA(cudaEventRecord(e1, copy_stream_));
+      c.pending.push_back({c.tag.empty() ? std::string("stage_rows") : c.tag + ":stage_rows", {e0, e1}});
+    }
     LB2_CUDA(cudaEventRecord(slot_ready_[slot], copy_stream_));
     staged_[slot] = true;
     staged_r0_[slot] = r0;

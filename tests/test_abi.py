@@ -41,6 +41,21 @@ def test_product_never_imports_oracle():
                     or f in ("_lib.py", "kmeans.cu"), f
 
 
+def test_every_environment_knob_is_in_the_integration_table():
+    """each LB2_* variable the library reads is listed in INTEGRATION.md's table of environment knobs"""
+    names = set()
+    csrc = os.path.join(ROOT, "lance_b200", "csrc")
+    for f in os.listdir(csrc):
+        if f.endswith((".cu", ".cuh")):
+            names |= set(re.findall(r'getenv\(\s*"(LB2_[A-Z0-9_]+)"', open(os.path.join(csrc, f)).read()))
+    assert "LB2_CHUNK_ROWS" in names and "LB2_MAX_RESIDENT_MB" in names
+    doc = open(os.path.join(ROOT, "INTEGRATION.md")).read()
+    table = doc.split("### Environment knobs", 1)[1].split("\n\n", 2)[1]
+    assert table.startswith("| Variable |")
+    documented = set(re.findall(r"`(LB2_[A-Z0-9_]+)", table))
+    assert sorted(names - documented) == []
+
+
 @pytest.mark.skipif(lb.device_count() > 0, reason="only meaningful on a box without a GPU")
 def test_no_gpu_fails_loudly():
     with pytest.raises(lb.LanceB200Error) as e:
