@@ -9,9 +9,9 @@
 //     in shared memory for the whole kernel (TMA, SWIZZLE_128B).
 //   * A operand: 64-row tiles of the (residual) vectors, TMA-streamed in 32-float chunks (= 4 sub-spaces).
 //   * two wgmmas (M64 N128 K8, tf32: one per half of the codebook) per (tile, sub-space) into register
-//     accumulators, two consumer warpgroups taking the work items in turns; the epilogue of one half overlaps
-//     the MMA of the next; it keeps the top-3 of  r.c - |c|^2/2  per row and classifies the row
-//     against tau = 3*2^-10 (|r_m|^2 + max|c_m|^2) exactly like tc_assign.cu;
+//     accumulators, consumer warpgroups taking the work items in turns (see Pipe); the epilogue keeps the
+//     top-3 of  r.c - |c|^2/2  per row and classifies the row against tau = 3*2^-10 (|r_m|^2 + max|c_m|^2)
+//     exactly like tc_assign.cu;
 //   * flag 0/1 rows are decided IN THE EPILOGUE with reference-order f32 arithmetic on the operands
 //     that are still in shared memory (sequential 8-term sum, l2.rs:69-79; strict-< / lowest index);
 //   * flag 2 (row, sub-space) pairs are appended to a list and finished by pq_fallback_kernel
@@ -28,11 +28,34 @@ namespace tcpq {
 using namespace tc;
 
 constexpr int DS = 8;
-constexpr int STAGES = 4;
 constexpr int MAX_M_RESIDENT = 16;  // d <= 128: the whole codebook matrix stays in shared memory
 constexpr int MAX_M = 256;          // d <= 2048: codebook chunk + its -|c|^2/2 slice streamed per work item
 constexpr int CNH_CHUNK_BYTES = 4 * TN * 4;                                       // 4 sub-spaces
 constexpr int STREAM_STAGE_BYTES = A_STAGE_BYTES + B_CHUNK_BYTES + CNH_CHUNK_BYTES;  // 44 KB
+
+// One TMA producer warpgroup and CONSUMERS warpgroups that take the work items in turns.  The epilogue is bound by
+// the ALU pipe, and a consumer warp stalls often (wgmma waits, the divergent decision code, barrier waits, the
+// shuffles of top3_finish); the resident variant runs four consumers (4 warps per scheduler) so that the others
+// fill those stalls.  The streamed ring (44 KB per stage) has no room for more than four stages, so the streamed
+// variant keeps two consumers.
+// ACC_SETS: 64-register accumulator sets of a consumer.  With two, the tournament of one 128-codeword half runs
+// while the MMA of the next is in flight; they do not fit the 112 registers of four consumers without spills,
+// so there one half is computed at a time and the other warpgroups fill the MMA latency.
+template <bool STREAM>
+struct Pipe {
+  static constexpr int CONSUMERS = STREAM ? 2 : 4;
+  static constexpr int STAGES = STREAM ? 4 : 8;
+  static constexpr int ACC_SETS = STREAM ? 2 : 1;
+  static constexpr int THREADS = 128 * (1 + CONSUMERS);
+  static constexpr int PRODUCER_REGS = STREAM ? 40 : 24;
+  static constexpr int CONSUMER_REGS = STREAM ? 232 : 112;
+  // every stage always serves the same warpgroup, so a stage is refilled only after its own consumer released it
+  static_assert(STAGES % CONSUMERS == 0, "stages are dealt to the consumer warpgroups in turns");
+  // setmaxnreg only moves registers between the warps of the CTA: the consumers can gain what the producer gives
+  // up of the launch allocation (THREADS x the per-thread count that __launch_bounds__ leaves, a multiple of 8)
+  static_assert(128 * (PRODUCER_REGS + CONSUMERS * CONSUMER_REGS) <= THREADS * ((65536 / THREADS) & ~7),
+                "register file");
+};
 
 // RESIDENT: [B: nkc x 32 KB][A ring: STAGES x 8 KB][cnh: M x 1 KB]
 // STREAM:   [ring: STAGES x (A 8 KB | B chunk 32 KB | cnh slice 4 KB)]
@@ -47,16 +70,16 @@ __host__ __device__ inline Layout layout(int nkc, int M, bool stream) {
     L.a_off = 0;                              // + s * stage_bytes
     L.cnh_off = A_STAGE_BYTES + B_CHUNK_BYTES;  // + s * stage_bytes
     L.stage_bytes = STREAM_STAGE_BYTES;
-    L.bar_off = STAGES * STREAM_STAGE_BYTES;
+    L.bar_off = Pipe<true>::STAGES * STREAM_STAGE_BYTES;
   } else {
     L.b_off = 0;
     L.a_off = nkc * B_CHUNK_BYTES;
-    L.cnh_off = L.a_off + STAGES * A_STAGE_BYTES;
+    L.cnh_off = L.a_off + Pipe<false>::STAGES * A_STAGE_BYTES;
     L.stage_bytes = A_STAGE_BYTES;
     L.bar_off = L.cnh_off + M * TN * 4;
   }
-  static_assert((2 * STAGES + 1) * 8 <= 128, "barriers");
-  L.cbm_off = L.bar_off + 128;              // max_c |c|^2 per sub-space
+  static_assert((2 * Pipe<false>::STAGES + 1) * 8 <= 256 && (2 * Pipe<true>::STAGES + 1) * 8 <= 256, "barriers");
+  L.cbm_off = L.bar_off + 256;              // max_c |c|^2 per sub-space
   L.misc_off = L.cbm_off + MAX_M * 4;
   L.total = L.misc_off + MAX_M;  // one "active" byte per sub-space
   return L;
@@ -75,18 +98,18 @@ __device__ __forceinline__ const float4* swz(const uint8_t* tile, int r, int u) 
 }
 
 // Work items = (64-row tile, 32-float chunk = 4 sub-spaces), finer than whole tiles so that the persistent CTAs
-// (one per SM) stay balanced on short inputs (65 536-row training calls: 1024 tiles).  The two consumer
-// warpgroups take the items with an active sub-space in turns; with an even number of stages every stage
-// always serves the same warpgroup, so a stage is refilled only after its own consumer released it.
-static_assert(STAGES % 2 == 0, "stages alternate between the two consumer warpgroups");
+// (one per SM) stay balanced on short inputs (65 536-row training calls: 1024 tiles).  The consumer warpgroups
+// take the items with an active sub-space in turns (see Pipe).
 template <bool TRAIN, bool STREAM>
-__global__ void __launch_bounds__(NUM_THREADS, 1)
+__global__ void __launch_bounds__(Pipe<STREAM>::THREADS, 1)
 tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ CUtensorMap map_b,
              uint64_t n, int M, const float* __restrict__ cnh_g, const float* __restrict__ cbmax2,
              const float* __restrict__ rn2, const uint8_t* __restrict__ row_valid,
              uint8_t* __restrict__ codes, uint32_t* __restrict__ ids, float* __restrict__ dists,
              uint8_t* __restrict__ valid, uint32_t* __restrict__ fb_pairs,
              uint32_t* __restrict__ fb_count, const uint8_t* __restrict__ active) {
+  using P = Pipe<STREAM>;
+  constexpr int STAGES = P::STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = smem_align1024(smem_raw);
   const int nkc = M / 4;
@@ -104,10 +127,10 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
 
   if (!STREAM) {
     float* cnh = reinterpret_cast<float*>(smem + L.cnh_off);
-    for (int i = threadIdx.x; i < M * TN; i += NUM_THREADS) cnh[i] = cnh_g[i];
+    for (int i = threadIdx.x; i < M * TN; i += P::THREADS) cnh[i] = cnh_g[i];
   }
   int any_active = 0;
-  for (int m = threadIdx.x; m < M; m += NUM_THREADS) {
+  for (int m = threadIdx.x; m < M; m += P::THREADS) {
     const uint8_t a = (!active || active[m]) ? 1 : 0;
     act_s[m] = a;
     cbm_s[m] = cbmax2[m];
@@ -131,7 +154,7 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
 
   if (warp < 4) {
     // ===== TMA producer =====
-    setmaxnreg_dec<PRODUCER_REGS>();
+    setmaxnreg_dec<P::PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       if (!STREAM) {
         mbar_expect_tx(b_full, (uint32_t)nkc * B_CHUNK_BYTES);
@@ -157,22 +180,21 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
     }
   } else {
     // ===== consumers: per active sub-space two wgmmas (K = 8, one per 128-codeword half), top-3, exact re-rank =====
-    // Each half is its own wgmma group: the tournament of half 0 runs while half 1 is in flight, and that of
-    // half 1 while the next sub-space's half 0, issued into the registers just read, is.  No MMA is in flight
-    // during the divergent decision code: the compiler would serialize every wgmma of the kernel otherwise.
-    setmaxnreg_inc<CONSUMER_REGS>();
-    const int w = (threadIdx.x >> 7) - 1;
+    // Each half is its own wgmma group.  No MMA is in flight during the divergent decision code: the compiler
+    // would serialize every wgmma of the kernel otherwise.
+    setmaxnreg_inc<P::CONSUMER_REGS>();
+    const uint32_t w = (threadIdx.x >> 7) - 1;
     if (!STREAM) mbar_wait(b_full, 0);
     const int h = lane & 1;      // lanes 0 / 1 of the quad finish rows r0 / r0 + 8
     const int rl = frag_row(h);  // row inside the tile
-    float acc[2][64];
+    float acc[P::ACC_SETS][64];
     uint32_t k = 0;  // ring index of the items with an active sub-space
     for (uint64_t item = blockIdx.x; item < num_tiles * nkc; item += gridDim.x) {
       const uint64_t tile = item / nkc;
       const int kc = (int)(item % nkc);
       const uint32_t cm = chunk_mask(kc);
       if (cm == 0) continue;
-      const uint32_t mine = (k & 1) == (uint32_t)w;
+      const bool mine = k % P::CONSUMERS == w;
       const int s = (int)(k % STAGES);
       const uint32_t ph = (k / STAGES) & 1;
       ++k;
@@ -182,47 +204,18 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
       // |r_m|^2 of the item's four sub-spaces (contiguous, 16-byte aligned: M % 4 == 0), fetched before the MMAs
       float4 rn4 = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
       if (decides) rn4 = *reinterpret_cast<const float4*>(rn2 + row * M + 4 * kc);
-      const float4 cb4 = *reinterpret_cast<const float4*>(cbm_s + 4 * kc);
       mbar_wait(full_bar(s), ph);
       const uint8_t* atile = smem + L.a_off + s * L.stage_bytes;
       const uint8_t* bt = smem + L.b_off + (STREAM ? s * L.stage_bytes : kc * B_CHUNK_BYTES);
       const float* cn4 = reinterpret_cast<const float*>(smem + L.cnh_off + (STREAM ? s * L.stage_bytes : kc * CNH_CHUNK_BYTES));
       const uint32_t a_addr = smem_u32(atile), b_addr = smem_u32(bt);
-      // half `hf` of sub-space j: codewords 128 hf .. 128 hf + 127 are B rows 128 hf.. (128 B each)
-      auto issue = [&](float* d, int j, int hf) {
-        __syncwarp();  // wgmma is warp-aligned: reconverge after the divergent re-rank and barrier polls
-        acc_fence<64>(d);
-        wgmma_fence();
-        wgmma_tf32_n128(d, make_desc(a_addr + j * 32), make_desc(b_addr + hf * (TN / 2) * 128 + j * 32), 0u);
-        wgmma_commit();
-      };
-      uint32_t rest = cm;
-      int j = __ffs(rest) - 1;
-      rest &= rest - 1;
-      issue(acc[0], j, 0);
-      issue(acc[1], j, 1);
-      for (;;) {
+      // flag, exact re-rank and outputs of the row for sub-space j, from its top 3 (mm); no MMA is in flight
+      auto decide = [&](int j, const float (&mm)[3]) {
         const int m = kc * 4 + j;
-        const int jn = rest ? __ffs(rest) - 1 : -1;  // next active sub-space of the item
-        Tour tour;
-        wgmma_wait<1>();
-        acc_fence<64>(acc[0]);
-        top3_half<0>(acc[0], cn4 + j * TN, tour);
-        if (jn >= 0) {
-          issue(acc[0], jn, 0);
-          wgmma_wait<1>();
-        } else {
-          wgmma_wait<0>();
-        }
-        acc_fence<64>(acc[1]);
-        top3_half<1>(acc[1], cn4 + j * TN, tour);
-        float mm[3];
-        top3_finish(tour, mm);
-        wgmma_wait<0>();
         if (decides) {
           const float m1 = mm[0], m2 = mm[1], m3 = mm[2];
           const float rn = j == 0 ? rn4.x : j == 1 ? rn4.y : j == 2 ? rn4.z : rn4.w;
-          const float cbm = j == 0 ? cb4.x : j == 1 ? cb4.y : j == 2 ? cb4.z : cb4.w;
+          const float cbm = cbm_s[m];
           const float tau = 0.0029296875f * (rn + cbm);
           uint32_t flag = 2;
           if (m1 - m2 > tau) flag = 0;
@@ -265,10 +258,63 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
             }
           }
         }
-        if (jn < 0) break;
-        issue(acc[1], jn, 1);
-        j = jn;
+      };
+      // half `hf` of sub-space j into d: codewords 128 hf .. 128 hf + 127 are B rows 128 hf.. (128 B each)
+      auto issue = [&](float* d, int j, int hf) {
+        __syncwarp();  // wgmma is warp-aligned: reconverge after the divergent re-rank and barrier polls
+        acc_fence<64>(d);
+        wgmma_fence();
+        wgmma_tf32_n128(d, make_desc(a_addr + j * 32), make_desc(b_addr + hf * (TN / 2) * 128 + j * 32), 0u);
+        wgmma_commit();
+      };
+      if constexpr (P::ACC_SETS == 2) {
+        // the tournament of half 0 runs while half 1 is in flight, and that of half 1 while the next sub-space's
+        // half 0, issued into the registers just read, is
+        uint32_t rest = cm;
+        int j = __ffs(rest) - 1;
         rest &= rest - 1;
+        issue(acc[0], j, 0);
+        issue(acc[1], j, 1);
+        for (;;) {
+          const int jn = rest ? __ffs(rest) - 1 : -1;  // next active sub-space of the item
+          Tour tour;
+          wgmma_wait<1>();
+          acc_fence<64>(acc[0]);
+          top3_half<0>(acc[0], cn4 + j * TN, tour);
+          if (jn >= 0) {
+            issue(acc[0], jn, 0);
+            wgmma_wait<1>();
+          } else {
+            wgmma_wait<0>();
+          }
+          acc_fence<64>(acc[1]);
+          top3_half<1>(acc[1], cn4 + j * TN, tour);
+          float mm[3];
+          top3_finish(tour, mm);
+          wgmma_wait<0>();
+          decide(j, mm);
+          if (jn < 0) break;
+          issue(acc[1], jn, 1);
+          j = jn;
+          rest &= rest - 1;
+        }
+      } else {
+        // one half at a time, into the same registers
+        for (uint32_t rest = cm; rest; rest &= rest - 1) {
+          const int j = __ffs(rest) - 1;
+          Tour tour;
+          issue(acc[0], j, 0);
+          wgmma_wait<0>();
+          acc_fence<64>(acc[0]);
+          top3_half<0>(acc[0], cn4 + j * TN, tour);
+          issue(acc[0], j, 1);
+          wgmma_wait<0>();
+          acc_fence<64>(acc[0]);
+          top3_half<1>(acc[0], cn4 + j * TN, tour);
+          float mm[3];
+          top3_finish(tour, mm);
+          decide(j, mm);
+        }
       }
       // every MMA of the item has completed (wait_group 0 above) and this warp's re-ranks have read the stage
       __syncwarp();
@@ -486,8 +532,8 @@ void tc_pq_assign(const float* r, const float* rn2, uint64_t n, int d, int M, co
 #define LB2_PQ_FILTER(TRAINV, STREAMV)                                                                      \
   do {                                                                                                      \
     set_smem(tc_pq_kernel<TRAINV, STREAMV>, smem);                                                          \
-    LB2_LAUNCH("tc_pq_filter", (tc_pq_kernel<TRAINV, STREAMV>), grid, tc::NUM_THREADS, smem, map_r, map_b, \
-               n, M, cnh, cbmax2, rn2, row_valid, codes, ids, dists, valid, ws->fb_pairs.p,                 \
+    LB2_LAUNCH("tc_pq_filter", (tc_pq_kernel<TRAINV, STREAMV>), grid, Pipe<STREAMV>::THREADS, smem, map_r,   \
+               map_b, n, M, cnh, cbmax2, rn2, row_valid, codes, ids, dists, valid, ws->fb_pairs.p,          \
                ws->fb_count.p, active);                                                                     \
   } while (0)
   if (codes) {
