@@ -176,13 +176,15 @@ class KMeans:
 
 
 def train_kmeans(array, dimension, k, max_iters=50, redos=1, distance_type="l2", sample_rate=256,
-                 balance_factor=0.0, tolerance=1e-4, seed=0, centroids=None):
-    """lance_index::vector::kmeans::train_kmeans (kmeans.rs:1309-1347)."""
+                 balance_factor=0.0, tolerance=1e-4, seed=0, centroids=None, hierarchical_k=16):
+    """lance_index::vector::kmeans::train_kmeans (kmeans.rs:1309-1347).
+    hierarchical_k: branching of the hierarchical scheme used for k > 256 without `centroids`; 0 or 1 = flat Lloyd."""
     array, dt = _typed(array)
     n = int(np.prod(array.shape)) // dimension
     p = _CKMeansParams()
     lib().lb2_kmeans_params_default(C.byref(p))
     p.max_iters, p.redos, p.sample_rate, p.seed = max_iters, redos, sample_rate, seed
+    p.hierarchical_k = hierarchical_k
     p.balance_factor, p.tolerance, p.metric = balance_factor, tolerance, _metric(distance_type)
     init = None if centroids is None else np.ascontiguousarray(centroids, dtype=_model_np(dt))
     ip, _k0 = as_ptr(init)

@@ -413,7 +413,9 @@ static void assign_dispatch(const float* x, uint64_t n, int d, const float* cent
                             const float* bias, bool bias_padded, uint32_t* part, float* dist,
                             uint8_t* valid, float* all_out, const uint8_t* active, TcWorkspace* ws) {
   if (n == 0) return;
-  if (d % 16 == 0 && d <= 256) {
+  // the tile kernel reads rows as float4: a row base that is not 16-byte aligned (a view into a caller's buffer)
+  // takes the scalar-load generic kernel, which returns the same bits
+  if (d % 16 == 0 && d <= 256 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
     const int Kp = (K + 63) / 64 * 64;
     TcWorkspace local;
     if (!ws) ws = &local;

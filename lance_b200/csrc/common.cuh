@@ -122,10 +122,19 @@ struct LaunchScope {
       ::lb2::fail(LB2_CUDA_ERROR, "launch %s failed: %s", name, cudaGetErrorString(_le)); \
   } while (0)
 
+// The limit is an attribute of the kernel, shared by every host thread: hierarchical training's split workers
+// launch the same kernel with different sizes at once, so the limit only ever rises (under a lock, set before
+// any launch that relies on it) -- lowering it could make another thread's launch fail with "invalid argument".
 template <class K>
 inline void set_smem(K kernel, size_t bytes) {
-  if (bytes > 32 * 1024)  // static shared memory counts against the 48 KB default as well
-    LB2_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  if (bytes <= 32 * 1024) return;  // static shared memory counts against the 48 KB default as well
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, size_t> limit;  // (device, kernel) -> limit set so far
+  std::lock_guard<std::mutex> lk(mu);
+  size_t& cur = limit[{ctx().device, reinterpret_cast<const void*>(kernel)}];
+  if (bytes <= cur) return;
+  LB2_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  cur = bytes;
 }
 
 // ------------------------------------------------------------------------------------------
