@@ -640,9 +640,9 @@ __global__ void reduce_partials_kernel(const uint8_t* __restrict__ gathered, int
   }
 }
 
-// sharded initialisation: the k picked rows are GLOBAL row numbers (rank-major order); every rank copies
-// the rows it owns into a zeroed buffer and the buffers are summed (each row has exactly one owner, x + 0
-// is exact) -- the picks, and with them the model, do not depend on how the sample is sharded
+// initialisation: the k picked rows are GLOBAL row numbers (rank-major order); every rank copies the rows it
+// owns into a zeroed buffer and a sharded run sums the buffers (each row has exactly one owner, x + 0 is exact)
+// -- the picks, and with them the model, do not depend on how the sample is sharded.  One rank owns every row.
 __global__ void gather_init_owned_kernel(const float* __restrict__ x, int ldx, int ds, int K, int B,
                                          const uint32_t* __restrict__ rows, uint32_t row_offset, uint32_t n_local,
                                          float* __restrict__ out) {
@@ -652,28 +652,6 @@ __global__ void gather_init_owned_kernel(const float* __restrict__ x, int ldx, i
   const uint32_t gr = rows[(size_t)b * K + k];
   const bool mine = gr >= row_offset && gr - row_offset < n_local;
   out[g] = mine ? x[(size_t)(gr - row_offset) * ldx + (size_t)b * ds + t] : 0.0f;
-}
-
-__global__ void split_kernel(float* __restrict__ c, int i, int j, int ds) {
-  const float eps = 1.0f / 1024.0f;
-  for (int t = threadIdx.x; t < ds; t += blockDim.x) {
-    const float cj = c[(size_t)j * ds + t];
-    if ((t & 1) == 0) {
-      c[(size_t)i * ds + t] = __fmul_rn(cj, 1.0f + eps);
-      c[(size_t)j * ds + t] = __fmul_rn(cj, 1.0f - eps);
-    } else {
-      c[(size_t)i * ds + t] = __fmul_rn(cj, 1.0f - eps);
-      c[(size_t)j * ds + t] = __fmul_rn(cj, 1.0f + eps);
-    }
-  }
-}
-
-__global__ void gather_init_kernel(const float* __restrict__ x, int ldx, int ds, int K, int B,
-                                   const uint32_t* __restrict__ rows, float* __restrict__ out) {
-  const size_t g = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (g >= (size_t)B * K * ds) return;
-  const int b = g / ((size_t)K * ds), k = (g / ds) % K, t = g % ds;
-  out[g] = x[(size_t)rows[(size_t)b * K + k] * ldx + (size_t)b * ds + t];
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -724,8 +702,7 @@ struct LloydState {  // one per problem, device resident
   float adjusted;     // adjusted_balance_factor (f32::MAX at start)
   float bf_cur;       // balance factor used by the membership step that just ran
   uint64_t rng;       // splitmix64 state
-  uint32_t iters;
-  uint32_t pad;
+  uint32_t iters;     // epilogues run while active
 };
 
 __device__ __forceinline__ uint64_t sm64_next(uint64_t& s) {
@@ -890,16 +867,14 @@ epilogue_kernel(int K, int ds, uint64_t n, float bf_param, double tolerance,
                 uint8_t* __restrict__ active, TcPqPrepArgs pq_prep, volatile uint32_t* host_words) {
   const int b = blockIdx.x;
   if (pq_prep.bm && threadIdx.x == 0) pq_prep.fb_count[b] = 0;  // next iteration's undecided-row list (active or not)
-  if (active[b])
-    epilogue_body<256>(b, K, ds, n, bf_param, tolerance, counts, losses, radius, last_row, cluster_sizes, bias, bias_ld,
-                       centroids, states, active, pq_prep);
+  if (!active[b]) return;
+  epilogue_body<256>(b, K, ds, n, bf_param, tolerance, counts, losses, radius, last_row, cluster_sizes, bias, bias_ld,
+                     centroids, states, active, pq_prep);
   // progress word of problem b in PINNED HOST memory (one posted 4-byte write over PCIe, no copy-engine operation
-  // in the stream): (number of epilogues run so far) << 1 | still active.  The host reads it to stop enqueuing
-  // iterations, without ever draining the stream (lloyd_train).
-  if (host_words && threadIdx.x == 0) {  // thread 0 also wrote active[b] above
-    const uint32_t tick = ++states[b].pad;
-    host_words[b] = (tick << 1) | (active[b] ? 1u : 0u);
-  }
+  // in the stream): iteration << 1 | still active.  Posted only while the problem is active, so the last word is
+  // the one of the iteration that converged it (PollWords).
+  if (threadIdx.x == 0)  // thread 0 wrote iters and active[b] above
+    host_words[b] = (states[b].iters << 1) | (active[b] ? 1u : 0u);
 }
 
 
@@ -1031,23 +1006,76 @@ static bool lloyd_small_ok(uint64_t n, int B, int ds, int K, bool dist) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// the Lloyd loop: no host round trip per iteration; the host only polls the `active` flags
+// the Lloyd loop: no host round trip per iteration; the host only reads the progress words
 // ------------------------------------------------------------------------------------------------
-// per-problem progress words in pinned (device-mapped) host memory, one block per (thread, device), kept for the
-// thread's lifetime: written by epilogue_kernel, read by lloyd_train's host loop
-struct PollWords {
-  static constexpr int LAG = 1, MAX_B = 256;
-  volatile uint32_t* host = nullptr;
-};
-static PollWords* poll_words() {
-  static thread_local std::map<int, PollWords> words;
-  PollWords& r = words[ctx().device];
-  if (!r.host) {
-    void* p = nullptr;
-    LB2_CUDA(cudaHostAlloc(&p, sizeof(uint32_t) * PollWords::MAX_B, cudaHostAllocMapped | cudaHostAllocPortable));
-    r.host = static_cast<volatile uint32_t*>(p);
+// Convergence is learnt WITHOUT draining the stream and without any operation in it: epilogue_kernel posts one
+// word per problem into pinned, device-mapped host memory -- iteration << 1 | active -- for as long as the problem
+// is active, so the last word it ever posts names the iteration that converged it.  After enqueuing iteration it,
+// the host asks whether every problem converged by want = it - 1; the device meanwhile has iteration it queued, and
+// at most one no-op iteration is enqueued past convergence (every kernel returns at once for an inactive problem).
+// The answer depends only on the iteration of convergence, not on when the host reads the word, so every rank of a
+// sharded run (bit-identical states) enqueues the same iterations and none waits in an exchange its peer skipped.
+// (A blocking copy + synchronise every 4 iterations left the GPU idle for a copy and a graph launch each time; an
+// asynchronous copy + event per iteration cost as much in the stream: measured, tools/iter_timing.py.)
+// One block per (thread, device), kept for the thread's lifetime and grown to the largest B it has served.
+class PollWords {
+ public:
+  // the calling thread's words for the current device, reset to 1 (iteration 0, active) for problems 0 .. B-1;
+  // the stream must be idle (no epilogue of an earlier run still to post)
+  static PollWords& reset(int B) {
+    static thread_local std::map<int, PollWords> per_device;
+    PollWords& w = per_device[ctx().device];
+    if (w.cap_ < B) {
+      if (w.host_) LB2_CUDA(cudaFreeHost(const_cast<uint32_t*>(w.host_)));
+      w.host_ = nullptr;
+      w.cap_ = 0;
+      void *p = nullptr, *dp = nullptr;
+      LB2_CUDA(cudaHostAlloc(&p, sizeof(uint32_t) * B, cudaHostAllocMapped | cudaHostAllocPortable));
+      w.host_ = static_cast<volatile uint32_t*>(p);
+      w.cap_ = B;
+      LB2_CUDA(cudaHostGetDevicePointer(&dp, p, 0));
+      w.dev_ = static_cast<uint32_t*>(dp);
+    }
+    for (int b = 0; b < B; ++b) w.host_[b] = 1u;
+    return w;
   }
-  return &r;
+  uint32_t* device() const { return dev_; }
+  // has every problem 0 .. B-1 converged at an iteration <= want?  Waits, for each problem, until its word is of
+  // iteration want or later, or shows it converged.
+  bool done(int B, uint32_t want) const {
+    uint64_t spins = 0;
+    for (int b = 0; b < B; ++b) {
+      uint32_t w;
+      while (!settled(w = host_[b], want)) {
+        if ((++spins & 0xFFFFF) == 0) {  // every ~1M reads: has the stream died or drained without reporting?
+          const cudaError_t q = cudaStreamQuery(ctx().stream);
+          if (q != cudaErrorNotReady) {
+            if (q != cudaSuccess) LB2_CUDA(q);
+            if (!settled(host_[b], want)) fail(LB2_CUDA_ERROR, "k-means progress word %d never arrived", b);
+          }
+        }
+      }
+      if ((w & 1u) || (w >> 1) > want) return false;
+    }
+    return true;
+  }
+
+ private:
+  static bool settled(uint32_t w, uint32_t want) { return !(w & 1u) || (w >> 1) >= want; }
+  volatile uint32_t* host_ = nullptr;
+  uint32_t* dev_ = nullptr;
+  int cap_ = 0;
+};
+
+// element-wise sum of a few host-side counters over the ranks of the current communicator (identity on one GPU)
+static void sum_over_ranks(std::vector<uint32_t>& v) {
+  Comm* cm = current_comm();
+  if (!cm || cm->nranks <= 1 || v.empty()) return;
+  DevBuf<uint32_t> d(v.size());
+  h2d(d.p, v.data(), v.size());
+  comm_allreduce_u32(d.p, v.size(), RedOp::Sum);
+  d2h(v.data(), d.p, v.size());
+  sync_stream();
 }
 
 void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, int metric,
@@ -1066,11 +1094,7 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     n = std::min<uint64_t>(n_in, ((uint64_t)K * 512 + cm->nranks - 1) / cm->nranks);
     std::vector<uint32_t> all(cm->nranks, 0);
     all[cm->rank] = (uint32_t)n;
-    DevBuf<uint32_t> all_d(cm->nranks);
-    h2d(all_d.p, all.data(), cm->nranks);
-    comm_allreduce_u32(all_d.p, cm->nranks, RedOp::Sum);
-    d2h(all.data(), all_d.p, cm->nranks);
-    sync_stream();
+    sum_over_ranks(all);
     n_global = 0;
     for (int r = 0; r < cm->nranks; ++r) {
       if (r < cm->rank) row_offset += all[r];
@@ -1093,7 +1117,6 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     h_states[b].adjusted = std::numeric_limits<float>::max();
     h_states[b].bf_cur = std::fmin(std::numeric_limits<float>::max(), balance_factor_param);
     h_states[b].iters = 0;
-    h_states[b].pad = 0;
   }
   if (init_dev) {
     if (init_dev != centroids) d2d(centroids, init_dev, BK * ds);
@@ -1104,7 +1127,6 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     // Sharded: the picks range over the GLOBAL rows (rank-major), see gather_init_owned_kernel.
     std::vector<uint32_t> rows(BK);
     std::unordered_map<uint64_t, uint32_t> moved;
-    const uint64_t n_pick = dist ? n_global : n;
     for (int b = 0; b < B; ++b) {
       SplitMix64 rng(seed + b);
       moved.clear();
@@ -1113,7 +1135,7 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
         return it == moved.end() ? (uint32_t)i : it->second;
       };
       for (int i = 0; i < K; ++i) {
-        const uint64_t j = i + rng.next() % (n_pick - i);
+        const uint64_t j = i + rng.next() % (n_global - i);
         const uint32_t vi = at(i), vj = at(j);
         moved[i] = vj;
         moved[j] = vi;
@@ -1123,14 +1145,9 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     }
     DevBuf<uint32_t> rows_d(BK);
     h2d(rows_d.p, rows.data(), BK);
-    if (!dist) {
-      LB2_LAUNCH("kmeans_init", gather_init_kernel, cdiv(BK * ds, 256), 256, 0, x, ldx, ds, K, B,
-                 rows_d.p, centroids);
-    } else {
-      LB2_LAUNCH("kmeans_init", gather_init_owned_kernel, cdiv(BK * ds, 256), 256, 0, x, ldx, ds, K, B,
-                 rows_d.p, (uint32_t)row_offset, (uint32_t)n, centroids);
-      comm_allreduce_f32(centroids, BK * ds, RedOp::Sum);
-    }
+    LB2_LAUNCH("kmeans_init", gather_init_owned_kernel, cdiv(BK * ds, 256), 256, 0, x, ldx, ds, K, B, rows_d.p,
+               (uint32_t)row_offset, (uint32_t)n, centroids);
+    if (dist) comm_allreduce_f32(centroids, BK * ds, RedOp::Sum);
     sync_stream();  // rows (host vector) must outlive the copy
   }
 
@@ -1143,8 +1160,20 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
   DevBuf<LloydState> states(B);
   cluster_sizes.zero();
   h2d(states.p, h_states.data(), B);
-  std::vector<uint8_t> active(B, 1);
-  h2d(active_d.p, active.data(), B);
+  LB2_CUDA(cudaMemsetAsync(active_d.p, 1, B, ctx().stream));
+  // the trained model is in `centroids`; the loss and iteration count of every problem come back here
+  auto read_back = [&]() {
+    d2h(h_states.data(), states.p, B);
+    sync_stream();
+    if (loss_out) {
+      loss_out->resize(B);
+      for (int b = 0; b < B; ++b) (*loss_out)[b] = h_states[b].last_loss;
+    }
+    if (iters_out) {
+      iters_out->resize(B);
+      for (int b = 0; b < B; ++b) (*iters_out)[b] = h_states[b].iters;
+    }
+  };
   if (!small) {
     bias.alloc(Kp);
     bias.zero();  // iteration 1: cluster sizes are all zero -> bias 0
@@ -1180,10 +1209,7 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     } while (0)
     if (metric == METRIC_DOT) LB2_SMALL(METRIC_DOT); else LB2_SMALL(METRIC_L2);
 #undef LB2_SMALL
-    d2h(h_states.data(), states.p, B);
-    sync_stream();
-    if (loss_out) loss_out->assign(1, h_states[0].last_loss);
-    if (iters_out) iters_out->assign(1, h_states[0].iters);
+    read_back();
     return;
   }
   TcWorkspace tcws;
@@ -1198,21 +1224,7 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     pq_prep = tc_pq_prep_args(B, ldx, &pqws);
   }
   sync_stream();
-
-  // progress words in pinned host memory (see "Convergence is polled" below)
-  static const bool blocking_poll = getenv("LB2_BLOCKING_POLL") && *getenv("LB2_BLOCKING_POLL");
-  // Single-rank runs only.  The host may read a word late and see the active bit of a LATER iteration than the one
-  // it waited for: harmless alone (it just stops a no-op earlier), but two ranks of a sharded run could then enqueue
-  // different numbers of iterations -- and the exchange inside the extra one would wait forever.  Sharded runs keep
-  // the blocking poll, which reads the flags of exactly iteration `it` on every rank.
-  PollWords* words = B <= PollWords::MAX_B && !blocking_poll && !ctx().profiling && !dist ? poll_words() : nullptr;
-  volatile uint32_t* words_dev = nullptr;
-  if (words) {
-    for (int b = 0; b < B; ++b) words->host[b] = 0;  // (the previous run of this thread ended with a synchronise)
-    void* dp = nullptr;
-    LB2_CUDA(cudaHostGetDevicePointer(&dp, const_cast<uint32_t*>(words->host), 0));
-    words_dev = static_cast<volatile uint32_t*>(dp);
-  }
+  const PollWords& words = PollWords::reset(B);  // (after the synchronise: no earlier epilogue still posts)
   // one Lloyd iteration = ~18 short kernels: membership, member sort, stats, update, scalar epilogue
   auto iteration = [&]() {
     if (!small) {
@@ -1233,15 +1245,6 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     const int warp_update = (ds % 8 == 0 && ldx % 4 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) ? 1 : 0;
     const unsigned ub = warp_update ? cdiv(BK * (uint64_t)(ds / 8), 4) : cdiv(BK * ds, 128);
     const unsigned sb = cdiv((uint64_t)BK * 32, 128);
-    static const bool split_us = getenv("LB2_SPLIT_UPDATE_STATS") && *getenv("LB2_SPLIT_UPDATE_STATS");
-    if (split_us) {  // diagnostics: time the two halves of the fused launch separately
-      LB2_LAUNCH("kmeans_update_only", update_stats_kernel, ub, 128, 0, ub, x, ldx, ds, K, B, n,
-                 ms.members.p, ms.offsets.p, dist ? sums_p : centroids, dists.p, losses.p, radius.p,
-                 last_row.p, active_d.p, dist ? 0 : 1, warp_update, hints.p);
-      LB2_LAUNCH("kmeans_stats_only", update_stats_kernel, sb, 128, 0, 0u, x, ldx, ds, K, B, n,
-                 ms.members.p, ms.offsets.p, dist ? sums_p : centroids, dists.p, losses.p, radius.p,
-                 last_row.p, active_d.p, dist ? 0 : 1, warp_update, hints.p);
-    } else
     LB2_LAUNCH("kmeans_update_stats", update_stats_kernel, ub + sb, 128, 0, ub, x, ldx, ds, K, B, n,
                ms.members.p, ms.offsets.p, dist ? sums_p : centroids, dists.p, losses.p, radius.p,
                last_row.p, active_d.p, dist ? 0 : 1, warp_update, hints.p);
@@ -1254,58 +1257,25 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     }
     LB2_LAUNCH("kmeans_epilogue", epilogue_kernel, B, 256, 0, K, ds, n_global, balance_factor_param,
                tolerance, ms.counts.p, losses.p, radius.p, last_row.p, cluster_sizes.p,
-               small ? nullptr : bias.p, Kp, centroids, states.p, active_d.p, pq_prep, words_dev);
+               small ? nullptr : bias.p, Kp, centroids, states.p, active_d.p, pq_prep, words.device());
   };
   // The first iteration runs eagerly (allocates every workspace, sets kernel attributes); the
   // iteration is then captured ONCE into a CUDA graph and replayed, so that the loop is not bound
   // by ~18 host launches per iteration.  (Event profiling and LB2_TC_STATS need eager launches.)
-  const bool stats_env = getenv("LB2_TC_STATS") && *getenv("LB2_TC_STATS");
   // (NCCL collectives are capturable; the sharded iteration is replayed from the graph like the local one)
   // (eager launches for the small splits of hierarchical training were tried and lose: 577 vs 481 ms for a
-  // K = 8192 tree -- the loop is bound by host launch throughput, which is what the graph relieves;
-  // LB2_GRAPH_MIN_ROWS=<rows> restores eager launches below that size)
-  const char* graph_min = getenv("LB2_GRAPH_MIN_ROWS");
-  const uint64_t graph_rows = graph_min && *graph_min ? strtoull(graph_min, nullptr, 10) : 0;
-  const bool use_graph = max_iters > 1 && !ctx().profiling && !stats_env && (dist || n * (uint64_t)B >= graph_rows) &&
+  // K = 8192 tree -- the loop is bound by host launch throughput, which is what the graph relieves)
+  const bool use_graph = max_iters > 1 && !ctx().profiling && !(getenv("LB2_TC_STATS") && *getenv("LB2_TC_STATS")) &&
                          !(getenv("LB2_NO_GRAPH") && *getenv("LB2_NO_GRAPH"));
-  cudaGraph_t graph = nullptr;
-  cudaGraphExec_t exec = nullptr;
-  uint64_t graph_nodes = 0;
-  auto poll_done = [&]() {
-    d2h(active.data(), active_d.p, B);
-    sync_stream();
-    for (int b = 0; b < B; ++b)
-      if (active[b]) return false;
-    return true;
-  };
-  // Convergence is polled WITHOUT draining the stream and without any operation in it: the epilogue kernel of every
-  // iteration posts one progress word per problem -- (epilogues run) << 1 | active -- into pinned host memory,
-  // and after enqueuing iteration `it` the host waits (plain memory reads) until every problem has reported
-  // iteration it - LAG, then looks at the active bits.  The device therefore always has the next iteration queued.
-  // (A blocking copy + synchronise every 4 iterations left the GPU idle for a copy and a graph launch each time;
-  // an asynchronous copy + event per iteration cost as much in the stream: measured, tools/iter_timing.py.)
-  // Iterations enqueued past convergence are no-ops: every kernel of an iteration returns at once for a problem
-  // whose `active` flag is 0.  (Event profiling keeps the blocking poll: launch counts are then those of real
-  // iterations; so do sharded runs, see `words` above.)
-  auto words_done = [&](int it) {
-    const uint32_t want = (uint32_t)it;
-    uint64_t spins = 0;
-    bool any_active = false;
-    for (int b = 0; b < B; ++b) {
-      uint32_t w;
-      while (((w = words->host[b]) >> 1) < want) {
-        if ((++spins & 0xFFFFF) == 0) {  // every ~1M reads: has the stream died or drained without reporting?
-          const cudaError_t q = cudaStreamQuery(ctx().stream);
-          if (q != cudaErrorNotReady) {
-            if (q != cudaSuccess) LB2_CUDA(q);
-            if ((words->host[b] >> 1) < want) fail(LB2_CUDA_ERROR, "k-means progress word %d never arrived", b);
-          }
-        }
-      }
-      any_active |= (w & 1u) != 0;
+  struct Graph {  // the captured iteration, released on every way out of lloyd_train
+    cudaGraph_t graph = nullptr;
+    cudaGraphExec_t exec = nullptr;
+    ~Graph() {
+      if (exec) cudaGraphExecDestroy(exec);
+      if (graph) cudaGraphDestroy(graph);
     }
-    return !any_active;
-  };
+  } g;
+  uint64_t graph_nodes = 0;
   iteration();
   bool done = max_iters == 1;
   if (!done && use_graph) {
@@ -1314,40 +1284,24 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     try {
       iteration();
     } catch (...) {
-      cudaStreamEndCapture(ctx().stream, &graph);
-      if (graph) cudaGraphDestroy(graph);
+      cudaStreamEndCapture(ctx().stream, &g.graph);
       throw;
     }
-    LB2_CUDA(cudaStreamEndCapture(ctx().stream, &graph));
+    LB2_CUDA(cudaStreamEndCapture(ctx().stream, &g.graph));
     graph_nodes = ctx().launches - l0;
     ctx().launches = l0;
-    LB2_CUDA(cudaGraphInstantiate(&exec, graph, 0));
+    LB2_CUDA(cudaGraphInstantiate(&g.exec, g.graph, 0));
   }
   for (int it = 2; it <= max_iters && !done; ++it) {
-    if (exec) {
-      LB2_CUDA(cudaGraphLaunch(exec, ctx().stream));
+    if (g.exec) {
+      LB2_CUDA(cudaGraphLaunch(g.exec, ctx().stream));
       ctx().launches += graph_nodes;
     } else {
       iteration();
     }
-    if (words) {
-      if (it - PollWords::LAG >= 1) done = words_done(it - PollWords::LAG);
-    } else if ((it & 3) == 0 || it == max_iters) {
-      done = poll_done();  // blocking poll every 4 iterations
-    }
+    done = words.done(B, (uint32_t)it - 1);  // (see PollWords)
   }
-  if (exec) cudaGraphExecDestroy(exec);
-  if (graph) cudaGraphDestroy(graph);
-  d2h(h_states.data(), states.p, B);
-  sync_stream();
-  if (loss_out) {
-    loss_out->resize(B);
-    for (int b = 0; b < B; ++b) (*loss_out)[b] = h_states[b].last_loss;
-  }
-  if (iters_out) {
-    iters_out->resize(B);
-    for (int b = 0; b < B; ++b) (*iters_out)[b] = h_states[b].iters;
-  }
+  read_back();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1531,29 +1485,15 @@ void hierarchical_train(const float* x, uint64_t n, int d, int K, int metric, fl
   Comm* cm = current_comm();
   const bool dist = cm && cm->nranks > 1;
   LB2_REQUIRE(n < 0xffffffffull, "KMeans: too many vectors");
-  const int kmax = std::max(std::min(hk, K), hk);
-  DevBuf<uint32_t> cnt_d(kmax);
   // local per-cluster counts -> global counts (identity on one GPU)
   auto global_counts = [&](const std::vector<uint32_t>& local, int k, std::vector<uint64_t>& out) {
-    out.assign(k, 0);
-    if (!dist) {
-      for (int i = 0; i < k; ++i) out[i] = local[i];
-      return;
-    }
-    std::vector<uint32_t> tmp(local.begin(), local.begin() + k);
-    h2d(cnt_d.p, tmp.data(), k);
-    comm_allreduce_u32(cnt_d.p, k, RedOp::Sum);
-    d2h(tmp.data(), cnt_d.p, k);
-    sync_stream();
-    for (int i = 0; i < k; ++i) out[i] = tmp[i];
+    std::vector<uint32_t> sum(local.begin(), local.begin() + k);
+    sum_over_ranks(sum);
+    out.assign(sum.begin(), sum.end());
   };
-  uint64_t n_global = n;
-  {
-    std::vector<uint32_t> one(1, (uint32_t)n);
-    std::vector<uint64_t> g;
-    global_counts(one, 1, g);
-    n_global = g[0];
-  }
+  std::vector<uint32_t> n_sum(1, (uint32_t)n);
+  sum_over_ranks(n_sum);
+  const uint64_t n_global = n_sum[0];
   LB2_REQUIRE(n_global >= (uint64_t)K, "KMeans: can not train %d centroids with %llu vectors", K,
               (unsigned long long)n_global);
   const int k0 = (int)std::min<uint64_t>(std::min(hk, K), n_global);

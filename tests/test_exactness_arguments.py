@@ -5,13 +5,14 @@
    integer multiple of 2^g and sum|term| < 2^(g+p) (p = 24 for f32, 53 for f64) no addition of ANY association rounds,
    so a parallel tree reduction returns the sequential result bit for bit.  Outside the condition it does not.
 
-2. Convergence polling through progress words (DESIGN.md section 3; kmeans.cu `PollWords`, `lloyd_train`): after
-   enqueuing iteration `it` the host waits until the problem has reported iteration it - 1, then reads the active
-   bit.  A thread-per-rank simulation checks (a) that a single rank always stops, at most one no-op iteration late,
-   however late it reads; (b) WHY sharded runs keep the blocking poll: a rank that reads late sees a later
-   iteration's bit, enqueues fewer iterations than its peer, and the peer's next collective never completes; (c) that
-   reporting the TICK OF CONVERGENCE instead of the current bit would make the decision independent of read timing
-   (the design noted for sharded runs in DESIGN.md section 8; not built)."""
+2. Convergence through progress words (DESIGN.md section 3; kmeans.cu `PollWords`, `epilogue_kernel`): a problem
+   posts iteration << 1 | active only while it is active, so its last word names the iteration that converged it;
+   the host resets the word to 1 and, after enqueuing iteration `it`, stops once every problem converged at an
+   iteration <= it - 1.  A thread-per-rank simulation checks (a) that a single rank always stops, at most one no-op
+   iteration late, however late it reads; (b) WHY the word is frozen at convergence rather than the current active
+   bit read: a rank that reads the current bit late sees a later iteration's bit, enqueues fewer iterations than its
+   peer, and the peer's next collective never completes; (c) that with the frozen word ranks reading late enqueue the
+   same iterations and never hang."""
 import threading
 import time
 
@@ -85,24 +86,42 @@ def test_outside_the_condition_the_order_matters():
     assert _seq_sum(big, np.float32) != np.float32(big.sum(dtype=np.float64)) or _tree_sum(big, np.float32) != _seq_sum(big, np.float32)
 
 
+def _settled(word, want, mode):
+    """PollWords::done waits on a problem until this holds"""
+    if mode == "frozen":
+        return not (word & 1) or (word >> 1) >= want
+    return (word >> 1) >= want
+
+
+def _converged_by(word, want, mode):
+    """the host's decision for one problem once its word has settled"""
+    if mode == "frozen":
+        return not (word & 1) and (word >> 1) <= want
+    return not (word & 1)
+
+
 class _Rank:
     """one rank of the simulation: a `device` thread executes enqueued iterations in order (each takes `iter_s`);
-    iteration j contains the collective of iteration j, i.e. it needs every rank's device to reach it (a barrier);
-    its epilogue posts conv (the tick at which the problem became inactive, 0 while active) and then the progress
-    word (tick << 1 | active).  The host loop is lloyd_train's; `late_by` makes the host read only once the device is
-    that many iterations further than it had to wait for (pre-emption, a slow graph launch, a CPU quota ...) --
-    scripted in ticks, not in seconds, so that the tests do not depend on the machine's speed."""
+    iteration j contains the collective of iteration j, i.e. it needs every rank's device to reach it (a barrier).
+    Its epilogue posts the progress word of `mode`:
+      * "frozen" (what lloyd_train does): j << 1 | active, posted only while the problem is active, so the last word
+        names the iteration that converged it; the host resets the word to 1 (iteration 0, active) before iteration 1;
+      * "current_bit": (epilogues run) << 1 | active, posted by every epilogue; the host resets it to 0.
+    The host loop is lloyd_train's; `late_by` makes the host read only once the device is that many iterations
+    further than it had to wait for (pre-emption, a slow graph launch, a CPU quota ...) -- scripted in ticks, not in
+    seconds, so that the tests do not depend on the machine's speed."""
 
     def __init__(self, world, barrier_for, converge_at, max_iters, mode, late_by=0, iter_s=0.0):
         self.world, self.barrier_for, self.converge_at, self.max_iters = world, barrier_for, converge_at, max_iters
         self.mode, self.late_by, self.iter_s = mode, late_by, iter_s
         self.queue, self.cv = [], threading.Condition()
-        self.word = self.conv = self.enqueued = self.executed_active = 0
-        self.hist = {0: (0, 0)}                        # tick -> (word, conv) as posted at that tick
+        self.word = 1 if mode == "frozen" else 0
+        self.executed = self.enqueued = self.executed_active = 0
+        self.hist = {0: self.word}                     # iteration -> the word once that iteration has run
         self.stop = self.hung = False
 
     def device(self):
-        active, tick = True, 0
+        active = True
         while True:
             with self.cv:
                 while not self.queue and not self.stop:
@@ -116,15 +135,14 @@ class _Rank:
                 self.hung = True                       # a peer never enqueued iteration j: NCCL would wait forever
                 return
             time.sleep(self.iter_s)
+            posts = active or self.mode == "current_bit"
             if active:
                 self.executed_active += 1
-                if j >= self.converge_at:              # kmeans.rs:704 on identical models: same j on every rank
-                    active = False
-            tick += 1
-            if not active and self.conv == 0:
-                self.conv = tick                       # written BEFORE the word (fence in between on the device)
-            self.hist[tick] = ((tick << 1) | int(active), self.conv)
-            self.word = (tick << 1) | int(active)
+                active = j < self.converge_at          # kmeans.rs:704 on identical models: same j on every rank
+            word = (j << 1) | int(active) if posts else self.word
+            self.hist[j] = word
+            self.executed = j
+            self.word = word
 
     def host(self):
         def launch(j):
@@ -138,26 +156,22 @@ class _Rank:
             launch(it)
             want = it - 1
             t0 = time.monotonic()
-            while (self.word >> 1) < want and not self.hung:   # (the real host spins; here it yields the interpreter lock)
+            while not _settled(self.word, want, self.mode) and not self.hung:  # (the real host spins)
                 time.sleep(0.0001)
                 assert time.monotonic() - t0 < 20, "progress word never arrived"
-            seen = min(want + self.late_by, self.enqueued)     # the tick whose posting this (late) read observes
+            seen = min(want + self.late_by, self.enqueued)     # the iteration whose word this (late) read observes
             t1 = time.monotonic()
-            while (self.word >> 1) < seen and not self.hung and time.monotonic() - t1 < 6.0:
+            while self.executed < seen and not self.hung and time.monotonic() - t1 < 6.0:
                 time.sleep(0.0001)
-            word, conv = self.hist[min(seen, self.word >> 1)]
-            if self.mode == "active_bit":
-                done = (word & 1) == 0                         # what is built (single rank)
-            else:
-                done = conv != 0 and conv <= want              # independent of WHEN the host reads
+            done = _converged_by(self.hist[min(seen, self.executed)], want, self.mode)
             it += 1
         t0 = time.monotonic()
-        while (self.word >> 1) < self.enqueued and not self.hung and time.monotonic() - t0 < 8:
+        while self.executed < self.enqueued and not self.hung and time.monotonic() - t0 < 8:
             time.sleep(0.0001)                                 # the final synchronise of lloyd_train
         self.stop = True
 
 
-def _simulate(world, converge_at, max_iters, mode="active_bit", late=None, iter_s=0.0):
+def _simulate(world, converge_at, max_iters, mode="frozen", late=None, iter_s=0.0):
     barriers, lock = {}, threading.Lock()
 
     def barrier_for(j):
@@ -176,26 +190,39 @@ def _simulate(world, converge_at, max_iters, mode="active_bit", late=None, iter_
     return ranks
 
 
+def test_the_reset_word_reads_as_active_and_a_zero_would_read_as_converged():
+    for want in range(1, 6):
+        assert not _settled(1, want, "frozen") and not _converged_by(1, want, "frozen")
+        assert _settled(0, want, "frozen") and _converged_by(0, want, "frozen")
+
+
 def test_single_rank_always_stops_at_most_one_noop_late_whatever_the_read_timing():
-    for converge_at, max_iters, late in ((7, 50, 0), (7, 50, 1), (1, 50, 0), (50, 50, 0), (60, 50, 1), (3, 4, 0), (1, 1, 0)):
-        r, = _simulate(1, converge_at, max_iters, late=[late], iter_s=0.0005)
-        last_real = min(converge_at, max_iters)
-        assert not r.hung and r.executed_active == last_real            # extra iterations were no-ops
-        assert last_real <= r.enqueued <= min(max_iters, last_real + 1)
+    for mode in ("frozen", "current_bit"):
+        for converge_at, max_iters, late in ((7, 50, 0), (7, 50, 1), (7, 50, 3), (1, 50, 0), (50, 50, 0), (60, 50, 1),
+                                             (3, 4, 0), (2, 4, 1), (1, 1, 0)):
+            r, = _simulate(1, converge_at, max_iters, mode=mode, late=[late], iter_s=0.0005)
+            last_real = min(converge_at, max_iters)
+            assert not r.hung and r.executed_active == last_real            # extra iterations were no-ops
+            assert last_real <= r.enqueued <= min(max_iters, last_real + 1)
+            if mode == "frozen":                                            # and the count does not depend on timing
+                assert r.enqueued == min(max_iters, last_real + 1)
 
 
-def test_two_ranks_reading_the_current_bit_can_diverge_which_is_why_sharded_runs_poll_blocking():
+def test_two_ranks_reading_the_current_bit_can_diverge_which_is_why_the_word_freezes_at_convergence():
     # rank 0 reads one iteration late: waiting for iteration 4 it already sees iteration 5's bit and stops after
     # enqueuing 5; rank 1 sees that bit one check later, after enqueuing 6 -- whose collective rank 0 never joins
-    ranks = _simulate(2, 5, 50, mode="active_bit", late=[1, 0], iter_s=0.0005)
+    ranks = _simulate(2, 5, 50, mode="current_bit", late=[1, 0], iter_s=0.0005)
     assert ranks[0].enqueued == 5 and ranks[1].enqueued == 6 and ranks[1].hung
 
 
 def test_reporting_the_tick_of_convergence_is_independent_of_read_timing():
-    for late in ([1, 0], [0, 1, 0], [1, 1]):
-        ranks = _simulate(len(late), 5, 50, mode="conv_tick", late=late, iter_s=0.0005)
+    for converge_at, max_iters, late in ((5, 50, [1, 0]), (5, 50, [0, 1, 0]), (5, 50, [1, 1]), (5, 50, [3, 0]),
+                                         (2, 50, [0, 2]), (3, 4, [1, 0]), (9, 6, [2, 0, 1])):
+        ranks = _simulate(len(late), converge_at, max_iters, late=late, iter_s=0.0005)
+        last_real = min(converge_at, max_iters)
         assert not any(r.hung for r in ranks)
-        assert {r.enqueued for r in ranks} == {6} and all(r.executed_active == 5 for r in ranks)
+        assert {r.enqueued for r in ranks} == {min(max_iters, last_real + 1)}
+        assert all(r.executed_active == last_real for r in ranks)
 
 
 # ---- 3. the k + 1 rule of every top-k path (DESIGN.md section 5 "Ties at the k-th distance"; search.cu) ----------

@@ -5,8 +5,9 @@ for bit to the CPU oracle.
 centroid bits, the same f64 loss and the same iteration count.  It reaches that promise by many routes:
   * fused: the whole run in one `lloyd_small_kernel` launch (K <= 16, n <= 16384, n*K*d <= 2^20, not profiling);
   * multi-kernel: one iteration = assignment, member sort, `update_stats_kernel`, `epilogue_kernel`, replayed from a
-    CUDA graph (default), launched eagerly with polled progress words (LB2_NO_GRAPH=1), or launched eagerly with a
-    blocking poll every 4 iterations (profiling on, which also turns the fused kernel off);
+    CUDA graph (default), launched eagerly (LB2_NO_GRAPH=1), or launched eagerly with event profiling on (which also
+    turns the fused kernel off); every one stops on the progress words at most one no-op iteration past convergence,
+    which the profiled run checks by counting launches;
   * centroid sums by one warp per (cluster, 8 dims) (`update_body_warp`: d % 8 == 0 and 16-byte aligned rows) or
     one thread per (cluster, dim) (`update_body`);
   * order-independent fast paths for the centroid sums and the f64 loss, which must reject any cluster whose sum
@@ -95,7 +96,10 @@ def _check_flat(data, d, k, *, fused, host=None, modes=MODES, **kw):
         prof = p if p is not None else prof
     if prof is not None:
         assert _count(prof, "kmeans_small_fused") == 0
-        assert _count(prof, "kmeans_update_stats") >= ref[2]
+        # at most one no-op iteration past convergence (several cases converge at iteration 5 or 9 well below
+        # max_iters, where stopping only at a multiple of 4 would launch more)
+        for name in ("kmeans_update_stats", "kmeans_epilogue"):
+            assert ref[2] <= _count(prof, name) <= ref[2] + 1, (name, _count(prof, name), ref[2])
         sort = "member_sort_cluster" if k <= 1024 else "member_sort"
         other = "member_sort" if k <= 1024 else "member_sort_cluster"
         assert _count(prof, sort) >= ref[2] and _count(prof, other) == 0
@@ -356,8 +360,10 @@ def _check_pq(data, M, nbits, metric, init=None, seed=0, max_iters=10):
         assert np.array_equal(pq.train_iters.astype(np.int32), iters_o)
         assert np.array_equal(_bits(pq.codebook), _bits(cbo))
     prof = lb.profile.dump()
-    assert _count(prof, "pq_assign_exact") > 0 and _count(prof, "kmeans_update_stats") > 0
-    assert _count(prof, "tc_pq_filter") == 0
+    assert _count(prof, "pq_assign_exact") > 0 and _count(prof, "tc_pq_filter") == 0
+    last = int(iters_o.max())  # the loop runs until the last sub-space converges, plus at most one no-op iteration
+    for name in ("kmeans_update_stats", "kmeans_epilogue"):
+        assert last <= _count(prof, name) <= last + 1, (name, _count(prof, name), last)
     return iters_o
 
 
@@ -366,6 +372,27 @@ def test_pq_narrow_and_wide_subvectors(ds, seeded):
     M, n = 4, 3000
     data = synth.gaussian_mixture(n, M * ds, n_components=300, seed=40 + ds)
     _check_pq(data, M, 8, "l2", init=None if seeded else _pq_init(data, M, 256, ds), seed=ds)
+
+
+@pytest.mark.parametrize("kind", ["mixture", "converging"])
+def test_pq_more_than_256_sub_spaces(kind):
+    """384 sub-spaces of width 2: more than 256 problems, and progress words, in one Lloyd loop.  mixture: every
+    sub-space runs to max_iters; converging: 256 groups per sub-space around the initial codewords, the noise growing
+    from sub-space to sub-space, so they converge at iterations 3 to 10 and the loop stops on the last of them"""
+    M, ds, n, K = 384, 2, 3000, 256
+    if kind == "mixture":
+        data = synth.gaussian_mixture(n, M * ds, n_components=300, seed=47)
+        iters = _check_pq(data, M, 8, "l2", seed=7)
+        assert (iters == 10).all()
+        return
+    rng = np.random.default_rng(47)
+    centers = (rng.standard_normal((M, K, ds)) * 50).astype(np.float32)
+    sigma = np.geomspace(1e-3, 1.0, M).astype(np.float32)
+    pick = rng.integers(0, K, (n, M))
+    noise = rng.standard_normal((n, M, ds)).astype(np.float32) * sigma[None, :, None]
+    data = np.ascontiguousarray((centers[np.arange(M)[None, :], pick] + noise).reshape(n, M * ds), np.float32)
+    iters = _check_pq(data, M, 8, "l2", init=centers, max_iters=16)
+    assert iters.min() < iters.max() < 15, iters
 
 
 def test_pq_dot_8_wide():
