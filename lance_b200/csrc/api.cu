@@ -900,7 +900,8 @@ static std::vector<uint64_t> sample_rows(uint64_t n, uint64_t s, uint64_t seed) 
   return out;
 }
 
-// one pass over a caller's matrix in chunks of rows: f(xf, r0, rows) with xf = the chunk as f32 on the device
+// one pass over a caller's matrix in chunks of rows: f(xf, xnat, r0, rows) with xf = the chunk as f32 on the device
+// and xnat = the same rows in the column's own type (for assign_f32: tc_assign.cu, "native 16-bit rows")
 template <class F>
 static void for_each_chunk(Source& src, F&& f) {
   const uint64_t n = src.n(), chunk = src.rows_per_chunk();
@@ -910,10 +911,7 @@ static void for_each_chunk(Source& src, F&& f) {
     const uint64_t rows = std::min(step, n - r0);
     const float* xf = src.rows_f32(r0, rows);
     if (r0 + rows < n) src.prefetch(r0 + rows, std::min(step, n - r0 - rows));
-    // f16 / bf16 columns: the tensor-core filter reads the native rows (tc_assign.cu, "native 16-bit rows")
-    tc_set_operand_hint(xf, src.last_native(), (int)src.dtype(), (size_t)rows * src.d());
-    f(xf, r0, rows);
-    tc_set_operand_hint(nullptr, nullptr, 0, 0);
+    f(xf, src.last_native(), r0, rows);
   }
 }
 
@@ -922,16 +920,19 @@ static void for_each_chunk(Source& src, F&& f) {
 // trained -- and therefore encodes -- with L2 whatever the index metric is: Q::build(&training_data,
 // DistanceType::L2, ..) (rust/lance/src/index/vector/builder.rs:460); the index metric only decides the partition
 // assignment, whether residuals are taken (not for dot, PQBuildParams::use_residual) and the query-time table.
-static void transform_chunk(const float* xf, uint64_t rows, int d, int m, const float* cent, int K, const float* codebook,
-                            int M, int nbits, DevBuf<float>& normbuf, uint32_t* part, uint8_t* codes, uint8_t* valid) {
+// xnat / dtype: the chunk's rows in their own type (for_each_chunk); a normalised chunk is assigned from f32 only
+static void transform_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m, const float* cent,
+                            int K, const float* codebook, int M, int nbits, DevBuf<float>& normbuf, uint32_t* part,
+                            uint8_t* codes, uint8_t* valid) {
   const float* xp = xf;
   if (m == METRIC_COSINE) {
     if (normbuf.n < (size_t)rows * d) normbuf.alloc((size_t)rows * d);
     LB2_LAUNCH("normalize", normalize_kernel, cdiv(rows, 128), 128, 0, xf, rows, d, normbuf.p);
     xp = normbuf.p;
+    xnat = nullptr;
   }
   const int am = m == METRIC_DOT ? METRIC_DOT : METRIC_L2;
-  assign_f32(xp, rows, d, cent, K, am, nullptr, part, nullptr, valid, nullptr);
+  assign_f32(xp, rows, d, cent, K, am, nullptr, part, nullptr, valid, nullptr, xnat, dtype);
   pq_encode_any(xp, rows, d, M, d / M, codebook, METRIC_L2, am == METRIC_DOT ? nullptr : cent,
                 am == METRIC_DOT ? nullptr : part, valid, nbits, codes);
 }
@@ -1192,9 +1193,9 @@ lb2_status lb2_compute_partitions(const void* centroids, uint32_t k, uint32_t d,
   if (n) {
     Source src(vectors, n, (int)d, dtype);
     src.start_resident_copy();
-    for_each_chunk(src, [&](const float* xf, uint64_t r0, uint64_t rows) {
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
       assign_f32(xf, rows, d, c.get(), k, m, nullptr, p.get() + r0, dd.get() ? dd.get() + r0 : nullptr,
-                 v.get() ? v.get() + r0 : nullptr, nullptr);
+                 v.get() ? v.get() + r0 : nullptr, nullptr, xnat, (int)src.dtype());
     });
   }
   p.commit(); dd.commit(); v.commit();
@@ -1387,9 +1388,9 @@ lb2_status lb2_ivfpq_transform(const void* centroids, uint32_t k, const void* co
     Source src(vectors, n, (int)d, dtype);
     src.start_resident_copy();
     DevBuf<float> normbuf;
-    for_each_chunk(src, [&](const float* xf, uint64_t r0, uint64_t rows) {
-      transform_chunk(xf, rows, (int)d, m, c.get(), (int)k, cb.get(), M, (int)num_bits, normbuf, p.get() + r0,
-                      co.get() + r0 * cw, vp + r0);
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, c.get(), (int)k, cb.get(), M, (int)num_bits, normbuf,
+                      p.get() + r0, co.get() + r0 * cw, vp + r0);
     });
   }
   p.commit(); co.commit(); v.commit();
@@ -2074,14 +2075,16 @@ lb2_status lb2_ivfflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype
   {
     TagScope tg("transform");
     DevBuf<float> normbuf;
-    for_each_chunk(src, [&](const float* xf, uint64_t r0, uint64_t rows) {
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
       const float* xp = xf;
       if (m == METRIC_COSINE) {  // NormalizeTransformer first (ivf.rs:158-166)
         if (normbuf.n < (size_t)rows * d) normbuf.alloc((size_t)rows * d);
         LB2_LAUNCH("normalize", normalize_kernel, cdiv(rows, 128), 128, 0, xf, rows, (int)d, normbuf.p);
         xp = normbuf.p;
+        xnat = nullptr;
       }
-      assign_f32(xp, rows, d, ix->centroids.p, K, am, nullptr, part.p + r0, nullptr, valid.p + r0, nullptr);
+      assign_f32(xp, rows, d, ix->centroids.p, K, am, nullptr, part.p + r0, nullptr, valid.p + r0, nullptr, xnat,
+                 (int)src.dtype());
     });
   }
   ev.record(2);
@@ -2255,9 +2258,9 @@ lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
     TagScope tg("transform");
     DevBuf<float> normbuf;
     const size_t cw = ix->code_bytes();
-    for_each_chunk(src, [&](const float* xf, uint64_t r0, uint64_t rows) {
-      transform_chunk(xf, rows, (int)d, m, ix->centroids.p, K, ix->codebook.p, M, nbits, normbuf, part.p + r0,
-                      codes.p + r0 * cw, valid.p + r0);
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, ix->codebook.p, M, nbits, normbuf,
+                      part.p + r0, codes.p + r0 * cw, valid.p + r0);
     });
   }
   ev.record(3);

@@ -410,39 +410,27 @@ generic_kernel(const float* __restrict__ x, uint64_t n, int d, const float* __re
 // ------------------------------------------------------------------------------------------------
 template <int METRIC>
 static void assign_dispatch(const float* x, uint64_t n, int d, const float* cent, int K,
-                            const float* bias, bool bias_padded, uint32_t* part, float* dist,
-                            uint8_t* valid, float* all_out, const uint8_t* active, TcWorkspace* ws) {
+                            const float* bias, uint32_t* part, float* dist,
+                            uint8_t* valid, float* all_out, const uint8_t* active, TcWorkspace& ws) {
   if (n == 0) return;
   // the tile kernel reads rows as float4: a row base that is not 16-byte aligned (a view into a caller's buffer)
   // takes the scalar-load generic kernel, which returns the same bits
   if (d % 16 == 0 && d <= 256 && (reinterpret_cast<uintptr_t>(x) & 15) == 0) {
     const int Kp = (K + 63) / 64 * 64;
-    TcWorkspace local;
-    if (!ws) ws = &local;
-    DevBuf<float>& cT = ws->cT;  // no allocation per call inside a training loop / CUDA graph
+    DevBuf<float>& cT = ws.cT;  // no allocation per call inside a training loop / CUDA graph
     if (cT.n < (size_t)d * Kp) cT.alloc((size_t)d * Kp);
     LB2_LAUNCH("transpose_centroids", transpose_pad_kernel, cdiv((uint64_t)d * Kp, 256), 256, 0,
                cent, K, d, Kp, cT.get());
-    DevBuf<float> biasp;
-    const float* bp = nullptr;
-    if (bias && bias_padded) {
-      bp = bias;
-    } else if (bias) {
-      biasp.alloc(Kp);
-      biasp.zero();
-      d2d(biasp.get(), bias, K);
-      bp = biasp.get();
-    }
     const size_t smem = sizeof(float) * (64 * (d + 1) + (size_t)d * 64);
     const unsigned grid = cdiv(n, 64);
     if (all_out) {
       set_smem(assign_tile_kernel<METRIC, true, 4>, smem);
       LB2_LAUNCH("assign_exact", (assign_tile_kernel<METRIC, true, 4>), grid, 256, smem, x, n, d,
-                 cT.get(), K, Kp, bp, part, dist, valid, all_out, active, nullptr, nullptr, 0u, 0xffffffffu);
+                 cT.get(), K, Kp, bias, part, dist, valid, all_out, active, nullptr, nullptr, 0u, 0xffffffffu);
     } else {
       set_smem(assign_tile_kernel<METRIC, false, 4>, smem);
       LB2_LAUNCH("assign_exact", (assign_tile_kernel<METRIC, false, 4>), grid, 256, smem, x, n, d,
-                 cT.get(), K, Kp, bp, part, dist, valid, all_out, active, nullptr, nullptr, 0u, 0xffffffffu);
+                 cT.get(), K, Kp, bias, part, dist, valid, all_out, active, nullptr, nullptr, 0u, 0xffffffffu);
     }
     return;
   }
@@ -467,9 +455,9 @@ static void assign_dispatch(const float* x, uint64_t n, int d, const float* cent
 
 // exact tile kernel over a device-side row list (count read on the device: no host sync)
 void assign_rows_f32(const float* x, uint64_t n_max, int d, const float* cent, int K, int metric,
-                     const float* bias_padded, const uint32_t* row_list, const uint32_t* row_count,
+                     const float* bias, const uint32_t* row_list, const uint32_t* row_count,
                      uint32_t* part, float* dist, uint8_t* valid, const uint8_t* active,
-                     TcWorkspace* ws, bool cT_ready) {
+                     TcWorkspace& ws, bool cT_ready) {
   if (metric != METRIC_L2) fail(LB2_UNSUPPORTED, "assign_rows_f32: metric not supported");
   if (!(d % 16 == 0 && d <= 256)) {
     // 8 rows per CTA: the list is short, more CTAs beat fewer centroid re-reads (measured)
@@ -478,31 +466,26 @@ void assign_rows_f32(const float* x, uint64_t n_max, int d, const float* cent, i
     // very short lists against many centroids: one CTA per (8 rows, range of centroids) + a merge
     const int gchunks = (int)std::min<uint64_t>(64, (uint64_t)K / 128);
     const uint32_t gtiny = gchunks > 1 ? (uint32_t)std::min<uint64_t>(4096, n_max + 1) : 0u;
-    TcWorkspace glocal;
-    if (!ws) ws = &glocal;
     if (gtiny) {
       const int kchunk = ((K + gchunks - 1) / gchunks + 15) / 16 * 16;
       const int nch = (K + kchunk - 1) / kchunk;
-      if (ws->split_scratch.n < (size_t)gtiny * nch * 3) ws->split_scratch.alloc((size_t)gtiny * nch * 3);
+      if (ws.split_scratch.n < (size_t)gtiny * nch * 3) ws.split_scratch.alloc((size_t)gtiny * nch * 3);
       set_smem((generic_kernel<METRIC_L2, false, 8, true>), gsmem);
       LB2_LAUNCH("assign_exact_fallback", (generic_kernel<METRIC_L2, false, 8, true>),
-                 dim3((unsigned)cdiv(gtiny, 8), (unsigned)nch), 256, gsmem, x, n_max, d, cent, K, bias_padded, part, dist,
-                 valid, nullptr, active, row_list, row_count, 0u, gtiny, kchunk, ws->split_scratch.p);
-      LB2_LAUNCH("assign_exact_fallback", split_merge_kernel, cdiv(gtiny, 256), 256, 0, ws->split_scratch.p, nch, row_list,
+                 dim3((unsigned)cdiv(gtiny, 8), (unsigned)nch), 256, gsmem, x, n_max, d, cent, K, bias, part, dist,
+                 valid, nullptr, active, row_list, row_count, 0u, gtiny, kchunk, ws.split_scratch.p);
+      LB2_LAUNCH("assign_exact_fallback", split_merge_kernel, cdiv(gtiny, 256), 256, 0, ws.split_scratch.p, nch, row_list,
                  row_count, gtiny, part, dist, valid, active);
     }
     set_smem(generic_kernel<METRIC_L2, false, 8>, gsmem);
     LB2_LAUNCH("assign_exact_fallback", (generic_kernel<METRIC_L2, false, 8>),
                (unsigned)std::min<uint64_t>(cdiv(n_max, 8), 8 * (uint64_t)ctx().num_sms), 256, gsmem, x,
-               n_max, d, cent, K, bias_padded, part, dist, valid, nullptr, active, row_list, row_count, gtiny,
+               n_max, d, cent, K, bias, part, dist, valid, nullptr, active, row_list, row_count, gtiny,
                0xffffffffu);
-    if (ws == &glocal) sync_stream();  // its scratch is freed on return
     return;
   }
   const int Kp = (K + 63) / 64 * 64;
-  TcWorkspace local;
-  if (!ws) ws = &local;
-  DevBuf<float>& cT = ws->cT;
+  DevBuf<float>& cT = ws.cT;
   if (cT.n < (size_t)d * Kp) cT.alloc((size_t)d * Kp);
   if (!cT_ready)
     LB2_LAUNCH("transpose_centroids", transpose_pad_kernel, cdiv((uint64_t)d * Kp, 256), 256, 0, cent,
@@ -517,67 +500,59 @@ void assign_rows_f32(const float* x, uint64_t n_max, int d, const float* cent, i
   const uint32_t split = K > 256 ? 64u * 2u * (uint32_t)ctx().num_sms : 0xffffffffu;
   const size_t smem = sizeof(float) * (16 * (d + 1) + (size_t)d * 64);
   if (tiny) {
-    if (ws->split_scratch.n < (size_t)tiny * nchunks * 3) ws->split_scratch.alloc((size_t)tiny * nchunks * 3);
+    if (ws.split_scratch.n < (size_t)tiny * nchunks * 3) ws.split_scratch.alloc((size_t)tiny * nchunks * 3);
     set_smem(assign_tile_kernel<METRIC_L2, false, 1, true>, smem);
     LB2_LAUNCH("assign_exact_fallback", (assign_tile_kernel<METRIC_L2, false, 1, true>),
-               dim3((unsigned)cdiv(tiny, 16), (unsigned)nchunks), 256, smem, x, n_max, d, cT.get(), K, Kp, bias_padded,
-               part, dist, valid, nullptr, active, row_list, row_count, 0u, tiny, ws->split_scratch.p);
-    LB2_LAUNCH("assign_exact_fallback", split_merge_kernel, cdiv(tiny, 256), 256, 0, ws->split_scratch.p, nchunks,
+               dim3((unsigned)cdiv(tiny, 16), (unsigned)nchunks), 256, smem, x, n_max, d, cT.get(), K, Kp, bias,
+               part, dist, valid, nullptr, active, row_list, row_count, 0u, tiny, ws.split_scratch.p);
+    LB2_LAUNCH("assign_exact_fallback", split_merge_kernel, cdiv(tiny, 256), 256, 0, ws.split_scratch.p, nchunks,
                row_list, row_count, tiny, part, dist, valid, active);
   }
   set_smem(assign_tile_kernel<METRIC_L2, false, 1>, smem);
   LB2_LAUNCH("assign_exact_fallback", (assign_tile_kernel<METRIC_L2, false, 1>),
              (unsigned)std::min<uint64_t>(cdiv(std::min<uint64_t>(n_max, split), 16), 4 * (uint64_t)ctx().num_sms), 256,
-             smem, x, n_max, d, cT.get(), K, Kp, bias_padded,
+             smem, x, n_max, d, cT.get(), K, Kp, bias,
              part, dist, valid, nullptr, active, row_list, row_count, tiny, split);
   if (n_max >= split) {
     const size_t smem4 = sizeof(float) * (64 * (d + 1) + (size_t)d * 64);
     set_smem(assign_tile_kernel<METRIC_L2, false, 4>, smem4);
     LB2_LAUNCH("assign_exact_fallback", (assign_tile_kernel<METRIC_L2, false, 4>),
                (unsigned)std::min<uint64_t>(cdiv(n_max, 64), 2 * (uint64_t)ctx().num_sms), 256, smem4,
-               x, n_max, d, cT.get(), K, Kp, bias_padded, part, dist, valid, nullptr, active, row_list,
+               x, n_max, d, cT.get(), K, Kp, bias, part, dist, valid, nullptr, active, row_list,
                row_count, split, 0xffffffffu);
   }
 }
 
 void assign_f32_ex(const float* x, uint64_t n, int d, const float* cent, int K, int metric,
-                   const float* bias, bool bias_padded, uint32_t* part, float* dist, uint8_t* valid,
-                   float* all_out, const uint8_t* active, TcWorkspace* ws) {
+                   const float* bias, uint32_t* part, float* dist, uint8_t* valid,
+                   float* all_out, const uint8_t* active, TcWorkspace& ws, const void* x16, int x16_dtype) {
   if (!all_out && n >= 256 && tc_assign_supported(n, d, K, metric, x)) {
     // tensor-core filter + exact re-rank: bit-identical outputs, ~10x less FP32 work
-    DevBuf<float> biasp;
-    const float* bp = bias;
-    if (bias && !bias_padded) {
-      const int Kp256 = (K + 255) / 256 * 256;
-      biasp.alloc(Kp256);
-      biasp.zero();
-      d2d(biasp.get(), bias, K);
-      bp = biasp.get();
-    }
     // large inputs in chunks of <= 2^20 rows (<= 4 GB of vectors): bounds the per-call scratch (row norms,
     // verdicts, the 3x-wide refinement rows) without changing any output
     const uint64_t chunk = std::max<uint64_t>(1ull << 16, std::min<uint64_t>(1ull << 20, (1ull << 30) / (uint64_t)d));
     if (n <= chunk + chunk / 2) {
-      tc_assign_f32(x, n, d, cent, K, bp, part, dist, valid, active, ws);
+      tc_assign_f32(x, n, d, cent, K, bias, part, dist, valid, active, ws, x16, x16_dtype);
       return;
     }
-    TcWorkspace local;
-    if (!ws) ws = &local;
     for (uint64_t r0 = 0; r0 < n; r0 += chunk) {
       const uint64_t rows = std::min(chunk, n - r0);
-      tc_assign_f32(x + r0 * d, rows, d, cent, K, bp, part + r0, dist ? dist + r0 : nullptr,
-                    valid ? valid + r0 : nullptr, active, ws);
+      tc_assign_f32(x + r0 * d, rows, d, cent, K, bias, part + r0, dist ? dist + r0 : nullptr,
+                    valid ? valid + r0 : nullptr, active, ws,
+                    x16 ? static_cast<const uint16_t*>(x16) + r0 * d : nullptr, x16_dtype);
     }
     return;
   }
   if (metric == METRIC_DOT)
-    assign_dispatch<METRIC_DOT>(x, n, d, cent, K, bias, bias_padded, part, dist, valid, all_out, active, ws);
+    assign_dispatch<METRIC_DOT>(x, n, d, cent, K, bias, part, dist, valid, all_out, active, ws);
   else
-    assign_dispatch<METRIC_L2>(x, n, d, cent, K, bias, bias_padded, part, dist, valid, all_out, active, ws);
+    assign_dispatch<METRIC_L2>(x, n, d, cent, K, bias, part, dist, valid, all_out, active, ws);
 }
 void assign_f32(const float* x, uint64_t n, int d, const float* cent, int K, int metric,
-                const float* bias, uint32_t* part, float* dist, uint8_t* valid, float* all_out) {
-  assign_f32_ex(x, n, d, cent, K, metric, bias, false, part, dist, valid, all_out, nullptr, nullptr);
+                const float* bias, uint32_t* part, float* dist, uint8_t* valid, float* all_out,
+                const void* x16, int x16_dtype) {
+  TcWorkspace ws;
+  assign_f32_ex(x, n, d, cent, K, metric, bias, part, dist, valid, all_out, nullptr, ws, x16, x16_dtype);
 }
 
 template <int DS, int METRIC>

@@ -2,21 +2,25 @@
 #pragma once
 #include <stdint.h>
 namespace lb2 {
+struct TcWorkspace;
 // part/dist/valid are [n]; all_out (nullable) receives the full [n][K] distance matrix instead.
 // bias (nullable, [K]) is added for the comparison only (kernels.rs:92-111).
+// x16 (nullable): the same rows as x in their own element type x16_dtype (LB2_F16 / LB2_BF16); the tensor-core
+// filter may read them instead of x (tc_assign.cu, "native 16-bit rows").
 void assign_f32(const float* x, uint64_t n, int d, const float* cent, int K, int metric,
-                const float* bias, uint32_t* part, float* dist, uint8_t* valid, float* all_out);
-// same, with a bias already padded to ceil(K/64)*64 floats and an optional device-side `active`
-// flag (active[0] == 0 -> the kernel returns immediately; used by the Lloyd loop)
-struct TcWorkspace;
+                const float* bias, uint32_t* part, float* dist, uint8_t* valid, float* all_out,
+                const void* x16 = nullptr, int x16_dtype = 0);
+// same, with an optional device-side `active` flag (active[0] == 0 -> the kernels return immediately; used by the
+// Lloyd loop) and the caller's workspace (a training loop keeps one across iterations and its CUDA graph)
 void assign_f32_ex(const float* x, uint64_t n, int d, const float* cent, int K, int metric,
-                   const float* bias, bool bias_padded, uint32_t* part, float* dist, uint8_t* valid,
-                   float* all_out, const uint8_t* active, TcWorkspace* ws);
+                   const float* bias, uint32_t* part, float* dist, uint8_t* valid,
+                   float* all_out, const uint8_t* active, TcWorkspace& ws,
+                   const void* x16 = nullptr, int x16_dtype = 0);
 // exact tile kernel restricted to row_list[0 .. *row_count) (both on the device)
 void assign_rows_f32(const float* x, uint64_t n_max, int d, const float* cent, int K, int metric,
-                     const float* bias_padded, const uint32_t* row_list, const uint32_t* row_count,
+                     const float* bias, const uint32_t* row_list, const uint32_t* row_count,
                      uint32_t* part, float* dist, uint8_t* valid, const uint8_t* active,
-                     TcWorkspace* ws, bool cT_ready = false);
+                     TcWorkspace& ws, bool cT_ready);
 // d < 16 path, batched over M sub-spaces; x row stride ldx, sub-space m reads columns [m*ds,(m+1)*ds).
 // codes != NULL -> u8 [n][M] out (PQ encode), else ids/dists/valid [M][n] (PQ training).
 bool small_d_supported(int ds);

@@ -1151,7 +1151,6 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     sync_stream();  // rows (host vector) must outlive the copy
   }
 
-  const int Kp = (K + 63) / 64 * 64;
   DevBuf<uint32_t> ids((size_t)B * n), last_row(BK);
   DevBuf<float> dists((size_t)B * n), radius(BK), bias;
   DevBuf<uint8_t> valid((size_t)B * n), active_d(B);
@@ -1175,7 +1174,7 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     }
   };
   if (!small) {
-    bias.alloc(Kp);
+    bias.alloc(K);
     bias.zero();  // iteration 1: cluster sizes are all zero -> bias 0
   }
   // multi-GPU: this rank's packed partial results and the gathered blobs of all ranks (see "ONE exchange")
@@ -1228,8 +1227,7 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
   // one Lloyd iteration = ~18 short kernels: membership, member sort, stats, update, scalar epilogue
   auto iteration = [&]() {
     if (!small) {
-      assign_f32_ex(x, n, ds, centroids, K, metric, bias.p, /*bias_padded=*/true, ids.p, dists.p,
-                    valid.p, nullptr, active_d.p, &tcws);
+      assign_f32_ex(x, n, ds, centroids, K, metric, bias.p, ids.p, dists.p, valid.p, nullptr, active_d.p, tcws);
     } else if (pq_tc) {
       // the first call prepares the operands itself; afterwards the epilogue of iteration i has
       // already written them for iteration i + 1
@@ -1257,7 +1255,7 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, i
     }
     LB2_LAUNCH("kmeans_epilogue", epilogue_kernel, B, 256, 0, K, ds, n_global, balance_factor_param,
                tolerance, ms.counts.p, losses.p, radius.p, last_row.p, cluster_sizes.p,
-               small ? nullptr : bias.p, Kp, centroids, states.p, active_d.p, pq_prep, words.device());
+               small ? nullptr : bias.p, K, centroids, states.p, active_d.p, pq_prep, words.device());
   };
   // The first iteration runs eagerly (allocates every workspace, sets kernel attributes); the
   // iteration is then captured ONCE into a CUDA graph and replayed, so that the loop is not bound

@@ -699,7 +699,7 @@ static void launch_general_dyn(int opk, int mode, unsigned grid, size_t smem, co
 #undef LB2_GEN
 }
 
-// Rows the first pass left undecided (ws->fb_rows / fb_count[0]).
+// Rows the first pass left undecided (ws.fb_rows / fb_count[0]).
 //   f32 rows (first pass TF32):  3xTF32 top-3 pass over the list -> exact re-rank of what it settles; the rest
 //       (fb_rows2 / fb_count[1]) -> 3xTF32 CANDIDATE pass: all columns within tau' of the best score -> exact
 //       decision among those candidates (cand_exact_kernel).
@@ -707,14 +707,14 @@ static void launch_general_dyn(int opk, int mode, unsigned grid, size_t smem, co
 //   What is still open (no candidate: NaN / Inf rows; > CAND_SLOTS candidates: duplicated centroids; rows that did
 //   not fit the gather buffers) runs through the full-K exact kernel (fb_rows3 / fb_count[2]).
 // `cpad` = zero-padded centroids [Kp][d], cnh / cmax2 as prepared for the first pass; x16 / cpad16 for OPK != 0.
-static void tc_refine_and_fallback(const float* x, uint64_t n, int d, const float* cent, int K, int Kp,
+// Returns whether the refinement passes ran (otherwise every undecided row took the full-K exact scan).
+static bool tc_refine_and_fallback(const float* x, uint64_t n, int d, const float* cent, int K, int Kp,
                                    const float* bias, const float* cpad, const float* cnh, const float* cmax2,
                                    uint32_t* part, float* dist, uint8_t* valid, const uint8_t* active,
-                                   TcWorkspace* ws, bool cT_ready, int opk = 0, const void* x16 = nullptr) {
+                                   TcWorkspace& ws, bool cT_ready, int opk, const void* x16) {
   using namespace tc;
-  const char* e_no = getenv("LB2_NO_REFINE");
   const char* e_force = getenv("LB2_FORCE_REFINE");
-  const bool no_refine = e_no && *e_no, force = e_force && *e_force;
+  const bool force = e_force && *e_force;
   const int d3 = 3 * d;
   const size_t row_bytes = opk ? (size_t)d * 2 : (size_t)d3 * 4;
   // room for 1/8 of the rows, at most ~1.5 GB of gathered rows (callers chunk large inputs, assign_f32_ex);
@@ -725,69 +725,70 @@ static void tc_refine_and_fallback(const float* x, uint64_t n, int d, const floa
   const size_t smem = L.total + 1024;
   // worth its launches only when the first pass was a large one (the undecided list of a 65 536-row training
   // call is a few hundred rows: the exact kernel finishes them sooner)
-  const bool refine = !no_refine && smem <= ctx().smem_optin && (force || (uint64_t)n * (uint64_t)K >= (1ull << 26) || (uint64_t)n * (uint64_t)K * (uint64_t)d >= (1ull << 32));
+  const bool refine = smem <= ctx().smem_optin && (force || (uint64_t)n * (uint64_t)K >= (1ull << 26) || (uint64_t)n * (uint64_t)K * (uint64_t)d >= (1ull << 32));
   if (!refine) {
-    assign_rows_f32(x, n, d, cent, K, METRIC_L2, bias, ws->fb_rows.p, ws->fb_count.p, part, dist, valid, active, ws,
+    assign_rows_f32(x, n, d, cent, K, METRIC_L2, bias, ws.fb_rows.p, ws.fb_count.p, part, dist, valid, active, ws,
                     cT_ready);
-    return;
+    return false;
   }
   const size_t a_floats = ((size_t)cap * row_bytes + 3) / 4;
-  if (ws->a3.n < a_floats) ws->a3.alloc(a_floats);
-  if (ws->rn2c.n < (size_t)2 * cap) ws->rn2c.alloc((size_t)2 * cap);  // |x|^2 and the candidate threshold
-  if (ws->res2.n < (size_t)3 * cap) ws->res2.alloc((size_t)3 * cap);  // verdicts (2) + best score of the pass
-  if (ws->fb_rows2.n < 2 * n) ws->fb_rows2.alloc(2 * n);              // lists 2 and 3
-  if (ws->cand.n < (size_t)cap * (CAND_SLOTS + 1)) ws->cand.alloc((size_t)cap * (CAND_SLOTS + 1));
-  if (ws->top1_val.n < n) ws->top1_val.alloc(n);
-  float* thr = ws->rn2c.p + cap;
-  uint32_t* cand_cnt = ws->cand.p;
-  uint32_t* cand = ws->cand.p + cap;
-  uint32_t* list1 = ws->fb_rows.p;
-  uint32_t* list2 = ws->fb_rows2.p;
-  uint32_t* list3 = ws->fb_rows2.p + n;
-  uint32_t* cnt = ws->fb_count.p;  // [0] list 1, [1] list 2, [2] list 3
+  if (ws.a3.n < a_floats) ws.a3.alloc(a_floats);
+  if (ws.rn2c.n < (size_t)2 * cap) ws.rn2c.alloc((size_t)2 * cap);  // |x|^2 and the candidate threshold
+  if (ws.res2.n < (size_t)3 * cap) ws.res2.alloc((size_t)3 * cap);  // verdicts (2) + best score of the pass
+  if (ws.fb_rows2.n < 2 * n) ws.fb_rows2.alloc(2 * n);              // lists 2 and 3
+  if (ws.cand.n < (size_t)cap * (CAND_SLOTS + 1)) ws.cand.alloc((size_t)cap * (CAND_SLOTS + 1));
+  if (ws.top1_val.n < n) ws.top1_val.alloc(n);
+  float* thr = ws.rn2c.p + cap;
+  uint32_t* cand_cnt = ws.cand.p;
+  uint32_t* cand = ws.cand.p + cap;
+  uint32_t* list1 = ws.fb_rows.p;
+  uint32_t* list2 = ws.fb_rows2.p;
+  uint32_t* list3 = ws.fb_rows2.p + n;
+  uint32_t* cnt = ws.fb_count.p;  // [0] list 1, [1] list 2, [2] list 3
   const unsigned sms = (unsigned)ctx().num_sms;
   const unsigned grid = (unsigned)std::min<uint64_t>(cdiv(cap, TM), (uint64_t)sms);
   const unsigned ggrid = (unsigned)std::min<uint64_t>(cdiv((uint64_t)cap * (d / 4), 256), 8 * sms);
   const unsigned rgrid = (unsigned)std::min<uint64_t>(cdiv((uint64_t)cap * 16, 256), 8 * sms);
   if (opk) {
     const float tau = tau16_scale(d);
-    uint16_t* a16 = reinterpret_cast<uint16_t*>(ws->a3.p);
-    LB2_LAUNCH("tc_refine_gather", gather16_kernel, ggrid, 256, 0, static_cast<const uint16_t*>(x16), d, ws->row_norm2.p,
-               list1, cnt, cap, a16, ws->rn2c.p, active, ws->top1_val.p, tau, cmax2, thr, cand_cnt);
+    uint16_t* a16 = reinterpret_cast<uint16_t*>(ws.a3.p);
+    LB2_LAUNCH("tc_refine_gather", gather16_kernel, ggrid, 256, 0, static_cast<const uint16_t*>(x16), d, ws.row_norm2.p,
+               list1, cnt, cap, a16, ws.rn2c.p, active, ws.top1_val.p, tau, cmax2, thr, cand_cnt);
     const CUtensorMap map_a = make_map_2d_16(a16, opk == 2, cap, d, TM);
-    const CUtensorMap map_b = make_map_2d_16(ws->cpad16.p, opk == 2, Kp, d, TN);
-    launch_general_dyn(opk, 1, grid, smem, map_a, map_b, (uint64_t)cap, d / (2 * KC), Kp / TN, cnh, ws->rn2c.p, cmax2,
+    const CUtensorMap map_b = make_map_2d_16(ws.cpad16.p, opk == 2, Kp, d, TN);
+    launch_general_dyn(opk, 1, grid, smem, map_a, map_b, (uint64_t)cap, d / (2 * KC), Kp / TN, cnh, ws.rn2c.p, cmax2,
                        nullptr, nullptr, active, tau, cnt, cap, nullptr, thr, cand_cnt, cand, "tc_candidates");
     // rows beyond the gather capacity: rerank_kernel's list mode only forwards them (res is not read for them)
     LB2_LAUNCH("tc_candidates_exact", cand_exact_kernel, rgrid, 256, 0, x, d, cent, bias, list1, cnt, cap, cand_cnt, cand,
                part, dist, valid, list3, cnt + 2, active);
     LB2_LAUNCH("tc_candidates_exact", forward_overflow_kernel, 8 * sms, 256, 0, list1, cnt, cap, list3, cnt + 2, active);
   } else {
-    if (ws->b3.n < (size_t)Kp * d3) ws->b3.alloc((size_t)Kp * d3);
+    if (ws.b3.n < (size_t)Kp * d3) ws.b3.alloc((size_t)Kp * d3);
     const float tau2 = tau3x_scale(d3);
-    LB2_LAUNCH("tc_refine_gather", gather_split_kernel, ggrid, 256, 0, x, d, ws->row_norm2.p, list1, cnt, cap, ws->a3.p,
-               ws->rn2c.p, active, (const float*)nullptr, 0.0f, (const float*)nullptr, (float*)nullptr,
+    LB2_LAUNCH("tc_refine_gather", gather_split_kernel, ggrid, 256, 0, x, d, ws.row_norm2.p, list1, cnt, cap, ws.a3.p,
+               ws.rn2c.p, active, (const float*)nullptr, 0.0f, (const float*)nullptr, (float*)nullptr,
                (uint32_t*)nullptr);
     LB2_LAUNCH("tc_refine_gather", split_centroids_kernel, cdiv((uint64_t)Kp * d, 256), 256, 0, cpad, (size_t)Kp * d, d,
-               ws->b3.p);
-    const CUtensorMap map_a = make_map_2d(ws->a3.p, cap, d3, TM);
-    const CUtensorMap map_b = make_map_2d(ws->b3.p, Kp, d3, TN);
-    float* val2 = reinterpret_cast<float*>(ws->res2.p + 2 * (size_t)cap);
-    launch_general_dyn(0, 0, grid, smem, map_a, map_b, (uint64_t)cap, d3 / KC, Kp / TN, cnh, ws->rn2c.p, cmax2, ws->res2.p,
-                       ws->res2.p + cap, active, tau2, cnt, cap, val2, nullptr, nullptr, nullptr, "tc_refine_filter");
+               ws.b3.p);
+    const CUtensorMap map_a = make_map_2d(ws.a3.p, cap, d3, TM);
+    const CUtensorMap map_b = make_map_2d(ws.b3.p, Kp, d3, TN);
+    float* val2 = reinterpret_cast<float*>(ws.res2.p + 2 * (size_t)cap);
+    launch_general_dyn(0, 0, grid, smem, map_a, map_b, (uint64_t)cap, d3 / KC, Kp / TN, cnh, ws.rn2c.p, cmax2, ws.res2.p,
+                       ws.res2.p + cap, active, tau2, cnt, cap, val2, nullptr, nullptr, nullptr, "tc_refine_filter");
     LB2_LAUNCH("tc_refine_rerank", rerank_kernel, (unsigned)std::min<uint64_t>(cdiv((uint64_t)n * 16, 256), 8 * sms), 256, 0,
-               x, n, d, cent, bias, ws->res2.p, (const uint32_t*)(ws->res2.p + cap), 1, part, dist, valid, list2, cnt + 1,
-               active, (const uint32_t*)list1, (const uint32_t*)cnt, cap, (const float*)val2, ws->top1_val.p, list3,
+               x, n, d, cent, bias, ws.res2.p, (const uint32_t*)(ws.res2.p + cap), 1, part, dist, valid, list2, cnt + 1,
+               active, (const uint32_t*)list1, (const uint32_t*)cnt, cap, (const float*)val2, ws.top1_val.p, list3,
                cnt + 2);
     // candidate pass over what the 3xTF32 top-3 left open (list 2 <= cap entries)
-    LB2_LAUNCH("tc_refine_gather", gather_split_kernel, ggrid, 256, 0, x, d, ws->row_norm2.p, list2, cnt + 1, cap, ws->a3.p,
-               ws->rn2c.p, active, (const float*)ws->top1_val.p, tau2, cmax2, thr, cand_cnt);
-    launch_general_dyn(0, 1, grid, smem, map_a, map_b, (uint64_t)cap, d3 / KC, Kp / TN, cnh, ws->rn2c.p, cmax2, nullptr,
+    LB2_LAUNCH("tc_refine_gather", gather_split_kernel, ggrid, 256, 0, x, d, ws.row_norm2.p, list2, cnt + 1, cap, ws.a3.p,
+               ws.rn2c.p, active, (const float*)ws.top1_val.p, tau2, cmax2, thr, cand_cnt);
+    launch_general_dyn(0, 1, grid, smem, map_a, map_b, (uint64_t)cap, d3 / KC, Kp / TN, cnh, ws.rn2c.p, cmax2, nullptr,
                        nullptr, active, tau2, cnt + 1, cap, nullptr, thr, cand_cnt, cand, "tc_candidates");
     LB2_LAUNCH("tc_candidates_exact", cand_exact_kernel, rgrid, 256, 0, x, d, cent, bias, list2, cnt + 1, cap, cand_cnt,
                cand, part, dist, valid, list3, cnt + 2, active);
   }
   assign_rows_f32(x, n, d, cent, K, METRIC_L2, bias, list3, cnt + 2, part, dist, valid, active, ws, cT_ready);
+  return true;
 }
 
 bool tc_assign_supported(uint64_t n, int d, int K, int metric, const float* x) {
@@ -797,169 +798,112 @@ bool tc_assign_supported(uint64_t n, int d, int K, int metric, const float* x) {
 }
 
 // ---- native 16-bit rows ----------------------------------------------------------------------------------------
-// The chunk loops of api.cu announce, next to the f32 view of a chunk, where the same rows lie in their own
-// f16 / bf16 type.  If the model is exactly representable in that type (models trained on such columns are,
-// round_model) the filter passes read the 16-bit rows directly: f16 / bf16 wgmma at twice the TF32 rate, exact
-// products, a tau ~10x smaller.  The exact kernels keep reading the f32 view (conversion is exact).
-struct OperandHint {
-  const float* f32 = nullptr;
-  const void* nat = nullptr;
-  int opk = 0;
-  size_t elems = 0;
-};
-static thread_local OperandHint g_hint;
-void tc_set_operand_hint(const float* f32, const void* native, int dtype, size_t elems) {
-  g_hint.f32 = f32;
-  g_hint.nat = native;
-  g_hint.opk = dtype == LB2_F16 ? 1 : dtype == LB2_BF16 ? 2 : 0;
-  g_hint.elems = elems;
-  if (!native || !g_hint.opk) g_hint = OperandHint();
-}
-static const void* hinted_rows(const float* x, uint64_t n, int d, int* opk) {
+// The chunk loops of api.cu pass, next to the f32 view x of a chunk, the same rows in their own f16 / bf16 type
+// (x16).  If the model is exactly representable in that type (models trained on such columns are, round_model) the
+// filter passes of the general shape read the 16-bit rows directly: f16 / bf16 wgmma at twice the TF32 rate, exact
+// products, a tau ~10x smaller.  The exact kernels keep reading x (conversion is exact).
+// Returns the operand kind of x16 (1: f16, 2: bf16), or 0 when the filter reads x.
+static int native_opk(const void* x16, int x16_dtype, int d) {
   const char* off = getenv("LB2_NO_NATIVE16");
-  if (!g_hint.f32 || (off && *off) || d % (2 * tc::KC) != 0) return nullptr;
-  if (x < g_hint.f32 || x + (size_t)n * d > g_hint.f32 + g_hint.elems) return nullptr;
-  const void* p = static_cast<const uint8_t*>(g_hint.nat) + (size_t)(x - g_hint.f32) * 2;
-  if (reinterpret_cast<uintptr_t>(p) & 15) return nullptr;
-  *opk = g_hint.opk;
-  return p;
+  if (!x16 || (off && *off) || d % (2 * tc::KC) != 0 || (reinterpret_cast<uintptr_t>(x16) & 15)) return 0;
+  return x16_dtype == LB2_F16 ? 1 : x16_dtype == LB2_BF16 ? 2 : 0;
 }
 
-// general shapes (centroid tiles streamed): same contract as tc_assign_f32
-static void tc_assign_general_f32(const float* x, uint64_t n, int d, const float* cent, int K, const float* bias,
-                                  uint32_t* part, float* dist, uint8_t* valid, const uint8_t* active,
-                                  TcWorkspace* ws) {
-  using namespace tc;
-  const int ntiles = (K + TN - 1) / TN, Kp = ntiles * TN;
-  const GenLayout L = gen_layout();
-  const size_t smem = L.total + 1024;
-  if (smem > ctx().smem_optin) fail(LB2_UNSUPPORTED, "tc_assign: shared memory");
-  if (ws->cpad.n < (size_t)Kp * d) ws->cpad.alloc((size_t)Kp * d);
-  if (ws->cnh.n < (size_t)2 * Kp + 1) ws->cnh.alloc((size_t)2 * Kp + 1);
-  if (ws->row_norm2.n < n || ws->norm_src != x || ws->norm_n != n) {
-    if (ws->row_norm2.n < n) ws->row_norm2.alloc(n);
-    LB2_LAUNCH("tc_row_norms", row_norm_kernel, cdiv(n * 16, 256), 256, 0, x, n, d, ws->row_norm2.p);
-    ws->norm_src = x;
-    ws->norm_n = n;
-  }
-  if (ws->res.n < 2 * n) ws->res.alloc(2 * n);
-  if (ws->fb_rows.n < n) ws->fb_rows.alloc(n);
-  if (ws->fb_count.n < 4) ws->fb_count.alloc(4);
-  float* cnh = ws->cnh.p;
-  float* cn2 = ws->cnh.p + Kp;
-  float* cmax2 = ws->cnh.p + 2 * (size_t)Kp;
-  LB2_LAUNCH("tc_prep_centroids", prep_centroids_general_kernel, cdiv(Kp, 8), 256, 0, cent, K, Kp, d, bias,
-             ws->cpad.p, cnh, cn2, ws->fb_count.p);
-  LB2_LAUNCH("tc_prep_centroids", max_reduce_kernel, 1, 1024, 0, cn2, Kp, cmax2);
-  int opk = 0;
-  const void* x16 = active ? nullptr : hinted_rows(x, n, d, &opk);  // (training loops never carry a hint)
-  if (x16) {
-    if (ws->cpad16.n < (size_t)Kp * d) ws->cpad16.alloc((size_t)Kp * d);
-    LB2_LAUNCH("tc_prep_centroids", prep16_kernel, cdiv((size_t)Kp * d, 256), 256, 0, ws->cpad.p, (size_t)Kp * d,
-               opk == 2 ? 1 : 0, ws->cpad16.p, ws->fb_count.p + 3);
-    uint32_t inexact = 0;
-    d2h(&inexact, ws->fb_count.p + 3, 1);
-    sync_stream();
-    if (inexact) { x16 = nullptr; opk = 0; }
-  }
-  const uint64_t tiles = (n + TM - 1) / TM;
-  const unsigned grid = (unsigned)std::min<uint64_t>(tiles, (uint64_t)ctx().num_sms);
-  if (x16) {
-    if (ws->top1_val.n < n) ws->top1_val.alloc(n);
-    const CUtensorMap map_x = make_map_2d_16(x16, opk == 2, n, d, TM);
-    const CUtensorMap map_c = make_map_2d_16(ws->cpad16.p, opk == 2, Kp, d, TN);
-    launch_general_dyn(opk, 0, grid, smem, map_x, map_c, n, d / (2 * KC), ntiles, cnh, ws->row_norm2.p, cmax2, ws->res.p,
-                       ws->res.p + n, active, tau16_scale(d), nullptr, 0u, ws->top1_val.p, nullptr, nullptr, nullptr,
-                       "tc_filter_general16");
-  } else {
-    const CUtensorMap map_x = make_map_2d(x, n, d, TM);
-    const CUtensorMap map_c = make_map_2d(ws->cpad.p, Kp, d, TN);
-    launch_general_dyn(0, 0, grid, smem, map_x, map_c, n, d / KC, ntiles, cnh, ws->row_norm2.p, cmax2, ws->res.p,
-                       ws->res.p + n, active, TAU_TF32, nullptr, 0u, nullptr, nullptr, nullptr, nullptr,
-                       "tc_filter_general");
-  }
-  LB2_LAUNCH("tc_rerank", rerank_kernel, cdiv(n * 16, 256), 256, 0, x, n, d, cent, bias, ws->res.p,
-             (const uint32_t*)(ws->res.p + n), dist != nullptr ? 1 : 0, part, dist, valid, ws->fb_rows.p,
-             ws->fb_count.p, active, (const uint32_t*)nullptr, (const uint32_t*)nullptr, 0u, (const float*)nullptr,
-             (float*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr);
-  if (getenv("LB2_TC_STATS") && *getenv("LB2_TC_STATS")) {
-    std::vector<uint32_t> h(n);
-    d2h(h.data(), ws->res.p, n);
-    sync_stream();
-    uint64_t f[4] = {0, 0, 0, 0};
-    for (uint64_t i = 0; i < n; ++i) f[h[i] >> 30]++;
-    fprintf(stderr, "[lb2 tc_filter_general%s] n=%llu K=%d d=%d: unique %.2f%%, two-candidate %.2f%%, undecided %.2f%%\n",
-            x16 ? "16" : "", (unsigned long long)n, K, d, 100.0 * f[0] / n, 100.0 * f[1] / n, 100.0 * f[2] / n);
-  }
-  tc_refine_and_fallback(x, n, d, cent, K, Kp, bias, ws->cpad.p, cnh, cmax2, part, dist, valid, active, ws,
-                         /*cT_ready=*/false, opk, x16);
-  if (getenv("LB2_TC_STATS") && *getenv("LB2_TC_STATS")) {
-    uint32_t c[3];
-    d2h(c, ws->fb_count.p, 3);
-    sync_stream();
-    fprintf(stderr, "[lb2 tc_filter_general] undecided after pass 1: %u, after the top-3 refinement: %u, full-K exact scan: %u\n",
-            c[0], c[1], c[2]);
-  }
-}
-
+// Two shapes: resident (d <= 128, K <= TN: tc_filter_kernel keeps the whole centroid tile in shared memory) and
+// general (tc_filter_general_kernel streams centroid tiles of TN with the rows, running top-3 over the tiles).
 void tc_assign_f32(const float* x, uint64_t n, int d, const float* cent, int K, const float* bias,
                    uint32_t* part, float* dist, uint8_t* valid, const uint8_t* active,
-                   TcWorkspace* ws) {
+                   TcWorkspace& ws, const void* x16, int x16_dtype) {
   using namespace tc;
-  TcWorkspace local0;
-  if (!ws) ws = &local0;
-  if (!tc_resident_shape(d, K)) {
-    tc_assign_general_f32(x, n, d, cent, K, bias, part, dist, valid, active, ws);
-    return;
+  const bool resident = tc_resident_shape(d, K);
+  const int ntiles = (K + TN - 1) / TN, Kp = ntiles * TN;
+  int stages = MAX_STAGES;  // resident: as many TMA stages as fit next to the centroid tile
+  size_t smem = gen_layout().total + 1024;
+  if (resident) {
+    SmemLayout L = smem_layout(d / KC, stages);
+    while (stages > 2 && L.total + 1024 > ctx().smem_optin) L = smem_layout(d / KC, --stages);
+    smem = L.total + 1024;
   }
-  const int nkc = d / KC;
-  int stages = MAX_STAGES;
-  SmemLayout L = smem_layout(nkc, stages);
-  while (stages > 2 && L.total + 1024 > ctx().smem_optin) L = smem_layout(nkc, --stages);
-  if (L.total + 1024 > ctx().smem_optin) fail(LB2_UNSUPPORTED, "tc_assign: shared memory");
-  TcWorkspace local;
-  if (!ws) ws = &local;
-  if (ws->cpad.n < (size_t)TN * d) ws->cpad.alloc((size_t)TN * d);
-  if (ws->cnh.n < 2 * TN + 1) ws->cnh.alloc(2 * TN + 1);
-  const int Kp = (K + 63) / 64 * 64;
-  if (ws->cT.n < (size_t)d * Kp) ws->cT.alloc((size_t)d * Kp);
-  if (ws->row_norm2.n < n || ws->norm_src != x || ws->norm_n != n) {
-    if (ws->row_norm2.n < n) ws->row_norm2.alloc(n);
-    LB2_LAUNCH("tc_row_norms", row_norm_kernel, cdiv(n * 16, 256), 256, 0, x, n, d, ws->row_norm2.p);
-    ws->norm_src = x;
-    ws->norm_n = n;
+  if (smem > ctx().smem_optin) fail(LB2_UNSUPPORTED, "tc_assign: shared memory");
+  if (ws.cpad.n < (size_t)Kp * d) ws.cpad.alloc((size_t)Kp * d);
+  if (ws.cnh.n < (size_t)2 * Kp + 1) ws.cnh.alloc((size_t)2 * Kp + 1);
+  if (ws.row_norm2.n < n || ws.norm_src != x || ws.norm_n != n) {
+    if (ws.row_norm2.n < n) ws.row_norm2.alloc(n);
+    LB2_LAUNCH("tc_row_norms", row_norm_kernel, cdiv(n * 16, 256), 256, 0, x, n, d, ws.row_norm2.p);
+    ws.norm_src = x;
+    ws.norm_n = n;
   }
-  if (ws->res.n < n) ws->res.alloc(n);
-  if (ws->fb_rows.n < n) ws->fb_rows.alloc(n);
-  if (ws->fb_count.n < 4) ws->fb_count.alloc(4);
-  LB2_LAUNCH("tc_prep_centroids", prep_centroids_kernel, TN / 8, 256, 0, cent, K, d, bias, ws->cpad.p,
-             ws->cnh.p, ws->cnh.p + TN, ws->cT.p, Kp, ws->fb_count.p);
-  LB2_LAUNCH("tc_prep_centroids", max_reduce_kernel, 1, 256, 0, ws->cnh.p + TN, TN, ws->cnh.p + 2 * TN);
-  const CUtensorMap map_x = make_map_2d(x, n, d, TM);
-  const CUtensorMap map_c = make_map_2d(ws->cpad.p, TN, d, TN);
+  const uint64_t res_n = resident ? n : 2 * n;  // general: the second candidate's full index in res[n ..]
+  if (ws.res.n < res_n) ws.res.alloc(res_n);
+  if (ws.fb_rows.n < n) ws.fb_rows.alloc(n);
+  if (ws.fb_count.n < 4) ws.fb_count.alloc(4);
+  float* cnh = ws.cnh.p;
+  float* cn2 = ws.cnh.p + Kp;
+  float* cmax2 = ws.cnh.p + 2 * (size_t)Kp;
+  if (resident) {  // the same launch writes the transposed copy the exact kernels read (cT_ready below)
+    const int Kp64 = (K + 63) / 64 * 64;
+    if (ws.cT.n < (size_t)d * Kp64) ws.cT.alloc((size_t)d * Kp64);
+    LB2_LAUNCH("tc_prep_centroids", prep_centroids_kernel, TN / 8, 256, 0, cent, K, d, bias, ws.cpad.p, cnh, cn2,
+               ws.cT.p, Kp64, ws.fb_count.p);
+  } else {
+    LB2_LAUNCH("tc_prep_centroids", prep_centroids_general_kernel, cdiv(Kp, 8), 256, 0, cent, K, Kp, d, bias,
+               ws.cpad.p, cnh, cn2, ws.fb_count.p);
+  }
+  LB2_LAUNCH("tc_prep_centroids", max_reduce_kernel, 1, resident ? 256 : 1024, 0, cn2, Kp, cmax2);
+  int opk = resident || active ? 0 : native_opk(x16, x16_dtype, d);  // (training loops never pass native rows)
+  if (opk) {
+    if (ws.cpad16.n < (size_t)Kp * d) ws.cpad16.alloc((size_t)Kp * d);
+    LB2_LAUNCH("tc_prep_centroids", prep16_kernel, cdiv((size_t)Kp * d, 256), 256, 0, ws.cpad.p, (size_t)Kp * d,
+               opk == 2 ? 1 : 0, ws.cpad16.p, ws.fb_count.p + 3);
+    uint32_t inexact = 0;
+    d2h(&inexact, ws.fb_count.p + 3, 1);
+    sync_stream();
+    if (inexact) opk = 0;
+  }
   const uint64_t tiles = (n + TM - 1) / TM;
   const unsigned grid = (unsigned)std::min<uint64_t>(tiles, (uint64_t)ctx().num_sms);
-  const size_t smem = L.total + 1024;
-  set_smem(tc_filter_kernel, smem);
-  LB2_LAUNCH("tc_filter", tc_filter_kernel, grid, NUM_THREADS, smem, map_x, map_c, n, nkc, stages,
-             ws->cnh.p, ws->row_norm2.p, ws->cnh.p + TN, ws->res.p, active, TAU_TF32);
-  LB2_LAUNCH("tc_rerank", rerank_kernel, cdiv(n * 16, 256), 256, 0, x, n, d, cent, bias, ws->res.p,
-             (const uint32_t*)nullptr, dist != nullptr ? 1 : 0, part, dist, valid, ws->fb_rows.p,
-             ws->fb_count.p, active, (const uint32_t*)nullptr, (const uint32_t*)nullptr, 0u, (const float*)nullptr,
-             (float*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr);
-  if (getenv("LB2_TC_STATS") && *getenv("LB2_TC_STATS")) {  // diagnostics: how selective was the filter?
+  const char* filter = resident ? "tc_filter" : opk ? "tc_filter_general16" : "tc_filter_general";
+  if (opk) {
+    if (ws.top1_val.n < n) ws.top1_val.alloc(n);
+    const CUtensorMap map_x = make_map_2d_16(x16, opk == 2, n, d, TM);
+    const CUtensorMap map_c = make_map_2d_16(ws.cpad16.p, opk == 2, Kp, d, TN);
+    launch_general_dyn(opk, 0, grid, smem, map_x, map_c, n, d / (2 * KC), ntiles, cnh, ws.row_norm2.p, cmax2, ws.res.p,
+                       ws.res.p + n, active, tau16_scale(d), nullptr, 0u, ws.top1_val.p, nullptr, nullptr, nullptr,
+                       filter);
+  } else {
+    const CUtensorMap map_x = make_map_2d(x, n, d, TM);
+    const CUtensorMap map_c = make_map_2d(ws.cpad.p, Kp, d, TN);
+    if (resident) {
+      set_smem(tc_filter_kernel, smem);
+      LB2_LAUNCH(filter, tc_filter_kernel, grid, NUM_THREADS, smem, map_x, map_c, n, d / KC, stages, cnh,
+                 ws.row_norm2.p, cn2, ws.res.p, active, TAU_TF32);
+    } else {
+      launch_general_dyn(0, 0, grid, smem, map_x, map_c, n, d / KC, ntiles, cnh, ws.row_norm2.p, cmax2, ws.res.p,
+                         ws.res.p + n, active, TAU_TF32, nullptr, 0u, nullptr, nullptr, nullptr, nullptr, filter);
+    }
+  }
+  LB2_LAUNCH("tc_rerank", rerank_kernel, cdiv(n * 16, 256), 256, 0, x, n, d, cent, bias, ws.res.p,
+             (const uint32_t*)(resident ? nullptr : ws.res.p + n), dist != nullptr ? 1 : 0, part, dist, valid,
+             ws.fb_rows.p, ws.fb_count.p, active, (const uint32_t*)nullptr, (const uint32_t*)nullptr, 0u,
+             (const float*)nullptr, (float*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr);
+  // undecided rows: the exact kernels over the compacted row list (grids sized for the worst case; CTAs beyond the
+  // device-side count exit immediately -> no host synchronisation)
+  const bool refined = tc_refine_and_fallback(x, n, d, cent, K, Kp, bias, ws.cpad.p, cnh, cmax2, part, dist, valid,
+                                              active, ws, /*cT_ready=*/resident, opk, x16);
+  if (getenv("LB2_TC_STATS") && *getenv("LB2_TC_STATS")) {  // diagnostics: how selective was each pass?
     std::vector<uint32_t> h(n);
-    d2h(h.data(), ws->res.p, n);
+    uint32_t c[3];
+    d2h(h.data(), ws.res.p, n);  // (the first pass's verdicts: the later passes keep their own)
+    d2h(c, ws.fb_count.p, 3);
     sync_stream();
     uint64_t f[4] = {0, 0, 0, 0};
     for (uint64_t i = 0; i < n; ++i) f[h[i] >> 30]++;
-    fprintf(stderr, "[lb2 tc_filter] n=%llu K=%d d=%d: unique %.2f%%, two-candidate %.2f%%, exact-fallback %.2f%%\n",
+    fprintf(stderr, "[lb2 %s] n=%llu K=%d d=%d: unique %.2f%%, two-candidate %.2f%%, undecided %.2f%%\n", filter,
             (unsigned long long)n, K, d, 100.0 * f[0] / n, 100.0 * f[1] / n, 100.0 * f[2] / n);
+    if (refined)
+      fprintf(stderr, "[lb2 %s] undecided after pass 1: %u, after the top-3 refinement: %u, full-K exact scan: %u\n",
+              filter, c[0], c[1], c[2]);
   }
-  // flag-2 rows: exact kernel over the compacted row list (grid sized for the worst case; CTAs
-  // beyond the device-side count exit immediately -> no host synchronisation)
-  tc_refine_and_fallback(x, n, d, cent, K, TN, bias, ws->cpad.p, ws->cnh.p, ws->cnh.p + 2 * TN, part, dist, valid,
-                         active, ws, /*cT_ready=*/true);
 }
 
 }  // namespace lb2

@@ -17,11 +17,9 @@ struct TcWorkspace {
   const float* norm_src = nullptr;  // row norms are cached per (pointer, n): valid inside one call
   uint64_t norm_n = 0;
 };
-// announce where the rows of an f32 chunk view lie in their native f16 / bf16 type (nullptr clears); thread-local
-void tc_set_operand_hint(const float* f32, const void* native, int dtype, size_t elems);
 bool tc_assign_supported(uint64_t n, int d, int K, int metric, const float* x);
-// same contract as assign_f32_ex (bias must be padded to 256 floats or NULL); bit-identical outputs
+// same contract as assign_f32_ex (L2, no all_out); bit-identical outputs
 void tc_assign_f32(const float* x, uint64_t n, int d, const float* cent, int K, const float* bias,
                    uint32_t* part, float* dist, uint8_t* valid, const uint8_t* active,
-                   TcWorkspace* ws);
+                   TcWorkspace& ws, const void* x16, int x16_dtype);
 }  // namespace lb2

@@ -230,26 +230,28 @@ def test_chunk_and_stream_paths_ran(make_src, monkeypatch):
 
 def test_native_16bit_rows_across_assignment_sub_chunks(monkeypatch):
     """A row chunk longer than 1.5 times the assignment's own chunk (2^20 rows at d = 64) is split again inside
-    assign_f32_ex; the second part then reads its native f16 rows at an offset from the chunk's operand hint."""
+    assign_f32_ex; the second part then reads its native f16 / bf16 rows at an offset from the chunk's native rows."""
     n, d, K = 1_600_000, 64, 300                 # K > 256: the general filter, which takes the native rows
-    rng = np.random.default_rng(700)
-    cent_m, cent = _model(_tight_groups(rng, K, d) * np.float32(0.05), "f16")
-    pool = (cent[rng.integers(0, K, 8192)] + (rng.standard_normal((8192, d)) * 0.015).astype(np.float32)).astype(np.float16)
-    x = pool[rng.integers(0, len(pool), n)]
-    dev = lb.DeviceArray.from_numpy(x)
-    rows = np.unique(np.concatenate([np.arange((1 << 20) - 64, (1 << 20) + 64), rng.choice(n, 2000, replace=False)]))
-    po, do, vo = ob.compute_membership(cent, x[rows].astype(np.float32), nthreads=NT)
-    _knobs(monkeypatch)                          # default: two row chunks, split at 2^20
-    ref = lb.compute_partitions(cent_m, dev)
-    _knobs(monkeypatch, chunk=1 << 21)           # one row chunk, split at 2^20 by the assignment
-    got = lb.compute_partitions(cent_m, dev)
-    assert all(_same(g, r) for g, r in zip(got, ref))
-    assert np.array_equal(got[2][rows], vo) and np.array_equal(got[0][rows], po) and np.array_equal(got[1][rows], do)
-    # one f16 -> f32 conversion for the centroids and one for the single row chunk; two native-operand filters
-    p = _profiled(lambda: lb.compute_partitions(cent_m, dev))
-    _knobs(monkeypatch)
-    assert _launches(p, "convert_to_f32") == 2 and _launches(p, "tc_filter_general16") == 2, p
-    dev.free()
+    for t, s, seed in (("f16", 0.05, 700), ("bf16", 1.0, 701)):
+        rng = np.random.default_rng(seed)
+        cent_m, cent = _model(_tight_groups(rng, K, d) * np.float32(s), t)
+        pool, pool32 = _typed(cent[rng.integers(0, K, 8192)] + (rng.standard_normal((8192, d)) * (0.3 * s)).astype(np.float32), t)
+        pick = rng.integers(0, len(pool), n)
+        dev = lb.DeviceArray.from_numpy(pool[pick])
+        rows = np.unique(np.concatenate([np.arange((1 << 20) - 64, (1 << 20) + 64), rng.choice(n, 2000, replace=False)]))
+        po, do, vo = ob.compute_membership(cent, pool32[pick[rows]], nthreads=NT)
+        part = lambda: lb.compute_partitions(cent_m, dev, bf16=t == "bf16")
+        _knobs(monkeypatch)                      # default: two row chunks, split at 2^20
+        ref = part()
+        _knobs(monkeypatch, chunk=1 << 21)       # one row chunk, split at 2^20 by the assignment
+        got = part()
+        assert all(_same(g, r) for g, r in zip(got, ref)), t
+        assert np.array_equal(got[2][rows], vo) and np.array_equal(got[0][rows], po) and np.array_equal(got[1][rows], do), t
+        # one conversion to f32 for the centroids and one for the single row chunk; two native-operand filters
+        p = _profiled(part)
+        _knobs(monkeypatch)
+        assert _launches(p, "convert_to_f32") == 2 and _launches(p, "tc_filter_general16") == 2, (t, p)
+        dev.free()
 
 
 # ---- 3. IvfPqIndex.build: unchunked from the device == chunked == chunked and streamed from host memory ---------
