@@ -15,6 +15,8 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
+#include <type_traits>
+
 #include "assign.cuh"
 #include "comm.cuh"
 #include "common.cuh"
@@ -1777,6 +1779,45 @@ void ivfflat_search_f32(const float* centroids, int K, int d, int metric, const 
 // refine: exact distances of k' = k * refine_factor candidates from the raw vectors, then the k
 // best by (distance, row id)  (scanner.rs:2884-2905, flat.rs:95-148)
 // ------------------------------------------------------------------------------------------------
+// The refine plan takes the distance function of the column's own element type (flat.rs:94-150), unlike the
+// IVF_FLAT scan, whose storage is f32 (flat/storage.rs:352-365):
+//  * f16 dot: dot_scalar::<f16, f32, 32> (dot.rs:30-58,133): lane l owns the accumulators l and l + 16, the d % 32
+//    tail comes first, the 32 sums are folded 0..31;
+//  * u8 L2 / dot: exact integer sums, one conversion to f32 (l2.rs:44-49, dot.rs:152-161); the query came in as
+//    u8 too, so its f32 view holds integers;
+//  * everything else (f16 L2, bf16, cosine) as flat_row_distance.
+template <int METRIC, class T>
+__device__ __forceinline__ float refine_row_distance(const float* __restrict__ q, const T* __restrict__ v, int d,
+                                                     int l, unsigned mask, float q_norm) {
+  if constexpr (std::is_same<T, uint8_t>::value && METRIC != METRIC_COSINE) {
+    uint32_t acc = 0;
+    for (int e = l; e < d; e += 16) {
+      const int x = __float2int_rn(q[e]), y = v[e];
+      acc += METRIC == METRIC_DOT ? (uint32_t)(x * y) : (uint32_t)((x - y) * (x - y));
+    }
+#pragma unroll
+    for (int off = 8; off >= 1; off >>= 1) acc += __shfl_xor_sync(mask, acc, off, 16);
+    return finish<METRIC>(__uint2float_rn(acc));
+  } else if constexpr (std::is_same<T, __half>::value && METRIC == METRIC_DOT) {
+    const int n32 = d & ~31;
+    float a0 = 0.0f, a1 = 0.0f;
+    for (int e = l; e < n32; e += 32) {
+      a0 = f_add(a0, __fmul_rn(q[e], ldf<T>(v, e)));
+      a1 = f_add(a1, __fmul_rn(q[e + 16], ldf<T>(v, e + 16)));
+    }
+    float s = 0.0f;  // sequential tail, every lane redundantly
+    for (int e = n32; e < d; ++e) s = f_add(s, __fmul_rn(q[e], ldf<T>(v, e)));
+    float t = 0.0f;
+#pragma unroll
+    for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, a0, qq, 16));
+#pragma unroll
+    for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, a1, qq, 16));
+    return finish<METRIC>(f_add(s, t));
+  } else {
+    return flat_row_distance<METRIC, T>(q, v, d, l, mask, q_norm);
+  }
+}
+
 template <int METRIC, class T>
 __global__ void __launch_bounds__(256)
 refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ vectors,
@@ -1811,7 +1852,7 @@ refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ ve
   for (uint32_t c = tid >> 4; c < cnt; c += 16) {
     const uint64_t id = ids[c];
     float dist = __int_as_float(0x7fc00000);
-    if (id < num_vectors) dist = flat_row_distance<METRIC, T>(qs, vectors + id * (uint64_t)d, d, l, hmask, qn);
+    if (id < num_vectors) dist = refine_row_distance<METRIC, T>(qs, vectors + id * (uint64_t)d, d, l, hmask, qn);
     if (l == 0) cd[c] = dist;
   }
   __syncthreads();

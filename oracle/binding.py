@@ -40,7 +40,9 @@ def lib():
         L.lo_norm_l2_f32.argtypes = [f32p, C.c_uint64]
         L.lo_l2_u8.restype = C.c_float
         L.lo_l2_u8.argtypes = [u8p, u8p, C.c_uint64]
-        for name in ("lo_l2_f16", "lo_l2_bf16"):
+        L.lo_dot_u8.restype = C.c_float
+        L.lo_dot_u8.argtypes = [u8p, u8p, C.c_uint64]
+        for name in ("lo_l2_f16", "lo_l2_bf16", "lo_dot_f16", "lo_dot_bf16"):
             getattr(L, name).restype = C.c_float
             getattr(L, name).argtypes = [C.POINTER(C.c_uint16), C.POINTER(C.c_uint16), C.c_uint64]
         L.lo_normalize_f32.restype = C.c_float
@@ -87,6 +89,36 @@ def l2_f16(x, y):
     x = np.ascontiguousarray(x, dtype=np.float16).view(np.uint16)
     y = np.ascontiguousarray(y, dtype=np.float16).view(np.uint16)
     return float(lib().lo_l2_f16(_p(x, C.c_uint16), _p(y, C.c_uint16), x.size))
+
+
+def _bits16(a, dtype):
+    """16-bit elements as uint16 bit patterns: float16 arrays, or uint16 arrays holding bfloat16 patterns."""
+    return np.ascontiguousarray(a, dtype=dtype).view(np.uint16)
+
+
+def l2_bf16(x, y):
+    """x, y: uint16 arrays of bfloat16 bit patterns (numpy has no bf16 dtype)."""
+    x, y = _bits16(x, np.uint16), _bits16(y, np.uint16)
+    return float(lib().lo_l2_bf16(_p(x, C.c_uint16), _p(y, C.c_uint16), x.size))
+
+
+def dot_f16(x, y):
+    """Dot for f16 (dot.rs:105-136 scalar fallback): 32 f32 lanes."""
+    x, y = _bits16(x, np.float16), _bits16(y, np.float16)
+    return float(lib().lo_dot_f16(_p(x, C.c_uint16), _p(y, C.c_uint16), x.size))
+
+
+def dot_bf16(x, y):
+    """Dot for bf16 (dot.rs:78-83): 32 f32 lanes; x, y are uint16 arrays of bfloat16 bit patterns."""
+    x, y = _bits16(x, np.uint16), _bits16(y, np.uint16)
+    return float(lib().lo_dot_bf16(_p(x, C.c_uint16), _p(y, C.c_uint16), x.size))
+
+
+def dot_u8(x, y):
+    """Dot for u8 (dot.rs:152-161): exact u32 sum, one conversion to f32."""
+    x = np.ascontiguousarray(x, dtype=np.uint8)
+    y = np.ascontiguousarray(y, dtype=np.uint8)
+    return float(lib().lo_dot_u8(_p(x, C.c_uint8), _p(y, C.c_uint8), x.size))
 
 
 def l2_batch(frm, to, d):

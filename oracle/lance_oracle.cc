@@ -363,6 +363,33 @@ float lo_l2_f16(const uint16_t* x, const uint16_t* y, uint64_t d) {
 float lo_l2_bf16(const uint16_t* x, const uint16_t* y, uint64_t d) {
   return l2_lanes16(x, y, d, [](uint16_t v) { return bf16_to_float(v); });
 }
+// f16 / bf16 dot: dot_scalar::<T, f32, 32> (dot.rs:30-58): every element converted to f32, the d % 32 tail summed
+// first, then 32 lane accumulators folded 0..31.  bf16 always takes it (dot.rs:78-83); f16 takes it where the
+// fp16kernels C kernel is not compiled in (dot.rs:105-136, fallback at :133).
+static float dot_lanes32(const uint16_t* x, const uint16_t* y, uint64_t d, float (*conv)(uint16_t)) {
+  const uint64_t n32 = d / 32 * 32;
+  float s = 0.0f;
+  for (uint64_t i = n32; i < d; ++i) s += conv(x[i]) * conv(y[i]);
+  float sums[32];
+  for (int l = 0; l < 32; ++l) sums[l] = 0.0f;
+  for (uint64_t c = 0; c < n32; c += 32)
+    for (int l = 0; l < 32; ++l) sums[l] += conv(x[c + l]) * conv(y[c + l]);
+  float t = 0.0f;
+  for (int l = 0; l < 32; ++l) t += sums[l];
+  return s + t;
+}
+float lo_dot_f16(const uint16_t* x, const uint16_t* y, uint64_t d) {
+  return dot_lanes32(x, y, d, half_to_float);
+}
+float lo_dot_bf16(const uint16_t* x, const uint16_t* y, uint64_t d) {
+  return dot_lanes32(x, y, d, bf16_to_float);
+}
+// u8 dot: exact u32 sum of the products, converted to f32 once (dot.rs:152-161)
+float lo_dot_u8(const uint8_t* x, const uint8_t* y, uint64_t d) {
+  uint32_t s = 0;
+  for (uint64_t i = 0; i < d; ++i) s += uint32_t(x[i]) * uint32_t(y[i]);
+  return float(s);
+}
 // cosine distance, scalar fallback form (cosine.rs:233-238 cosine_scalar with x_norm = norm_l2(x)).
 // The reference f32 path uses f32x16 FMA + platform reduce_sum (cosine.rs:143-174) whose summation
 // order is ISA-specific: tolerance parity only (the reference itself tests at assert_relative_eq).

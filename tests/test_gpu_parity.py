@@ -723,10 +723,28 @@ def test_ivf_flat_matches_oracle_and_full_probe_recall_is_one(metric):
         ids, dists = ix.search(q, k=k, nprobes=nprobes)
         oi, od, oc = ob.ivfflat_search(parts["centroids"], parts["part_offsets"], parts["vectors"],
                                        parts["row_ids"], q, k, nprobes, metric=metric, nthreads=NT)
+        qn = ob.normalize_rows(q, nthreads=NT)
+        off = parts["part_offsets"].astype(np.int64)
         for i in range(len(q)):
             c = int(oc[i])
-            if metric == "cosine":  # FMA lane order differs from the reference's SIMD: tolerance parity
-                assert np.allclose(np.sort(dists[i, :c]), np.sort(od[i, :c]), rtol=1e-5, atol=1e-6)
+            if metric == "cosine":
+                # FMA lanes + shuffle tree, not the reference's scalar order: every distance within
+                # B = 3 (ceil(d/16) + 4) 2^-24 S + 2^-24 of its f64 value (S = sum|q y| / |q||y|, derived in
+                # tests/test_exact_search_variants.py::_cosine_bound), the ids the f64 top-k up to rows within 2B
+                # of the k-th, ascending by (distance, id)
+                def f64(r):
+                    y, x = stored[r].astype(np.float64), qn[i].astype(np.float64)
+                    nrm = np.linalg.norm(x) * np.linalg.norm(y, axis=-1)
+                    return 1.0 - (y @ x) / nrm, 3.0 * (-(-d // 16) + 4) * 2.0 ** -24 * np.abs(y * x).sum(-1) / nrm + 2.0 ** -24
+                got = ids[i, :c].astype(np.int64)
+                ex, bnd = f64(got)
+                assert np.all(np.abs(dists[i, :c] - ex) <= bnd), i
+                assert all((dists[i, j], got[j]) < (dists[i, j + 1], got[j + 1]) for j in range(c - 1)), i
+                pids, _ = ob.find_partitions(parts["centroids"], qn[i], nprobes)
+                cand = np.concatenate([parts["row_ids"][off[p]:off[p + 1]] for p in pids]).astype(np.int64)
+                all_ex, all_b = f64(cand)
+                kth, b2 = np.sort(all_ex)[c - 1], 2 * all_b.max()
+                assert set(cand[all_ex < kth - b2].tolist()) <= set(got.tolist()) and np.all(ex <= kth + b2), i
             else:
                 _check_topk(ids[i, :c], dists[i, :c], oi[i, :c], od[i, :c], k)
     gt, _ = ob.brute_force_topk(stored if metric == "cosine" else data, q if metric != "cosine" else ob.normalize_rows(q), 10,
