@@ -100,10 +100,6 @@ __device__ __forceinline__ void rheap_offer(uint32_t* hk, uint32_t* hp, uint32_t
 // ------------------------------------------------------------------------------------------------
 // block-level helpers
 // ------------------------------------------------------------------------------------------------
-struct KeyIdx {
-  int32_t key;   // total-order key of the distance
-  uint32_t idx;  // tie-breaker (position / id)
-};
 __device__ __forceinline__ bool ki_less(int32_t k1, uint64_t i1, int32_t k2, uint64_t i2) {
   return k1 < k2 || (k1 == k2 && i1 < i2);
 }
@@ -142,26 +138,42 @@ __device__ inline int block_argmin(bool has, int32_t key, uint64_t tie, int32_t*
   return winner;
 }
 
-// per-thread sorted (ascending) list of the k best (distance, position) seen by this thread
-template <int KMAX>
-struct ThreadTopK {
-  float d[KMAX];
-  uint32_t j[KMAX];
-  int cnt = 0;
-  __device__ __forceinline__ void push(float dist, uint32_t pos, int k) {
-    const int32_t key = total_order_key(dist);
-    if (cnt == k && !(key < total_order_key(d[cnt - 1]))) return;  // ties keep earlier rows
-    int p = cnt < k ? cnt : k - 1;
-    while (p > 0 && total_order_key(d[p - 1]) > key) {
-      d[p] = d[p - 1];
-      j[p] = j[p - 1];
-      --p;
+// Ordered emission: round r finds the smallest (key, tie) strictly after round r - 1's among the candidates
+// i in [0, n) for which cand(i, key, tie) returns true, and emit(r, i, key, tie) runs on the thread that proposed
+// it.  Stops after `rounds` rounds or when no candidate is left; returns the number of rounds that emitted.
+template <int NT, class Cand, class Emit>
+__device__ __forceinline__ uint32_t emit_ascending(uint32_t rounds, uint32_t n, Cand cand, Emit emit) {
+  __shared__ int32_t s_key[NT / 32];
+  __shared__ uint64_t s_tie[NT / 32];
+  __shared__ int s_tid[NT / 32 + 1];
+  __shared__ int32_t prev_key;
+  __shared__ uint64_t prev_tie;
+  const int tid = threadIdx.x;
+  uint32_t r = 0;
+  for (; r < rounds; ++r) {
+    int32_t bk = 0;
+    uint64_t bt = 0;
+    uint32_t bi = 0;
+    bool has = false;
+    const int32_t pk = r ? prev_key : 0;
+    const uint64_t pt = r ? prev_tie : 0;
+    for (uint32_t i = tid; i < n; i += NT) {
+      int32_t key;
+      uint64_t tie;
+      if (!cand(i, key, tie) || (r && !ki_less(pk, pt, key, tie))) continue;  // none, or already emitted
+      if (!has || ki_less(key, tie, bk, bt)) { bk = key; bt = tie; bi = i; has = true; }
     }
-    d[p] = dist;
-    j[p] = pos;
-    if (cnt < k) ++cnt;
+    const int w = block_argmin<NT>(has, bk, bt, s_key, s_tie, s_tid);
+    if (w < 0) break;
+    if (tid == w) {
+      prev_key = bk;
+      prev_tie = bt;
+      emit(r, bi, bk, bt);
+    }
+    __syncthreads();
   }
-};
+  return r;
+}
 
 // ------------------------------------------------------------------------------------------------
 // coarse probe selection: nprobes smallest (distance, id), ascending (kmeans.rs:1152-1157)
@@ -169,36 +181,18 @@ struct ThreadTopK {
 __global__ void __launch_bounds__(128)
 select_probes_kernel(const float* __restrict__ all_dists, int K, int nprobes,
                      uint32_t* __restrict__ ids, float* __restrict__ dists) {
-  __shared__ int32_t s_key[4];
-  __shared__ uint64_t s_tie[4];
-  __shared__ int s_tid[5];
-  __shared__ int32_t prev_key;
-  __shared__ uint32_t prev_id;
   const float* row = all_dists + (size_t)blockIdx.x * K;
-  const int tid = threadIdx.x;
-  bool first = true;
-  for (int r = 0; r < nprobes; ++r) {
-    int32_t bk = 0;
-    uint32_t bi = 0;
-    bool has = false;
-    const int32_t pk = first ? 0 : prev_key;
-    const uint32_t pi = first ? 0 : prev_id;
-    for (int c = tid; c < K; c += 128) {
-      const int32_t key = total_order_key(row[c]);
-      if (!first && !ki_less(pk, pi, key, c)) continue;  // already emitted
-      if (!has || ki_less(key, c, bk, bi)) { bk = key; bi = c; has = true; }
-    }
-    const int w = block_argmin<128>(has, bk, bi, s_key, s_tie, s_tid);
-    if (w < 0) break;
-    if (tid == w) {
-      prev_key = bk;
-      prev_id = bi;
-      ids[(size_t)blockIdx.x * nprobes + r] = bi;
-      dists[(size_t)blockIdx.x * nprobes + r] = row[bi];
-    }
-    __syncthreads();
-    first = false;
-  }
+  emit_ascending<128>(
+      nprobes, K,
+      [&](uint32_t c, int32_t& key, uint64_t& tie) {
+        key = total_order_key(row[c]);
+        tie = c;
+        return true;
+      },
+      [&](uint32_t r, uint32_t c, int32_t, uint64_t) {
+        ids[(size_t)blockIdx.x * nprobes + r] = c;
+        dists[(size_t)blockIdx.x * nprobes + r] = row[c];
+      });
 }
 
 // LUT[m][c] = dist(q_m, cb[m][c])  (pq/distance.rs:38-56).  For the common sub-vector widths the
@@ -254,11 +248,6 @@ __device__ __forceinline__ float key_to_float(int32_t key) {
   return __int_as_float(key ^ (int32_t)((uint32_t)(key >> 31) >> 1));
 }
 
-// ------------------------------------------------------------------------------------------------
-// general k (16 < k <= 1024, e.g. k * refine_factor): per chunk the k-th smallest key is found by a
-// 4-pass MSB radix select over shared-memory keys (256-bin histograms), everything below it is
-// kept, ties AT the k-th key are resolved by position (earliest rows survive).
-// ------------------------------------------------------------------------------------------------
 // arguments shared by the fused scan kernels (one slot = one (query, probed partition) pair)
 struct ScanArgs {
   const float* queries; int d; const float* centroids; const float* codebook; int M, ds;
@@ -267,26 +256,309 @@ struct ScanArgs {
   ScanFilter flt;
 };
 
+// the residual query of partition p (v2.rs:316-332) and its LUT, in shared memory (256 threads)
+template <int METRIC, int NBITS>
+__device__ __forceinline__ void stage_query_lut(float* lut, float* qr, const ScanArgs& a, size_t qi, uint32_t p) {
+  const float* q = a.queries + qi * a.d;
+  for (int t = threadIdx.x; t < a.d; t += 256)
+    qr[t] = METRIC == METRIC_DOT ? q[t] : __fsub_rn(q[t], a.centroids[(size_t)p * a.d + t]);
+  __syncthreads();
+  if (NBITS == 8) {
+    build_lut_smem<METRIC>(lut, qr, a.codebook, a.M, a.ds, threadIdx.x);
+  } else {
+    for (int idx = threadIdx.x; idx < a.M * 16; idx += 256)
+      lut[idx] = dist_exact_thread<METRIC>(qr + (idx / 16) * a.ds, a.codebook + (size_t)idx * a.ds, a.ds);
+  }
+  __syncthreads();
+}
+
+// one row's 8-bit ADC distance: the reference's m-ascending f32 sum of LUT[m][code[m]] (pq/distance.rs:109-144)
+__device__ __forceinline__ float pq8_row_distance(const float* lut, const uint8_t* __restrict__ rp, int M) {
+  float dist = 0.0f;
+  if ((M & 15) == 0) {
+    const uint4* rp4 = reinterpret_cast<const uint4*>(rp);
+    for (int c16 = 0; c16 < M / 16; ++c16) {
+      const uint4 v = __ldg(rp4 + c16);
+      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+      const float* l0 = lut + c16 * 16 * 256;
+#pragma unroll
+      for (int aa = 0; aa < 4; ++aa)
+#pragma unroll
+        for (int bb = 0; bb < 4; ++bb)
+          dist = f_add(dist, l0[(aa * 4 + bb) * 256 + ((w[aa] >> (8 * bb)) & 0xff)]);
+    }
+  } else {
+    for (int m = 0; m < M; ++m) dist = f_add(dist, lut[m * 256 + rp[m]]);
+  }
+  return dist;
+}
+
+// 4-bit table quantisation (pq/distance.rs:147-242), one block of 256 threads: qmin = min(table) (f32::min ignores
+// NaN), qmax = max of the flat rows' distances flat_dist(j), j < flat_num, in total order; qt = the table quantised
+// to u8, params = {qmin, (qmax - qmin) / 255}.  r_mx / r_mn: 256 entries of reduction scratch each.
+template <class FlatDist>
+__device__ __forceinline__ void pq4_quantize(const float* lut, int M, uint64_t flat_num, FlatDist flat_dist, uint8_t* qt,
+                             float* params, int32_t* r_mx, float* r_mn) {
+  const int tid = threadIdx.x;
+  int32_t mx = (int32_t)0x80000000;
+  for (uint64_t j = tid; j < flat_num; j += 256) mx = max(mx, total_order_key(flat_dist(j)));
+  float mn = __int_as_float(0x7f800000);
+  for (int i = tid; i < M * 16; i += 256) mn = fminf(mn, lut[i]);
+  r_mx[tid] = mx;
+  r_mn[tid] = mn;
+  __syncthreads();
+  for (int o = 128; o >= 1; o >>= 1) {
+    if (tid < o) {
+      r_mx[tid] = max(r_mx[tid], r_mx[tid + o]);
+      r_mn[tid] = fminf(r_mn[tid], r_mn[tid + o]);
+    }
+    __syncthreads();
+  }
+  const float qmax = key_to_float(r_mx[0]), qmin = r_mn[0];
+  __syncthreads();
+  const float factor = __fdiv_rn(255.0f, __fsub_rn(qmax, qmin));
+  for (int i = tid; i < M * 16; i += 256) {
+    const float v = roundf(__fmul_rn(__fsub_rn(lut[i], qmin), factor));  // f32::round: half away from zero
+    qt[i] = (v != v) ? 0 : v <= 0.0f ? 0 : v >= 255.0f ? 255 : (uint8_t)v;  // `as u8`: saturating, NaN -> 0
+  }
+  if (tid == 0) {
+    params[0] = qmin;
+    params[1] = __fdiv_rn(__fsub_rn(qmax, qmin), 255.0f);
+  }
+  __syncthreads();
+}
+
+// ------------------------------------------------------------------------------------------------
+// Exact top-k of one slot (16 < k <= 1024 in the PQ scan, every k in the IVF_FLAT scan and lb2_flat_topk), 256
+// threads.  A row's distance is an unsigned order key (unsigned order == f32::total_cmp order); the caller's fill
+// step writes the keys of rows [c0, c0 + clen) to ukey.  Per chunk of SCAN_CHUNK rows the kk = k + 1 smallest
+// (key, position) pairs of the chunk and the winners carried from earlier chunks are found by a 4-pass MSB radix
+// select over shared-memory keys (256-bin histograms): everything below the kk-th key is kept, ties AT it are
+// resolved by position (earliest rows survive).  Selecting one more than asked for exposes ties that overflow the
+// k-th place; those slots are replayed through the reference's heap.
+// ------------------------------------------------------------------------------------------------
+// shared memory of one slot (u32 words): ukey[SCAN_CHUNK + kk] (a chunk's keys, then the carried winners' keys),
+// cpos[kk] (the carried winners' positions), nkey[kk] / npos[kk] (the next winners; the result; the replay heap)
+__host__ __device__ constexpr size_t slot_smem_bytes(int k) {
+  return sizeof(uint32_t) * (SCAN_CHUNK + 4 * (size_t)(k + 1));
+}
+struct SlotSmem {
+  uint32_t *ukey, *cpos, *nkey, *npos;
+  __device__ SlotSmem(void* base, int kk)
+      : ukey(static_cast<uint32_t*>(base)), cpos(ukey + SCAN_CHUNK + kk), nkey(cpos + kk), npos(nkey + kk) {}
+};
+
+// a row the prefilter (bit at off + row) or the range removes
+__device__ __forceinline__ bool slot_excluded(const ScanFilter& f, uint64_t off, uint32_t row, uint32_t ukey) {
+  return !row_allowed(f.allow, off + row) || !key_in_range(f, (int32_t)(ukey ^ 0x80000000u));
+}
+
+// The kk smallest (key, position) pairs of rows [0, n); excluded rows take the maximal key, so they only surface when
+// fewer than kk rows are left.  Returns their number; they are left unordered at ukey[SCAN_CHUNK ..) / cpos.
+template <class Fill>
+__device__ __forceinline__ uint32_t slot_select(const SlotSmem& s, uint32_t n, uint32_t kk, const ScanFilter& flt, uint64_t off,
+                                Fill fill) {
+  __shared__ uint32_t hist[256], s_wsum[8];
+  __shared__ uint32_t s_prefix, s_need, s_eq, s_out;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const bool filtering = flt.allow != nullptr || flt.range;
+  uint32_t nw = 0;
+  // once kk winners are carried, a chunk row whose key is >= lim (>= the kk-th carried key) cannot enter: kk
+  // carried winners precede it in (key, position) order.  Such rows are left out of the pool.
+  uint32_t lim = 0xffffffffu;
+  bool full = false;
+  for (uint32_t c0 = 0; c0 < n; c0 += SCAN_CHUNK) {
+    const uint32_t clen = min((uint32_t)SCAN_CHUNK, n - c0);
+    fill(c0, clen);
+    __syncthreads();
+    if (filtering) {
+      for (uint32_t j = tid; j < clen; j += 256)
+        if (slot_excluded(flt, off, c0 + j, s.ukey[j])) s.ukey[j] = 0xffffffffu;
+      __syncthreads();
+    }
+    // pool element i: i < clen -> (ukey[i], c0 + i), else the carried winner i - clen at ukey[SCAN_CHUNK ..)
+    const uint32_t pool = clen + nw;
+    auto key_at = [&](uint32_t i) { return i < clen ? s.ukey[i] : s.ukey[SCAN_CHUNK + (i - clen)]; };
+    auto pos_at = [&](uint32_t i) { return i < clen ? c0 + i : s.cpos[i - clen]; };
+    auto pooled = [&](uint32_t i, uint32_t kv) { return !full || i >= clen || kv < lim; };
+    if (pool <= kk) {
+      for (uint32_t i = tid; i < pool; i += 256) { s.nkey[i] = key_at(i); s.npos[i] = pos_at(i); }
+      __syncthreads();
+      for (uint32_t i = tid; i < pool; i += 256) { s.ukey[SCAN_CHUNK + i] = s.nkey[i]; s.cpos[i] = s.npos[i]; }
+      nw = pool;
+      full = nw == kk;
+      __syncthreads();
+      continue;
+    }
+    if (tid == 0) { s_prefix = 0; s_need = kk; }
+    uint32_t mask = 0;
+    for (int shift = 24; shift >= 0; shift -= 8) {
+      hist[tid] = 0;
+      __syncthreads();
+      const uint32_t prefix = s_prefix, need = s_need;
+      for (uint32_t i = tid; i < pool; i += 256) {
+        const uint32_t kv = key_at(i);
+        if (pooled(i, kv) && (kv & mask) == prefix) atomicAdd(&hist[(kv >> shift) & 255u], 1u);
+      }
+      __syncthreads();
+      // the bin of the need-th key: the one whose inclusive prefix sum first reaches `need` (bin = thread)
+      const uint32_t h = hist[tid];
+      uint32_t cum = h;
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t v = __shfl_up_sync(0xffffffffu, cum, o);
+        if (lane >= o) cum += v;
+      }
+      if (lane == 31) s_wsum[warp] = cum;
+      __syncthreads();
+      for (int w = 0; w < warp; ++w) cum += s_wsum[w];
+      if (cum >= need && cum - h < need) {
+        s_need = need - (cum - h);
+        s_prefix = prefix | ((uint32_t)tid << shift);
+        s_eq = h;
+      }
+      mask |= 0xffu << shift;
+      __syncthreads();
+    }
+    const uint32_t T = s_prefix, need = s_need, eq = s_eq;  // take all keys < T and `need` of the `eq` keys == T
+    if (tid == 0) s_out = 0;
+    __syncthreads();
+    for (uint32_t i = tid; i < pool; i += 256) {
+      const uint32_t kv = key_at(i);
+      if (pooled(i, kv) && (kv < T || (kv == T && eq == need))) {
+        const uint32_t at = atomicAdd(&s_out, 1u);
+        s.nkey[at] = kv;
+        s.npos[at] = pos_at(i);
+      }
+    }
+    __syncthreads();
+    if (eq != need)  // ties at the last key: the `need` smallest positions survive (rare)
+      emit_ascending<256>(
+          need, pool,
+          [&](uint32_t i, int32_t& key, uint64_t& tie) {
+            const uint32_t kv = key_at(i);
+            key = 0;
+            tie = pos_at(i);
+            return kv == T && pooled(i, kv);
+          },
+          [&](uint32_t, uint32_t, int32_t, uint64_t tie) {
+            const uint32_t at = s_out;
+            s.nkey[at] = T;
+            s.npos[at] = (uint32_t)tie;
+            s_out = at + 1;
+          });
+    const uint32_t got = s_out;  // == kk
+    __syncthreads();
+    for (uint32_t i = tid; i < got; i += 256) { s.ukey[SCAN_CHUNK + i] = s.nkey[i]; s.cpos[i] = s.npos[i]; }
+    nw = got;
+    full = true;
+    lim = T;
+    __syncthreads();
+  }
+  return nw;
+}
+
+// The finish, on the nw <= kk winners in (key, position) order: excluded winners at the end are dropped (they carry
+// the maximal key; an admitted row whose key is the maximal one, e.g. a NaN distance, keeps the excluded winners before
+// it).  If kk winners remain and the last two share a key, more rows tie at the k-th distance than fit and the
+// reference's heap decides: returns false.  Otherwise leaves the admitted winners among the first k at nkey / npos
+// (unordered), sets *cnt and returns true.
+__device__ __forceinline__ bool slot_finish(const SlotSmem& s, uint32_t nw, uint32_t kk, const ScanFilter& flt, uint64_t off,
+                            uint32_t* cnt) {
+  __shared__ uint32_t s_kept, s_max, s_maxcnt, s_last, s_mid, s_out;
+  const int tid = threadIdx.x;
+  if (tid == 0) { s_kept = 0; s_max = 0; s_maxcnt = 0; s_last = 0; s_mid = 0; s_out = 0; }
+  __syncthreads();
+  for (uint32_t i = tid; i < nw; i += 256) {
+    const uint32_t key = s.ukey[SCAN_CHUNK + i], pos = s.cpos[i];
+    if (slot_excluded(flt, off, pos, key)) continue;
+    atomicAdd(&s_kept, 1u);
+    atomicMax(&s_max, key);
+    if (key == 0xffffffffu) atomicMax(&s_last, pos + 1);  // 1 + the last admitted position at the maximal key
+  }
+  __syncthreads();
+  const uint32_t mx = s_max, last = s_last;
+  for (uint32_t i = tid; i < nw; i += 256) {
+    const uint32_t key = s.ukey[SCAN_CHUNK + i], pos = s.cpos[i];
+    if (slot_excluded(flt, off, pos, key)) {
+      if (pos + 1 < last) atomicAdd(&s_mid, 1u);  // excluded, but in front of an admitted winner
+    } else if (key == mx) {
+      atomicAdd(&s_maxcnt, 1u);
+    }
+  }
+  __syncthreads();
+  const uint32_t kept = s_kept, mid = s_mid;
+  const bool at_k = kept + mid == kk;
+  if (at_k && s_maxcnt + mid >= 2) return false;  // block-uniform
+  for (uint32_t i = tid; i < nw; i += 256) {
+    const uint32_t key = s.ukey[SCAN_CHUNK + i], pos = s.cpos[i];
+    if (slot_excluded(flt, off, pos, key) || (at_k && key == mx)) continue;  // at_k: the (k+1)-th is the unique max
+    const uint32_t at = atomicAdd(&s_out, 1u);
+    s.nkey[at] = key;
+    s.npos[at] = pos;
+  }
+  __syncthreads();
+  *cnt = s_out;
+  return true;
+}
+
+// The reference's own loop (flat/index.rs:116-165): rows in storage order, keys filled one chunk ahead of the single
+// thread that drives the heap.  Leaves the heap's content at nkey / npos and returns its size.
+template <class Fill>
+__device__ __forceinline__ uint32_t slot_replay(const SlotSmem& s, uint32_t n, uint32_t k, const ScanFilter& flt, uint64_t off,
+                                Fill fill) {
+  __shared__ uint32_t s_len;
+  const bool filtering = flt.allow != nullptr || flt.range;
+  uint32_t len = 0;
+  for (uint32_t c0 = 0; c0 < n; c0 += SCAN_CHUNK) {
+    const uint32_t clen = min((uint32_t)SCAN_CHUNK, n - c0);
+    fill(c0, clen);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (uint32_t j = 0; j < clen; ++j) {
+        const uint32_t key = s.ukey[j];
+        if (filtering && slot_excluded(flt, off, c0 + j, key)) continue;
+        rheap_offer(s.nkey, s.npos, len, k, key, c0 + j);
+      }
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) s_len = len;
+  __syncthreads();
+  return s_len;
+}
+
+// The exact top-k of a slot of n rows: <= k winners at nkey / npos (unordered); returns their number.  replay: go
+// straight to the heap loop.
+template <class Fill>
+__device__ __forceinline__ uint32_t slot_topk(const SlotSmem& s, uint32_t n, int k, const ScanFilter& flt, uint64_t off, bool replay,
+                              Fill fill) {
+  if (!replay) {
+    uint32_t cnt;
+    if (slot_finish(s, slot_select(s, n, k + 1, flt, off, fill), k + 1, flt, off, &cnt)) return cnt;
+    __syncthreads();
+  }
+  return slot_replay(s, n, k, flt, off, fill);
+}
+
+// a slot's winners -> its candidate list (unordered)
+__device__ __forceinline__ void write_slot(const SlotSmem& s, uint32_t cnt, size_t slot, int k, uint64_t off,
+                                           const uint64_t* __restrict__ row_ids, float* __restrict__ cand_d,
+                                           uint64_t* __restrict__ cand_id, uint32_t* __restrict__ cand_cnt) {
+  for (uint32_t i = threadIdx.x; i < cnt; i += 256) {
+    cand_d[slot * k + i] = key_to_float((int32_t)(s.nkey[i] ^ 0x80000000u));
+    cand_id[slot * k + i] = row_ids[off + s.npos[i]];
+  }
+  if (threadIdx.x == 0) cand_cnt[slot] = cnt;
+}
+
 template <int METRIC, int NBITS>
 __device__ void radix_slot(const ScanArgs& a, size_t slot, bool replay) {
   extern __shared__ float smem[];
-  constexpr int NCODE = 1 << NBITS;
-  const int M = a.M, ds = a.ds, d = a.d, k = a.k, np = a.np;
-  const int kk = k + 1;  // one more than asked for: exposes ties that overflow the k-th place
-  const uint64_t* __restrict__ allow = a.flt.allow;
-  const bool filtering = allow != nullptr || a.flt.range;
-  float* lut = smem;                                                   // [M*NCODE] (8-bit: M*256)
-  float* qr = lut + M * 256;                                           // [d]
-  uint32_t* ukey = reinterpret_cast<uint32_t*>(qr + d);                // [SCAN_CHUNK + kk] order-preserving keys
-  uint32_t* cpos = ukey + SCAN_CHUNK + kk;                             // [kk] positions of carried winners
-  uint32_t* nkey = cpos + kk;                                          // [kk] next winners / the replay heap
-  uint32_t* npos = nkey + kk;                                          // [kk]
-  __shared__ uint32_t hist[256];
-  __shared__ uint32_t s_prefix, s_need, s_eq, s_out, s_max, s_maxcnt;
-  __shared__ int32_t s_key[8];
-  __shared__ uint64_t s_tie[8];
-  __shared__ int s_tid[9];
-  __shared__ uint32_t prev_pos;
+  const int M = a.M, d = a.d, k = a.k, np = a.np;
+  float* lut = smem;                   // [M*16] (4-bit) or [M*256] (8-bit)
+  float* qr = lut + M * 256;           // [d]
+  const SlotSmem s(qr + d, k + 1);
   const int tid = threadIdx.x;
   const int pi = (int)(slot % np);
   const size_t qi = slot / np;
@@ -297,25 +569,13 @@ __device__ void radix_slot(const ScanArgs& a, size_t slot, bool replay) {
     if (tid == 0) a.cand_cnt[slot] = 0;
     return;
   }
-  const float* q = a.queries + qi * d;
-  for (int t = tid; t < d; t += 256)
-    qr[t] = METRIC == METRIC_DOT ? q[t] : __fsub_rn(q[t], a.centroids[(size_t)p * d + t]);  // v2.rs:316-332
-  __syncthreads();
-  if (NBITS == 8) {
-    build_lut_smem<METRIC>(lut, qr, a.codebook, M, ds, tid);
-  } else {
-    for (int idx = tid; idx < M * NCODE; idx += 256)
-      lut[idx] = dist_exact_thread<METRIC>(qr + (idx / NCODE) * ds, a.codebook + (size_t)idx * ds, ds);
-  }
-  __syncthreads();
-  constexpr int CW_DIV = NBITS == 4 ? 2 : 1;
-  const int cw = M / CW_DIV;  // code bytes per row
+  stage_query_lut<METRIC, NBITS>(lut, qr, a, qi, p);
+  const int cw = NBITS == 4 ? M / 2 : M;  // code bytes per row
   const uint8_t* pc = a.codes + off * cw;
   const float dot_fix = (float)M - 1.0f;
   // ---- 4-bit (pq/distance.rs:147-242): rows [0, flat_num) and the last n_p % 16 rows are exact f32 sums;
-  // the others go through the table quantised to u8 with qmin = min(table), qmax = max(flat rows).
-  // With a prefilter the reference scores row by row with DistCalculator::distance (exact, pq/storage.rs:
-  // 895-916), so every row is exact then.
+  // the others go through the table quantised to u8.  With a prefilter the reference scores row by row with
+  // DistCalculator::distance (exact, pq/storage.rs:895-916), so every row is exact then.
   __shared__ uint8_t qt[NBITS == 4 ? 256 * 16 : 1];  // M <= 256 sub-vectors x 16 entries
   __shared__ float s_q[2];                                // qmin, (qmax - qmin) / 255
   const uint32_t flat_num = NBITS == 4 ? min((uint32_t)max(200, k), n_p) : 0;
@@ -330,233 +590,35 @@ __device__ void radix_slot(const ScanArgs& a, size_t slot, bool replay) {
     }
     return dist;
   };
-  if (NBITS == 4 && allow == nullptr) {
-    int32_t mx = (int32_t)0x80000000;
-    for (uint32_t j = tid; j < flat_num; j += 256) mx = max(mx, total_order_key(exact4(j)));
-    float mn = __int_as_float(0x7f800000);
-    for (int i = tid; i < M * 16; i += 256) mn = fminf(mn, lut[i]);
-    // block reduce through the (still unused) selection scratch
-    int32_t* r_mx = reinterpret_cast<int32_t*>(hist);
-    float* r_mn = reinterpret_cast<float*>(ukey);
-    r_mx[tid] = mx;
-    r_mn[tid] = mn;
-    __syncthreads();
-    for (int o = 128; o >= 1; o >>= 1) {
-      if (tid < o) {
-        r_mx[tid] = max(r_mx[tid], r_mx[tid + o]);
-        r_mn[tid] = fminf(r_mn[tid], r_mn[tid + o]);
-      }
-      __syncthreads();
-    }
-    const float qmax = key_to_float(r_mx[0]), qmin = r_mn[0];
-    __syncthreads();
-    const float factor = __fdiv_rn(255.0f, __fsub_rn(qmax, qmin));
-    for (int i = tid; i < M * 16; i += 256) {
-      const float v = roundf(__fmul_rn(__fsub_rn(lut[i], qmin), factor));
-      qt[i] = (v != v) ? 0 : v <= 0.0f ? 0 : v >= 255.0f ? 255 : (uint8_t)v;
-    }
-    if (tid == 0) {
-      s_q[0] = qmin;
-      s_q[1] = __fdiv_rn(__fsub_rn(qmax, qmin), 255.0f);
-    }
-    __syncthreads();
-  }
-  // unsigned order key of row `row`'s distance (unsigned order == f32::total_cmp order)
-  auto row_key = [&](uint32_t row) -> uint32_t {
-    float dist = 0.0f;
-    if (NBITS == 4) {
-      if (allow != nullptr || row < flat_num || row >= n_p - rem16) {
-        dist = exact4(row);
+  if (NBITS == 4 && a.flt.allow == nullptr)  // the selection's (still unused) key buffer is the scratch
+    pq4_quantize(lut, M, flat_num, exact4, qt, s_q, reinterpret_cast<int32_t*>(s.ukey),
+                 reinterpret_cast<float*>(s.ukey + 256));
+  auto fill = [&](uint32_t c0, uint32_t clen) {
+    for (uint32_t j = tid; j < clen; j += 256) {
+      const uint32_t row = c0 + j;
+      float dist;
+      if constexpr (NBITS == 4) {
+        if (a.flt.allow != nullptr || row < flat_num || row >= n_p - rem16) {
+          dist = exact4(row);
+        } else {
+          const uint8_t* rp = pc + (size_t)row * cw;
+          uint32_t qs = 0;  // saturating u8 adds of non-negative terms == min(255, sum)
+          for (int i2 = 0; i2 < cw; ++i2) {
+            const uint8_t c = rp[i2];
+            qs += qt[(2 * i2) * 16 + (c & 0xF)];
+            qs += qt[(2 * i2 + 1) * 16 + (c >> 4)];
+          }
+          dist = __fadd_rn(__fmul_rn((float)min(qs, 255u), s_q[1]), s_q[0]);
+        }
       } else {
-        const uint8_t* rp = pc + (size_t)row * cw;
-        uint32_t qs = 0;  // saturating u8 adds of non-negative terms == min(255, sum)
-        for (int i2 = 0; i2 < cw; ++i2) {
-          const uint8_t c = rp[i2];
-          qs += qt[(2 * i2) * 16 + (c & 0xF)];
-          qs += qt[(2 * i2 + 1) * 16 + (c >> 4)];
-        }
-        dist = __fadd_rn(__fmul_rn((float)min(qs, 255u), s_q[1]), s_q[0]);
+        dist = pq8_row_distance(lut, pc + (size_t)row * M, M);
       }
-    } else if ((M & 15) == 0) {
-      const uint4* rp = reinterpret_cast<const uint4*>(pc + (size_t)row * M);
-      for (int c16 = 0; c16 < M / 16; ++c16) {
-        const uint4 v = __ldg(rp + c16);
-        const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-        const float* l0 = lut + c16 * 16 * 256;
-#pragma unroll
-        for (int aa = 0; aa < 4; ++aa)
-#pragma unroll
-          for (int bb = 0; bb < 4; ++bb)
-            dist = f_add(dist, l0[(aa * 4 + bb) * 256 + ((w[aa] >> (8 * bb)) & 0xff)]);
-      }
-    } else {
-      const uint8_t* rp = pc + (size_t)row * M;
-      for (int m = 0; m < M; ++m) dist = f_add(dist, lut[m * 256 + rp[m]]);
+      if (METRIC == METRIC_DOT) dist = __fsub_rn(dist, dot_fix);  // pq/storage.rs:957-958
+      s.ukey[j] = (uint32_t)total_order_key(dist) ^ 0x80000000u;
     }
-    if (METRIC == METRIC_DOT) dist = __fsub_rn(dist, dot_fix);
-    return (uint32_t)total_order_key(dist) ^ 0x80000000u;
   };
-  auto excluded = [&](uint32_t row, uint32_t key) -> bool {
-    return !row_allowed(allow, off + row) || !key_in_range(a.flt, (int32_t)(key ^ 0x80000000u));
-  };
-
-  uint32_t nw = 0;
-  if (!replay) {
-    for (uint32_t c0 = 0; c0 < n_p; c0 += SCAN_CHUNK) {
-      const uint32_t clen = min((uint32_t)SCAN_CHUNK, n_p - c0);
-      for (uint32_t j = tid; j < clen; j += 256) {
-        if (!row_allowed(allow, off + c0 + j)) {
-          ukey[j] = 0xffffffffu;
-          continue;
-        }
-        const uint32_t key = row_key(c0 + j);
-        ukey[j] = key_in_range(a.flt, (int32_t)(key ^ 0x80000000u)) ? key : 0xffffffffu;
-      }
-      // carried winners sit at ukey[SCAN_CHUNK ..); pool element i: i < clen -> (ukey[i], c0+i), else carried
-      __syncthreads();
-      const uint32_t pool = clen + nw;
-      auto key_at = [&](uint32_t i) { return i < clen ? ukey[i] : ukey[SCAN_CHUNK + (i - clen)]; };
-      auto pos_at = [&](uint32_t i) { return i < clen ? c0 + i : cpos[i - clen]; };
-      if (pool <= (uint32_t)kk) {
-        for (uint32_t i = tid; i < pool; i += 256) { nkey[i] = key_at(i); npos[i] = pos_at(i); }
-        __syncthreads();
-        for (uint32_t i = tid; i < pool; i += 256) { ukey[SCAN_CHUNK + i] = nkey[i]; cpos[i] = npos[i]; }
-        nw = pool;
-        __syncthreads();
-        continue;
-      }
-      if (tid == 0) { s_prefix = 0; s_need = (uint32_t)kk; }
-      uint32_t mask = 0;
-      for (int shift = 24; shift >= 0; shift -= 8) {
-        hist[tid] = 0;
-        __syncthreads();
-        const uint32_t prefix = s_prefix;
-        for (uint32_t i = tid; i < pool; i += 256) {
-          const uint32_t kv = key_at(i);
-          if ((kv & mask) == prefix) atomicAdd(&hist[(kv >> shift) & 255u], 1u);
-        }
-        __syncthreads();
-        if (tid == 0) {
-          uint32_t need = s_need, cum = 0;
-          int b = 0;
-          for (; b < 256; ++b) {
-            if (cum + hist[b] >= need) break;
-            cum += hist[b];
-          }
-          s_need = need - cum;
-          s_prefix = prefix | ((uint32_t)b << shift);
-          s_eq = hist[b];
-        }
-        mask |= 0xffu << shift;
-        __syncthreads();
-      }
-      const uint32_t T = s_prefix, need = s_need, eq = s_eq;  // take all keys < T and `need` of the `eq` keys == T
-      if (tid == 0) s_out = 0;
-      __syncthreads();
-      for (uint32_t i = tid; i < pool; i += 256) {
-        const uint32_t kv = key_at(i);
-        if (kv < T || (kv == T && eq == need)) {
-          const uint32_t at = atomicAdd(&s_out, 1u);
-          nkey[at] = kv;
-          npos[at] = pos_at(i);
-        }
-      }
-      __syncthreads();
-      if (eq != need) {  // ties at the last key: the `need` smallest positions survive (rare)
-        bool first = true;
-        for (uint32_t r = 0; r < need; ++r) {
-          uint32_t bp = 0xffffffffu;
-          bool has = false;
-          const uint32_t pp = first ? 0 : prev_pos;
-          for (uint32_t i = tid; i < pool; i += 256) {
-            if (key_at(i) != T) continue;
-            const uint32_t ps = pos_at(i);
-            if (!first && ps <= pp) continue;
-            if (!has || ps < bp) { bp = ps; has = true; }
-          }
-          const int w = block_argmin<256>(has, 0, bp, s_key, s_tie, s_tid);
-          if (tid == w) {
-            prev_pos = bp;
-            const uint32_t at = s_out;
-            nkey[at] = T;
-            npos[at] = bp;
-            s_out = at + 1;
-          }
-          __syncthreads();
-          first = false;
-        }
-      }
-      const uint32_t got = s_out;  // == kk
-      __syncthreads();
-      for (uint32_t i = tid; i < got; i += 256) { ukey[SCAN_CHUNK + i] = nkey[i]; cpos[i] = npos[i]; }
-      nw = got;
-      __syncthreads();
-    }
-    // ---- the kk = k + 1 smallest (key, position) pairs are in hand.  Excluded rows (prefilter / range)
-    // carry the maximal key and are dropped here; if the two largest survivors share a key, more rows tie
-    // at the k-th distance than fit and the reference's heap decides -> replay
-    if (tid == 0) { s_out = 0; s_max = 0; s_maxcnt = 0; }
-    __syncthreads();
-    for (uint32_t i = tid; i < nw; i += 256) {
-      const uint32_t key = ukey[SCAN_CHUNK + i], pos = cpos[i];
-      const bool keep = !filtering || (row_allowed(allow, off + pos) && !(a.flt.range && key == 0xffffffffu));
-      if (keep) {
-        const uint32_t at = atomicAdd(&s_out, 1u);
-        nkey[at] = key;
-        npos[at] = pos;
-        atomicMax(&s_max, key);
-      }
-    }
-    __syncthreads();
-    nw = s_out;
-    if (nw == (uint32_t)kk) {
-      for (uint32_t i = tid; i < nw; i += 256)
-        if (nkey[i] == s_max) atomicAdd(&s_maxcnt, 1u);
-      __syncthreads();
-      replay = s_maxcnt >= 2;  // block-uniform
-    }
-    if (!replay) {
-      const bool drop_max = nw == (uint32_t)kk;
-      const uint32_t mx = s_max;
-      __syncthreads();
-      if (tid == 0) s_out = 0;
-      __syncthreads();
-      for (uint32_t i = tid; i < nw; i += 256) {
-        if (drop_max && nkey[i] == mx) continue;
-        const uint32_t at = atomicAdd(&s_out, 1u);
-        a.cand_d[slot * k + at] = key_to_float((int32_t)(nkey[i] ^ 0x80000000u));
-        a.cand_id[slot * k + at] = a.row_ids[off + npos[i]];
-      }
-      __syncthreads();
-      if (tid == 0) a.cand_cnt[slot] = s_out;
-      return;
-    }
-    __syncthreads();
-  }
-  // ---- replay: the reference's own loop (flat/index.rs:116-165), rows in storage order, distances
-  // computed in parallel one chunk ahead of the single thread that drives the heap
-  uint32_t len = 0;
-  for (uint32_t c0 = 0; c0 < n_p; c0 += SCAN_CHUNK) {
-    const uint32_t clen = min((uint32_t)SCAN_CHUNK, n_p - c0);
-    for (uint32_t j = tid; j < clen; j += 256) ukey[j] = row_key(c0 + j);
-    __syncthreads();
-    if (tid == 0) {
-      for (uint32_t j = 0; j < clen; ++j) {
-        const uint32_t key = ukey[j];
-        if (filtering && excluded(c0 + j, key)) continue;
-        rheap_offer(nkey, npos, len, (uint32_t)k, key, c0 + j);
-      }
-    }
-    __syncthreads();
-  }
-  if (tid == 0) s_out = len;
-  __syncthreads();
-  len = s_out;
-  for (uint32_t i = tid; i < len; i += 256) {
-    a.cand_d[slot * k + i] = key_to_float((int32_t)(nkey[i] ^ 0x80000000u));
-    a.cand_id[slot * k + i] = a.row_ids[off + npos[i]];
-  }
-  if (tid == 0) a.cand_cnt[slot] = len;
+  const uint32_t cnt = slot_topk(s, n_p, k, a.flt, off, replay, fill);
+  write_slot(s, cnt, slot, k, off, a.row_ids, a.cand_d, a.cand_id, a.cand_cnt);
 }
 
 // grid (np, nq): one CTA per slot; or, with a replay list (slots the fast kernel could not settle because of
@@ -585,6 +647,32 @@ __device__ __forceinline__ uint64_t pack_cand(int32_t key, uint32_t pos) {
 }
 __device__ __forceinline__ int32_t cand_key(uint64_t c) { return (int32_t)((uint32_t)(c >> 32) ^ 0x80000000u); }
 __device__ __forceinline__ uint32_t cand_pos(uint64_t c) { return (uint32_t)c; }
+
+// End of a fast 8-bit slot, threads t = 0 .. nt - 1: win[0..nw) ascending by (key, position), nw <= k + 1.  If the
+// k-th and the (k+1)-th share a key, more rows tie at the k-th distance than fit: which of them the reference's
+// BinaryHeap keeps depends on its sift order, so the slot goes on the replay list (ivfpq_scan_radix_kernel in list
+// mode restates that loop); so does a slot the kernel could not settle (replay).  Otherwise the first min(nw, k).
+__device__ __forceinline__ void fast_slot_epilogue(const ScanArgs& a, uint32_t slot, uint64_t off, const uint64_t* win,
+                                                   uint32_t nw, bool replay, int t, int nt, uint32_t* rlist,
+                                                   uint32_t* rcount) {
+  const int k = a.k;
+  if (!replay && nw == (uint32_t)k + 1) {
+    replay = cand_key(win[k]) == cand_key(win[k - 1]);
+    nw = k;
+  }
+  if (replay) {
+    if (t == 0) {
+      rlist[atomicAdd(rcount, 1u)] = slot;
+      a.cand_cnt[slot] = 0;
+    }
+    return;
+  }
+  for (uint32_t i = t; i < nw; i += nt) {
+    a.cand_d[(size_t)slot * k + i] = key_to_float(cand_key(win[i]));
+    a.cand_id[(size_t)slot * k + i] = a.row_ids[off + cand_pos(win[i])];
+  }
+  if (t == 0) a.cand_cnt[slot] = nw;
+}
 
 // bitonic merge of a 32-lane bitonic sequence into ascending order (5 compare-exchange steps)
 __device__ __forceinline__ uint64_t warp_bitonic_merge32(uint64_t v, int lane) {
@@ -633,7 +721,7 @@ __global__ void __launch_bounds__(256, 6)
 ivfpq_scan_kernel(const ScanArgs a, uint32_t* __restrict__ rlist, uint32_t* __restrict__ rcount) {
   constexpr int RPT = SCAN_CHUNK / 256;  // rows per thread and chunk (16)
   extern __shared__ float smem[];
-  const int M = a.M, ds = a.ds, d = a.d, k = a.k, np = a.np;
+  const int M = a.M, k = a.k, np = a.np;
   const int kk = k + 1;  // <= SCAN_KFAST: one more than asked for, to expose ties that overflow the k-th place
   const uint64_t* __restrict__ allow = a.flt.allow;
   float* lut = smem;          // [M*256]
@@ -653,13 +741,8 @@ ivfpq_scan_kernel(const ScanArgs a, uint32_t* __restrict__ rlist, uint32_t* __re
     if (tid == 0) a.cand_cnt[slot] = 0;
     return;
   }
-  const float* q = a.queries + qi * d;
-  for (int t = tid; t < d; t += 256)
-    qr[t] = METRIC == METRIC_DOT ? q[t] : __fsub_rn(q[t], a.centroids[(size_t)p * d + t]);  // v2.rs:316-332
   if (tid == 0) s_nw = 0;
-  __syncthreads();
-  build_lut_smem<METRIC>(lut, qr, a.codebook, M, ds, tid);
-  __syncthreads();
+  stage_query_lut<METRIC, 8>(lut, qr, a, qi, p);
 
   const uint8_t* pc = a.codes + off * M;
   const float dot_fix = (float)M - 1.0f;
@@ -675,23 +758,7 @@ ivfpq_scan_kernel(const ScanArgs a, uint32_t* __restrict__ rlist, uint32_t* __re
       const uint32_t j = wbase + lane + 32 * u;
       key[u] = 0x7fffffff;
       if (j < clen && (!FILTER || row_allowed(allow, off + c0 + j))) {
-        float dist = 0.0f;
-        if ((M & 15) == 0) {
-          const uint4* rp = reinterpret_cast<const uint4*>(pc + (size_t)(c0 + j) * M);
-          for (int c16 = 0; c16 < M / 16; ++c16) {
-            const uint4 v = __ldg(rp + c16);
-            const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-            const float* l0 = lut + c16 * 16 * 256;
-#pragma unroll
-            for (int aa = 0; aa < 4; ++aa)
-#pragma unroll
-              for (int bb = 0; bb < 4; ++bb)
-                dist = f_add(dist, l0[(aa * 4 + bb) * 256 + ((w[aa] >> (8 * bb)) & 0xff)]);
-          }
-        } else {
-          const uint8_t* rp = pc + (size_t)(c0 + j) * M;
-          for (int m = 0; m < M; ++m) dist = f_add(dist, lut[m * 256 + rp[m]]);
-        }
+        float dist = pq8_row_distance(lut, pc + (size_t)(c0 + j) * M, M);
         if (METRIC == METRIC_DOT) dist = __fsub_rn(dist, dot_fix);  // pq/storage.rs:957-958
         const int32_t kv = total_order_key(dist);
         if (!FILTER || key_in_range(a.flt, kv)) {
@@ -746,25 +813,7 @@ ivfpq_scan_kernel(const ScanArgs a, uint32_t* __restrict__ rlist, uint32_t* __re
     }
     __syncthreads();
   }
-  // car[0..nw) ascending by (key, position).  If the k-th and the (k+1)-th share a key, more rows tie at the
-  // k-th distance than fit: which of them the reference's BinaryHeap keeps depends on its sift order, so the
-  // slot goes on the replay list (ivfpq_scan_radix_kernel in list mode restates that loop).
-  uint32_t nw = s_nw;
-  if (nw == (uint32_t)kk) {
-    if (cand_key(car[k]) == cand_key(car[k - 1])) {
-      if (tid == 0) {
-        rlist[atomicAdd(rcount, 1u)] = (uint32_t)slot;
-        a.cand_cnt[slot] = 0;
-      }
-      return;
-    }
-    nw = k;
-  }
-  for (uint32_t i = tid; i < nw; i += 256) {
-    a.cand_d[slot * k + i] = key_to_float(cand_key(car[i]));
-    a.cand_id[slot * k + i] = a.row_ids[off + cand_pos(car[i])];
-  }
-  if (tid == 0) a.cand_cnt[slot] = nw;
+  fast_slot_epilogue(a, (uint32_t)slot, off, car, s_nw, false, tid, 256, rlist, rcount);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1123,25 +1172,7 @@ ivfpq_scan_skew_kernel(const ScanArgs a, const uint64_t* __restrict__ slab_off, 
       }
       team_sync<TT>(team);
     }
-    const uint64_t* win = car + par * SCAN_KFAST;  // ascending by (key, position)
-    // If the k-th and the (k+1)-th share a key, more rows tie at the k-th distance than fit: which of them the
-    // reference's BinaryHeap keeps depends on its sift order, so the slot goes on the replay list.
-    if (!replay && nw == (uint32_t)kk) {
-      if (cand_key(win[k]) == cand_key(win[k - 1])) replay = true;
-      nw = k;
-    }
-    if (replay) {
-      if (ttid == 0) {
-        rlist[atomicAdd(rcount, 1u)] = slot;
-        a.cand_cnt[slot] = 0;
-      }
-      continue;
-    }
-    for (uint32_t i = ttid; i < nw; i += TT) {
-      a.cand_d[(size_t)slot * k + i] = key_to_float(cand_key(win[i]));
-      a.cand_id[(size_t)slot * k + i] = a.row_ids[off + cand_pos(win[i])];
-    }
-    if (ttid == 0) a.cand_cnt[slot] = nw;
+    fast_slot_epilogue(a, slot, off, car + par * SCAN_KFAST, nw, replay, ttid, TT, rlist, rcount);
   }
 }
 
@@ -1195,20 +1226,8 @@ ivfflat_scan_kernel(const float* __restrict__ queries, int d, const uint32_t* __
                     float* __restrict__ cand_d, uint64_t* __restrict__ cand_id,
                     uint32_t* __restrict__ cand_cnt, const ScanFilter flt) {
   extern __shared__ float smem[];
-  __shared__ uint32_t s_outc;
-  const int kk = k + 1;  // see radix_slot: exposes ties that overflow the k-th place
-  const uint64_t* __restrict__ allow = flt.allow;
-  const bool filtering = allow != nullptr || flt.range;
   float* qs = smem;                          // [d]
-  float* cd = qs + d;                        // [SCAN_CHUNK + kk]
-  uint32_t* cp = reinterpret_cast<uint32_t*>(cd + SCAN_CHUNK + kk);
-  float* wd = reinterpret_cast<float*>(cp + kk);
-  uint32_t* wp = reinterpret_cast<uint32_t*>(wd + kk);
-  __shared__ int32_t s_key[8];
-  __shared__ uint64_t s_tie[8];
-  __shared__ int s_tid[9];
-  __shared__ int32_t prev_key;
-  __shared__ uint32_t prev_pos;
+  const SlotSmem s(qs + d, k + 1);
   __shared__ float s_qnorm;
   const int tid = threadIdx.x, l = tid & 15;
   const unsigned hmask = 0xffffu << (16 * ((tid >> 4) & 1));
@@ -1233,115 +1252,14 @@ ivfflat_scan_kernel(const float* __restrict__ queries, int d, const uint32_t* __
   }
   __syncthreads();
   const float qn = METRIC == METRIC_COSINE ? s_qnorm : 0.0f;
-  const float excluded_key = __int_as_float(0x7fffffff);  // maximal key of the total order
-  uint32_t nw = 0;
-  for (uint32_t c0 = 0; c0 < n_p; c0 += SCAN_CHUNK) {
-    const uint32_t clen = min((uint32_t)SCAN_CHUNK, n_p - c0);
+  auto fill = [&](uint32_t c0, uint32_t clen) {
     for (uint32_t j = tid >> 4; j < clen; j += 16) {  // 16 rows per pass, 16 lanes each
-      if (!row_allowed(allow, off + c0 + j)) {  // uniform per half-warp
-        if (l == 0) cd[j] = excluded_key;
-        continue;
-      }
       const float dist = flat_row_distance<METRIC, T>(qs, vectors + (off + c0 + j) * (uint64_t)d, d, l, hmask, qn);
-      if (l == 0) cd[j] = key_in_range(flt, total_order_key(dist)) ? dist : excluded_key;
+      if (l == 0) s.ukey[j] = (uint32_t)total_order_key(dist) ^ 0x80000000u;
     }
-    __syncthreads();
-    const uint32_t pool = clen + nw;
-    const uint32_t rounds = pool < (uint32_t)kk ? pool : (uint32_t)kk;
-    bool first = true;
-    for (uint32_t r = 0; r < rounds; ++r) {
-      int32_t bk = 0;
-      uint32_t bpos = 0, bslot = 0;
-      bool has = false;
-      const int32_t pk = first ? 0 : prev_key;
-      const uint32_t pp = first ? 0 : prev_pos;
-      for (uint32_t i = tid; i < pool; i += 256) {
-        const int32_t key = total_order_key(cd[i < clen ? i : SCAN_CHUNK + (i - clen)]);
-        const uint32_t pos = i < clen ? c0 + i : cp[i - clen];
-        if (!first && !ki_less(pk, pp, key, pos)) continue;
-        if (!has || ki_less(key, pos, bk, bpos)) { bk = key; bpos = pos; bslot = i; has = true; }
-      }
-      const int w = block_argmin<256>(has, bk, bpos, s_key, s_tie, s_tid);
-      if (tid == w) {
-        prev_key = bk;
-        prev_pos = bpos;
-        wd[r] = cd[bslot < clen ? bslot : SCAN_CHUNK + (bslot - clen)];
-        wp[r] = bpos;
-      }
-      __syncthreads();
-      first = false;
-    }
-    for (uint32_t i = tid; i < rounds; i += 256) {
-      cd[SCAN_CHUNK + i] = wd[i];
-      cp[i] = wp[i];
-    }
-    nw = rounds;
-    __syncthreads();
-  }
-  // winners ascending by (key, position) in cd[SCAN_CHUNK ..), cp[]; excluded rows (maximal key) sort last
-  auto dropped = [&](uint32_t i) -> bool {
-    return !row_allowed(allow, off + cp[i]) || (flt.range && __float_as_int(cd[SCAN_CHUNK + i]) == 0x7fffffff);
   };
-  if (filtering) {
-    uint32_t keep = nw;
-    while (keep > 0 && dropped(keep - 1)) --keep;
-    nw = keep;  // every thread computes the same value
-  }
-  bool replay = false;
-  if (nw == (uint32_t)kk) {
-    replay = total_order_key(cd[SCAN_CHUNK + k]) == total_order_key(cd[SCAN_CHUNK + k - 1]);
-    nw = k;
-  }
-  if (!replay) {
-    if (filtering) {  // (a NaN distance can leave a dropped row in front of the tail: re-test every entry)
-      if (tid == 0) s_outc = 0;
-      __syncthreads();
-      for (uint32_t i = tid; i < nw; i += 256)
-        if (!dropped(i)) {
-          const uint32_t at = atomicAdd(&s_outc, 1u);
-          cand_d[slot * k + at] = cd[SCAN_CHUNK + i];
-          cand_id[slot * k + at] = row_ids[off + cp[i]];
-        }
-      __syncthreads();
-      if (tid == 0) cand_cnt[slot] = s_outc;
-      return;
-    }
-    for (uint32_t i = tid; i < nw; i += 256) {
-      cand_d[slot * k + i] = cd[SCAN_CHUNK + i];
-      cand_id[slot * k + i] = row_ids[off + cp[i]];
-    }
-    if (tid == 0) cand_cnt[slot] = nw;
-    return;
-  }
-  // ---- ties overflow the k-th place: the reference's heap loop (flat/index.rs:116-165), see radix_slot
-  __syncthreads();
-  uint32_t* hk = reinterpret_cast<uint32_t*>(wd);
-  uint32_t* hp = wp;
-  uint32_t len = 0;
-  for (uint32_t c0 = 0; c0 < n_p; c0 += SCAN_CHUNK) {
-    const uint32_t clen = min((uint32_t)SCAN_CHUNK, n_p - c0);
-    for (uint32_t j = tid >> 4; j < clen; j += 16) {
-      const float dist = flat_row_distance<METRIC, T>(qs, vectors + (off + c0 + j) * (uint64_t)d, d, l, hmask, qn);
-      if (l == 0) cd[j] = dist;
-    }
-    __syncthreads();
-    if (tid == 0) {
-      for (uint32_t j = 0; j < clen; ++j) {
-        const int32_t key = total_order_key(cd[j]);
-        if (filtering && (!row_allowed(allow, off + c0 + j) || !key_in_range(flt, key))) continue;
-        rheap_offer(hk, hp, len, (uint32_t)k, (uint32_t)key ^ 0x80000000u, c0 + j);
-      }
-    }
-    __syncthreads();
-  }
-  if (tid == 0) s_outc = len;
-  __syncthreads();
-  len = s_outc;
-  for (uint32_t i = tid; i < len; i += 256) {
-    cand_d[slot * k + i] = key_to_float((int32_t)(hk[i] ^ 0x80000000u));
-    cand_id[slot * k + i] = row_ids[off + hp[i]];
-  }
-  if (tid == 0) cand_cnt[slot] = len;
+  const uint32_t cnt = slot_topk(s, n_p, k, flt, off, false, fill);
+  write_slot(s, cnt, slot, k, off, row_ids, cand_d, cand_id, cand_cnt);
 }
 
 // global merge per query: ascending (distance, row id), first k.  Candidate e of list pi of query qi sits
@@ -1403,41 +1321,21 @@ merge_kernel(const float* __restrict__ cand_d, const uint64_t* __restrict__ cand
              const uint32_t* __restrict__ cand_cnt, int np, int k, size_t stride_p_d, size_t stride_p_id,
              size_t stride_q, size_t cnt_stride_p, size_t cnt_stride_q, uint64_t* __restrict__ out_id,
              float* __restrict__ out_d, uint32_t* __restrict__ out_cnt) {
-  __shared__ int32_t s_key[4];
-  __shared__ uint64_t s_tie[4];
-  __shared__ int s_tid[5];
-  __shared__ int32_t prev_key;
-  __shared__ uint64_t prev_id;
   const size_t qi = blockIdx.x;
   const int tid = threadIdx.x;
-  const int total = np * k;
-  bool first = true;
-  int r = 0;
-  for (; r < k; ++r) {
-    int32_t bk = 0;
-    uint64_t bi = 0;
-    int bslot = -1;
-    const int32_t pk = first ? 0 : prev_key;
-    const uint64_t pid = first ? 0 : prev_id;
-    for (int c = tid; c < total; c += 128) {
-      const int pi = c / k, e = c % k;
-      if ((uint32_t)e >= cand_cnt[pi * cnt_stride_p + qi * cnt_stride_q]) continue;
-      const int32_t key = total_order_key(cand_d[pi * stride_p_d + qi * stride_q + e]);
-      const uint64_t id = cand_id[pi * stride_p_id + qi * stride_q + e];
-      if (!first && !ki_less(pk, pid, key, id)) continue;
-      if (bslot < 0 || ki_less(key, id, bk, bi)) { bk = key; bi = id; bslot = c; }
-    }
-    const int w = block_argmin<128>(bslot >= 0, bk, bi, s_key, s_tie, s_tid);
-    if (w < 0) break;
-    if (tid == w) {
-      prev_key = bk;
-      prev_id = bi;
-      out_id[qi * k + r] = bi;
-      out_d[qi * k + r] = cand_d[(bslot / k) * stride_p_d + qi * stride_q + (bslot % k)];
-    }
-    __syncthreads();
-    first = false;
-  }
+  const int r = (int)emit_ascending<128>(
+      k, np * k,
+      [&](uint32_t c, int32_t& key, uint64_t& id) {
+        const int pi = c / k, e = c % k;
+        if ((uint32_t)e >= cand_cnt[pi * cnt_stride_p + qi * cnt_stride_q]) return false;
+        key = total_order_key(cand_d[pi * stride_p_d + qi * stride_q + e]);
+        id = cand_id[pi * stride_p_id + qi * stride_q + e];
+        return true;
+      },
+      [&](uint32_t r, uint32_t c, int32_t, uint64_t id) {
+        out_id[qi * k + r] = id;
+        out_d[qi * k + r] = cand_d[(c / k) * stride_p_d + qi * stride_q + (c % k)];
+      });
   for (int e = r + tid; e < k; e += 128) {
     out_id[qi * k + e] = ~0ull;
     out_d[qi * k + e] = __int_as_float(0x7f800000);
@@ -1471,87 +1369,30 @@ __global__ void pq_scan_transposed_kernel(const float* __restrict__ lut, int M,
   out[j] = dist;
 }
 
-// FlatIndex::search over a distance array (flat/index.rs:97-127): the heap's final content, written
-// ascending by (distance, row id).  Selection of k + 1 by per-thread sorted lists; when rows tie at the
-// k-th distance beyond what fits, thread 0 replays the reference's loop through the Rust heap.
-template <int KMAX>
+// FlatIndex::search over a distance array (flat/index.rs:97-127): the heap's final content (the exact top-k of one
+// slot, position = index into dists), written ascending by (distance, row id).
 __global__ void __launch_bounds__(256)
 flat_topk_kernel(const float* __restrict__ dists, const uint64_t* __restrict__ row_ids, uint64_t n,
                  int k, const ScanFilter flt, uint64_t* __restrict__ out_id, float* __restrict__ out_d,
                  uint32_t* __restrict__ out_cnt) {
-  __shared__ int32_t s_key[8];
-  __shared__ uint64_t s_tie[8];
-  __shared__ int s_tid[9];
-  __shared__ uint32_t wk[KMAX], wpos[KMAX];  // winners: unsigned order key, position
-  __shared__ uint32_t s_len;
-  const int tid = threadIdx.x;
-  const int kk = k + 1;
-  ThreadTopK<KMAX> top;
-  for (uint64_t j = tid; j < n; j += 256) {
-    const float dv = dists[j];
-    if (key_in_range(flt, total_order_key(dv))) top.push(dv, (uint32_t)j, kk);
-  }
-  int head = 0;
-  uint32_t cnt = 0;
-  for (int r = 0; r < kk; ++r) {
-    const bool has = head < top.cnt;
-    const int32_t key = has ? total_order_key(top.d[head]) : 0;
-    const uint64_t tie = has ? top.j[head] : 0;
-    const int w = block_argmin<256>(has, key, tie, s_key, s_tie, s_tid);
-    if (w < 0) break;
-    if (tid == w) {
-      wk[r] = (uint32_t)key ^ 0x80000000u;
-      wpos[r] = top.j[head];
-      ++head;
-    }
-    ++cnt;
-  }
-  __syncthreads();
-  if (cnt == (uint32_t)kk) {
-    if (wk[k] == wk[k - 1]) {  // block-uniform: replay (see radix_slot)
-      __syncthreads();
-      if (tid == 0) {
-        uint32_t len = 0;
-        for (uint64_t j = 0; j < n; ++j) {
-          const int32_t key = total_order_key(dists[j]);
-          if (!key_in_range(flt, key)) continue;
-          rheap_offer(wk, wpos, len, (uint32_t)k, (uint32_t)key ^ 0x80000000u, (uint32_t)j);
-        }
-        s_len = len;
-      }
-      __syncthreads();
-      cnt = s_len;
-    } else {
-      cnt = k;
-    }
-  }
-  // ascending (distance, row id) over the <= k survivors
-  __shared__ int32_t prev_key;
-  __shared__ uint64_t prev_id;
-  bool first = true;
-  for (uint32_t r = 0; r < cnt; ++r) {
-    int32_t bk = 0;
-    uint64_t bi = 0;
-    bool has = false;
-    const int32_t pk = first ? 0 : prev_key;
-    const uint64_t pid = first ? 0 : prev_id;
-    for (uint32_t i = tid; i < cnt; i += 256) {
-      const int32_t key = (int32_t)(wk[i] ^ 0x80000000u);
-      const uint64_t id = row_ids ? row_ids[wpos[i]] : (uint64_t)wpos[i];
-      if (!first && !ki_less(pk, pid, key, id)) continue;
-      if (!has || ki_less(key, id, bk, bi)) { bk = key; bi = id; has = true; }
-    }
-    const int w = block_argmin<256>(has, bk, bi, s_key, s_tie, s_tid);
-    if (tid == w) {
-      prev_key = bk;
-      prev_id = bi;
-      out_d[r] = key_to_float(bk);
-      out_id[r] = bi;
-    }
-    __syncthreads();
-    first = false;
-  }
-  if (tid == 0) *out_cnt = cnt;
+  extern __shared__ float smem[];
+  const SlotSmem s(smem, k + 1);
+  auto fill = [&](uint32_t c0, uint32_t clen) {
+    for (uint32_t j = threadIdx.x; j < clen; j += 256) s.ukey[j] = (uint32_t)total_order_key(dists[c0 + j]) ^ 0x80000000u;
+  };
+  const uint32_t cnt = slot_topk(s, (uint32_t)n, k, flt, 0, false, fill);
+  emit_ascending<256>(
+      cnt, cnt,
+      [&](uint32_t i, int32_t& key, uint64_t& id) {
+        key = (int32_t)(s.nkey[i] ^ 0x80000000u);
+        id = row_ids ? row_ids[s.npos[i]] : (uint64_t)s.npos[i];
+        return true;
+      },
+      [&](uint32_t r, uint32_t, int32_t key, uint64_t id) {
+        out_d[r] = key_to_float(key);
+        out_id[r] = id;
+      });
+  if (threadIdx.x == 0) *out_cnt = cnt;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1638,6 +1479,42 @@ static void merge_lists(const char* name, uint64_t nq, const float* cand_d, cons
   }
 }
 
+// The IVF query skeleton: the nprobes nearest partitions of every query, one candidate list of <= k per (query,
+// probe) slot, the lists merged per query.  scan(q0, qn, probe_ids, cand_d, cand_id, cand_cnt) fills the lists of
+// queries [q0, q0 + qn) (at most 32768 of them: the grid.y limit).
+constexpr uint64_t SEARCH_SLAB = 32768;
+template <class Scan>
+static void ivf_search(const float* centroids, int K, int d, int metric, const float* queries, uint64_t nq, int k,
+                       int np, uint64_t* out_ids, float* out_dists, uint32_t* out_counts, Scan scan) {
+  // partitions are found with L2 on the (normalised) vectors for cosine (ivf.rs:149-185)
+  const int cmetric = metric == METRIC_DOT ? METRIC_DOT : METRIC_L2;
+  DevBuf<uint32_t> pids((size_t)nq * np), cand_cnt((size_t)nq * np);
+  DevBuf<float> pd((size_t)nq * np), cand_d((size_t)nq * np * k);
+  DevBuf<uint64_t> cand_id((size_t)nq * np * k);
+  find_partitions_f32(centroids, K, d, cmetric, queries, nq, np, pids.p, pd.p);
+  for (uint64_t q0 = 0; q0 < nq; q0 += SEARCH_SLAB)
+    scan(q0, std::min<uint64_t>(SEARCH_SLAB, nq - q0), pids.p + q0 * np, cand_d.p + q0 * np * k,
+         cand_id.p + q0 * np * k, cand_cnt.p + q0 * np);
+  merge_lists("merge_topk", nq, cand_d.p, cand_id.p, cand_cnt.p, np, k, (size_t)k, (size_t)k, (size_t)np * k, (size_t)1,
+              (size_t)np, out_ids, out_dists, out_counts);
+}
+
+// f(metric, element) with the metric as a std::integral_constant and the element type as a type_tag
+template <class T> struct type_tag { using type = T; };
+template <bool WITH_U8, class F>
+static void dispatch_metric_elem(int metric, int vdt, F&& f) {
+  auto by_elem = [&](auto m) {
+    if (vdt == LB2_F16) f(m, type_tag<__half>{});
+    else if (vdt == LB2_BF16) f(m, type_tag<__nv_bfloat16>{});
+    else if constexpr (WITH_U8) {
+      if (vdt == LB2_U8) f(m, type_tag<uint8_t>{}); else f(m, type_tag<float>{});
+    } else f(m, type_tag<float>{});
+  };
+  if (metric == METRIC_DOT) by_elem(std::integral_constant<int, METRIC_DOT>{});
+  else if (metric == METRIC_COSINE) by_elem(std::integral_constant<int, METRIC_COSINE>{});
+  else by_elem(std::integral_constant<int, METRIC_L2>{});
+}
+
 // the skewed copy of an index's codes (see ivfpq_scan_skew_kernel); sizes: slab_off u64[K + 1],
 // skew (n / 512 + K) slabs of 8704 bytes at most
 bool skew_layout_applies(int M, int d, int nbits) { return nbits == 8 && M == 16 && d == 128; }
@@ -1659,28 +1536,19 @@ void ivfpq_search_f32(const float* centroids, int K, int d, int metric, const fl
   if (nbits == 4 && (M % 2 != 0 || M > 256)) fail(LB2_UNSUPPORTED, "4-bit PQ needs an even num_sub_vectors <= 256");
   if (k > 1024) fail(LB2_UNSUPPORTED, "k (incl. refine factor) > 1024 is not implemented");
   const int np = nprobes < K ? nprobes : K;
-  const int ds = d / M;
-  const int cmetric = metric == METRIC_DOT ? METRIC_DOT : METRIC_L2;
-  DevBuf<uint32_t> pids((size_t)nq * np), cand_cnt((size_t)nq * np);
-  DevBuf<float> pd((size_t)nq * np), cand_d((size_t)nq * np * k);
-  DevBuf<uint64_t> cand_id((size_t)nq * np * k);
-  find_partitions_f32(centroids, K, d, cmetric, queries, nq, np, pids.p, pd.p);
-  const size_t smem = sizeof(float) * ((size_t)M * 256 + d + SCAN_CHUNK + 4 * (size_t)(k + 1));
+  const size_t smem = sizeof(float) * ((size_t)M * 256 + d) + slot_smem_bytes(k);
   if (smem > ctx().smem_optin) fail(LB2_UNSUPPORTED, "LUT of %zu bytes exceeds shared memory", smem);
-  const uint64_t slab = 32768;  // grid.y limit: queries are processed in slabs
-  DevBuf<uint32_t> rlist((size_t)std::min<uint64_t>(nq, slab) * np), rcount(1);
-  for (uint64_t q0 = 0; q0 < nq; q0 += slab) {
-    const uint64_t qn = std::min<uint64_t>(slab, nq - q0);
-    dim3 g(np, (unsigned)qn);
-    ScanArgs a{queries + q0 * d, d, centroids, codebook, M, ds, pids.p + q0 * np, np, part_offsets, codes, row_ids, k,
-               cand_d.p + q0 * np * k, cand_id.p + q0 * np * k, cand_cnt.p + q0 * np, flt};
-    if (cmetric == METRIC_DOT)
-      scan_launch<METRIC_DOT>(nbits, g, smem, a, rlist.p, rcount.p, slab_off, skew);
-    else
-      scan_launch<METRIC_L2>(nbits, g, smem, a, rlist.p, rcount.p, slab_off, skew);
-  }
-  merge_lists("merge_topk", nq, cand_d.p, cand_id.p, cand_cnt.p, np, k, (size_t)k, (size_t)k, (size_t)np * k, (size_t)1,
-              (size_t)np, out_ids, out_dists, out_counts);
+  DevBuf<uint32_t> rlist((size_t)std::min<uint64_t>(nq, SEARCH_SLAB) * np), rcount(1);
+  ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
+             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, float* cd, uint64_t* cid, uint32_t* ccnt) {
+               const ScanArgs a{queries + q0 * d, d, centroids, codebook, M, d / M, pids, np, part_offsets, codes,
+                                row_ids, k, cd, cid, ccnt, flt};
+               const dim3 g(np, (unsigned)qn);
+               if (metric == METRIC_DOT)
+                 scan_launch<METRIC_DOT>(nbits, g, smem, a, rlist.p, rcount.p, slab_off, skew);
+               else
+                 scan_launch<METRIC_L2>(nbits, g, smem, a, rlist.p, rcount.p, slab_off, skew);
+             });
 }
 
 // Row-sharded index (SURVEY 8e search (ii)): every rank has searched its own shard; the per-rank top-k lists
@@ -1740,39 +1608,19 @@ void ivfflat_search_f32(const float* centroids, int K, int d, int metric, const 
                         const ScanFilter& flt) {
   if (nq == 0 || k == 0) return;
   if (k > 1024) fail(LB2_UNSUPPORTED, "k (incl. refine factor) > 1024 is not implemented");
-  const int np = nprobes < K ? nprobes : K;
-  // partitions are found with L2 on the (normalised) vectors for cosine (ivf.rs:149-185)
-  const int cmetric = metric == METRIC_DOT ? METRIC_DOT : METRIC_L2;
-  DevBuf<uint32_t> pids((size_t)nq * np), cand_cnt((size_t)nq * np);
-  DevBuf<float> pd((size_t)nq * np), cand_d((size_t)nq * np * k);
-  DevBuf<uint64_t> cand_id((size_t)nq * np * k);
-  find_partitions_f32(centroids, K, d, cmetric, queries, nq, np, pids.p, pd.p);
-  const size_t smem = sizeof(float) * ((size_t)d + SCAN_CHUNK + 4 * (size_t)(k + 1));
+  const size_t smem = sizeof(float) * (size_t)d + slot_smem_bytes(k);
   if (smem > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the flat scan", d);
-  for (uint64_t q0 = 0; q0 < nq; q0 += 32768) {
-    const uint64_t qn = std::min<uint64_t>(32768, nq - q0);
-    dim3 g(np, (unsigned)qn);
-#define LB2_FLAT_T(MET, TT)                                                                             \
-    {                                                                                                   \
-      set_smem((ivfflat_scan_kernel<MET, TT>), smem);                                                   \
-      LB2_LAUNCH("flat_scan", (ivfflat_scan_kernel<MET, TT>), g, 256, smem, queries + q0 * d, d,         \
-                 pids.p + q0 * np, np, part_offsets, reinterpret_cast<const TT*>(vectors), row_ids, k,   \
-                 cand_d.p + q0 * np * k, cand_id.p + q0 * np * k, cand_cnt.p + q0 * np, flt);            \
-    }
-#define LB2_FLAT(MET)                                                                                   \
-    {                                                                                                   \
-      if (vdt == LB2_F16) LB2_FLAT_T(MET, __half)                                                       \
-      else if (vdt == LB2_BF16) LB2_FLAT_T(MET, __nv_bfloat16)                                          \
-      else LB2_FLAT_T(MET, float)                                                                       \
-    }
-    if (metric == METRIC_DOT) LB2_FLAT(METRIC_DOT)
-    else if (metric == METRIC_COSINE) LB2_FLAT(METRIC_COSINE)
-    else LB2_FLAT(METRIC_L2)
-#undef LB2_FLAT_T
-#undef LB2_FLAT
-  }
-  merge_lists("merge_topk", nq, cand_d.p, cand_id.p, cand_cnt.p, np, k, (size_t)k, (size_t)k, (size_t)np * k, (size_t)1,
-              (size_t)np, out_ids, out_dists, out_counts);
+  const int np = nprobes < K ? nprobes : K;
+  ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
+             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, float* cd, uint64_t* cid, uint32_t* ccnt) {
+               dispatch_metric_elem<false>(metric, vdt, [&](auto m, auto e) {
+                 using T = typename decltype(e)::type;
+                 auto kern = ivfflat_scan_kernel<decltype(m)::value, T>;
+                 set_smem(kern, smem);
+                 LB2_LAUNCH("flat_scan", kern, dim3(np, (unsigned)qn), 256, smem, queries + q0 * d, d, pids, np,
+                            part_offsets, reinterpret_cast<const T*>(vectors), row_ids, k, cd, cid, ccnt, flt);
+               });
+             });
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1827,11 +1675,6 @@ refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ ve
   extern __shared__ float smem[];
   float* qs = smem;       // [d]
   float* cd = qs + d;     // [kc]
-  __shared__ int32_t s_key[8];
-  __shared__ uint64_t s_tie[8];
-  __shared__ int s_tid[9];
-  __shared__ int32_t prev_key;
-  __shared__ uint64_t prev_id;
   __shared__ float s_qnorm;
   const size_t qi = blockIdx.x;
   const int tid = threadIdx.x, l = tid & 15;
@@ -1856,37 +1699,20 @@ refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ ve
     if (l == 0) cd[c] = dist;
   }
   __syncthreads();
-  bool first = true;
-  uint32_t r = 0;
-  const uint32_t rounds = cnt < (uint32_t)k ? cnt : (uint32_t)k;
   auto passes = [&](float dv) {  // LanceFilterExec(_distance >= lower AND _distance < upper): SQL compares
     return (!has_lower || dv >= lower) && (!has_upper || dv < upper);
   };
-  for (; r < rounds; ++r) {
-    int32_t bk = 0;
-    uint64_t bi = 0;
-    uint32_t bslot = 0;
-    bool has = false;
-    const int32_t pk = first ? 0 : prev_key;
-    const uint64_t pid = first ? 0 : prev_id;
-    for (uint32_t c = tid; c < cnt; c += 256) {
-      if (!passes(cd[c])) continue;
-      const int32_t key = total_order_key(cd[c]);
-      const uint64_t id = ids[c];
-      if (!first && !ki_less(pk, pid, key, id)) continue;
-      if (!has || ki_less(key, id, bk, bi)) { bk = key; bi = id; bslot = c; has = true; }
-    }
-    const int w = block_argmin<256>(has, bk, bi, s_key, s_tie, s_tid);
-    if (w < 0) break;
-    if (tid == w) {
-      prev_key = bk;
-      prev_id = bi;
-      out_id[qi * k + r] = bi;
-      out_d[qi * k + r] = cd[bslot];
-    }
-    __syncthreads();
-    first = false;
-  }
+  const uint32_t r = emit_ascending<256>(
+      min(cnt, (uint32_t)k), cnt,
+      [&](uint32_t c, int32_t& key, uint64_t& id) {
+        key = total_order_key(cd[c]);
+        id = ids[c];
+        return passes(cd[c]);
+      },
+      [&](uint32_t r, uint32_t c, int32_t, uint64_t id) {
+        out_id[qi * k + r] = id;
+        out_d[qi * k + r] = cd[c];
+      });
   for (uint32_t e = r + tid; e < (uint32_t)k; e += 256) {
     out_id[qi * k + e] = ~0ull;
     out_d[qi * k + e] = __int_as_float(0x7f800000);
@@ -1900,25 +1726,13 @@ void refine_f32(const float* queries, uint64_t nq, int d, int metric, const void
                 float upper) {
   if (nq == 0) return;
   const size_t smem = sizeof(float) * ((size_t)d + kc);
-#define LB2_REF_T(MET, TT)                                                                           \
-  {                                                                                                   \
-    set_smem((refine_kernel<MET, TT>), smem);                                                         \
-    LB2_LAUNCH("refine", (refine_kernel<MET, TT>), (unsigned)nq, 256, smem, queries, d,                \
-               reinterpret_cast<const TT*>(vectors), num_vectors, cand_id, cand_cnt, kc, k, out_id,    \
-               out_d, out_cnt, has_lower, lower, has_upper, upper);                                    \
-  }
-#define LB2_REF(MET)                                                                                  \
-  {                                                                                                   \
-    if (vdt == LB2_F16) LB2_REF_T(MET, __half)                                                        \
-    else if (vdt == LB2_BF16) LB2_REF_T(MET, __nv_bfloat16)                                           \
-    else if (vdt == LB2_U8) LB2_REF_T(MET, uint8_t)                                                   \
-    else LB2_REF_T(MET, float)                                                                        \
-  }
-  if (metric == METRIC_DOT) LB2_REF(METRIC_DOT)
-  else if (metric == METRIC_COSINE) LB2_REF(METRIC_COSINE)
-  else LB2_REF(METRIC_L2)
-#undef LB2_REF_T
-#undef LB2_REF
+  dispatch_metric_elem<true>(metric, vdt, [&](auto m, auto e) {
+    using T = typename decltype(e)::type;
+    auto kern = refine_kernel<decltype(m)::value, T>;
+    set_smem(kern, smem);
+    LB2_LAUNCH("refine", kern, (unsigned)nq, 256, smem, queries, d, reinterpret_cast<const T*>(vectors), num_vectors,
+               cand_id, cand_cnt, kc, k, out_id, out_d, out_cnt, has_lower, lower, has_upper, upper);
+  });
 }
 
 void build_lut_f32(const float* codebook, int M, int nbits, int d, int metric, const float* query,
@@ -1967,31 +1781,7 @@ __global__ void pq4_quantize_kernel(const float* __restrict__ lut, int M, const 
                                     uint64_t flat_num, uint8_t* __restrict__ qt, float* __restrict__ params) {
   __shared__ int32_t s_max[256];
   __shared__ float s_min[256];
-  const int tid = threadIdx.x;
-  int32_t mx = (int32_t)0x80000000;
-  for (uint64_t j = tid; j < flat_num; j += 256) mx = max(mx, total_order_key(flat[j]));
-  float mn = __int_as_float(0x7f800000);
-  for (int i = tid; i < M * 16; i += 256) mn = fminf(mn, lut[i]);
-  s_max[tid] = mx;
-  s_min[tid] = mn;
-  __syncthreads();
-  for (int o = 128; o >= 1; o >>= 1) {
-    if (tid < o) {
-      s_max[tid] = max(s_max[tid], s_max[tid + o]);
-      s_min[tid] = fminf(s_min[tid], s_min[tid + o]);
-    }
-    __syncthreads();
-  }
-  const float qmax = key_to_float(s_max[0]), qmin = s_min[0];
-  const float factor = __fdiv_rn(255.0f, __fsub_rn(qmax, qmin));
-  for (int i = tid; i < M * 16; i += 256) {
-    const float v = roundf(__fmul_rn(__fsub_rn(lut[i], qmin), factor));  // f32::round: half away from zero
-    qt[i] = (v != v) ? 0 : v <= 0.0f ? 0 : v >= 255.0f ? 255 : (uint8_t)v;  // `as u8`: saturating, NaN -> 0
-  }
-  if (tid == 0) {
-    params[0] = qmin;
-    params[1] = __fdiv_rn(__fsub_rn(qmax, qmin), 255.0f);
-  }
+  pq4_quantize(lut, M, flat_num, [&](uint64_t j) { return flat[j]; }, qt, params, s_max, s_min);
 }
 __global__ void pq4_quant_scan_kernel(const uint8_t* __restrict__ qt, int nb, const uint8_t* __restrict__ codes_t,
                                       uint64_t n, uint64_t begin, uint64_t end,
@@ -2050,12 +1840,7 @@ void pack_nibbles(const uint8_t* codes, uint64_t n, int M, uint8_t* out) {
 void flat_topk_f32(const float* dists, const uint64_t* row_ids, uint64_t n, int k, const ScanFilter& flt,
                    uint64_t* out_id, float* out_d, uint32_t* out_cnt) {
   if (k > 1024) fail(LB2_UNSUPPORTED, "k > 1024 is not implemented");
-  if (k < 16)
-    LB2_LAUNCH("flat_topk", flat_topk_kernel<16>, 1, 256, 0, dists, row_ids, n, k, flt, out_id, out_d, out_cnt);
-  else if (k < 128)
-    LB2_LAUNCH("flat_topk", flat_topk_kernel<128>, 1, 256, 0, dists, row_ids, n, k, flt, out_id, out_d, out_cnt);
-  else
-    LB2_LAUNCH("flat_topk", flat_topk_kernel<1025>, 1, 256, 0, dists, row_ids, n, k, flt, out_id, out_d, out_cnt);
+  LB2_LAUNCH("flat_topk", flat_topk_kernel, 1, 256, slot_smem_bytes(k), dists, row_ids, n, k, flt, out_id, out_d, out_cnt);
 }
 
 }  // namespace lb2

@@ -380,6 +380,23 @@ def test_index_search_with_row_mask_matches_oracle(kind):
     i0, d0 = ix.search(q, k=10, nprobes=4)
     i1, d1 = ix.search_ex(q, k=10, nprobes=4)
     assert np.array_equal(i0, i1) and np.array_equal(d0, d1)
+    # a NaN query: every distance's order key is the one filtered rows carry.  With the first 5 rows of every
+    # partition blocked, the k + 1 smallest (key, position) of a slot (k + 1 > 16: the radix path for IVF_PQ) end in
+    # an admitted row, so the slot is replayed through the reference's heap and keeps k admitted rows.
+    off = parts["part_offsets"].astype(np.int64)
+    b = np.concatenate([parts["row_ids"][o:o + 5] for o in off[:-1]])
+    bm = ix.row_mask(None, b)
+    qn = q[:1].copy()
+    qn[0, 0] = np.nan
+    ids, dists = ix.search_ex(qn, k=40, nprobes=6, allow_bitmap=bm)
+    if kind == "pq":
+        oi, od, oc = ob.ivfpq_search(parts["centroids"], parts["codebook"], parts["part_offsets"], parts["codes"],
+                                     parts["row_ids"], qn, 40, 6, nthreads=NT, block=b)
+    else:
+        oi, od, oc = ob.ivfflat_search(parts["centroids"], parts["part_offsets"], parts["vectors"], parts["row_ids"],
+                                       qn, 40, 6, nthreads=NT, block=b)
+    assert int(oc[0]) == 40 and np.isnan(od).all()
+    assert np.array_equal(ids, oi) and np.isnan(dists).all()
 
 
 def test_build_transform_equals_oracle_and_recall():
@@ -1010,18 +1027,19 @@ def test_config5_shape_u8_m32():
 # ---- round 2: parity loose ends -----------------------------------------------------------------------
 def test_flat_topk_ties_and_range_equal_reference_heap():
     rng = np.random.default_rng(2001)
-    d = rng.integers(0, 12, size=5000).astype(np.float32)          # at most 12 distinct values: ties everywhere
-    rid = rng.permutation(5000).astype(np.uint64)
-    for k in (1, 2, 7, 15, 16, 17, 100, 127, 128, 500, 1024):
-        ids, dist = lb.flat_topk(d, rid, k)
-        oi, od = ob.flat_topk(d, rid, k)
-        _check_topk(ids, dist, oi, od, k)
-        assert np.all(np.diff(dist) >= 0)
-    for lo, hi in ((2.0, 7.0), (None, 3.0), (5.0, None), (3.0, 3.0), (11.0, 100.0)):
-        for k in (5, 40):
-            ids, dist = lb.flat_topk(d, rid, k, lower_bound=lo, upper_bound=hi)
-            oi, od = ob.flat_topk(d, rid, k, lower=lo, upper=hi)
+    for n in (5000, 12003):                                       # 12003: three 4096-row chunks, ties across them
+        d = rng.integers(0, 12, size=n).astype(np.float32)         # at most 12 distinct values: ties everywhere
+        rid = rng.permutation(n).astype(np.uint64)
+        for k in (1, 2, 7, 15, 16, 17, 100, 127, 128, 500, 1024):
+            ids, dist = lb.flat_topk(d, rid, k)
+            oi, od = ob.flat_topk(d, rid, k)
             _check_topk(ids, dist, oi, od, k)
+            assert np.all(np.diff(dist) >= 0)
+        for lo, hi in ((2.0, 7.0), (None, 3.0), (5.0, None), (3.0, 3.0), (11.0, 100.0)):
+            for k in (5, 40):
+                ids, dist = lb.flat_topk(d, rid, k, lower_bound=lo, upper_bound=hi)
+                oi, od = ob.flat_topk(d, rid, k, lower=lo, upper=hi)
+                _check_topk(ids, dist, oi, od, k)
     x = np.array([np.inf, -np.inf, 1.0, 2.0], np.float32)          # an absent bound is f32::MIN / f32::MAX
     assert lb.flat_topk(x, None, 4, upper_bound=5.0)[1].tolist() == [1.0, 2.0]
     assert lb.flat_topk(x, None, 4, lower_bound=-5.0)[1].tolist() == [1.0, 2.0]
