@@ -350,6 +350,53 @@ lb2_status lb2_index_export_flat(const lb2_index* index, void* centroids_out,
                                  uint64_t* part_offsets_out, void* vectors_out,
                                  uint64_t* row_ids_out);
 
+/* ---- IVF_SQ: IVFIndex<FlatIndex, ScalarQuantizer> (lance-index/src/vector/sq*.rs) ---------------
+ * create_index(.., "IVF_SQ") builds an IvfIndexBuilder<FlatIndex, ScalarQuantizer> (rust/lance/src/index/vector.rs:
+ * 429-450).  One byte per dimension: code = scale_to_u8 of the vector (normalised first under cosine) with the
+ * index's bounds; no residuals (Quantization::use_residual is false, quantizer.rs:52).  A search encodes the
+ * (normalised) query with the same bounds and ranks rows by an exact integer distance, so its results are
+ * bit-identical to the reference, ties at the k-th distance included.  d % 4 == 0 and d * 255^2 < 2^32.
+ * lb2_index_search / _search_refine / _search_ex / _search_async / _search_sharded / _row_mask / _info
+ * (num_sub_vectors 0, num_bits 8) / _repartition / _destroy take an IVF_SQ handle; lb2_index_update, _load,
+ * _export and _export_partition do not. */
+/* ScalarQuantizer::build (lance-index/src/vector/sq.rs:67-89,152-182): the bounds are the fold of every one of the
+ * n * d elements as f64 from (f64::MAX, f64::MIN) with f64::min / f64::max (NaN elements are ignored). */
+lb2_status lb2_sq_train(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, double* lower_out,
+                        double* upper_out);
+/* ScalarQuantizer::quantize = scale_to_u8 (sq.rs:263-277): codes_out[n][d], code = ((v - lower) * 255 / (upper -
+ * lower)) in f64, then `as u8` (truncation toward zero, saturating, NaN -> 0); all codes are 0 when lower == upper. */
+lb2_status lb2_sq_encode(const void* vectors, uint64_t n, uint32_t d, lb2_dtype dtype, double lower, double upper,
+                         uint8_t* codes_out);
+/* IvfIndexBuilder<FlatIndex, ScalarQuantizer>::build (rust/lance/src/index/vector/builder.rs:398-468): the IVF stage
+ * of lb2_ivfflat_build (same sample, seed and assignment), then the bounds over sample_rate * 2^num_bits rows drawn
+ * with seed + 1 (normalised under cosine, rows that are not finite dropped, values as the index stores them), then
+ * every kept row encoded and grouped by partition.  The quantizer stage is timed in stats->ms_pq_train.
+ * num_bits other than 8 -> LB2_UNSUPPORTED (the reference has no SQ4, sq.rs:115); so is a build with a
+ * communicator of more than one rank. */
+typedef struct {
+  uint32_t num_partitions;
+  lb2_kmeans_params ivf;
+  uint32_t num_bits;    /* SQBuildParams (sq/builder.rs:7-28): 8 */
+  uint64_t sample_rate; /* 256 */
+  uint64_t seed;        /* training-sample selection */
+} lb2_ivfsq_build_params;
+void lb2_ivfsq_build_params_default(lb2_ivfsq_build_params* p);
+lb2_status lb2_ivfsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                           const lb2_ivfsq_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                           lb2_build_stats* stats);
+/* An index from a reference-built model: centroids in the model type of `dtype`, the `lance:sq` metadata's bounds
+ * {dim, num_bits, bounds} (lance-index/src/vector/sq/storage.rs:38-45); finite, lower <= upper (else
+ * LB2_INVALID_ARG). */
+lb2_status lb2_index_create_sq(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                               double lower, double upper, lb2_index** out);
+/* codes [n][d] (the __sq_code column), grouped by partition on the device (stable) */
+lb2_status lb2_index_load_sq(lb2_index* index, const uint32_t* part_ids, const uint8_t* codes,
+                             const uint64_t* row_ids, uint64_t n);
+/* any pointer may be NULL: bounds_out[2] = {lower, upper}; part_offsets[k+1]; codes [num_rows][d] and row_ids
+ * [num_rows] in partition order */
+lb2_status lb2_index_export_sq(const lb2_index* index, void* centroids_out, double* bounds_out,
+                               uint64_t* part_offsets_out, uint8_t* codes_out, uint64_t* row_ids_out);
+
 /* ---- multi-GPU (one process per GPU) -----------------------------------------------------------
  * With a communicator every training / build call takes THIS RANK'S ROW SHARD: the k-means loops
  * (flat and hierarchical) exchange their packed per-cluster partial results once per Lloyd iteration

@@ -13,13 +13,14 @@ import numpy as np
 
 from ._lib import (BF16, COSINE, DOT, F16, F32, L2, METRICS, U8, BuildParams, BuildStats, FlatBuildParams,
                    DeviceArray, KMeansParams as _CKMeansParams, LanceB200Error, PinnedArray,
-                   PQParams as _CPQParams, as_ptr, check, device_count, lib)
+                   PQParams as _CPQParams, SqBuildParams as _CSqBuildParams, as_ptr, check, device_count, lib)
 
 __all__ = ["device_count", "DeviceArray", "PinnedArray", "LanceB200Error", "train_kmeans",
            "compute_partitions", "kmeans_find_partitions", "compute_residual", "normalize_fsl",
            "l2_distance_batch", "dot_distance_batch", "cosine_distance_batch", "PQBuildParams", "ProductQuantizer",
            "build_distance_table_l2", "compute_pq_distance", "flat_topk", "IvfPqIndex",
-           "IvfBuildParams", "IvfFlatIndex", "launch_count", "profile"]
+           "IvfBuildParams", "IvfFlatIndex", "SQBuildParams", "ScalarQuantizer", "IvfSqIndex", "launch_count",
+           "profile"]
 
 
 def _metric(m):
@@ -724,3 +725,110 @@ class IvfFlatIndex(IvfPqIndex):
         check(lib().lb2_index_export_flat(self._h, C.c_void_p(cent.ctypes.data), C.c_void_p(off.ctypes.data),
                                           C.c_void_p(vec.ctypes.data), C.c_void_p(rid.ctypes.data)))
         return dict(centroids=cent, part_offsets=off, vectors=vec, row_ids=rid)
+
+
+# ---- lance-index::vector::sq -----------------------------------------------------------------
+class SQBuildParams:
+    """lance_index::vector::sq::builder::SQBuildParams (sq/builder.rs:7-28)."""
+
+    def __init__(self, num_bits=8, sample_rate=256):
+        self.num_bits, self.sample_rate = num_bits, sample_rate
+
+
+class ScalarQuantizer:
+    """lance_index::vector::sq::ScalarQuantizer (sq.rs): 8-bit codes under the bounds [lower, upper]."""
+
+    def __init__(self, dimension, bounds=None, num_bits=8):
+        self.dimension, self.num_bits = dimension, num_bits
+        self.bounds = None if bounds is None else (float(bounds[0]), float(bounds[1]))
+
+    def build(self, data, bf16=False):
+        """ScalarQuantizer::build (sq.rs:67-89,152-182): the (min, max) fold over every element -> bounds."""
+        data, dt = _typed(data, bf16)
+        n = int(np.prod(data.shape)) // self.dimension
+        lo, hi = C.c_double(0), C.c_double(0)
+        dp, _k = as_ptr(data)
+        check(lib().lb2_sq_train(dp, C.c_uint64(n), C.c_uint32(self.dimension), C.c_int(dt), C.byref(lo),
+                                 C.byref(hi)))
+        self.bounds = (lo.value, hi.value)
+        return self.bounds
+
+    def transform(self, vectors, bf16=False):
+        """ScalarQuantizer::quantize = scale_to_u8 (sq.rs:263-277) -> u8 codes [n][d]."""
+        vectors, dt = _typed(vectors, bf16)
+        n = int(np.prod(vectors.shape)) // self.dimension
+        out = np.empty((n, self.dimension), np.uint8)
+        vp, _k = as_ptr(vectors)
+        check(lib().lb2_sq_encode(vp, n, self.dimension, dt, self.bounds[0], self.bounds[1],
+                                  C.c_void_p(out.ctypes.data)))
+        return out
+
+
+class IvfSqIndex(IvfPqIndex):
+    """Device-resident IVFIndex<FlatIndex, ScalarQuantizer> (IVF_SQ): 8-bit scalar codes, searched with the
+    reference's exact integer distances (lance-index/src/vector/sq/storage.rs:432-468)."""
+
+    @classmethod
+    def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
+              centroids=None, row_ids=None, bf16=False, sq_params=None):
+        """create_index(.., "IVF_SQ"); the IVF stage equals IvfFlatIndex.build's with the same arguments.
+        bf16=True: `data` is a uint16 array holding bfloat16 bit patterns."""
+        sq_params = sq_params or SQBuildParams()
+        data, dt = _typed(data, bf16)
+        n, d = data.shape
+        bp = _CSqBuildParams()
+        lib().lb2_ivfsq_build_params_default(C.byref(bp))
+        bp.num_partitions = num_partitions
+        bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed, bp.seed = max_iters, sample_rate, seed, seed
+        bp.num_bits, bp.sample_rate = sq_params.num_bits, sq_params.sample_rate
+        keep = None
+        if centroids is not None:
+            keep = _f32(centroids)
+            bp.ivf.init_centroids = as_ptr(keep)[0].value
+        rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
+                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
+        h = C.c_void_p()
+        st = BuildStats()
+        dp, _k1 = as_ptr(data)
+        rp, _k2 = as_ptr(rid)
+        check(lib().lb2_ivfsq_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt), C.c_int(_metric(distance_type)),
+                                    C.byref(bp), rp, C.byref(h), C.byref(st)))
+        ix = cls(h, st)
+        ix._dt = dt
+        return ix
+
+    @classmethod
+    def from_parts(cls, centroids, bounds, part_ids, codes, row_ids=None, distance_type="l2", dtype=np.float32,
+                   bf16=False):
+        """Open a reference-built IVF_SQ index: centroids, the `lance:sq` bounds (lower, upper), and the shuffle
+        output (partition ids, codes [n][d], row ids).  dtype / bf16: the element type of the queries and of the
+        raw column used by refine (bf16=True: uint16 bit patterns)."""
+        dt = BF16 if bf16 else _DTYPES[np.dtype(dtype)]
+        centroids = np.ascontiguousarray(centroids, dtype=_model_np(dt))
+        k, d = centroids.shape
+        h = C.c_void_p()
+        check(lib().lb2_index_create_sq(C.c_void_p(centroids.ctypes.data), k, d, dt, _metric(distance_type),
+                                        float(bounds[0]), float(bounds[1]), C.byref(h)))
+        ix = cls(h)
+        ix._dt = dt
+        part_ids = np.ascontiguousarray(part_ids, dtype=np.uint32)
+        codes = np.ascontiguousarray(codes, dtype=np.uint8)
+        rid = None if row_ids is None else np.ascontiguousarray(row_ids, dtype=np.uint64)
+        rp, _k = as_ptr(rid)
+        check(lib().lb2_index_load_sq(h, C.c_void_p(part_ids.ctypes.data), C.c_void_p(codes.ctypes.data), rp,
+                                      C.c_uint64(part_ids.size)))
+        return ix
+
+    def export(self):
+        i = self.info()
+        K, d, n = i["num_partitions"], i["dimension"], i["num_rows"]
+        cent = np.empty((K, d), np.float32)
+        bounds = np.empty(2, np.float64)
+        off = np.empty(K + 1, np.uint64)
+        codes = np.empty((n, d), np.uint8)
+        rid = np.empty(n, np.uint64)
+        check(lib().lb2_index_export_sq(self._h, C.c_void_p(cent.ctypes.data), C.c_void_p(bounds.ctypes.data),
+                                        C.c_void_p(off.ctypes.data), C.c_void_p(codes.ctypes.data),
+                                        C.c_void_p(rid.ctypes.data)))
+        return dict(centroids=cent, bounds=(float(bounds[0]), float(bounds[1])), part_offsets=off, codes=codes,
+                    row_ids=rid)

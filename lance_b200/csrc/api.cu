@@ -14,6 +14,7 @@
 #include "exact.cuh"
 #include "kmeans.cuh"
 #include "search.cuh"
+#include "sq.cuh"
 #include "tc_assign.cuh"
 #include "tc_pq.cuh"
 
@@ -652,7 +653,7 @@ using namespace lb2;
 
 // the handle
 struct lb2_index {
-  int kind = 0;  // 0 = IVF_PQ, 1 = IVF_FLAT
+  int kind = 0;  // 0 = IVF_PQ, 1 = IVF_FLAT, 2 = IVF_SQ
   lb2_dtype dtype = LB2_F32;  // element type of the vectors / queries the caller passes
   // IVF_FLAT: the (normalised for cosine) vectors in partition order, in the vectors' own element type
   // (f32 / f16 / bf16; u8 columns are held as f32, the reference's model type for them, ivf.rs:1917-1929)
@@ -667,7 +668,11 @@ struct lb2_index {
   // the conflict-free scan's skewed copy of `codes` (search.cu: ivfpq_scan_skew_kernel); empty for other shapes
   DevBuf<uint64_t> slab_off;
   DevBuf<uint8_t> codes_skew;
-  int code_bytes() const { return nbits == 4 ? M / 2 : M; }  // bytes per row of `codes` (pq.rs:168-173)
+  // IVF_SQ: `codes` are the 8-bit scalar codes [n][d] of the (normalised for cosine) vectors, under the bounds
+  // [sq_lower, sq_upper] (sq/storage.rs:38-45)
+  double sq_lower = 0.0, sq_upper = 0.0;
+  // bytes per row of `codes` (PQ: pq.rs:168-173; SQ: one per dimension)
+  int code_bytes() const { return kind == 2 ? d : (nbits == 4 ? M / 2 : M); }
   size_t codebook_len() const { return ((size_t)1 << nbits) * d; }
 };
 
@@ -1474,13 +1479,22 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
   uint32_t* sc = refine ? ccnt.p : oc.get();
   TagScope tg("search");
   const ScanFilter flt = make_filter(allow_bitmap ? allow.get() : nullptr, has_lower, lower, has_upper, upper);
-  if (index->kind == 1)
+  DevBuf<uint8_t> qcodes;
+  if (index->kind == 1) {
     ivfflat_search_f32(index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->vectors.p,
                        (int)index->vdtype(), index->row_ids.p, qp, nq, (int)kc, nprobes, si, sd, sc, flt);
-  else
+  } else if (index->kind == 2) {
+    // the (normalised) query is encoded with the index's bounds, not turned into a residual (sq/storage.rs:404-430)
+    qcodes.alloc(std::max<uint64_t>(1, nq * d));
+    sq_encode_f32(qp, nq * d, index->sq_lower, index->sq_upper, qcodes.p);
+    const float rf = (float)(index->sq_upper - index->sq_lower);  // inverse_scalar_dist (sq.rs:279-287)
+    ivfsq_search_f32(index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->codes.p,
+                     index->row_ids.p, rf * rf, qp, qcodes.p, nq, (int)kc, nprobes, si, sd, sc, flt);
+  } else {
     ivfpq_search_f32(index->centroids.p, index->K, d, index->metric, index->codebook.p, index->M, index->nbits,
                      index->part_offsets.p, index->codes.p, index->row_ids.p, qp, nq, (int)kc, nprobes, si, sd,
                      sc, flt, index->slab_off.p, index->codes_skew.p);
+  }
   if (refine) {
     // exact re-rank with the true metric on the ORIGINAL (un-normalised) query, as flat_knn does; the
     // plan then filters `_distance >= lower AND _distance < upper` on the exact distances (scanner.rs:3342-3377)
@@ -1640,6 +1654,7 @@ lb2_status lb2_index_repartition(const lb2_index* shard, lb2_index** owned_out) 
   Comm* cm = current_comm();
   const int G = cm ? cm->nranks : 1, me = cm ? cm->rank : 0;
   const int K = shard->K;
+  // the row payload: IVF_FLAT's vectors, or the codes of IVF_PQ / IVF_SQ (code_bytes() = d for IVF_SQ)
   const int rb = shard->kind == 1 ? (int)shard->vrow_bytes() : shard->code_bytes();
   const uint8_t* payload = shard->kind == 1 ? shard->vectors.p : shard->codes.p;
   // every rank's partition sizes (one all-gather of K counters), then the layouts on the host
@@ -1701,6 +1716,7 @@ lb2_status lb2_index_repartition(const lb2_index* shard, lb2_index** owned_out) 
   std::unique_ptr<lb2_index> ix(new lb2_index());
   ix->kind = shard->kind; ix->dtype = shard->dtype; ix->K = K; ix->d = shard->d; ix->M = shard->M;
   ix->nbits = shard->nbits; ix->metric = shard->metric; ix->n = n_new;
+  ix->sq_lower = shard->sq_lower; ix->sq_upper = shard->sq_upper;
   ix->centroids.alloc((size_t)K * shard->d);
   d2d(ix->centroids.p, shard->centroids.p, (size_t)K * shard->d);
   if (shard->kind == 0) {
@@ -1900,13 +1916,12 @@ void lb2_ivfflat_build_params_default(lb2_ivfflat_build_params* p) {
   p->seed = 0;
 }
 
-lb2_status lb2_index_create_flat(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype,
-                                 lb2_metric metric, lb2_index** out) {
-  LB2_API_BEGIN
-  LB2_REQUIRE(out && centroids, "null argument");
+// an empty IVF_FLAT / IVF_SQ index with the caller's centroids (in the model type of `dtype`)
+static lb2_index* index_with_centroids(int kind, const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype,
+                                       lb2_metric metric) {
   ctx();
-  lb2_index* ix = new lb2_index();
-  ix->kind = 1; ix->K = k; ix->d = d; ix->M = 0; ix->nbits = 0; ix->metric = metric_of(metric);
+  std::unique_ptr<lb2_index> ix(new lb2_index());
+  ix->kind = kind; ix->K = k; ix->d = d; ix->M = 0; ix->nbits = 0; ix->metric = metric_of(metric);
   ix->dtype = dtype;
   ix->centroids.alloc((size_t)k * d);
   {
@@ -1917,7 +1932,14 @@ lb2_status lb2_index_create_flat(const void* centroids, uint32_t k, uint32_t d, 
   ix->part_offsets.alloc(k + 1);
   ix->part_offsets.zero();
   sync_stream();
-  *out = ix;
+  return ix.release();
+}
+
+lb2_status lb2_index_create_flat(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype,
+                                 lb2_metric metric, lb2_index** out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(out && centroids, "null argument");
+  *out = index_with_centroids(1, centroids, k, d, dtype, metric);
   LB2_API_END
 }
 
@@ -2036,6 +2058,43 @@ void train_ivf(const float* xs, uint64_t s, int d, int K, int am, const lb2_kmea
 }
 }  // namespace
 
+// The IVF stage shared by the IVF_FLAT and IVF_SQ builds: sample (ivf.rs:1237-1241) -> drop rows that are not
+// finite -> train (normalised first under cosine) -> centroids rounded to the column's type.  Starts the bulk copy.
+static void train_ivf_stage(Source& src, lb2_index* ix, const lb2_kmeans_params& kp, uint64_t seed, uint64_t nranks,
+                            std::vector<double>* loss, std::vector<uint32_t>* iters) {
+  TagScope tg("ivf_train");
+  const uint64_t n = src.n();
+  const int d = src.d(), K = ix->K, m = ix->metric;
+  const int am = m == METRIC_DOT ? METRIC_DOT : METRIC_L2;
+  const uint64_t s0 = std::min<uint64_t>(n, ((uint64_t)K * kp.sample_rate + nranks - 1) / nranks);
+  std::vector<uint64_t> rows = sample_rows(n, s0, seed);
+  DevBuf<float> sample;
+  const uint64_t s = gather_finite_sample(src, rows, m == METRIC_COSINE, sample);
+  src.start_resident_copy();  // host rows: the bulk copy runs on its own stream while the centroids train
+  LB2_REQUIRE(nranks > 1 || s >= (uint64_t)K, "KMeans: can not train %d centroids with %llu finite vectors", K,
+              (unsigned long long)s);
+  VecIn init(kp.init_centroids, (size_t)K * d, model_dtype(ix->dtype));
+  train_ivf(sample.p, s, d, K, am, kp, nranks, init.get(), ix->centroids.p, loss, iters);
+  round_model(ix->centroids.p, (size_t)K * d, ix->dtype);
+}
+
+// partition assignment of one chunk of rows (IVF_FLAT / IVF_SQ transform); returns the chunk as f32 as the index
+// sees it: normalised under cosine (NormalizeTransformer first, ivf.rs:158-166)
+static const float* assign_flat_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
+                                      const float* cent, int K, DevBuf<float>& normbuf, uint32_t* part,
+                                      uint8_t* valid) {
+  const int am = m == METRIC_DOT ? METRIC_DOT : METRIC_L2;
+  const float* xp = xf;
+  if (m == METRIC_COSINE) {
+    if (normbuf.n < (size_t)rows * d) normbuf.alloc((size_t)rows * d);
+    LB2_LAUNCH("normalize", normalize_kernel, cdiv(rows, 128), 128, 0, xf, rows, d, normbuf.p);
+    xp = normbuf.p;
+    xnat = nullptr;
+  }
+  assign_f32(xp, rows, d, cent, K, am, nullptr, part, nullptr, valid, nullptr, xnat, dtype);
+  return xp;
+}
+
 lb2_status lb2_ivfflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype,
                              lb2_metric metric, const lb2_ivfflat_build_params* params,
                              const uint64_t* row_ids, lb2_index** out, lb2_build_stats* stats) {
@@ -2050,25 +2109,12 @@ lb2_status lb2_ivfflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype
   EventSet ev(4);
   ev.record(0);
   Source src(data, n, (int)d, dtype);
-  const int am = m == METRIC_DOT ? METRIC_DOT : METRIC_L2;
   std::unique_ptr<lb2_index> ix(new lb2_index());
   ix->kind = 1; ix->K = K; ix->d = d; ix->M = 0; ix->nbits = 0; ix->metric = m; ix->dtype = dtype;
   ix->centroids.alloc((size_t)K * d);
   std::vector<double> loss;
   std::vector<uint32_t> iters;
-  {
-    TagScope tg("ivf_train");
-    const uint64_t s0 = std::min<uint64_t>(n, ((uint64_t)K * params->ivf.sample_rate + nranks - 1) / nranks);
-    std::vector<uint64_t> rows = sample_rows(n, s0, params->seed);
-    DevBuf<float> sample;
-    const uint64_t s = gather_finite_sample(src, rows, m == METRIC_COSINE, sample);
-    src.start_resident_copy();  // host rows: the bulk copy runs on its own stream while the centroids train
-    LB2_REQUIRE(nranks > 1 || s >= (uint64_t)K, "KMeans: can not train %d centroids with %llu finite vectors", K,
-                (unsigned long long)s);
-    VecIn init(params->ivf.init_centroids, (size_t)K * d, model_dtype(dtype));
-    train_ivf(sample.p, s, d, K, am, params->ivf, nranks, init.get(), ix->centroids.p, &loss, &iters);
-    round_model(ix->centroids.p, (size_t)K * d, dtype);
-  }
+  train_ivf_stage(src, ix.get(), params->ivf, params->seed, nranks, &loss, &iters);
   ev.record(1);
   DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
   DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1));
@@ -2076,15 +2122,8 @@ lb2_status lb2_ivfflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype
     TagScope tg("transform");
     DevBuf<float> normbuf;
     for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
-      const float* xp = xf;
-      if (m == METRIC_COSINE) {  // NormalizeTransformer first (ivf.rs:158-166)
-        if (normbuf.n < (size_t)rows * d) normbuf.alloc((size_t)rows * d);
-        LB2_LAUNCH("normalize", normalize_kernel, cdiv(rows, 128), 128, 0, xf, rows, (int)d, normbuf.p);
-        xp = normbuf.p;
-        xnat = nullptr;
-      }
-      assign_f32(xp, rows, d, ix->centroids.p, K, am, nullptr, part.p + r0, nullptr, valid.p + r0, nullptr, xnat,
-                 (int)src.dtype());
+      assign_flat_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, normbuf, part.p + r0,
+                        valid.p + r0);
     });
   }
   ev.record(2);
@@ -2101,6 +2140,163 @@ lb2_status lb2_ivfflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype
     stats->ms_transform = ev.ms(1, 2);
     stats->ms_group = ev.ms(2, 3);
     stats->ms_total = ev.ms(0, 3);
+    stats->ivf_iters = iters.empty() ? 0 : iters[0];
+    stats->ivf_loss = loss.empty() ? 0.0 : loss[0];
+  }
+  *out = ix.release();
+  LB2_API_END
+}
+
+// ---- IVF_SQ: IVFIndex<FlatIndex, ScalarQuantizer> (lance-index/src/vector/sq*.rs) --------------------------------
+static void sq_check_dim(uint32_t d) {
+  LB2_REQUIRE(d > 0 && d % 4 == 0, "IVF_SQ needs a dimension that is a multiple of 4");
+  // the scan sums d terms of up to 255^2 in u32 (sq/storage.rs:432-468)
+  LB2_REQUIRE((uint64_t)d * 255 * 255 < (1ull << 32), "IVF_SQ: d * 255^2 must be below 2^32, d = %u", d);
+}
+
+lb2_status lb2_sq_train(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, double* lower_out,
+                        double* upper_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE((data || n == 0) && lower_out && upper_out, "null argument");
+  ctx();
+  VecIn x(data, (size_t)n * d, dtype);
+  sq_bounds_f32(x.get(), (uint64_t)n * d, lower_out, upper_out);
+  LB2_API_END
+}
+
+lb2_status lb2_sq_encode(const void* vectors, uint64_t n, uint32_t d, lb2_dtype dtype, double lower, double upper,
+                         uint8_t* codes_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE((vectors && codes_out) || n == 0, "null argument");
+  ctx();
+  VecIn x(vectors, (size_t)n * d, dtype);
+  OutArg<uint8_t> o(codes_out, (size_t)n * d);
+  sq_encode_f32(x.get(), (uint64_t)n * d, lower, upper, o.get());
+  o.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_index_create_sq(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                               double lower, double upper, lb2_index** out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(out && centroids, "null argument");
+  sq_check_dim(d);
+  LB2_REQUIRE(std::isfinite(lower) && std::isfinite(upper) && lower <= upper,
+              "IVF_SQ: the bounds must be finite with lower <= upper, got [%g, %g]", lower, upper);
+  std::unique_ptr<lb2_index> ix(index_with_centroids(2, centroids, k, d, dtype, metric));
+  ix->nbits = 8;
+  ix->sq_lower = lower;
+  ix->sq_upper = upper;
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_index_load_sq(lb2_index* index, const uint32_t* part_ids, const uint8_t* codes,
+                             const uint64_t* row_ids, uint64_t n) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == 2, "not an IVF_SQ index");
+  InArg<uint32_t> p(part_ids, n);
+  InArg<uint8_t> c(codes, (size_t)n * index->d);
+  InArg<uint64_t> r(row_ids, n);
+  check_part_ids(p.get(), n, (uint32_t)index->K, "index_load_sq");
+  index_load_dev(index, p.get(), c.get(), r.get(), n);
+  LB2_API_END
+}
+
+lb2_status lb2_index_export_sq(const lb2_index* index, void* centroids_out, double* bounds_out,
+                               uint64_t* part_offsets_out, uint8_t* codes_out, uint64_t* row_ids_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == 2, "not an IVF_SQ index");
+  cudaStream_t s = ctx().stream;
+  if (bounds_out) {
+    bounds_out[0] = index->sq_lower;
+    bounds_out[1] = index->sq_upper;
+  }
+  if (centroids_out)
+    LB2_CUDA(cudaMemcpyAsync(centroids_out, index->centroids.p, sizeof(float) * index->K * index->d, cudaMemcpyDefault, s));
+  if (part_offsets_out)
+    LB2_CUDA(cudaMemcpyAsync(part_offsets_out, index->part_offsets.p, sizeof(uint64_t) * (index->K + 1), cudaMemcpyDefault, s));
+  if (codes_out && index->n)
+    LB2_CUDA(cudaMemcpyAsync(codes_out, index->codes.p, index->n * index->code_bytes(), cudaMemcpyDefault, s));
+  if (row_ids_out && index->n)
+    LB2_CUDA(cudaMemcpyAsync(row_ids_out, index->row_ids.p, sizeof(uint64_t) * index->n, cudaMemcpyDefault, s));
+  sync_stream();
+  LB2_API_END
+}
+
+void lb2_ivfsq_build_params_default(lb2_ivfsq_build_params* p) {
+  p->num_partitions = 256;
+  lb2_kmeans_params_default(&p->ivf);
+  p->ivf.balance_factor = 1.0f;
+  p->num_bits = 8;
+  p->sample_rate = 256;
+  p->seed = 0;
+}
+
+lb2_status lb2_ivfsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                           const lb2_ivfsq_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                           lb2_build_stats* stats) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(data && params && out, "null argument");
+  sq_check_dim(d);
+  if (params->num_bits != 8) fail(LB2_UNSUPPORTED, "IVF_SQ: num_bits = %u is not implemented (8 only)", params->num_bits);
+  if (current_comm() && current_comm()->nranks > 1)
+    fail(LB2_UNSUPPORTED, "IVF_SQ: builds sharded over ranks are not implemented (the bounds would need an exchange)");
+  const int m = metric_of(metric);
+  const int K = params->num_partitions;
+  LB2_REQUIRE(K > 0 && n >= (uint64_t)K, "KMeans: can not train %d centroids with %llu vectors", K, (unsigned long long)n);
+  EventSet ev(5);
+  ev.record(0);
+  Source src(data, n, (int)d, dtype);
+  std::unique_ptr<lb2_index> ix(new lb2_index());
+  ix->kind = 2; ix->K = K; ix->d = d; ix->M = 0; ix->nbits = 8; ix->metric = m; ix->dtype = dtype;
+  ix->centroids.alloc((size_t)K * d);
+  std::vector<double> loss;
+  std::vector<uint32_t> iters;
+  // 1. IVF: the same stage as lb2_ivfflat_build (same sample, seed, training)
+  train_ivf_stage(src, ix.get(), params->ivf, params->seed, 1, &loss, &iters);
+  ev.record(1);
+  // 2. ScalarQuantizer::build (sq.rs:152-182) on sample_rate * 2^num_bits rows (builder.rs:410-421), normalised
+  //    under cosine, rows that are not finite dropped (builder.rs:436), no residuals (quantizer.rs:52).  The bounds
+  //    are taken over the values the index stores: normalised, in the column's element type.
+  {
+    TagScope tg("sq_train");
+    std::vector<uint64_t> rows = sample_rows(n, std::min<uint64_t>(n, params->sample_rate * 256), params->seed + 1);
+    DevBuf<float> sample;
+    const uint64_t s = gather_finite_sample(src, rows, m == METRIC_COSINE, sample);
+    round_model(sample.p, (size_t)s * d, dtype);
+    sq_bounds_f32(sample.p, (uint64_t)s * d, &ix->sq_lower, &ix->sq_upper);
+  }
+  ev.record(2);
+  // 3. transform (ivf.rs:238-279): partition, then the SQ codes of the stored vectors themselves
+  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
+  DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1)), codes(std::max<uint64_t>(1, (uint64_t)n * d));
+  {
+    TagScope tg("transform");
+    DevBuf<float> normbuf;
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      const float* xs = assign_flat_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, normbuf,
+                                          part.p + r0, valid.p + r0);
+      if (m == METRIC_COSINE) round_model(normbuf.p, (size_t)rows * d, dtype);  // as IVF_FLAT stores them
+      sq_encode_f32(xs, (uint64_t)rows * d, ix->sq_lower, ix->sq_upper, codes.p + r0 * d);
+    });
+  }
+  ev.record(3);
+  {
+    TagScope tg("group");
+    InArg<uint64_t> rid(row_ids, n);
+    index_load_dev(ix.get(), part.p, codes.p, rid.get(), n, valid.p);
+  }
+  ev.record(4);
+  sync_stream();
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->ms_ivf_train = ev.ms(0, 1);
+    stats->ms_pq_train = ev.ms(1, 2);
+    stats->ms_transform = ev.ms(2, 3);
+    stats->ms_group = ev.ms(3, 4);
+    stats->ms_total = ev.ms(0, 4);
     stats->ivf_iters = iters.empty() ? 0 : iters[0];
     stats->ivf_loss = loss.empty() ? 0.0 : loss[0];
   }

@@ -35,6 +35,12 @@ void ivfflat_search_f32(const float* centroids, int K, int d, int metric, const 
                         const void* vectors, int vdt, const uint64_t* row_ids, const float* queries, uint64_t nq,
                         int k, int nprobes, uint64_t* out_ids, float* out_dists, uint32_t* out_counts,
                         const ScanFilter& flt = ScanFilter());
+// codes: the index's SQ codes [n][d] in partition order; qcodes: the queries' codes [nq][d] under the same bounds;
+// r2 = rf * rf with rf = (float)(upper - lower); queries: f32 (normalised for cosine), for the probe selection
+void ivfsq_search_f32(const float* centroids, int K, int d, int metric, const uint64_t* part_offsets,
+                      const uint8_t* codes, const uint64_t* row_ids, float r2, const float* queries,
+                      const uint8_t* qcodes, uint64_t nq, int k, int nprobes, uint64_t* out_ids, float* out_dists,
+                      uint32_t* out_counts, const ScanFilter& flt = ScanFilter());
 // all ranks' [nq][k] results of a row-sharded index -> the global top-k by (distance, row id) on every rank
 void merge_sharded_topk(const uint64_t* ids, const float* dists, const uint32_t* counts, uint64_t nq, int k,
                         uint64_t* out_ids, float* out_dists, uint32_t* out_counts);
