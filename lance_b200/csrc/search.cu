@@ -293,6 +293,18 @@ __device__ __forceinline__ float pq8_row_distance(const float* lut, const uint8_
   return dist;
 }
 
+// The 4-bit quantisation range (qmax - qmin) / 255 and the dequantisation q * range + qmin as x86 (where the reference
+// runs) evaluates them when the table is not finite: r = a op b, but an invalid operation (0 * Inf, Inf - Inf) gives
+// the default NaN 0xFFC00000, whose sign bit puts it before every number in f32::total_cmp order, and a NaN operand
+// passes through.  The device's own NaN is 0x7FFFFFFF, which orders after every number.
+__device__ __forceinline__ float x86_nan(float r, float a, float b) {
+  return r == r ? r : a != a ? a : b != b ? b : __int_as_float(0xffc00000);
+}
+__device__ __forceinline__ float pq4_dequantize(uint32_t q, const float* params) {
+  const float qf = (float)q, p = x86_nan(__fmul_rn(qf, params[1]), qf, params[1]);
+  return x86_nan(__fadd_rn(p, params[0]), p, params[0]);
+}
+
 // 4-bit table quantisation (pq/distance.rs:147-242), one block of 256 threads: qmin = min(table) (f32::min ignores
 // NaN), qmax = max of the flat rows' distances flat_dist(j), j < flat_num, in total order; qt = the table quantised
 // to u8, params = {qmin, (qmax - qmin) / 255}.  r_mx / r_mn: 256 entries of reduction scratch each.
@@ -323,7 +335,8 @@ __device__ __forceinline__ void pq4_quantize(const float* lut, int M, uint64_t f
   }
   if (tid == 0) {
     params[0] = qmin;
-    params[1] = __fdiv_rn(__fsub_rn(qmax, qmin), 255.0f);
+    const float span = x86_nan(__fsub_rn(qmax, qmin), qmax, qmin);
+    params[1] = x86_nan(__fdiv_rn(span, 255.0f), span, 255.0f);
   }
   __syncthreads();
 }
@@ -355,11 +368,12 @@ __device__ __forceinline__ bool slot_excluded(const ScanFilter& f, uint64_t off,
 
 // The kk smallest (key, position) pairs of rows [0, n); excluded rows take the maximal key, so they only surface when
 // fewer than kk rows are left.  Returns their number; they are left unordered at ukey[SCAN_CHUNK ..) / cpos.
+// max_admitted: some admitted row has the maximal key too (a NaN distance), so it ties with the excluded rows.
 template <class Fill>
 __device__ __forceinline__ uint32_t slot_select(const SlotSmem& s, uint32_t n, uint32_t kk, const ScanFilter& flt, uint64_t off,
-                                Fill fill) {
+                                Fill fill, bool& max_admitted) {
   __shared__ uint32_t hist[256], s_wsum[8];
-  __shared__ uint32_t s_prefix, s_need, s_eq, s_out;
+  __shared__ uint32_t s_prefix, s_need, s_eq, s_out, s_maxadm;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const bool filtering = flt.allow != nullptr || flt.range;
   uint32_t nw = 0;
@@ -367,13 +381,16 @@ __device__ __forceinline__ uint32_t slot_select(const SlotSmem& s, uint32_t n, u
   // carried winners precede it in (key, position) order.  Such rows are left out of the pool.
   uint32_t lim = 0xffffffffu;
   bool full = false;
+  if (tid == 0) s_maxadm = 0;  // ordered before any store by the barrier after the first fill
   for (uint32_t c0 = 0; c0 < n; c0 += SCAN_CHUNK) {
     const uint32_t clen = min((uint32_t)SCAN_CHUNK, n - c0);
     fill(c0, clen);
     __syncthreads();
     if (filtering) {
-      for (uint32_t j = tid; j < clen; j += 256)
+      for (uint32_t j = tid; j < clen; j += 256) {
         if (slot_excluded(flt, off, c0 + j, s.ukey[j])) s.ukey[j] = 0xffffffffu;
+        else if (s.ukey[j] == 0xffffffffu) s_maxadm = 1;
+      }
       __syncthreads();
     }
     // pool element i: i < clen -> (ukey[i], c0 + i), else the carried winner i - clen at ukey[SCAN_CHUNK ..)
@@ -455,16 +472,19 @@ __device__ __forceinline__ uint32_t slot_select(const SlotSmem& s, uint32_t n, u
     lim = T;
     __syncthreads();
   }
+  max_admitted = n > 0 && s_maxadm != 0;  // every pass of the loop ends in a barrier
   return nw;
 }
 
 // The finish, on the nw <= kk winners in (key, position) order: excluded winners at the end are dropped (they carry
 // the maximal key; an admitted row whose key is the maximal one, e.g. a NaN distance, keeps the excluded winners before
 // it).  If kk winners remain and the last two share a key, more rows tie at the k-th distance than fit and the
-// reference's heap decides: returns false.  Otherwise leaves the admitted winners among the first k at nkey / npos
-// (unordered), sets *cnt and returns true.
-__device__ __forceinline__ bool slot_finish(const SlotSmem& s, uint32_t nw, uint32_t kk, const ScanFilter& flt, uint64_t off,
-                            uint32_t* cnt) {
+// reference's heap decides: returns false.  So it does when excluded winners were dropped from the end of a full
+// selection while an admitted row shares their key (max_admitted): admitted rows behind the kk may then belong in the
+// result.  Otherwise leaves the admitted winners among the first k at nkey / npos (unordered), sets *cnt and returns
+// true.
+__device__ __forceinline__ bool slot_finish(const SlotSmem& s, uint32_t nw, uint32_t kk, bool max_admitted,
+                            const ScanFilter& flt, uint64_t off, uint32_t* cnt) {
   __shared__ uint32_t s_kept, s_max, s_maxcnt, s_last, s_mid, s_out;
   const int tid = threadIdx.x;
   if (tid == 0) { s_kept = 0; s_max = 0; s_maxcnt = 0; s_last = 0; s_mid = 0; s_out = 0; }
@@ -490,6 +510,7 @@ __device__ __forceinline__ bool slot_finish(const SlotSmem& s, uint32_t nw, uint
   const uint32_t kept = s_kept, mid = s_mid;
   const bool at_k = kept + mid == kk;
   if (at_k && s_maxcnt + mid >= 2) return false;  // block-uniform
+  if (nw == kk && !at_k && max_admitted) return false;
   for (uint32_t i = tid; i < nw; i += 256) {
     const uint32_t key = s.ukey[SCAN_CHUNK + i], pos = s.cpos[i];
     if (slot_excluded(flt, off, pos, key) || (at_k && key == mx)) continue;  // at_k: the (k+1)-th is the unique max
@@ -535,7 +556,9 @@ __device__ __forceinline__ uint32_t slot_topk(const SlotSmem& s, uint32_t n, int
                               Fill fill) {
   if (!replay) {
     uint32_t cnt;
-    if (slot_finish(s, slot_select(s, n, k + 1, flt, off, fill), k + 1, flt, off, &cnt)) return cnt;
+    bool max_admitted;
+    const uint32_t nw = slot_select(s, n, k + 1, flt, off, fill, max_admitted);
+    if (slot_finish(s, nw, k + 1, max_admitted, flt, off, &cnt)) return cnt;
     __syncthreads();
   }
   return slot_replay(s, n, k, flt, off, fill);
@@ -556,8 +579,8 @@ template <int METRIC, int NBITS>
 __device__ void radix_slot(const ScanArgs& a, size_t slot, bool replay) {
   extern __shared__ float smem[];
   const int M = a.M, d = a.d, k = a.k, np = a.np;
-  float* lut = smem;                   // [M*16] (4-bit) or [M*256] (8-bit)
-  float* qr = lut + M * 256;           // [d]
+  float* lut = smem;                         // [M*16] (4-bit) or [M*256] (8-bit)
+  float* qr = lut + M * (NBITS == 4 ? 16 : 256);  // [d]
   const SlotSmem s(qr + d, k + 1);
   const int tid = threadIdx.x;
   const int pi = (int)(slot % np);
@@ -608,12 +631,13 @@ __device__ void radix_slot(const ScanArgs& a, size_t slot, bool replay) {
             qs += qt[(2 * i2) * 16 + (c & 0xF)];
             qs += qt[(2 * i2 + 1) * 16 + (c >> 4)];
           }
-          dist = __fadd_rn(__fmul_rn((float)min(qs, 255u), s_q[1]), s_q[0]);
+          dist = pq4_dequantize(min(qs, 255u), s_q);
         }
       } else {
         dist = pq8_row_distance(lut, pc + (size_t)row * M, M);
       }
-      if (METRIC == METRIC_DOT) dist = __fsub_rn(dist, dot_fix);  // pq/storage.rs:957-958
+      // pq/storage.rs:957-958; a NaN passes through, as on x86 (the device's own NaN would stay canonical anyway)
+      if (METRIC == METRIC_DOT && dist == dist) dist = __fsub_rn(dist, dot_fix);
       s.ukey[j] = (uint32_t)total_order_key(dist) ^ 0x80000000u;
     }
   };
@@ -1471,6 +1495,15 @@ flat_topk_kernel(const float* __restrict__ dists, const uint64_t* __restrict__ r
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
+// the shared memory a launch of `kernel` with `dyn` dynamic bytes takes: its static shared memory counts against the
+// same per-block opt-in limit, and cudaFuncSetAttribute refuses a dynamic size that leaves no room for it
+template <class Kern>
+static size_t smem_with_static(Kern kernel, size_t dyn) {
+  cudaFuncAttributes fa;
+  LB2_CUDA(cudaFuncGetAttributes(&fa, kernel));
+  return dyn + fa.sharedSizeBytes;
+}
+
 void find_partitions_f32(const float* centroids, int K, int d, int metric, const float* queries,
                          uint64_t nq, int nprobes, uint32_t* ids, float* dists) {
   if (nq == 0) return;
@@ -1609,8 +1642,24 @@ void ivfpq_search_f32(const float* centroids, int K, int d, int metric, const fl
   if (nbits == 4 && (M % 2 != 0 || M > 256)) fail(LB2_UNSUPPORTED, "4-bit PQ needs an even num_sub_vectors <= 256");
   if (k > 1024) fail(LB2_UNSUPPORTED, "k (incl. refine factor) > 1024 is not implemented");
   const int np = nprobes < K ? nprobes : K;
-  const size_t smem = sizeof(float) * ((size_t)M * 256 + d) + slot_smem_bytes(k);
-  if (smem > ctx().smem_optin) fail(LB2_UNSUPPORTED, "LUT of %zu bytes exceeds shared memory", smem);
+  const size_t smem = sizeof(float) * ((size_t)M * (nbits == 4 ? 16 : 256) + d) + slot_smem_bytes(k);
+  // every kernel the scan may launch must fit: the radix kernel (the scan itself, or the tie replay of the fast
+  // 8-bit kernels) and, for k + 1 <= SCAN_KFAST, the classic fast kernel with its LUT and larger static lists
+  size_t need = 0;
+  auto need_of = [&](auto m) {
+    constexpr int METRIC = decltype(m)::value;
+    need = nbits == 4 ? smem_with_static(ivfpq_scan_radix_kernel<METRIC, 4>, smem)
+                      : smem_with_static(ivfpq_scan_radix_kernel<METRIC, 8>, smem);
+    if (nbits == 8 && k + 1 <= SCAN_KFAST) {
+      const size_t fast = sizeof(float) * ((size_t)M * 256 + d);
+      const bool filtering = flt.allow != nullptr || flt.range;
+      need = std::max(need, filtering ? smem_with_static(ivfpq_scan_kernel<METRIC, true>, fast)
+                                      : smem_with_static(ivfpq_scan_kernel<METRIC, false>, fast));
+    }
+  };
+  if (metric == METRIC_DOT) need_of(std::integral_constant<int, METRIC_DOT>{});
+  else need_of(std::integral_constant<int, METRIC_L2>{});
+  if (need > ctx().smem_optin) fail(LB2_UNSUPPORTED, "LUT and top-k scratch of %zu bytes exceed shared memory", need);
   DevBuf<uint32_t> rlist((size_t)std::min<uint64_t>(nq, SEARCH_SLAB) * np), rcount(1);
   ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
              [&](uint64_t q0, uint64_t qn, const uint32_t* pids, float* cd, uint64_t* cid, uint32_t* ccnt) {
@@ -1682,7 +1731,11 @@ void ivfflat_search_f32(const float* centroids, int K, int d, int metric, const 
   if (nq == 0 || k == 0) return;
   if (k > 1024) fail(LB2_UNSUPPORTED, "k (incl. refine factor) > 1024 is not implemented");
   const size_t smem = sizeof(float) * (size_t)d + slot_smem_bytes(k);
-  if (smem > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the flat scan", d);
+  size_t need = 0;
+  dispatch_metric_elem<false>(metric, vdt, [&](auto m, auto e) {
+    need = smem_with_static(ivfflat_scan_kernel<decltype(m)::value, typename decltype(e)::type>, smem);
+  });
+  if (need > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the flat scan", d);
   const int np = nprobes < K ? nprobes : K;
   ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
              [&](uint64_t q0, uint64_t qn, const uint32_t* pids, float* cd, uint64_t* cid, uint32_t* ccnt) {
@@ -1703,21 +1756,25 @@ void ivfsq_search_f32(const float* centroids, int K, int d, int metric, const ui
   if (nq == 0 || k == 0) return;
   if (k > 1024) fail(LB2_UNSUPPORTED, "k (incl. refine factor) > 1024 is not implemented");
   const size_t smem = (size_t)(d + 15) / 16 * 16 + slot_smem_bytes(k);
-  if (smem > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the SQ scan", d);
+  auto with_kernel = [&](auto f) {
+    const bool vec4 = d % 16 == 0;
+    if (metric == METRIC_DOT) {
+      if (vec4) f(ivfsq_scan_kernel<METRIC_DOT, true>); else f(ivfsq_scan_kernel<METRIC_DOT, false>);
+    } else {  // cosine: L2 on the normalised vectors' codes (sq/storage.rs:436-440)
+      if (vec4) f(ivfsq_scan_kernel<METRIC_L2, true>); else f(ivfsq_scan_kernel<METRIC_L2, false>);
+    }
+  };
+  size_t need = 0;
+  with_kernel([&](auto kern) { need = smem_with_static(kern, smem); });
+  if (need > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the SQ scan", d);
   const int np = nprobes < K ? nprobes : K;
   ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
              [&](uint64_t q0, uint64_t qn, const uint32_t* pids, float* cd, uint64_t* cid, uint32_t* ccnt) {
-               auto go = [&](auto kern) {
+               with_kernel([&](auto kern) {
                  set_smem(kern, smem);
                  LB2_LAUNCH("sq_scan", kern, dim3(np, (unsigned)qn), 256, smem, qcodes + q0 * d, d, r2, pids, np,
                             part_offsets, codes, row_ids, k, cd, cid, ccnt, flt);
-               };
-               const bool vec4 = d % 16 == 0;
-               if (metric == METRIC_DOT) {
-                 if (vec4) go(ivfsq_scan_kernel<METRIC_DOT, true>); else go(ivfsq_scan_kernel<METRIC_DOT, false>);
-               } else {  // cosine: L2 on the normalised vectors' codes (sq/storage.rs:436-440)
-                 if (vec4) go(ivfsq_scan_kernel<METRIC_L2, true>); else go(ivfsq_scan_kernel<METRIC_L2, false>);
-               }
+               });
              });
 }
 
@@ -1896,11 +1953,11 @@ __global__ void pq4_quant_scan_kernel(const uint8_t* __restrict__ qt, int nb, co
     q += s_qt[(2 * i + 1) * 16 + (c >> 4)];
   }
   q = min(q, 255u);
-  out[j] = __fadd_rn(__fmul_rn((float)q, params[1]), params[0]);
+  out[j] = pq4_dequantize(q, params);
 }
 __global__ void sub_scalar_kernel(float* __restrict__ v, uint64_t n, float s) {
   const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < n) v[j] = __fsub_rn(v[j], s);
+  if (j < n && v[j] == v[j]) v[j] = __fsub_rn(v[j], s);  // a NaN passes through (see x86_nan)
 }
 void pq_scan_4bit_f32(const float* lut, int M, int metric, const uint8_t* codes_t, uint64_t n, uint64_t k_hint,
                       float* out) {

@@ -1289,7 +1289,7 @@ def test_skew_scan_kernel_matches_oracle_and_classic(metric):
     bm = ix.row_mask(allow, None)
     lb.profile.reset()
     lb.profile.enable(True)
-    for k, nprobes in ((1, 3), (10, K), (15, 7), (5, 1), (100, 6), (135, K), (40, 2)):   # k > 15: the refine sizes
+    for k, nprobes in ((1, 3), (10, K), (15, 7), (5, 1), (100, 6), (135, K), (40, 2)):   # k > 15: the radix slot
         oi, od, oc = ob.ivfpq_search(parts["centroids"], parts["codebook"], parts["part_offsets"], parts["codes"],
                                      parts["row_ids"], q, k, nprobes, metric=metric, nthreads=NT)
         for mode in ("skew", "skew4", "classic"):
