@@ -18,8 +18,8 @@
 // relative error <= 2^-10 (truncation); |x.c - tf32(x).tf32(c)| <= 2^-9 * sum|x_i||c_i|
 // <= 2^-10 (|x|^2 + |c|^2).  Two scores are compared, index packing perturbs by 2^-15 |score|, the
 // f32 accumulation by far less: tau = 3 * 2^-10 * (|x|^2 + max_c |c|^2) covers 2x the bound with
-// 20% to spare.  Whatever tau is, results stay exact as long as the bound holds; a larger tau only
-// sends more rows to the exact paths.
+// 20% to spare; below the normal f32 range the norm term has a floor (cert_tau, tc_common.cuh).  Whatever
+// tau is, results stay exact as long as the bound holds; a larger tau only sends more rows to the exact paths.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -140,7 +140,7 @@ tc_filter_kernel(const __grid_constant__ CUtensorMap map_x, const __grid_constan
       if ((lane & 3) < 2) {  // lanes 0 / 1 of the quad write rows r0 / r0 + 8
         const uint64_t row = tile * TM + frag_row(lane & 1);
         if (row < n) {
-          const uint32_t flag = verdict(m[0], m[1], m[2], tau_scale * (row_norm2[row] + cmax2));
+          const uint32_t flag = verdict(m[0], m[1], m[2], cert_tau(tau_scale, row_norm2[row] + cmax2));
           res[row] = (__float_as_uint(m[0]) & 0xFFu) | ((__float_as_uint(m[1]) & 0xFFu) << 12) | (flag << 30);
         }
       }
@@ -281,7 +281,7 @@ tc_filter_general_kernel(const __grid_constant__ CUtensorMap map_x, const __grid
       if (nt == ntiles - 1 && (lane & 3) < 2) {  // row tile complete: lanes 0 / 1 of the quad write rows r0 / r0 + 8
         const uint64_t row = (lane & 1) ? row1 : row0;
         if (row < n) {
-          const uint32_t flag = verdict(g[0], g[1], g[2], tau_scale * (row_norm2[row] + cmax2));
+          const uint32_t flag = verdict(g[0], g[1], g[2], cert_tau(tau_scale, row_norm2[row] + cmax2));
           res[row] = gi[0] | (flag << 30);
           res_hi[row] = gi[1];
           if (top1_val && flag == 2) top1_val[row] = g[0];
@@ -494,7 +494,7 @@ __global__ void gather_split_kernel(const float* __restrict__ x, int d, const fl
       const float rn = row_norm2[row];
       rn2c[i] = rn;
       if (thr) {  // candidate pass: everything within tau of the best score the previous pass saw
-        thr[i] = top1_val[row] - tau_scale * (rn + *cmax2);
+        thr[i] = top1_val[row] - cert_tau(tau_scale, rn + *cmax2);
         cand_cnt[i] = 0;
       }
     }
@@ -519,7 +519,7 @@ __global__ void gather16_kernel(const uint16_t* __restrict__ x, int d, const flo
     if (e == 0) {
       const float rn = row_norm2[row];
       rn2c[i] = rn;
-      thr[i] = top1_val[row] - tau_scale * (rn + *cmax2);
+      thr[i] = top1_val[row] - cert_tau(tau_scale, rn + *cmax2);
       cand_cnt[i] = 0;
     }
   }

@@ -23,6 +23,17 @@ constexpr int NUM_THREADS = 384;  // warpgroup 0: TMA producer (one thread); war
                                   // alternate tiles, so that one warpgroup's epilogue overlaps the other's MMAs
 constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;  // 128 * 40 + 256 * 232 <= 64 K registers
 
+// The certificate of every filter: tau = tau_scale * max(|x|^2 + max|c|^2, NORM_FLOOR) (DESIGN.md section 5).
+// The relative bounds hold while operands, products and sums are normal f32 numbers.  Below that range roundings are
+// absolute (<= 2^-149 each; a product flushed to zero loses < 2^-126; the packed column index moves a subnormal score
+// by < 2^-141) while tau_scale * (|x|^2 + max|c|^2) underflows to 0.  With the floor tau >= 2^-13 * 2^-90 = 2^-103,
+// twice the worst absolute error of a score (d * 2^-126 + 2^-141 <= 2^-114 at d <= 4096): rows below the floor become
+// undecided and take the exact path, tau of every other row is unchanged.  `s < F ? F : s` keeps NaN / Inf norms.
+constexpr float NORM_FLOOR = 0x1p-90f;
+__device__ __forceinline__ float cert_tau(float tau_scale, float norm2) {
+  return tau_scale * (norm2 < NORM_FLOOR ? NORM_FLOOR : norm2);
+}
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

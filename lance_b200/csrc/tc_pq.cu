@@ -11,7 +11,7 @@
 //   * two wgmmas (M64 N128 K8, tf32: one per half of the codebook) per (tile, sub-space) into register
 //     accumulators, consumer warpgroups taking the work items in turns (see Pipe); the epilogue keeps the
 //     top-3 of  r.c - |c|^2/2  per row and classifies the row against tau = 3*2^-10 (|r_m|^2 + max|c_m|^2)
-//     exactly like tc_assign.cu;
+//     (with the norm floor of cert_tau) exactly like tc_assign.cu;
 //   * flag 0/1 rows are decided IN THE EPILOGUE with reference-order f32 arithmetic on the operands
 //     that are still in shared memory (sequential 8-term sum, l2.rs:69-79; strict-< / lowest index);
 //   * flag 2 (row, sub-space) pairs are appended to a list and finished by pq_fallback_kernel
@@ -216,7 +216,7 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
           const float m1 = mm[0], m2 = mm[1], m3 = mm[2];
           const float rn = j == 0 ? rn4.x : j == 1 ? rn4.y : j == 2 ? rn4.z : rn4.w;
           const float cbm = cbm_s[m];
-          const float tau = 0.0029296875f * (rn + cbm);
+          const float tau = cert_tau(0.0029296875f, rn + cbm);
           uint32_t flag = 2;
           if (m1 - m2 > tau) flag = 0;
           else if (m1 - m3 > tau) flag = 1;
@@ -364,7 +364,8 @@ __global__ void residual_norms_kernel(const float* x, const float* __restrict__ 
 //   1. pre-screen with fused multiply-adds: s'(c) = r.c - |c|^2/2, 8 FFMA per codeword instead of 24 separately
 //      rounded operations.  s' is within 2^-21 (|r|^2 + |c|^2) of the true score (8 fused steps, one rounding
 //      each, plus the rounded |c|^2), and the reference's own f32 distances are within 2^-20 (|r|^2 + |c|^2) of
-//      the true ones, so the reference's argmin has s'(c) >= max s' - 2^-18 (|r|^2 + max|c|^2) (twice the sum);
+//      the true ones, so the reference's argmin has s'(c) >= max s' - 2^-18 (|r|^2 + max|c|^2) (twice the sum;
+//      the norm term has the floor of cert_tau: below the normal range both roundings are absolute, <= 2^-149 each);
 //   2. only those few codewords get the reference-order distance (sequential 8-term sum, l2.rs:69-79), with the
 //      reference's strict-< / lowest-index rule among them.
 // A NaN anywhere makes the threshold or the scores NaN: `!(s' < thr)` then keeps the codeword and the exact
@@ -454,7 +455,7 @@ pq_fallback_kernel(const float* __restrict__ r, uint64_t n, int M, const float* 
     for (int q = 0; q < FB_P; ++q) {
 #pragma unroll
       for (int off = 8; off >= 1; off >>= 1) smax[q] = fmaxf(smax[q], __shfl_xor_sync(mask, smax[q], off, 16));
-      const float thr = smax[q] - 3.814697265625e-6f * (rn[q] + cmax);  // 2^-18
+      const float thr = smax[q] - cert_tau(3.814697265625e-6f, rn[q] + cmax);  // 2^-18
       float bv = __int_as_float(0x7f800000);
       uint32_t bi = 0xffffffffu;
 #pragma unroll

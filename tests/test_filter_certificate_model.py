@@ -2,10 +2,10 @@
 
 The product decides most rows from a reduced-precision GEMM: score_j = x.c_j - (|c_j|^2 + bias_j)/2 with the column
 index packed into the low mantissa byte, top-3 per row, and a row is *unique* when top1 - top2 > tau, *two-candidate*
-when top1 - top3 > tau, else *undecided* -- with tau = tau_scale (|x|^2 + max|c|^2).  The claim the bit-exactness of
-the whole build rests on: for a unique row the reference's argmin (exact f32 arithmetic in reference order, strict `<`,
-lowest index; lance-linalg/src/kernels.rs:79-111 over l2.rs:57-91) IS top1's column, for a two-candidate row it is one
-of top1 / top2.  The GPU tests check that end to end on an H100; this file checks the ARGUMENT on the CPU, against the
+when top1 - top3 > tau, else *undecided* -- with tau = tau_scale max(|x|^2 + max|c|^2, 2^-90) (tau_of).  The claim
+the bit-exactness of the whole build rests on: for a unique row the reference's argmin (exact f32 arithmetic in
+reference order, strict `<`, lowest index; lance-linalg/src/kernels.rs:79-111 over l2.rs:57-91) IS top1's column,
+for a two-candidate row it is one of top1 / top2.  The GPU tests check that end to end on an H100; this file checks the ARGUMENT on the CPU, against the
 oracle, under every rounding behaviour the hardware could have inside the error budget the kernels assume:
 
   * operands cut to TF32 by truncation or by round-to-nearest-even,
@@ -14,13 +14,32 @@ oracle, under every rounding behaviour the hardware could have inside the error 
   * native f16 operands (exact products) with tau16 = (2^-13 + d 2^-23)(...),
 
 on clustered data, integer-valued (SIFT-like) data full of exact ties, rows placed on bisectors of two centroids,
-duplicated centroids and a balance bias.  No GPU, no product code: numpy + the oracle only."""
+duplicated centroids and a balance bias.  No GPU, no product code: numpy + the oracle only.
+
+The norm floor.  Every error term above is relative to |x|^2 + max|c|^2, which holds while the operands, products and
+partial sums are normal f32 numbers.  Below that range roundings are absolute: up to 2^-149 per rounded operation, a
+product flushed to zero loses < 2^-126 (a flushed subnormal operand x_i loses < 2^-126 |c_i|: inside the relative
+bound while |c| >= 2^-110, inside the floor below), and packing the column index into the low mantissa byte moves a
+subnormal score by up to 255 * 2^-149 < 2^-141 -- while tau_scale (|x|^2 + max|c|^2) itself underflows to 0 (then
+the filter certifies whichever column packs highest).  So the norm term gets a floor F = 2^-90: tau >= 2^-13 F =
+2^-103 for the smallest tau_scale, which covers twice the worst absolute error of one compared score,
+d 2^-126 + 2^-141 <= 2^-114 at d <= 4096, with or without flushing.  Rows whose norms sit below the floor simply
+become undecided and take the exact path; for every other row tau is unchanged.  The comparison is `s < F ? F : s`,
+so a NaN or Inf norm still makes tau NaN / Inf and the row undecided.  test_assignment_routes.py
+checks the floor at magnitudes from 2^62 down to 2^-100."""
 import numpy as np
 import pytest
 
 from oracle import binding as ob
 
 TAU_TF32 = np.float32(3.0 * 2.0 ** -10)          # tc_assign.cu: TAU_TF32
+NORM_FLOOR = np.float32(2.0 ** -90)              # tc_common.cuh: NORM_FLOOR (module docstring)
+
+
+def tau_of(tau_scale, rn2, cmax2):
+    """tau = tau_scale * max(|x|^2 + max|c|^2, NORM_FLOOR) in f32, NaN-preserving (tc_common.cuh: cert_tau)"""
+    s = (np.asarray(rn2, np.float32) + np.float32(cmax2)).astype(np.float32)
+    return (np.float32(tau_scale) * np.where(s < NORM_FLOOR, NORM_FLOOR, s)).astype(np.float32)
 
 
 def tau3x_scale(d3):                              # tc_assign.cu: tau3x_scale(3d)
@@ -115,7 +134,7 @@ def test_tf32_first_pass_certificate(cut, accumulate, d, K):
         assert valid.all()
         cutf = tf32_trunc if cut == "trunc" else tf32_rne
         n2 = (cent * cent).sum(1, dtype=np.float32)
-        tau = TAU_TF32 * ((x * x).sum(1, dtype=np.float32) + n2.max())
+        tau = tau_of(TAU_TF32, (x * x).sum(1, dtype=np.float32), n2.max())
         flag, idx = certificate(cutf(x), cutf(cent), np.float32(-0.5) * n2, tau, accumulate)
         check(flag, idx, ref, min_decided)
 
@@ -130,7 +149,7 @@ def test_tf32_first_pass_with_balance_bias():
     ref, _, _ = ob.compute_membership(cent, x, balance_factor=bf, cluster_sizes=sizes)
     bias = (np.float32(bf) * sizes.astype(np.float32)).astype(np.float32)      # kmeans.rs:234-237
     n2 = (cent * cent).sum(1, dtype=np.float32)
-    tau = TAU_TF32 * ((x * x).sum(1, dtype=np.float32) + n2.max())
+    tau = tau_of(TAU_TF32, (x * x).sum(1, dtype=np.float32), n2.max())
     for accumulate in ("exact", "toward_zero"):
         flag, idx = certificate(tf32_trunc(x), tf32_trunc(cent), np.float32(-0.5) * (n2 + bias), tau, accumulate)
         check(flag, idx, ref, 0.5)
@@ -147,7 +166,7 @@ def test_3xtf32_refinement_certificate(accumulate):
         a3 = np.concatenate([xh, xh, xl], 1)                                   # gather_split_kernel
         b3 = np.concatenate([ch, cl, ch], 1)                                   # split_centroids_kernel
         n2 = (cent * cent).sum(1, dtype=np.float32)
-        tau = tau3x_scale(3 * d) * ((x * x).sum(1, dtype=np.float32) + n2.max())
+        tau = tau_of(tau3x_scale(3 * d), (x * x).sum(1, dtype=np.float32), n2.max())
         flag, idx = certificate(a3, b3, np.float32(-0.5) * n2, tau, accumulate)
         # the refinement is ~20x sharper than the first pass: it must decide nearly everything that has no true tie
         check(flag, idx, ref, 0.9 if name == "clustered" else 0.0)
@@ -162,7 +181,7 @@ def test_native_f16_operand_certificate(accumulate):
         cf, xf = c16.astype(np.float32), x16.astype(np.float32)
         ref, _, _ = ob.compute_membership(cf, xf)                               # l2.rs:100-106: converted exactly, f32 sums
         n2 = (cf * cf).sum(1, dtype=np.float32)
-        tau = tau16_scale(d) * ((xf * xf).sum(1, dtype=np.float32) + n2.max())
+        tau = tau_of(tau16_scale(d), (xf * xf).sum(1, dtype=np.float32), n2.max())
         flag, idx = certificate(xf, cf, np.float32(-0.5) * n2, tau, accumulate)
         check(flag, idx, ref, 0.9 if name == "clustered" else 0.0)
 
@@ -183,7 +202,8 @@ def test_model_would_catch_a_tau_that_is_too_small():
 # ---- the FMA pre-screen of pq_fallback_kernel (tc_pq.cu) -------------------------------------------------------
 # Undecided (row, sub-space) pairs are finished by a scan of all 256 codewords that first computes
 #   s'(c) = fma-chain(r . c) - |c|^2/2   (8 fused steps, cnh from an fma chain too)
-# and gives the reference-order distance only to the codewords with s'(c) >= max s' - 2^-18 (|r|^2 + max|c|^2).
+# and gives the reference-order distance only to the codewords with s'(c) >= max s' - 2^-18 max(|r|^2 + max|c|^2, 2^-90)
+# (the norm floor of the module docstring: below it the roundings of s' and of the reference are absolute).
 # Claim: the reference's argmin (sequential 8-term f32 sum, l2.rs:69-79; strict `<`, lowest index) is among them.
 def _fma(a, b, c):
     """fused multiply-add in f32: the product of two f32 is exact in f64; one rounding of the f64 sum to f32
@@ -215,7 +235,7 @@ def test_pq_fallback_prescreen_keeps_the_reference_argmin():
         s = np.broadcast_to(cnh[None, :], (n, K)).astype(np.float32)
         for t in range(ds):
             s = _fma(np.broadcast_to(r[:, t:t + 1], (n, K)), np.broadcast_to(cb[None, :, t], (n, K)), s)
-        thr = s.max(1) - np.float32(2.0 ** -18) * (rn + n2.max())
+        thr = s.max(1) - tau_of(2.0 ** -18, rn, n2.max())
         kept = ~(s < thr[:, None])
         assert kept[np.arange(n), ref].all(), "the pre-screen dropped the reference's argmin"
         assert kept.sum(1).mean() < (64 if near_ties else 8)      # ... and it is selective (that is its point)
