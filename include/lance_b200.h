@@ -397,6 +397,58 @@ lb2_status lb2_index_load_sq(lb2_index* index, const uint32_t* part_ids, const u
 lb2_status lb2_index_export_sq(const lb2_index* index, void* centroids_out, double* bounds_out,
                                uint64_t* part_offsets_out, uint8_t* codes_out, uint64_t* row_ids_out);
 
+/* ---- IVF_RQ: IVFIndex<FlatIndex, RabitQuantizer> (lance-index/src/vector/bq/) ------------------------------------
+ * create_index(.., "IVF_RQ") builds an IvfIndexBuilder<FlatIndex, RabitQuantizer> (rust/lance/src/index/vector.rs:
+ * 452-470).  code_dim = d * num_bits; the rotation R is code_dim x code_dim, of which the first d columns are used.
+ * Per row (IvfTransformer::with_rq, ivf.rs:281-328; RQTransformer, bq/transform.rs:70-220): normalised under cosine
+ * (L2 from there on), partition and dist_v_c, residual = v - c, rot[j] = dot(R[j, :d], residual); code bit j =
+ * rot[j] >= +0.0 by sign bit, LSB-first, code_dim / 8 bytes; add / scale factors.  A search rotates the (normalised)
+ * query's residual to each probed centroid the same way and scores rows from the reference's 4-bit tables
+ * (bq/storage.rs:160-445).  The rotation of a data row is defined as that same 16-lane f32 dot (the reference's GEMM
+ * has no specified order), so codes, factors and results are bit-identical to the restatement, ties included.
+ * f32 columns only: bf16 / u8 -> LB2_INVALID_ARG (the reference rejects them, bq/builder.rs:194-210), f16 ->
+ * LB2_UNSUPPORTED; code_dim % 8 != 0 -> LB2_INVALID_ARG; a code_dim whose tables do not fit shared memory, or a
+ * build with more than one rank -> LB2_UNSUPPORTED.
+ * lb2_index_search / _search_refine / _search_ex / _search_async / _search_sharded / _row_mask / _info
+ * (num_sub_vectors 0, num_bits) / _destroy take an IVF_RQ handle; lb2_index_update, _load, _export and
+ * _export_partition reject it with LB2_INVALID_ARG, lb2_index_repartition with LB2_UNSUPPORTED. */
+/* random_orthogonal (bq/builder.rs:309-367): the Q factor of a Householder QR of a standard-normal f64 matrix,
+ * cast to f32; ours is drawn with Philox from `seed` (the reference's rng is unseeded).  rotation_out[code_dim]
+ * [code_dim], row-major. */
+lb2_status lb2_rq_rotation(uint32_t code_dim, uint64_t seed, float* rotation_out);
+/* the batch transform of rows to append (replaces the transformer chain of ivf.rs:281-328): part_out[n],
+ * codes_out[n][code_dim / 8], add_out[n], scale_out[n], valid_out[n] (0: the row is not finite, or zero under
+ * cosine; its outputs are 0).  Any output may be NULL. */
+lb2_status lb2_ivfrq_transform(const void* centroids, uint32_t k, const void* rotation, uint32_t d, uint32_t num_bits,
+                               lb2_dtype dtype, lb2_metric metric, const void* vectors, uint64_t n, uint32_t* part_out,
+                               uint8_t* codes_out, float* add_out, float* scale_out, uint8_t* valid_out);
+/* IvfIndexBuilder<FlatIndex, RabitQuantizer>::build: the IVF stage of lb2_ivfflat_build (same sample, seed and
+ * centroids), the rotation from seed + 1 (timed in stats->ms_pq_train), every kept row transformed
+ * (stats->ms_transform) and grouped by partition. */
+typedef struct {
+  uint32_t num_partitions;
+  lb2_kmeans_params ivf;
+  uint32_t num_bits; /* RQBuildParams (bq/builder.rs:30-45): 1 */
+  uint64_t seed;     /* training sample; the rotation uses seed + 1 */
+} lb2_ivfrq_build_params;
+void lb2_ivfrq_build_params_default(lb2_ivfrq_build_params* p);
+lb2_status lb2_ivfrq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                           const lb2_ivfrq_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                           lb2_build_stats* stats);
+/* An index from a reference-built model: centroids and the `lance:rabit` rotation (code_dim x code_dim) in the model
+ * type of `dtype` (bq/storage.rs:40-60). */
+lb2_status lb2_index_create_rq(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                               const void* rotation, uint32_t num_bits, lb2_index** out);
+/* codes [n][code_dim / 8] row-major (unpacked: unpack_codes, bq/storage.rs:546-600), the __add_factors and
+ * __scale_factors columns, grouped by partition on the device (stable) */
+lb2_status lb2_index_load_rq(lb2_index* index, const uint32_t* part_ids, const uint8_t* codes, const float* add_factors,
+                             const float* scale_factors, const uint64_t* row_ids, uint64_t n);
+/* any pointer may be NULL: rotation [code_dim][code_dim]; part_offsets[k+1]; codes [num_rows][code_dim / 8],
+ * add / scale [num_rows] and row_ids [num_rows] in partition order */
+lb2_status lb2_index_export_rq(const lb2_index* index, void* centroids_out, void* rotation_out,
+                               uint64_t* part_offsets_out, uint8_t* codes_out, float* add_out, float* scale_out,
+                               uint64_t* row_ids_out);
+
 /* ---- multi-GPU (one process per GPU) -----------------------------------------------------------
  * With a communicator every training / build call takes THIS RANK'S ROW SHARD: the k-means loops
  * (flat and hierarchical) exchange their packed per-cluster partial results once per Lloyd iteration

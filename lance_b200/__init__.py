@@ -13,14 +13,15 @@ import numpy as np
 
 from ._lib import (BF16, COSINE, DOT, F16, F32, L2, METRICS, U8, BuildParams, BuildStats, FlatBuildParams,
                    DeviceArray, KMeansParams as _CKMeansParams, LanceB200Error, PinnedArray,
-                   PQParams as _CPQParams, SqBuildParams as _CSqBuildParams, as_ptr, check, device_count, lib)
+                   PQParams as _CPQParams, RqBuildParams as _CRqBuildParams, SqBuildParams as _CSqBuildParams, as_ptr,
+                   check, device_count, lib)
 
 __all__ = ["device_count", "DeviceArray", "PinnedArray", "LanceB200Error", "train_kmeans",
            "compute_partitions", "kmeans_find_partitions", "compute_residual", "normalize_fsl",
            "l2_distance_batch", "dot_distance_batch", "cosine_distance_batch", "PQBuildParams", "ProductQuantizer",
            "build_distance_table_l2", "compute_pq_distance", "flat_topk", "IvfPqIndex",
-           "IvfBuildParams", "IvfFlatIndex", "SQBuildParams", "ScalarQuantizer", "IvfSqIndex", "launch_count",
-           "profile"]
+           "IvfBuildParams", "IvfFlatIndex", "SQBuildParams", "ScalarQuantizer", "IvfSqIndex", "RQBuildParams",
+           "RabitQuantizer", "IvfRqIndex", "launch_count", "profile"]
 
 
 def _metric(m):
@@ -832,3 +833,124 @@ class IvfSqIndex(IvfPqIndex):
                                         C.c_void_p(rid.ctypes.data)))
         return dict(centroids=cent, bounds=(float(bounds[0]), float(bounds[1])), part_offsets=off, codes=codes,
                     row_ids=rid)
+
+
+# ---- lance-index::vector::bq (RaBitQ) -------------------------------------------------------------
+class RQBuildParams:
+    """lance_index::vector::bq::builder::RQBuildParams (bq/builder.rs:30-45)."""
+
+    def __init__(self, num_bits=1):
+        self.num_bits = num_bits
+
+
+class RabitQuantizer:
+    """lance_index::vector::bq::builder::RabitQuantizer: the rotation R [code_dim][code_dim] (code_dim = d * num_bits,
+    of which the first d columns are used) and the transform of rows into sign codes and factors."""
+
+    def __init__(self, dimension, num_bits=1, rotation=None):
+        self.dimension, self.num_bits = dimension, num_bits
+        self.code_dim = dimension * num_bits
+        self.rotation = None if rotation is None else np.ascontiguousarray(rotation, dtype=np.float32)
+
+    def build(self, seed=0):
+        """random_orthogonal (bq/builder.rs:309-367), drawn on the device from `seed` -> rotation."""
+        r = np.empty((self.code_dim, self.code_dim), np.float32)
+        check(lib().lb2_rq_rotation(self.code_dim, seed, C.c_void_p(r.ctypes.data)))
+        self.rotation = r
+        return r
+
+    def transform(self, centroids, vectors, distance_type="l2"):
+        """The IVF_RQ transform of rows (ivf.rs:281-328, bq/transform.rs:70-220) -> dict of part_ids, codes
+        [n][code_dim / 8], add_factors, scale_factors and valid (False: the row was dropped)."""
+        centroids = np.ascontiguousarray(centroids, dtype=np.float32)
+        vectors, dt = _typed(vectors)
+        k, d = centroids.shape
+        n = vectors.shape[0]
+        part, valid = np.empty(n, np.uint32), np.empty(n, np.uint8)
+        codes = np.empty((n, self.code_dim // 8), np.uint8)
+        add, scale = np.empty(n, np.float32), np.empty(n, np.float32)
+        vp, _k = as_ptr(vectors)
+        check(lib().lb2_ivfrq_transform(C.c_void_p(centroids.ctypes.data), C.c_uint32(k),
+                                        C.c_void_p(self.rotation.ctypes.data), C.c_uint32(d),
+                                        C.c_uint32(self.num_bits), C.c_int(dt), C.c_int(_metric(distance_type)), vp,
+                                        C.c_uint64(n), C.c_void_p(part.ctypes.data), C.c_void_p(codes.ctypes.data),
+                                        C.c_void_p(add.ctypes.data), C.c_void_p(scale.ctypes.data),
+                                        C.c_void_p(valid.ctypes.data)))
+        return dict(part_ids=part, codes=codes, add_factors=add, scale_factors=scale, valid=valid.astype(bool))
+
+
+class IvfRqIndex(IvfPqIndex):
+    """Device-resident IVFIndex<FlatIndex, RabitQuantizer> (IVF_RQ): 1-bit codes of rotated residuals, scored from
+    the reference's 4-bit distance tables (lance-index/src/vector/bq/storage.rs:160-445)."""
+
+    @classmethod
+    def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
+              centroids=None, row_ids=None, rq_params=None):
+        """create_index(.., "IVF_RQ"); the IVF stage equals IvfFlatIndex.build's with the same arguments, the
+        rotation is drawn from seed + 1.  f32 columns."""
+        rq_params = rq_params or RQBuildParams()
+        data, dt = _typed(data)
+        n, d = data.shape
+        bp = _CRqBuildParams()
+        lib().lb2_ivfrq_build_params_default(C.byref(bp))
+        bp.num_partitions = num_partitions
+        bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed, bp.seed = max_iters, sample_rate, seed, seed
+        bp.num_bits = rq_params.num_bits
+        keep = None
+        if centroids is not None:
+            keep = _f32(centroids)
+            bp.ivf.init_centroids = as_ptr(keep)[0].value
+        rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
+                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
+        h = C.c_void_p()
+        st = BuildStats()
+        dp, _k1 = as_ptr(data)
+        rp, _k2 = as_ptr(rid)
+        check(lib().lb2_ivfrq_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt), C.c_int(_metric(distance_type)),
+                                    C.byref(bp), rp, C.byref(h), C.byref(st)))
+        ix = cls(h, st)
+        ix._dt = dt
+        return ix
+
+    @classmethod
+    def from_parts(cls, centroids, rotation, part_ids, codes, add_factors, scale_factors, row_ids=None,
+                   distance_type="l2", num_bits=1, dtype=np.float32):
+        """Open a reference-built IVF_RQ index: centroids, the `lance:rabit` rotation [code_dim][code_dim], and the
+        rows (partition ids, unpacked codes [n][code_dim / 8], add / scale factors, row ids)."""
+        dt = _DTYPES[np.dtype(dtype)]
+        centroids = np.ascontiguousarray(centroids, dtype=_model_np(dt))
+        rotation = np.ascontiguousarray(rotation, dtype=_model_np(dt))
+        k, d = centroids.shape
+        h = C.c_void_p()
+        check(lib().lb2_index_create_rq(C.c_void_p(centroids.ctypes.data), C.c_uint32(k), C.c_uint32(d), C.c_int(dt),
+                                        C.c_int(_metric(distance_type)), C.c_void_p(rotation.ctypes.data),
+                                        C.c_uint32(num_bits), C.byref(h)))
+        ix = cls(h)
+        ix._dt = dt
+        part_ids = np.ascontiguousarray(part_ids, dtype=np.uint32)
+        codes = np.ascontiguousarray(codes, dtype=np.uint8)
+        add = np.ascontiguousarray(add_factors, dtype=np.float32)
+        scale = np.ascontiguousarray(scale_factors, dtype=np.float32)
+        rid = None if row_ids is None else np.ascontiguousarray(row_ids, dtype=np.uint64)
+        rp, _k = as_ptr(rid)
+        check(lib().lb2_index_load_rq(h, C.c_void_p(part_ids.ctypes.data), C.c_void_p(codes.ctypes.data),
+                                      C.c_void_p(add.ctypes.data), C.c_void_p(scale.ctypes.data), rp,
+                                      C.c_uint64(part_ids.size)))
+        return ix
+
+    def export(self):
+        i = self.info()
+        K, d, nb, n = i["num_partitions"], i["dimension"], i["num_bits"], i["num_rows"]
+        cd = d * nb
+        cent = np.empty((K, d), np.float32)
+        rot = np.empty((cd, cd), np.float32)
+        off = np.empty(K + 1, np.uint64)
+        codes = np.empty((n, cd // 8), np.uint8)
+        add, scale = np.empty(n, np.float32), np.empty(n, np.float32)
+        rid = np.empty(n, np.uint64)
+        check(lib().lb2_index_export_rq(self._h, C.c_void_p(cent.ctypes.data), C.c_void_p(rot.ctypes.data),
+                                        C.c_void_p(off.ctypes.data), C.c_void_p(codes.ctypes.data),
+                                        C.c_void_p(add.ctypes.data), C.c_void_p(scale.ctypes.data),
+                                        C.c_void_p(rid.ctypes.data)))
+        return dict(centroids=cent, rotation=rot, part_offsets=off, codes=codes, add_factors=add,
+                    scale_factors=scale, row_ids=rid)

@@ -13,6 +13,7 @@
 #include "common.cuh"
 #include "exact.cuh"
 #include "kmeans.cuh"
+#include "rq.cuh"
 #include "search.cuh"
 #include "sq.cuh"
 #include "tc_assign.cuh"
@@ -653,7 +654,7 @@ using namespace lb2;
 
 // the handle
 struct lb2_index {
-  int kind = 0;  // 0 = IVF_PQ, 1 = IVF_FLAT, 2 = IVF_SQ
+  int kind = 0;  // 0 = IVF_PQ, 1 = IVF_FLAT, 2 = IVF_SQ, 3 = IVF_RQ
   lb2_dtype dtype = LB2_F32;  // element type of the vectors / queries the caller passes
   // IVF_FLAT: the (normalised for cosine) vectors in partition order, in the vectors' own element type
   // (f32 / f16 / bf16; u8 columns are held as f32, the reference's model type for them, ivf.rs:1917-1929)
@@ -671,8 +672,13 @@ struct lb2_index {
   // IVF_SQ: `codes` are the 8-bit scalar codes [n][d] of the (normalised for cosine) vectors, under the bounds
   // [sq_lower, sq_upper] (sq/storage.rs:38-45)
   double sq_lower = 0.0, sq_upper = 0.0;
-  // bytes per row of `codes` (PQ: pq.rs:168-173; SQ: one per dimension)
-  int code_bytes() const { return kind == 2 ? d : (nbits == 4 ? M / 2 : M); }
+  // IVF_RQ: `codes` are the sign codes [n][code_dim / 8] of the rotated residuals (num_bits = nbits, code_dim =
+  // d * nbits), with the per-row factors rq_add / rq_scale [n] and the rotation rq_rot [code_dim][code_dim]
+  // (bq/storage.rs:110-121)
+  DevBuf<float> rq_rot, rq_add, rq_scale;
+  int code_dim() const { return d * nbits; }
+  // bytes per row of `codes` (PQ: pq.rs:168-173; SQ: one per dimension; RQ: one bit per code dimension)
+  int code_bytes() const { return kind == 3 ? code_dim() / 8 : kind == 2 ? d : (nbits == 4 ? M / 2 : M); }
   size_t codebook_len() const { return ((size_t)1 << nbits) * d; }
 };
 
@@ -709,8 +715,16 @@ static uint64_t member_sort_index(MemberSort& ms, lb2_index* ix, const uint32_t*
   return kept;
 }
 
+__global__ void gather_f32_kernel(const uint32_t* __restrict__ members, uint64_t n, const float* __restrict__ src,
+                                  float* __restrict__ dst) {
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < n) dst[g] = src[members[g]];
+}
+
+// rq_add / rq_scale (IVF_RQ only): the rows' factors, grouped with their codes
 static void index_load_dev(lb2_index* ix, const uint32_t* part_ids, const uint8_t* codes,
-                           const uint64_t* row_ids, uint64_t n, const uint8_t* valid = nullptr) {
+                           const uint64_t* row_ids, uint64_t n, const uint8_t* valid = nullptr,
+                           const float* rq_add = nullptr, const float* rq_scale = nullptr) {
   MemberSort ms;
   const uint64_t kept = member_sort_index(ms, ix, part_ids, valid, n);
   ix->codes.alloc(std::max<uint64_t>(1, kept * ix->code_bytes()));
@@ -718,6 +732,15 @@ static void index_load_dev(lb2_index* ix, const uint32_t* part_ids, const uint8_
   if (kept)
     LB2_LAUNCH("group_by_partition", group_kernel, cdiv(kept, 256), 256, 0, ms.members.p, kept, ix->code_bytes(),
                codes, row_ids, ix->codes.p, ix->row_ids.p);
+  if (ix->kind == 3) {
+    ix->rq_add.alloc(std::max<uint64_t>(1, kept));
+    ix->rq_scale.alloc(std::max<uint64_t>(1, kept));
+    if (kept) {
+      LB2_LAUNCH("group_by_partition", gather_f32_kernel, cdiv(kept, 256), 256, 0, ms.members.p, kept, rq_add, ix->rq_add.p);
+      LB2_LAUNCH("group_by_partition", gather_f32_kernel, cdiv(kept, 256), 256, 0, ms.members.p, kept, rq_scale,
+                 ix->rq_scale.p);
+    }
+  }
   ix->n = kept;
   if (kept && skew_layout_applies(ix->M, ix->d, ix->nbits)) {
     ix->slab_off.alloc(ix->K + 1);
@@ -1483,6 +1506,11 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
   if (index->kind == 1) {
     ivfflat_search_f32(index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->vectors.p,
                        (int)index->vdtype(), index->row_ids.p, qp, nq, (int)kc, nprobes, si, sd, sc, flt);
+  } else if (index->kind == 3) {
+    // the (normalised) query's residual to each probed centroid is rotated (v2.rs:316-332, bq/storage.rs:407-445)
+    ivfrq_search_f32(index->centroids.p, index->K, d, index->metric, index->rq_rot.p, index->code_dim(),
+                     index->part_offsets.p, index->codes.p, index->rq_add.p, index->rq_scale.p, index->row_ids.p, qp,
+                     nq, (int)kc, nprobes, si, sd, sc, flt);
   } else if (index->kind == 2) {
     // the (normalised) query is encoded with the index's bounds, not turned into a residual (sq/storage.rs:404-430)
     qcodes.alloc(std::max<uint64_t>(1, nq * d));
@@ -1651,6 +1679,7 @@ __global__ void repart_unpack_kernel(const uint64_t* __restrict__ seg_prefix /*[
 lb2_status lb2_index_repartition(const lb2_index* shard, lb2_index** owned_out) {
   LB2_API_BEGIN
   LB2_REQUIRE(shard && owned_out, "null argument");
+  if (shard->kind == 3) fail(LB2_UNSUPPORTED, "lb2_index_repartition: IVF_RQ indexes are not implemented");
   Comm* cm = current_comm();
   const int G = cm ? cm->nranks : 1, me = cm ? cm->rank : 0;
   const int K = shard->K;
@@ -2082,7 +2111,7 @@ static void train_ivf_stage(Source& src, lb2_index* ix, const lb2_kmeans_params&
 // sees it: normalised under cosine (NormalizeTransformer first, ivf.rs:158-166)
 static const float* assign_flat_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
                                       const float* cent, int K, DevBuf<float>& normbuf, uint32_t* part,
-                                      uint8_t* valid) {
+                                      uint8_t* valid, float* dist = nullptr) {
   const int am = m == METRIC_DOT ? METRIC_DOT : METRIC_L2;
   const float* xp = xf;
   if (m == METRIC_COSINE) {
@@ -2091,7 +2120,7 @@ static const float* assign_flat_chunk(const float* xf, const void* xnat, int dty
     xp = normbuf.p;
     xnat = nullptr;
   }
-  assign_f32(xp, rows, d, cent, K, am, nullptr, part, nullptr, valid, nullptr, xnat, dtype);
+  assign_f32(xp, rows, d, cent, K, am, nullptr, part, dist, valid, nullptr, xnat, dtype);
   return xp;
 }
 
@@ -2301,6 +2330,224 @@ lb2_status lb2_ivfsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
     stats->ivf_loss = loss.empty() ? 0.0 : loss[0];
   }
   *out = ix.release();
+  LB2_API_END
+}
+
+// ---- IVF_RQ: IVFIndex<FlatIndex, RabitQuantizer> (lance-index/src/vector/bq/*.rs) ---------------------------------
+static void rq_check(uint32_t d, lb2_dtype dtype, uint32_t num_bits) {
+  // RabitQuantizer::build takes f16 / f32 / f64 columns only (bq/builder.rs:194-210)
+  if (dtype == LB2_BF16 || dtype == LB2_U8) fail(LB2_INVALID_ARG, "IVF_RQ: unsupported data type %d", (int)dtype);
+  if (dtype != LB2_F32)
+    fail(LB2_UNSUPPORTED, "IVF_RQ: f16 columns are not implemented (the reference rotates them in f16)");
+  LB2_REQUIRE(d > 0 && num_bits > 0, "IVF_RQ: the dimension and num_bits must be positive");
+  const uint64_t cd = (uint64_t)d * num_bits;
+  LB2_REQUIRE(cd % 8 == 0, "IVF_RQ: code_dim = d * num_bits = %llu is not a multiple of 8", (unsigned long long)cd);
+  if (cd > 65536 || !rq_scan_fits((int)cd, 1))
+    fail(LB2_UNSUPPORTED, "IVF_RQ: the tables of code_dim %llu do not fit the scan's shared memory",
+         (unsigned long long)cd);
+}
+
+// IVF_RQ transform of one chunk (IvfTransformer::with_rq, ivf.rs:281-328): [normalise] -> partition and dist_v_c ->
+// residual -> rotation -> sign codes and factors.  Cosine is L2 on the normalised rows from there on.
+struct RqWork {
+  DevBuf<float> normbuf, dist, res, rot;
+};
+static void rq_transform_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
+                               const float* cent, int K, const float* rotation, int num_bits, const float* cnorm,
+                               RqWork& w, uint32_t* part, uint8_t* valid, uint8_t* codes, float* add, float* scale) {
+  const int cd = d * num_bits;
+  if (w.dist.n < rows) w.dist.alloc(rows);
+  if (w.res.n < rows * d) w.res.alloc(rows * d);
+  if (w.rot.n < rows * cd) w.rot.alloc(rows * cd);
+  const float* xs = assign_flat_chunk(xf, xnat, dtype, rows, d, m, cent, K, w.normbuf, part, valid, w.dist.p);
+  rq_residual_f32(xs, rows, d, cent, part, valid, w.res.p);
+  rq_rotate_f32(rotation, cd, d, w.res.p, rows, w.rot.p);
+  rq_encode_f32(w.rot.p, w.res.p, w.dist.p, part, cnorm, valid, rows, d, num_bits,
+                m == METRIC_DOT ? METRIC_DOT : METRIC_L2, codes, add, scale);
+}
+
+// |c|^2 per centroid (norm_squared_fsl, RQTransformer::new, bq/transform.rs:42-59): dot only
+static void rq_centroid_norms(int metric, const float* cent, int K, int d, DevBuf<float>& out) {
+  if (metric != METRIC_DOT) return;
+  out.alloc(K);
+  rq_norm_sq_f32(cent, K, d, out.p);
+}
+
+lb2_status lb2_rq_rotation(uint32_t code_dim, uint64_t seed, float* rotation_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(rotation_out && code_dim > 0 && code_dim <= 65536, "bad argument");
+  ctx();
+  OutArg<float> o(rotation_out, (size_t)code_dim * code_dim);
+  rq_rotation_f32((int)code_dim, seed, o.get());
+  o.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_ivfrq_transform(const void* centroids, uint32_t k, const void* rotation, uint32_t d, uint32_t num_bits,
+                               lb2_dtype dtype, lb2_metric metric, const void* vectors, uint64_t n, uint32_t* part_out,
+                               uint8_t* codes_out, float* add_out, float* scale_out, uint8_t* valid_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(centroids && rotation && (vectors || n == 0) && k > 0, "null argument");
+  rq_check(d, dtype, num_bits);
+  const int m = metric_of(metric);
+  const uint64_t cd = (uint64_t)d * num_bits;
+  VecIn c(centroids, (size_t)k * d, dtype), r(rotation, cd * cd, dtype);
+  DevBuf<float> cnorm;
+  rq_centroid_norms(m, c.get(), (int)k, (int)d, cnorm);
+  OutArg<uint32_t> p(part_out, n);
+  OutArg<uint8_t> co(codes_out, (size_t)(n * cd / 8)), v(valid_out, n);
+  OutArg<float> ao(add_out, n), so(scale_out, n);
+  DevBuf<uint32_t> ptmp;
+  DevBuf<uint8_t> vtmp, ctmp;
+  DevBuf<float> atmp, stmp;
+  uint32_t* pp = p.get();
+  uint8_t *vp = v.get(), *cp = co.get();
+  float *ap = ao.get(), *sp = so.get();
+  if (!pp) { ptmp.alloc(std::max<uint64_t>(n, 1)); pp = ptmp.p; }
+  if (!vp) { vtmp.alloc(std::max<uint64_t>(n, 1)); vp = vtmp.p; }
+  if (!cp) { ctmp.alloc(std::max<uint64_t>(n * cd / 8, 1)); cp = ctmp.p; }
+  if (!ap) { atmp.alloc(std::max<uint64_t>(n, 1)); ap = atmp.p; }
+  if (!sp) { stmp.alloc(std::max<uint64_t>(n, 1)); sp = stmp.p; }
+  if (n) {
+    Source src(vectors, n, (int)d, dtype);
+    src.start_resident_copy();
+    RqWork w;
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      rq_transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, c.get(), (int)k, r.get(),
+                         (int)num_bits, cnorm.p, w, pp + r0, vp + r0, cp + r0 * (cd / 8), ap + r0, sp + r0);
+    });
+  }
+  p.commit(); co.commit(); v.commit(); ao.commit(); so.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+void lb2_ivfrq_build_params_default(lb2_ivfrq_build_params* p) {
+  p->num_partitions = 256;
+  lb2_kmeans_params_default(&p->ivf);
+  p->ivf.balance_factor = 1.0f;
+  p->num_bits = 1;
+  p->seed = 0;
+}
+
+lb2_status lb2_ivfrq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                           const lb2_ivfrq_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                           lb2_build_stats* stats) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(data && params && out, "null argument");
+  rq_check(d, dtype, params->num_bits);
+  if (current_comm() && current_comm()->nranks > 1)
+    fail(LB2_UNSUPPORTED, "IVF_RQ: builds sharded over ranks are not implemented");
+  const int m = metric_of(metric);
+  const int K = params->num_partitions;
+  LB2_REQUIRE(K > 0 && n >= (uint64_t)K, "KMeans: can not train %d centroids with %llu vectors", K, (unsigned long long)n);
+  EventSet ev(5);
+  ev.record(0);
+  Source src(data, n, (int)d, dtype);
+  std::unique_ptr<lb2_index> ix(new lb2_index());
+  ix->kind = 3; ix->K = K; ix->d = d; ix->M = 0; ix->nbits = (int)params->num_bits; ix->metric = m; ix->dtype = dtype;
+  ix->centroids.alloc((size_t)K * d);
+  const int cd = ix->code_dim();
+  std::vector<double> loss;
+  std::vector<uint32_t> iters;
+  // 1. IVF: the same stage as lb2_ivfflat_build (same sample, seed, training)
+  train_ivf_stage(src, ix.get(), params->ivf, params->seed, 1, &loss, &iters);
+  ev.record(1);
+  // 2. RabitQuantizer::new (bq/builder.rs:52-70): the rotation, from seed + 1
+  {
+    TagScope tg("rq_train");
+    ix->rq_rot.alloc((size_t)cd * cd);
+    rq_rotation_f32(cd, params->seed + 1, ix->rq_rot.p);
+  }
+  ev.record(2);
+  // 3. transform (ivf.rs:281-328) of every row
+  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
+  DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1)), codes(std::max<uint64_t>(1, n * (cd / 8)));
+  DevBuf<float> add(std::max<uint64_t>(n, 1)), scale(std::max<uint64_t>(n, 1)), cnorm;
+  {
+    TagScope tg("transform");
+    rq_centroid_norms(m, ix->centroids.p, K, (int)d, cnorm);
+    RqWork w;
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      rq_transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, ix->rq_rot.p, ix->nbits,
+                         cnorm.p, w, part.p + r0, valid.p + r0, codes.p + r0 * (cd / 8), add.p + r0, scale.p + r0);
+    });
+  }
+  ev.record(3);
+  {
+    TagScope tg("group");
+    InArg<uint64_t> rid(row_ids, n);
+    index_load_dev(ix.get(), part.p, codes.p, rid.get(), n, valid.p, add.p, scale.p);
+  }
+  ev.record(4);
+  sync_stream();
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->ms_ivf_train = ev.ms(0, 1);
+    stats->ms_pq_train = ev.ms(1, 2);
+    stats->ms_transform = ev.ms(2, 3);
+    stats->ms_group = ev.ms(3, 4);
+    stats->ms_total = ev.ms(0, 4);
+    stats->ivf_iters = iters.empty() ? 0 : iters[0];
+    stats->ivf_loss = loss.empty() ? 0.0 : loss[0];
+  }
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_index_create_rq(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                               const void* rotation, uint32_t num_bits, lb2_index** out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(out && centroids && rotation, "null argument");
+  rq_check(d, dtype, num_bits);
+  std::unique_ptr<lb2_index> ix(index_with_centroids(3, centroids, k, d, dtype, metric));
+  ix->nbits = (int)num_bits;
+  const size_t cd = ix->code_dim();
+  ix->rq_rot.alloc(cd * cd);
+  VecIn r(rotation, cd * cd, dtype);
+  d2d(ix->rq_rot.p, r.get(), cd * cd);
+  ix->rq_add.alloc(1);
+  ix->rq_scale.alloc(1);
+  sync_stream();
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_index_load_rq(lb2_index* index, const uint32_t* part_ids, const uint8_t* codes, const float* add_factors,
+                             const float* scale_factors, const uint64_t* row_ids, uint64_t n) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == 3, "not an IVF_RQ index");
+  LB2_REQUIRE(n == 0 || (part_ids && codes && add_factors && scale_factors), "null argument");
+  InArg<uint32_t> p(part_ids, n);
+  InArg<uint8_t> c(codes, (size_t)n * index->code_bytes());
+  InArg<float> a(add_factors, n), s(scale_factors, n);
+  InArg<uint64_t> r(row_ids, n);
+  check_part_ids(p.get(), n, (uint32_t)index->K, "index_load_rq");
+  index_load_dev(index, p.get(), c.get(), r.get(), n, nullptr, a.get(), s.get());
+  LB2_API_END
+}
+
+lb2_status lb2_index_export_rq(const lb2_index* index, void* centroids_out, void* rotation_out,
+                               uint64_t* part_offsets_out, uint8_t* codes_out, float* add_out, float* scale_out,
+                               uint64_t* row_ids_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == 3, "not an IVF_RQ index");
+  cudaStream_t s = ctx().stream;
+  const size_t cd = index->code_dim(), n = index->n;
+  if (centroids_out)
+    LB2_CUDA(cudaMemcpyAsync(centroids_out, index->centroids.p, sizeof(float) * index->K * index->d, cudaMemcpyDefault, s));
+  if (rotation_out)
+    LB2_CUDA(cudaMemcpyAsync(rotation_out, index->rq_rot.p, sizeof(float) * cd * cd, cudaMemcpyDefault, s));
+  if (part_offsets_out)
+    LB2_CUDA(cudaMemcpyAsync(part_offsets_out, index->part_offsets.p, sizeof(uint64_t) * (index->K + 1), cudaMemcpyDefault, s));
+  if (codes_out && n)
+    LB2_CUDA(cudaMemcpyAsync(codes_out, index->codes.p, n * index->code_bytes(), cudaMemcpyDefault, s));
+  if (add_out && n) LB2_CUDA(cudaMemcpyAsync(add_out, index->rq_add.p, sizeof(float) * n, cudaMemcpyDefault, s));
+  if (scale_out && n) LB2_CUDA(cudaMemcpyAsync(scale_out, index->rq_scale.p, sizeof(float) * n, cudaMemcpyDefault, s));
+  if (row_ids_out && n)
+    LB2_CUDA(cudaMemcpyAsync(row_ids_out, index->row_ids.p, sizeof(uint64_t) * n, cudaMemcpyDefault, s));
+  sync_stream();
   LB2_API_END
 }
 

@@ -21,6 +21,7 @@
 #include "comm.cuh"
 #include "common.cuh"
 #include "exact.cuh"
+#include "rq.cuh"
 #include "search.cuh"
 
 namespace lb2 {
@@ -1359,6 +1360,140 @@ ivfsq_scan_kernel(const uint8_t* __restrict__ qcodes, int d, float r2, const uin
   write_slot(s, cnt, slot, k, off, row_ids, cand_d, cand_id, cand_cnt);
 }
 
+// ------------------------------------------------------------------------------------------------
+// IVF_RQ: RabitDistCalculator (lance-index/src/vector/bq/storage.rs:160-445) + top-k, one CTA per (probe, query).
+// rq = the slot's rotated residual query (dot(R[i, :d], q - c_p), storage.rs:130-156).  In shared memory:
+//   - the code_dim / 4 sub-tables of 16 entries by the lowbit chain t[j] = t[j - lowbit(j)] + rq[4s + ctz(j)]
+//     (storage.rs:210-245), which fixes the rounding order;
+//   - sum_q = the sequential f32 sum of rq from -0.0 (Rust's float Sum);
+//   - the table quantised to u8 with qmin / qmax over the whole table in total_cmp order (storage.rs:249-267).
+// distance_all (storage.rs:319-369): the rows before the partition's last n_p % 32 sum u8 entries in 16-bit lanes
+// that wrap mod 2^16, as the x86 kernels do (dist_table.rs:96-160, dist_table.c) -- an exact u32 sum & 0xffff --
+// and are dequantised as q * ((qmax - qmin) / 255) + (code_dim / 4) * qmin; the last n_p % 32 rows take the exact
+// f32 sum of the pairs t_lo[lo] + t_hi[hi] from 0.0.  With a prefilter every row takes DistCalculator::distance
+// (storage.rs:297-316), the same pair sums from -0.0; no table entry is -0.0 (t[0] = +0.0 and x + y is -0.0 only
+// when both are), so the start does not matter.  Then ((2 dist - sum_q) / sqrt_d) * scale + add + q_factor, each
+// operation rounded on its own.  Codes are row-major [n][code_dim / 8]; the 32-row rule uses the partition-local row.
+// ------------------------------------------------------------------------------------------------
+static size_t rq_scan_smem_bytes(int code_dim, int k) {
+  return (size_t)code_dim * 4 * (sizeof(float) + 1) + slot_smem_bytes(k);
+}
+
+__global__ void __launch_bounds__(256)
+ivfrq_scan_kernel(const float* __restrict__ rq, int code_dim, float sqrt_d, int q_minus_one,
+                  const uint32_t* __restrict__ probe_ids, const float* __restrict__ probe_dists, int np,
+                  const uint64_t* __restrict__ part_offsets, const uint8_t* __restrict__ codes,
+                  const float* __restrict__ add, const float* __restrict__ scale, const uint64_t* __restrict__ row_ids,
+                  int k, float* __restrict__ cand_d, uint64_t* __restrict__ cand_id, uint32_t* __restrict__ cand_cnt,
+                  const ScanFilter flt) {
+  extern __shared__ float rq_smem[];
+  const int nt = code_dim >> 2;  // sub-tables of 16 entries
+  float* tab = rq_smem;                                      // [nt * 16] f32
+  uint8_t* qt = reinterpret_cast<uint8_t*>(tab + nt * 16);  // [nt * 16] u8 (code_dim % 8 == 0: 4-byte aligned end)
+  const SlotSmem s(qt + nt * 16, k + 1);
+  __shared__ int32_t s_mn, s_mx;
+  __shared__ float s_sum_q;
+  const int tid = threadIdx.x;
+  const int pi = blockIdx.x;
+  const size_t qi = blockIdx.y;
+  const size_t slot = qi * np + pi;
+  const uint32_t p = probe_ids[slot];
+  const uint64_t off = part_offsets[p];
+  const uint32_t n_p = (uint32_t)(part_offsets[p + 1] - off);
+  if (n_p == 0) {
+    if (tid == 0) cand_cnt[slot] = 0;
+    return;
+  }
+  const float* r = rq + slot * (size_t)code_dim;
+  if (tid == 0) { s_mn = 0x7fffffff; s_mx = (int32_t)0x80000000; }
+  for (int st = tid; st < nt; st += 256) {
+    float t[16];
+    t[0] = 0.0f;
+#pragma unroll
+    for (int j = 1; j < 16; ++j) {
+      const int ctz = (j & 1) ? 0 : (j & 2) ? 1 : (j & 4) ? 2 : 3;
+      t[j] = __fadd_rn(t[j - (j & -j)], r[4 * st + ctz]);
+    }
+#pragma unroll
+    for (int j = 0; j < 16; ++j) tab[st * 16 + j] = t[j];
+  }
+  __syncthreads();
+  int32_t mn = 0x7fffffff, mx = (int32_t)0x80000000;
+  for (int i = tid; i < nt * 16; i += 256) {
+    const int32_t kv = total_order_key(tab[i]);
+    mn = min(mn, kv);
+    mx = max(mx, kv);
+  }
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) {
+    mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  }
+  if ((tid & 31) == 0) { atomicMin(&s_mn, mn); atomicMax(&s_mx, mx); }
+  if (tid == 0) {
+    float sq = -0.0f;
+    for (int i = 0; i < code_dim; ++i) sq = __fadd_rn(sq, r[i]);
+    s_sum_q = sq;
+  }
+  __syncthreads();
+  const float qmin = key_to_float(s_mn), qmax = key_to_float(s_mx);
+  if (flt.allow == nullptr) {
+    const bool flat = qmin == qmax;  // e.g. a zero residual query: all codes 0
+    const float factor = flat ? 0.0f : __fdiv_rn(255.0f, __fsub_rn(qmax, qmin));
+    for (int i = tid; i < nt * 16; i += 256) {
+      const float v = flat ? 0.0f : roundf(__fmul_rn(__fsub_rn(tab[i], qmin), factor));  // f32::round
+      qt[i] = (v != v) ? 0 : v <= 0.0f ? 0 : v >= 255.0f ? 255 : (uint8_t)v;           // `as u8`
+    }
+  }
+  __syncthreads();
+  const float range = __fdiv_rn(__fsub_rn(qmax, qmin), 255.0f), sum_min = __fmul_rn((float)nt, qmin);
+  const float sum_q = s_sum_q, dqc = probe_dists[slot];
+  const float q_factor = q_minus_one ? __fsub_rn(dqc, 1.0f) : dqc;  // storage.rs:427-434
+  const int cb = code_dim >> 3;
+  const uint8_t* pc = codes + off * cb;
+  const uint32_t n_quant = flt.allow ? 0u : n_p - n_p % 32;
+  auto fill = [&](uint32_t c0, uint32_t clen) {
+    for (uint32_t j = tid; j < clen; j += 256) {
+      const uint32_t row = c0 + j;
+      const uint8_t* rp = pc + (size_t)row * cb;
+      float dist;
+      if (row < n_quant) {
+        uint32_t qs = 0;
+        for (int i = 0; i < cb; ++i) {
+          const uint32_t c = __ldg(rp + i);
+          qs += (uint32_t)qt[(2 * i) * 16 + (c & 15)] + (uint32_t)qt[(2 * i + 1) * 16 + (c >> 4)];
+        }
+        dist = __fadd_rn(__fmul_rn(__uint2float_rn(qs & 0xffffu), range), sum_min);
+      } else {
+        dist = 0.0f;
+        for (int i = 0; i < cb; ++i) {
+          const uint32_t c = __ldg(rp + i);
+          dist = __fadd_rn(dist, __fadd_rn(tab[(2 * i) * 16 + (c & 15)], tab[(2 * i + 1) * 16 + (c >> 4)]));
+        }
+      }
+      const float dvq = __fdiv_rn(__fsub_rn(__fmul_rn(2.0f, dist), sum_q), sqrt_d);
+      float out = __fadd_rn(__fadd_rn(__fmul_rn(dvq, scale[off + row]), add[off + row]), q_factor);
+      // x86's default NaN (0xFFC00000, ordered before every number): with finite rows a NaN only comes from invalid
+      // operations, e.g. on a normalised zero query under cosine, and the reference runs on x86
+      if (out != out) out = __int_as_float(0xffc00000);
+      s.ukey[j] = (uint32_t)total_order_key(out) ^ 0x80000000u;
+    }
+  };
+  const uint32_t cnt = slot_topk(s, n_p, k, flt, off, false, fill);
+  write_slot(s, cnt, slot, k, off, row_ids, cand_d, cand_id, cand_cnt);
+}
+
+// residual queries of `nq` queries x np probes: out[(q np + pi) d + t] = queries[q d + t] - c_{probe}[t]
+__global__ void rq_query_residual_kernel(const float* __restrict__ queries, uint64_t nq, int np, int d,
+                                         const float* __restrict__ centroids, const uint32_t* __restrict__ probe_ids,
+                                         float* __restrict__ out) {
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= nq * np * d) return;
+  const uint64_t sl = g / d;
+  const int t = (int)(g % d);
+  out[g] = __fsub_rn(queries[(sl / np) * d + t], centroids[(size_t)probe_ids[sl] * d + t]);
+}
+
 // global merge per query: ascending (distance, row id), first k.  Candidate e of list pi of query qi sits
 // at cand[pi * stride_p + qi * stride_q + e] (per-partition lists of one GPU: stride_p = k, stride_q = np * k;
 // per-rank results gathered from a sharded index: stride_p = the rank stride, stride_q = k).
@@ -1586,8 +1721,9 @@ static void merge_lists(const char* name, uint64_t nq, const float* cand_d, cons
 }
 
 // The IVF query skeleton: the nprobes nearest partitions of every query, one candidate list of <= k per (query,
-// probe) slot, the lists merged per query.  scan(q0, qn, probe_ids, cand_d, cand_id, cand_cnt) fills the lists of
-// queries [q0, q0 + qn) (at most 32768 of them: the grid.y limit).
+// probe) slot, the lists merged per query.  scan(q0, qn, probe_ids, probe_dists, cand_d, cand_id, cand_cnt) fills the
+// lists of queries [q0, q0 + qn) (at most 32768 of them: the grid.y limit); probe_dists are find_partitions'
+// distances of the probed centroids (dist_q_c).
 constexpr uint64_t SEARCH_SLAB = 32768;
 template <class Scan>
 static void ivf_search(const float* centroids, int K, int d, int metric, const float* queries, uint64_t nq, int k,
@@ -1599,7 +1735,7 @@ static void ivf_search(const float* centroids, int K, int d, int metric, const f
   DevBuf<uint64_t> cand_id((size_t)nq * np * k);
   find_partitions_f32(centroids, K, d, cmetric, queries, nq, np, pids.p, pd.p);
   for (uint64_t q0 = 0; q0 < nq; q0 += SEARCH_SLAB)
-    scan(q0, std::min<uint64_t>(SEARCH_SLAB, nq - q0), pids.p + q0 * np, cand_d.p + q0 * np * k,
+    scan(q0, std::min<uint64_t>(SEARCH_SLAB, nq - q0), pids.p + q0 * np, pd.p + q0 * np, cand_d.p + q0 * np * k,
          cand_id.p + q0 * np * k, cand_cnt.p + q0 * np);
   merge_lists("merge_topk", nq, cand_d.p, cand_id.p, cand_cnt.p, np, k, (size_t)k, (size_t)k, (size_t)np * k, (size_t)1,
               (size_t)np, out_ids, out_dists, out_counts);
@@ -1662,7 +1798,7 @@ void ivfpq_search_f32(const float* centroids, int K, int d, int metric, const fl
   if (need > ctx().smem_optin) fail(LB2_UNSUPPORTED, "LUT and top-k scratch of %zu bytes exceed shared memory", need);
   DevBuf<uint32_t> rlist((size_t)std::min<uint64_t>(nq, SEARCH_SLAB) * np), rcount(1);
   ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
-             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, float* cd, uint64_t* cid, uint32_t* ccnt) {
+             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, const float*, float* cd, uint64_t* cid, uint32_t* ccnt) {
                const ScanArgs a{queries + q0 * d, d, centroids, codebook, M, d / M, pids, np, part_offsets, codes,
                                 row_ids, k, cd, cid, ccnt, flt};
                const dim3 g(np, (unsigned)qn);
@@ -1738,7 +1874,7 @@ void ivfflat_search_f32(const float* centroids, int K, int d, int metric, const 
   if (need > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the flat scan", d);
   const int np = nprobes < K ? nprobes : K;
   ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
-             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, float* cd, uint64_t* cid, uint32_t* ccnt) {
+             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, const float*, float* cd, uint64_t* cid, uint32_t* ccnt) {
                dispatch_metric_elem<false>(metric, vdt, [&](auto m, auto e) {
                  using T = typename decltype(e)::type;
                  auto kern = ivfflat_scan_kernel<decltype(m)::value, T>;
@@ -1769,12 +1905,48 @@ void ivfsq_search_f32(const float* centroids, int K, int d, int metric, const ui
   if (need > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the SQ scan", d);
   const int np = nprobes < K ? nprobes : K;
   ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
-             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, float* cd, uint64_t* cid, uint32_t* ccnt) {
+             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, const float*, float* cd, uint64_t* cid, uint32_t* ccnt) {
                with_kernel([&](auto kern) {
                  set_smem(kern, smem);
                  LB2_LAUNCH("sq_scan", kern, dim3(np, (unsigned)qn), 256, smem, qcodes + q0 * d, d, r2, pids, np,
                             part_offsets, codes, row_ids, k, cd, cid, ccnt, flt);
                });
+             });
+}
+
+bool rq_scan_fits(int code_dim, int k) {
+  return smem_with_static(ivfrq_scan_kernel, rq_scan_smem_bytes(code_dim, k)) <= ctx().smem_optin;
+}
+
+void ivfrq_search_f32(const float* centroids, int K, int d, int metric, const float* rotation, int code_dim,
+                      const uint64_t* part_offsets, const uint8_t* codes, const float* add, const float* scale,
+                      const uint64_t* row_ids, const float* queries, uint64_t nq, int k, int nprobes,
+                      uint64_t* out_ids, float* out_dists, uint32_t* out_counts, const ScanFilter& flt) {
+  if (nq == 0 || k == 0) return;
+  if (k > 1024) fail(LB2_UNSUPPORTED, "k (incl. refine factor) > 1024 is not implemented");
+  if (!rq_scan_fits(code_dim, k))
+    fail(LB2_UNSUPPORTED, "IVF_RQ: the tables of code_dim %d do not fit the scan's shared memory", code_dim);
+  const size_t smem = rq_scan_smem_bytes(code_dim, k);
+  const int np = nprobes < K ? nprobes : K;
+  const float sqrt_d = sqrtf((float)code_dim);  // (dim as f32 * num_bits as f32).sqrt(): the product is exact
+  const int q_minus_one = metric != METRIC_L2;    // the storage's metric: cosine / dot -> dist_q_c - 1.0
+  ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
+             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, const float* pdists, float* cd, uint64_t* cid,
+                 uint32_t* ccnt) {
+               // the (query, probe) residuals are rotated in groups of queries that keep both buffers near 256 MB
+               const uint64_t per_q = (uint64_t)np * (d + code_dim) * sizeof(float);
+               const uint64_t qc = std::max<uint64_t>(1, std::min<uint64_t>(qn, (256ull << 20) / per_q));
+               DevBuf<float> res(qc * np * d), rot(qc * np * code_dim);
+               set_smem(ivfrq_scan_kernel, smem);
+               for (uint64_t a = 0; a < qn; a += qc) {
+                 const uint64_t b = std::min(qc, qn - a);
+                 LB2_LAUNCH("rq_query_residual", rq_query_residual_kernel, cdiv(b * np * d, 256), 256, 0,
+                            queries + (q0 + a) * d, b, np, d, centroids, pids + a * np, res.p);
+                 rq_rotate_f32(rotation, code_dim, d, res.p, b * np, rot.p);
+                 LB2_LAUNCH("rq_scan", ivfrq_scan_kernel, dim3(np, (unsigned)b), 256, smem, rot.p, code_dim, sqrt_d,
+                            q_minus_one, pids + a * np, pdists + a * np, np, part_offsets, codes, add, scale, row_ids,
+                            k, cd + a * np * k, cid + a * np * k, ccnt + a * np, flt);
+               }
              });
 }
 

@@ -41,6 +41,13 @@ void ivfsq_search_f32(const float* centroids, int K, int d, int metric, const ui
                       const uint8_t* codes, const uint64_t* row_ids, float r2, const float* queries,
                       const uint8_t* qcodes, uint64_t nq, int k, int nprobes, uint64_t* out_ids, float* out_dists,
                       uint32_t* out_counts, const ScanFilter& flt = ScanFilter());
+// IVF_RQ: rotation [code_dim][code_dim]; codes [n][code_dim / 8] and the add / scale factors [n] in partition order;
+// queries: f32 (normalised for cosine).  rq_scan_fits: the scan's tables and a k-slot fit shared memory.
+bool rq_scan_fits(int code_dim, int k);
+void ivfrq_search_f32(const float* centroids, int K, int d, int metric, const float* rotation, int code_dim,
+                      const uint64_t* part_offsets, const uint8_t* codes, const float* add, const float* scale,
+                      const uint64_t* row_ids, const float* queries, uint64_t nq, int k, int nprobes,
+                      uint64_t* out_ids, float* out_dists, uint32_t* out_counts, const ScanFilter& flt = ScanFilter());
 // all ranks' [nq][k] results of a row-sharded index -> the global top-k by (distance, row id) on every rank
 void merge_sharded_topk(const uint64_t* ids, const float* dists, const uint32_t* counts, uint64_t nq, int k,
                         uint64_t* out_ids, float* out_dists, uint32_t* out_counts);
