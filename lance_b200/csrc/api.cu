@@ -182,6 +182,17 @@ __global__ void finite_rows_kernel(const float* __restrict__ x, uint64_t n, int 
   if (lane == 0) flag[w] = ok ? 1 : 0;
 }
 
+// valid[w] = 0 for a row with a non-finite element (KeepFiniteVectors, transform.rs:86-150); warp per row
+__global__ void drop_nonfinite_rows_kernel(const float* __restrict__ x, uint64_t n, int d, uint8_t* __restrict__ valid) {
+  const uint64_t w = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (w >= n) return;
+  bool ok = true;
+  for (int e = lane; e < d; e += 32) ok &= isfinite(x[w * d + e]);
+  ok = __all_sync(0xffffffffu, ok);
+  if (lane == 0 && !ok) valid[w] = 0;
+}
+
 // l2_distance_uint_scalar (lance-linalg/src/distance/l2.rs:44-49, impl L2 for u8 :93-98): sum of |x - y|^2 in
 // u32 (wrapping, like Rust's release-mode `sum::<u32>()`), then `as f32` (round to nearest even); warp per row
 __global__ void l2_u8_kernel(const uint8_t* __restrict__ from, const uint8_t* __restrict__ to, uint64_t n, int d,
@@ -2107,8 +2118,11 @@ static void train_ivf_stage(Source& src, lb2_index* ix, const lb2_kmeans_params&
   round_model(ix->centroids.p, (size_t)K * d, ix->dtype);
 }
 
-// partition assignment of one chunk of rows (IVF_FLAT / IVF_SQ transform); returns the chunk as f32 as the index
-// sees it: normalised under cosine (NormalizeTransformer first, ivf.rs:158-166)
+// partition assignment of one chunk of rows (IVF_FLAT / IVF_SQ / IVF_RQ transform); returns the chunk as f32 as the
+// index sees it: normalised under cosine (NormalizeTransformer first, ivf.rs:158-166).  Rows with a non-finite
+// element are dropped in every metric (KeepFiniteVectors precedes the partition transform, ivf.rs:166, 256,
+// 299).  Under L2 and cosine such a row has no finite distance and the assignment already drops it;
+// under dot a +-inf element can still give a -inf best distance, so the elements are checked.
 static const float* assign_flat_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
                                       const float* cent, int K, DevBuf<float>& normbuf, uint32_t* part,
                                       uint8_t* valid, float* dist = nullptr) {
@@ -2121,6 +2135,8 @@ static const float* assign_flat_chunk(const float* xf, const void* xnat, int dty
     xnat = nullptr;
   }
   assign_f32(xp, rows, d, cent, K, am, nullptr, part, dist, valid, nullptr, xnat, dtype);
+  if (am == METRIC_DOT && rows)
+    LB2_LAUNCH("drop_nonfinite_rows", drop_nonfinite_rows_kernel, cdiv(rows * 32, 256), 256, 0, xp, rows, d, valid);
   return xp;
 }
 
@@ -2349,6 +2365,8 @@ static void rq_check(uint32_t d, lb2_dtype dtype, uint32_t num_bits) {
 
 // IVF_RQ transform of one chunk (IvfTransformer::with_rq, ivf.rs:281-328): [normalise] -> partition and dist_v_c ->
 // residual -> rotation -> sign codes and factors.  Cosine is L2 on the normalised rows from there on.
+// The row chunk is bounded by d (Source::rows_per_chunk), the rotated rows by code_dim = d * num_bits: they are
+// rotated and encoded in sub-chunks of at most 2^28 / code_dim rows (1 GB of f32).
 struct RqWork {
   DevBuf<float> normbuf, dist, res, rot;
 };
@@ -2356,14 +2374,18 @@ static void rq_transform_chunk(const float* xf, const void* xnat, int dtype, uin
                                const float* cent, int K, const float* rotation, int num_bits, const float* cnorm,
                                RqWork& w, uint32_t* part, uint8_t* valid, uint8_t* codes, float* add, float* scale) {
   const int cd = d * num_bits;
+  const uint64_t sub = std::min<uint64_t>(rows, std::max<uint64_t>(1, (1ull << 28) / (uint64_t)cd));
   if (w.dist.n < rows) w.dist.alloc(rows);
   if (w.res.n < rows * d) w.res.alloc(rows * d);
-  if (w.rot.n < rows * cd) w.rot.alloc(rows * cd);
+  if (w.rot.n < sub * cd) w.rot.alloc(sub * cd);
   const float* xs = assign_flat_chunk(xf, xnat, dtype, rows, d, m, cent, K, w.normbuf, part, valid, w.dist.p);
   rq_residual_f32(xs, rows, d, cent, part, valid, w.res.p);
-  rq_rotate_f32(rotation, cd, d, w.res.p, rows, w.rot.p);
-  rq_encode_f32(w.rot.p, w.res.p, w.dist.p, part, cnorm, valid, rows, d, num_bits,
-                m == METRIC_DOT ? METRIC_DOT : METRIC_L2, codes, add, scale);
+  for (uint64_t r0 = 0; r0 < rows; r0 += sub) {
+    const uint64_t rs = std::min(sub, rows - r0);
+    rq_rotate_f32(rotation, cd, d, w.res.p + r0 * d, rs, w.rot.p);
+    rq_encode_f32(w.rot.p, w.res.p + r0 * d, w.dist.p + r0, part + r0, cnorm, valid + r0, rs, d, num_bits,
+                  m == METRIC_DOT ? METRIC_DOT : METRIC_L2, codes + r0 * (cd / 8), add + r0, scale + r0);
+  }
 }
 
 // |c|^2 per centroid (norm_squared_fsl, RQTransformer::new, bq/transform.rs:42-59): dot only

@@ -131,21 +131,21 @@ def rq_distances(rq, codes, add, scale, q_factor, exact_all=False):
     codes = np.asarray(codes, np.uint8)
     n, cb = codes.shape
     t = dist_table(rq)
-    sum_q = seq_sum(rq[:, None], axis=0, start=-0.0)[0]
+    # the fold from -0.0: -0.0 + a0 == a0, so it equals numpy's accumulate, which adds strictly left to right
+    sum_q = np.add.accumulate(rq, dtype=np.float32)[-1] if rq.size else np.float32(-0.0)
     sqrt_d = np.sqrt(np.float32(rq.size))
     lo, hi = (codes & 15).astype(np.int64), (codes >> 4).astype(np.int64)
     i2 = np.arange(cb)
-    pairs = t[2 * i2, lo] + t[2 * i2 + 1, hi]                       # [n][cb] f32
-    exact = seq_sum(pairs, axis=1, start=-0.0 if exact_all else 0.0)
-    dist = exact
     nq = 0 if exact_all else n - n % 32
+    dist = np.empty(n, np.float32)
+    pairs = t[2 * i2, lo[nq:]] + t[2 * i2 + 1, hi[nq:]]             # [n - nq][cb] f32
+    dist[nq:] = seq_sum(pairs, axis=1, start=-0.0 if exact_all else 0.0)
     if nq:
         qmin, qmax, qt = quantize_table(t)
         qt = qt.astype(np.int64)
         qs = (qt[2 * i2, lo[:nq]] + qt[2 * i2 + 1, hi[:nq]]).sum(axis=1) & 0xFFFF   # u16 lanes that wrap
         rng = (qmax - qmin) / np.float32(255.0)
         sum_min = np.float32(t.shape[0]) * qmin
-        dist = exact.copy()
         dist[:nq] = qs.astype(np.float32) * rng + sum_min
     dvq = (np.float32(2.0) * dist - sum_q) / sqrt_d
     return ((dvq * np.asarray(scale, np.float32)) + np.asarray(add, np.float32)) + np.float32(q_factor)
