@@ -258,6 +258,45 @@ typedef struct {
 lb2_status lb2_index_search_ex(lb2_index* index, const void* queries, uint64_t nq,
                                const lb2_search_params* params, uint64_t* row_ids_out, float* dists_out,
                                uint32_t* counts_out);
+/* Search with a minimum and a maximum number of probes, as ANNIvfSubIndexExec runs a query
+ * (rust/lance/src/io/exec/knn.rs:714-1130).  lb2_index_search_ex is the case minimum == maximum
+ * (Scanner::nprobes, scanner.rs:1103-1111); a plain nearest() query is minimum 1, maximum None
+ * (scanner.rs:1064-1077).  Per query, with kc = k * max(1, refine_factor) and K partitions:
+ *   - P = the L = min(maximum or K, K) nearest partitions, ascending by (distance, id);
+ *   - early pruning (knn.rs:1117-1130): the count of P's distances <= d0 * f (Rust's partition_point),
+ *     f = 0.6 / 7 / 81 for k = 1 / 2..=10 / > 10; min_np = min(max(minimum, pruned), L) (adjust_probes,
+ *     knn.rs:1108-1115);
+ *   - c_p = min(kc, rows of p the allow bitmap and the range admit) (flat/index.rs:97-165);
+ *     found0 = min(k, sum of c over P[0, min_np)) (initial_search, knn.rs:837-882);
+ *   - the search stops there if L <= min_np or found0 >= k;
+ *   - shortcut (knn.rs:746-783): with max_len and mask_ids given and found0 < max_len <= k, the mask ids
+ *     the initial search did not return are added at +inf, and nothing more is searched;
+ *   - late search (knn.rs:714-835): late partition t = P[min_np + t] is searched while
+ *     found0 + sum of c over the late partitions u <= t - late_width is below min(k, max_len if given).
+ *     In the reference how many late partitions run depends on when futures complete; this rule is
+ *     take_while ahead of buffered(late_width) with in-order completion (DESIGN.md section 2).
+ * The result is the top kc by (distance, row id) of the partitions searched and the shortcut rows, then
+ * refine and the range filter as in lb2_index_search_ex (shortcut rows get exact distances there).
+ * nprobes_out[q] (nullable) = partitions searched (the reference's partitions_searched).
+ * The ranking sorts all K centroid distances per query whatever the number of probes.  With a range
+ * bound c_p depends on the distances, so P[0, L) is scanned and cut afterwards: such a search costs
+ * as much as one with nprobes = L.
+ * LB2_INVALID_ARG: sp->nprobes != 0, minimum_nprobes == 0, maximum_nprobes < minimum_nprobes,
+ * late_width == 0, or max_len / mask_ids without sp->allow_bitmap.  LB2_UNSUPPORTED on a thread with a
+ * communicator of more than one rank (each rank's c_p would count only its own shard). */
+typedef struct {
+  uint32_t minimum_nprobes;   /* Query::minimum_nprobes, >= 1 */
+  uint32_t maximum_nprobes;   /* Query::maximum_nprobes; 0 = None (every partition); else >= minimum */
+  uint32_t late_width;        /* partitions the late search keeps in flight, >= 1 (get_num_compute_intensive_cpus()) */
+  uint32_t has_max_len;       /* RowIdMask::max_len() is Some (there is an allow list) */
+  uint64_t max_len;
+  const uint64_t* mask_ids;   /* RowIdMask::iter_ids(), ascending; NULL = not iterable (no shortcut) */
+  uint64_t num_mask_ids;
+} lb2_probe_params;
+lb2_status lb2_index_search_probed(lb2_index* index, const void* queries, uint64_t nq,
+                                   const lb2_search_params* sp /* nprobes must be 0 */,
+                                   const lb2_probe_params* pp, uint64_t* row_ids_out, float* dists_out,
+                                   uint32_t* counts_out, uint32_t* nprobes_out /* nullable, [nq] */);
 /* Incremental update: the device half of optimize_indices / split / join (SURVEY 8f-4).
  * The reference expresses an optimize step as per-partition AssignOp::Add / AssignOp::Remove lists against a new
  * centroid set (rust/lance/src/index/vector/builder.rs:1219-1333 split_partition_impl, :1476-1530

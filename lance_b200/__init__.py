@@ -586,6 +586,44 @@ class IvfPqIndex:
         check(lib().lb2_index_search_ex(self._h, qp, C.c_uint64(nq), C.byref(sp), ip, dp, None))
         return ids, dists
 
+    def search_probed(self, queries, k, minimum_nprobes=1, maximum_nprobes=None, late_width=1, allow_bitmap=None,
+                      mask_ids=None, mask_max_len=None, refine_factor=0, vectors=None, lower_bound=None,
+                      upper_bound=None):
+        """lb2_index_search_probed: a query with minimum / maximum nprobes as ANNIvfSubIndexExec runs it (early
+        pruning, late search, the no-rows shortcut; knn.rs:714-1130).  maximum_nprobes=None probes up to every
+        partition; late_width = the late search's concurrency (get_num_compute_intensive_cpus()).  allow_bitmap as in
+        search_ex; mask_max_len = RowIdMask::max_len(), mask_ids = RowIdMask::iter_ids() (None: not iterable).
+        Returns (ids, dists, counts, nprobes): nprobes[q] = partitions the query searched."""
+        from ._lib import ProbeParams, SearchParams
+        dt = getattr(self, "_dt", F32)
+        npdt = {F32: np.float32, F16: np.float16, U8: np.uint8, BF16: np.uint16}[dt]
+        if not isinstance(queries, (DeviceArray, PinnedArray)):
+            queries = np.ascontiguousarray(queries, dtype=npdt)
+        if vectors is not None and not isinstance(vectors, (DeviceArray, PinnedArray)):
+            vectors = np.ascontiguousarray(vectors, dtype=npdt)
+        nq = queries.shape[0]
+        ids, dists = np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32)
+        counts, nprobes = np.empty(nq, np.uint32), np.empty(nq, np.uint32)
+        if mask_ids is not None and not isinstance(mask_ids, (DeviceArray, PinnedArray)):
+            mask_ids = np.ascontiguousarray(np.sort(np.asarray(mask_ids, dtype=np.uint64)))
+        qp, _k1 = as_ptr(queries)
+        vp, _k0 = as_ptr(vectors)
+        bp, _k4 = as_ptr(None if allow_bitmap is None else (allow_bitmap if isinstance(allow_bitmap, (DeviceArray, PinnedArray)) else np.ascontiguousarray(allow_bitmap, dtype=np.uint64)))
+        mp, _k5 = as_ptr(mask_ids)
+        if mask_ids is not None and mp.value is None:  # an empty numpy array has no buffer address to pass
+            _k5 = np.zeros(1, np.uint64)
+            mp = C.c_void_p(_k5.ctypes.data)
+        sp = SearchParams(k, 0, refine_factor, vp.value if vp is not None else None,
+                          0 if vectors is None else vectors.shape[0], bp.value if bp is not None else None,
+                          int(lower_bound is not None), int(upper_bound is not None),
+                          float(lower_bound or 0.0), float(upper_bound or 0.0))
+        pp = ProbeParams(minimum_nprobes, maximum_nprobes or 0, late_width, int(mask_max_len is not None),
+                         int(mask_max_len or 0), mp.value if mp is not None else None,
+                         0 if mask_ids is None else int(mask_ids.shape[0]))
+        check(lib().lb2_index_search_probed(self._h, qp, C.c_uint64(nq), C.byref(sp), C.byref(pp), as_ptr(ids)[0],
+                                            as_ptr(dists)[0], as_ptr(counts)[0], as_ptr(nprobes)[0]))
+        return ids, dists, counts, nprobes
+
     def search_async(self, queries, out, k=10, nprobes=1, cuda_stream=None, done_event=None, allow_bitmap=None,
                      lower_bound=None, upper_bound=None):
         """lb2_index_search_async: enqueue a search on `cuda_stream` (cudaStream_t handle as int) and return at once.

@@ -1482,8 +1482,8 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
                               uint32_t refine_factor, const void* vectors, uint64_t num_vectors,
                               const uint64_t* allow_bitmap, uint64_t* row_ids_out, float* dists_out,
                               uint32_t* counts_out, int has_lower = 0, float lower = 0.0f, int has_upper = 0,
-                              float upper = 0.0f) {
-  LB2_REQUIRE(index && k > 0 && nprobes > 0, "bad argument");
+                              float upper = 0.0f, ProbeRule* pr = nullptr) {
+  LB2_REQUIRE(index && k > 0 && (nprobes > 0 || pr), "bad argument");
   const bool refine = refine_factor > 0 && vectors != nullptr;
   const uint64_t kc = refine ? (uint64_t)k * refine_factor : k;
   if (kc > 1024) fail(LB2_UNSUPPORTED, "k * refine_factor = %llu > 1024 is not implemented", (unsigned long long)kc);
@@ -1516,23 +1516,23 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
   DevBuf<uint8_t> qcodes;
   if (index->kind == 1) {
     ivfflat_search_f32(index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->vectors.p,
-                       (int)index->vdtype(), index->row_ids.p, qp, nq, (int)kc, nprobes, si, sd, sc, flt);
+                       (int)index->vdtype(), index->row_ids.p, qp, nq, (int)kc, nprobes, si, sd, sc, flt, pr);
   } else if (index->kind == 3) {
     // the (normalised) query's residual to each probed centroid is rotated (v2.rs:316-332, bq/storage.rs:407-445)
     ivfrq_search_f32(index->centroids.p, index->K, d, index->metric, index->rq_rot.p, index->code_dim(),
                      index->part_offsets.p, index->codes.p, index->rq_add.p, index->rq_scale.p, index->row_ids.p, qp,
-                     nq, (int)kc, nprobes, si, sd, sc, flt);
+                     nq, (int)kc, nprobes, si, sd, sc, flt, pr);
   } else if (index->kind == 2) {
     // the (normalised) query is encoded with the index's bounds, not turned into a residual (sq/storage.rs:404-430)
     qcodes.alloc(std::max<uint64_t>(1, nq * d));
     sq_encode_f32(qp, nq * d, index->sq_lower, index->sq_upper, qcodes.p);
     const float rf = (float)(index->sq_upper - index->sq_lower);  // inverse_scalar_dist (sq.rs:279-287)
     ivfsq_search_f32(index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->codes.p,
-                     index->row_ids.p, rf * rf, qp, qcodes.p, nq, (int)kc, nprobes, si, sd, sc, flt);
+                     index->row_ids.p, rf * rf, qp, qcodes.p, nq, (int)kc, nprobes, si, sd, sc, flt, pr);
   } else {
     ivfpq_search_f32(index->centroids.p, index->K, d, index->metric, index->codebook.p, index->M, index->nbits,
                      index->part_offsets.p, index->codes.p, index->row_ids.p, qp, nq, (int)kc, nprobes, si, sd,
-                     sc, flt, index->slab_off.p, index->codes_skew.p);
+                     sc, flt, index->slab_off.p, index->codes_skew.p, pr);
   }
   if (refine) {
     // exact re-rank with the true metric on the ORIGINAL (un-normalised) query, as flat_knn does; the
@@ -1576,6 +1576,41 @@ lb2_status lb2_index_search_ex(lb2_index* index, const void* queries, uint64_t n
   index_search_impl(index, queries, nq, sp->k, sp->nprobes, sp->refine_factor, sp->refine_vectors,
                     sp->num_vectors, sp->allow_bitmap, row_ids_out, dists_out, counts_out, sp->has_lower_bound != 0,
                     sp->lower_bound, sp->has_upper_bound != 0, sp->upper_bound);
+  LB2_API_END
+}
+
+lb2_status lb2_index_search_probed(lb2_index* index, const void* queries, uint64_t nq, const lb2_search_params* sp,
+                                   const lb2_probe_params* pp, uint64_t* row_ids_out, float* dists_out,
+                                   uint32_t* counts_out, uint32_t* nprobes_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(sp && pp && index, "null argument");
+  LB2_REQUIRE(sp->nprobes == 0, "nprobes must be 0: the probe parameters decide the probes");
+  LB2_REQUIRE(sp->refine_factor == 0 || sp->refine_vectors, "refine_factor > 0 needs refine_vectors");
+  LB2_REQUIRE(pp->minimum_nprobes >= 1, "minimum_nprobes must be at least 1");
+  LB2_REQUIRE(pp->maximum_nprobes == 0 || pp->maximum_nprobes >= pp->minimum_nprobes,
+              "maximum_nprobes %u is below minimum_nprobes %u", pp->maximum_nprobes, pp->minimum_nprobes);
+  LB2_REQUIRE(pp->late_width >= 1, "late_width must be at least 1");
+  LB2_REQUIRE(sp->allow_bitmap || (!pp->has_max_len && !pp->mask_ids), "max_len and mask_ids need an allow bitmap");
+  if (current_comm() && current_comm()->nranks > 1)
+    fail(LB2_UNSUPPORTED, "a search with minimum / maximum nprobes on a row-sharded index is not implemented");
+  InArg<uint64_t> mask(pp->mask_ids, pp->mask_ids ? pp->num_mask_ids : 0);
+  DevBuf<uint64_t> no_ids(pp->mask_ids && pp->num_mask_ids == 0 ? 1 : 0);  // an iterable, empty allow list
+  OutArg<uint32_t> np_out(nprobes_out, nq);
+  ProbeRule pr;
+  pr.min_np = pp->minimum_nprobes;
+  pr.max_np = pp->maximum_nprobes;
+  pr.late_width = pp->late_width;
+  pr.k = sp->k;
+  pr.has_max_len = pp->has_max_len != 0;
+  pr.max_len = pp->max_len;
+  pr.mask_ids = pp->mask_ids ? (mask.get() ? mask.get() : no_ids.p) : nullptr;
+  pr.num_mask_ids = pp->mask_ids ? pp->num_mask_ids : 0;
+  pr.nprobes_out = np_out.get();
+  index_search_impl(index, queries, nq, sp->k, 0, sp->refine_factor, sp->refine_vectors, sp->num_vectors,
+                    sp->allow_bitmap, row_ids_out, dists_out, counts_out, sp->has_lower_bound != 0, sp->lower_bound,
+                    sp->has_upper_bound != 0, sp->upper_bound, &pr);
+  np_out.commit();
+  sync_stream();
   LB2_API_END
 }
 

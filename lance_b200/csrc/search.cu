@@ -21,6 +21,7 @@
 #include "comm.cuh"
 #include "common.cuh"
 #include "exact.cuh"
+#include "probe.cuh"
 #include "rq.cuh"
 #include "search.cuh"
 
@@ -1484,14 +1485,16 @@ ivfrq_scan_kernel(const float* __restrict__ rq, int code_dim, float sqrt_d, int 
 }
 
 // residual queries of `nq` queries x np probes: out[(q np + pi) d + t] = queries[q d + t] - c_{probe}[t]
+// (a probe id >= K is an empty slot of a search with minimum / maximum nprobes: its residual is 0)
 __global__ void rq_query_residual_kernel(const float* __restrict__ queries, uint64_t nq, int np, int d,
-                                         const float* __restrict__ centroids, const uint32_t* __restrict__ probe_ids,
-                                         float* __restrict__ out) {
+                                         const float* __restrict__ centroids, int K,
+                                         const uint32_t* __restrict__ probe_ids, float* __restrict__ out) {
   const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= nq * np * d) return;
   const uint64_t sl = g / d;
   const int t = (int)(g % d);
-  out[g] = __fsub_rn(queries[(sl / np) * d + t], centroids[(size_t)probe_ids[sl] * d + t]);
+  const uint32_t p = probe_ids[sl];
+  out[g] = p < (uint32_t)K ? __fsub_rn(queries[(sl / np) * d + t], centroids[(size_t)p * d + t]) : 0.0f;
 }
 
 // global merge per query: ascending (distance, row id), first k.  Candidate e of list pi of query qi sits
@@ -1721,13 +1724,14 @@ static void merge_lists(const char* name, uint64_t nq, const float* cand_d, cons
 }
 
 // The IVF query skeleton: the nprobes nearest partitions of every query, one candidate list of <= k per (query,
-// probe) slot, the lists merged per query.  scan(q0, qn, probe_ids, probe_dists, cand_d, cand_id, cand_cnt) fills the
-// lists of queries [q0, q0 + qn) (at most 32768 of them: the grid.y limit); probe_dists are find_partitions'
-// distances of the probed centroids (dist_q_c).
+// probe) slot, the lists merged per query.  scan(q0, qn, np, offsets, probe_ids, probe_dists, cand_d, cand_id,
+// cand_cnt) fills the lists of queries [q0, q0 + qn) (at most 32768 of them: the grid.y limit), np slots per query; probe_dists are
+// find_partitions' distances of the probed centroids (dist_q_c).
 constexpr uint64_t SEARCH_SLAB = 32768;
 template <class Scan>
 static void ivf_search(const float* centroids, int K, int d, int metric, const float* queries, uint64_t nq, int k,
-                       int np, uint64_t* out_ids, float* out_dists, uint32_t* out_counts, Scan scan) {
+                       int np, const uint64_t* part_offsets, uint64_t* out_ids, float* out_dists, uint32_t* out_counts,
+                       Scan scan) {
   // partitions are found with L2 on the (normalised) vectors for cosine (ivf.rs:149-185)
   const int cmetric = metric == METRIC_DOT ? METRIC_DOT : METRIC_L2;
   DevBuf<uint32_t> pids((size_t)nq * np), cand_cnt((size_t)nq * np);
@@ -1735,10 +1739,88 @@ static void ivf_search(const float* centroids, int K, int d, int metric, const f
   DevBuf<uint64_t> cand_id((size_t)nq * np * k);
   find_partitions_f32(centroids, K, d, cmetric, queries, nq, np, pids.p, pd.p);
   for (uint64_t q0 = 0; q0 < nq; q0 += SEARCH_SLAB)
-    scan(q0, std::min<uint64_t>(SEARCH_SLAB, nq - q0), pids.p + q0 * np, pd.p + q0 * np, cand_d.p + q0 * np * k,
+    scan(q0, std::min<uint64_t>(SEARCH_SLAB, nq - q0), np, part_offsets, pids.p + q0 * np, pd.p + q0 * np, cand_d.p + q0 * np * k,
          cand_id.p + q0 * np * k, cand_cnt.p + q0 * np);
   merge_lists("merge_topk", nq, cand_d.p, cand_id.p, cand_cnt.p, np, k, (size_t)k, (size_t)k, (size_t)np * k, (size_t)1,
               (size_t)np, out_ids, out_dists, out_counts);
+}
+
+// The same skeleton with a per-query probe count (probe.cu): per slab of queries every centroid distance is ranked
+// (P = the first L = min(maximum_nprobes or K, K)), the cutoff fixes how many of P each query searches, and the scan
+// runs over a grid as wide as the slab's largest count.  A query's slots past its own count hold the partition id K,
+// which `ext_offsets` (part_offsets with one more empty partition) makes an empty partition for every scan kernel.
+// With a mask the query may answer from (`pr.mask_ids`), every query gets one more slot: the shortcut list.
+// With a range bound c_p depends on the distances: all L partitions are scanned, the cutoff reads the scan's list
+// counts and empties the lists past it.  Candidate memory is bounded by sub-slabs of about 256 MB.
+template <class Scan>
+static void ivf_search_probed(const float* centroids, int K, int d, int metric, const float* queries, uint64_t nq,
+                              int kc, const uint64_t* part_offsets, const ScanFilter& flt, const ProbeRule& pr,
+                              uint64_t* out_ids, float* out_dists, uint32_t* out_counts, Scan scan) {
+  if (nq == 0) return;
+  const int cmetric = metric == METRIC_DOT ? METRIC_DOT : METRIC_L2;
+  const int L = pr.max_np ? (int)std::min<uint32_t>(pr.max_np, (uint32_t)K) : K;
+  const bool by_scan = flt.range != 0;
+  const int extra = pr.mask_ids ? 1 : 0;
+  DevBuf<uint64_t> ext_offsets((size_t)K + 2);
+  d2d(ext_offsets.p, part_offsets, (size_t)K + 1);
+  d2d(ext_offsets.p + K + 1, part_offsets + K, 1);
+  DevBuf<uint32_t> cpart;
+  if (!by_scan) {
+    cpart.alloc(K);
+    partition_counts(part_offsets, K, flt.allow, (uint32_t)kc, cpart.p);
+  }
+  // the ranking's buffers: distances, and two runs of packed words above one tile
+  const uint64_t rank_bytes = (uint64_t)K * (K > RANK_TILE ? 20 : 4) + (uint64_t)L * 8;
+  const uint64_t qs = std::max<uint64_t>(1, std::min<uint64_t>(SEARCH_SLAB, (256ull << 20) / rank_bytes));
+  DevBuf<float> all(std::min(qs, nq) * K), pd(std::min(qs, nq) * L);
+  DevBuf<uint32_t> pids(std::min(qs, nq) * L), nsearch(std::min(qs, nq)), shortcut(std::min(qs, nq)), nmax(1);
+  for (uint64_t q0 = 0; q0 < nq; q0 += qs) {
+    const uint64_t qn = std::min(qs, nq - q0);
+    assign_f32(queries + q0 * d, qn, d, centroids, K, cmetric, nullptr, nullptr, nullptr, nullptr, all.p);
+    rank_probes(all.p, qn, K, L, pids.p, pd.p);
+    uint32_t* nprobes_out = pr.nprobes_out ? pr.nprobes_out + q0 : nullptr;
+    int np = L;
+    if (!by_scan) {
+      nmax.zero();
+      probe_cutoff(pr, qn, L, pids.p, pd.p, cpart.p, nullptr, 0, nsearch.p, shortcut.p, nmax.p, nprobes_out);
+      uint32_t h = 0;
+      d2h(&h, nmax.p, 1);
+      sync_stream();
+      np = (int)h;
+    }
+    const int nl = np + extra;  // slots per query
+    DevBuf<uint32_t> sp((size_t)qn * nl);
+    DevBuf<float> spd((size_t)qn * nl);
+    gather_probes(qn, L, pids.p, pd.p, by_scan ? nullptr : nsearch.p, nl, (uint32_t)K, sp.p, spd.p);
+    const uint64_t per_q = (uint64_t)nl * kc * 12 + 4 * (uint64_t)nl;
+    const uint64_t sub = std::max<uint64_t>(1, std::min<uint64_t>(qn, (256ull << 20) / per_q));
+    DevBuf<float> cd(sub * nl * kc);
+    DevBuf<uint64_t> cid(sub * nl * kc);
+    DevBuf<uint32_t> ccnt(sub * nl);
+    for (uint64_t a = 0; a < qn; a += sub) {
+      const uint64_t b = std::min(sub, qn - a);
+      scan(q0 + a, b, nl, ext_offsets.p, sp.p + a * nl, spd.p + a * nl, cd.p, cid.p, ccnt.p);
+      if (by_scan)
+        probe_cutoff(pr, b, L, pids.p + a * L, pd.p + a * L, nullptr, ccnt.p, nl, nsearch.p + a, shortcut.p + a,
+                     nmax.p, nprobes_out ? nprobes_out + a : nullptr);
+      if (extra) shortcut_lists(b, shortcut.p + a, pr.mask_ids, pr.num_mask_ids, nl, kc, cd.p, cid.p, ccnt.p);
+      merge_lists("merge_topk", b, cd.p, cid.p, ccnt.p, nl, kc, (size_t)kc, (size_t)kc, (size_t)nl * kc, (size_t)1,
+                  (size_t)nl, out_ids + (q0 + a) * kc, out_dists + (q0 + a) * kc, out_counts ? out_counts + q0 + a : nullptr);
+    }
+  }
+}
+
+// the fixed-nprobes skeleton, or with a probe rule the per-query one
+template <class Scan>
+static void run_ivf_search(const float* centroids, int K, int d, int metric, const float* queries, uint64_t nq, int k,
+                           int nprobes, const uint64_t* part_offsets, const ScanFilter& flt, const ProbeRule* pr,
+                           uint64_t* out_ids, float* out_dists, uint32_t* out_counts, Scan scan) {
+  if (pr)
+    ivf_search_probed(centroids, K, d, metric, queries, nq, k, part_offsets, flt, *pr, out_ids, out_dists, out_counts,
+                      scan);
+  else
+    ivf_search(centroids, K, d, metric, queries, nq, k, nprobes < K ? nprobes : K, part_offsets, out_ids, out_dists,
+               out_counts, scan);
 }
 
 // f(metric, element) with the metric as a std::integral_constant and the element type as a type_tag
@@ -1772,7 +1854,7 @@ void ivfpq_search_f32(const float* centroids, int K, int d, int metric, const fl
                       int nbits, const uint64_t* part_offsets, const uint8_t* codes,
                       const uint64_t* row_ids, const float* queries, uint64_t nq, int k, int nprobes,
                       uint64_t* out_ids, float* out_dists, uint32_t* out_counts, const ScanFilter& flt,
-                      const uint64_t* slab_off, const uint8_t* skew) {
+                      const uint64_t* slab_off, const uint8_t* skew, const ProbeRule* pr) {
   if (nq == 0 || k == 0) return;
   if (nbits != 8 && nbits != 4) fail(LB2_INVALID_ARG, "PQ: num_bits must be 4 or 8, got %d", nbits);
   if (nbits == 4 && (M % 2 != 0 || M > 256)) fail(LB2_UNSUPPORTED, "4-bit PQ needs an even num_sub_vectors <= 256");
@@ -1797,9 +1879,11 @@ void ivfpq_search_f32(const float* centroids, int K, int d, int metric, const fl
   else need_of(std::integral_constant<int, METRIC_L2>{});
   if (need > ctx().smem_optin) fail(LB2_UNSUPPORTED, "LUT and top-k scratch of %zu bytes exceed shared memory", need);
   DevBuf<uint32_t> rlist((size_t)std::min<uint64_t>(nq, SEARCH_SLAB) * np), rcount(1);
-  ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
-             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, const float*, float* cd, uint64_t* cid, uint32_t* ccnt) {
-               const ScanArgs a{queries + q0 * d, d, centroids, codebook, M, d / M, pids, np, part_offsets, codes,
+  run_ivf_search(centroids, K, d, metric, queries, nq, k, np, part_offsets, flt, pr, out_ids, out_dists, out_counts,
+             [&](uint64_t q0, uint64_t qn, int np, const uint64_t* offs, const uint32_t* pids, const float*, float* cd,
+                 uint64_t* cid, uint32_t* ccnt) {
+               if (rlist.n < qn * np) rlist.alloc(qn * np);
+               const ScanArgs a{queries + q0 * d, d, centroids, codebook, M, d / M, pids, np, offs, codes,
                                 row_ids, k, cd, cid, ccnt, flt};
                const dim3 g(np, (unsigned)qn);
                if (metric == METRIC_DOT)
@@ -1863,7 +1947,7 @@ void row_mask_f32(const uint64_t* row_ids, uint64_t n, const uint64_t* allow, ui
 void ivfflat_search_f32(const float* centroids, int K, int d, int metric, const uint64_t* part_offsets,
                         const void* vectors, int vdt, const uint64_t* row_ids, const float* queries, uint64_t nq,
                         int k, int nprobes, uint64_t* out_ids, float* out_dists, uint32_t* out_counts,
-                        const ScanFilter& flt) {
+                        const ScanFilter& flt, const ProbeRule* pr) {
   if (nq == 0 || k == 0) return;
   if (k > 1024) fail(LB2_UNSUPPORTED, "k (incl. refine factor) > 1024 is not implemented");
   const size_t smem = sizeof(float) * (size_t)d + slot_smem_bytes(k);
@@ -1872,15 +1956,15 @@ void ivfflat_search_f32(const float* centroids, int K, int d, int metric, const 
     need = smem_with_static(ivfflat_scan_kernel<decltype(m)::value, typename decltype(e)::type>, smem);
   });
   if (need > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the flat scan", d);
-  const int np = nprobes < K ? nprobes : K;
-  ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
-             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, const float*, float* cd, uint64_t* cid, uint32_t* ccnt) {
+  run_ivf_search(centroids, K, d, metric, queries, nq, k, nprobes, part_offsets, flt, pr, out_ids, out_dists, out_counts,
+             [&](uint64_t q0, uint64_t qn, int np, const uint64_t* offs, const uint32_t* pids, const float*, float* cd,
+                 uint64_t* cid, uint32_t* ccnt) {
                dispatch_metric_elem<false>(metric, vdt, [&](auto m, auto e) {
                  using T = typename decltype(e)::type;
                  auto kern = ivfflat_scan_kernel<decltype(m)::value, T>;
                  set_smem(kern, smem);
                  LB2_LAUNCH("flat_scan", kern, dim3(np, (unsigned)qn), 256, smem, queries + q0 * d, d, pids, np,
-                            part_offsets, reinterpret_cast<const T*>(vectors), row_ids, k, cd, cid, ccnt, flt);
+                            offs, reinterpret_cast<const T*>(vectors), row_ids, k, cd, cid, ccnt, flt);
                });
              });
 }
@@ -1888,7 +1972,7 @@ void ivfflat_search_f32(const float* centroids, int K, int d, int metric, const 
 void ivfsq_search_f32(const float* centroids, int K, int d, int metric, const uint64_t* part_offsets,
                       const uint8_t* codes, const uint64_t* row_ids, float r2, const float* queries,
                       const uint8_t* qcodes, uint64_t nq, int k, int nprobes, uint64_t* out_ids, float* out_dists,
-                      uint32_t* out_counts, const ScanFilter& flt) {
+                      uint32_t* out_counts, const ScanFilter& flt, const ProbeRule* pr) {
   if (nq == 0 || k == 0) return;
   if (k > 1024) fail(LB2_UNSUPPORTED, "k (incl. refine factor) > 1024 is not implemented");
   const size_t smem = (size_t)(d + 15) / 16 * 16 + slot_smem_bytes(k);
@@ -1903,13 +1987,13 @@ void ivfsq_search_f32(const float* centroids, int K, int d, int metric, const ui
   size_t need = 0;
   with_kernel([&](auto kern) { need = smem_with_static(kern, smem); });
   if (need > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the SQ scan", d);
-  const int np = nprobes < K ? nprobes : K;
-  ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
-             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, const float*, float* cd, uint64_t* cid, uint32_t* ccnt) {
+  run_ivf_search(centroids, K, d, metric, queries, nq, k, nprobes, part_offsets, flt, pr, out_ids, out_dists, out_counts,
+             [&](uint64_t q0, uint64_t qn, int np, const uint64_t* offs, const uint32_t* pids, const float*, float* cd,
+                 uint64_t* cid, uint32_t* ccnt) {
                with_kernel([&](auto kern) {
                  set_smem(kern, smem);
                  LB2_LAUNCH("sq_scan", kern, dim3(np, (unsigned)qn), 256, smem, qcodes + q0 * d, d, r2, pids, np,
-                            part_offsets, codes, row_ids, k, cd, cid, ccnt, flt);
+                            offs, codes, row_ids, k, cd, cid, ccnt, flt);
                });
              });
 }
@@ -1921,18 +2005,18 @@ bool rq_scan_fits(int code_dim, int k) {
 void ivfrq_search_f32(const float* centroids, int K, int d, int metric, const float* rotation, int code_dim,
                       const uint64_t* part_offsets, const uint8_t* codes, const float* add, const float* scale,
                       const uint64_t* row_ids, const float* queries, uint64_t nq, int k, int nprobes,
-                      uint64_t* out_ids, float* out_dists, uint32_t* out_counts, const ScanFilter& flt) {
+                      uint64_t* out_ids, float* out_dists, uint32_t* out_counts, const ScanFilter& flt,
+                      const ProbeRule* pr) {
   if (nq == 0 || k == 0) return;
   if (k > 1024) fail(LB2_UNSUPPORTED, "k (incl. refine factor) > 1024 is not implemented");
   if (!rq_scan_fits(code_dim, k))
     fail(LB2_UNSUPPORTED, "IVF_RQ: the tables of code_dim %d do not fit the scan's shared memory", code_dim);
   const size_t smem = rq_scan_smem_bytes(code_dim, k);
-  const int np = nprobes < K ? nprobes : K;
   const float sqrt_d = sqrtf((float)code_dim);  // (dim as f32 * num_bits as f32).sqrt(): the product is exact
   const int q_minus_one = metric != METRIC_L2;    // the storage's metric: cosine / dot -> dist_q_c - 1.0
-  ivf_search(centroids, K, d, metric, queries, nq, k, np, out_ids, out_dists, out_counts,
-             [&](uint64_t q0, uint64_t qn, const uint32_t* pids, const float* pdists, float* cd, uint64_t* cid,
-                 uint32_t* ccnt) {
+  run_ivf_search(centroids, K, d, metric, queries, nq, k, nprobes, part_offsets, flt, pr, out_ids, out_dists, out_counts,
+             [&](uint64_t q0, uint64_t qn, int np, const uint64_t* offs, const uint32_t* pids, const float* pdists,
+                 float* cd, uint64_t* cid, uint32_t* ccnt) {
                // the (query, probe) residuals are rotated in groups of queries that keep both buffers near 256 MB
                const uint64_t per_q = (uint64_t)np * (d + code_dim) * sizeof(float);
                const uint64_t qc = std::max<uint64_t>(1, std::min<uint64_t>(qn, (256ull << 20) / per_q));
@@ -1941,10 +2025,10 @@ void ivfrq_search_f32(const float* centroids, int K, int d, int metric, const fl
                for (uint64_t a = 0; a < qn; a += qc) {
                  const uint64_t b = std::min(qc, qn - a);
                  LB2_LAUNCH("rq_query_residual", rq_query_residual_kernel, cdiv(b * np * d, 256), 256, 0,
-                            queries + (q0 + a) * d, b, np, d, centroids, pids + a * np, res.p);
+                            queries + (q0 + a) * d, b, np, d, centroids, K, pids + a * np, res.p);
                  rq_rotate_f32(rotation, code_dim, d, res.p, b * np, rot.p);
                  LB2_LAUNCH("rq_scan", ivfrq_scan_kernel, dim3(np, (unsigned)b), 256, smem, rot.p, code_dim, sqrt_d,
-                            q_minus_one, pids + a * np, pdists + a * np, np, part_offsets, codes, add, scale, row_ids,
+                            q_minus_one, pids + a * np, pdists + a * np, np, offs, codes, add, scale, row_ids,
                             k, cd + a * np * k, cid + a * np * k, ccnt + a * np, flt);
                }
              });

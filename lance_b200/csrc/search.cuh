@@ -2,6 +2,8 @@
 #pragma once
 #include <stdint.h>
 #include <string.h>
+
+#include "probe.cuh"
 namespace lb2 {
 // what FlatIndex::search lets into its heap (flat/index.rs:97-165): the prefilter bitmap over storage
 // positions (nullable) and the [lower, upper) range in f32::total_cmp order as signed order keys
@@ -23,7 +25,7 @@ void ivfpq_search_f32(const float* centroids, int K, int d, int metric, const fl
                       const uint64_t* row_ids, const float* queries, uint64_t nq, int k, int nprobes,
                       uint64_t* out_ids, float* out_dists, uint32_t* out_counts,
                       const ScanFilter& flt = ScanFilter(), const uint64_t* slab_off = nullptr,
-                      const uint8_t* skew = nullptr);
+                      const uint8_t* skew = nullptr, const ProbeRule* pr = nullptr);
 // the conflict-free scan's copy of the codes (8-bit, 16 sub-spaces of 8 dimensions): per 512-row slab and lane the
 // lane's 16 rows as one byte stream delayed by lane mod 16 bytes, in 17 coalesced 16-byte units
 bool skew_layout_applies(int M, int d, int nbits);
@@ -34,20 +36,23 @@ void build_skew_codes(const uint64_t* part_offsets, int K, const uint8_t* codes,
 void ivfflat_search_f32(const float* centroids, int K, int d, int metric, const uint64_t* part_offsets,
                         const void* vectors, int vdt, const uint64_t* row_ids, const float* queries, uint64_t nq,
                         int k, int nprobes, uint64_t* out_ids, float* out_dists, uint32_t* out_counts,
-                        const ScanFilter& flt = ScanFilter());
+                        const ScanFilter& flt = ScanFilter(), const ProbeRule* pr = nullptr);
 // codes: the index's SQ codes [n][d] in partition order; qcodes: the queries' codes [nq][d] under the same bounds;
 // r2 = rf * rf with rf = (float)(upper - lower); queries: f32 (normalised for cosine), for the probe selection
 void ivfsq_search_f32(const float* centroids, int K, int d, int metric, const uint64_t* part_offsets,
                       const uint8_t* codes, const uint64_t* row_ids, float r2, const float* queries,
                       const uint8_t* qcodes, uint64_t nq, int k, int nprobes, uint64_t* out_ids, float* out_dists,
-                      uint32_t* out_counts, const ScanFilter& flt = ScanFilter());
+                      uint32_t* out_counts, const ScanFilter& flt = ScanFilter(), const ProbeRule* pr = nullptr);
+// pr (nullable): search with the probe rule instead of nprobes (the search's k is k * refine_factor, pr->k the
+// query's k)
 // IVF_RQ: rotation [code_dim][code_dim]; codes [n][code_dim / 8] and the add / scale factors [n] in partition order;
 // queries: f32 (normalised for cosine).  rq_scan_fits: the scan's tables and a k-slot fit shared memory.
 bool rq_scan_fits(int code_dim, int k);
 void ivfrq_search_f32(const float* centroids, int K, int d, int metric, const float* rotation, int code_dim,
                       const uint64_t* part_offsets, const uint8_t* codes, const float* add, const float* scale,
                       const uint64_t* row_ids, const float* queries, uint64_t nq, int k, int nprobes,
-                      uint64_t* out_ids, float* out_dists, uint32_t* out_counts, const ScanFilter& flt = ScanFilter());
+                      uint64_t* out_ids, float* out_dists, uint32_t* out_counts, const ScanFilter& flt = ScanFilter(),
+                      const ProbeRule* pr = nullptr);
 // all ranks' [nq][k] results of a row-sharded index -> the global top-k by (distance, row id) on every rank
 void merge_sharded_topk(const uint64_t* ids, const float* dists, const uint32_t* counts, uint64_t nq, int k,
                         uint64_t* out_ids, float* out_dists, uint32_t* out_counts);
