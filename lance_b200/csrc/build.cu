@@ -1,0 +1,698 @@
+// build.cu -- the whole-index builds (IVF_PQ, IVF_FLAT, IVF_SQ, IVF_RQ), their training stages and the per-row
+// transforms they share with lb2_ivfpq_transform / lb2_ivfrq_transform.
+#include <chrono>
+#include <memory>
+
+#include "assign.cuh"
+#include "build.cuh"
+#include "comm.cuh"
+#include "index.cuh"
+#include "kmeans.cuh"
+#include "rq.cuh"
+#include "search.cuh"
+#include "sq.cuh"
+#include "tc_assign.cuh"
+#include "tc_pq.cuh"
+
+namespace lb2 {
+
+__global__ void residual_kernel(const float* x, const float* __restrict__ cent,
+                                const uint32_t* __restrict__ part, uint64_t n, int d, float* out) {
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n * d) return;
+  const uint64_t r = g / d;
+  const int t = g % d;
+  out[g] = __fsub_rn(x[g], cent[(size_t)part[r] * d + t]);  // residual.rs:93
+}
+
+void check_pq_shape(uint32_t d, uint32_t M, uint32_t nbits, PqUse use) {
+  LB2_REQUIRE(M > 0 && d % M == 0, "num_sub_vectors must divide vector dimension %u, but got %u", d, M);
+  if (nbits != 8 && nbits != 4)  // pq/builder.rs: only 4 and 8 exist in the reference
+    fail(LB2_INVALID_ARG, "PQ: num_bits must be 4 or 8, got %u", nbits);
+  if (use == PqUse::TRAIN) return;
+  LB2_REQUIRE(nbits == 8 || M % 2 == 0, "PQ: num_sub_vectors must be divisible by 2 for num_bits=4, but got %u", M);
+  if (use == PqUse::ENCODE && !small_d_supported((int)(d / M)))
+    fail(LB2_UNSUPPORTED, "PQ sub-vector width %d not supported yet", (int)(d / M));
+}
+
+// ProductQuantizer::transform_impl for either code width (pq.rs:116-191): 8-bit -> [n][M] through the
+// tensor path where it applies; 4-bit -> 16 codewords per sub-space, exact kernel, two codes per byte
+void pq_encode_any(const float* x, uint64_t n, int d, int M, int ds, const float* codebook, int metric,
+                   const float* cent, const uint32_t* part, const uint8_t* row_valid, int nbits, uint8_t* codes) {
+  if (nbits == 8) {
+    pq_encode_dev(x, n, d, M, ds, codebook, metric, cent, part, row_valid, codes);
+    return;
+  }
+  if (n == 0) return;
+  DevBuf<uint8_t> wide((size_t)n * M);
+  small_d_assign_f32(x, n, d, M, ds, codebook, 16, metric, cent, part, row_valid, wide.p, nullptr, nullptr,
+                     nullptr, nullptr);
+  pack_nibbles(wide.p, n, M, codes);
+  sync_stream();  // `wide` is freed on return
+}
+
+// KMeansParams::redos (kmeans.rs:643-716).  Every redo starts from `rng.clone()` of the same generator
+// (kmeans.rs:645-653), i.e. from the SAME initial centroids; the only state carried from one redo to the
+// next is cluster_sizes / adjusted_balance_factor, which only enter through the balance bias.  With
+// balance_factor == 0 (every PQ codebook, pq/builder.rs:100) all redos are therefore identical and
+// "best of redos" is the single run; with a balance bias the redo loop is not implemented -> UNSUPPORTED.
+void check_redos(uint32_t redos, float balance_factor) {
+  if (redos == 0) fail(LB2_INVALID_ARG, "KMeans: redos must be at least 1");
+  if (redos > 1 && balance_factor != 0.0f)
+    fail(LB2_UNSUPPORTED, "KMeans: redos = %u with a balance factor is not implemented (redos = 1 only)", redos);
+}
+
+void pq_train_dev(const float* data, uint64_t n, int d, int metric, const lb2_pq_params* p, float* codebook,
+                  std::vector<uint32_t>* iters) {
+  const int M = p->num_sub_vectors, K = 1 << p->num_bits;
+  check_pq_shape(d, M, p->num_bits, PqUse::TRAIN);
+  check_redos(p->kmeans_redos, 0.0f);
+  LB2_REQUIRE(current_comm() || n >= (uint64_t)K, "Not enough rows to train PQ. Requires %d rows but only %llu available",
+              K, (unsigned long long)n);
+  // free fn train_kmeans (kmeans.rs:1328-1340): first sample_rate*k rows (per-rank share when sharded)
+  const uint64_t nranks = current_comm() ? current_comm()->nranks : 1;
+  const uint64_t cap = (p->sample_rate * K + nranks - 1) / nranks;
+  const uint64_t rows = n > cap ? cap : n;
+  InArg<float> init(p->codebook, (size_t)M * K * (d / M));
+  lloyd_train(data, rows, d, M, d / M, K, metric == METRIC_DOT ? METRIC_DOT : METRIC_L2, 0.0f,
+              (int)p->max_iters, 1e-4, p->seed, init.get(), codebook, nullptr, iters);
+}
+
+namespace {
+// CUDA events of a build, destroyed on every path
+struct EventSet {
+  std::vector<cudaEvent_t> ev;
+  explicit EventSet(int n) : ev(n, nullptr) {
+    for (auto& e : ev) LB2_CUDA(cudaEventCreate(&e));
+  }
+  ~EventSet() {
+    for (auto& e : ev)
+      if (e) cudaEventDestroy(e);
+  }
+  void record(int i) { LB2_CUDA(cudaEventRecord(ev[i], ctx().stream)); }
+  float ms(int i, int j) const {
+    float t = 0.f;
+    cudaEventElapsedTime(&t, ev[i], ev[j]);
+    return t;
+  }
+};
+// KMeans::new_with_params (kmeans.rs:1008-1030): hierarchical for k > 256, flat Lloyd otherwise
+void train_ivf(const float* xs, uint64_t s, int d, int K, int am, const lb2_kmeans_params& kp, uint64_t nranks,
+               const float* init, float* centroids, std::vector<double>* loss, std::vector<uint32_t>* iters) {
+  check_redos(kp.redos, kp.balance_factor);
+  if (K > 256 && kp.hierarchical_k > 1 && !init) {
+    loss->assign(1, 0.0);
+    iters->assign(1, 0);
+    if (nranks > 1) {
+      // Sharded build: the hierarchical tree is thousands of small dependent Lloyd runs -- with a collective in
+      // every iteration it is latency-bound on the exchange.  The sample (K * sample_rate rows) is small next to
+      // the data, so when it fits every rank gathers ALL sample shards (rank order) and trains the same tree on
+      // them without a communicator: identical arithmetic on identical input gives bit-identical models on all
+      // ranks, and the splits train concurrently (kmeans.cu: SplitWorkers).  Otherwise: the sharded tree.
+      DevBuf<uint64_t> cnt_in(1), cnt_all(nranks);
+      h2d(cnt_in.p, &s, 1);
+      comm_allgather_bytes(cnt_in.p, cnt_all.p, sizeof(uint64_t));
+      std::vector<uint64_t> cnt(nranks);
+      d2h(cnt.data(), cnt_all.p, nranks);
+      sync_stream();
+      uint64_t total = 0, mx = 0;
+      for (uint64_t c : cnt) { total += c; mx = std::max(mx, c); }
+      size_t free_b = 0, total_b = 0;
+      cudaMemGetInfo(&free_b, &total_b);
+      const bool off = getenv("LB2_SHARDED_TREE") && *getenv("LB2_SHARDED_TREE");
+      if (!off && total < 0xffffffffull && (size_t)nranks * mx * d * 4 * 3 <= free_b) {
+        DevBuf<float> pad, all((size_t)nranks * mx * d);
+        const float* in = xs;
+        if (s < mx) {
+          pad.alloc((size_t)mx * d);
+          pad.zero();
+          if (s) d2d(pad.p, xs, (size_t)s * d);
+          in = pad.p;
+        }
+        comm_allgather_bytes(in, all.p, (size_t)mx * d * sizeof(float));
+        pad.release();
+        if (total != nranks * mx) {  // unequal shards: close the gaps (rank order is kept)
+          DevBuf<float> full(std::max<uint64_t>(total, 1) * d);
+          uint64_t o = 0;
+          for (uint64_t r = 0; r < nranks; ++r) {
+            if (cnt[r]) d2d(full.p + o * d, all.p + r * mx * d, cnt[r] * d);
+            o += cnt[r];
+          }
+          all = std::move(full);
+        }
+        Comm* saved = comm_swap(nullptr);
+        try {
+          hierarchical_train(all.p, total, d, K, am, kp.balance_factor / (float)total, (int)kp.max_iters, kp.tolerance,
+                             (int)kp.hierarchical_k, kp.seed, centroids);
+        } catch (...) {
+          comm_swap(saved);
+          throw;
+        }
+        comm_swap(saved);
+        return;
+      }
+    }
+    hierarchical_train(xs, s, d, K, am, kp.balance_factor / (float)(s * nranks), (int)kp.max_iters, kp.tolerance,
+                       (int)kp.hierarchical_k, kp.seed, centroids);
+  } else {
+    lloyd_train(xs, s, d, 1, d, K, am, kp.balance_factor / (float)(s * nranks), (int)kp.max_iters, kp.tolerance,
+                kp.seed, init, centroids, loss, iters);
+  }
+}
+}  // namespace
+
+// The IVF stage of every build, in two halves so that IVF_PQ can gather its own sample in between:
+// (a) the IVF training sample's rows (ivf.rs:1237-1241), to be gathered with gather_finite_sample (rows that are not
+// finite dropped, normalised first under cosine);
+static std::vector<uint64_t> ivf_sample_rows(uint64_t n, int K, const lb2_kmeans_params& kp, uint64_t seed,
+                                             uint64_t nranks) {
+  return sample_rows(n, std::min<uint64_t>(n, ((uint64_t)K * kp.sample_rate + nranks - 1) / nranks), seed);
+}
+// (b) after the caller started the bulk copy: train on the s gathered rows, centroids rounded to the column's type
+static void train_ivf_model(const float* sample, uint64_t s, lb2_index* ix, const lb2_kmeans_params& kp,
+                            uint64_t nranks, std::vector<double>* loss, std::vector<uint32_t>* iters) {
+  const int K = ix->K, d = ix->d;
+  LB2_REQUIRE(nranks > 1 || s >= (uint64_t)K, "KMeans: can not train %d centroids with %llu finite vectors", K,
+              (unsigned long long)s);
+  TagScope tg("ivf_train");
+  VecIn init(kp.init_centroids, (size_t)K * d, model_dtype(ix->dtype));
+  train_ivf(sample, s, d, K, ix->metric == METRIC_DOT ? METRIC_DOT : METRIC_L2, kp, nranks, init.get(),
+            ix->centroids.p, loss, iters);
+  round_model(ix->centroids.p, (size_t)K * d, ix->dtype);
+}
+// both halves, with the bulk copy started in between (IVF_FLAT, IVF_SQ, IVF_RQ)
+static void train_ivf_stage(Source& src, lb2_index* ix, const lb2_kmeans_params& kp, uint64_t seed, uint64_t nranks,
+                            std::vector<double>* loss, std::vector<uint32_t>* iters) {
+  TagScope tg("ivf_train");
+  std::vector<uint64_t> rows = ivf_sample_rows(src.n(), ix->K, kp, seed, nranks);
+  DevBuf<float> sample;
+  const uint64_t s = gather_finite_sample(src, rows, ix->metric == METRIC_COSINE, sample);
+  src.start_resident_copy();  // host rows: the bulk copy runs on its own stream while the centroids train
+  train_ivf_model(sample.p, s, ix, kp, nranks, loss, iters);
+}
+
+// the stage times of a build from its events: start, IVF trained, [quantizer trained,] transformed, grouped (IVF_FLAT
+// has no quantizer stage: 4 events, ms_pq_train 0)
+static void fill_stats(lb2_build_stats* stats, const EventSet& ev, const std::vector<double>& loss,
+                       const std::vector<uint32_t>& iters, const std::vector<uint32_t>& pq_iters = {}) {
+  if (!stats) return;
+  memset(stats, 0, sizeof(*stats));
+  const int q = (int)ev.ev.size() - 4;
+  stats->ms_ivf_train = ev.ms(0, 1);
+  if (q) stats->ms_pq_train = ev.ms(1, 2);
+  stats->ms_transform = ev.ms(1 + q, 2 + q);
+  stats->ms_group = ev.ms(2 + q, 3 + q);
+  stats->ms_total = ev.ms(0, 3 + q);
+  stats->ivf_iters = iters.empty() ? 0 : iters[0];
+  for (auto v : pq_iters) stats->pq_iters_max = std::max(stats->pq_iters_max, v);
+  stats->ivf_loss = loss.empty() ? 0.0 : loss[0];
+}
+
+// IvfTransformer's partition step over one chunk of rows (ivf.rs:158-166): normalised first under cosine, then
+// assigned (by dot or L2) from f32, or from the rows' own type (xnat / dtype, for_each_chunk) when not normalised.
+// Returns the chunk as the index sees it.
+static const float* normalize_assign(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
+                                     const float* cent, int K, DevBuf<float>& normbuf, uint32_t* part, uint8_t* valid,
+                                     float* dist) {
+  const float* xp = xf;
+  if (m == METRIC_COSINE) {
+    if (normbuf.n < (size_t)rows * d) normbuf.alloc((size_t)rows * d);
+    normalize_rows(xf, rows, d, normbuf.p);
+    xp = normbuf.p;
+    xnat = nullptr;
+  }
+  assign_f32(xp, rows, d, cent, K, m == METRIC_DOT ? METRIC_DOT : METRIC_L2, nullptr, part, dist, valid, nullptr,
+             xnat, dtype);
+  return xp;
+}
+
+// IvfTransformer::transform over one chunk of rows already on the device as f32 (lance-index/src/vector/ivf.rs:
+// 188-236,357): [normalise if cosine] -> partition id -> residual -> PQ code.  The quantizer of an index build is
+// trained -- and therefore encodes -- with L2 whatever the index metric is: Q::build(&training_data,
+// DistanceType::L2, ..) (rust/lance/src/index/vector/builder.rs:460); the index metric only decides the partition
+// assignment, whether residuals are taken (not for dot, PQBuildParams::use_residual) and the query-time table.
+static void transform_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m, const float* cent,
+                            int K, const float* codebook, int M, int nbits, DevBuf<float>& normbuf, uint32_t* part,
+                            uint8_t* codes, uint8_t* valid) {
+  const float* xp = normalize_assign(xf, xnat, dtype, rows, d, m, cent, K, normbuf, part, valid, nullptr);
+  const bool dot = m == METRIC_DOT;
+  pq_encode_any(xp, rows, d, M, d / M, codebook, METRIC_L2, dot ? nullptr : cent, dot ? nullptr : part, valid, nbits,
+                codes);
+}
+
+// partition assignment of one chunk of rows (IVF_FLAT / IVF_SQ / IVF_RQ transform); returns the chunk as f32 as the
+// index sees it: normalised under cosine.  Rows with a non-finite element are dropped in every metric
+// (KeepFiniteVectors precedes the partition transform, ivf.rs:166, 256, 299).  Under L2 and cosine such a row has
+// no finite distance and the assignment already drops it; under dot a +-inf element can still give a -inf best
+// distance, so the elements are checked.
+static const float* assign_flat_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
+                                      const float* cent, int K, DevBuf<float>& normbuf, uint32_t* part,
+                                      uint8_t* valid, float* dist = nullptr) {
+  const float* xp = normalize_assign(xf, xnat, dtype, rows, d, m, cent, K, normbuf, part, valid, dist);
+  if (m == METRIC_DOT && rows)
+    LB2_LAUNCH("drop_nonfinite_rows", finite_rows_kernel, cdiv(rows * 32, 256), 256, 0, xp, rows, d, valid, 1);
+  return xp;
+}
+
+// ---- IVF_SQ: IVFIndex<FlatIndex, ScalarQuantizer> (lance-index/src/vector/sq*.rs) --------------------------------
+void sq_check_dim(uint32_t d) {
+  LB2_REQUIRE(d > 0 && d % 4 == 0, "IVF_SQ needs a dimension that is a multiple of 4");
+  // the scan sums d terms of up to 255^2 in u32 (sq/storage.rs:432-468)
+  LB2_REQUIRE((uint64_t)d * 255 * 255 < (1ull << 32), "IVF_SQ: d * 255^2 must be below 2^32, d = %u", d);
+}
+
+// ---- IVF_RQ: IVFIndex<FlatIndex, RabitQuantizer> (lance-index/src/vector/bq/*.rs) ---------------------------------
+void rq_check(uint32_t d, lb2_dtype dtype, uint32_t num_bits) {
+  // RabitQuantizer::build takes f16 / f32 / f64 columns only (bq/builder.rs:194-210)
+  if (dtype == LB2_BF16 || dtype == LB2_U8) fail(LB2_INVALID_ARG, "IVF_RQ: unsupported data type %d", (int)dtype);
+  if (dtype != LB2_F32)
+    fail(LB2_UNSUPPORTED, "IVF_RQ: f16 columns are not implemented (the reference rotates them in f16)");
+  LB2_REQUIRE(d > 0 && num_bits > 0, "IVF_RQ: the dimension and num_bits must be positive");
+  const uint64_t cd = (uint64_t)d * num_bits;
+  LB2_REQUIRE(cd % 8 == 0, "IVF_RQ: code_dim = d * num_bits = %llu is not a multiple of 8", (unsigned long long)cd);
+  if (cd > 65536 || !rq_scan_fits((int)cd, 1))
+    fail(LB2_UNSUPPORTED, "IVF_RQ: the tables of code_dim %llu do not fit the scan's shared memory",
+         (unsigned long long)cd);
+}
+
+// IVF_RQ transform of one chunk (IvfTransformer::with_rq, ivf.rs:281-328): [normalise] -> partition and dist_v_c ->
+// residual -> rotation -> sign codes and factors.  Cosine is L2 on the normalised rows from there on.
+// The row chunk is bounded by d (Source::rows_per_chunk), the rotated rows by code_dim = d * num_bits: they are
+// rotated and encoded in sub-chunks of at most 2^28 / code_dim rows (1 GB of f32).
+struct RqWork {
+  DevBuf<float> normbuf, dist, res, rot;
+};
+static void rq_transform_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
+                               const float* cent, int K, const float* rotation, int num_bits, const float* cnorm,
+                               RqWork& w, uint32_t* part, uint8_t* valid, uint8_t* codes, float* add, float* scale) {
+  const int cd = d * num_bits;
+  const uint64_t sub = std::min<uint64_t>(rows, std::max<uint64_t>(1, (1ull << 28) / (uint64_t)cd));
+  if (w.dist.n < rows) w.dist.alloc(rows);
+  if (w.res.n < rows * d) w.res.alloc(rows * d);
+  if (w.rot.n < sub * cd) w.rot.alloc(sub * cd);
+  const float* xs = assign_flat_chunk(xf, xnat, dtype, rows, d, m, cent, K, w.normbuf, part, valid, w.dist.p);
+  rq_residual_f32(xs, rows, d, cent, part, valid, w.res.p);
+  for (uint64_t r0 = 0; r0 < rows; r0 += sub) {
+    const uint64_t rs = std::min(sub, rows - r0);
+    rq_rotate_f32(rotation, cd, d, w.res.p + r0 * d, rs, w.rot.p);
+    rq_encode_f32(w.rot.p, w.res.p + r0 * d, w.dist.p + r0, part + r0, cnorm, valid + r0, rs, d, num_bits,
+                  m == METRIC_DOT ? METRIC_DOT : METRIC_L2, codes + r0 * (cd / 8), add + r0, scale + r0);
+  }
+}
+
+// |c|^2 per centroid (norm_squared_fsl, RQTransformer::new, bq/transform.rs:42-59): dot only
+static void rq_centroid_norms(int metric, const float* cent, int K, int d, DevBuf<float>& out) {
+  if (metric != METRIC_DOT) return;
+  out.alloc(K);
+  rq_norm_sq_f32(cent, K, d, out.p);
+}
+
+}  // namespace lb2
+
+using namespace lb2;
+
+extern "C" {
+
+void lb2_ivfpq_build_params_default(lb2_ivfpq_build_params* p) {
+  p->num_partitions = 256;
+  lb2_kmeans_params_default(&p->ivf);
+  p->ivf.balance_factor = 1.0f;  // rust/lance/src/index/vector/ivf.rs:1858
+  lb2_pq_params_default(&p->pq);
+  p->seed = 0;
+}
+
+void lb2_ivfflat_build_params_default(lb2_ivfflat_build_params* p) {
+  p->num_partitions = 256;
+  lb2_kmeans_params_default(&p->ivf);
+  p->ivf.balance_factor = 1.0f;
+  p->seed = 0;
+}
+
+void lb2_ivfsq_build_params_default(lb2_ivfsq_build_params* p) {
+  p->num_partitions = 256;
+  lb2_kmeans_params_default(&p->ivf);
+  p->ivf.balance_factor = 1.0f;
+  p->num_bits = 8;
+  p->sample_rate = 256;
+  p->seed = 0;
+}
+
+void lb2_ivfrq_build_params_default(lb2_ivfrq_build_params* p) {
+  p->num_partitions = 256;
+  lb2_kmeans_params_default(&p->ivf);
+  p->ivf.balance_factor = 1.0f;
+  p->num_bits = 1;
+  p->seed = 0;
+}
+
+lb2_status lb2_ivfpq_transform(const void* centroids, uint32_t k, const void* codebook,
+                               uint32_t num_sub_vectors, uint32_t num_bits, uint32_t d,
+                               lb2_dtype dtype, lb2_metric metric, const void* vectors, uint64_t n,
+                               uint32_t* part_out, uint8_t* codes_out, uint8_t* valid_out) {
+  LB2_API_BEGIN
+  check_pq_shape(d, num_sub_vectors, num_bits, PqUse::ENCODE);
+  const int M = num_sub_vectors;
+  const int m = metric_of(metric);
+  VecIn c(centroids, (size_t)k * d, model_dtype(dtype)), cb(codebook, ((size_t)1 << num_bits) * d, model_dtype(dtype));
+  const size_t cw = num_bits == 4 ? M / 2 : M;
+  OutArg<uint32_t> p(part_out, n);
+  OutArg<uint8_t> co(codes_out, (size_t)n * cw), v(valid_out, n);
+  DevBuf<uint8_t> vtmp;
+  uint8_t* vp = v.get();
+  if (!vp) { vtmp.alloc(std::max<uint64_t>(n, 1)); vp = vtmp.p; }
+  if (n) {
+    Source src(vectors, n, (int)d, dtype);
+    src.start_resident_copy();
+    DevBuf<float> normbuf;
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, c.get(), (int)k, cb.get(), M, (int)num_bits, normbuf,
+                      p.get() + r0, co.get() + r0 * cw, vp + r0);
+    });
+  }
+  p.commit(); co.commit(); v.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_ivfrq_transform(const void* centroids, uint32_t k, const void* rotation, uint32_t d, uint32_t num_bits,
+                               lb2_dtype dtype, lb2_metric metric, const void* vectors, uint64_t n, uint32_t* part_out,
+                               uint8_t* codes_out, float* add_out, float* scale_out, uint8_t* valid_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(centroids && rotation && (vectors || n == 0) && k > 0, "null argument");
+  rq_check(d, dtype, num_bits);
+  const int m = metric_of(metric);
+  const uint64_t cd = (uint64_t)d * num_bits;
+  VecIn c(centroids, (size_t)k * d, dtype), r(rotation, cd * cd, dtype);
+  DevBuf<float> cnorm;
+  rq_centroid_norms(m, c.get(), (int)k, (int)d, cnorm);
+  OutArg<uint32_t> p(part_out, n);
+  OutArg<uint8_t> co(codes_out, (size_t)(n * cd / 8)), v(valid_out, n);
+  OutArg<float> ao(add_out, n), so(scale_out, n);
+  DevBuf<uint32_t> ptmp;
+  DevBuf<uint8_t> vtmp, ctmp;
+  DevBuf<float> atmp, stmp;
+  uint32_t* pp = p.get();
+  uint8_t *vp = v.get(), *cp = co.get();
+  float *ap = ao.get(), *sp = so.get();
+  if (!pp) { ptmp.alloc(std::max<uint64_t>(n, 1)); pp = ptmp.p; }
+  if (!vp) { vtmp.alloc(std::max<uint64_t>(n, 1)); vp = vtmp.p; }
+  if (!cp) { ctmp.alloc(std::max<uint64_t>(n * cd / 8, 1)); cp = ctmp.p; }
+  if (!ap) { atmp.alloc(std::max<uint64_t>(n, 1)); ap = atmp.p; }
+  if (!sp) { stmp.alloc(std::max<uint64_t>(n, 1)); sp = stmp.p; }
+  if (n) {
+    Source src(vectors, n, (int)d, dtype);
+    src.start_resident_copy();
+    RqWork w;
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      rq_transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, c.get(), (int)k, r.get(),
+                         (int)num_bits, cnorm.p, w, pp + r0, vp + r0, cp + r0 * (cd / 8), ap + r0, sp + r0);
+    });
+  }
+  p.commit(); co.commit(); v.commit(); ao.commit(); so.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_ivfflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype,
+                             lb2_metric metric, const lb2_ivfflat_build_params* params,
+                             const uint64_t* row_ids, lb2_index** out, lb2_build_stats* stats) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(data && params && out, "null argument");
+  LB2_REQUIRE(d % 4 == 0, "IVF_FLAT needs a dimension that is a multiple of 4");
+  const int m = metric_of(metric);
+  const int K = params->num_partitions;
+  const uint64_t nranks = current_comm() ? current_comm()->nranks : 1;
+  LB2_REQUIRE(K > 0 && (nranks > 1 || n >= (uint64_t)K), "KMeans: can not train %d centroids with %llu vectors", K,
+              (unsigned long long)n);
+  EventSet ev(4);
+  ev.record(0);
+  Source src(data, n, (int)d, dtype);
+  std::unique_ptr<lb2_index> ix = make_index(IndexKind::FLAT, K, d, m, dtype);
+  std::vector<double> loss;
+  std::vector<uint32_t> iters;
+  train_ivf_stage(src, ix.get(), params->ivf, params->seed, nranks, &loss, &iters);
+  ev.record(1);
+  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
+  DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1));
+  {
+    TagScope tg("transform");
+    DevBuf<float> normbuf;
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      assign_flat_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, normbuf, part.p + r0,
+                        valid.p + r0);
+    });
+  }
+  ev.record(2);
+  InArg<uint64_t> rid(row_ids, n);
+  {
+    TagScope tg("group");  // the stored vectors are the normalised ones when the metric is cosine
+    index_load_flat_src(ix.get(), part.p, src, rid.get(), valid.p, m == METRIC_COSINE);
+  }
+  ev.record(3);
+  sync_stream();
+  fill_stats(stats, ev, loss, iters);
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_ivfsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                           const lb2_ivfsq_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                           lb2_build_stats* stats) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(data && params && out, "null argument");
+  sq_check_dim(d);
+  if (params->num_bits != 8) fail(LB2_UNSUPPORTED, "IVF_SQ: num_bits = %u is not implemented (8 only)", params->num_bits);
+  if (current_comm() && current_comm()->nranks > 1)
+    fail(LB2_UNSUPPORTED, "IVF_SQ: builds sharded over ranks are not implemented (the bounds would need an exchange)");
+  const int m = metric_of(metric);
+  const int K = params->num_partitions;
+  LB2_REQUIRE(K > 0 && n >= (uint64_t)K, "KMeans: can not train %d centroids with %llu vectors", K, (unsigned long long)n);
+  EventSet ev(5);
+  ev.record(0);
+  Source src(data, n, (int)d, dtype);
+  std::unique_ptr<lb2_index> ix = make_index(IndexKind::SQ, K, d, m, dtype);
+  ix->nbits = 8;
+  std::vector<double> loss;
+  std::vector<uint32_t> iters;
+  // 1. IVF: the same stage as lb2_ivfflat_build (same sample, seed, training)
+  train_ivf_stage(src, ix.get(), params->ivf, params->seed, 1, &loss, &iters);
+  ev.record(1);
+  // 2. ScalarQuantizer::build (sq.rs:152-182) on sample_rate * 2^num_bits rows (builder.rs:410-421), normalised
+  //    under cosine, rows that are not finite dropped (builder.rs:436), no residuals (quantizer.rs:52).  The bounds
+  //    are taken over the values the index stores: normalised, in the column's element type.
+  {
+    TagScope tg("sq_train");
+    std::vector<uint64_t> rows = sample_rows(n, std::min<uint64_t>(n, params->sample_rate * 256), params->seed + 1);
+    DevBuf<float> sample;
+    const uint64_t s = gather_finite_sample(src, rows, m == METRIC_COSINE, sample);
+    round_model(sample.p, (size_t)s * d, dtype);
+    sq_bounds_f32(sample.p, (uint64_t)s * d, &ix->sq_lower, &ix->sq_upper);
+  }
+  ev.record(2);
+  // 3. transform (ivf.rs:238-279): partition, then the SQ codes of the stored vectors themselves
+  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
+  DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1)), codes(std::max<uint64_t>(1, (uint64_t)n * d));
+  {
+    TagScope tg("transform");
+    DevBuf<float> normbuf;
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      const float* xs = assign_flat_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, normbuf,
+                                          part.p + r0, valid.p + r0);
+      if (m == METRIC_COSINE) round_model(normbuf.p, (size_t)rows * d, dtype);  // as IVF_FLAT stores them
+      sq_encode_f32(xs, (uint64_t)rows * d, ix->sq_lower, ix->sq_upper, codes.p + r0 * d);
+    });
+  }
+  ev.record(3);
+  {
+    TagScope tg("group");
+    InArg<uint64_t> rid(row_ids, n);
+    index_load_dev(ix.get(), part.p, codes.p, rid.get(), n, valid.p);
+  }
+  ev.record(4);
+  sync_stream();
+  fill_stats(stats, ev, loss, iters);
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_ivfrq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                           const lb2_ivfrq_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                           lb2_build_stats* stats) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(data && params && out, "null argument");
+  rq_check(d, dtype, params->num_bits);
+  if (current_comm() && current_comm()->nranks > 1)
+    fail(LB2_UNSUPPORTED, "IVF_RQ: builds sharded over ranks are not implemented");
+  const int m = metric_of(metric);
+  const int K = params->num_partitions;
+  LB2_REQUIRE(K > 0 && n >= (uint64_t)K, "KMeans: can not train %d centroids with %llu vectors", K, (unsigned long long)n);
+  EventSet ev(5);
+  ev.record(0);
+  Source src(data, n, (int)d, dtype);
+  std::unique_ptr<lb2_index> ix = make_index(IndexKind::RQ, K, d, m, dtype);
+  ix->nbits = (int)params->num_bits;
+  const int cd = ix->code_dim();
+  std::vector<double> loss;
+  std::vector<uint32_t> iters;
+  // 1. IVF: the same stage as lb2_ivfflat_build (same sample, seed, training)
+  train_ivf_stage(src, ix.get(), params->ivf, params->seed, 1, &loss, &iters);
+  ev.record(1);
+  // 2. RabitQuantizer::new (bq/builder.rs:52-70): the rotation, from seed + 1
+  {
+    TagScope tg("rq_train");
+    ix->rq_rot.alloc((size_t)cd * cd);
+    rq_rotation_f32(cd, params->seed + 1, ix->rq_rot.p);
+  }
+  ev.record(2);
+  // 3. transform (ivf.rs:281-328) of every row
+  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
+  DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1)), codes(std::max<uint64_t>(1, n * (cd / 8)));
+  DevBuf<float> add(std::max<uint64_t>(n, 1)), scale(std::max<uint64_t>(n, 1)), cnorm;
+  {
+    TagScope tg("transform");
+    rq_centroid_norms(m, ix->centroids.p, K, (int)d, cnorm);
+    RqWork w;
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      rq_transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, ix->rq_rot.p, ix->nbits,
+                         cnorm.p, w, part.p + r0, valid.p + r0, codes.p + r0 * (cd / 8), add.p + r0, scale.p + r0);
+    });
+  }
+  ev.record(3);
+  {
+    TagScope tg("group");
+    InArg<uint64_t> rid(row_ids, n);
+    index_load_dev(ix.get(), part.p, codes.p, rid.get(), n, valid.p, add.p, scale.p);
+  }
+  ev.record(4);
+  sync_stream();
+  fill_stats(stats, ev, loss, iters);
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype,
+                           lb2_metric metric, const lb2_ivfpq_build_params* params,
+                           const uint64_t* row_ids, lb2_index** out, lb2_build_stats* stats) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(data && params && out, "null argument");
+  const int m = metric_of(metric);
+  const int K = params->num_partitions, M = params->pq.num_sub_vectors;
+  const uint64_t nranks = current_comm() ? current_comm()->nranks : 1;  // sharded build: this rank's rows
+  LB2_REQUIRE(K > 0 && (nranks > 1 || n >= (uint64_t)K), "KMeans: can not train %d centroids with %llu vectors", K,
+              (unsigned long long)n);
+  check_pq_shape(d, M, params->pq.num_bits, PqUse::ENCODE);
+  const int nbits = (int)params->pq.num_bits;
+  EventSet ev(5);
+  ev.record(0);
+
+  // Staging (class Source).  Device rows: used in place.  Host rows: both training samples (<= K * 256 and
+  // 65 536 rows) are gathered straight out of the caller's memory (zero-copy reads over PCIe when it is pinned),
+  // then the matrix is copied ONCE, in its own element type, on a second stream while both trainings run; the
+  // per-row pass waits for it and converts one chunk of rows at a time.  A matrix too large for that is streamed
+  // chunk by chunk during the per-row pass instead (double buffered).  No whole-matrix f32 copy exists.
+  // (declared before `src`: on an error path ~Source waits for the copy stream, which may still be writing the PQ
+  // sample, before these buffers go back to the pool)
+  DevBuf<float> sample_ivf, sample_pq;
+  Source src(data, n, (int)d, dtype);
+
+  std::unique_ptr<lb2_index> ix = make_index(IndexKind::PQ, K, d, m, dtype);
+  ix->M = M;
+  ix->nbits = nbits;
+  ix->codebook.alloc(ix->codebook_len());
+  std::vector<double> ivf_loss;
+  std::vector<uint32_t> ivf_iters, pq_iters;
+  // 0. both training samples are gathered first (IVF: K*sample_rate rows, rust/lance/src/index/
+  //    vector/ivf.rs:1237-1241; PQ: 256*2^nbits rows, builder.rs:410-421), normalised for cosine; rows that are
+  //    not finite are dropped from them (builder.rs:436); then the bulk copy starts
+  const uint64_t s_pq0 = std::min<uint64_t>(n, (params->pq.sample_rate * ((uint64_t)1 << nbits) + nranks - 1) / nranks);
+  uint64_t s_ivf = 0, s_pq = 0;
+  std::vector<uint64_t> rows_pq;
+  bool pq_deferred = false;
+  // LB2_TRACE_BUILD=1: host wall-clock stamps of the staging steps on stderr (diagnostics; adds synchronisations)
+  static const bool trace = getenv("LB2_TRACE_BUILD") && *getenv("LB2_TRACE_BUILD");
+  const auto tr0 = std::chrono::steady_clock::now();
+  auto stamp = [&](const char* what) {
+    if (!trace) return;
+    sync_stream();
+    fprintf(stderr, "[lb2 build] %-22s +%.3f ms\n", what,
+            std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tr0).count());
+  };
+  {
+    std::vector<uint64_t> rows = ivf_sample_rows(n, K, params->ivf, params->seed, nranks);
+    stamp("sample_rows(ivf)");
+    s_ivf = gather_finite_sample(src, rows, m == METRIC_COSINE, sample_ivf);
+    stamp("gather(ivf sample)");
+    rows_pq = sample_rows(n, s_pq0, params->seed + 1);
+    // the PQ sample is not needed before the IVF model exists: from pinned f32 rows it is gathered on the copy
+    // stream (in front of the bulk copy) while the IVF training runs; otherwise here
+    if (m != METRIC_COSINE && !trace && !rows_pq.empty()) {
+      sample_pq.alloc(rows_pq.size() * (uint64_t)d);
+      pq_deferred = src.gather_f32_async(rows_pq, sample_pq.p);
+    }
+    if (!pq_deferred) {
+      s_pq = gather_finite_sample(src, rows_pq, m == METRIC_COSINE, sample_pq);
+      stamp("gather(pq sample)");
+    }
+  }
+  src.start_resident_copy();
+  if (trace) fprintf(stderr, "[lb2 build] %-22s +%.3f ms (host, no sync)\n", "bulk copy issued",
+                     std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tr0).count());
+  // 1. IVF
+  train_ivf_model(sample_ivf.p, s_ivf, ix.get(), params->ivf, nranks, &ivf_loss, &ivf_iters);
+  stamp("ivf trained");
+  if (pq_deferred) {
+    if (src.finish_async_sample()) {
+      s_pq = rows_pq.size();
+    } else {  // rare: some sampled rows are not finite -> the synchronous path drops them and gathers again
+      s_pq = gather_finite_sample(src, rows_pq, false, sample_pq);
+    }
+  }
+  sample_ivf.release();
+  ev.record(1);
+  // 2. PQ: residuals of its sample w.r.t. the IVF centroids (builder.rs:439-450)
+  {
+    TagScope tg("pq_train");
+    if (m != METRIC_DOT && s_pq) {
+      DevBuf<uint32_t> part(s_pq);
+      assign_f32(sample_pq.p, s_pq, d, ix->centroids.p, K, METRIC_L2, nullptr, part.p, nullptr, nullptr, nullptr);
+      LB2_LAUNCH("residual", residual_kernel, cdiv(s_pq * d, 256), 256, 0, sample_pq.p, ix->centroids.p,
+                 part.p, s_pq, (int)d, sample_pq.p);
+    }
+    VecIn cb_init(params->pq.codebook, ix->codebook_len(), model_dtype(dtype));
+    lb2_pq_params pqp = params->pq;
+    pqp.codebook = cb_init.get();
+    // always L2 k-means (builder.rs:460: Q::build(&training_data, DistanceType::L2, ..)); for a dot index
+    // the sample is the raw vectors (no residual), for L2 / cosine the residuals computed above
+    pq_train_dev(sample_pq.p, s_pq, d, METRIC_L2, &pqp, ix->codebook.p, &pq_iters);
+    round_model(ix->codebook.p, ix->codebook_len(), dtype);
+  }
+  sample_pq.release();
+  ev.record(2);
+  // 3. transform every row (lance-index/src/vector/ivf.rs:357: partition -> residual -> PQ), chunk by chunk
+  const size_t cw = ix->row_bytes();
+  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
+  DevBuf<uint8_t> codes(std::max<uint64_t>(1, (size_t)n * cw)), valid(std::max<uint64_t>(n, 1));
+  {
+    TagScope tg("transform");
+    DevBuf<float> normbuf;
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, ix->codebook.p, M, nbits, normbuf,
+                      part.p + r0, codes.p + r0 * cw, valid.p + r0);
+    });
+  }
+  ev.record(3);
+  {
+    // 4. group the kept rows by partition (shuffle + build_partitions, builder.rs:501-937); rows the
+    //    transform marked invalid are dropped, as KeepFiniteVectors does (transform.rs:112-159)
+    TagScope tg("group");
+    InArg<uint64_t> rid(row_ids, n);
+    index_load_dev(ix.get(), part.p, codes.p, rid.get(), n, valid.p);
+  }
+  ev.record(4);
+  sync_stream();
+  fill_stats(stats, ev, ivf_loss, ivf_iters, pq_iters);
+  *out = ix.release();
+  LB2_API_END
+}
+
+}  // extern "C"

@@ -1,0 +1,24 @@
+// build.cuh -- the parts of the index builds that the stand-alone primitives and the index handle share
+#pragma once
+#include "staging.cuh"
+
+namespace lb2 {
+
+// x - centroid of its partition, row by row (x and out may alias: the in-place residual of the PQ training sample)
+__global__ void residual_kernel(const float* x, const float* __restrict__ cent, const uint32_t* __restrict__ part,
+                                uint64_t n, int d, float* out);
+
+// What a ProductQuantizer of M sub-vectors and num_bits codes needs: M divides d (pq/utils.rs:25) and num_bits is 4
+// or 8 (INDEX and ENCODE: M is even for 4-bit codes, pq.rs:132-140; ENCODE: the sub-vector width is one the encode
+// kernels implement -> LB2_UNSUPPORTED)
+enum class PqUse { TRAIN, INDEX, ENCODE };
+void check_pq_shape(uint32_t d, uint32_t M, uint32_t nbits, PqUse use);
+void check_redos(uint32_t redos, float balance_factor);
+void pq_train_dev(const float* data, uint64_t n, int d, int metric, const lb2_pq_params* p, float* codebook,
+                  std::vector<uint32_t>* iters);
+void pq_encode_any(const float* x, uint64_t n, int d, int M, int ds, const float* codebook, int metric,
+                   const float* cent, const uint32_t* part, const uint8_t* row_valid, int nbits, uint8_t* codes);
+void sq_check_dim(uint32_t d);
+void rq_check(uint32_t d, lb2_dtype dtype, uint32_t num_bits);
+
+}  // namespace lb2

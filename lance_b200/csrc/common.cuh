@@ -236,6 +236,16 @@ struct TagScope {
 
 inline unsigned cdiv(uint64_t a, uint64_t b) { return (unsigned)((a + b - 1) / b); }
 
+// v is one of the n ascending values of a
+__device__ __forceinline__ bool sorted_contains(const uint64_t* __restrict__ a, uint64_t n, uint64_t v) {
+  uint64_t lo = 0, hi = n;
+  while (lo < hi) {
+    const uint64_t mid = (lo + hi) >> 1;
+    if (a[mid] < v) lo = mid + 1; else hi = mid;
+  }
+  return lo < n && a[lo] == v;
+}
+
 // our reproducible rng (the reference's is unseeded: kmeans.rs:181,645)
 struct SplitMix64 {
   uint64_t s;

@@ -1,0 +1,905 @@
+// index.cu -- the device-resident index: creation, loads and exports of every kind, the grouping of rows by
+// partition, search dispatch, incremental update and the partition exchange of a row-sharded index.
+#include <algorithm>
+#include <memory>
+
+#include "build.cuh"
+#include "comm.cuh"
+#include "index.cuh"
+#include "kmeans.cuh"
+#include "search.cuh"
+#include "sq.cuh"
+
+namespace lb2 {
+
+std::unique_ptr<lb2_index> make_index(IndexKind kind, uint32_t K, uint32_t d, int metric, lb2_dtype dtype) {
+  std::unique_ptr<lb2_index> ix(new lb2_index());
+  ix->kind = kind; ix->K = K; ix->d = d; ix->metric = metric; ix->dtype = dtype;
+  ix->centroids.alloc((size_t)K * d);
+  return ix;
+}
+
+// an empty index with the caller's centroids (in the model type of `dtype`)
+static std::unique_ptr<lb2_index> index_with_centroids(IndexKind kind, const void* centroids, uint32_t k, uint32_t d,
+                                                       lb2_dtype dtype, lb2_metric metric) {
+  ctx();
+  std::unique_ptr<lb2_index> ix = make_index(kind, k, d, metric_of(metric), dtype);
+  {
+    VecIn c(centroids, (size_t)k * d, model_dtype(dtype));
+    d2d(ix->centroids.p, c.get(), (size_t)k * d);
+    sync_stream();
+  }
+  ix->part_offsets.alloc(k + 1);
+  ix->part_offsets.zero();
+  sync_stream();
+  return ix;
+}
+
+// the model of `from` in `to`, an index of the same kind from make_index: the centroids (or `new_centroids`, in the
+// model type of the index, when given), M, nbits, and the codebook, SQ bounds or RQ rotation as the kind has them
+static void copy_model(const lb2_index* from, lb2_index* to, const void* new_centroids = nullptr) {
+  const size_t kd = (size_t)to->K * to->d;
+  if (new_centroids) {
+    VecIn c(new_centroids, kd, model_dtype(to->dtype));
+    d2d(to->centroids.p, c.get(), kd);
+    sync_stream();
+  } else {
+    d2d(to->centroids.p, from->centroids.p, kd);
+  }
+  to->M = from->M;
+  to->nbits = from->nbits;
+  switch (from->kind) {
+    case IndexKind::PQ:
+      to->codebook.alloc(from->codebook_len());
+      d2d(to->codebook.p, from->codebook.p, from->codebook_len());
+      break;
+    case IndexKind::SQ:
+      to->sq_lower = from->sq_lower;
+      to->sq_upper = from->sq_upper;
+      break;
+    case IndexKind::RQ:
+      to->rq_rot.alloc((size_t)from->code_dim() * from->code_dim());
+      d2d(to->rq_rot.p, from->rq_rot.p, (size_t)from->code_dim() * from->code_dim());
+      break;
+    case IndexKind::FLAT:
+      break;
+  }
+}
+
+// largest partition id of a caller-supplied id column (range check before it indexes device memory)
+__global__ void max_u32_kernel(const uint32_t* __restrict__ v, uint64_t n, uint32_t* __restrict__ out) {
+  uint32_t m = 0;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+    m = max(m, v[i]);
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if ((threadIdx.x & 31) == 0 && m) atomicMax(out, m);
+}
+
+void check_part_ids(const uint32_t* part_ids, uint64_t n, uint32_t K, const char* what) {
+  if (n == 0) return;
+  DevBuf<uint32_t> mx(1);
+  mx.zero();
+  LB2_LAUNCH("check_part_ids", max_u32_kernel, (unsigned)std::min<uint64_t>(cdiv(n, 1024), 1024), 256, 0, part_ids, n, mx.p);
+  uint32_t h = 0;
+  d2h(&h, mx.p, 1);
+  sync_stream();
+  if (h >= K) fail(LB2_INVALID_ARG, "%s: partition id %u out of range (the index has %u partitions)", what, h, K);
+}
+
+__global__ void widen_offsets_kernel(const uint32_t* __restrict__ off32, int K,
+                                     uint64_t* __restrict__ off64) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i <= K) off64[i] = off32[i];
+}
+
+// stable grouping of the kept rows by partition; rows with valid[r] == 0 (KeepFiniteVectors,
+// transform.rs:112-159: NaN / Inf rows, zero vectors under cosine) never enter the index
+static uint64_t member_sort_index(MemberSort& ms, lb2_index* ix, const uint32_t* part_ids, const uint8_t* valid,
+                                  uint64_t n) {
+  LB2_REQUIRE(n < 0xffffffffull, "more than 2^32-1 rows per index shard");
+  ms.run(part_ids, valid, n, ix->K, 1, nullptr);
+  ix->part_offsets.alloc(ix->K + 1);
+  if (n == 0) {
+    ix->part_offsets.zero();
+    return 0;
+  }
+  LB2_LAUNCH("widen_offsets", widen_offsets_kernel, cdiv(ix->K + 1, 256), 256, 0, ms.offsets.p,
+             ix->K, ix->part_offsets.p);
+  uint32_t kept = 0;
+  d2h(&kept, ms.offsets.p + ix->K, 1);
+  sync_stream();
+  return kept;
+}
+
+// the conflict-free scan's skewed copy of the codes, for the shapes that have one
+static void build_skew(lb2_index* ix) {
+  if (ix->n && skew_layout_applies(ix->M, ix->d, ix->nbits)) {
+    ix->slab_off.alloc(ix->K + 1);
+    ix->codes_skew.alloc(skew_bytes_bound(ix->n, ix->K));
+    build_skew_codes(ix->part_offsets.p, ix->K, ix->codes.p, ix->n, ix->slab_off.p, ix->codes_skew.p);
+  } else {
+    ix->slab_off.release();
+    ix->codes_skew.release();
+  }
+}
+
+__global__ void group_kernel(const uint32_t* __restrict__ members, uint64_t n, int M,
+                             const uint8_t* __restrict__ codes, const uint64_t* __restrict__ row_ids,
+                             uint8_t* __restrict__ codes_out, uint64_t* __restrict__ row_ids_out) {
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n) return;
+  const uint32_t src = members[g];
+  row_ids_out[g] = row_ids ? row_ids[src] : (uint64_t)src;
+  for (int m = 0; m < M; ++m) codes_out[g * M + m] = codes[(size_t)src * M + m];
+}
+
+__global__ void gather_f32_kernel(const uint32_t* __restrict__ members, uint64_t n, const float* __restrict__ src,
+                                  float* __restrict__ dst) {
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < n) dst[g] = src[members[g]];
+}
+
+void index_load_dev(lb2_index* ix, const uint32_t* part_ids, const uint8_t* codes, const uint64_t* row_ids,
+                    uint64_t n, const uint8_t* valid, const float* rq_add, const float* rq_scale) {
+  MemberSort ms;
+  const uint64_t kept = member_sort_index(ms, ix, part_ids, valid, n);
+  const int cb = (int)ix->row_bytes();
+  ix->codes.alloc(std::max<uint64_t>(1, kept * cb));
+  ix->row_ids.alloc(std::max<uint64_t>(1, kept));
+  if (kept)
+    LB2_LAUNCH("group_by_partition", group_kernel, cdiv(kept, 256), 256, 0, ms.members.p, kept, cb, codes, row_ids,
+               ix->codes.p, ix->row_ids.p);
+  if (ix->kind == IndexKind::RQ) {
+    ix->rq_add.alloc(std::max<uint64_t>(1, kept));
+    ix->rq_scale.alloc(std::max<uint64_t>(1, kept));
+    if (kept) {
+      LB2_LAUNCH("group_by_partition", gather_f32_kernel, cdiv(kept, 256), 256, 0, ms.members.p, kept, rq_add, ix->rq_add.p);
+      LB2_LAUNCH("group_by_partition", gather_f32_kernel, cdiv(kept, 256), 256, 0, ms.members.p, kept, rq_scale,
+                 ix->rq_scale.p);
+    }
+  }
+  ix->n = kept;
+  build_skew(ix);
+  sync_stream();
+}
+
+__global__ void copy_row_ids_kernel(const uint32_t* __restrict__ members, uint64_t n, const uint64_t* __restrict__ row_ids,
+                                    uint64_t* __restrict__ out) {
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < n) out[g] = row_ids ? row_ids[members[g]] : (uint64_t)members[g];
+}
+__global__ void members_to_u64_kernel(const uint32_t* __restrict__ members, uint64_t n, uint64_t* __restrict__ out) {
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g < n) out[g] = members[g];
+}
+
+// IVF_FLAT storage: the kept rows grouped by partition (stable), normalised when the metric is cosine
+// (IvfTransformer::new_flat, lance-index/src/vector/ivf.rs:149-185), written in the index's element type.
+// Rows are pulled from the caller's matrix in chunks of output positions (never a whole-matrix f32 copy).
+// rows `members[i]` of a matrix in its own element type -> consecutive rows (16 bytes per thread)
+__global__ void gather_rows_native_kernel(const uint4* __restrict__ src, uint32_t vec_per_row,
+                                          const uint32_t* __restrict__ members, uint64_t kept, uint4* __restrict__ dst) {
+  const uint64_t total = kept * vec_per_row;
+  for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t i = g / vec_per_row;
+    const uint32_t v = (uint32_t)(g % vec_per_row);
+    dst[g] = src[(uint64_t)members[i] * vec_per_row + v];
+  }
+}
+
+void index_load_flat_src(lb2_index* ix, const uint32_t* part_ids, Source& src, const uint64_t* row_ids,
+                         const uint8_t* valid, bool normalize) {
+  const uint64_t n = src.n();
+  MemberSort ms;
+  const uint64_t kept = member_sort_index(ms, ix, part_ids, valid, n);
+  const lb2_dtype vdt = ix->vdtype();
+  const size_t rb = ix->row_bytes();
+  ix->vectors.alloc(std::max<size_t>(1, kept * rb));
+  ix->row_ids.alloc(std::max<uint64_t>(1, kept));
+  ix->n = kept;
+  if (!kept) { sync_stream(); return; }
+  LB2_LAUNCH("group_row_ids", copy_row_ids_kernel, cdiv(kept, 256), 256, 0, ms.members.p, kept, row_ids, ix->row_ids.p);
+  const void* nat = src.native_device();
+  if (!nat) fail(LB2_OOM, "IVF_FLAT keeps a copy of the vectors: the %llu x %d matrix must fit in device memory",
+                 (unsigned long long)n, ix->d);
+  const int d = ix->d;
+  if (!normalize && vdt == src.dtype() && rb % 16 == 0 && (reinterpret_cast<uintptr_t>(nat) & 15) == 0) {
+    // stored type == column type: one pass, no f32 round trip (a C4 shard: 2 x 19 GB of bf16 at HBM speed)
+    const uint32_t vpr = (uint32_t)(rb / 16);
+    LB2_LAUNCH("group_vectors", gather_rows_native_kernel, (unsigned)std::min<uint64_t>(cdiv(kept * vpr, 256), 64ull * ctx().num_sms),
+               256, 0, static_cast<const uint4*>(nat), vpr, ms.members.p, kept, reinterpret_cast<uint4*>(ix->vectors.p));
+    sync_stream();
+    return;
+  }
+  const uint64_t chunk = src.rows_per_chunk();
+  DevBuf<uint64_t> rows64(std::min(chunk, kept));
+  DevBuf<float> tmp, tmp2;
+  const bool direct = vdt == LB2_F32 && !normalize;
+  if (!direct) tmp.alloc(std::min(chunk, kept) * d);
+  if (normalize && vdt != LB2_F32) tmp2.alloc(std::min(chunk, kept) * d);
+  for (uint64_t p0 = 0; p0 < kept; p0 += chunk) {
+    const uint64_t rows = std::min(chunk, kept - p0);
+    LB2_LAUNCH("group_vectors", members_to_u64_kernel, cdiv(rows, 256), 256, 0, ms.members.p + p0, rows, rows64.p);
+    uint8_t* dst = ix->vectors.p + p0 * rb;
+    float* g = direct ? reinterpret_cast<float*>(dst) : tmp.p;
+    LB2_LAUNCH("group_vectors", gather_rows_typed_kernel, cdiv(rows * d, 256), 256, 0, nat, (int)src.dtype(), rows64.p, rows, d, g);
+    if (normalize) {
+      float* o = vdt == LB2_F32 ? reinterpret_cast<float*>(dst) : tmp2.p;
+      normalize_rows(g, rows, d, o);
+      g = o;
+    }
+    if (vdt != LB2_F32)
+      LB2_LAUNCH("convert_from_f32", from_f32_kernel, cdiv(rows * d, 256), 256, 0, g, (int)vdt, (size_t)rows * d, (void*)dst);
+  }
+  sync_stream();
+}
+
+// the code loads of IVF_PQ, IVF_SQ and IVF_RQ (add / scale: IVF_RQ's factors)
+static void load_codes(lb2_index* index, const uint32_t* part_ids, const uint8_t* codes, const uint64_t* row_ids,
+                       uint64_t n, const char* what, const float* add = nullptr, const float* scale = nullptr) {
+  InArg<uint32_t> p(part_ids, n);
+  InArg<uint8_t> c(codes, (size_t)n * index->row_bytes());
+  InArg<float> a(add, n), s(scale, n);
+  InArg<uint64_t> r(row_ids, n);
+  check_part_ids(p.get(), n, (uint32_t)index->K, what);
+  index_load_dev(index, p.get(), c.get(), r.get(), n, nullptr, a.get(), s.get());
+}
+
+// what every kind exports: centroids, partition offsets, the row payload and the row ids (each output nullable, host
+// or device memory); the caller adds its kind's model and synchronises
+static void export_common(const lb2_index* index, void* centroids_out, uint64_t* part_offsets_out, void* payload_out,
+                          uint64_t* row_ids_out) {
+  cudaStream_t s = ctx().stream;
+  if (centroids_out)
+    LB2_CUDA(cudaMemcpyAsync(centroids_out, index->centroids.p, sizeof(float) * index->K * index->d, cudaMemcpyDefault, s));
+  if (part_offsets_out)
+    LB2_CUDA(cudaMemcpyAsync(part_offsets_out, index->part_offsets.p, sizeof(uint64_t) * (index->K + 1), cudaMemcpyDefault, s));
+  if (payload_out && index->n)
+    LB2_CUDA(cudaMemcpyAsync(payload_out, index->payload().p, index->n * index->row_bytes(), cudaMemcpyDefault, s));
+  if (row_ids_out && index->n)
+    LB2_CUDA(cudaMemcpyAsync(row_ids_out, index->row_ids.p, sizeof(uint64_t) * index->n, cudaMemcpyDefault, s));
+}
+
+// one implementation behind every lb2_index_search* (pr: the probe rule of lb2_index_search_probed)
+static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq, const lb2_search_params& sp,
+                              uint64_t* row_ids_out, float* dists_out, uint32_t* counts_out, ProbeRule* pr = nullptr) {
+  const uint32_t k = sp.k, nprobes = sp.nprobes;
+  LB2_REQUIRE(index && k > 0 && (nprobes > 0 || pr), "bad argument");
+  const bool refine = sp.refine_factor > 0 && sp.refine_vectors != nullptr;
+  const uint64_t kc = refine ? (uint64_t)k * sp.refine_factor : k;
+  if (kc > 1024) fail(LB2_UNSUPPORTED, "k * refine_factor = %llu > 1024 is not implemented", (unsigned long long)kc);
+  const int d = index->d;
+  VecIn q(queries, (size_t)nq * d, index->dtype);
+  const float* qp = q.get();
+  DevBuf<float> qn;
+  if (index->metric == METRIC_COSINE) {  // knn.rs:497-499
+    qn.alloc((size_t)nq * d);
+    normalize_rows(qp, nq, d, qn.p);
+    qp = qn.p;
+  }
+  InArg<uint64_t> allow(sp.allow_bitmap, sp.allow_bitmap ? (size_t)((index->n + 63) / 64) : 0);
+  OutArg<uint64_t> oi(row_ids_out, (size_t)nq * k);
+  OutArg<float> od(dists_out, (size_t)nq * k);
+  OutArg<uint32_t> oc(counts_out, nq);
+  DevBuf<uint64_t> cid;
+  DevBuf<float> cdist;
+  DevBuf<uint32_t> ccnt;
+  if (refine) {
+    cid.alloc((size_t)nq * kc);
+    cdist.alloc((size_t)nq * kc);
+    ccnt.alloc(nq);
+  }
+  uint64_t* si = refine ? cid.p : oi.get();
+  float* sd = refine ? cdist.p : od.get();
+  uint32_t* sc = refine ? ccnt.p : oc.get();
+  TagScope tg("search");
+  const ScanFilter flt = make_filter(sp.allow_bitmap ? allow.get() : nullptr, sp.has_lower_bound != 0, sp.lower_bound,
+                                    sp.has_upper_bound != 0, sp.upper_bound);
+  DevBuf<uint8_t> qcodes;
+  switch (index->kind) {
+    case IndexKind::FLAT:
+      ivfflat_search_f32(index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->vectors.p,
+                         (int)index->vdtype(), index->row_ids.p, qp, nq, (int)kc, nprobes, si, sd, sc, flt, pr);
+      break;
+    case IndexKind::RQ:
+      // the (normalised) query's residual to each probed centroid is rotated (v2.rs:316-332, bq/storage.rs:407-445)
+      ivfrq_search_f32(index->centroids.p, index->K, d, index->metric, index->rq_rot.p, index->code_dim(),
+                       index->part_offsets.p, index->codes.p, index->rq_add.p, index->rq_scale.p, index->row_ids.p, qp,
+                       nq, (int)kc, nprobes, si, sd, sc, flt, pr);
+      break;
+    case IndexKind::SQ: {
+      // the (normalised) query is encoded with the index's bounds, not turned into a residual (sq/storage.rs:404-430)
+      qcodes.alloc(std::max<uint64_t>(1, nq * d));
+      sq_encode_f32(qp, nq * d, index->sq_lower, index->sq_upper, qcodes.p);
+      const float rf = (float)(index->sq_upper - index->sq_lower);  // inverse_scalar_dist (sq.rs:279-287)
+      ivfsq_search_f32(index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->codes.p,
+                       index->row_ids.p, rf * rf, qp, qcodes.p, nq, (int)kc, nprobes, si, sd, sc, flt, pr);
+      break;
+    }
+    case IndexKind::PQ:
+      ivfpq_search_f32(index->centroids.p, index->K, d, index->metric, index->codebook.p, index->M, index->nbits,
+                       index->part_offsets.p, index->codes.p, index->row_ids.p, qp, nq, (int)kc, nprobes, si, sd,
+                       sc, flt, index->slab_off.p, index->codes_skew.p, pr);
+      break;
+  }
+  if (refine) {
+    // exact re-rank with the true metric on the ORIGINAL (un-normalised) query, as flat_knn does; the
+    // plan then filters `_distance >= lower AND _distance < upper` on the exact distances (scanner.rs:3342-3377)
+    InArg<uint8_t> v(sp.refine_vectors, (size_t)sp.num_vectors * d * dtype_size(index->dtype));  // raw column, native type
+    refine_f32(q.get(), nq, d, index->metric, v.get(), (int)index->dtype, sp.num_vectors, cid.p, ccnt.p, (int)kc, (int)k,
+               oi.get(), od.get(), oc.get(), sp.has_lower_bound != 0, sp.lower_bound, sp.has_upper_bound != 0,
+               sp.upper_bound);
+  }
+  oi.commit(); od.commit(); oc.commit();
+  if (!ctx().async_call) sync_stream();
+}
+
+// ---- partition ownership: device all-to-all (SURVEY 8e "partition build", 8f-4) ---------------------------------
+// The reference groups the transformed rows by partition with a disk shuffler on the host
+// (rust/lance-index/src/vector/v3/shuffler.rs:105).  For a build sharded by rows over G GPUs the same grouping
+// is one exchange over NVLink: rank g becomes the owner of every partition p with p % G == g.
+
+// the last p < n with offsets[p] <= i (offsets ascending from offsets[0] <= i)
+__device__ __forceinline__ int segment_of(const uint64_t* __restrict__ offsets, int n, uint64_t i) {
+  int lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (offsets[mid] <= i) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
+// (these kernels have C linkage: their symbols are the bare names)
+extern "C" {
+// row i of the shard (storage order) -> slot in the send buffer: rows are grouped by destination rank, inside a
+// destination by partition, inside a partition in storage order
+__global__ void repart_pack_kernel(const uint64_t* __restrict__ part_offsets, int K, uint64_t n, int row_bytes,
+                                   const uint64_t* __restrict__ send_base /*[K]*/, const uint8_t* __restrict__ payload,
+                                   const uint64_t* __restrict__ row_ids, uint8_t* __restrict__ payload_out,
+                                   uint64_t* __restrict__ row_ids_out) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int p = segment_of(part_offsets, K, i);
+  const uint64_t dst = send_base[p] + (i - part_offsets[p]);
+  row_ids_out[dst] = row_ids[i];
+  const uint8_t* src = payload + i * (uint64_t)row_bytes;
+  uint8_t* o = payload_out + dst * (uint64_t)row_bytes;
+  if ((row_bytes & 15) == 0) {
+    for (int b = 0; b < row_bytes; b += 16) *reinterpret_cast<uint4*>(o + b) = *reinterpret_cast<const uint4*>(src + b);
+  } else {
+    for (int b = 0; b < row_bytes; ++b) o[b] = src[b];
+  }
+}
+// received row j of source rank r (rows of my partitions in ascending partition order) -> final storage position
+__global__ void repart_unpack_kernel(const uint64_t* __restrict__ seg_prefix /*[nown + 1] rows of r before owned part i*/,
+                                     const uint64_t* __restrict__ seg_dst /*[nown] final position of r's first row*/,
+                                     int nown, uint64_t nrows, int row_bytes, const uint8_t* __restrict__ payload,
+                                     const uint64_t* __restrict__ row_ids, uint8_t* __restrict__ payload_out,
+                                     uint64_t* __restrict__ row_ids_out) {
+  const uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= nrows) return;
+  const int s = segment_of(seg_prefix, nown, j);
+  const uint64_t dst = seg_dst[s] + (j - seg_prefix[s]);
+  row_ids_out[dst] = row_ids[j];
+  const uint8_t* src = payload + j * (uint64_t)row_bytes;
+  uint8_t* o = payload_out + dst * (uint64_t)row_bytes;
+  if ((row_bytes & 15) == 0) {
+    for (int b = 0; b < row_bytes; b += 16) *reinterpret_cast<uint4*>(o + b) = *reinterpret_cast<const uint4*>(src + b);
+  } else {
+    for (int b = 0; b < row_bytes; ++b) o[b] = src[b];
+  }
+}
+
+// ---- incremental update of an IVF_PQ index: the data path of optimize / split / join (SURVEY 8f-4) --------------
+// The reference turns an optimize step into per-partition AssignOp::Add / AssignOp::Remove lists against a new
+// centroid set (rust/lance/src/index/vector/builder.rs:1219-1333 split, :1476-1530 join, :1534-1650
+// build_assign_batch) and merges them with the existing partitions when it writes the index.  The decisions --
+// which partition to split or join, which rows to move -- stay on the host (they need the dataset); this entry
+// point is the merge: old rows keep their codes, follow `part_map`, removed row ids are dropped, added rows join
+// the end of their partitions.
+__global__ void update_old_rows_kernel(const uint64_t* __restrict__ part_offsets, int K, uint64_t n,
+                                       const uint32_t* __restrict__ part_map /*nullable*/,
+                                       const uint64_t* __restrict__ row_ids, const uint64_t* __restrict__ removed,
+                                       uint64_t n_removed, uint32_t new_k, uint32_t* __restrict__ part_out,
+                                       uint8_t* __restrict__ valid_out, uint32_t* __restrict__ bad) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int p = segment_of(part_offsets, K, i);
+  const uint32_t np_ = part_map ? part_map[p] : (uint32_t)p;
+  bool keep = np_ != 0xffffffffu;
+  if (keep && np_ >= new_k) { atomicMax(bad, np_); keep = false; }
+  if (keep && n_removed) keep = !sorted_contains(removed, n_removed, row_ids[i]);
+  part_out[i] = keep ? np_ : 0u;
+  valid_out[i] = keep ? 1 : 0;
+}
+__global__ void fill_u8_kernel(uint8_t* __restrict__ p, uint64_t n, uint8_t v) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) p[i] = v;
+}
+
+}  // extern "C"
+
+// row-major codes [n][cw] of one partition -> the reference's storage layout [cw][n] (pq/storage.rs:430-450)
+__global__ void transpose_codes_kernel(const uint8_t* __restrict__ codes, uint64_t n, int cw, uint8_t* __restrict__ out) {
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n * cw) return;
+  const uint64_t j = g % n;
+  const int m = (int)(g / n);
+  out[g] = codes[j * cw + m];
+}
+
+}  // namespace lb2
+
+using namespace lb2;
+
+extern "C" {
+
+lb2_status lb2_index_create(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype,
+                            lb2_metric metric, const void* codebook, uint32_t num_sub_vectors,
+                            uint32_t num_bits, lb2_index** out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(out && centroids && codebook, "null argument");
+  check_pq_shape(d, num_sub_vectors, num_bits, PqUse::INDEX);
+  std::unique_ptr<lb2_index> ix = index_with_centroids(IndexKind::PQ, centroids, k, d, dtype, metric);
+  ix->M = num_sub_vectors;
+  ix->nbits = num_bits;
+  ix->codebook.alloc(ix->codebook_len());
+  {
+    VecIn cb(codebook, ix->codebook_len(), model_dtype(dtype));
+    d2d(ix->codebook.p, cb.get(), ix->codebook_len());
+    sync_stream();
+  }
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_index_create_flat(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype,
+                                 lb2_metric metric, lb2_index** out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(out && centroids, "null argument");
+  *out = index_with_centroids(IndexKind::FLAT, centroids, k, d, dtype, metric).release();
+  LB2_API_END
+}
+
+lb2_status lb2_index_create_sq(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                               double lower, double upper, lb2_index** out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(out && centroids, "null argument");
+  sq_check_dim(d);
+  LB2_REQUIRE(std::isfinite(lower) && std::isfinite(upper) && lower <= upper,
+              "IVF_SQ: the bounds must be finite with lower <= upper, got [%g, %g]", lower, upper);
+  std::unique_ptr<lb2_index> ix = index_with_centroids(IndexKind::SQ, centroids, k, d, dtype, metric);
+  ix->nbits = 8;
+  ix->sq_lower = lower;
+  ix->sq_upper = upper;
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_index_create_rq(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                               const void* rotation, uint32_t num_bits, lb2_index** out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(out && centroids && rotation, "null argument");
+  rq_check(d, dtype, num_bits);
+  std::unique_ptr<lb2_index> ix = index_with_centroids(IndexKind::RQ, centroids, k, d, dtype, metric);
+  ix->nbits = (int)num_bits;
+  const size_t cd = ix->code_dim();
+  ix->rq_rot.alloc(cd * cd);
+  VecIn r(rotation, cd * cd, dtype);
+  d2d(ix->rq_rot.p, r.get(), cd * cd);
+  ix->rq_add.alloc(1);
+  ix->rq_scale.alloc(1);
+  sync_stream();
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_index_load(lb2_index* index, const uint32_t* part_ids, const uint8_t* codes,
+                          const uint64_t* row_ids, uint64_t n) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == IndexKind::PQ, "not an IVF_PQ index");
+  load_codes(index, part_ids, codes, row_ids, n, "index_load");
+  LB2_API_END
+}
+
+lb2_status lb2_index_load_flat(lb2_index* index, const uint32_t* part_ids, const void* vectors,
+                               const uint64_t* row_ids, uint64_t n) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == IndexKind::FLAT, "not an IVF_FLAT index");
+  LB2_REQUIRE(index->d % 4 == 0, "IVF_FLAT needs a dimension that is a multiple of 4");
+  InArg<uint32_t> p(part_ids, n);
+  InArg<uint64_t> r(row_ids, n);
+  check_part_ids(p.get(), n, (uint32_t)index->K, "index_load_flat");
+  Source src(vectors, n, index->d, index->dtype);
+  src.start_resident_copy();
+  index_load_flat_src(index, p.get(), src, r.get(), nullptr, /*normalize=*/false);
+  LB2_API_END
+}
+
+lb2_status lb2_index_load_sq(lb2_index* index, const uint32_t* part_ids, const uint8_t* codes,
+                             const uint64_t* row_ids, uint64_t n) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == IndexKind::SQ, "not an IVF_SQ index");
+  load_codes(index, part_ids, codes, row_ids, n, "index_load_sq");
+  LB2_API_END
+}
+
+lb2_status lb2_index_load_rq(lb2_index* index, const uint32_t* part_ids, const uint8_t* codes, const float* add_factors,
+                             const float* scale_factors, const uint64_t* row_ids, uint64_t n) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == IndexKind::RQ, "not an IVF_RQ index");
+  LB2_REQUIRE(n == 0 || (part_ids && codes && add_factors && scale_factors), "null argument");
+  load_codes(index, part_ids, codes, row_ids, n, "index_load_rq", add_factors, scale_factors);
+  LB2_API_END
+}
+
+lb2_status lb2_index_export(const lb2_index* index, void* centroids_out, void* codebook_out,
+                            uint64_t* part_offsets_out, uint8_t* codes_out, uint64_t* row_ids_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == IndexKind::PQ, "not an IVF_PQ index");
+  export_common(index, centroids_out, part_offsets_out, codes_out, row_ids_out);
+  if (codebook_out)
+    LB2_CUDA(cudaMemcpyAsync(codebook_out, index->codebook.p, sizeof(float) * index->codebook_len(), cudaMemcpyDefault,
+                             ctx().stream));
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_index_export_flat(const lb2_index* index, void* centroids_out,
+                                 uint64_t* part_offsets_out, void* vectors_out,
+                                 uint64_t* row_ids_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == IndexKind::FLAT, "not an IVF_FLAT index");
+  export_common(index, centroids_out, part_offsets_out, vectors_out, row_ids_out);
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_index_export_sq(const lb2_index* index, void* centroids_out, double* bounds_out,
+                               uint64_t* part_offsets_out, uint8_t* codes_out, uint64_t* row_ids_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == IndexKind::SQ, "not an IVF_SQ index");
+  if (bounds_out) {
+    bounds_out[0] = index->sq_lower;
+    bounds_out[1] = index->sq_upper;
+  }
+  export_common(index, centroids_out, part_offsets_out, codes_out, row_ids_out);
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_index_export_rq(const lb2_index* index, void* centroids_out, void* rotation_out,
+                               uint64_t* part_offsets_out, uint8_t* codes_out, float* add_out, float* scale_out,
+                               uint64_t* row_ids_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == IndexKind::RQ, "not an IVF_RQ index");
+  export_common(index, centroids_out, part_offsets_out, codes_out, row_ids_out);
+  cudaStream_t s = ctx().stream;
+  const size_t cd = index->code_dim(), n = index->n;
+  if (rotation_out)
+    LB2_CUDA(cudaMemcpyAsync(rotation_out, index->rq_rot.p, sizeof(float) * cd * cd, cudaMemcpyDefault, s));
+  if (add_out && n) LB2_CUDA(cudaMemcpyAsync(add_out, index->rq_add.p, sizeof(float) * n, cudaMemcpyDefault, s));
+  if (scale_out && n) LB2_CUDA(cudaMemcpyAsync(scale_out, index->rq_scale.p, sizeof(float) * n, cudaMemcpyDefault, s));
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_index_export_partition(const lb2_index* index, uint32_t partition, uint8_t* codes_transposed_out,
+                                      uint64_t* row_ids_out, uint64_t* num_rows_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == IndexKind::PQ, "not an IVF_PQ index");
+  LB2_REQUIRE(partition < (uint32_t)index->K, "partition %u out of range (the index has %d)", partition, index->K);
+  uint64_t off[2];
+  d2h(off, index->part_offsets.p + partition, 2);
+  sync_stream();
+  const uint64_t np = off[1] - off[0];
+  const int cw = (int)index->row_bytes();
+  if (num_rows_out) *num_rows_out = np;
+  if (np && codes_transposed_out) {
+    OutArg<uint8_t> o(codes_transposed_out, (size_t)np * cw);
+    LB2_LAUNCH("transpose_codes", transpose_codes_kernel, cdiv(np * cw, 256), 256, 0, index->codes.p + off[0] * cw, np, cw, o.get());
+    o.commit();
+  }
+  if (np && row_ids_out)
+    LB2_CUDA(cudaMemcpyAsync(row_ids_out, index->row_ids.p + off[0], sizeof(uint64_t) * np, cudaMemcpyDefault, ctx().stream));
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_index_search(lb2_index* index, const void* queries, uint64_t nq, uint32_t k,
+                            uint32_t nprobes, uint64_t* row_ids_out, float* dists_out,
+                            uint32_t* counts_out) {
+  LB2_API_BEGIN
+  const lb2_search_params sp = {k, nprobes};
+  index_search_impl(index, queries, nq, sp, row_ids_out, dists_out, counts_out);
+  LB2_API_END
+}
+
+lb2_status lb2_index_search_refine(lb2_index* index, const void* vectors, uint64_t num_vectors,
+                                   const void* queries, uint64_t nq, uint32_t k, uint32_t nprobes,
+                                   uint32_t refine_factor, uint64_t* row_ids_out, float* dists_out,
+                                   uint32_t* counts_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(vectors && refine_factor > 0, "bad argument");
+  const lb2_search_params sp = {k, nprobes, refine_factor, vectors, num_vectors};
+  index_search_impl(index, queries, nq, sp, row_ids_out, dists_out, counts_out);
+  LB2_API_END
+}
+
+lb2_status lb2_index_search_ex(lb2_index* index, const void* queries, uint64_t nq,
+                               const lb2_search_params* sp, uint64_t* row_ids_out, float* dists_out,
+                               uint32_t* counts_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(sp, "null search params");
+  LB2_REQUIRE(sp->refine_factor == 0 || sp->refine_vectors, "refine_factor > 0 needs refine_vectors");
+  index_search_impl(index, queries, nq, *sp, row_ids_out, dists_out, counts_out);
+  LB2_API_END
+}
+
+lb2_status lb2_index_search_probed(lb2_index* index, const void* queries, uint64_t nq, const lb2_search_params* sp,
+                                   const lb2_probe_params* pp, uint64_t* row_ids_out, float* dists_out,
+                                   uint32_t* counts_out, uint32_t* nprobes_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(sp && pp && index, "null argument");
+  LB2_REQUIRE(sp->nprobes == 0, "nprobes must be 0: the probe parameters decide the probes");
+  LB2_REQUIRE(sp->refine_factor == 0 || sp->refine_vectors, "refine_factor > 0 needs refine_vectors");
+  LB2_REQUIRE(pp->minimum_nprobes >= 1, "minimum_nprobes must be at least 1");
+  LB2_REQUIRE(pp->maximum_nprobes == 0 || pp->maximum_nprobes >= pp->minimum_nprobes,
+              "maximum_nprobes %u is below minimum_nprobes %u", pp->maximum_nprobes, pp->minimum_nprobes);
+  LB2_REQUIRE(pp->late_width >= 1, "late_width must be at least 1");
+  LB2_REQUIRE(sp->allow_bitmap || (!pp->has_max_len && !pp->mask_ids), "max_len and mask_ids need an allow bitmap");
+  if (current_comm() && current_comm()->nranks > 1)
+    fail(LB2_UNSUPPORTED, "a search with minimum / maximum nprobes on a row-sharded index is not implemented");
+  InArg<uint64_t> mask(pp->mask_ids, pp->mask_ids ? pp->num_mask_ids : 0);
+  DevBuf<uint64_t> no_ids(pp->mask_ids && pp->num_mask_ids == 0 ? 1 : 0);  // an iterable, empty allow list
+  OutArg<uint32_t> np_out(nprobes_out, nq);
+  ProbeRule pr;
+  pr.min_np = pp->minimum_nprobes;
+  pr.max_np = pp->maximum_nprobes;
+  pr.late_width = pp->late_width;
+  pr.k = sp->k;
+  pr.has_max_len = pp->has_max_len != 0;
+  pr.max_len = pp->max_len;
+  pr.mask_ids = pp->mask_ids ? (mask.get() ? mask.get() : no_ids.p) : nullptr;
+  pr.num_mask_ids = pp->mask_ids ? pp->num_mask_ids : 0;
+  pr.nprobes_out = np_out.get();
+  index_search_impl(index, queries, nq, *sp, row_ids_out, dists_out, counts_out, &pr);
+  np_out.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+// RAII: route the thread's work to the caller's stream for one asynchronous call
+namespace {
+struct AsyncScope {
+  Ctx& c;
+  cudaStream_t saved;
+  explicit AsyncScope(void* stream) : c(ctx()), saved(c.stream) {
+    if (stream) c.stream = static_cast<cudaStream_t>(stream);
+    c.async_call = true;
+  }
+  ~AsyncScope() {
+    c.async_call = false;
+    c.stream = saved;
+  }
+};
+}  // namespace
+
+lb2_status lb2_index_search_async(lb2_index* index, const void* queries, uint64_t nq,
+                                  const lb2_search_params* sp, uint64_t* row_ids_out, float* dists_out,
+                                  uint32_t* counts_out, void* cuda_stream, void* done_event) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(sp, "null search params");
+  LB2_REQUIRE(sp->refine_factor == 0 || sp->refine_vectors, "refine_factor > 0 needs refine_vectors");
+  AsyncScope scope(cuda_stream);
+  index_search_impl(index, queries, nq, *sp, row_ids_out, dists_out, counts_out);
+  if (done_event) LB2_CUDA(cudaEventRecord(static_cast<cudaEvent_t>(done_event), ctx().stream));
+  LB2_API_END
+}
+
+lb2_status lb2_index_search_sharded(lb2_index* index, const void* queries, uint64_t nq,
+                                    const lb2_search_params* sp, uint64_t* row_ids_out, float* dists_out,
+                                    uint32_t* counts_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(sp && index, "null argument");
+  LB2_REQUIRE(sp->refine_factor == 0 || sp->refine_vectors, "refine_factor > 0 needs refine_vectors");
+  const uint32_t k = sp->k;
+  DevBuf<uint64_t> li((size_t)std::max<uint64_t>(1, nq * k));
+  DevBuf<float> ld((size_t)std::max<uint64_t>(1, nq * k));
+  DevBuf<uint32_t> lc(std::max<uint64_t>(1, nq));
+  index_search_impl(index, queries, nq, *sp, li.p, ld.p, lc.p);
+  OutArg<uint64_t> oi(row_ids_out, (size_t)nq * k);
+  OutArg<float> od(dists_out, (size_t)nq * k);
+  OutArg<uint32_t> oc(counts_out, nq);
+  DevBuf<uint32_t> ctmp;
+  uint32_t* cp = oc.get();
+  if (!cp) { ctmp.alloc(std::max<uint64_t>(1, nq)); cp = ctmp.p; }
+  if (nq) merge_sharded_topk(li.p, ld.p, lc.p, nq, (int)k, oi.get(), od.get(), cp);
+  oi.commit(); od.commit(); oc.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_index_row_mask(const lb2_index* index, const uint64_t* allow_ids, uint64_t n_allow,
+                              int has_allow, const uint64_t* block_ids, uint64_t n_block, int has_block,
+                              uint64_t* bitmap_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && bitmap_out, "bad argument");
+  LB2_REQUIRE((!has_allow || n_allow == 0 || allow_ids) && (!has_block || n_block == 0 || block_ids), "null id list");
+  InArg<uint64_t> a(allow_ids, has_allow ? (size_t)n_allow : 0), b(block_ids, has_block ? (size_t)n_block : 0);
+  OutArg<uint64_t> bm(bitmap_out, (size_t)((index->n + 63) / 64));
+  row_mask_f32(index->row_ids.p, index->n, a.get(), n_allow, has_allow != 0, b.get(), n_block, has_block != 0,
+               bm.get());
+  bm.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_index_info(const lb2_index* index, uint32_t* k, uint32_t* d, uint32_t* num_sub_vectors,
+                          uint32_t* num_bits, uint64_t* num_rows) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index, "null index");
+  if (k) *k = index->K;
+  if (d) *d = index->d;
+  if (num_sub_vectors) *num_sub_vectors = index->M;
+  if (num_bits) *num_bits = index->nbits;
+  if (num_rows) *num_rows = index->n;
+  LB2_API_END
+}
+
+lb2_status lb2_index_update(const lb2_index* old, const void* new_centroids, uint32_t new_k, const uint32_t* part_map,
+                            const uint32_t* add_part_ids, const uint8_t* add_codes, const uint64_t* add_row_ids,
+                            uint64_t n_add, const uint64_t* remove_row_ids, uint64_t n_remove, lb2_index** out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(old && out && old->kind == IndexKind::PQ, "lb2_index_update takes an IVF_PQ index");
+  LB2_REQUIRE(new_k > 0 && (new_centroids || new_k == (uint32_t)old->K), "a changed partition count needs new centroids");
+  LB2_REQUIRE(n_add == 0 || (add_part_ids && add_codes && add_row_ids), "added rows need partition ids, codes and row ids");
+  LB2_REQUIRE(n_remove == 0 || remove_row_ids, "null remove list");
+  const int cbw = (int)old->row_bytes();
+  const uint64_t n_old = old->n, n_all = n_old + n_add;
+  LB2_REQUIRE(n_all < 0xffffffffull, "more than 2^32-1 rows per index shard");
+  std::unique_ptr<lb2_index> ix = make_index(old->kind, new_k, old->d, old->metric, old->dtype);
+  copy_model(old, ix.get(), new_centroids);
+  InArg<uint32_t> pm(part_map, part_map ? (size_t)old->K : 0), ap(add_part_ids, n_add);
+  InArg<uint8_t> ac(add_codes, (size_t)n_add * cbw);
+  InArg<uint64_t> ar(add_row_ids, n_add), rm(remove_row_ids, n_remove);
+  if (n_add) check_part_ids(ap.get(), n_add, new_k, "index_update");
+  // one row list: old rows in storage order, then the added rows (so a partition keeps its old rows first)
+  DevBuf<uint32_t> part(std::max<uint64_t>(1, n_all)), bad(1);
+  DevBuf<uint8_t> valid(std::max<uint64_t>(1, n_all)), codes(std::max<uint64_t>(1, n_all * cbw));
+  DevBuf<uint64_t> rid(std::max<uint64_t>(1, n_all));
+  bad.zero();
+  if (n_old) {
+    LB2_LAUNCH("update_old_rows", update_old_rows_kernel, cdiv(n_old, 256), 256, 0, old->part_offsets.p, old->K, n_old,
+               pm.get(), (const uint64_t*)old->row_ids.p, rm.get(), n_remove, new_k, part.p, valid.p, bad.p);
+    d2d(codes.p, old->codes.p, (size_t)n_old * cbw);
+    d2d(rid.p, old->row_ids.p, (size_t)n_old);
+  }
+  if (n_add) {
+    d2d(part.p + n_old, ap.get(), (size_t)n_add);
+    d2d(codes.p + n_old * cbw, ac.get(), (size_t)n_add * cbw);
+    d2d(rid.p + n_old, ar.get(), (size_t)n_add);
+    LB2_LAUNCH("fill_valid", fill_u8_kernel, cdiv(n_add, 256), 256, 0, valid.p + n_old, n_add, (uint8_t)1);
+  }
+  uint32_t hbad = 0;
+  d2h(&hbad, bad.p, 1);
+  sync_stream();
+  if (hbad) fail(LB2_INVALID_ARG, "index_update: part_map sends a partition to %u, the new index has %u partitions", hbad, new_k);
+  index_load_dev(ix.get(), part.p, codes.p, rid.p, n_all, valid.p);
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_index_repartition(const lb2_index* shard, lb2_index** owned_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(shard && owned_out, "null argument");
+  if (shard->kind == IndexKind::RQ) fail(LB2_UNSUPPORTED, "lb2_index_repartition: IVF_RQ indexes are not implemented");
+  Comm* cm = current_comm();
+  const int G = cm ? cm->nranks : 1, me = cm ? cm->rank : 0;
+  const int K = shard->K;
+  const int rb = (int)shard->row_bytes();
+  const uint8_t* payload = shard->payload().p;
+  // every rank's partition sizes (one all-gather of K counters), then the layouts on the host
+  std::vector<uint64_t> offs(K + 1);
+  d2h(offs.data(), shard->part_offsets.p, (size_t)K + 1);
+  sync_stream();
+  std::vector<uint64_t> mine(K), all((size_t)G * K);
+  for (int p = 0; p < K; ++p) mine[p] = offs[p + 1] - offs[p];
+  {
+    DevBuf<uint64_t> dm(K), da((size_t)G * K);
+    h2d(dm.p, mine.data(), K);
+    comm_allgather_bytes(dm.p, da.p, (size_t)K * 8);
+    d2h(all.data(), da.p, (size_t)G * K);
+    sync_stream();
+  }
+  // send side: rows for destination g = partitions p % G == g, ascending p
+  std::vector<size_t> s_off(G), r_off(G);
+  std::vector<uint64_t> s_rows(G, 0), r_rows(G, 0), send_base(K);
+  for (int p = 0; p < K; ++p) s_rows[p % G] += mine[p];
+  {
+    std::vector<uint64_t> run(G, 0);
+    uint64_t acc = 0;
+    std::vector<uint64_t> gbase(G);
+    for (int g = 0; g < G; ++g) { gbase[g] = acc; acc += s_rows[g]; }
+    for (int p = 0; p < K; ++p) { send_base[p] = gbase[p % G] + run[p % G]; run[p % G] += mine[p]; }
+    for (int g = 0; g < G; ++g) s_off[g] = gbase[g];
+  }
+  // receive side: from source r the rows of my partitions; final order inside a partition = source rank order
+  const int nown = (K - me + G - 1) / G;  // partitions me, me + G, ...
+  uint64_t n_new = 0;
+  std::vector<uint64_t> new_off(K + 1, 0);
+  for (int p = 0; p < K; ++p) {
+    new_off[p] = n_new;
+    if (p % G == me) for (int r = 0; r < G; ++r) n_new += all[(size_t)r * K + p];
+  }
+  new_off[K] = n_new;
+  LB2_REQUIRE(n_new < 0xffffffffull, "more than 2^32-1 rows per index shard");
+  {
+    uint64_t acc = 0;
+    for (int r = 0; r < G; ++r) {
+      for (int i = 0; i < nown; ++i) r_rows[r] += all[(size_t)r * K + (me + (size_t)i * G)];
+      r_off[r] = acc; acc += r_rows[r];
+    }
+  }
+  const uint64_t n = shard->n;
+  DevBuf<uint8_t> sp(std::max<uint64_t>(1, n * rb)), rp(std::max<uint64_t>(1, n_new * rb));
+  DevBuf<uint64_t> si(std::max<uint64_t>(1, n)), ri(std::max<uint64_t>(1, n_new)), dbase(K);
+  h2d(dbase.p, send_base.data(), K);
+  if (n)
+    LB2_LAUNCH("repartition_pack", repart_pack_kernel, cdiv(n, 256), 256, 0, shard->part_offsets.p, K, n, rb,
+               (const uint64_t*)dbase.p, payload, (const uint64_t*)shard->row_ids.p, sp.p, si.p);
+  {
+    std::vector<size_t> so(G), sb(G), ro(G), rbv(G);
+    for (int g = 0; g < G; ++g) { so[g] = s_off[g] * rb; sb[g] = s_rows[g] * rb; ro[g] = r_off[g] * rb; rbv[g] = r_rows[g] * rb; }
+    comm_alltoallv_bytes(sp.p, so.data(), sb.data(), rp.p, ro.data(), rbv.data());
+    for (int g = 0; g < G; ++g) { so[g] = s_off[g] * 8; sb[g] = s_rows[g] * 8; ro[g] = r_off[g] * 8; rbv[g] = r_rows[g] * 8; }
+    comm_alltoallv_bytes(si.p, so.data(), sb.data(), ri.p, ro.data(), rbv.data());
+  }
+  std::unique_ptr<lb2_index> ix = make_index(shard->kind, K, shard->d, shard->metric, shard->dtype);
+  copy_model(shard, ix.get());
+  ix->n = n_new;
+  ix->part_offsets.alloc(K + 1);
+  h2d(ix->part_offsets.p, new_off.data(), (size_t)K + 1);
+  DevBuf<uint8_t>& dstp = ix->payload();
+  dstp.alloc(std::max<uint64_t>(1, n_new * rb));
+  ix->row_ids.alloc(std::max<uint64_t>(1, n_new));
+  // place every (source rank, owned partition) segment: seg_prefix = rows of r before its i-th owned partition
+  std::vector<uint64_t> pre((size_t)nown + 1), dst(std::max(1, nown));
+  DevBuf<uint64_t> dpre((size_t)nown + 1), ddst(std::max(1, nown));
+  std::vector<uint64_t> before(std::max(1, nown), 0);  // rows of lower ranks already placed in owned partition i
+  for (int r = 0; r < G; ++r) {
+    uint64_t acc = 0;
+    for (int i = 0; i < nown; ++i) {
+      const int p = me + i * G;
+      pre[i] = acc;
+      dst[i] = new_off[p] + before[i];
+      acc += all[(size_t)r * K + p];
+      before[i] += all[(size_t)r * K + p];
+    }
+    pre[nown] = acc;
+    if (!acc) continue;
+    h2d(dpre.p, pre.data(), (size_t)nown + 1);
+    h2d(ddst.p, dst.data(), (size_t)nown);
+    LB2_LAUNCH("repartition_unpack", repart_unpack_kernel, cdiv(acc, 256), 256, 0, (const uint64_t*)dpre.p,
+               (const uint64_t*)ddst.p, nown, acc, rb, (const uint8_t*)(rp.p + r_off[r] * rb),
+               (const uint64_t*)(ri.p + r_off[r]), dstp.p, ix->row_ids.p);
+    sync_stream();  // pre / dst are reused by the next source rank
+  }
+  build_skew(ix.get());
+  sync_stream();
+  *owned_out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_index_destroy(lb2_index* index) {
+  LB2_API_BEGIN
+  if (index) {
+    ctx();
+    delete index;
+    sync_stream();
+  }
+  LB2_API_END
+}
+
+}  // extern "C"

@@ -1914,14 +1914,6 @@ void merge_sharded_topk(const uint64_t* ids, const float* dists, const uint32_t*
   sync_stream();  // the exchange buffers are freed on return
 }
 
-__device__ __forceinline__ bool sorted_contains(const uint64_t* __restrict__ a, uint64_t n, uint64_t v) {
-  uint64_t lo = 0, hi = n;
-  while (lo < hi) {
-    const uint64_t mid = (lo + hi) >> 1;
-    if (a[mid] < v) lo = mid + 1; else hi = mid;
-  }
-  return lo < n && a[lo] == v;
-}
 __global__ void row_mask_kernel(const uint64_t* __restrict__ row_ids, uint64_t n,
                                 const uint64_t* __restrict__ allow, uint64_t n_allow, int has_allow,
                                 const uint64_t* __restrict__ block, uint64_t n_block, int has_block,

@@ -18,6 +18,15 @@ inline int32_t host_total_key(float f) {
   memcpy(&b, &f, 4);
   return b ^ (int32_t)((uint32_t)(b >> 31) >> 1);
 }
+inline ScanFilter make_filter(const uint64_t* allow, int has_lower, float lower, int has_upper, float upper) {
+  ScanFilter f;
+  f.allow = allow;
+  f.range = (has_lower || has_upper) ? 1 : 0;
+  // flat/index.rs:101-102: lower_bound.unwrap_or(f32::MIN), upper_bound.unwrap_or(f32::MAX)
+  f.lo_key = host_total_key(has_lower ? lower : -3.40282347e+38f);
+  f.hi_key = host_total_key(has_upper ? upper : 3.40282347e+38f);
+  return f;
+}
 void find_partitions_f32(const float* centroids, int K, int d, int metric, const float* queries,
                          uint64_t nq, int nprobes, uint32_t* ids, float* dists);
 void ivfpq_search_f32(const float* centroids, int K, int d, int metric, const float* codebook, int M,

@@ -1480,7 +1480,7 @@ def test_split_partition_flow_on_device_primitives():
         assert np.array_equal(a[key], b[key]), key
 
 
-# ---- the bulk-copy staging cache (api.cu StagingCache): repeated host-sourced builds reuse one landing buffer --
+# ---- the bulk-copy staging cache (staging.cuh StagingCache): repeated host-sourced builds reuse one landing buffer --
 def test_host_sourced_builds_reuse_staging_buffer_and_equal_device_builds():
     n, d, K, M = 30000, 64, 16, 8
     prm = lb.IvfBuildParams(num_partitions=K, num_sub_vectors=M, max_iters=6, pq_max_iters=5, seed=11)
