@@ -10,9 +10,10 @@
 #include "common.cuh"
 #include "exact.cuh"
 #include "index.cuh"
+#include "ivf_search.cuh"
 #include "kmeans.cuh"
 #include "rq.cuh"
-#include "search.cuh"
+#include "scan.cuh"
 #include "sq.cuh"
 #include "staging.cuh"
 #include "tc_assign.cuh"

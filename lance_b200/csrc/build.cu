@@ -9,7 +9,7 @@
 #include "index.cuh"
 #include "kmeans.cuh"
 #include "rq.cuh"
-#include "search.cuh"
+#include "scan.cuh"
 #include "sq.cuh"
 #include "tc_assign.cuh"
 #include "tc_pq.cuh"

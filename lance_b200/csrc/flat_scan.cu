@@ -1,0 +1,279 @@
+// flat_scan.cu -- the exact-distance query kernels: the IVF_FLAT partition scan, the refine step over raw vectors
+// and the top-k of a distance array.
+//
+// Replaces  FlatDistanceCal::distance_all        lance-index/src/vector/flat/storage.rs:397-403
+//           FlatIndex::search heap top-k         lance-index/src/vector/flat/index.rs:82-177
+#include <cuda_bf16.h>
+#include <cuda_fp16.h>
+
+#include <type_traits>
+
+#include "common.cuh"
+#include "exact.cuh"
+#include "ivf_search.cuh"
+#include "scan.cuh"
+#include "topk.cuh"
+
+namespace lb2 {
+
+// ------------------------------------------------------------------------------------------------
+// IVF_FLAT: exact distances of the query to every row of a probed partition
+// (FlatDistanceCal::distance_all, lance-index/src/vector/flat/storage.rs:397-403) + top-k.
+// 16 lanes per row: lane l owns the reference's lane-accumulator l (elements 16c + l), so the L2 /
+// dot results are bit-identical to l2.rs:57-91 / dot.rs:30-58; cosine follows cosine.rs:143-174 in
+// structure (f32 FMA lanes) and is checked to the reference's own tolerance.
+// ------------------------------------------------------------------------------------------------
+// element of a stored / raw vector as f32 (l2.rs:100-106,156: f16 / bf16 elements are converted one by one)
+template <class T> __device__ __forceinline__ float ldf(const T* p, int e);
+template <> __device__ __forceinline__ float ldf<float>(const float* p, int e) { return p[e]; }
+template <> __device__ __forceinline__ float ldf<__half>(const __half* p, int e) { return __half2float(p[e]); }
+template <> __device__ __forceinline__ float ldf<__nv_bfloat16>(const __nv_bfloat16* p, int e) { return __bfloat162float(p[e]); }
+template <> __device__ __forceinline__ float ldf<uint8_t>(const uint8_t* p, int e) { return (float)p[e]; }
+
+template <int METRIC, class T = float>
+__device__ __forceinline__ float flat_row_distance(const float* __restrict__ q, const T* __restrict__ v,
+                                                   int d, int l, unsigned mask, float q_norm) {
+  const int n16 = d & ~15;
+  if (METRIC == METRIC_COSINE) {
+    float xy = 0.0f, yy = 0.0f;
+    for (int e = l; e < d; e += 16) {
+      const float y = ldf<T>(v, e);
+      xy = fmaf(q[e], y, xy);
+      yy = fmaf(y, y, yy);
+    }
+#pragma unroll
+    for (int off = 8; off >= 1; off >>= 1) {
+      xy += __shfl_xor_sync(mask, xy, off, 16);
+      yy += __shfl_xor_sync(mask, yy, off, 16);
+    }
+    return 1.0f - xy / q_norm / sqrtf(yy);
+  }
+  float acc = 0.0f;
+  for (int e = l; e < n16; e += 16) acc = f_add(acc, term<METRIC>(q[e], ldf<T>(v, e)));
+  float s = 0.0f;  // sequential tail, every lane redundantly (l2.rs:69-79)
+  for (int e = n16; e < d; ++e) s = f_add(s, term<METRIC>(q[e], ldf<T>(v, e)));
+  float t = 0.0f;
+#pragma unroll
+  for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, acc, qq, 16));
+  return finish<METRIC>(f_add(s, t));
+}
+
+template <int METRIC, class T>
+__global__ void __launch_bounds__(256)
+ivfflat_scan_kernel(const float* __restrict__ queries, int d, const uint32_t* __restrict__ probe_ids,
+                    int np, const uint64_t* __restrict__ part_offsets,
+                    const T* __restrict__ vectors, const uint64_t* __restrict__ row_ids, int k,
+                    float* __restrict__ cand_d, uint64_t* __restrict__ cand_id,
+                    uint32_t* __restrict__ cand_cnt, const ScanFilter flt) {
+  extern __shared__ float smem[];
+  float* qs = smem;                          // [d]
+  const SlotSmem s(qs + d, k + 1);
+  __shared__ float s_qnorm;
+  const int tid = threadIdx.x, l = tid & 15;
+  const unsigned hmask = 0xffffu << (16 * ((tid >> 4) & 1));
+  size_t qi, slot;
+  uint32_t p, n_p;
+  uint64_t off;
+  if (!slot_partition(probe_ids, np, part_offsets, cand_cnt, qi, slot, p, off, n_p)) return;
+  for (int t = tid; t < d; t += 256) qs[t] = queries[qi * d + t];
+  __syncthreads();
+  if (METRIC == METRIC_COSINE && tid < 32) {  // norm_l2(query): 16 lanes + sqrt (norm_l2.rs:106-130)
+    float a = 0.0f;
+    for (int e = (tid & 15); e < d; e += 16) a = fmaf(qs[e], qs[e], a);
+#pragma unroll
+    for (int o = 8; o >= 1; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o, 16);
+    if (tid == 0) s_qnorm = sqrtf(a);
+  }
+  __syncthreads();
+  const float qn = METRIC == METRIC_COSINE ? s_qnorm : 0.0f;
+  auto fill = [&](uint32_t c0, uint32_t clen) {
+    for (uint32_t j = tid >> 4; j < clen; j += 16) {  // 16 rows per pass, 16 lanes each
+      const float dist = flat_row_distance<METRIC, T>(qs, vectors + (off + c0 + j) * (uint64_t)d, d, l, hmask, qn);
+      if (l == 0) s.ukey[j] = (uint32_t)total_order_key(dist) ^ 0x80000000u;
+    }
+  };
+  const uint32_t cnt = slot_topk(s, n_p, k, flt, off, false, fill);
+  write_slot(s, cnt, slot, k, off, row_ids, cand_d, cand_id, cand_cnt);
+}
+
+// FlatIndex::search over a distance array (flat/index.rs:97-127): the heap's final content (the exact top-k of one
+// slot, position = index into dists), written ascending by (distance, row id).
+__global__ void __launch_bounds__(256)
+flat_topk_kernel(const float* __restrict__ dists, const uint64_t* __restrict__ row_ids, uint64_t n,
+                 int k, const ScanFilter flt, uint64_t* __restrict__ out_id, float* __restrict__ out_d,
+                 uint32_t* __restrict__ out_cnt) {
+  extern __shared__ float smem[];
+  const SlotSmem s(smem, k + 1);
+  auto fill = [&](uint32_t c0, uint32_t clen) {
+    for (uint32_t j = threadIdx.x; j < clen; j += 256) s.ukey[j] = (uint32_t)total_order_key(dists[c0 + j]) ^ 0x80000000u;
+  };
+  const uint32_t cnt = slot_topk(s, (uint32_t)n, k, flt, 0, false, fill);
+  emit_ascending<256>(
+      cnt, cnt,
+      [&](uint32_t i, int32_t& key, uint64_t& id) {
+        key = (int32_t)(s.nkey[i] ^ 0x80000000u);
+        id = row_ids ? row_ids[s.npos[i]] : (uint64_t)s.npos[i];
+        return true;
+      },
+      [&](uint32_t r, uint32_t, int32_t key, uint64_t id) {
+        out_d[r] = key_to_float(key);
+        out_id[r] = id;
+      });
+  if (threadIdx.x == 0) *out_cnt = cnt;
+}
+
+// f(metric, element) with the metric as a std::integral_constant and the element type as a type_tag
+template <class T> struct type_tag { using type = T; };
+template <bool WITH_U8, class F>
+static void dispatch_metric_elem(int metric, int vdt, F&& f) {
+  auto by_elem = [&](auto m) {
+    if (vdt == LB2_F16) f(m, type_tag<__half>{});
+    else if (vdt == LB2_BF16) f(m, type_tag<__nv_bfloat16>{});
+    else if constexpr (WITH_U8) {
+      if (vdt == LB2_U8) f(m, type_tag<uint8_t>{}); else f(m, type_tag<float>{});
+    } else f(m, type_tag<float>{});
+  };
+  if (metric == METRIC_DOT) by_elem(std::integral_constant<int, METRIC_DOT>{});
+  else if (metric == METRIC_COSINE) by_elem(std::integral_constant<int, METRIC_COSINE>{});
+  else by_elem(std::integral_constant<int, METRIC_L2>{});
+}
+
+void ivfflat_search(const IvfSearch& s, const void* vectors, int vdt) {
+  const int d = s.d, k = s.k;
+  const size_t smem = sizeof(float) * (size_t)d + slot_smem_bytes(k);
+  size_t need = 0;
+  dispatch_metric_elem<false>(s.metric, vdt, [&](auto m, auto e) {
+    need = smem_with_static(ivfflat_scan_kernel<decltype(m)::value, typename decltype(e)::type>, smem);
+  });
+  if (!ivf_search_begin(s, need, "dimension %zu too large for the flat scan", (size_t)d)) return;
+  run_ivf_search(s, [&](const ScanSlots& sl) {
+    dispatch_metric_elem<false>(s.metric, vdt, [&](auto m, auto e) {
+      using T = typename decltype(e)::type;
+      auto kern = ivfflat_scan_kernel<decltype(m)::value, T>;
+      set_smem(kern, smem);
+      LB2_LAUNCH("flat_scan", kern, dim3(sl.np, (unsigned)sl.qn), 256, smem, s.queries + sl.q0 * d, d, sl.probe_ids,
+                 sl.np, sl.offsets, reinterpret_cast<const T*>(vectors), s.row_ids, k, sl.cand_d, sl.cand_id,
+                 sl.cand_cnt, s.flt);
+    });
+  });
+}
+
+// ------------------------------------------------------------------------------------------------
+// refine: exact distances of k' = k * refine_factor candidates from the raw vectors, then the k
+// best by (distance, row id)  (scanner.rs:2884-2905, flat.rs:95-148)
+// ------------------------------------------------------------------------------------------------
+// The refine plan takes the distance function of the column's own element type (flat.rs:94-150), unlike the
+// IVF_FLAT scan, whose storage is f32 (flat/storage.rs:352-365):
+//  * f16 dot: dot_scalar::<f16, f32, 32> (dot.rs:30-58,133): lane l owns the accumulators l and l + 16, the d % 32
+//    tail comes first, the 32 sums are folded 0..31;
+//  * u8 L2 / dot: exact integer sums, one conversion to f32 (l2.rs:44-49, dot.rs:152-161); the query came in as
+//    u8 too, so its f32 view holds integers;
+//  * everything else (f16 L2, bf16, cosine) as flat_row_distance.
+template <int METRIC, class T>
+__device__ __forceinline__ float refine_row_distance(const float* __restrict__ q, const T* __restrict__ v, int d,
+                                                     int l, unsigned mask, float q_norm) {
+  if constexpr (std::is_same<T, uint8_t>::value && METRIC != METRIC_COSINE) {
+    uint32_t acc = 0;
+    for (int e = l; e < d; e += 16) {
+      const int x = __float2int_rn(q[e]), y = v[e];
+      acc += METRIC == METRIC_DOT ? (uint32_t)(x * y) : (uint32_t)((x - y) * (x - y));
+    }
+#pragma unroll
+    for (int off = 8; off >= 1; off >>= 1) acc += __shfl_xor_sync(mask, acc, off, 16);
+    return finish<METRIC>(__uint2float_rn(acc));
+  } else if constexpr (std::is_same<T, __half>::value && METRIC == METRIC_DOT) {
+    const int n32 = d & ~31;
+    float a0 = 0.0f, a1 = 0.0f;
+    for (int e = l; e < n32; e += 32) {
+      a0 = f_add(a0, __fmul_rn(q[e], ldf<T>(v, e)));
+      a1 = f_add(a1, __fmul_rn(q[e + 16], ldf<T>(v, e + 16)));
+    }
+    float s = 0.0f;  // sequential tail, every lane redundantly
+    for (int e = n32; e < d; ++e) s = f_add(s, __fmul_rn(q[e], ldf<T>(v, e)));
+    float t = 0.0f;
+#pragma unroll
+    for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, a0, qq, 16));
+#pragma unroll
+    for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, a1, qq, 16));
+    return finish<METRIC>(f_add(s, t));
+  } else {
+    return flat_row_distance<METRIC, T>(q, v, d, l, mask, q_norm);
+  }
+}
+
+template <int METRIC, class T>
+__global__ void __launch_bounds__(256)
+refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ vectors,
+              uint64_t num_vectors, const uint64_t* __restrict__ cand_id, const uint32_t* __restrict__ cand_cnt,
+              int kc, int k, uint64_t* __restrict__ out_id, float* __restrict__ out_d,
+              uint32_t* __restrict__ out_cnt, int has_lower, float lower, int has_upper, float upper) {
+  extern __shared__ float smem[];
+  float* qs = smem;       // [d]
+  float* cd = qs + d;     // [kc]
+  __shared__ float s_qnorm;
+  const size_t qi = blockIdx.x;
+  const int tid = threadIdx.x, l = tid & 15;
+  const unsigned hmask = 0xffffu << (16 * ((tid >> 4) & 1));
+  const uint32_t cnt = min(cand_cnt[qi], (uint32_t)kc);
+  for (int t = tid; t < d; t += 256) qs[t] = queries[qi * d + t];
+  __syncthreads();
+  if (METRIC == METRIC_COSINE && tid < 32) {
+    float a = 0.0f;
+    for (int e = (tid & 15); e < d; e += 16) a = fmaf(qs[e], qs[e], a);
+#pragma unroll
+    for (int o = 8; o >= 1; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o, 16);
+    if (tid == 0) s_qnorm = sqrtf(a);
+  }
+  __syncthreads();
+  const float qn = METRIC == METRIC_COSINE ? s_qnorm : 0.0f;
+  const uint64_t* ids = cand_id + qi * kc;
+  for (uint32_t c = tid >> 4; c < cnt; c += 16) {
+    const uint64_t id = ids[c];
+    float dist = __int_as_float(0x7fc00000);
+    if (id < num_vectors) dist = refine_row_distance<METRIC, T>(qs, vectors + id * (uint64_t)d, d, l, hmask, qn);
+    if (l == 0) cd[c] = dist;
+  }
+  __syncthreads();
+  auto passes = [&](float dv) {  // LanceFilterExec(_distance >= lower AND _distance < upper): SQL compares
+    return (!has_lower || dv >= lower) && (!has_upper || dv < upper);
+  };
+  const uint32_t r = emit_ascending<256>(
+      min(cnt, (uint32_t)k), cnt,
+      [&](uint32_t c, int32_t& key, uint64_t& id) {
+        key = total_order_key(cd[c]);
+        id = ids[c];
+        return passes(cd[c]);
+      },
+      [&](uint32_t r, uint32_t c, int32_t, uint64_t id) {
+        out_id[qi * k + r] = id;
+        out_d[qi * k + r] = cd[c];
+      });
+  for (uint32_t e = r + tid; e < (uint32_t)k; e += 256) {
+    out_id[qi * k + e] = ~0ull;
+    out_d[qi * k + e] = __int_as_float(0x7f800000);
+  }
+  if (tid == 0 && out_cnt) out_cnt[qi] = r;
+}
+
+void refine_f32(const float* queries, uint64_t nq, int d, int metric, const void* vectors, int vdt,
+                uint64_t num_vectors, const uint64_t* cand_id, const uint32_t* cand_cnt, int kc, int k,
+                uint64_t* out_id, float* out_d, uint32_t* out_cnt, int has_lower, float lower, int has_upper,
+                float upper) {
+  if (nq == 0) return;
+  const size_t smem = sizeof(float) * ((size_t)d + kc);
+  dispatch_metric_elem<true>(metric, vdt, [&](auto m, auto e) {
+    using T = typename decltype(e)::type;
+    auto kern = refine_kernel<decltype(m)::value, T>;
+    set_smem(kern, smem);
+    LB2_LAUNCH("refine", kern, (unsigned)nq, 256, smem, queries, d, reinterpret_cast<const T*>(vectors), num_vectors,
+               cand_id, cand_cnt, kc, k, out_id, out_d, out_cnt, has_lower, lower, has_upper, upper);
+  });
+}
+
+void flat_topk_f32(const float* dists, const uint64_t* row_ids, uint64_t n, int k, const ScanFilter& flt,
+                   uint64_t* out_id, float* out_d, uint32_t* out_cnt) {
+  if (k > 1024) fail(LB2_UNSUPPORTED, "k > 1024 is not implemented");
+  LB2_LAUNCH("flat_topk", flat_topk_kernel, 1, 256, slot_smem_bytes(k), dists, row_ids, n, k, flt, out_id, out_d, out_cnt);
+}
+
+}  // namespace lb2

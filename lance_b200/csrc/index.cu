@@ -6,8 +6,10 @@
 #include "build.cuh"
 #include "comm.cuh"
 #include "index.cuh"
+#include "ivf_search.cuh"
 #include "kmeans.cuh"
-#include "search.cuh"
+#include "rq.cuh"
+#include "scan.cuh"
 #include "sq.cuh"
 
 namespace lb2 {
@@ -296,31 +298,28 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
   TagScope tg("search");
   const ScanFilter flt = make_filter(sp.allow_bitmap ? allow.get() : nullptr, sp.has_lower_bound != 0, sp.lower_bound,
                                     sp.has_upper_bound != 0, sp.upper_bound);
+  const IvfSearch s{index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->row_ids.p, qp, nq,
+                    (int)kc, (int)nprobes, si, sd, sc, flt, pr};
   DevBuf<uint8_t> qcodes;
   switch (index->kind) {
     case IndexKind::FLAT:
-      ivfflat_search_f32(index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->vectors.p,
-                         (int)index->vdtype(), index->row_ids.p, qp, nq, (int)kc, nprobes, si, sd, sc, flt, pr);
+      ivfflat_search(s, index->vectors.p, (int)index->vdtype());
       break;
     case IndexKind::RQ:
       // the (normalised) query's residual to each probed centroid is rotated (v2.rs:316-332, bq/storage.rs:407-445)
-      ivfrq_search_f32(index->centroids.p, index->K, d, index->metric, index->rq_rot.p, index->code_dim(),
-                       index->part_offsets.p, index->codes.p, index->rq_add.p, index->rq_scale.p, index->row_ids.p, qp,
-                       nq, (int)kc, nprobes, si, sd, sc, flt, pr);
+      ivfrq_search(s, index->rq_rot.p, index->code_dim(), index->codes.p, index->rq_add.p, index->rq_scale.p);
       break;
     case IndexKind::SQ: {
       // the (normalised) query is encoded with the index's bounds, not turned into a residual (sq/storage.rs:404-430)
       qcodes.alloc(std::max<uint64_t>(1, nq * d));
       sq_encode_f32(qp, nq * d, index->sq_lower, index->sq_upper, qcodes.p);
       const float rf = (float)(index->sq_upper - index->sq_lower);  // inverse_scalar_dist (sq.rs:279-287)
-      ivfsq_search_f32(index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->codes.p,
-                       index->row_ids.p, rf * rf, qp, qcodes.p, nq, (int)kc, nprobes, si, sd, sc, flt, pr);
+      ivfsq_search(s, index->codes.p, rf * rf, qcodes.p);
       break;
     }
     case IndexKind::PQ:
-      ivfpq_search_f32(index->centroids.p, index->K, d, index->metric, index->codebook.p, index->M, index->nbits,
-                       index->part_offsets.p, index->codes.p, index->row_ids.p, qp, nq, (int)kc, nprobes, si, sd,
-                       sc, flt, index->slab_off.p, index->codes_skew.p, pr);
+      ivfpq_search(s, index->codebook.p, index->M, index->nbits, index->codes.p, index->slab_off.p,
+                   index->codes_skew.p);
       break;
   }
   if (refine) {
@@ -419,6 +418,29 @@ __global__ void fill_u8_kernel(uint8_t* __restrict__ p, uint64_t n, uint8_t v) {
 }
 
 }  // extern "C"
+
+// bit i of bitmap = RowIdMask::selected(row_ids[i]) (lance-core/src/utils/mask.rs:84-93); lists sorted
+__global__ void row_mask_kernel(const uint64_t* __restrict__ row_ids, uint64_t n,
+                                const uint64_t* __restrict__ allow, uint64_t n_allow, int has_allow,
+                                const uint64_t* __restrict__ block, uint64_t n_block, int has_block,
+                                uint32_t* __restrict__ bitmap32) {
+  const uint64_t pos = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;  // n padded to 64 by the grid
+  bool sel = false;
+  if (pos < n) {
+    const uint64_t id = row_ids[pos];
+    sel = (!has_allow || sorted_contains(allow, n_allow, id)) && !(has_block && sorted_contains(block, n_block, id));
+  }
+  const unsigned bal = __ballot_sync(0xffffffffu, sel);
+  // the bitmap holds ceil(n / 64) u64 words; the last CTA may reach beyond it
+  if ((threadIdx.x & 31) == 0 && (pos >> 5) < ((n + 63) / 64) * 2) bitmap32[pos >> 5] = bal;
+}
+static void row_mask_f32(const uint64_t* row_ids, uint64_t n, const uint64_t* allow, uint64_t n_allow, bool has_allow,
+                  const uint64_t* block, uint64_t n_block, bool has_block, uint64_t* bitmap) {
+  const uint64_t padded = (n + 63) / 64 * 64;
+  if (padded == 0) return;
+  LB2_LAUNCH("row_mask", row_mask_kernel, cdiv(padded, 256), 256, 0, row_ids, n, allow, n_allow,
+             has_allow ? 1 : 0, block, n_block, has_block ? 1 : 0, reinterpret_cast<uint32_t*>(bitmap));
+}
 
 // row-major codes [n][cw] of one partition -> the reference's storage layout [cw][n] (pq/storage.rs:430-450)
 __global__ void transpose_codes_kernel(const uint8_t* __restrict__ codes, uint64_t n, int cw, uint8_t* __restrict__ out) {

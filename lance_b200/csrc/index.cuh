@@ -21,7 +21,7 @@ struct lb2_index {
   lb2::DevBuf<float> centroids, codebook;
   lb2::DevBuf<uint64_t> part_offsets, row_ids;
   lb2::DevBuf<uint8_t> codes;
-  // the conflict-free scan's skewed copy of `codes` (search.cu: ivfpq_scan_skew_kernel); empty for other shapes
+  // the conflict-free scan's skewed copy of `codes` (pq_scan.cu: ivfpq_scan_skew_kernel); empty for other shapes
   lb2::DevBuf<uint64_t> slab_off;
   lb2::DevBuf<uint8_t> codes_skew;
   // IVF_SQ: `codes` are the 8-bit scalar codes [n][d] of the (normalised for cosine) vectors, under the bounds

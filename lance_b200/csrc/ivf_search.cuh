@@ -1,0 +1,87 @@
+// ivf_search.cuh -- what an IVF search is, for the index (which fills one IvfSearch) and the scan drivers of the
+// four index kinds (which run it with their own scan); internal interface of ivf_search.cu
+#pragma once
+#include <stdint.h>
+#include <string.h>
+
+#include "common.cuh"
+#include "probe.cuh"
+namespace lb2 {
+// what FlatIndex::search lets into its heap (flat/index.rs:97-165): the prefilter bitmap over storage
+// positions (nullable) and the [lower, upper) range in f32::total_cmp order as signed order keys
+struct ScanFilter {
+  const uint64_t* allow = nullptr;
+  int range = 0;
+  int32_t lo_key = 0, hi_key = 0;
+};
+// total-order key of a float on the host (graph.rs:80-84: f32::total_cmp)
+inline int32_t host_total_key(float f) {
+  int32_t b;
+  memcpy(&b, &f, 4);
+  return b ^ (int32_t)((uint32_t)(b >> 31) >> 1);
+}
+inline ScanFilter make_filter(const uint64_t* allow, int has_lower, float lower, int has_upper, float upper) {
+  ScanFilter f;
+  f.allow = allow;
+  f.range = (has_lower || has_upper) ? 1 : 0;
+  // flat/index.rs:101-102: lower_bound.unwrap_or(f32::MIN), upper_bound.unwrap_or(f32::MAX)
+  f.lo_key = host_total_key(has_lower ? lower : -3.40282347e+38f);
+  f.hi_key = host_total_key(has_upper ? upper : 3.40282347e+38f);
+  return f;
+}
+
+// One search of an IVF index, whatever its kind: the coarse model, the partition layout, the queries (f32,
+// normalised for cosine), what to return and where.  pr (nullable): search with the probe rule instead of nprobes
+// (k is then k * refine_factor, pr->k the query's k).
+struct IvfSearch {
+  const float* centroids; int K, d, metric;
+  const uint64_t* part_offsets; const uint64_t* row_ids;
+  const float* queries; uint64_t nq; int k; int nprobes;
+  uint64_t* out_ids; float* out_dists; uint32_t* out_counts;
+  ScanFilter flt; const ProbeRule* pr;
+};
+
+// What a scan is asked to fill: the candidate lists of queries [q0, q0 + qn) (at most SEARCH_SLAB of them: the
+// grid.y limit), np slots per query.  Slot (q, pi) probes partition probe_ids[q * np + pi] of `offsets` (the
+// index's, or with a probe rule its copy with one more, empty, partition); probe_dists are the distances of the
+// probed centroids (dist_q_c).  The arrays start at query q0's first slot.
+struct ScanSlots {
+  uint64_t q0, qn; int np;
+  const uint64_t* offsets; const uint32_t* probe_ids; const float* probe_dists;
+  float* cand_d; uint64_t* cand_id; uint32_t* cand_cnt;
+};
+constexpr uint64_t SEARCH_SLAB = 32768;
+
+// a reference to a driver's scan (a lambda over ScanSlots) that lives as long as the call it is passed to
+class ScanRef {
+  const void* obj;
+  void (*call)(const void*, const ScanSlots&);
+
+ public:
+  template <class F>
+  ScanRef(const F& f) : obj(&f), call([](const void* o, const ScanSlots& s) { (*static_cast<const F*>(o))(s); }) {}
+  void operator()(const ScanSlots& s) const { call(obj, s); }
+};
+
+// the shared memory a launch of `kernel` with `dyn` dynamic bytes takes: its static shared memory counts against the
+// same per-block opt-in limit, and cudaFuncSetAttribute refuses a dynamic size that leaves no room for it
+template <class Kern>
+size_t smem_with_static(Kern kernel, size_t dyn) {
+  cudaFuncAttributes fa;
+  LB2_CUDA(cudaFuncGetAttributes(&fa, kernel));
+  return dyn + fa.sharedSizeBytes;
+}
+
+// What every driver settles before it launches anything: false when the search is empty; refuses k > 1024, and a
+// search whose largest kernel needs more than the device's shared memory (`need` bytes, static included) with the
+// driver's own text, which formats `refusal_arg` with one %zu.
+bool ivf_search_begin(const IvfSearch& s, size_t need, const char* refusal, size_t refusal_arg);
+// the fixed-nprobes skeleton (probe selection, scan, per-query merge), or with a probe rule the per-query one
+void run_ivf_search(const IvfSearch& s, ScanRef scan);
+
+void find_partitions_f32(const float* centroids, int K, int d, int metric, const float* queries,
+                         uint64_t nq, int nprobes, uint32_t* ids, float* dists);
+// all ranks' [nq][k] results of a row-sharded index -> the global top-k by (distance, row id) on every rank
+void merge_sharded_topk(const uint64_t* ids, const float* dists, const uint32_t* counts, uint64_t nq, int k,
+                        uint64_t* out_ids, float* out_dists, uint32_t* out_counts);
+}  // namespace lb2

@@ -4,6 +4,7 @@
 //           RabitQuantizer::transform            bq/builder.rs:143-181 (the sign codes)
 //           codes_res_dot_dists                  bq/builder.rs:100-141 (the per-row |rot| sum)
 //           RQTransformer::transform             bq/transform.rs:70-220 (add / scale factors)
+//           RabitDistCalculator                  bq/storage.rs:160-445 (the partition scan of a search)
 //
 // Exactness: the reference rotates data rows with an ndarray GEMM whose summation order is unspecified.  Here the
 // rotation of a row is defined as the query side's rotation, the 16-lane f32 `dot` (dot.rs:30-58, the order of
@@ -17,11 +18,14 @@
 // formed as a matrix.
 #include <curand_kernel.h>
 
+#include <algorithm>
 #include <cfloat>
 
 #include "common.cuh"
 #include "exact.cuh"
+#include "ivf_search.cuh"
 #include "rq.cuh"
+#include "topk.cuh"
 
 namespace lb2 {
 
@@ -278,6 +282,168 @@ void rq_encode_f32(const float* rot, const float* residual, const float* dist_v_
   const float sqrt_d = sqrtf((float)d * (float)num_bits);  // (dim as f32 * num_bits as f32).sqrt(), builder.rs:137
   LB2_LAUNCH("rq_encode", rq_encode_kernel, cdiv(m * 32, 256), 256, 0, rot, residual, dist_v_c, part, cnorm_sq, valid,
              m, d, code_dim, sqrt_d, metric, codes, add, scale);
+}
+
+// ------------------------------------------------------------------------------------------------
+// IVF_RQ: RabitDistCalculator (lance-index/src/vector/bq/storage.rs:160-445) + top-k, one CTA per (probe, query).
+// rq = the slot's rotated residual query (dot(R[i, :d], q - c_p), storage.rs:130-156).  In shared memory:
+//   - the code_dim / 4 sub-tables of 16 entries by the lowbit chain t[j] = t[j - lowbit(j)] + rq[4s + ctz(j)]
+//     (storage.rs:210-245), which fixes the rounding order;
+//   - sum_q = the sequential f32 sum of rq from -0.0 (Rust's float Sum);
+//   - the table quantised to u8 with qmin / qmax over the whole table in total_cmp order (storage.rs:249-267).
+// distance_all (storage.rs:319-369): the rows before the partition's last n_p % 32 sum u8 entries in 16-bit lanes
+// that wrap mod 2^16, as the x86 kernels do (dist_table.rs:96-160, dist_table.c) -- an exact u32 sum & 0xffff --
+// and are dequantised as q * ((qmax - qmin) / 255) + (code_dim / 4) * qmin; the last n_p % 32 rows take the exact
+// f32 sum of the pairs t_lo[lo] + t_hi[hi] from 0.0.  With a prefilter every row takes DistCalculator::distance
+// (storage.rs:297-316), the same pair sums from -0.0; no table entry is -0.0 (t[0] = +0.0 and x + y is -0.0 only
+// when both are), so the start does not matter.  Then ((2 dist - sum_q) / sqrt_d) * scale + add + q_factor, each
+// operation rounded on its own.  Codes are row-major [n][code_dim / 8]; the 32-row rule uses the partition-local row.
+// ------------------------------------------------------------------------------------------------
+static size_t rq_scan_smem_bytes(int code_dim, int k) {
+  return (size_t)code_dim * 4 * (sizeof(float) + 1) + slot_smem_bytes(k);
+}
+
+__global__ void __launch_bounds__(256)
+ivfrq_scan_kernel(const float* __restrict__ rq, int code_dim, float sqrt_d, int q_minus_one,
+                  const uint32_t* __restrict__ probe_ids, const float* __restrict__ probe_dists, int np,
+                  const uint64_t* __restrict__ part_offsets, const uint8_t* __restrict__ codes,
+                  const float* __restrict__ add, const float* __restrict__ scale, const uint64_t* __restrict__ row_ids,
+                  int k, float* __restrict__ cand_d, uint64_t* __restrict__ cand_id, uint32_t* __restrict__ cand_cnt,
+                  const ScanFilter flt) {
+  extern __shared__ float rq_smem[];
+  const int nt = code_dim >> 2;  // sub-tables of 16 entries
+  float* tab = rq_smem;                                      // [nt * 16] f32
+  uint8_t* qt = reinterpret_cast<uint8_t*>(tab + nt * 16);  // [nt * 16] u8 (code_dim % 8 == 0: 4-byte aligned end)
+  const SlotSmem s(qt + nt * 16, k + 1);
+  __shared__ int32_t s_mn, s_mx;
+  __shared__ float s_sum_q;
+  const int tid = threadIdx.x;
+  size_t qi, slot;
+  uint32_t p, n_p;
+  uint64_t off;
+  if (!slot_partition(probe_ids, np, part_offsets, cand_cnt, qi, slot, p, off, n_p)) return;
+  const float* r = rq + slot * (size_t)code_dim;
+  if (tid == 0) { s_mn = 0x7fffffff; s_mx = (int32_t)0x80000000; }
+  for (int st = tid; st < nt; st += 256) {
+    float t[16];
+    t[0] = 0.0f;
+#pragma unroll
+    for (int j = 1; j < 16; ++j) {
+      const int ctz = (j & 1) ? 0 : (j & 2) ? 1 : (j & 4) ? 2 : 3;
+      t[j] = __fadd_rn(t[j - (j & -j)], r[4 * st + ctz]);
+    }
+#pragma unroll
+    for (int j = 0; j < 16; ++j) tab[st * 16 + j] = t[j];
+  }
+  __syncthreads();
+  int32_t mn = 0x7fffffff, mx = (int32_t)0x80000000;
+  for (int i = tid; i < nt * 16; i += 256) {
+    const int32_t kv = total_order_key(tab[i]);
+    mn = min(mn, kv);
+    mx = max(mx, kv);
+  }
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) {
+    mn = min(mn, __shfl_xor_sync(0xffffffffu, mn, o));
+    mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+  }
+  if ((tid & 31) == 0) { atomicMin(&s_mn, mn); atomicMax(&s_mx, mx); }
+  if (tid == 0) {
+    float sq = -0.0f;
+    for (int i = 0; i < code_dim; ++i) sq = __fadd_rn(sq, r[i]);
+    s_sum_q = sq;
+  }
+  __syncthreads();
+  const float qmin = key_to_float(s_mn), qmax = key_to_float(s_mx);
+  if (flt.allow == nullptr) {
+    const bool flat = qmin == qmax;  // e.g. a zero residual query: all codes 0
+    const float factor = flat ? 0.0f : __fdiv_rn(255.0f, __fsub_rn(qmax, qmin));
+    for (int i = tid; i < nt * 16; i += 256) {
+      const float v = flat ? 0.0f : roundf(__fmul_rn(__fsub_rn(tab[i], qmin), factor));  // f32::round
+      qt[i] = (v != v) ? 0 : v <= 0.0f ? 0 : v >= 255.0f ? 255 : (uint8_t)v;           // `as u8`
+    }
+  }
+  __syncthreads();
+  const float range = __fdiv_rn(__fsub_rn(qmax, qmin), 255.0f), sum_min = __fmul_rn((float)nt, qmin);
+  const float sum_q = s_sum_q, dqc = probe_dists[slot];
+  const float q_factor = q_minus_one ? __fsub_rn(dqc, 1.0f) : dqc;  // storage.rs:427-434
+  const int cb = code_dim >> 3;
+  const uint8_t* pc = codes + off * cb;
+  const uint32_t n_quant = flt.allow ? 0u : n_p - n_p % 32;
+  auto fill = [&](uint32_t c0, uint32_t clen) {
+    for (uint32_t j = tid; j < clen; j += 256) {
+      const uint32_t row = c0 + j;
+      const uint8_t* rp = pc + (size_t)row * cb;
+      float dist;
+      if (row < n_quant) {
+        uint32_t qs = 0;
+        for (int i = 0; i < cb; ++i) {
+          const uint32_t c = __ldg(rp + i);
+          qs += (uint32_t)qt[(2 * i) * 16 + (c & 15)] + (uint32_t)qt[(2 * i + 1) * 16 + (c >> 4)];
+        }
+        dist = __fadd_rn(__fmul_rn(__uint2float_rn(qs & 0xffffu), range), sum_min);
+      } else {
+        dist = 0.0f;
+        for (int i = 0; i < cb; ++i) {
+          const uint32_t c = __ldg(rp + i);
+          dist = __fadd_rn(dist, __fadd_rn(tab[(2 * i) * 16 + (c & 15)], tab[(2 * i + 1) * 16 + (c >> 4)]));
+        }
+      }
+      const float dvq = __fdiv_rn(__fsub_rn(__fmul_rn(2.0f, dist), sum_q), sqrt_d);
+      float out = __fadd_rn(__fadd_rn(__fmul_rn(dvq, scale[off + row]), add[off + row]), q_factor);
+      // x86's default NaN (0xFFC00000, ordered before every number): with finite rows a NaN only comes from invalid
+      // operations, e.g. on a normalised zero query under cosine, and the reference runs on x86
+      if (out != out) out = __int_as_float(0xffc00000);
+      s.ukey[j] = (uint32_t)total_order_key(out) ^ 0x80000000u;
+    }
+  };
+  const uint32_t cnt = slot_topk(s, n_p, k, flt, off, false, fill);
+  write_slot(s, cnt, slot, k, off, row_ids, cand_d, cand_id, cand_cnt);
+}
+
+// residual queries of `nq` queries x np probes: out[(q np + pi) d + t] = queries[q d + t] - c_{probe}[t]
+// (a probe id >= K is an empty slot of a search with minimum / maximum nprobes: its residual is 0)
+__global__ void rq_query_residual_kernel(const float* __restrict__ queries, uint64_t nq, int np, int d,
+                                         const float* __restrict__ centroids, int K,
+                                         const uint32_t* __restrict__ probe_ids, float* __restrict__ out) {
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= nq * np * d) return;
+  const uint64_t sl = g / d;
+  const int t = (int)(g % d);
+  const uint32_t p = probe_ids[sl];
+  out[g] = p < (uint32_t)K ? __fsub_rn(queries[(sl / np) * d + t], centroids[(size_t)p * d + t]) : 0.0f;
+}
+
+bool rq_scan_fits(int code_dim, int k) {
+  return smem_with_static(ivfrq_scan_kernel, rq_scan_smem_bytes(code_dim, k)) <= ctx().smem_optin;
+}
+
+void ivfrq_search(const IvfSearch& s, const float* rotation, int code_dim, const uint8_t* codes, const float* add,
+                  const float* scale) {
+  const int d = s.d, k = s.k;
+  const size_t smem = rq_scan_smem_bytes(code_dim, k);
+  if (!ivf_search_begin(s, smem_with_static(ivfrq_scan_kernel, smem),
+                        "IVF_RQ: the tables of code_dim %zu do not fit the scan's shared memory", (size_t)code_dim))
+    return;
+  const float sqrt_d = sqrtf((float)code_dim);  // (dim as f32 * num_bits as f32).sqrt(): the product is exact
+  const int q_minus_one = s.metric != METRIC_L2;  // the storage's metric: cosine / dot -> dist_q_c - 1.0
+  run_ivf_search(s, [&](const ScanSlots& sl) {
+    const int np = sl.np;
+    // the (query, probe) residuals are rotated in groups of queries that keep both buffers near 256 MB
+    const uint64_t per_q = (uint64_t)np * (d + code_dim) * sizeof(float);
+    const uint64_t qc = std::max<uint64_t>(1, std::min<uint64_t>(sl.qn, (256ull << 20) / per_q));
+    DevBuf<float> res(qc * np * d), rot(qc * np * code_dim);
+    set_smem(ivfrq_scan_kernel, smem);
+    for (uint64_t a = 0; a < sl.qn; a += qc) {
+      const uint64_t b = std::min(qc, sl.qn - a);
+      LB2_LAUNCH("rq_query_residual", rq_query_residual_kernel, cdiv(b * np * d, 256), 256, 0,
+                 s.queries + (sl.q0 + a) * d, b, np, d, s.centroids, s.K, sl.probe_ids + a * np, res.p);
+      rq_rotate_f32(rotation, code_dim, d, res.p, b * np, rot.p);
+      LB2_LAUNCH("rq_scan", ivfrq_scan_kernel, dim3(np, (unsigned)b), 256, smem, rot.p, code_dim, sqrt_d, q_minus_one,
+                 sl.probe_ids + a * np, sl.probe_dists + a * np, np, sl.offsets, codes, add, scale, s.row_ids, k,
+                 sl.cand_d + a * np * k, sl.cand_id + a * np * k, sl.cand_cnt + a * np, s.flt);
+    }
+  });
 }
 
 }  // namespace lb2

@@ -19,4 +19,10 @@ void rq_norm_sq_f32(const float* x, uint64_t m, int d, float* out);
 void rq_encode_f32(const float* rot, const float* residual, const float* dist_v_c, const uint32_t* part,
                    const float* cnorm_sq, const uint8_t* valid, uint64_t m, int d, int num_bits, int metric,
                    uint8_t* codes, float* add, float* scale);
+// IVF_RQ: rotation [code_dim][code_dim]; codes [n][code_dim / 8] and the add / scale factors [n] in partition order;
+// s.queries: f32 (normalised for cosine).  rq_scan_fits: the scan's tables and a k-slot fit shared memory.
+struct IvfSearch;
+bool rq_scan_fits(int code_dim, int k);
+void ivfrq_search(const IvfSearch& s, const float* rotation, int code_dim, const uint8_t* codes, const float* add,
+                  const float* scale);
 }  // namespace lb2

@@ -3,6 +3,7 @@
 // Replaces  ScalarQuantizer::update_bounds   sq.rs:67-89 (the bounds of ScalarQuantizer::build, :152-182)
 //           scale_to_u8                      sq.rs:263-277 (quantize / transform, and the query's codes,
 //                                            sq/storage.rs:404-430)
+//           SQDistCalculator::distance_all   sq/storage.rs:432-468 (the partition scan of a search)
 //
 // The bounds are a min / max: exact in f32 and widened to f64 afterwards, so any reduction order gives the
 // reference's fold.  The encoding is restated in f64 with explicitly rounded operations (no mul-add contraction).
@@ -11,7 +12,10 @@
 #include <vector>
 
 #include "common.cuh"
+#include "exact.cuh"
+#include "ivf_search.cuh"
 #include "sq.cuh"
+#include "topk.cuh"
 
 namespace lb2 {
 
@@ -75,6 +79,96 @@ __global__ void sq_encode_kernel(const float* __restrict__ x, uint64_t count, do
 
 void sq_encode_f32(const float* x, uint64_t count, double lower, double upper, uint8_t* codes) {
   if (count) LB2_LAUNCH("sq_encode", sq_encode_kernel, cdiv(count, 256), 256, 0, x, count, lower, upper, codes);
+}
+
+// ------------------------------------------------------------------------------------------------
+// IVF_SQ: SQDistCalculator::distance_all (lance-index/src/vector/sq/storage.rs:432-468) + top-k.
+// A row's distance is an exact u32 integer sum over its d code bytes -- l2_distance_uint_scalar
+// (lance-linalg/src/distance/l2.rs:44-49) for L2 / cosine, the u8 dot (dot.rs:152-161) for dot -- so
+// any split of a row over lanes and any reduction order gives the reference's integer; d * 255^2 < 2^32
+// (checked on the host) keeps it from wrapping.  Then inverse_scalar_dist (sq.rs:279-287) in f32:
+// (f * (rf * rf)) / 255^2 with f = s as f32 (dot: 1 - s as f32); r2 = rf * rf comes from the host.
+// 8 lanes per row; VEC4: d % 16 == 0, 16-byte loads, otherwise 4-byte words.
+// ------------------------------------------------------------------------------------------------
+template <int METRIC>
+__device__ __forceinline__ uint32_t sq_word(uint32_t x, uint32_t q, uint32_t acc) {
+  if (METRIC == METRIC_DOT) return __dp4a(x, q, acc);
+  const uint32_t df = __vabsdiffu4(x, q);
+  return __dp4a(df, df, acc);
+}
+
+template <int METRIC, bool VEC4>
+__global__ void __maxnreg__(128)  // 256 threads; under __launch_bounds__(256) ptxas spills the selection's state
+ivfsq_scan_kernel(const uint8_t* __restrict__ qcodes, int d, float r2, const uint32_t* __restrict__ probe_ids, int np,
+                  const uint64_t* __restrict__ part_offsets, const uint8_t* __restrict__ codes,
+                  const uint64_t* __restrict__ row_ids, int k, float* __restrict__ cand_d, uint64_t* __restrict__ cand_id,
+                  uint32_t* __restrict__ cand_cnt, const ScanFilter flt) {
+  extern __shared__ uint4 sq_smem[];
+  const int nw = d >> 2;                                   // 4-byte words per row
+  uint32_t* qw = reinterpret_cast<uint32_t*>(sq_smem);     // the query's codes, [nw] words (16-byte aligned)
+  const SlotSmem s(qw + ((nw + 3) & ~3), k + 1);
+  const int tid = threadIdx.x, l = tid & 7;
+  const unsigned gmask = 0xffu << (8 * ((tid >> 3) & 3));  // the row's 8 lanes
+  size_t qi, slot;
+  uint32_t p, n_p;
+  uint64_t off;
+  if (!slot_partition(probe_ids, np, part_offsets, cand_cnt, qi, slot, p, off, n_p)) return;
+  const uint32_t* qsrc = reinterpret_cast<const uint32_t*>(qcodes + qi * (size_t)d);  // d % 4 == 0: word aligned
+  for (int t = tid; t < nw; t += 256) qw[t] = qsrc[t];
+  __syncthreads();
+  auto fill = [&](uint32_t c0, uint32_t clen) {
+    for (uint32_t j = tid >> 3; j < clen; j += 32) {  // 32 rows per pass, 8 lanes each
+      const uint8_t* row = codes + (off + c0 + j) * (uint64_t)d;
+      uint32_t acc = 0;
+      if constexpr (VEC4) {
+        const uint4* r4 = reinterpret_cast<const uint4*>(row);
+        const uint4* q4 = reinterpret_cast<const uint4*>(qw);
+        for (int w = l; w < (nw >> 2); w += 8) {
+          const uint4 x = __ldg(r4 + w), q = q4[w];
+          acc = sq_word<METRIC>(x.x, q.x, acc);
+          acc = sq_word<METRIC>(x.y, q.y, acc);
+          acc = sq_word<METRIC>(x.z, q.z, acc);
+          acc = sq_word<METRIC>(x.w, q.w, acc);
+        }
+      } else {
+        const uint32_t* r1 = reinterpret_cast<const uint32_t*>(row);
+        for (int w = l; w < nw; w += 8) acc = sq_word<METRIC>(__ldg(r1 + w), qw[w], acc);
+      }
+#pragma unroll
+      for (int o = 4; o >= 1; o >>= 1) acc += __shfl_xor_sync(gmask, acc, o, 8);
+      if (l == 0) {
+        float f = __uint2float_rn(acc);
+        if (METRIC == METRIC_DOT) f = __fsub_rn(1.0f, f);
+        const float dist = __fdiv_rn(__fmul_rn(f, r2), 65025.0f);
+        s.ukey[j] = (uint32_t)total_order_key(dist) ^ 0x80000000u;
+      }
+    }
+  };
+  const uint32_t cnt = slot_topk(s, n_p, k, flt, off, false, fill);
+  write_slot(s, cnt, slot, k, off, row_ids, cand_d, cand_id, cand_cnt);
+}
+
+void ivfsq_search(const IvfSearch& s, const uint8_t* codes, float r2, const uint8_t* qcodes) {
+  const int d = s.d, k = s.k;
+  const size_t smem = (size_t)(d + 15) / 16 * 16 + slot_smem_bytes(k);
+  auto with_kernel = [&](auto f) {
+    const bool vec4 = d % 16 == 0;
+    if (s.metric == METRIC_DOT) {
+      if (vec4) f(ivfsq_scan_kernel<METRIC_DOT, true>); else f(ivfsq_scan_kernel<METRIC_DOT, false>);
+    } else {  // cosine: L2 on the normalised vectors' codes (sq/storage.rs:436-440)
+      if (vec4) f(ivfsq_scan_kernel<METRIC_L2, true>); else f(ivfsq_scan_kernel<METRIC_L2, false>);
+    }
+  };
+  size_t need = 0;
+  with_kernel([&](auto kern) { need = smem_with_static(kern, smem); });
+  if (!ivf_search_begin(s, need, "dimension %zu too large for the SQ scan", (size_t)d)) return;
+  run_ivf_search(s, [&](const ScanSlots& sl) {
+    with_kernel([&](auto kern) {
+      set_smem(kern, smem);
+      LB2_LAUNCH("sq_scan", kern, dim3(sl.np, (unsigned)sl.qn), 256, smem, qcodes + sl.q0 * d, d, r2, sl.probe_ids,
+                 sl.np, sl.offsets, codes, s.row_ids, k, sl.cand_d, sl.cand_id, sl.cand_cnt, s.flt);
+    });
+  });
 }
 
 }  // namespace lb2

@@ -8,4 +8,8 @@ void sq_bounds_f32(const float* x, uint64_t count, double* lower, double* upper)
 // scale_to_u8 (sq.rs:263-277) of x[count]: ((v - lower) * 255 / (upper - lower)) in f64, `as u8` (truncation toward
 // zero, saturating, NaN -> 0); every code is 0 when lower == upper.  Stream-ordered, no synchronisation.
 void sq_encode_f32(const float* x, uint64_t count, double lower, double upper, uint8_t* codes);
+// codes: the index's SQ codes [n][d] in partition order; qcodes: the queries' codes [nq][d] under the same bounds;
+// r2 = rf * rf with rf = (float)(upper - lower); s.queries: f32 (normalised for cosine), for the probe selection
+struct IvfSearch;
+void ivfsq_search(const IvfSearch& s, const uint8_t* codes, float r2, const uint8_t* qcodes);
 }  // namespace lb2

@@ -15,7 +15,7 @@ from oracle import binding as ob
 
 pytestmark = pytest.mark.gpu
 NT = 16
-SLAB = 32768          # queries per scan launch (grid.y limit, search.cu)
+SLAB = 32768          # queries per scan launch (grid.y limit, ivf_search.cuh)
 TYPES = ("f32", "f16", "bf16", "u8")
 
 

@@ -225,7 +225,7 @@ def test_reporting_the_tick_of_convergence_is_independent_of_read_timing():
         assert all(r.executed_active == last_real for r in ranks)
 
 
-# ---- 3. the k + 1 rule of every top-k path (DESIGN.md section 5 "Ties at the k-th distance"; search.cu) ----------
+# ---- 3. the k + 1 rule of every top-k path (DESIGN.md section 5 "Ties at the k-th distance"; topk.cuh) ----------
 # The GPU selects k + 1 candidates per list.  Argument: when the (k+1)-th smallest distance differs from the k-th, the
 # reference's BinaryHeap result (flat/index.rs:82-177, restated in the oracle) is the unique set of the k smallest --
 # whatever order the rows were pushed in -- so any selection algorithm returns it; only when they are equal does the

@@ -23,7 +23,7 @@ from sq_reference import ivfsq_search, sq_bounds, sq_encode
 pytestmark = pytest.mark.gpu
 
 U64MAX = np.iinfo(np.uint64).max
-SLAB = 32768                          # queries per scan launch (ivf_search, search.cu)
+SLAB = 32768                          # queries per scan launch (ivf_search, ivf_search.cu)
 GROUP_BYTES = 256 << 20               # ivfrq_search_f32 rotates (query, probe) residuals ~256 MB at a time
 SIZES = (0, 31, 32, 33, 4097)         # every probed partition: none, tail only, 32-row blocks, both, past 4096 rows
 
