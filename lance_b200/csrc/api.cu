@@ -312,7 +312,7 @@ lb2_status lb2_distance_batch(const void* from, const void* to, uint64_t n, uint
     sync_stream();
     return LB2_OK;
   }
-  assign_f32(f.get(), 1, d, t.get(), (int)n, m, nullptr, nullptr, nullptr, nullptr, o.get());
+  centroid_distances(f.get(), 1, d, t.get(), (int)n, m, o.get());
   o.commit();
   sync_stream();
   LB2_API_END
@@ -340,25 +340,15 @@ lb2_status lb2_kmeans_train(const void* data, uint64_t n, uint32_t d, lb2_dtype 
   LB2_REQUIRE(current_comm() || n >= k, "KMeans: can not train %u centroids with %llu vectors, choose a smaller K (< %llu) instead",
               k, (unsigned long long)n, (unsigned long long)n);
   // free fn train_kmeans (kmeans.rs:1328-1344); sharded: every rank contributes its share of the cap
-  const uint64_t kr0 = current_comm() ? current_comm()->nranks : 1;
-  const uint64_t cap = (params->sample_rate * k + kr0 - 1) / kr0;
+  const uint64_t nranks = comm_nranks();
+  const uint64_t cap = (params->sample_rate * k + nranks - 1) / nranks;
   const uint64_t rows = n > cap ? cap : n;
   VecIn x(data, (size_t)rows * d, dtype);
   VecIn init(params->init_centroids, (size_t)k * d, model_dtype(dtype));
   DevBuf<float> cent((size_t)k * d);
   std::vector<double> loss;
   std::vector<uint32_t> iters;
-  const uint64_t kr = current_comm() ? current_comm()->nranks : 1;  // sharded: every rank passes its rows
-  if (k > 256 && params->hierarchical_k > 1 && !params->init_centroids) {  // kmeans.rs:1027
-    hierarchical_train(x.get(), rows, d, k, m, params->balance_factor / (float)(rows * kr),
-                       (int)params->max_iters, params->tolerance, (int)params->hierarchical_k, params->seed, cent.p);
-    loss.assign(1, 0.0);
-    iters.assign(1, 0);
-  } else {
-    lloyd_train(x.get(), rows, d, 1, d, k, m, params->balance_factor / (float)(rows * kr),
-                (int)params->max_iters, params->tolerance, params->seed, init.get(), cent.p, &loss,
-                &iters);
-  }
+  train_kmeans(x.get(), rows, d, k, m, *params, init.get(), cent.p, &loss, &iters);
   VecOut o(centroids_out, (size_t)k * d, model_dtype(dtype));
   d2d(o.get(), cent.p, (size_t)k * d);
   o.commit();
@@ -383,7 +373,7 @@ lb2_status lb2_compute_partitions(const void* centroids, uint32_t k, uint32_t d,
     src.start_resident_copy();
     for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
       assign_f32(xf, rows, d, c.get(), k, m, nullptr, p.get() + r0, dd.get() ? dd.get() + r0 : nullptr,
-                 v.get() ? v.get() + r0 : nullptr, nullptr, xnat, (int)src.dtype());
+                 v.get() ? v.get() + r0 : nullptr, xnat, (int)src.dtype());
     });
   }
   p.commit(); dd.commit(); v.commit();

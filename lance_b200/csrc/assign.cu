@@ -408,7 +408,7 @@ generic_kernel(const float* __restrict__ x, uint64_t n, int d, const float* __re
 // ------------------------------------------------------------------------------------------------
 // host dispatch
 // ------------------------------------------------------------------------------------------------
-template <int METRIC>
+template <int METRIC, bool WRITE_ALL>
 static void assign_dispatch(const float* x, uint64_t n, int d, const float* cent, int K,
                             const float* bias, uint32_t* part, float* dist,
                             uint8_t* valid, float* all_out, const uint8_t* active, TcWorkspace& ws) {
@@ -423,15 +423,9 @@ static void assign_dispatch(const float* x, uint64_t n, int d, const float* cent
                cent, K, d, Kp, cT.get());
     const size_t smem = sizeof(float) * (64 * (d + 1) + (size_t)d * 64);
     const unsigned grid = cdiv(n, 64);
-    if (all_out) {
-      set_smem(assign_tile_kernel<METRIC, true, 4>, smem);
-      LB2_LAUNCH("assign_exact", (assign_tile_kernel<METRIC, true, 4>), grid, 256, smem, x, n, d,
-                 cT.get(), K, Kp, bias, part, dist, valid, all_out, active, nullptr, nullptr, 0u, 0xffffffffu);
-    } else {
-      set_smem(assign_tile_kernel<METRIC, false, 4>, smem);
-      LB2_LAUNCH("assign_exact", (assign_tile_kernel<METRIC, false, 4>), grid, 256, smem, x, n, d,
-                 cT.get(), K, Kp, bias, part, dist, valid, all_out, active, nullptr, nullptr, 0u, 0xffffffffu);
-    }
+    set_smem(assign_tile_kernel<METRIC, WRITE_ALL, 4>, smem);
+    LB2_LAUNCH("assign_exact", (assign_tile_kernel<METRIC, WRITE_ALL, 4>), grid, 256, smem, x, n, d,
+               cT.get(), K, Kp, bias, part, dist, valid, all_out, active, nullptr, nullptr, 0u, 0xffffffffu);
     return;
   }
   // 16 rows per CTA halve the centroid re-reads from L2; wide vectors fall back to 8 rows
@@ -439,17 +433,13 @@ static void assign_dispatch(const float* x, uint64_t n, int d, const float* cent
   const size_t smem = sizeof(float) * (r16 ? 16 : 8) * (size_t)d;
   if (smem > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the exact kernel", d);
   const unsigned grid = cdiv(n, r16 ? 16 : 8);
-#define LB2_GENERIC(WA, RR)                                                                        \
-  do {                                                                                             \
-    set_smem(generic_kernel<METRIC, WA, RR>, smem);                                                \
-    LB2_LAUNCH("assign_exact_generic", (generic_kernel<METRIC, WA, RR>), grid, 256, smem, x, n, d, \
-               cent, K, bias, part, dist, valid, all_out, active, nullptr, nullptr);               \
+#define LB2_GENERIC(RR)                                                                                \
+  do {                                                                                                 \
+    set_smem(generic_kernel<METRIC, WRITE_ALL, RR>, smem);                                             \
+    LB2_LAUNCH("assign_exact_generic", (generic_kernel<METRIC, WRITE_ALL, RR>), grid, 256, smem, x, n, \
+               d, cent, K, bias, part, dist, valid, all_out, active, nullptr, nullptr);                \
   } while (0)
-  if (all_out) {
-    if (r16) LB2_GENERIC(true, 16); else LB2_GENERIC(true, 8);
-  } else {
-    if (r16) LB2_GENERIC(false, 16); else LB2_GENERIC(false, 8);
-  }
+  if (r16) LB2_GENERIC(16); else LB2_GENERIC(8);
 #undef LB2_GENERIC
 }
 
@@ -525,8 +515,8 @@ void assign_rows_f32(const float* x, uint64_t n_max, int d, const float* cent, i
 
 void assign_f32_ex(const float* x, uint64_t n, int d, const float* cent, int K, int metric,
                    const float* bias, uint32_t* part, float* dist, uint8_t* valid,
-                   float* all_out, const uint8_t* active, TcWorkspace& ws, const void* x16, int x16_dtype) {
-  if (!all_out && n >= 256 && tc_assign_supported(n, d, K, metric, x)) {
+                   const uint8_t* active, TcWorkspace& ws, const void* x16, int x16_dtype) {
+  if (n >= 256 && tc_assign_supported(n, d, K, metric, x)) {
     // tensor-core filter + exact re-rank: bit-identical outputs, ~10x less FP32 work
     // large inputs in chunks of <= 2^20 rows (<= 4 GB of vectors): bounds the per-call scratch (row norms,
     // verdicts, the 3x-wide refinement rows) without changing any output
@@ -544,15 +534,21 @@ void assign_f32_ex(const float* x, uint64_t n, int d, const float* cent, int K, 
     return;
   }
   if (metric == METRIC_DOT)
-    assign_dispatch<METRIC_DOT>(x, n, d, cent, K, bias, part, dist, valid, all_out, active, ws);
+    assign_dispatch<METRIC_DOT, false>(x, n, d, cent, K, bias, part, dist, valid, nullptr, active, ws);
   else
-    assign_dispatch<METRIC_L2>(x, n, d, cent, K, bias, part, dist, valid, all_out, active, ws);
+    assign_dispatch<METRIC_L2, false>(x, n, d, cent, K, bias, part, dist, valid, nullptr, active, ws);
 }
 void assign_f32(const float* x, uint64_t n, int d, const float* cent, int K, int metric,
-                const float* bias, uint32_t* part, float* dist, uint8_t* valid, float* all_out,
-                const void* x16, int x16_dtype) {
+                const float* bias, uint32_t* part, float* dist, uint8_t* valid, const void* x16, int x16_dtype) {
   TcWorkspace ws;
-  assign_f32_ex(x, n, d, cent, K, metric, bias, part, dist, valid, all_out, nullptr, ws, x16, x16_dtype);
+  assign_f32_ex(x, n, d, cent, K, metric, bias, part, dist, valid, nullptr, ws, x16, x16_dtype);
+}
+void centroid_distances(const float* x, uint64_t n, int d, const float* cent, int K, int metric, float* out) {
+  TcWorkspace ws;
+  if (metric == METRIC_DOT)
+    assign_dispatch<METRIC_DOT, true>(x, n, d, cent, K, nullptr, nullptr, nullptr, nullptr, out, nullptr, ws);
+  else
+    assign_dispatch<METRIC_L2, true>(x, n, d, cent, K, nullptr, nullptr, nullptr, nullptr, out, nullptr, ws);
 }
 
 template <int DS, int METRIC>

@@ -3,19 +3,21 @@
 #include <stdint.h>
 namespace lb2 {
 struct TcWorkspace;
-// part/dist/valid are [n]; all_out (nullable) receives the full [n][K] distance matrix instead.
-// bias (nullable, [K]) is added for the comparison only (kernels.rs:92-111).
+// part/dist/valid are [n] (dist and valid nullable): each row's nearest centroid, its distance, and 0 in valid where
+// no centroid is at a finite distance.  bias (nullable, [K]) is added for the comparison only (kernels.rs:92-111).
 // x16 (nullable): the same rows as x in their own element type x16_dtype (LB2_F16 / LB2_BF16); the tensor-core
 // filter may read them instead of x (tc_assign.cu, "native 16-bit rows").
 void assign_f32(const float* x, uint64_t n, int d, const float* cent, int K, int metric,
-                const float* bias, uint32_t* part, float* dist, uint8_t* valid, float* all_out,
+                const float* bias, uint32_t* part, float* dist, uint8_t* valid,
                 const void* x16 = nullptr, int x16_dtype = 0);
 // same, with an optional device-side `active` flag (active[0] == 0 -> the kernels return immediately; used by the
 // Lloyd loop) and the caller's workspace (a training loop keeps one across iterations and its CUDA graph)
 void assign_f32_ex(const float* x, uint64_t n, int d, const float* cent, int K, int metric,
                    const float* bias, uint32_t* part, float* dist, uint8_t* valid,
-                   float* all_out, const uint8_t* active, TcWorkspace& ws,
+                   const uint8_t* active, TcWorkspace& ws,
                    const void* x16 = nullptr, int x16_dtype = 0);
+// the full [n][K] distance matrix, out[r * K + k] = dist(x[r], cent[k]), by the same exact kernels
+void centroid_distances(const float* x, uint64_t n, int d, const float* cent, int K, int metric, float* out);
 // exact tile kernel restricted to row_list[0 .. *row_count) (both on the device)
 void assign_rows_f32(const float* x, uint64_t n_max, int d, const float* cent, int K, int metric,
                      const float* bias, const uint32_t* row_list, const uint32_t* row_count,

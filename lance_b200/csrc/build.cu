@@ -70,12 +70,12 @@ void pq_train_dev(const float* data, uint64_t n, int d, int metric, const lb2_pq
   LB2_REQUIRE(current_comm() || n >= (uint64_t)K, "Not enough rows to train PQ. Requires %d rows but only %llu available",
               K, (unsigned long long)n);
   // free fn train_kmeans (kmeans.rs:1328-1340): first sample_rate*k rows (per-rank share when sharded)
-  const uint64_t nranks = current_comm() ? current_comm()->nranks : 1;
+  const uint64_t nranks = comm_nranks();
   const uint64_t cap = (p->sample_rate * K + nranks - 1) / nranks;
   const uint64_t rows = n > cap ? cap : n;
   InArg<float> init(p->codebook, (size_t)M * K * (d / M));
-  lloyd_train(data, rows, d, M, d / M, K, metric == METRIC_DOT ? METRIC_DOT : METRIC_L2, 0.0f,
-              (int)p->max_iters, 1e-4, p->seed, init.get(), codebook, nullptr, iters);
+  const LloydParams lp{metric == METRIC_DOT ? METRIC_DOT : METRIC_L2, 0.0f, (int)p->max_iters, 1e-4, p->seed};
+  lloyd_train(data, rows, d, M, d / M, K, lp, init.get(), codebook, nullptr, iters);
 }
 
 namespace {
@@ -96,99 +96,91 @@ struct EventSet {
     return t;
   }
 };
-// KMeans::new_with_params (kmeans.rs:1008-1030): hierarchical for k > 256, flat Lloyd otherwise
-void train_ivf(const float* xs, uint64_t s, int d, int K, int am, const lb2_kmeans_params& kp, uint64_t nranks,
-               const float* init, float* centroids, std::vector<double>* loss, std::vector<uint32_t>* iters) {
+// KMeans::new_with_params on the IVF training sample (train_kmeans).  Sharded build: the hierarchical tree is
+// thousands of small dependent Lloyd runs -- with a collective in every iteration it is latency-bound on the exchange.
+// The sample (K * sample_rate rows) is small next to the data, so when it fits every rank gathers ALL sample shards
+// (rank order) and trains the same tree on them without a communicator: identical arithmetic on identical input gives
+// bit-identical models on all ranks, and the splits train concurrently (kmeans.cu: SplitWorkers).  Otherwise: the
+// sharded tree.
+void train_ivf(const float* xs, uint64_t s, int d, int K, int am, const lb2_kmeans_params& kp, const float* init,
+               float* centroids, std::vector<double>* loss, std::vector<uint32_t>* iters) {
   check_redos(kp.redos, kp.balance_factor);
-  if (K > 256 && kp.hierarchical_k > 1 && !init) {
-    loss->assign(1, 0.0);
-    iters->assign(1, 0);
-    if (nranks > 1) {
-      // Sharded build: the hierarchical tree is thousands of small dependent Lloyd runs -- with a collective in
-      // every iteration it is latency-bound on the exchange.  The sample (K * sample_rate rows) is small next to
-      // the data, so when it fits every rank gathers ALL sample shards (rank order) and trains the same tree on
-      // them without a communicator: identical arithmetic on identical input gives bit-identical models on all
-      // ranks, and the splits train concurrently (kmeans.cu: SplitWorkers).  Otherwise: the sharded tree.
-      DevBuf<uint64_t> cnt_in(1), cnt_all(nranks);
-      h2d(cnt_in.p, &s, 1);
-      comm_allgather_bytes(cnt_in.p, cnt_all.p, sizeof(uint64_t));
-      std::vector<uint64_t> cnt(nranks);
-      d2h(cnt.data(), cnt_all.p, nranks);
-      sync_stream();
-      uint64_t total = 0, mx = 0;
-      for (uint64_t c : cnt) { total += c; mx = std::max(mx, c); }
-      size_t free_b = 0, total_b = 0;
-      cudaMemGetInfo(&free_b, &total_b);
-      const bool off = getenv("LB2_SHARDED_TREE") && *getenv("LB2_SHARDED_TREE");
-      if (!off && total < 0xffffffffull && (size_t)nranks * mx * d * 4 * 3 <= free_b) {
-        DevBuf<float> pad, all((size_t)nranks * mx * d);
-        const float* in = xs;
-        if (s < mx) {
-          pad.alloc((size_t)mx * d);
-          pad.zero();
-          if (s) d2d(pad.p, xs, (size_t)s * d);
-          in = pad.p;
-        }
-        comm_allgather_bytes(in, all.p, (size_t)mx * d * sizeof(float));
-        pad.release();
-        if (total != nranks * mx) {  // unequal shards: close the gaps (rank order is kept)
-          DevBuf<float> full(std::max<uint64_t>(total, 1) * d);
-          uint64_t o = 0;
-          for (uint64_t r = 0; r < nranks; ++r) {
-            if (cnt[r]) d2d(full.p + o * d, all.p + r * mx * d, cnt[r] * d);
-            o += cnt[r];
-          }
-          all = std::move(full);
-        }
-        Comm* saved = comm_swap(nullptr);
-        try {
-          hierarchical_train(all.p, total, d, K, am, kp.balance_factor / (float)total, (int)kp.max_iters, kp.tolerance,
-                             (int)kp.hierarchical_k, kp.seed, centroids);
-        } catch (...) {
-          comm_swap(saved);
-          throw;
-        }
-        comm_swap(saved);
-        return;
+  const uint64_t nranks = comm_nranks();
+  if (nranks > 1 && kmeans_uses_tree(K, kp, init)) {
+    DevBuf<uint64_t> cnt_in(1), cnt_all(nranks);
+    h2d(cnt_in.p, &s, 1);
+    comm_allgather_bytes(cnt_in.p, cnt_all.p, sizeof(uint64_t));
+    std::vector<uint64_t> cnt(nranks);
+    d2h(cnt.data(), cnt_all.p, nranks);
+    sync_stream();
+    uint64_t total = 0, mx = 0;
+    for (uint64_t c : cnt) { total += c; mx = std::max(mx, c); }
+    size_t free_b = 0, total_b = 0;
+    cudaMemGetInfo(&free_b, &total_b);
+    const bool off = getenv("LB2_SHARDED_TREE") && *getenv("LB2_SHARDED_TREE");
+    if (!off && total < 0xffffffffull && (size_t)nranks * mx * d * 4 * 3 <= free_b) {
+      DevBuf<float> pad, all((size_t)nranks * mx * d);
+      const float* in = xs;
+      if (s < mx) {
+        pad.alloc((size_t)mx * d);
+        pad.zero();
+        if (s) d2d(pad.p, xs, (size_t)s * d);
+        in = pad.p;
       }
+      comm_allgather_bytes(in, all.p, (size_t)mx * d * sizeof(float));
+      pad.release();
+      if (total != nranks * mx) {  // unequal shards: close the gaps (rank order is kept)
+        DevBuf<float> full(std::max<uint64_t>(total, 1) * d);
+        uint64_t o = 0;
+        for (uint64_t r = 0; r < nranks; ++r) {
+          if (cnt[r]) d2d(full.p + o * d, all.p + r * mx * d, cnt[r] * d);
+          o += cnt[r];
+        }
+        all = std::move(full);
+      }
+      Comm* saved = comm_swap(nullptr);
+      try {
+        train_kmeans(all.p, total, d, K, am, kp, init, centroids, loss, iters);
+      } catch (...) {
+        comm_swap(saved);
+        throw;
+      }
+      comm_swap(saved);
+      return;
     }
-    hierarchical_train(xs, s, d, K, am, kp.balance_factor / (float)(s * nranks), (int)kp.max_iters, kp.tolerance,
-                       (int)kp.hierarchical_k, kp.seed, centroids);
-  } else {
-    lloyd_train(xs, s, d, 1, d, K, am, kp.balance_factor / (float)(s * nranks), (int)kp.max_iters, kp.tolerance,
-                kp.seed, init, centroids, loss, iters);
   }
+  train_kmeans(xs, s, d, K, am, kp, init, centroids, loss, iters);
 }
 }  // namespace
 
 // The IVF stage of every build, in two halves so that IVF_PQ can gather its own sample in between:
 // (a) the IVF training sample's rows (ivf.rs:1237-1241), to be gathered with gather_finite_sample (rows that are not
 // finite dropped, normalised first under cosine);
-static std::vector<uint64_t> ivf_sample_rows(uint64_t n, int K, const lb2_kmeans_params& kp, uint64_t seed,
-                                             uint64_t nranks) {
+static std::vector<uint64_t> ivf_sample_rows(uint64_t n, int K, const lb2_kmeans_params& kp, uint64_t seed) {
+  const uint64_t nranks = comm_nranks();  // sharded build: this rank's share
   return sample_rows(n, std::min<uint64_t>(n, ((uint64_t)K * kp.sample_rate + nranks - 1) / nranks), seed);
 }
 // (b) after the caller started the bulk copy: train on the s gathered rows, centroids rounded to the column's type
 static void train_ivf_model(const float* sample, uint64_t s, lb2_index* ix, const lb2_kmeans_params& kp,
-                            uint64_t nranks, std::vector<double>* loss, std::vector<uint32_t>* iters) {
+                            std::vector<double>* loss, std::vector<uint32_t>* iters) {
   const int K = ix->K, d = ix->d;
-  LB2_REQUIRE(nranks > 1 || s >= (uint64_t)K, "KMeans: can not train %d centroids with %llu finite vectors", K,
+  LB2_REQUIRE(comm_nranks() > 1 || s >= (uint64_t)K, "KMeans: can not train %d centroids with %llu finite vectors", K,
               (unsigned long long)s);
   TagScope tg("ivf_train");
   VecIn init(kp.init_centroids, (size_t)K * d, model_dtype(ix->dtype));
-  train_ivf(sample, s, d, K, ix->metric == METRIC_DOT ? METRIC_DOT : METRIC_L2, kp, nranks, init.get(),
-            ix->centroids.p, loss, iters);
+  train_ivf(sample, s, d, K, ix->metric == METRIC_DOT ? METRIC_DOT : METRIC_L2, kp, init.get(), ix->centroids.p, loss,
+            iters);
   round_model(ix->centroids.p, (size_t)K * d, ix->dtype);
 }
 // both halves, with the bulk copy started in between (IVF_FLAT, IVF_SQ, IVF_RQ)
-static void train_ivf_stage(Source& src, lb2_index* ix, const lb2_kmeans_params& kp, uint64_t seed, uint64_t nranks,
+static void train_ivf_stage(Source& src, lb2_index* ix, const lb2_kmeans_params& kp, uint64_t seed,
                             std::vector<double>* loss, std::vector<uint32_t>* iters) {
   TagScope tg("ivf_train");
-  std::vector<uint64_t> rows = ivf_sample_rows(src.n(), ix->K, kp, seed, nranks);
+  std::vector<uint64_t> rows = ivf_sample_rows(src.n(), ix->K, kp, seed);
   DevBuf<float> sample;
   const uint64_t s = gather_finite_sample(src, rows, ix->metric == METRIC_COSINE, sample);
   src.start_resident_copy();  // host rows: the bulk copy runs on its own stream while the centroids train
-  train_ivf_model(sample.p, s, ix, kp, nranks, loss, iters);
+  train_ivf_model(sample.p, s, ix, kp, loss, iters);
 }
 
 // the stage times of a build from its events: start, IVF trained, [quantizer trained,] transformed, grouped (IVF_FLAT
@@ -221,8 +213,7 @@ static const float* normalize_assign(const float* xf, const void* xnat, int dtyp
     xp = normbuf.p;
     xnat = nullptr;
   }
-  assign_f32(xp, rows, d, cent, K, m == METRIC_DOT ? METRIC_DOT : METRIC_L2, nullptr, part, dist, valid, nullptr,
-             xnat, dtype);
+  assign_f32(xp, rows, d, cent, K, m == METRIC_DOT ? METRIC_DOT : METRIC_L2, nullptr, part, dist, valid, xnat, dtype);
   return xp;
 }
 
@@ -421,8 +412,7 @@ lb2_status lb2_ivfflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype
   LB2_REQUIRE(d % 4 == 0, "IVF_FLAT needs a dimension that is a multiple of 4");
   const int m = metric_of(metric);
   const int K = params->num_partitions;
-  const uint64_t nranks = current_comm() ? current_comm()->nranks : 1;
-  LB2_REQUIRE(K > 0 && (nranks > 1 || n >= (uint64_t)K), "KMeans: can not train %d centroids with %llu vectors", K,
+  LB2_REQUIRE(K > 0 && (comm_nranks() > 1 || n >= (uint64_t)K), "KMeans: can not train %d centroids with %llu vectors", K,
               (unsigned long long)n);
   EventSet ev(4);
   ev.record(0);
@@ -430,7 +420,7 @@ lb2_status lb2_ivfflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype
   std::unique_ptr<lb2_index> ix = make_index(IndexKind::FLAT, K, d, m, dtype);
   std::vector<double> loss;
   std::vector<uint32_t> iters;
-  train_ivf_stage(src, ix.get(), params->ivf, params->seed, nranks, &loss, &iters);
+  train_ivf_stage(src, ix.get(), params->ivf, params->seed, &loss, &iters);
   ev.record(1);
   DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
   DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1));
@@ -475,7 +465,7 @@ lb2_status lb2_ivfsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   std::vector<double> loss;
   std::vector<uint32_t> iters;
   // 1. IVF: the same stage as lb2_ivfflat_build (same sample, seed, training)
-  train_ivf_stage(src, ix.get(), params->ivf, params->seed, 1, &loss, &iters);
+  train_ivf_stage(src, ix.get(), params->ivf, params->seed, &loss, &iters);
   ev.record(1);
   // 2. ScalarQuantizer::build (sq.rs:152-182) on sample_rate * 2^num_bits rows (builder.rs:410-421), normalised
   //    under cosine, rows that are not finite dropped (builder.rs:436), no residuals (quantizer.rs:52).  The bounds
@@ -535,7 +525,7 @@ lb2_status lb2_ivfrq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   std::vector<double> loss;
   std::vector<uint32_t> iters;
   // 1. IVF: the same stage as lb2_ivfflat_build (same sample, seed, training)
-  train_ivf_stage(src, ix.get(), params->ivf, params->seed, 1, &loss, &iters);
+  train_ivf_stage(src, ix.get(), params->ivf, params->seed, &loss, &iters);
   ev.record(1);
   // 2. RabitQuantizer::new (bq/builder.rs:52-70): the rotation, from seed + 1
   {
@@ -577,7 +567,7 @@ lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   LB2_REQUIRE(data && params && out, "null argument");
   const int m = metric_of(metric);
   const int K = params->num_partitions, M = params->pq.num_sub_vectors;
-  const uint64_t nranks = current_comm() ? current_comm()->nranks : 1;  // sharded build: this rank's rows
+  const uint64_t nranks = comm_nranks();  // sharded build: this rank's rows
   LB2_REQUIRE(K > 0 && (nranks > 1 || n >= (uint64_t)K), "KMeans: can not train %d centroids with %llu vectors", K,
               (unsigned long long)n);
   check_pq_shape(d, M, params->pq.num_bits, PqUse::ENCODE);
@@ -618,7 +608,7 @@ lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
             std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tr0).count());
   };
   {
-    std::vector<uint64_t> rows = ivf_sample_rows(n, K, params->ivf, params->seed, nranks);
+    std::vector<uint64_t> rows = ivf_sample_rows(n, K, params->ivf, params->seed);
     stamp("sample_rows(ivf)");
     s_ivf = gather_finite_sample(src, rows, m == METRIC_COSINE, sample_ivf);
     stamp("gather(ivf sample)");
@@ -638,7 +628,7 @@ lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   if (trace) fprintf(stderr, "[lb2 build] %-22s +%.3f ms (host, no sync)\n", "bulk copy issued",
                      std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tr0).count());
   // 1. IVF
-  train_ivf_model(sample_ivf.p, s_ivf, ix.get(), params->ivf, nranks, &ivf_loss, &ivf_iters);
+  train_ivf_model(sample_ivf.p, s_ivf, ix.get(), params->ivf, &ivf_loss, &ivf_iters);
   stamp("ivf trained");
   if (pq_deferred) {
     if (src.finish_async_sample()) {
@@ -654,7 +644,7 @@ lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
     TagScope tg("pq_train");
     if (m != METRIC_DOT && s_pq) {
       DevBuf<uint32_t> part(s_pq);
-      assign_f32(sample_pq.p, s_pq, d, ix->centroids.p, K, METRIC_L2, nullptr, part.p, nullptr, nullptr, nullptr);
+      assign_f32(sample_pq.p, s_pq, d, ix->centroids.p, K, METRIC_L2, nullptr, part.p, nullptr, nullptr);
       LB2_LAUNCH("residual", residual_kernel, cdiv(s_pq * d, 256), 256, 0, sample_pq.p, ix->centroids.p,
                  part.p, s_pq, (int)d, sample_pq.p);
     }

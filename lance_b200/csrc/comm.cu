@@ -124,6 +124,15 @@ void comm_broadcast_bytes(void* buf, size_t bytes, int root) {
   if (!c || c->nranks <= 1 || bytes == 0) return;
   nccl_check(api().Broadcast(buf, buf, bytes, ncclUint8, root, (ncclComm_t)c->handle, ctx().stream), "ncclBroadcast");
 }
+void sum_over_ranks(std::vector<uint32_t>& v) {
+  Comm* cm = current_comm();
+  if (!cm || cm->nranks <= 1 || v.empty()) return;
+  DevBuf<uint32_t> d(v.size());
+  h2d(d.p, v.data(), v.size());
+  comm_allreduce_u32(d.p, v.size(), RedOp::Sum);
+  d2h(v.data(), d.p, v.size());
+  sync_stream();
+}
 
 }  // namespace lb2
 

@@ -7,7 +7,7 @@
 #include "comm.cuh"
 #include "index.cuh"
 #include "ivf_search.cuh"
-#include "kmeans.cuh"
+#include "member_sort.cuh"
 #include "rq.cuh"
 #include "scan.cuh"
 #include "sq.cuh"

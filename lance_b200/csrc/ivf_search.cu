@@ -120,7 +120,7 @@ void find_partitions_f32(const float* centroids, int K, int d, int metric, const
                          uint64_t nq, int nprobes, uint32_t* ids, float* dists) {
   if (nq == 0) return;
   DevBuf<float> all((size_t)nq * K);
-  assign_f32(queries, nq, d, centroids, K, metric, nullptr, nullptr, nullptr, nullptr, all.p);
+  centroid_distances(queries, nq, d, centroids, K, metric, all.p);
   LB2_LAUNCH("select_probes", select_probes_kernel, (unsigned)nq, 128, 0, all.p, K, nprobes, ids, dists);
 }
 
@@ -188,8 +188,7 @@ static void ivf_search_probed(const IvfSearch& s, ScanRef scan) {
   DevBuf<uint32_t> pids(std::min(qs, nq) * L), nsearch(std::min(qs, nq)), shortcut(std::min(qs, nq)), nmax(1);
   for (uint64_t q0 = 0; q0 < nq; q0 += qs) {
     const uint64_t qn = std::min(qs, nq - q0);
-    assign_f32(s.queries + q0 * d, qn, d, s.centroids, K, probe_metric(s.metric), nullptr, nullptr, nullptr, nullptr,
-               all.p);
+    centroid_distances(s.queries + q0 * d, qn, d, s.centroids, K, probe_metric(s.metric), all.p);
     rank_probes(all.p, qn, K, L, pids.p, pd.p);
     uint32_t* nprobes_out = pr.nprobes_out ? pr.nprobes_out + q0 : nullptr;
     int np = L;

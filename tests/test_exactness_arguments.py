@@ -1,11 +1,11 @@
 """Arguments the device code relies on, checked on the CPU (no GPU, no product code; section 3 is at the end).
 
-1. Order-independent sums (DESIGN.md section 3; kmeans.cu `update_body_warp` / `stats_body` fast paths): the reference
+1. Order-independent sums (DESIGN.md section 3; lloyd.cu `update_body_warp` / `stats_body` fast paths): the reference
    adds a cluster's members sequentially (f32 centroid sums kmeans.rs:388-418, f64 loss :266-280).  If every term is an
    integer multiple of 2^g and sum|term| < 2^(g+p) (p = 24 for f32, 53 for f64) no addition of ANY association rounds,
    so a parallel tree reduction returns the sequential result bit for bit.  Outside the condition it does not.
 
-2. Convergence through progress words (DESIGN.md section 3; kmeans.cu `PollWords`, `epilogue_kernel`): a problem
+2. Convergence through progress words (DESIGN.md section 3; lloyd.cu `PollWords`, `epilogue_kernel`): a problem
    posts iteration << 1 | active only while it is active, so its last word names the iteration that converged it;
    the host resets the word to 1 and, after enqueuing iteration `it`, stops once every problem converged at an
    iteration <= it - 1.  A thread-per-rank simulation checks (a) that a single rank always stops, at most one no-op
@@ -36,7 +36,7 @@ def _seq_sum(v, dtype):
 
 
 def _granule(v):
-    """largest g with every non-zero term a multiple of 2^g (kmeans.cu pow2_granule)"""
+    """largest g with every non-zero term a multiple of 2^g (lloyd.cu pow2_granule)"""
     g = None
     for t in v:
         if t == 0:

@@ -1,7 +1,7 @@
 """GPU parity tests: the CUDA path (through the C ABI) against the CPU oracle on the same seeded
 inputs.  Integer outputs (partition ids, PQ codes, probe ids) and f32 L2/Dot/ADC distances must be
 BIT-EXACT; trained models are bit-exact given the same initial centroids (our training is
-deterministic by construction, see lance_b200/csrc/kmeans.cu)."""
+deterministic by construction, see lance_b200/csrc/lloyd.cu)."""
 import numpy as np
 import pytest
 

@@ -1,7 +1,7 @@
 """Every execution variant of the device Lloyd loop, and the grouping sort past its one-launch limits, pinned bit
 for bit to the CPU oracle.
 
-`lloyd_train` (lance_b200/csrc/kmeans.cu) promises the reference's model for the same initial centroids: the same
+`lloyd_train` (lance_b200/csrc/lloyd.cu) promises the reference's model for the same initial centroids: the same
 centroid bits, the same f64 loss and the same iteration count.  It reaches that promise by many routes:
   * fused: the whole run in one `lloyd_small_kernel` launch (K <= 16, n <= 16384, n*K*d <= 2^20, not profiling);
   * multi-kernel: one iteration = assignment, member sort, `update_stats_kernel`, `epilogue_kernel`, replayed from a
