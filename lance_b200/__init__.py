@@ -129,24 +129,25 @@ def timer_stop():
 
 
 # ---- lance-linalg ---------------------------------------------------------------------------
-def l2_distance_batch(frm, to, dimension):
+def l2_distance_batch(frm, to, dimension, bf16=False):
     """lance_linalg::distance::l2_distance_batch (l2.rs:194-203)."""
-    return _distance_batch(frm, to, dimension, L2)
+    return _distance_batch(frm, to, dimension, L2, bf16)
 
 
-def dot_distance_batch(frm, to, dimension):
+def dot_distance_batch(frm, to, dimension, bf16=False):
     """lance_linalg::distance::dot_distance_batch (dot.rs:164-172): 1 - dot."""
-    return _distance_batch(frm, to, dimension, DOT)
+    return _distance_batch(frm, to, dimension, DOT, bf16)
 
 
-def cosine_distance_batch(frm, to, dimension):
+def cosine_distance_batch(frm, to, dimension, bf16=False):
     """lance_linalg::distance::cosine_distance_batch (cosine.rs:266-290)."""
-    return _distance_batch(frm, to, dimension, COSINE)
+    return _distance_batch(frm, to, dimension, COSINE, bf16)
 
 
-def _distance_batch(frm, to, d, metric):
-    """f32 / f16 / u8 inputs keep their element type (u8 L2 = the reference's integer sum, l2.rs:44-49)."""
-    to, dt = _typed(to)
+def _distance_batch(frm, to, d, metric, bf16=False):
+    """f32 / f16 / u8 inputs keep their element type, and so do bf16 ones given as uint16 bit patterns with
+    bf16=True: the arithmetic is the reference's rule for that type (u8: exact integer sums, 16-bit dot: 32 lanes)."""
+    to, dt = _typed(to, bf16)
     frm = np.ascontiguousarray(frm, dtype=to.dtype) if not isinstance(frm, (DeviceArray, PinnedArray)) else frm
     n = int(np.prod(to.shape)) // d
     out = np.empty(n, np.float32)
@@ -157,13 +158,14 @@ def _distance_batch(frm, to, d, metric):
     return out
 
 
-def normalize_fsl(vectors):
-    """lance_linalg::kernels::normalize_fsl (kernels.rs:201-211)."""
-    vectors = _f32(vectors)
+def normalize_fsl(vectors, bf16=False):
+    """lance_linalg::kernels::normalize_fsl (kernels.rs:201-211).  The result has the model type: the input's own
+    type for f32 / f16 / bf16 (bf16=True: uint16 bit patterns), f32 for u8."""
+    vectors, dt = _typed(vectors, bf16)
     n, d = vectors.shape
-    out = np.empty((n, d), np.float32)
+    out = np.empty((n, d), _model_np(dt))
     vp, _k = as_ptr(vectors)
-    check(lib().lb2_normalize(vp, C.c_uint64(n), C.c_uint32(d), C.c_int(F32),
+    check(lib().lb2_normalize(vp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt),
                               C.c_void_p(out.ctypes.data)))
     return out
 
@@ -220,35 +222,37 @@ def compute_partitions(centroids, vectors, distance_type="l2", bf16=False):
     return part, dist, valid.astype(bool)
 
 
-def kmeans_find_partitions(centroids, queries, nprobes, distance_type="l2"):
-    """kmeans_find_partitions_arrow_array (kmeans.rs:1076-1158), batched over queries."""
-    centroids, queries = _f32(centroids), _f32(queries)
-    single = queries.ndim == 1
-    if single:
-        queries = queries.reshape(1, -1)
+def kmeans_find_partitions(centroids, queries, nprobes, distance_type="l2", bf16=False):
+    """kmeans_find_partitions_arrow_array (kmeans.rs:1076-1158), batched over queries.  The queries keep their element
+    type (bf16=True: uint16 bit patterns); the centroids are given in the model type."""
+    queries, dt = _typed(queries, bf16)
+    centroids = np.ascontiguousarray(centroids, dtype=_model_np(dt))
+    single = len(queries.shape) == 1
     k, d = centroids.shape
-    nq = queries.shape[0]
+    nq = 1 if single else queries.shape[0]
     ids = np.empty((nq, nprobes), np.uint32)
     dists = np.empty((nq, nprobes), np.float32)
     cp, _k1 = as_ptr(centroids)
     qp, _k2 = as_ptr(queries)
-    check(lib().lb2_find_partitions(cp, C.c_uint32(k), C.c_uint32(d), C.c_int(F32),
+    check(lib().lb2_find_partitions(cp, C.c_uint32(k), C.c_uint32(d), C.c_int(dt),
                                     C.c_int(_metric(distance_type)), qp, C.c_uint64(nq),
                                     C.c_uint32(nprobes), C.c_void_p(ids.ctypes.data),
                                     C.c_void_p(dists.ctypes.data)))
     return (ids[0], dists[0]) if single else (ids, dists)
 
 
-def compute_residual(centroids, vectors, partitions):
-    """lance_index::vector::residual::compute_residual (residual.rs:111-154)."""
-    centroids, vectors = _f32(centroids), _f32(vectors)
+def compute_residual(centroids, vectors, partitions, bf16=False):
+    """lance_index::vector::residual::compute_residual (residual.rs:111-154).  The vectors keep their element type
+    (bf16=True: uint16 bit patterns); centroids and residuals have the model type."""
+    vectors, dt = _typed(vectors, bf16)
+    centroids = np.ascontiguousarray(centroids, dtype=_model_np(dt))
     k, d = centroids.shape
     n = vectors.shape[0]
     parts = np.ascontiguousarray(partitions, dtype=np.uint32)
-    out = np.empty((n, d), np.float32)
+    out = np.empty((n, d), _model_np(dt))
     cp, _k1 = as_ptr(centroids)
     vp, _k2 = as_ptr(vectors)
-    check(lib().lb2_compute_residual(cp, C.c_uint32(k), C.c_uint32(d), C.c_int(F32), vp,
+    check(lib().lb2_compute_residual(cp, C.c_uint32(k), C.c_uint32(d), C.c_int(dt), vp,
                                      C.c_uint64(n), C.c_void_p(parts.ctypes.data),
                                      C.c_void_p(out.ctypes.data)))
     return out

@@ -91,22 +91,6 @@ bool is_device_ptr(const void* p) {
 }
 
 
-// l2_distance_uint_scalar (lance-linalg/src/distance/l2.rs:44-49, impl L2 for u8 :93-98): sum of |x - y|^2 in
-// u32 (wrapping, like Rust's release-mode `sum::<u32>()`), then `as f32` (round to nearest even); warp per row
-__global__ void l2_u8_kernel(const uint8_t* __restrict__ from, const uint8_t* __restrict__ to, uint64_t n, int d,
-                             float* __restrict__ out) {
-  const uint64_t w = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (w >= n) return;
-  uint32_t s = 0;
-  for (int e = lane; e < d; e += 32) {
-    const int df = (int)from[e] - (int)to[w * d + e];
-    s += (uint32_t)(df * df);
-  }
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if (lane == 0) out[w] = __uint2float_rn(s);
-}
 // cosine_distance_batch (cosine.rs:143-174,266-290): 1 - xy / |x| / sqrt(yy) with f32 FMA lanes; the
 // reference's own lane order is ISA specific, so parity is the reference's tolerance (cosine.rs:361-393)
 __global__ void cosine_f32_kernel(const float* __restrict__ from, const float* __restrict__ to, uint64_t n, int d,
@@ -298,21 +282,27 @@ lb2_status lb2_distance_batch(const void* from, const void* to, uint64_t n, uint
   LB2_REQUIRE(d > 0, "dimension must be positive");
   LB2_REQUIRE(n < (1ull << 31), "too many rows");
   OutArg<float> o(out, n);
-  if (dtype == LB2_U8 && m == METRIC_L2) {  // integer arithmetic (l2.rs:44-49)
-    InArg<uint8_t> f8(from, d), t8(to, (size_t)n * d);
-    if (n) LB2_LAUNCH("l2_u8", l2_u8_kernel, cdiv(n * 32, 256), 256, 0, f8.get(), t8.get(), n, (int)d, o.get());
+  VecIn f(from, d, dtype);
+  // the reference picks the arithmetic by element type: u8 sums are exact integers, 16-bit dot products take 32
+  // lanes; the rows are read in their own type
+  if (distance_batch_typed_applies(dtype, m)) {
+    InArg<uint8_t> t(to, (size_t)n * d * dtype_size(dtype));
+    distance_batch_typed(f.get(), t.get(), dtype, n, (int)d, m, o.get());
     o.commit();
     sync_stream();
     return LB2_OK;
   }
-  VecIn f(from, d, dtype), t(to, (size_t)n * d, dtype);
+  VecIn t(to, (size_t)n * d, dtype);
   if (m == METRIC_COSINE) {
     if (n) LB2_LAUNCH("cosine_batch", cosine_f32_kernel, cdiv(n * 32, 256), 256, 0, f.get(), t.get(), n, (int)d, o.get());
     o.commit();
     sync_stream();
     return LB2_OK;
   }
-  centroid_distances(f.get(), 1, d, t.get(), (int)n, m, o.get());
+  // f32 L2 / dot and 16-bit L2 (each element converted, l2.rs:100-106): the 16-lane f32 loop of the assignment
+  // kernels, `from` as the one row and `to` as n centroids (none for n == 0: the tile kernel cannot lay out an empty
+  // centroid matrix)
+  if (n) centroid_distances(f.get(), 1, d, t.get(), (int)n, m, o.get());
   o.commit();
   sync_stream();
   LB2_API_END

@@ -431,10 +431,11 @@ static void assign_dispatch(const float* x, uint64_t n, int d, const float* cent
   // 16 rows per CTA halve the centroid re-reads from L2; wide vectors fall back to 8 rows
   const bool r16 = sizeof(float) * 16 * (size_t)d <= 96 * 1024;
   const size_t smem = sizeof(float) * (r16 ? 16 : 8) * (size_t)d;
-  if (smem > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the exact kernel", d);
   const unsigned grid = cdiv(n, r16 ? 16 : 8);
 #define LB2_GENERIC(RR)                                                                                \
   do {                                                                                                 \
+    if (smem_with_static(generic_kernel<METRIC, WRITE_ALL, RR>, smem) > ctx().smem_optin)              \
+      fail(LB2_UNSUPPORTED, "dimension %d too large for the exact kernel", d);                         \
     set_smem(generic_kernel<METRIC, WRITE_ALL, RR>, smem);                                             \
     LB2_LAUNCH("assign_exact_generic", (generic_kernel<METRIC, WRITE_ALL, RR>), grid, 256, smem, x, n, \
                d, cent, K, bias, part, dist, valid, all_out, active, nullptr, nullptr);                \
@@ -452,7 +453,8 @@ void assign_rows_f32(const float* x, uint64_t n_max, int d, const float* cent, i
   if (!(d % 16 == 0 && d <= 256)) {
     // 8 rows per CTA: the list is short, more CTAs beat fewer centroid re-reads (measured)
     const size_t gsmem = sizeof(float) * 8 * (size_t)d;
-    if (gsmem > ctx().smem_optin) fail(LB2_UNSUPPORTED, "dimension %d too large for the exact kernel", d);
+    if (smem_with_static(generic_kernel<METRIC_L2, false, 8>, gsmem) > ctx().smem_optin)
+      fail(LB2_UNSUPPORTED, "dimension %d too large for the exact kernel", d);
     // very short lists against many centroids: one CTA per (8 rows, range of centroids) + a merge
     const int gchunks = (int)std::min<uint64_t>(64, (uint64_t)K / 128);
     const uint32_t gtiny = gchunks > 1 ? (uint32_t)std::min<uint64_t>(4096, n_max + 1) : 0u;

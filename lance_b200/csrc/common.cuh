@@ -136,6 +136,14 @@ inline void set_smem(K kernel, size_t bytes) {
   LB2_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
   cur = bytes;
 }
+// the shared memory a launch of `kernel` with `dyn` dynamic bytes takes: its static shared memory counts against the
+// same per-block opt-in limit, and cudaFuncSetAttribute refuses a dynamic size that leaves no room for it
+template <class Kern>
+size_t smem_with_static(Kern kernel, size_t dyn) {
+  cudaFuncAttributes fa;
+  LB2_CUDA(cudaFuncGetAttributes(&fa, kernel));
+  return dyn + fa.sharedSizeBytes;
+}
 
 // ------------------------------------------------------------------------------------------
 // memory

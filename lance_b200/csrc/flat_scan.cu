@@ -162,40 +162,55 @@ void ivfflat_search(const IvfSearch& s, const void* vectors, int vdt) {
 // refine: exact distances of k' = k * refine_factor candidates from the raw vectors, then the k
 // best by (distance, row id)  (scanner.rs:2884-2905, flat.rs:95-148)
 // ------------------------------------------------------------------------------------------------
+// u8 L2 / dot: exact integer sums (wrapping like the reference's release build), one conversion to f32 (l2.rs:44-49,
+// dot.rs:152-161); q holds the u8 values of the other vector as f32
+template <int METRIC>
+__device__ __forceinline__ float u8_row_distance(const float* __restrict__ q, const uint8_t* __restrict__ v, int d,
+                                                 int l, unsigned mask) {
+  uint32_t acc = 0;
+  for (int e = l; e < d; e += 16) {
+    const int x = __float2int_rn(q[e]), y = v[e];
+    acc += METRIC == METRIC_DOT ? (uint32_t)(x * y) : (uint32_t)((x - y) * (x - y));
+  }
+#pragma unroll
+  for (int off = 8; off >= 1; off >>= 1) acc += __shfl_xor_sync(mask, acc, off, 16);
+  return finish<METRIC>(__uint2float_rn(acc));
+}
+
+// 16-bit dot: dot_scalar::<T, f32, 32> (dot.rs:30-58) -- bf16 always (dot.rs:78-83), f16 without the fp16 C kernel
+// (dot.rs:133): lane l owns the accumulators l and l + 16, the d % 32 tail comes first, the 32 sums are folded 0..31
+template <class T>
+__device__ __forceinline__ float dot32_row_distance(const float* __restrict__ q, const T* __restrict__ v, int d,
+                                                    int l, unsigned mask) {
+  const int n32 = d & ~31;
+  float a0 = 0.0f, a1 = 0.0f;
+  for (int e = l; e < n32; e += 32) {
+    a0 = f_add(a0, __fmul_rn(q[e], ldf<T>(v, e)));
+    a1 = f_add(a1, __fmul_rn(q[e + 16], ldf<T>(v, e + 16)));
+  }
+  float s = 0.0f;  // sequential tail, every lane redundantly
+  for (int e = n32; e < d; ++e) s = f_add(s, __fmul_rn(q[e], ldf<T>(v, e)));
+  float t = 0.0f;
+#pragma unroll
+  for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, a0, qq, 16));
+#pragma unroll
+  for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, a1, qq, 16));
+  return finish<METRIC_DOT>(f_add(s, t));
+}
+
 // The refine plan takes the distance function of the column's own element type (flat.rs:94-150), unlike the
 // IVF_FLAT scan, whose storage is f32 (flat/storage.rs:352-365):
-//  * f16 dot: dot_scalar::<f16, f32, 32> (dot.rs:30-58,133): lane l owns the accumulators l and l + 16, the d % 32
-//    tail comes first, the 32 sums are folded 0..31;
-//  * u8 L2 / dot: exact integer sums, one conversion to f32 (l2.rs:44-49, dot.rs:152-161); the query came in as
-//    u8 too, so its f32 view holds integers;
-//  * everything else (f16 L2, bf16, cosine) as flat_row_distance.
+//  * f16 dot: the 32-lane dot_scalar;
+//  * u8 L2 / dot: exact integer sums; the query came in as u8 too, so its f32 view holds integers;
+//  * everything else (f16 L2, bf16, cosine) as flat_row_distance: the reference refuses bf16 keys in refine, so bf16
+//    keeps the scan's 16-lane rule (DESIGN.md section 5).
 template <int METRIC, class T>
 __device__ __forceinline__ float refine_row_distance(const float* __restrict__ q, const T* __restrict__ v, int d,
                                                      int l, unsigned mask, float q_norm) {
   if constexpr (std::is_same<T, uint8_t>::value && METRIC != METRIC_COSINE) {
-    uint32_t acc = 0;
-    for (int e = l; e < d; e += 16) {
-      const int x = __float2int_rn(q[e]), y = v[e];
-      acc += METRIC == METRIC_DOT ? (uint32_t)(x * y) : (uint32_t)((x - y) * (x - y));
-    }
-#pragma unroll
-    for (int off = 8; off >= 1; off >>= 1) acc += __shfl_xor_sync(mask, acc, off, 16);
-    return finish<METRIC>(__uint2float_rn(acc));
+    return u8_row_distance<METRIC>(q, v, d, l, mask);
   } else if constexpr (std::is_same<T, __half>::value && METRIC == METRIC_DOT) {
-    const int n32 = d & ~31;
-    float a0 = 0.0f, a1 = 0.0f;
-    for (int e = l; e < n32; e += 32) {
-      a0 = f_add(a0, __fmul_rn(q[e], ldf<T>(v, e)));
-      a1 = f_add(a1, __fmul_rn(q[e + 16], ldf<T>(v, e + 16)));
-    }
-    float s = 0.0f;  // sequential tail, every lane redundantly
-    for (int e = n32; e < d; ++e) s = f_add(s, __fmul_rn(q[e], ldf<T>(v, e)));
-    float t = 0.0f;
-#pragma unroll
-    for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, a0, qq, 16));
-#pragma unroll
-    for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, a1, qq, 16));
-    return finish<METRIC>(f_add(s, t));
+    return dot32_row_distance<T>(q, v, d, l, mask);
   } else {
     return flat_row_distance<METRIC, T>(q, v, d, l, mask, q_norm);
   }
@@ -268,6 +283,45 @@ void refine_f32(const float* queries, uint64_t nq, int d, int metric, const void
     LB2_LAUNCH("refine", kern, (unsigned)nq, 256, smem, queries, d, reinterpret_cast<const T*>(vectors), num_vectors,
                cand_id, cand_cnt, kc, k, out_id, out_d, out_cnt, has_lower, lower, has_upper, upper);
   });
+}
+
+// ------------------------------------------------------------------------------------------------
+// lb2_distance_batch where the reference's arithmetic depends on the element type (l2_distance_batch /
+// dot_distance_batch, l2.rs:194-203, dot.rs:164-172): u8 L2 / dot and 16-bit dot.  Half-warp per row of `to`, read
+// in its own type; `from` as f32.
+// ------------------------------------------------------------------------------------------------
+template <int METRIC, class T>
+__global__ void __launch_bounds__(256)
+distance_batch_kernel(const float* __restrict__ from, const T* __restrict__ to, uint64_t n, int d,
+                      float* __restrict__ out) {
+  const uint64_t row = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 4;
+  if (row >= n) return;  // a whole half-warp leaves: the shuffles below only name its own lanes
+  const int l = threadIdx.x & 15;
+  const unsigned hmask = 0xffffu << (16 * ((threadIdx.x >> 4) & 1));
+  float dist;
+  if constexpr (std::is_same<T, uint8_t>::value) dist = u8_row_distance<METRIC>(from, to + row * d, d, l, hmask);
+  else dist = dot32_row_distance<T>(from, to + row * d, d, l, hmask);
+  if (l == 0) out[row] = dist;
+}
+
+bool distance_batch_typed_applies(int dt, int metric) {
+  return metric != METRIC_COSINE && (dt == LB2_U8 || (metric == METRIC_DOT && (dt == LB2_F16 || dt == LB2_BF16)));
+}
+
+void distance_batch_typed(const float* from, const void* to, int dt, uint64_t n, int d, int metric, float* out) {
+  if (!distance_batch_typed_applies(dt, metric)) fail(LB2_UNSUPPORTED, "no typed distance for dtype %d, metric %d", dt, metric);
+  if (n == 0) return;
+  auto launch = [&](auto kern, auto rows) {
+    LB2_LAUNCH("distance_batch", kern, cdiv(n * 16, 256), 256, 0, from, rows, n, d, out);
+  };
+  if (dt == LB2_U8 && metric == METRIC_DOT)
+    launch(distance_batch_kernel<METRIC_DOT, uint8_t>, static_cast<const uint8_t*>(to));
+  else if (dt == LB2_U8)
+    launch(distance_batch_kernel<METRIC_L2, uint8_t>, static_cast<const uint8_t*>(to));
+  else if (dt == LB2_F16)
+    launch(distance_batch_kernel<METRIC_DOT, __half>, static_cast<const __half*>(to));
+  else
+    launch(distance_batch_kernel<METRIC_DOT, __nv_bfloat16>, static_cast<const __nv_bfloat16*>(to));
 }
 
 void flat_topk_f32(const float* dists, const uint64_t* row_ids, uint64_t n, int k, const ScanFilter& flt,

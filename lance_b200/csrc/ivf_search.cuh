@@ -63,15 +63,6 @@ class ScanRef {
   void operator()(const ScanSlots& s) const { call(obj, s); }
 };
 
-// the shared memory a launch of `kernel` with `dyn` dynamic bytes takes: its static shared memory counts against the
-// same per-block opt-in limit, and cudaFuncSetAttribute refuses a dynamic size that leaves no room for it
-template <class Kern>
-size_t smem_with_static(Kern kernel, size_t dyn) {
-  cudaFuncAttributes fa;
-  LB2_CUDA(cudaFuncGetAttributes(&fa, kernel));
-  return dyn + fa.sharedSizeBytes;
-}
-
 // What every driver settles before it launches anything: false when the search is empty; refuses k > 1024, and a
 // search whose largest kernel needs more than the device's shared memory (`need` bytes, static included) with the
 // driver's own text, which formats `refusal_arg` with one %zu.

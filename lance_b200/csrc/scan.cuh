@@ -30,4 +30,8 @@ void refine_f32(const float* queries, uint64_t nq, int d, int metric, const void
                 int has_upper = 0, float upper = 0.0f);
 void flat_topk_f32(const float* dists, const uint64_t* row_ids, uint64_t n, int k, const ScanFilter& flt,
                    uint64_t* out_id, float* out_d, uint32_t* out_cnt);
+// lb2_distance_batch with the reference's per-type rule: u8 L2 / dot (exact integer sums) and f16 / bf16 dot
+// (32 lanes); `from` is the f32 view of one row, `to` n rows of element type dt (lb2_dtype)
+bool distance_batch_typed_applies(int dt, int metric);
+void distance_batch_typed(const float* from, const void* to, int dt, uint64_t n, int d, int metric, float* out);
 }  // namespace lb2
