@@ -217,40 +217,56 @@ __device__ __forceinline__ int frag_row(int h) { return 16 * ((threadIdx.x >> 5)
 // M64 N128 wgmma each, or the two halves of an N256 fragment); a lane holds 32 values of each half and row:
 // levels 0..4 pair those, level 5 pairs the winners of the two halves.
 constexpr int TOUR_LEVELS = 6;
+// COLUMN UNITS.  With UNIT = 2 the entrants are the 128 column PAIRS (c, c ^ 1) of the row, which are the two
+// columns of a lane's j: level 0 is one max of the two raw scores, packed once with the PAIR id (col >> 1), and
+// has no loser.  The top 3 are then the three best pair maxima, all distinct by their ids, and the same argument
+// holds between pairs: m1 - m2 > tau proves every column outside pair 1 below m1 - tau, m1 - m3 > tau every column
+// outside pairs 1 and 2.  The caller ranks the columns of the certified pair(s) exactly (tc_pq.cu).  Per score:
+// half a max and half a pack at level 0 instead of a pack, a max, a min and a running max.
+constexpr int tour_first_level(int unit) { return unit == 2 ? 1 : 0; }  // levels below it have no losers
 
 struct Tour {
   float top[2];              // winner so far of fragment row h
   float L[2][TOUR_LEVELS];   // largest level-lvl loser so far
 };
 
-// score with its column in the low mantissa byte: byte b of the column word cw (one PRMT, b a constant)
+// score with its column (or unit) in the low mantissa byte: byte b of the id word cw (one PRMT, b a constant)
 __device__ __forceinline__ float pack_col(float f, uint32_t cw, int b) {
   return __uint_as_float(__byte_perm(__float_as_uint(f), cw, 0x3214 + b));
 }
 
 // Folds one 128-column half of both fragment rows into the tournament (half 0 starts it, half 1 completes it):
-// score acc + cn[col], packed with its column.  a: the half's 64 accumulators, a[4j + 2h + e] = (row r0 + 8h,
+// score acc + cn[col], packed with its column (UNIT = 1) or the maximum of a column pair packed with the pair id
+// (UNIT = 2).  a: the half's 64 accumulators, a[4j + 2h + e] = (row r0 + 8h,
 // column 128 HALF + 8j + 2 (t % 4) + e), j < 16; cn: the 256 values of -|c|^2/2 (shared or global memory).
-template <int HALF>
+template <int HALF, int UNIT = 1>
 __device__ __forceinline__ void top3_half(const float* a, const float* cn, Tour& st) {
-  const uint32_t q2 = 2 * (threadIdx.x & 3);
-  // cw[e][i], byte b: the column of j = 4i + b, 128 HALF + 32i + 8b + q2 + e (< 256: no carry between bytes)
+  static_assert(UNIT == 1 || UNIT == 2, "columns or column pairs");
+  const uint32_t q = threadIdx.x & 3, q2 = 2 * q;
+  // cw[e][i], byte b: the column of j = 4i + b, 128 HALF + 32i + 8b + q2 + e (< 256: no carry between bytes);
+  // for pairs one word per i: the pair of j = 4i + b, 64 HALF + 16i + 4b + q
   uint32_t cw[2][4];
 #pragma unroll
   for (int e = 0; e < 2; ++e)
 #pragma unroll
-    for (int i = 0; i < 4; ++i) cw[e][i] = (HALF ? 0x98908880u : 0x18100800u) + 0x20202020u * i + 0x01010101u * (q2 + e);
+    for (int i = 0; i < 4; ++i)
+      cw[e][i] = UNIT == 2 ? (HALF ? 0x4C484440u : 0x0C080400u) + 0x10101010u * i + 0x01010101u * q
+                           : (HALF ? 0x98908880u : 0x18100800u) + 0x20202020u * i + 0x01010101u * (q2 + e);
   float w[2][16];
 #pragma unroll
   for (int j = 0; j < 16; ++j) {  // level 0: the two columns of a j
     const float2 cv = *reinterpret_cast<const float2*>(cn + 128 * HALF + 8 * j + q2);
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const float x = pack_col(a[4 * j + 2 * h] + cv.x, cw[0][j >> 2], j & 3);
-      const float y = pack_col(a[4 * j + 2 * h + 1] + cv.y, cw[1][j >> 2], j & 3);
-      w[h][j] = fmaxf(x, y);
-      const float lo = fminf(x, y);
-      st.L[h][0] = (HALF == 0 && j == 0) ? lo : fmaxf(st.L[h][0], lo);
+      if (UNIT == 2) {
+        w[h][j] = pack_col(fmaxf(a[4 * j + 2 * h] + cv.x, a[4 * j + 2 * h + 1] + cv.y), cw[0][j >> 2], j & 3);
+      } else {
+        const float x = pack_col(a[4 * j + 2 * h] + cv.x, cw[0][j >> 2], j & 3);
+        const float y = pack_col(a[4 * j + 2 * h + 1] + cv.y, cw[1][j >> 2], j & 3);
+        w[h][j] = fmaxf(x, y);
+        const float lo = fminf(x, y);
+        st.L[h][0] = (HALF == 0 && j == 0) ? lo : fmaxf(st.L[h][0], lo);
+      }
     }
   }
 #pragma unroll
@@ -284,15 +300,17 @@ __device__ __forceinline__ void top3_merge(float (&a)[3], const float (&b)[3]) {
   a[2] = fmaxf(fminf(x, y), z);
 }
 
-// The finished tournament: m = the top-3 (sorted, column in the low mantissa byte) of all 256 columns of the
-// fragment row r0 + 8 (lane & 1), in every lane of the quad.
+// The finished tournament: m = the top-3 (sorted, column or pair id in the low mantissa byte) of all 256 columns
+// (128 pairs) of the fragment row r0 + 8 (lane & 1), in every lane of the quad.
+template <int UNIT = 1>
 __device__ __forceinline__ void top3_finish(const Tour& st, float (&m)[3]) {
+  constexpr int F = tour_first_level(UNIT);
   float t[2][3];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    float a = fmaxf(st.L[h][0], st.L[h][1]), b = fminf(st.L[h][0], st.L[h][1]);
+    float a = fmaxf(st.L[h][F], st.L[h][F + 1]), b = fminf(st.L[h][F], st.L[h][F + 1]);
 #pragma unroll
-    for (int lvl = 2; lvl < TOUR_LEVELS; ++lvl) {
+    for (int lvl = F + 2; lvl < TOUR_LEVELS; ++lvl) {
       b = fmaxf(b, fminf(a, st.L[h][lvl]));
       a = fmaxf(a, st.L[h][lvl]);
     }

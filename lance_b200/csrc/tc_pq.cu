@@ -10,10 +10,12 @@
 //   * A operand: 64-row tiles of the (residual) vectors, TMA-streamed in 32-float chunks (= 4 sub-spaces).
 //   * two wgmmas (M64 N128 K8, tf32: one per half of the codebook) per (tile, sub-space) into register
 //     accumulators, consumer warpgroups taking the work items in turns (see Pipe); the epilogue keeps the
-//     top-3 of  r.c - |c|^2/2  per row and classifies the row against tau = 3*2^-10 (|r_m|^2 + max|c_m|^2)
-//     (with the norm floor of cert_tau) exactly like tc_assign.cu;
-//   * flag 0/1 rows are decided IN THE EPILOGUE with reference-order f32 arithmetic on the operands
-//     that are still in shared memory (sequential 8-term sum, l2.rs:69-79; strict-< / lowest index);
+//     top-3 of  r.c - |c|^2/2  over the 128 codeword PAIRS (c, c ^ 1) of the row (tc_common.cuh: column units) and
+//     classifies the row against tau = 3*2^-10 (|r_m|^2 + max|c_m|^2) (with the norm floor of cert_tau) like
+//     tc_assign.cu: flag 0 certifies the two codewords of the best pair, flag 1 the four of the two best;
+//   * flag 0/1 rows are decided IN THE EPILOGUE: each certified codeword gets the reference-order f32 distance
+//     from the operands that are still in shared memory (sequential 8-term sum, l2.rs:69-79; strict-< / lowest
+//     index);
 //   * flag 2 (row, sub-space) pairs are appended to a list and finished by pq_fallback_kernel
 //     (half-warp per pair, exact scan of all 256 codewords).
 #include "assign.cuh"
@@ -28,13 +30,15 @@ namespace tcpq {
 using namespace tc;
 
 constexpr int DS = 8;
+constexpr int UNIT = 2;  // the tournament's entrants are column pairs (tc_common.cuh); decide() ranks their columns
 constexpr int MAX_M_RESIDENT = 16;  // d <= 128: the whole codebook matrix stays in shared memory
 constexpr int MAX_M = 256;          // d <= 2048: codebook chunk + its -|c|^2/2 slice streamed per work item
 constexpr int CNH_CHUNK_BYTES = 4 * TN * 4;                                       // 4 sub-spaces
 constexpr int STREAM_STAGE_BYTES = A_STAGE_BYTES + B_CHUNK_BYTES + CNH_CHUNK_BYTES;  // 44 KB
 
 // One TMA producer warpgroup and CONSUMERS warpgroups that take the work items in turns.  The epilogue is bound by
-// the ALU pipe, and a consumer warp stalls often (wgmma waits, the divergent decision code, barrier waits, the
+// the ALU pipe (per 128 scores of a lane 64 pair maxima, 64 packs and about 210 min/max of the pair tournament,
+// against 128 adds on the FMA pipe), and a consumer warp stalls often (wgmma waits, the divergent decision code, barrier waits, the
 // shuffles of top3_finish); the resident variant runs four consumers (4 warps per scheduler) so that the others
 // fill those stalls.  The streamed ring (44 KB per stage) has no room for more than four stages, so the streamed
 // variant keeps two consumers.
@@ -219,29 +223,34 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
           const float tau = cert_tau(0.0029296875f, rn + cbm);
           uint32_t flag = 2;
           if (m1 - m2 > tau) flag = 0;
-          else if (m1 - m3 > tau) flag = 1;
-          const uint32_t i1 = __float_as_uint(m1) & 0xFFu, i2 = __float_as_uint(m2) & 0xFFu;
-          uint32_t best_idx = i1;
+          // two pairs with the same score bits are duplicated codewords: such rows keep their route through
+          // pq_fallback_kernel, which handles any multiplicity (tests/test_assignment_routes.py pins the routes)
+          else if (m1 - m3 > tau && ((__float_as_uint(m1) ^ __float_as_uint(m2)) >> 8) != 0) flag = 1;
+          // the low byte is a PAIR of columns (2p, 2p + 1): flag 0 certifies pair 1, flag 1 pairs 1 and 2
+          const uint32_t p1 = __float_as_uint(m1) & 0xFFu, p2 = __float_as_uint(m2) & 0xFFu;
+          uint32_t best_idx = 0;
           float best_val = 0.0f;
           bool ok = true;
           if (flag == 2) {
             fb_pairs[(size_t)m * n + atomicAdd(fb_count + m, 1u)] = (uint32_t)row;  // per-sub-space list
-          } else if (TRAIN || flag == 1) {
-            // exact, reference-order distance(s) from the operands still in shared memory
+          } else {
+            // exact, reference-order distances of the certified columns, in ascending column order, from the
+            // operands still in shared memory
             const float4 r0 = *swz(atile, rl, j * 2), r1 = *swz(atile, rl, j * 2 + 1);
             const float rv[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
             float bv = __int_as_float(0x7f800000);
             uint32_t bi = 0xffffffffu;
-            const int ncand = flag == 0 ? 1 : 2;
+            const uint32_t plo = flag == 0 ? p1 : min(p1, p2), phi = max(p1, p2);
+            const int ncand = flag == 0 ? 2 : 4;
             for (int c = 0; c < ncand; ++c) {
-              const uint32_t ci = c == 0 ? i1 : i2;
+              const uint32_t ci = 2 * (c < 2 ? plo : phi) + (c & 1);
               const float4 c0v = *swz(bt, (int)ci, j * 2), c1v = *swz(bt, (int)ci, j * 2 + 1);
               const float cv[8] = {c0v.x, c0v.y, c0v.z, c0v.w, c1v.x, c1v.y, c1v.z, c1v.w};
               float sacc = 0.0f;
   #pragma unroll
               for (int t = 0; t < 8; ++t) sacc = f_add(sacc, sq_diff(rv[t], cv[t]));
               const float vv = f_add(sacc, 0.0f);
-              if (vv < bv || (vv == bv && ci < bi)) { bv = vv; bi = ci; }
+              if (vv < bv) { bv = vv; bi = ci; }  // strict <: the lowest index wins a tie
             }
             ok = bi != 0xffffffffu;
             best_idx = ok ? bi : 0u;
@@ -280,7 +289,7 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
           Tour tour;
           wgmma_wait<1>();
           acc_fence<64>(acc[0]);
-          top3_half<0>(acc[0], cn4 + j * TN, tour);
+          top3_half<0, UNIT>(acc[0], cn4 + j * TN, tour);
           if (jn >= 0) {
             issue(acc[0], jn, 0);
             wgmma_wait<1>();
@@ -288,9 +297,9 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
             wgmma_wait<0>();
           }
           acc_fence<64>(acc[1]);
-          top3_half<1>(acc[1], cn4 + j * TN, tour);
+          top3_half<1, UNIT>(acc[1], cn4 + j * TN, tour);
           float mm[3];
-          top3_finish(tour, mm);
+          top3_finish<UNIT>(tour, mm);
           wgmma_wait<0>();
           decide(j, mm);
           if (jn < 0) break;
@@ -306,13 +315,13 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
           issue(acc[0], j, 0);
           wgmma_wait<0>();
           acc_fence<64>(acc[0]);
-          top3_half<0>(acc[0], cn4 + j * TN, tour);
+          top3_half<0, UNIT>(acc[0], cn4 + j * TN, tour);
           issue(acc[0], j, 1);
           wgmma_wait<0>();
           acc_fence<64>(acc[0]);
-          top3_half<1>(acc[0], cn4 + j * TN, tour);
+          top3_half<1, UNIT>(acc[0], cn4 + j * TN, tour);
           float mm[3];
-          top3_finish(tour, mm);
+          top3_finish<UNIT>(tour, mm);
           decide(j, mm);
         }
       }
