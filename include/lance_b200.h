@@ -195,6 +195,33 @@ lb2_status lb2_flat_topk_range(const float* dists, const uint64_t* row_ids, uint
                                int has_lower, float lower, int has_upper, float upper,
                                uint64_t* ids_out, float* dists_out, uint32_t* count_out);
 
+/* flat_knn over one vector column (rust/lance/src/dataset/scanner.rs:3336-3411), batched over nq queries: the plan
+ * of a nearest() query without an index (scanner.rs:2912-2941) and its unindexed half (knn_combined, :2946-3027).
+ *   - every row's distance to the query is compute_distance's (lance-index/src/vector/flat.rs:94-150), with the
+ *     function of the element type, the same arithmetic as the refine step: f32 L2 / dot, f16 L2 and bf16 in 16 f32
+ *     lanes; f16 dot in 32 lanes (dot_scalar); u8 L2 / dot as exact integer sums; cosine within the f64 bound;
+ *   - a row whose allow bit is clear (a null vector, or one the prefilter removes) is never returned;
+ *   - the optional range keeps lower <= distance < upper (LanceFilterExec, scanner.rs:3342-3377; NaN fails it);
+ *   - SortExec(_distance, _rowid).fetch(k) (scanner.rs:3450-3466): the k smallest (distance, row id) pairs in the
+ *     f32 total order (a NaN the device produces is positive and sorts after +inf), ties at the k-th distance going
+ *     to the smallest row ids.  (On x86 the reference turns inf - inf into a NEGATIVE NaN, which sorts first; such
+ *     rows sort last here.)
+ * vectors [n][d] and queries [nq][d] are of element type `dtype`; host or device memory (device rows are read in
+ * place, host rows are staged in chunks).  Outputs [nq][k] ascending by (distance, row id); unused slots row id
+ * UINT64_MAX, distance +inf; counts_out [nq] nullable.  LB2_INVALID_ARG: k == 0; LB2_UNSUPPORTED: k > 1024, or a d
+ * whose tile of queries and rows does not fit the device's shared memory. */
+typedef struct {
+  uint32_t k;                    /* 1..1024 */
+  const uint64_t* allow_bitmap;  /* nullable; (n+63)/64 words, bit i = row i (input order) may be returned.  The
+                                    caller clears null vectors here too (Arrow validity AND prefilter). */
+  uint32_t has_lower_bound, has_upper_bound;
+  float lower_bound, upper_bound;
+} lb2_flat_search_params;
+lb2_status lb2_flat_search(const void* vectors, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                           const uint64_t* row_ids /* NULL = 0..n; must be distinct */, const void* queries,
+                           uint64_t nq, const lb2_flat_search_params* p, uint64_t* row_ids_out, float* dists_out,
+                           uint32_t* counts_out);
+
 /* IvfTransformer::transform for IVF_PQ (lance-index/src/vector/ivf.rs:188-236,357): for a batch,
  * [normalise if cosine] -> partition id -> residual -> PQ code, in one pass over the vectors.
  * `metric` is the index metric: it selects the partition assignment and whether residuals are taken
@@ -297,6 +324,33 @@ lb2_status lb2_index_search_probed(lb2_index* index, const void* queries, uint64
                                    const lb2_search_params* sp /* nprobes must be 0 */,
                                    const lb2_probe_params* pp, uint64_t* row_ids_out, float* dists_out,
                                    uint32_t* counts_out, uint32_t* nprobes_out /* nullable, [nq] */);
+/* knn_combined (rust/lance/src/dataset/scanner.rs:2946-3027): a nearest() query on an index that does not yet cover
+ * every row of its table.  The reference takes the raw vectors of the ANN rows and re-scores them exactly, runs a
+ * flat KNN with the index metric over the unindexed rows (with the query's prefilter), and sorts the union by
+ * (_distance, _rowid), range-filtered, fetched to k.  Since the refine step's distances already are exact, this is:
+ *   1. the index search (lb2_index_search_ex, or lb2_index_search_probed when pp != NULL) with refine factor
+ *      max(1, sp->refine_factor);
+ *   2. lb2_flat_search over *u with the index's metric, sp->k and sp's range, on the original (not normalised)
+ *      query;
+ *   3. the two k-lists of every query merged by (distance, row id).
+ * Plan selection stays with the caller: with fast_search, or without unindexed fragments, the plain index search
+ * answers; unindexed fragments whose rows are all filtered or deleted still take this call (u->n rows with clear
+ * allow bits, or u->n == 0), because the ANN rows are re-scored either way.
+ * Queries are of the index's element type.  LB2_INVALID_ARG: k == 0, sp->refine_vectors NULL, u or u->row_ids NULL,
+ * nprobes_out without pp, and what lb2_index_search_ex / _probed refuse.  LB2_UNSUPPORTED: k * max(1, refine_factor)
+ * > 1024, what lb2_flat_search refuses, and a thread whose communicator has more than one rank (as
+ * lb2_index_search_probed). */
+typedef struct {
+  const void* vectors;           /* [n][d], the index's element type */
+  uint64_t n;
+  const uint64_t* row_ids;       /* required: the unindexed rows' _rowid values */
+  const uint64_t* allow_bitmap;  /* nullable, over these rows: the query filter + null vectors */
+} lb2_unindexed_rows;
+lb2_status lb2_index_search_combined(lb2_index* index, const void* queries, uint64_t nq,
+                                     const lb2_search_params* sp /* refine_vectors required; nprobes 0 with pp */,
+                                     const lb2_probe_params* pp /* nullable */, const lb2_unindexed_rows* u,
+                                     uint64_t* row_ids_out, float* dists_out, uint32_t* counts_out,
+                                     uint32_t* nprobes_out /* nullable; requires pp */);
 /* Incremental update: the device half of optimize_indices / split / join (SURVEY 8f-4).
  * The reference expresses an optimize step as per-partition AssignOp::Add / AssignOp::Remove lists against a new
  * centroid set (rust/lance/src/index/vector/builder.rs:1219-1333 split_partition_impl, :1476-1530

@@ -19,7 +19,7 @@ from ._lib import (BF16, COSINE, DOT, F16, F32, L2, METRICS, U8, BuildParams, Bu
 __all__ = ["device_count", "DeviceArray", "PinnedArray", "LanceB200Error", "train_kmeans",
            "compute_partitions", "kmeans_find_partitions", "compute_residual", "normalize_fsl",
            "l2_distance_batch", "dot_distance_batch", "cosine_distance_batch", "PQBuildParams", "ProductQuantizer",
-           "build_distance_table_l2", "compute_pq_distance", "flat_topk", "IvfPqIndex",
+           "build_distance_table_l2", "compute_pq_distance", "flat_topk", "flat_search", "IvfPqIndex",
            "IvfBuildParams", "IvfFlatIndex", "SQBuildParams", "ScalarQuantizer", "IvfSqIndex", "RQBuildParams",
            "RabitQuantizer", "IvfRqIndex", "launch_count", "profile"]
 
@@ -371,6 +371,45 @@ def flat_topk(dists, row_ids, k, lower_bound=None, upper_bound=None):
     return oi[:cnt[0]], od[:cnt[0]]
 
 
+def _bitmap(a):
+    """an allow bitmap (uint64 words) as numpy / Pinned / Device array, or None"""
+    if a is None or isinstance(a, (DeviceArray, PinnedArray)):
+        return a
+    return np.ascontiguousarray(a, dtype=np.uint64)
+
+
+def _row_ids(a):
+    if a is None or isinstance(a, (DeviceArray, PinnedArray)):
+        return a
+    return np.ascontiguousarray(a, dtype=np.uint64)
+
+
+def flat_search(vectors, queries, k, distance_type="l2", row_ids=None, allow_bitmap=None, lower_bound=None,
+                upper_bound=None, bf16=False):
+    """flat_knn over one vector column (scanner.rs:3336-3411), batched: the k smallest (distance, row id) pairs of
+    every query, with compute_distance's arithmetic for the column's element type (flat.rs:94-150).  `vectors` [n][d]
+    and `queries` [nq][d] share the element type (bf16=True: uint16 bit patterns); row_ids (distinct) default to the
+    row numbers; allow_bitmap: (n + 63) // 64 uint64 words, bit i = row i may be returned (validity AND filter);
+    the range keeps lower <= distance < upper.  Returns (ids [nq][k], dists [nq][k], counts [nq]); unused slots hold
+    (2**64 - 1, +inf)."""
+    from ._lib import FlatSearchParams
+    vectors, dt = _typed(vectors, bf16)
+    if not isinstance(queries, (DeviceArray, PinnedArray)):
+        queries = np.ascontiguousarray(queries, dtype=vectors.dtype)
+    n, d = vectors.shape
+    nq = queries.shape[0]
+    ids, dists, counts = np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32), np.empty(nq, np.uint32)
+    vp, _k0 = as_ptr(vectors)
+    qp, _k1 = as_ptr(queries)
+    rp, _k2 = as_ptr(_row_ids(row_ids))
+    bp, _k3 = as_ptr(_bitmap(allow_bitmap))
+    p = FlatSearchParams(k, bp.value if bp is not None else None, int(lower_bound is not None),
+                         int(upper_bound is not None), float(lower_bound or 0.0), float(upper_bound or 0.0))
+    check(lib().lb2_flat_search(vp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt), C.c_int(_metric(distance_type)), rp,
+                                qp, C.c_uint64(nq), C.byref(p), as_ptr(ids)[0], as_ptr(dists)[0], as_ptr(counts)[0]))
+    return ids, dists, counts
+
+
 def ivfpq_transform(centroids, codebook, vectors, distance_type="l2", num_bits=8, bf16=False):
     """IvfTransformer::transform for IVF_PQ (lance-index/src/vector/ivf.rs:188-236,357).
     The rows keep their element type; the model has the rows' model type (bf16=True: uint16 bit patterns)."""
@@ -627,6 +666,59 @@ class IvfPqIndex:
         check(lib().lb2_index_search_probed(self._h, qp, C.c_uint64(nq), C.byref(sp), C.byref(pp), as_ptr(ids)[0],
                                             as_ptr(dists)[0], as_ptr(counts)[0], as_ptr(nprobes)[0]))
         return ids, dists, counts, nprobes
+
+    def search_combined(self, queries, k, vectors, unindexed_vectors, unindexed_row_ids, nprobes=None,
+                        minimum_nprobes=None, maximum_nprobes=None, late_width=1, refine_factor=0, allow_bitmap=None,
+                        unindexed_allow_bitmap=None, mask_ids=None, mask_max_len=None, lower_bound=None,
+                        upper_bound=None):
+        """lb2_index_search_combined: a nearest() query on an index that does not cover every row (knn_combined,
+        scanner.rs:2946-3027).  The index search (fixed `nprobes`, or minimum / maximum nprobes as in search_probed)
+        runs with refine factor max(1, refine_factor) against `vectors` (the indexed column, row id = row number);
+        the unindexed rows (`unindexed_vectors` with their `unindexed_row_ids`, filtered by `unindexed_allow_bitmap`)
+        are searched flat with the index metric; the two lists are merged by (distance, row id).
+        Returns (ids, dists, counts, nprobes); nprobes is None with a fixed nprobes."""
+        from ._lib import ProbeParams, SearchParams, UnindexedRows
+        dt = getattr(self, "_dt", F32)
+        npdt = {F32: np.float32, F16: np.float16, U8: np.uint8, BF16: np.uint16}[dt]
+        probed = nprobes is None
+        if not isinstance(queries, (DeviceArray, PinnedArray)):
+            queries = np.ascontiguousarray(queries, dtype=npdt)
+        if not isinstance(vectors, (DeviceArray, PinnedArray)):
+            vectors = np.ascontiguousarray(vectors, dtype=npdt)
+        if not isinstance(unindexed_vectors, (DeviceArray, PinnedArray)):
+            unindexed_vectors = np.ascontiguousarray(unindexed_vectors, dtype=npdt)
+        nq = queries.shape[0]
+        ids, dists, counts = np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32), np.empty(nq, np.uint32)
+        nprobes_out = np.empty(nq, np.uint32) if probed else None
+        if mask_ids is not None and not isinstance(mask_ids, (DeviceArray, PinnedArray)):
+            mask_ids = np.ascontiguousarray(np.sort(np.asarray(mask_ids, dtype=np.uint64)))
+        qp, _k1 = as_ptr(queries)
+        vp, _k0 = as_ptr(vectors)
+        bp, _k2 = as_ptr(_bitmap(allow_bitmap))
+        uvp, _k3 = as_ptr(unindexed_vectors)
+        urp, _k4 = as_ptr(_row_ids(unindexed_row_ids))
+        ubp, _k5 = as_ptr(_bitmap(unindexed_allow_bitmap))
+        mp, _k6 = as_ptr(mask_ids)
+        if mask_ids is not None and mp.value is None:  # an empty numpy array has no buffer address to pass
+            _k6 = np.zeros(1, np.uint64)
+            mp = C.c_void_p(_k6.ctypes.data)
+        if urp is not None and urp.value is None:      # no unindexed rows: any valid address stands for the empty list
+            _k4 = np.zeros(1, np.uint64)
+            urp = C.c_void_p(_k4.ctypes.data)
+        sp = SearchParams(k, 0 if probed else nprobes, refine_factor, vp.value, vectors.shape[0],
+                          bp.value if bp is not None else None, int(lower_bound is not None),
+                          int(upper_bound is not None), float(lower_bound or 0.0), float(upper_bound or 0.0))
+        pp = None
+        if probed:
+            pp = ProbeParams(minimum_nprobes or 1, maximum_nprobes or 0, late_width, int(mask_max_len is not None),
+                             int(mask_max_len or 0), mp.value if mp is not None else None,
+                             0 if mask_ids is None else int(mask_ids.shape[0]))
+        u = UnindexedRows(uvp.value, unindexed_vectors.shape[0], urp.value if urp is not None else None,
+                          ubp.value if ubp is not None else None)
+        check(lib().lb2_index_search_combined(self._h, qp, C.c_uint64(nq), C.byref(sp),
+                                              C.byref(pp) if pp is not None else None, C.byref(u), as_ptr(ids)[0],
+                                              as_ptr(dists)[0], as_ptr(counts)[0], as_ptr(nprobes_out)[0]))
+        return ids, dists, counts, nprobes_out
 
     def search_async(self, queries, out, k=10, nprobes=1, cuda_stream=None, done_event=None, allow_bitmap=None,
                      lower_bound=None, upper_bound=None):

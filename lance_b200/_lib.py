@@ -82,7 +82,7 @@ EXPORTS = [
     "lb2_sq_train", "lb2_sq_encode", "lb2_ivfsq_build_params_default", "lb2_ivfsq_build", "lb2_index_create_sq",
     "lb2_index_load_sq", "lb2_index_export_sq", "lb2_rq_rotation", "lb2_ivfrq_transform",
     "lb2_ivfrq_build_params_default", "lb2_ivfrq_build", "lb2_index_create_rq", "lb2_index_load_rq",
-    "lb2_index_export_rq", "lb2_index_search_probed",
+    "lb2_index_export_rq", "lb2_index_search_probed", "lb2_flat_search", "lb2_index_search_combined",
 ]
 
 _lib = None
@@ -140,6 +140,17 @@ class ProbeParams(C.Structure):
     _fields_ = [("minimum_nprobes", C.c_uint32), ("maximum_nprobes", C.c_uint32), ("late_width", C.c_uint32),
                 ("has_max_len", C.c_uint32), ("max_len", C.c_uint64), ("mask_ids", C.c_void_p),
                 ("num_mask_ids", C.c_uint64)]
+
+
+class FlatSearchParams(C.Structure):
+    """lb2_flat_search_params (include/lance_b200.h)."""
+    _fields_ = [("k", C.c_uint32), ("allow_bitmap", C.c_void_p), ("has_lower_bound", C.c_uint32),
+                ("has_upper_bound", C.c_uint32), ("lower_bound", C.c_float), ("upper_bound", C.c_float)]
+
+
+class UnindexedRows(C.Structure):
+    """lb2_unindexed_rows (include/lance_b200.h)."""
+    _fields_ = [("vectors", C.c_void_p), ("n", C.c_uint64), ("row_ids", C.c_void_p), ("allow_bitmap", C.c_void_p)]
 
 
 class DeviceArray:

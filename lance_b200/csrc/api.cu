@@ -9,6 +9,7 @@
 #include "comm.cuh"
 #include "common.cuh"
 #include "exact.cuh"
+#include "flat_search.cuh"
 #include "index.cuh"
 #include "ivf_search.cuh"
 #include "kmeans.cuh"
@@ -518,6 +519,34 @@ lb2_status lb2_flat_topk_range(const float* dists, const uint64_t* row_ids, uint
 lb2_status lb2_flat_topk(const float* dists, const uint64_t* row_ids, uint64_t n, uint32_t k,
                          uint64_t* ids_out, float* dists_out, uint32_t* count_out) {
   return lb2_flat_topk_range(dists, row_ids, n, k, 0, 0.0f, 0, 0.0f, ids_out, dists_out, count_out);
+}
+
+lb2_status lb2_flat_search(const void* vectors, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                           const uint64_t* row_ids, const void* queries, uint64_t nq, const lb2_flat_search_params* p,
+                           uint64_t* row_ids_out, float* dists_out, uint32_t* counts_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(p, "null flat search params");
+  LB2_REQUIRE(p->k > 0, "k must be positive");
+  LB2_REQUIRE(d > 0, "dimension must be positive");
+  LB2_REQUIRE(dtype >= LB2_F32 && dtype <= LB2_U8, "unknown element type %d", (int)dtype);
+  LB2_REQUIRE((n == 0 || vectors) && (nq == 0 || queries) && (nq == 0 || (row_ids_out && dists_out)), "null argument");
+  const int m = metric_of(metric);
+  flat_search_check((int)d, dtype, m, (int)std::min<uint32_t>(p->k, 1025));
+  VecIn q(queries, (size_t)nq * d, dtype);
+  InArg<uint64_t> rid(row_ids, n), allow(p->allow_bitmap, p->allow_bitmap ? (size_t)((n + 63) / 64) : 0);
+  OutArg<uint64_t> oi(row_ids_out, (size_t)nq * p->k);
+  OutArg<float> od(dists_out, (size_t)nq * p->k);
+  OutArg<uint32_t> oc(counts_out, nq);
+  FlatFilter flt;
+  flt.allow = allow.get();
+  flt.has_lower = p->has_lower_bound != 0;
+  flt.has_upper = p->has_upper_bound != 0;
+  flt.lower = p->lower_bound;
+  flt.upper = p->upper_bound;
+  flat_search(q.get(), nq, (int)d, m, vectors, n, dtype, rid.get(), flt, (int)p->k, oi.get(), od.get(), oc.get());
+  oi.commit(); od.commit(); oc.commit();
+  sync_stream();
+  LB2_API_END
 }
 
 lb2_status lb2_comm_info(int* rank, int* nranks) {

@@ -11,6 +11,7 @@
 #include "common.cuh"
 #include "exact.cuh"
 #include "ivf_search.cuh"
+#include "row_distance.cuh"
 #include "scan.cuh"
 #include "topk.cuh"
 
@@ -23,41 +24,6 @@ namespace lb2 {
 // dot results are bit-identical to l2.rs:57-91 / dot.rs:30-58; cosine follows cosine.rs:143-174 in
 // structure (f32 FMA lanes) and is checked to the reference's own tolerance.
 // ------------------------------------------------------------------------------------------------
-// element of a stored / raw vector as f32 (l2.rs:100-106,156: f16 / bf16 elements are converted one by one)
-template <class T> __device__ __forceinline__ float ldf(const T* p, int e);
-template <> __device__ __forceinline__ float ldf<float>(const float* p, int e) { return p[e]; }
-template <> __device__ __forceinline__ float ldf<__half>(const __half* p, int e) { return __half2float(p[e]); }
-template <> __device__ __forceinline__ float ldf<__nv_bfloat16>(const __nv_bfloat16* p, int e) { return __bfloat162float(p[e]); }
-template <> __device__ __forceinline__ float ldf<uint8_t>(const uint8_t* p, int e) { return (float)p[e]; }
-
-template <int METRIC, class T = float>
-__device__ __forceinline__ float flat_row_distance(const float* __restrict__ q, const T* __restrict__ v,
-                                                   int d, int l, unsigned mask, float q_norm) {
-  const int n16 = d & ~15;
-  if (METRIC == METRIC_COSINE) {
-    float xy = 0.0f, yy = 0.0f;
-    for (int e = l; e < d; e += 16) {
-      const float y = ldf<T>(v, e);
-      xy = fmaf(q[e], y, xy);
-      yy = fmaf(y, y, yy);
-    }
-#pragma unroll
-    for (int off = 8; off >= 1; off >>= 1) {
-      xy += __shfl_xor_sync(mask, xy, off, 16);
-      yy += __shfl_xor_sync(mask, yy, off, 16);
-    }
-    return 1.0f - xy / q_norm / sqrtf(yy);
-  }
-  float acc = 0.0f;
-  for (int e = l; e < n16; e += 16) acc = f_add(acc, term<METRIC>(q[e], ldf<T>(v, e)));
-  float s = 0.0f;  // sequential tail, every lane redundantly (l2.rs:69-79)
-  for (int e = n16; e < d; ++e) s = f_add(s, term<METRIC>(q[e], ldf<T>(v, e)));
-  float t = 0.0f;
-#pragma unroll
-  for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, acc, qq, 16));
-  return finish<METRIC>(f_add(s, t));
-}
-
 template <int METRIC, class T>
 __global__ void __launch_bounds__(256)
 ivfflat_scan_kernel(const float* __restrict__ queries, int d, const uint32_t* __restrict__ probe_ids,
@@ -122,22 +88,6 @@ flat_topk_kernel(const float* __restrict__ dists, const uint64_t* __restrict__ r
   if (threadIdx.x == 0) *out_cnt = cnt;
 }
 
-// f(metric, element) with the metric as a std::integral_constant and the element type as a type_tag
-template <class T> struct type_tag { using type = T; };
-template <bool WITH_U8, class F>
-static void dispatch_metric_elem(int metric, int vdt, F&& f) {
-  auto by_elem = [&](auto m) {
-    if (vdt == LB2_F16) f(m, type_tag<__half>{});
-    else if (vdt == LB2_BF16) f(m, type_tag<__nv_bfloat16>{});
-    else if constexpr (WITH_U8) {
-      if (vdt == LB2_U8) f(m, type_tag<uint8_t>{}); else f(m, type_tag<float>{});
-    } else f(m, type_tag<float>{});
-  };
-  if (metric == METRIC_DOT) by_elem(std::integral_constant<int, METRIC_DOT>{});
-  else if (metric == METRIC_COSINE) by_elem(std::integral_constant<int, METRIC_COSINE>{});
-  else by_elem(std::integral_constant<int, METRIC_L2>{});
-}
-
 void ivfflat_search(const IvfSearch& s, const void* vectors, int vdt) {
   const int d = s.d, k = s.k;
   const size_t smem = sizeof(float) * (size_t)d + slot_smem_bytes(k);
@@ -162,60 +112,6 @@ void ivfflat_search(const IvfSearch& s, const void* vectors, int vdt) {
 // refine: exact distances of k' = k * refine_factor candidates from the raw vectors, then the k
 // best by (distance, row id)  (scanner.rs:2884-2905, flat.rs:95-148)
 // ------------------------------------------------------------------------------------------------
-// u8 L2 / dot: exact integer sums (wrapping like the reference's release build), one conversion to f32 (l2.rs:44-49,
-// dot.rs:152-161); q holds the u8 values of the other vector as f32
-template <int METRIC>
-__device__ __forceinline__ float u8_row_distance(const float* __restrict__ q, const uint8_t* __restrict__ v, int d,
-                                                 int l, unsigned mask) {
-  uint32_t acc = 0;
-  for (int e = l; e < d; e += 16) {
-    const int x = __float2int_rn(q[e]), y = v[e];
-    acc += METRIC == METRIC_DOT ? (uint32_t)(x * y) : (uint32_t)((x - y) * (x - y));
-  }
-#pragma unroll
-  for (int off = 8; off >= 1; off >>= 1) acc += __shfl_xor_sync(mask, acc, off, 16);
-  return finish<METRIC>(__uint2float_rn(acc));
-}
-
-// 16-bit dot: dot_scalar::<T, f32, 32> (dot.rs:30-58) -- bf16 always (dot.rs:78-83), f16 without the fp16 C kernel
-// (dot.rs:133): lane l owns the accumulators l and l + 16, the d % 32 tail comes first, the 32 sums are folded 0..31
-template <class T>
-__device__ __forceinline__ float dot32_row_distance(const float* __restrict__ q, const T* __restrict__ v, int d,
-                                                    int l, unsigned mask) {
-  const int n32 = d & ~31;
-  float a0 = 0.0f, a1 = 0.0f;
-  for (int e = l; e < n32; e += 32) {
-    a0 = f_add(a0, __fmul_rn(q[e], ldf<T>(v, e)));
-    a1 = f_add(a1, __fmul_rn(q[e + 16], ldf<T>(v, e + 16)));
-  }
-  float s = 0.0f;  // sequential tail, every lane redundantly
-  for (int e = n32; e < d; ++e) s = f_add(s, __fmul_rn(q[e], ldf<T>(v, e)));
-  float t = 0.0f;
-#pragma unroll
-  for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, a0, qq, 16));
-#pragma unroll
-  for (int qq = 0; qq < 16; ++qq) t = f_add(t, __shfl_sync(mask, a1, qq, 16));
-  return finish<METRIC_DOT>(f_add(s, t));
-}
-
-// The refine plan takes the distance function of the column's own element type (flat.rs:94-150), unlike the
-// IVF_FLAT scan, whose storage is f32 (flat/storage.rs:352-365):
-//  * f16 dot: the 32-lane dot_scalar;
-//  * u8 L2 / dot: exact integer sums; the query came in as u8 too, so its f32 view holds integers;
-//  * everything else (f16 L2, bf16, cosine) as flat_row_distance: the reference refuses bf16 keys in refine, so bf16
-//    keeps the scan's 16-lane rule (DESIGN.md section 5).
-template <int METRIC, class T>
-__device__ __forceinline__ float refine_row_distance(const float* __restrict__ q, const T* __restrict__ v, int d,
-                                                     int l, unsigned mask, float q_norm) {
-  if constexpr (std::is_same<T, uint8_t>::value && METRIC != METRIC_COSINE) {
-    return u8_row_distance<METRIC>(q, v, d, l, mask);
-  } else if constexpr (std::is_same<T, __half>::value && METRIC == METRIC_DOT) {
-    return dot32_row_distance<T>(q, v, d, l, mask);
-  } else {
-    return flat_row_distance<METRIC, T>(q, v, d, l, mask, q_norm);
-  }
-}
-
 template <int METRIC, class T>
 __global__ void __launch_bounds__(256)
 refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ vectors,

@@ -5,6 +5,7 @@
 
 #include "build.cuh"
 #include "comm.cuh"
+#include "flat_search.cuh"
 #include "index.cuh"
 #include "ivf_search.cuh"
 #include "member_sort.cuh"
@@ -659,35 +660,97 @@ lb2_status lb2_index_search_ex(lb2_index* index, const void* queries, uint64_t n
   LB2_API_END
 }
 
+// the probe rule of lb2_index_search_probed, its checks and its staged arguments (alive as long as the object)
+namespace {
+struct ProbedSearch {
+  InArg<uint64_t> mask;
+  DevBuf<uint64_t> no_ids;  // an iterable, empty allow list
+  OutArg<uint32_t> np_out;
+  ProbeRule pr;
+  ProbedSearch(const lb2_search_params* sp, const lb2_probe_params* pp, uint64_t nq, uint32_t* nprobes_out) {
+    LB2_REQUIRE(sp->nprobes == 0, "nprobes must be 0: the probe parameters decide the probes");
+    LB2_REQUIRE(sp->refine_factor == 0 || sp->refine_vectors, "refine_factor > 0 needs refine_vectors");
+    LB2_REQUIRE(pp->minimum_nprobes >= 1, "minimum_nprobes must be at least 1");
+    LB2_REQUIRE(pp->maximum_nprobes == 0 || pp->maximum_nprobes >= pp->minimum_nprobes,
+                "maximum_nprobes %u is below minimum_nprobes %u", pp->maximum_nprobes, pp->minimum_nprobes);
+    LB2_REQUIRE(pp->late_width >= 1, "late_width must be at least 1");
+    LB2_REQUIRE(sp->allow_bitmap || (!pp->has_max_len && !pp->mask_ids), "max_len and mask_ids need an allow bitmap");
+    if (current_comm() && current_comm()->nranks > 1)
+      fail(LB2_UNSUPPORTED, "a search with minimum / maximum nprobes on a row-sharded index is not implemented");
+    mask.set(pp->mask_ids, pp->mask_ids ? pp->num_mask_ids : 0);
+    if (pp->mask_ids && pp->num_mask_ids == 0) no_ids.alloc(1);
+    np_out.set(nprobes_out, nq);
+    pr.min_np = pp->minimum_nprobes;
+    pr.max_np = pp->maximum_nprobes;
+    pr.late_width = pp->late_width;
+    pr.k = sp->k;
+    pr.has_max_len = pp->has_max_len != 0;
+    pr.max_len = pp->max_len;
+    pr.mask_ids = pp->mask_ids ? (mask.get() ? mask.get() : no_ids.p) : nullptr;
+    pr.num_mask_ids = pp->mask_ids ? pp->num_mask_ids : 0;
+    pr.nprobes_out = np_out.get();
+  }
+};
+}  // namespace
+
 lb2_status lb2_index_search_probed(lb2_index* index, const void* queries, uint64_t nq, const lb2_search_params* sp,
                                    const lb2_probe_params* pp, uint64_t* row_ids_out, float* dists_out,
                                    uint32_t* counts_out, uint32_t* nprobes_out) {
   LB2_API_BEGIN
   LB2_REQUIRE(sp && pp && index, "null argument");
-  LB2_REQUIRE(sp->nprobes == 0, "nprobes must be 0: the probe parameters decide the probes");
-  LB2_REQUIRE(sp->refine_factor == 0 || sp->refine_vectors, "refine_factor > 0 needs refine_vectors");
-  LB2_REQUIRE(pp->minimum_nprobes >= 1, "minimum_nprobes must be at least 1");
-  LB2_REQUIRE(pp->maximum_nprobes == 0 || pp->maximum_nprobes >= pp->minimum_nprobes,
-              "maximum_nprobes %u is below minimum_nprobes %u", pp->maximum_nprobes, pp->minimum_nprobes);
-  LB2_REQUIRE(pp->late_width >= 1, "late_width must be at least 1");
-  LB2_REQUIRE(sp->allow_bitmap || (!pp->has_max_len && !pp->mask_ids), "max_len and mask_ids need an allow bitmap");
+  ProbedSearch ps(sp, pp, nq, nprobes_out);
+  index_search_impl(index, queries, nq, *sp, row_ids_out, dists_out, counts_out, &ps.pr);
+  ps.np_out.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_index_search_combined(lb2_index* index, const void* queries, uint64_t nq, const lb2_search_params* sp,
+                                     const lb2_probe_params* pp, const lb2_unindexed_rows* u, uint64_t* row_ids_out,
+                                     float* dists_out, uint32_t* counts_out, uint32_t* nprobes_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && sp, "null argument");
+  LB2_REQUIRE(sp->k > 0, "k must be positive");
+  LB2_REQUIRE(sp->refine_vectors, "the combined search re-scores the index's rows exactly: refine_vectors is required");
+  LB2_REQUIRE(u && u->row_ids, "the unindexed rows and their row ids are required");
+  LB2_REQUIRE(u->n == 0 || u->vectors, "null unindexed vectors");
+  LB2_REQUIRE(!nprobes_out || pp, "nprobes_out needs probe parameters");
   if (current_comm() && current_comm()->nranks > 1)
-    fail(LB2_UNSUPPORTED, "a search with minimum / maximum nprobes on a row-sharded index is not implemented");
-  InArg<uint64_t> mask(pp->mask_ids, pp->mask_ids ? pp->num_mask_ids : 0);
-  DevBuf<uint64_t> no_ids(pp->mask_ids && pp->num_mask_ids == 0 ? 1 : 0);  // an iterable, empty allow list
-  OutArg<uint32_t> np_out(nprobes_out, nq);
-  ProbeRule pr;
-  pr.min_np = pp->minimum_nprobes;
-  pr.max_np = pp->maximum_nprobes;
-  pr.late_width = pp->late_width;
-  pr.k = sp->k;
-  pr.has_max_len = pp->has_max_len != 0;
-  pr.max_len = pp->max_len;
-  pr.mask_ids = pp->mask_ids ? (mask.get() ? mask.get() : no_ids.p) : nullptr;
-  pr.num_mask_ids = pp->mask_ids ? pp->num_mask_ids : 0;
-  pr.nprobes_out = np_out.get();
-  index_search_impl(index, queries, nq, *sp, row_ids_out, dists_out, counts_out, &pr);
-  np_out.commit();
+    fail(LB2_UNSUPPORTED, "a combined search on a row-sharded index is not implemented");
+  const int k = (int)sp->k, d = index->d;
+  flat_search_check(d, index->dtype, index->metric, (int)std::min<uint32_t>(sp->k, 1025));
+  std::unique_ptr<ProbedSearch> ps;
+  if (pp) ps.reset(new ProbedSearch(sp, pp, nq, nprobes_out));
+  // the index's rows: refined, so their distances are exact (scanner.rs:2884-2905)
+  lb2_search_params s = *sp;
+  s.refine_factor = std::max<uint32_t>(1, sp->refine_factor);
+  const size_t nk = (size_t)nq * k;
+  DevBuf<uint64_t> ids(std::max<size_t>(1, 2 * nk));
+  DevBuf<float> dists(std::max<size_t>(1, 2 * nk));
+  DevBuf<uint32_t> cnts(std::max<uint64_t>(1, 2 * nq));
+  index_search_impl(index, queries, nq, s, ids.p, dists.p, cnts.p, ps ? &ps->pr : nullptr);
+  // the unindexed rows: flat_knn with the index metric on the original query (scanner.rs:2993-3013)
+  VecIn q(queries, (size_t)nq * d, index->dtype);
+  InArg<uint64_t> rid(u->row_ids, u->n), allow(u->allow_bitmap, u->allow_bitmap ? (size_t)((u->n + 63) / 64) : 0);
+  FlatFilter flt;
+  flt.allow = allow.get();
+  flt.has_lower = sp->has_lower_bound != 0;
+  flt.has_upper = sp->has_upper_bound != 0;
+  flt.lower = sp->lower_bound;
+  flt.upper = sp->upper_bound;
+  flat_search(q.get(), nq, d, index->metric, u->vectors, u->n, index->dtype, rid.get(), flt, k, ids.p + nk,
+              dists.p + nk, cnts.p + nq);
+  // the union by (_distance, _rowid), first k
+  OutArg<uint64_t> oi(row_ids_out, nk);
+  OutArg<float> od(dists_out, nk);
+  OutArg<uint32_t> oc(counts_out, nq);
+  {
+    TagScope tg("search");
+    merge_lists("merge_combined", nq, dists.p, ids.p, cnts.p, 2, k, nk, nk, (size_t)k, nq, 1, oi.get(), od.get(),
+                oc.get());
+  }
+  oi.commit(); od.commit(); oc.commit();
+  if (ps) ps->np_out.commit();
   sync_stream();
   LB2_API_END
 }

@@ -38,6 +38,8 @@ select_probes_kernel(const float* __restrict__ all_dists, int K, int nprobes,
 // global merge per query: ascending (distance, row id), first k.  Candidate e of list pi of query qi sits
 // at cand[pi * stride_p + qi * stride_q + e] (per-partition lists of one GPU: stride_p = k, stride_q = np * k;
 // per-rank results gathered from a sharded index: stride_p = the rank stride, stride_q = k).
+// A query may hold nl > np lists: they are merged in groups of np consecutive lists, output row qi * ng + g for group
+// g (ng = ceil(nl / np)); nl = np is the plain merge.  Block b merges group b % ng of query b / ng.
 // Lists of up to MERGE_RANK_MAX candidates in total are merged by RANK COUNTING in shared memory: every candidate
 // counts the candidates that precede it in (distance, row id) order -- the pairs are unique -- and the ones with rank
 // < k are the output, already in place.  (The k-round argmin below re-reads all candidates from global memory per
@@ -46,7 +48,7 @@ constexpr int MERGE_RANK_MAX = 2048;
 __global__ void __launch_bounds__(256)
 merge_rank_kernel(const float* __restrict__ cand_d, const uint64_t* __restrict__ cand_id,
                   const uint32_t* __restrict__ cand_cnt, int np, int k, size_t stride_p_d, size_t stride_p_id,
-                  size_t stride_q, size_t cnt_stride_p, size_t cnt_stride_q, uint64_t* __restrict__ out_id,
+                  size_t stride_q, size_t cnt_stride_p, size_t cnt_stride_q, int nl, uint64_t* __restrict__ out_id,
                   float* __restrict__ out_d, uint32_t* __restrict__ out_cnt) {
   extern __shared__ __align__(16) unsigned char mr_smem[];
   const int total = np * k;
@@ -54,15 +56,18 @@ merge_rank_kernel(const float* __restrict__ cand_d, const uint64_t* __restrict__
   int32_t* s_key = reinterpret_cast<int32_t*>(s_id + total);         // [total]; invalid entries: key = INT_MAX, id = ~0
   __shared__ uint32_t s_valid;
   const size_t qi = blockIdx.x;
+  const int ng = nl > np ? (nl + np - 1) / np : 1;
+  const size_t q = qi / ng;
+  const int first = (int)(qi % ng) * np;
   const int tid = threadIdx.x;
   if (tid == 0) s_valid = 0;
   __syncthreads();
   uint32_t myvalid = 0;
   for (int c = tid; c < total; c += 256) {
-    const int pi = c / k, e = c % k;
-    const bool ok = (uint32_t)e < cand_cnt[pi * cnt_stride_p + qi * cnt_stride_q];
-    s_key[c] = ok ? total_order_key(cand_d[pi * stride_p_d + qi * stride_q + e]) : 0x7fffffff;
-    s_id[c] = ok ? cand_id[pi * stride_p_id + qi * stride_q + e] : ~0ull;
+    const int pi = first + c / k, e = c % k;
+    const bool ok = pi < nl && (uint32_t)e < cand_cnt[pi * cnt_stride_p + q * cnt_stride_q];
+    s_key[c] = ok ? total_order_key(cand_d[pi * stride_p_d + q * stride_q + e]) : 0x7fffffff;
+    s_id[c] = ok ? cand_id[pi * stride_p_id + q * stride_q + e] : ~0ull;
     myvalid += ok ? 1u : 0u;
   }
   if (myvalid) atomicAdd(&s_valid, myvalid);
@@ -92,22 +97,25 @@ merge_rank_kernel(const float* __restrict__ cand_d, const uint64_t* __restrict__
 __global__ void __launch_bounds__(128)
 merge_kernel(const float* __restrict__ cand_d, const uint64_t* __restrict__ cand_id,
              const uint32_t* __restrict__ cand_cnt, int np, int k, size_t stride_p_d, size_t stride_p_id,
-             size_t stride_q, size_t cnt_stride_p, size_t cnt_stride_q, uint64_t* __restrict__ out_id,
+             size_t stride_q, size_t cnt_stride_p, size_t cnt_stride_q, int nl, uint64_t* __restrict__ out_id,
              float* __restrict__ out_d, uint32_t* __restrict__ out_cnt) {
   const size_t qi = blockIdx.x;
+  const int ng = nl > np ? (nl + np - 1) / np : 1;
+  const size_t q = qi / ng;
+  const int first = (int)(qi % ng) * np;
   const int tid = threadIdx.x;
   const int r = (int)emit_ascending<128>(
       k, np * k,
       [&](uint32_t c, int32_t& key, uint64_t& id) {
-        const int pi = c / k, e = c % k;
-        if ((uint32_t)e >= cand_cnt[pi * cnt_stride_p + qi * cnt_stride_q]) return false;
-        key = total_order_key(cand_d[pi * stride_p_d + qi * stride_q + e]);
-        id = cand_id[pi * stride_p_id + qi * stride_q + e];
+        const int pi = first + c / k, e = c % k;
+        if (pi >= nl || (uint32_t)e >= cand_cnt[pi * cnt_stride_p + q * cnt_stride_q]) return false;
+        key = total_order_key(cand_d[pi * stride_p_d + q * stride_q + e]);
+        id = cand_id[pi * stride_p_id + q * stride_q + e];
         return true;
       },
       [&](uint32_t r, uint32_t c, int32_t, uint64_t id) {
         out_id[qi * k + r] = id;
-        out_d[qi * k + r] = cand_d[(c / k) * stride_p_d + qi * stride_q + (c % k)];
+        out_d[qi * k + r] = cand_d[(first + c / k) * stride_p_d + q * stride_q + (c % k)];
       });
   for (int e = r + tid; e < k; e += 128) {
     out_id[qi * k + e] = ~0ull;
@@ -124,19 +132,46 @@ void find_partitions_f32(const float* centroids, int K, int d, int metric, const
   LB2_LAUNCH("select_probes", select_probes_kernel, (unsigned)nq, 128, 0, all.p, K, nprobes, ids, dists);
 }
 
-// np lists of <= k candidates per query -> the k smallest by (distance, row id)
-static void merge_lists(const char* name, uint64_t nq, const float* cand_d, const uint64_t* cand_id, const uint32_t* cand_cnt,
-                        int np, int k, size_t stride_p_d, size_t stride_p_id, size_t stride_q, size_t cnt_stride_p,
-                        size_t cnt_stride_q, uint64_t* out_ids, float* out_dists, uint32_t* out_counts) {
+void merge_lists(const char* name, uint64_t nq, const float* cand_d, const uint64_t* cand_id, const uint32_t* cand_cnt,
+                 int np, int k, size_t stride_p_d, size_t stride_p_id, size_t stride_q, size_t cnt_stride_p,
+                 size_t cnt_stride_q, uint64_t* out_ids, float* out_dists, uint32_t* out_counts, int nl) {
   if (nq == 0) return;
+  if (nl < np) nl = np;
+  const uint64_t blocks = nq * (uint64_t)(nl > np ? (nl + np - 1) / np : 1);
   const size_t total = (size_t)np * k;
   if (total <= (size_t)MERGE_RANK_MAX) {
-    LB2_LAUNCH(name, merge_rank_kernel, (unsigned)nq, 256, total * 12, cand_d, cand_id, cand_cnt, np, k, stride_p_d, stride_p_id,
-               stride_q, cnt_stride_p, cnt_stride_q, out_ids, out_dists, out_counts);
+    LB2_LAUNCH(name, merge_rank_kernel, (unsigned)blocks, 256, total * 12, cand_d, cand_id, cand_cnt, np, k, stride_p_d,
+               stride_p_id, stride_q, cnt_stride_p, cnt_stride_q, nl, out_ids, out_dists, out_counts);
   } else {
-    LB2_LAUNCH(name, merge_kernel, (unsigned)nq, 128, 0, cand_d, cand_id, cand_cnt, np, k, stride_p_d, stride_p_id, stride_q,
-               cnt_stride_p, cnt_stride_q, out_ids, out_dists, out_counts);
+    LB2_LAUNCH(name, merge_kernel, (unsigned)blocks, 128, 0, cand_d, cand_id, cand_cnt, np, k, stride_p_d, stride_p_id,
+               stride_q, cnt_stride_p, cnt_stride_q, nl, out_ids, out_dists, out_counts);
   }
+}
+
+// nl lists per query, laid out [nq][nl][k] with counts [nq][nl]: groups of MERGE_RANK_MAX / k lists are merged by rank
+// counting, level by level (one launch per level), until one merge of at most MERGE_RANK_MAX candidates is left
+void merge_list_tree(const char* name, uint64_t nq, const float* cand_d, const uint64_t* cand_id,
+                     const uint32_t* cand_cnt, int nl, int k, uint64_t* out_ids, float* out_dists,
+                     uint32_t* out_counts) {
+  if (nq == 0) return;
+  const int G = std::max(2, MERGE_RANK_MAX / k);
+  DevBuf<float> lvl_d[2];
+  DevBuf<uint64_t> lvl_id[2];
+  DevBuf<uint32_t> lvl_cnt[2];
+  for (int cur = 0; nl > G; cur ^= 1) {
+    const int ng = (nl + G - 1) / G;
+    lvl_d[cur].alloc(nq * ng * k);
+    lvl_id[cur].alloc(nq * ng * k);
+    lvl_cnt[cur].alloc(nq * ng);
+    merge_lists(name, nq, cand_d, cand_id, cand_cnt, G, k, (size_t)k, (size_t)k, (size_t)nl * k, 1, (size_t)nl,
+                lvl_id[cur].p, lvl_d[cur].p, lvl_cnt[cur].p, nl);
+    cand_d = lvl_d[cur].p;
+    cand_id = lvl_id[cur].p;
+    cand_cnt = lvl_cnt[cur].p;
+    nl = ng;
+  }
+  merge_lists(name, nq, cand_d, cand_id, cand_cnt, nl, k, (size_t)k, (size_t)k, (size_t)nl * k, 1, (size_t)nl, out_ids,
+              out_dists, out_counts);
 }
 
 // partitions are found with L2 on the (normalised) vectors for cosine (ivf.rs:149-185)

@@ -72,6 +72,17 @@ void run_ivf_search(const IvfSearch& s, ScanRef scan);
 
 void find_partitions_f32(const float* centroids, int K, int d, int metric, const float* queries,
                          uint64_t nq, int nprobes, uint32_t* ids, float* dists);
+// np lists of <= k candidates per query -> the k smallest by (distance, row id) per query, ascending; unused slots
+// (~0, +inf).  List pi of query q: distances at cand_d[pi * stride_p_d + q * stride_q], ids likewise, count at
+// cand_cnt[pi * cnt_stride_p + q * cnt_stride_q].  nl > np: the query's nl lists are merged in groups of np
+// (output row q * ceil(nl / np) + group).
+void merge_lists(const char* name, uint64_t nq, const float* cand_d, const uint64_t* cand_id, const uint32_t* cand_cnt,
+                 int np, int k, size_t stride_p_d, size_t stride_p_id, size_t stride_q, size_t cnt_stride_p,
+                 size_t cnt_stride_q, uint64_t* out_ids, float* out_dists, uint32_t* out_counts, int nl = 0);
+// [nq][nl][k] lists (counts [nq][nl]) -> [nq][k], any nl >= 1, by rank-counting merges only
+void merge_list_tree(const char* name, uint64_t nq, const float* cand_d, const uint64_t* cand_id,
+                     const uint32_t* cand_cnt, int nl, int k, uint64_t* out_ids, float* out_dists,
+                     uint32_t* out_counts);
 // all ranks' [nq][k] results of a row-sharded index -> the global top-k by (distance, row id) on every rank
 void merge_sharded_topk(const uint64_t* ids, const float* dists, const uint32_t* counts, uint64_t nq, int k,
                         uint64_t* out_ids, float* out_dists, uint32_t* out_counts);

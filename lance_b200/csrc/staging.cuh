@@ -387,13 +387,17 @@ class Source {
 uint64_t gather_finite_sample(Source& src, std::vector<uint64_t>& rows, bool normalize, DevBuf<float>& out);
 std::vector<uint64_t> sample_rows(uint64_t n, uint64_t s, uint64_t seed);
 
+// the rows per call of for_each_chunk (a little more than one chunk is not split: SIFT-1M is one call)
+inline uint64_t chunk_step(const Source& src) {
+  const uint64_t n = src.n(), chunk = src.rows_per_chunk();
+  return n <= chunk + chunk / 2 ? std::max<uint64_t>(n, 1) : chunk;
+}
+
 // one pass over a caller's matrix in chunks of rows: f(xf, xnat, r0, rows) with xf = the chunk as f32 on the device
 // and xnat = the same rows in the column's own type (for assign_f32: tc_assign.cu, "native 16-bit rows")
 template <class F>
 void for_each_chunk(Source& src, F&& f) {
-  const uint64_t n = src.n(), chunk = src.rows_per_chunk();
-  // (a little more than one chunk is not split: SIFT-1M is one call)
-  const uint64_t step = n <= chunk + chunk / 2 ? std::max<uint64_t>(n, 1) : chunk;
+  const uint64_t n = src.n(), step = chunk_step(src);
   for (uint64_t r0 = 0; r0 < n; r0 += step) {
     const uint64_t rows = std::min(step, n - r0);
     const float* xf = src.rows_f32(r0, rows);
