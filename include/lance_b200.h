@@ -490,6 +490,56 @@ lb2_status lb2_index_load_sq(lb2_index* index, const uint32_t* part_ids, const u
 lb2_status lb2_index_export_sq(const lb2_index* index, void* centroids_out, double* bounds_out,
                                uint64_t* part_offsets_out, uint8_t* codes_out, uint64_t* row_ids_out);
 
+/* ---- IVF_HNSW_SQ: IVFIndex<HNSW, ScalarQuantizer> (lance-index/src/vector/hnsw/builder.rs) ------------------
+ * An IVF_SQ index (same IVF stage, bounds and codes for the same arguments) with an HNSW graph per partition over
+ * the partition's SQ codes; every distance, row to row and query to row, is the SQ distance of lb2_index_search on
+ * IVF_SQ (sq/storage.rs:387-444, storage.rs:102-105).  Node i of partition p is its storage position
+ * part_offsets[p] + i.  The graph of a partition is HNSW::index_vectors (builder.rs:742-775) with the nodes
+ * inserted 1 .. n_p - 1 in ascending order (the reference inserts in parallel); node 0 has max_level levels and is
+ * the entry point (:354-376), node i >= 1 gets 1 + random_level() levels (:386-393) from a u32 draw keyed by (seed,
+ * p, i) compared against floor(2^32 / m^l).  Ties in select_neighbors_heuristic (hnsw.rs:60-88) keep their order.
+ * Searches go through lb2_index_search / _refine / _ex / _probed / _combined / _async / _sharded with the default ef
+ * k' + k' / 2, k' = k * refine_factor (:563-573), or through lb2_index_search_hnsw with an explicit ef: each probed
+ * partition is HNSW::search (builder.rs:678-739); ef < k' is LB2_INVALID_ARG (:687-692).  A prefilter that leaves fewer than
+ * n_p * 10 / 100 rows of a partition takes the flat branch (:238-280, range lower < d <= upper), otherwise the
+ * graph (:164-201, range lower <= d < upper).  lb2_index_repartition, _update and _load_sq refuse the index; so
+ * does a build with a communicator of more than one rank.
+ *
+ * The graph crosses the ABI in the device layout: levels[n] (levels per row), level 0 dense (counts0[n],
+ * neighbors0 / dists0 [n][2m]) and the upper levels node by node in storage order: a row with L levels owns L - 1
+ * consecutive upper rows, levels 1 .. L-1 (counts_up[r], neighbors_up / dists_up [r][m]).  Lists are in the order of
+ * level_neighbors_ranked (graph/builder.rs:33-48); neighbour ids are partition-local. */
+typedef struct {
+  lb2_ivfsq_build_params sq;
+  uint32_t max_level;       /* HnswBuildParams (hnsw/builder.rs:63-72): 7 */
+  uint32_t m;               /* 20; level 0 keeps up to 2m neighbours, the others m */
+  uint32_t ef_construction; /* 150 */
+} lb2_ivfhnswsq_build_params;
+void lb2_ivfhnswsq_build_params_default(lb2_ivfhnswsq_build_params* p);
+/* IvfIndexBuilder<HNSW, ScalarQuantizer>::build: lb2_ivfsq_build, then every partition's graph on the device (one
+ * warp per partition, the largest partitions first); the level draws use params->sq.seed. */
+lb2_status lb2_ivfhnswsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                               const lb2_ivfhnswsq_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                               lb2_build_stats* stats);
+/* attach a graph (host or device arrays in the layout above) to an IVF_SQ index made by lb2_index_create_sq +
+ * lb2_index_load_sq; every neighbour must be a node of its partition that has the level (else LB2_INVALID_ARG) */
+lb2_status lb2_index_load_hnsw_sq(lb2_index* index, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                                  const uint8_t* levels, const uint32_t* counts0, const uint32_t* neighbors0,
+                                  const float* dists0, const uint32_t* counts_up, const uint32_t* neighbors_up,
+                                  const float* dists_up);
+/* the graph's parameters and its number of upper-level rows (any pointer may be NULL) */
+lb2_status lb2_index_hnsw_sq_info(const lb2_index* index, uint32_t* max_level, uint32_t* m, uint32_t* ef_construction,
+                                  uint64_t* num_upper_rows);
+/* the graph in the layout above; any pointer may be NULL */
+lb2_status lb2_index_export_hnsw_sq(const lb2_index* index, uint8_t* levels_out, uint32_t* counts0_out,
+                                    uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
+                                    uint32_t* neighbors_up_out, float* dists_up_out);
+/* lb2_index_search_ex (pp NULL) or lb2_index_search_probed (pp set; nprobes_out nullable) of an IVF_HNSW_SQ index with
+ * the graph search's ef for this call (Query::ef, HnswQueryParams::ef, builder.rs:563-573); ef = 0: k' + k' / 2 */
+lb2_status lb2_index_search_hnsw(lb2_index* index, const void* queries, uint64_t nq, const lb2_search_params* sp,
+                                 const lb2_probe_params* pp, uint32_t ef, uint64_t* row_ids_out, float* dists_out,
+                                 uint32_t* counts_out, uint32_t* nprobes_out);
+
 /* ---- IVF_RQ: IVFIndex<FlatIndex, RabitQuantizer> (lance-index/src/vector/bq/) ------------------------------------
  * create_index(.., "IVF_RQ") builds an IvfIndexBuilder<FlatIndex, RabitQuantizer> (rust/lance/src/index/vector.rs:
  * 452-470).  code_dim = d * num_bits; the rotation R is code_dim x code_dim, of which the first d columns are used.

@@ -13,14 +13,16 @@ import numpy as np
 
 from ._lib import (BF16, COSINE, DOT, F16, F32, L2, METRICS, U8, BuildParams, BuildStats, FlatBuildParams,
                    DeviceArray, KMeansParams as _CKMeansParams, LanceB200Error, PinnedArray,
-                   PQParams as _CPQParams, RqBuildParams as _CRqBuildParams, SqBuildParams as _CSqBuildParams, as_ptr,
+                   PQParams as _CPQParams, RqBuildParams as _CRqBuildParams, SqBuildParams as _CSqBuildParams,
+                   HnswSqBuildParams as _CHnswSqBuildParams, as_ptr,
                    check, device_count, lib)
 
 __all__ = ["device_count", "DeviceArray", "PinnedArray", "LanceB200Error", "train_kmeans",
            "compute_partitions", "kmeans_find_partitions", "compute_residual", "normalize_fsl",
            "l2_distance_batch", "dot_distance_batch", "cosine_distance_batch", "PQBuildParams", "ProductQuantizer",
            "build_distance_table_l2", "compute_pq_distance", "flat_topk", "flat_search", "IvfPqIndex",
-           "IvfBuildParams", "IvfFlatIndex", "SQBuildParams", "ScalarQuantizer", "IvfSqIndex", "RQBuildParams",
+           "IvfBuildParams", "IvfFlatIndex", "SQBuildParams", "ScalarQuantizer", "IvfSqIndex", "HnswBuildParams",
+           "IvfHnswSqIndex", "RQBuildParams",
            "RabitQuantizer", "IvfRqIndex", "launch_count", "profile"]
 
 
@@ -967,6 +969,154 @@ class IvfSqIndex(IvfPqIndex):
                                         C.c_void_p(rid.ctypes.data)))
         return dict(centroids=cent, bounds=(float(bounds[0]), float(bounds[1])), part_offsets=off, codes=codes,
                     row_ids=rid)
+
+
+# ---- lance-index::vector::hnsw over SQ storage (IVF_HNSW_SQ) ---------------------------------------------
+class HnswBuildParams:
+    """lance_index::vector::hnsw::builder::HnswBuildParams (hnsw/builder.rs:47-72)."""
+
+    def __init__(self, max_level=7, m=20, ef_construction=150):
+        self.max_level, self.m, self.ef_construction = max_level, m, ef_construction
+
+
+class IvfHnswSqIndex(IvfSqIndex):
+    """Device-resident IVFIndex<HNSW, ScalarQuantizer> (IVF_HNSW_SQ): IVF_SQ's partitions, bounds and codes with an
+    HNSW graph per partition over the codes (lance-index/src/vector/hnsw/builder.rs).  search, search_refine,
+    search_ex and search_probed take ef= (lb2_index_search_hnsw); the other search methods use k' + k' / 2."""
+
+    @classmethod
+    def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
+              centroids=None, row_ids=None, bf16=False, sq_params=None, hnsw_params=None):
+        """create_index(.., "IVF_HNSW_SQ"); the IVF stage, bounds and codes equal IvfSqIndex.build's with the same
+        arguments.  The graphs' level draws use `seed`."""
+        sq_params = sq_params or SQBuildParams()
+        hnsw_params = hnsw_params or HnswBuildParams()
+        data, dt = _typed(data, bf16)
+        n, d = data.shape
+        bp = _CHnswSqBuildParams()
+        lib().lb2_ivfhnswsq_build_params_default(C.byref(bp))
+        bp.sq.num_partitions = num_partitions
+        bp.sq.ivf.max_iters, bp.sq.ivf.sample_rate, bp.sq.ivf.seed, bp.sq.seed = max_iters, sample_rate, seed, seed
+        bp.sq.num_bits, bp.sq.sample_rate = sq_params.num_bits, sq_params.sample_rate
+        bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
+        keep = None
+        if centroids is not None:
+            keep = _f32(centroids)
+            bp.sq.ivf.init_centroids = as_ptr(keep)[0].value
+        rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
+                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
+        h = C.c_void_p()
+        st = BuildStats()
+        dp, _k1 = as_ptr(data)
+        rp, _k2 = as_ptr(rid)
+        check(lib().lb2_ivfhnswsq_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt),
+                                        C.c_int(_metric(distance_type)), C.byref(bp), rp, C.byref(h), C.byref(st)))
+        ix = cls(h, st)
+        ix._dt = dt
+        return ix
+
+    @classmethod
+    def from_parts(cls, centroids, bounds, part_ids, codes, row_ids=None, distance_type="l2", dtype=np.float32,
+                   bf16=False, graph=None):
+        """IvfSqIndex.from_parts plus `graph`: a dict as export()["graph"] returns (max_level, m, ef_construction,
+        levels, counts0, neighbors0, dists0, counts_up, neighbors_up, dists_up) over the rows in partition order."""
+        if graph is None:
+            raise ValueError("IvfHnswSqIndex.from_parts needs graph= (the dict export()['graph'] returns)")
+        ix = super().from_parts(centroids, bounds, part_ids, codes, row_ids, distance_type, dtype, bf16)
+        g = graph
+        arr = {k: np.ascontiguousarray(g[k], dtype=t) for k, t in (
+            ("levels", np.uint8), ("counts0", np.uint32), ("neighbors0", np.uint32), ("dists0", np.float32),
+            ("counts_up", np.uint32), ("neighbors_up", np.uint32), ("dists_up", np.float32))}
+        ptr = {k: C.c_void_p(v.ctypes.data) if v.size else None for k, v in arr.items()}
+        check(lib().lb2_index_load_hnsw_sq(ix._h, C.c_uint32(g["max_level"]), C.c_uint32(g["m"]),
+                                           C.c_uint32(g.get("ef_construction", 0)), ptr["levels"], ptr["counts0"],
+                                           ptr["neighbors0"], ptr["dists0"], ptr["counts_up"], ptr["neighbors_up"],
+                                           ptr["dists_up"]))
+        return ix
+
+    def export(self):
+        """IvfSqIndex.export plus "graph": the HNSW graphs in the device layout of include/lance_b200.h."""
+        out = super().export()
+        n = self.info()["num_rows"]
+        ml, m, efc, nu = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint64()
+        check(lib().lb2_index_hnsw_sq_info(self._h, C.byref(ml), C.byref(m), C.byref(efc), C.byref(nu)))
+        m, nu = m.value, nu.value
+        g = dict(max_level=ml.value, m=m, ef_construction=efc.value, levels=np.empty(n, np.uint8),
+                 counts0=np.empty(n, np.uint32), neighbors0=np.empty((n, 2 * m), np.uint32),
+                 dists0=np.empty((n, 2 * m), np.float32), counts_up=np.empty(nu, np.uint32),
+                 neighbors_up=np.empty((nu, m), np.uint32), dists_up=np.empty((nu, m), np.float32))
+        ptr = {k: C.c_void_p(v.ctypes.data) if isinstance(v, np.ndarray) and v.size else None for k, v in g.items()}
+        check(lib().lb2_index_export_hnsw_sq(self._h, ptr["levels"], ptr["counts0"], ptr["neighbors0"], ptr["dists0"],
+                                             ptr["counts_up"], ptr["neighbors_up"], ptr["dists_up"]))
+        out["graph"] = g
+        return out
+
+    def _search_hnsw(self, queries, k, nprobes, ef, probe=None, allow_bitmap=None, refine_factor=0, vectors=None,
+                     lower_bound=None, upper_bound=None):
+        """lb2_index_search_hnsw: search_ex (probe None) or search_probed (probe = ProbeParams) with this call's ef"""
+        from ._lib import SearchParams
+        npdt = {F32: np.float32, F16: np.float16, U8: np.uint8, BF16: np.uint16}[getattr(self, "_dt", F32)]
+        if not isinstance(queries, (DeviceArray, PinnedArray)):
+            queries = np.ascontiguousarray(queries, dtype=npdt)
+        if vectors is not None and not isinstance(vectors, (DeviceArray, PinnedArray)):
+            vectors = np.ascontiguousarray(vectors, dtype=npdt)
+        nq = queries.shape[0]
+        ids, dists = np.empty((nq, k), np.uint64), np.empty((nq, k), np.float32)
+        counts, nprobes_out = np.empty(nq, np.uint32), np.empty(nq, np.uint32)
+        qp, _k1 = as_ptr(queries)
+        vp, _k0 = as_ptr(vectors)
+        bp, _k4 = as_ptr(None if allow_bitmap is None else (allow_bitmap if isinstance(allow_bitmap, (DeviceArray, PinnedArray)) else np.ascontiguousarray(allow_bitmap, dtype=np.uint64)))
+        sp = SearchParams(k, nprobes, refine_factor, vp.value if vp is not None else None,
+                          0 if vectors is None else vectors.shape[0], bp.value if bp is not None else None,
+                          int(lower_bound is not None), int(upper_bound is not None),
+                          float(lower_bound or 0.0), float(upper_bound or 0.0))
+        check(lib().lb2_index_search_hnsw(self._h, qp, C.c_uint64(nq), C.byref(sp),
+                                          None if probe is None else C.byref(probe), C.c_uint32(int(ef)),
+                                          as_ptr(ids)[0], as_ptr(dists)[0], as_ptr(counts)[0],
+                                          None if probe is None else as_ptr(nprobes_out)[0]))
+        return ids, dists, counts, nprobes_out
+
+    def search(self, queries, k=10, nprobes=1, out=None, ef=None):
+        """IvfPqIndex.search; ef: the graph search's ef for this call (None: k + k / 2)."""
+        if ef is None:
+            return super().search(queries, k, nprobes, out)
+        ids, dists, _, _ = self._search_hnsw(queries, k, nprobes, ef)
+        if out is not None:
+            out[0][...], out[1][...] = ids, dists
+            return out
+        return ids, dists
+
+    def search_refine(self, vectors, queries, k=10, nprobes=1, refine_factor=1, out=None, ef=None):
+        """IvfPqIndex.search_refine; ef as in search (None: k' + k' / 2, k' = k * refine_factor)."""
+        if ef is None:
+            return super().search_refine(vectors, queries, k, nprobes, refine_factor, out)
+        ids, dists, _, _ = self._search_hnsw(queries, k, nprobes, ef, refine_factor=refine_factor, vectors=vectors)
+        return ids, dists
+
+    def search_ex(self, queries, k=10, nprobes=1, allow_bitmap=None, refine_factor=0, vectors=None, out=None,
+                  lower_bound=None, upper_bound=None, ef=None):
+        """IvfPqIndex.search_ex; ef as in search_refine."""
+        if ef is None:
+            return super().search_ex(queries, k, nprobes, allow_bitmap, refine_factor, vectors, out, lower_bound,
+                                     upper_bound)
+        ids, dists, _, _ = self._search_hnsw(queries, k, nprobes, ef, None, allow_bitmap, refine_factor, vectors,
+                                             lower_bound, upper_bound)
+        return ids, dists
+
+    def search_probed(self, queries, k, minimum_nprobes=1, maximum_nprobes=None, late_width=1, allow_bitmap=None,
+                      mask_ids=None, mask_max_len=None, refine_factor=0, vectors=None, lower_bound=None,
+                      upper_bound=None, ef=None):
+        """IvfPqIndex.search_probed; ef as in search_refine (mask_ids needs ef=None)."""
+        if ef is None:
+            return super().search_probed(queries, k, minimum_nprobes, maximum_nprobes, late_width, allow_bitmap,
+                                         mask_ids, mask_max_len, refine_factor, vectors, lower_bound, upper_bound)
+        if mask_ids is not None:
+            raise ValueError("search_probed with ef: mask_ids is not supported; pass ef=None")
+        from ._lib import ProbeParams
+        pp = ProbeParams(minimum_nprobes, maximum_nprobes or 0, late_width, int(mask_max_len is not None),
+                         int(mask_max_len or 0), None, 0)
+        return self._search_hnsw(queries, k, 0, ef, pp, allow_bitmap, refine_factor, vectors, lower_bound,
+                                 upper_bound)
 
 
 # ---- lance-index::vector::bq (RaBitQ) -------------------------------------------------------------

@@ -53,6 +53,11 @@ class SqBuildParams(C.Structure):
                 ("sample_rate", C.c_uint64), ("seed", C.c_uint64)]
 
 
+class HnswSqBuildParams(C.Structure):
+    """lb2_ivfhnswsq_build_params (include/lance_b200.h)."""
+    _fields_ = [("sq", SqBuildParams), ("max_level", C.c_uint32), ("m", C.c_uint32), ("ef_construction", C.c_uint32)]
+
+
 class RqBuildParams(C.Structure):
     """lb2_ivfrq_build_params (include/lance_b200.h)."""
     _fields_ = [("num_partitions", C.c_uint32), ("ivf", KMeansParams), ("num_bits", C.c_uint32),
@@ -80,7 +85,8 @@ EXPORTS = [
     "lb2_index_load_flat", "lb2_index_export_flat", "lb2_comm_unique_id", "lb2_comm_init", "lb2_comm_destroy",
     "lb2_comm_info", "lb2_index_search_sharded", "lb2_set_stream", "lb2_trim_memory", "lb2_index_search_async", "lb2_index_repartition", "lb2_index_update",
     "lb2_sq_train", "lb2_sq_encode", "lb2_ivfsq_build_params_default", "lb2_ivfsq_build", "lb2_index_create_sq",
-    "lb2_index_load_sq", "lb2_index_export_sq", "lb2_rq_rotation", "lb2_ivfrq_transform",
+    "lb2_index_load_sq", "lb2_index_export_sq", "lb2_ivfhnswsq_build_params_default", "lb2_ivfhnswsq_build",
+    "lb2_index_load_hnsw_sq", "lb2_index_hnsw_sq_info", "lb2_index_export_hnsw_sq", "lb2_index_search_hnsw", "lb2_rq_rotation", "lb2_ivfrq_transform",
     "lb2_ivfrq_build_params_default", "lb2_ivfrq_build", "lb2_index_create_rq", "lb2_index_load_rq",
     "lb2_index_export_rq", "lb2_index_search_probed", "lb2_flat_search", "lb2_index_search_combined",
 ]
@@ -106,7 +112,8 @@ def lib():
             if name not in ("lb2_version", "lb2_last_error", "lb2_device_count", "lb2_profile_dump",
                             "lb2_kmeans_params_default", "lb2_pq_params_default",
                             "lb2_ivfpq_build_params_default", "lb2_ivfflat_build_params_default",
-                            "lb2_ivfsq_build_params_default", "lb2_ivfrq_build_params_default"):
+                            "lb2_ivfsq_build_params_default", "lb2_ivfrq_build_params_default",
+                            "lb2_ivfhnswsq_build_params_default"):
                 getattr(L, name).restype = C.c_int
         L.lb2_sq_encode.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_int, C.c_double, C.c_double, C.c_void_p]
         L.lb2_index_create_sq.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int, C.c_int, C.c_double,

@@ -6,6 +6,7 @@
 #include "assign.cuh"
 #include "build.cuh"
 #include "comm.cuh"
+#include "hnsw.cuh"
 #include "index.cuh"
 #include "kmeans.cuh"
 #include "rq.cuh"
@@ -326,6 +327,13 @@ void lb2_ivfsq_build_params_default(lb2_ivfsq_build_params* p) {
   p->num_bits = 8;
   p->sample_rate = 256;
   p->seed = 0;
+}
+
+void lb2_ivfhnswsq_build_params_default(lb2_ivfhnswsq_build_params* p) {
+  lb2_ivfsq_build_params_default(&p->sq);
+  p->max_level = 7;  // HnswBuildParams::default (hnsw/builder.rs:63-72)
+  p->m = 20;
+  p->ef_construction = 150;
 }
 
 void lb2_ivfrq_build_params_default(lb2_ivfrq_build_params* p) {
@@ -681,6 +689,39 @@ lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   ev.record(4);
   sync_stream();
   fill_stats(stats, ev, ivf_loss, ivf_iters, pq_iters);
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_ivfhnswsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                               const lb2_ivfhnswsq_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                               lb2_build_stats* stats) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(data && params && out, "null argument");
+  LB2_REQUIRE(params->max_level >= 1 && params->max_level <= 64, "IVF_HNSW_SQ: max_level must be in 1 .. 64, got %u",
+              params->max_level);
+  LB2_REQUIRE(params->m >= 1 && params->m <= 1024, "IVF_HNSW_SQ: m must be in 1 .. 1024, got %u", params->m);
+  LB2_REQUIRE(params->ef_construction >= 1, "IVF_HNSW_SQ: ef_construction must be at least 1");
+  // 1. the IVF stage, bounds and codes of IVF_SQ with the same arguments
+  lb2_index* sq = nullptr;
+  const lb2_status st = lb2_ivfsq_build(data, n, d, dtype, metric, &params->sq, row_ids, &sq, stats);
+  if (st != LB2_OK) return st;  // its message is already the last error
+  std::unique_ptr<lb2_index> ix(sq);
+  // 2. HNSW::index_vectors per partition over its codes (v3 IvfIndexBuilder with an HNSW sub-index)
+  EventSet ev(2);
+  ev.record(0);
+  {
+    TagScope tg("hnsw_build");
+    ix->hnsw.reset(new HnswGraph());
+    HnswGraph& g = *ix->hnsw;
+    g.max_level = (int)params->max_level;
+    g.m = (int)params->m;
+    g.ef_construction = (int)params->ef_construction;
+    const float rf = (float)(ix->sq_upper - ix->sq_lower);
+    hnsw_build(g, ix->part_offsets.p, ix->K, ix->codes.p, (int)d, ix->metric, rf * rf, params->sq.seed);
+  }
+  ev.record(1);
+  if (stats) stats->ms_total += ev.ms(0, 1);  // the graph build is counted in the total only
   *out = ix.release();
   LB2_API_END
 }

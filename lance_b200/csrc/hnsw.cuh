@@ -1,0 +1,49 @@
+// hnsw.cuh -- the per-partition HNSW graphs of IVF_HNSW_SQ (lance-index/src/vector/hnsw/builder.rs) and their
+// device layout; internal interface of hnsw.cu
+#pragma once
+#include <stdint.h>
+
+#include "common.cuh"
+namespace lb2 {
+struct IvfSearch;
+
+// One graph per partition over the partition's storage order (node i = storage position off_p + i).
+//   level 0, dense over every row:  cnt0[n], nbr0[n][2m] (partition-local node ids), dst0[n][2m]
+//   levels 1.., compact:            a node with L levels owns rows up_base[row] .. up_base[row] + L - 2, one per
+//                                   level 1 .. L-1, each cntu, nbru[m], dstu[m]
+// Lists keep the reference's order of level_neighbors_ranked (graph/builder.rs:33-48); the distances are those of
+// the ranked list.  Node 0 of every partition has max_level levels and is the entry point (builder.rs:354-376).
+struct HnswGraph {
+  int max_level = 0, m = 0, ef_construction = 0;
+  uint64_t max_part = 0;  // rows of the largest partition (scratch sizing)
+  uint64_t n_up = 0;      // upper-level rows
+  DevBuf<uint8_t> nlev;
+  DevBuf<uint32_t> up_base, cnt0, nbr0, cntu, nbru;
+  DevBuf<float> dst0, dstu;
+};
+
+// The level thresholds of random_level (builder.rs:386-393): node i >= 1 of a partition gets 1 + #{l in 1 ..
+// max_level - 1 : u < thr[l]} levels, u the u32 draw of hnsw_level_draw; thr[l] = floor(2^32 / m^l), so P(level >= l)
+// is m^-l as in the reference's -ln(r) / ln(m).  thr[0] is unused.
+void hnsw_level_thresholds(int m, int max_level, uint64_t* thr);
+// the counter-based draw of node i of partition p (splitmix64 of seed + (p << 32 | i) * golden ratio, high half)
+inline uint32_t hnsw_level_draw(uint64_t seed, uint32_t p, uint32_t i) {
+  uint64_t x = seed + ((((uint64_t)p << 32) | i) * 0x9E3779B97F4A7C15ull);
+  x = (x ^ (x >> 30)) * 0xBF58476D1CE4E5B9ull;
+  x = (x ^ (x >> 27)) * 0x94D049BB133111EBull;
+  x ^= x >> 31;
+  return (uint32_t)(x >> 32);
+}
+
+// HNSW::index_vectors (builder.rs:742-775) of every partition, nodes inserted 1 .. n_p - 1 in ascending order;
+// codes [n][d] in partition order, part_offsets on the device.  Fills g (its parameters set by the caller).
+void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, int d, int metric, float r2,
+                uint64_t seed);
+// a graph from the caller's arrays in the layout above (host or device memory), checked against the partitions
+void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* levels, const uint32_t* counts0,
+               const uint32_t* nbr0, const float* dist0, const uint32_t* counts_up, const uint32_t* nbr_up,
+               const float* dist_up);
+// HNSW::search (builder.rs:678-739) as the scan of every probed partition; ef = 0: k' + k' / 2 (builder.rs:563-573)
+void hnsw_search(const IvfSearch& s, const HnswGraph& g, const uint8_t* codes, float r2, const uint8_t* qcodes,
+                 uint32_t ef);
+}  // namespace lb2

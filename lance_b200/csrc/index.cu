@@ -264,9 +264,11 @@ static void export_common(const lb2_index* index, void* centroids_out, uint64_t*
     LB2_CUDA(cudaMemcpyAsync(row_ids_out, index->row_ids.p, sizeof(uint64_t) * index->n, cudaMemcpyDefault, s));
 }
 
-// one implementation behind every lb2_index_search* (pr: the probe rule of lb2_index_search_probed)
+// one implementation behind every lb2_index_search* (pr: the probe rule of lb2_index_search_probed; ef: the graph
+// search's ef of lb2_index_search_hnsw, 0 for k' + k' / 2)
 static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq, const lb2_search_params& sp,
-                              uint64_t* row_ids_out, float* dists_out, uint32_t* counts_out, ProbeRule* pr = nullptr) {
+                              uint64_t* row_ids_out, float* dists_out, uint32_t* counts_out, ProbeRule* pr = nullptr,
+                              uint32_t ef = 0) {
   const uint32_t k = sp.k, nprobes = sp.nprobes;
   LB2_REQUIRE(index && k > 0 && (nprobes > 0 || pr), "bad argument");
   const bool refine = sp.refine_factor > 0 && sp.refine_vectors != nullptr;
@@ -315,7 +317,10 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
       qcodes.alloc(std::max<uint64_t>(1, nq * d));
       sq_encode_f32(qp, nq * d, index->sq_lower, index->sq_upper, qcodes.p);
       const float rf = (float)(index->sq_upper - index->sq_lower);  // inverse_scalar_dist (sq.rs:279-287)
-      ivfsq_search(s, index->codes.p, rf * rf, qcodes.p);
+      if (index->hnsw)  // IVF_HNSW_SQ: the same query codes, searched through each partition's graph
+        hnsw_search(s, *index->hnsw, index->codes.p, rf * rf, qcodes.p, ef);
+      else
+        ivfsq_search(s, index->codes.p, rf * rf, qcodes.p);
       break;
     }
     case IndexKind::PQ:
@@ -544,6 +549,7 @@ lb2_status lb2_index_load_sq(lb2_index* index, const uint32_t* part_ids, const u
                              const uint64_t* row_ids, uint64_t n) {
   LB2_API_BEGIN
   LB2_REQUIRE(index && index->kind == IndexKind::SQ, "not an IVF_SQ index");
+  LB2_REQUIRE(!index->hnsw, "lb2_index_load_sq: the index already has an HNSW graph over its rows");
   load_codes(index, part_ids, codes, row_ids, n, "index_load_sq");
   LB2_API_END
 }
@@ -588,6 +594,57 @@ lb2_status lb2_index_export_sq(const lb2_index* index, void* centroids_out, doub
     bounds_out[1] = index->sq_upper;
   }
   export_common(index, centroids_out, part_offsets_out, codes_out, row_ids_out);
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_index_load_hnsw_sq(lb2_index* index, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                                  const uint8_t* levels, const uint32_t* counts0, const uint32_t* neighbors0,
+                                  const float* dists0, const uint32_t* counts_up, const uint32_t* neighbors_up,
+                                  const float* dists_up) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->kind == IndexKind::SQ, "not an IVF_SQ index");
+  LB2_REQUIRE(max_level >= 1 && max_level <= 64 && m >= 1 && m <= 1024, "IVF_HNSW_SQ: max_level %u or m %u out of range",
+              max_level, m);
+  std::unique_ptr<HnswGraph> g(new HnswGraph());
+  g->max_level = (int)max_level;
+  g->m = (int)m;
+  g->ef_construction = (int)ef_construction;
+  hnsw_load(*g, index->part_offsets.p, index->K, levels, counts0, neighbors0, dists0, counts_up, neighbors_up, dists_up);
+  index->hnsw = std::move(g);
+  LB2_API_END
+}
+
+lb2_status lb2_index_hnsw_sq_info(const lb2_index* index, uint32_t* max_level, uint32_t* m, uint32_t* ef_construction,
+                                  uint64_t* num_upper_rows) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->hnsw, "not an IVF_HNSW_SQ index");
+  const HnswGraph& g = *index->hnsw;
+  if (max_level) *max_level = (uint32_t)g.max_level;
+  if (m) *m = (uint32_t)g.m;
+  if (ef_construction) *ef_construction = (uint32_t)g.ef_construction;
+  if (num_upper_rows) *num_upper_rows = g.n_up;
+  LB2_API_END
+}
+
+lb2_status lb2_index_export_hnsw_sq(const lb2_index* index, uint8_t* levels_out, uint32_t* counts0_out,
+                                    uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
+                                    uint32_t* neighbors_up_out, float* dists_up_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index && index->hnsw, "not an IVF_HNSW_SQ index");
+  const HnswGraph& g = *index->hnsw;
+  const size_t n = index->n, nu = g.n_up, m = (size_t)g.m;
+  cudaStream_t st = ctx().stream;
+  auto out = [&](void* dst, const void* src, size_t bytes) {
+    if (dst && bytes) LB2_CUDA(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDefault, st));
+  };
+  out(levels_out, g.nlev.p, n);
+  out(counts0_out, g.cnt0.p, 4 * n);
+  out(neighbors0_out, g.nbr0.p, 4 * n * 2 * m);
+  out(dists0_out, g.dst0.p, 4 * n * 2 * m);
+  out(counts_up_out, g.cntu.p, 4 * nu);
+  out(neighbors_up_out, g.nbru.p, 4 * nu * m);
+  out(dists_up_out, g.dstu.p, 4 * nu * m);
   sync_stream();
   LB2_API_END
 }
@@ -701,6 +758,25 @@ lb2_status lb2_index_search_probed(lb2_index* index, const void* queries, uint64
   ProbedSearch ps(sp, pp, nq, nprobes_out);
   index_search_impl(index, queries, nq, *sp, row_ids_out, dists_out, counts_out, &ps.pr);
   ps.np_out.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+lb2_status lb2_index_search_hnsw(lb2_index* index, const void* queries, uint64_t nq, const lb2_search_params* sp,
+                                 const lb2_probe_params* pp, uint32_t ef, uint64_t* row_ids_out, float* dists_out,
+                                 uint32_t* counts_out, uint32_t* nprobes_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(sp && index, "null argument");
+  LB2_REQUIRE(index->hnsw, "not an IVF_HNSW_SQ index");
+  LB2_REQUIRE(!nprobes_out || pp, "nprobes_out needs probe parameters");
+  if (pp) {
+    ProbedSearch ps(sp, pp, nq, nprobes_out);
+    index_search_impl(index, queries, nq, *sp, row_ids_out, dists_out, counts_out, &ps.pr, ef);
+    ps.np_out.commit();
+  } else {
+    LB2_REQUIRE(sp->refine_factor == 0 || sp->refine_vectors, "refine_factor > 0 needs refine_vectors");
+    index_search_impl(index, queries, nq, *sp, row_ids_out, dists_out, counts_out, nullptr, ef);
+  }
   sync_stream();
   LB2_API_END
 }
@@ -880,6 +956,7 @@ lb2_status lb2_index_repartition(const lb2_index* shard, lb2_index** owned_out) 
   LB2_API_BEGIN
   LB2_REQUIRE(shard && owned_out, "null argument");
   if (shard->kind == IndexKind::RQ) fail(LB2_UNSUPPORTED, "lb2_index_repartition: IVF_RQ indexes are not implemented");
+  if (shard->hnsw) fail(LB2_UNSUPPORTED, "lb2_index_repartition: IVF_HNSW_SQ indexes are not implemented");
   Comm* cm = current_comm();
   const int G = cm ? cm->nranks : 1, me = cm ? cm->rank : 0;
   const int K = shard->K;

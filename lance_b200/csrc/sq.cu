@@ -90,13 +90,6 @@ void sq_encode_f32(const float* x, uint64_t count, double lower, double upper, u
 // (f * (rf * rf)) / 255^2 with f = s as f32 (dot: 1 - s as f32); r2 = rf * rf comes from the host.
 // 8 lanes per row; VEC4: d % 16 == 0, 16-byte loads, otherwise 4-byte words.
 // ------------------------------------------------------------------------------------------------
-template <int METRIC>
-__device__ __forceinline__ uint32_t sq_word(uint32_t x, uint32_t q, uint32_t acc) {
-  if (METRIC == METRIC_DOT) return __dp4a(x, q, acc);
-  const uint32_t df = __vabsdiffu4(x, q);
-  return __dp4a(df, df, acc);
-}
-
 template <int METRIC, bool VEC4>
 __global__ void __maxnreg__(128)  // 256 threads; under __launch_bounds__(256) ptxas spills the selection's state
 ivfsq_scan_kernel(const uint8_t* __restrict__ qcodes, int d, float r2, const uint32_t* __restrict__ probe_ids, int np,
@@ -137,10 +130,7 @@ ivfsq_scan_kernel(const uint8_t* __restrict__ qcodes, int d, float r2, const uin
 #pragma unroll
       for (int o = 4; o >= 1; o >>= 1) acc += __shfl_xor_sync(gmask, acc, o, 8);
       if (l == 0) {
-        float f = __uint2float_rn(acc);
-        if (METRIC == METRIC_DOT) f = __fsub_rn(1.0f, f);
-        const float dist = __fdiv_rn(__fmul_rn(f, r2), 65025.0f);
-        s.ukey[j] = (uint32_t)total_order_key(dist) ^ 0x80000000u;
+        s.ukey[j] = (uint32_t)total_order_key(sq_distance<METRIC>(acc, r2)) ^ 0x80000000u;
       }
     }
   };

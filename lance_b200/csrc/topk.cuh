@@ -74,6 +74,33 @@ __device__ __forceinline__ void rheap_pop(uint32_t* hk, uint32_t* hp, uint32_t& 
   hp[pos] = ep;
   rheap_sift_up(hk, hp, pos);
 }
+// BinaryHeap::into_sorted_vec: the heap sort (swap the root with the last, then sift_down_range(0, end)); the
+// heap's arrays end ascending, and the order among equal keys is the reference's
+__device__ __forceinline__ void rheap_into_sorted(uint32_t* hk, uint32_t* hp, uint32_t len) {
+  for (uint32_t end = len; end > 1;) {
+    --end;
+    const uint32_t ek = hk[end], ep = hp[end];
+    hk[end] = hk[0];
+    hp[end] = hp[0];
+    uint32_t pos = 0, child = 1;
+    bool placed = false;
+    while (child + 1 < end) {
+      if (hk[child] <= hk[child + 1]) child += 1;
+      if (ek >= hk[child]) { placed = true; break; }
+      hk[pos] = hk[child];
+      hp[pos] = hp[child];
+      pos = child;
+      child = 2 * pos + 1;
+    }
+    if (!placed && child + 1 == end && ek < hk[child]) {
+      hk[pos] = hk[child];
+      hp[pos] = hp[child];
+      pos = child;
+    }
+    hk[pos] = ek;
+    hp[pos] = ep;
+  }
+}
 // FlatIndex::search's insertion rule for one row (flat/index.rs:116-126); keys are unsigned order keys
 __device__ __forceinline__ void rheap_offer(uint32_t* hk, uint32_t* hp, uint32_t& len, uint32_t k, uint32_t key,
                                             uint32_t pos) {
