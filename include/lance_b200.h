@@ -540,6 +540,48 @@ lb2_status lb2_index_search_hnsw(lb2_index* index, const void* queries, uint64_t
                                  const lb2_probe_params* pp, uint32_t ef, uint64_t* row_ids_out, float* dists_out,
                                  uint32_t* counts_out, uint32_t* nprobes_out);
 
+/* ---- IVF_HNSW_PQ: IVFIndex<HNSW, ProductQuantizer> (rust/lance/src/index/vector.rs:494-520) ---------------------
+ * An IVF_PQ index (same IVF stage, codebook and codes for the same arguments) with an HNSW graph per partition over
+ * the partition's PQ storage (lance-index/src/vector/pq/storage.rs:600-1037).  Levels, insertion order, tie handling,
+ * the graph layout, ef, the prefilter switch and the refusals are IVF_HNSW_SQ's (above); the distances are the PQ
+ * storage's, and cosine is L2 on the normalised rows throughout (the storage carries L2, pq/storage.rs:465-468):
+ *  - query to node (search): PQDistCalculator::distance (storage.rs:891-919) on the IVF_PQ scan's table of the
+ *    query (its residual to the probed centroid under L2 / cosine, the raw query under dot): 8-bit codes the
+ *    m-ascending f32 sum of table[m][code[m]], the distance of lb2_index_search on IVF_PQ; 4-bit codes the sum, in
+ *    byte order, of table[2i][lo] + table[2i+1][hi] (f32 entries, not the 4-bit scan's quantised table); dot
+ *    subtracts M - 1;
+ *  - node to node while node i is inserted: the same sum on the table of node i's decoded codes
+ *    (dist_calculator_from_id, storage.rs:675-749), entry point included; these are the distances in the lists;
+ *  - the heuristic (hnsw.rs:82): dist_between (storage.rs:751-841), the distance of the two decoded rows with the
+ *    column type's rule (16 f32 lanes; 32 lanes for f16 / bf16 dot).
+ * The graph crosses the ABI in IVF_HNSW_SQ's layout. */
+typedef struct {
+  lb2_ivfpq_build_params pq;
+  uint32_t max_level;       /* HnswBuildParams (hnsw/builder.rs:63-72): 7 */
+  uint32_t m;               /* 20; level 0 keeps up to 2m neighbours, the others m */
+  uint32_t ef_construction; /* 150 */
+} lb2_ivfhnswpq_build_params;
+void lb2_ivfhnswpq_build_params_default(lb2_ivfhnswpq_build_params* p);
+/* IvfIndexBuilder<HNSW, ProductQuantizer>::build (vector.rs:507-520): lb2_ivfpq_build, then every partition's graph on
+ * the device (one warp per partition, the largest partitions first); the level draws use params->pq.seed.  The graph
+ * stage is counted in stats->ms_total only.  A communicator of more than one rank is LB2_UNSUPPORTED. */
+lb2_status lb2_ivfhnswpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                               const lb2_ivfhnswpq_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                               lb2_build_stats* stats);
+/* attach a graph (host or device arrays in the IVF_HNSW_SQ layout) to an IVF_PQ index made by lb2_index_create +
+ * lb2_index_load; the checks of lb2_index_load_hnsw_sq.  `dtype` of lb2_index_create picks the heuristic's rule. */
+lb2_status lb2_index_load_hnsw_pq(lb2_index* index, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                                  const uint8_t* levels, const uint32_t* counts0, const uint32_t* neighbors0,
+                                  const float* dists0, const uint32_t* counts_up, const uint32_t* neighbors_up,
+                                  const float* dists_up);
+/* as lb2_index_hnsw_sq_info / lb2_index_export_hnsw_sq for an IVF_HNSW_PQ index */
+lb2_status lb2_index_hnsw_pq_info(const lb2_index* index, uint32_t* max_level, uint32_t* m, uint32_t* ef_construction,
+                                  uint64_t* num_upper_rows);
+lb2_status lb2_index_export_hnsw_pq(const lb2_index* index, uint8_t* levels_out, uint32_t* counts0_out,
+                                    uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
+                                    uint32_t* neighbors_up_out, float* dists_up_out);
+/* lb2_index_search_hnsw takes an IVF_HNSW_SQ or an IVF_HNSW_PQ index. */
+
 /* ---- IVF_RQ: IVFIndex<FlatIndex, RabitQuantizer> (lance-index/src/vector/bq/) ------------------------------------
  * create_index(.., "IVF_RQ") builds an IvfIndexBuilder<FlatIndex, RabitQuantizer> (rust/lance/src/index/vector.rs:
  * 452-470).  code_dim = d * num_bits; the rotation R is code_dim x code_dim, of which the first d columns are used.

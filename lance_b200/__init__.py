@@ -14,7 +14,7 @@ import numpy as np
 from ._lib import (BF16, COSINE, DOT, F16, F32, L2, METRICS, U8, BuildParams, BuildStats, FlatBuildParams,
                    DeviceArray, KMeansParams as _CKMeansParams, LanceB200Error, PinnedArray,
                    PQParams as _CPQParams, RqBuildParams as _CRqBuildParams, SqBuildParams as _CSqBuildParams,
-                   HnswSqBuildParams as _CHnswSqBuildParams, as_ptr,
+                   HnswSqBuildParams as _CHnswSqBuildParams, HnswPqBuildParams as _CHnswPqBuildParams, as_ptr,
                    check, device_count, lib)
 
 __all__ = ["device_count", "DeviceArray", "PinnedArray", "LanceB200Error", "train_kmeans",
@@ -22,7 +22,7 @@ __all__ = ["device_count", "DeviceArray", "PinnedArray", "LanceB200Error", "trai
            "l2_distance_batch", "dot_distance_batch", "cosine_distance_batch", "PQBuildParams", "ProductQuantizer",
            "build_distance_table_l2", "compute_pq_distance", "flat_topk", "flat_search", "IvfPqIndex",
            "IvfBuildParams", "IvfFlatIndex", "SQBuildParams", "ScalarQuantizer", "IvfSqIndex", "HnswBuildParams",
-           "IvfHnswSqIndex", "RQBuildParams",
+           "IvfHnswSqIndex", "IvfHnswPqIndex", "RQBuildParams",
            "RabitQuantizer", "IvfRqIndex", "launch_count", "profile"]
 
 
@@ -63,6 +63,14 @@ def _typed(a, bf16=False):
 
 def _model_np(dt):
     return {F32: np.float32, F16: np.float16, BF16: np.uint16, U8: np.float32}[dt]
+
+
+def _model_arr(a, dt):
+    """a model array in the model type of `dt`; f32 arrays of a bf16 model (as exports return them) keep their bits"""
+    a = np.asarray(a)
+    if dt == BF16 and a.dtype == np.float32:
+        return np.ascontiguousarray((np.ascontiguousarray(a).view(np.uint32) >> 16).astype(np.uint16))
+    return np.ascontiguousarray(a, dtype=_model_np(dt))
 
 
 def set_device(i):
@@ -444,6 +452,25 @@ class IvfBuildParams:
         self.pq_sample_rate, self.seed, self.centroids, self.codebook = pq_sample_rate, seed, centroids, codebook
 
 
+def _fill_build_params(bp, params):
+    """lb2_ivfpq_build_params from IvfBuildParams; returns the arrays bp points into (keep them alive)"""
+    bp.num_partitions = params.num_partitions
+    bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed = params.max_iters, params.sample_rate, params.seed
+    bp.pq.num_sub_vectors, bp.pq.num_bits = params.num_sub_vectors, params.num_bits
+    bp.pq.max_iters, bp.pq.sample_rate, bp.pq.seed = params.pq_max_iters, params.pq_sample_rate, params.seed + 1000
+    bp.seed = params.seed
+    keep = []
+    if params.centroids is not None:
+        c = _f32(params.centroids)
+        keep.append(c)
+        bp.ivf.init_centroids = as_ptr(c)[0].value
+    if params.codebook is not None:
+        c = _f32(params.codebook)
+        keep.append(c)
+        bp.pq.codebook = as_ptr(c)[0].value
+    return keep
+
+
 class IvfPqIndex:
     """Device-resident IVFIndex<FlatIndex, ProductQuantizer> (ivf/v2.rs:104)."""
 
@@ -460,20 +487,7 @@ class IvfPqIndex:
         n, d = data.shape
         bp = BuildParams()
         lib().lb2_ivfpq_build_params_default(C.byref(bp))
-        bp.num_partitions = params.num_partitions
-        bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed = params.max_iters, params.sample_rate, params.seed
-        bp.pq.num_sub_vectors, bp.pq.num_bits = params.num_sub_vectors, params.num_bits
-        bp.pq.max_iters, bp.pq.sample_rate, bp.pq.seed = params.pq_max_iters, params.pq_sample_rate, params.seed + 1000
-        bp.seed = params.seed
-        keep = []
-        if params.centroids is not None:
-            c = _f32(params.centroids)
-            keep.append(c)
-            bp.ivf.init_centroids = as_ptr(c)[0].value
-        if params.codebook is not None:
-            c = _f32(params.codebook)
-            keep.append(c)
-            bp.pq.codebook = as_ptr(c)[0].value
+        keep = _fill_build_params(bp, params)
         rid = None if row_ids is None else (row_ids if isinstance(row_ids, DeviceArray)
                                             else np.ascontiguousarray(row_ids, dtype=np.uint64))
         h = C.c_void_p()
@@ -979,74 +993,42 @@ class HnswBuildParams:
         self.max_level, self.m, self.ef_construction = max_level, m, ef_construction
 
 
-class IvfHnswSqIndex(IvfSqIndex):
-    """Device-resident IVFIndex<HNSW, ScalarQuantizer> (IVF_HNSW_SQ): IVF_SQ's partitions, bounds and codes with an
-    HNSW graph per partition over the codes (lance-index/src/vector/hnsw/builder.rs).  search, search_refine,
-    search_ex and search_probed take ef= (lb2_index_search_hnsw); the other search methods use k' + k' / 2."""
+class _HnswGraphs:
+    """The graph half of IvfHnswSqIndex and IvfHnswPqIndex: attach, export and search with ef=.  search,
+    search_refine, search_ex and search_probed take ef= (lb2_index_search_hnsw); the other search methods use
+    k' + k' / 2."""
+    _KIND = None   # "sq" or "pq": the suffix of the kind's C entry points
 
     @classmethod
-    def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
-              centroids=None, row_ids=None, bf16=False, sq_params=None, hnsw_params=None):
-        """create_index(.., "IVF_HNSW_SQ"); the IVF stage, bounds and codes equal IvfSqIndex.build's with the same
-        arguments.  The graphs' level draws use `seed`."""
-        sq_params = sq_params or SQBuildParams()
-        hnsw_params = hnsw_params or HnswBuildParams()
-        data, dt = _typed(data, bf16)
-        n, d = data.shape
-        bp = _CHnswSqBuildParams()
-        lib().lb2_ivfhnswsq_build_params_default(C.byref(bp))
-        bp.sq.num_partitions = num_partitions
-        bp.sq.ivf.max_iters, bp.sq.ivf.sample_rate, bp.sq.ivf.seed, bp.sq.seed = max_iters, sample_rate, seed, seed
-        bp.sq.num_bits, bp.sq.sample_rate = sq_params.num_bits, sq_params.sample_rate
-        bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
-        keep = None
-        if centroids is not None:
-            keep = _f32(centroids)
-            bp.sq.ivf.init_centroids = as_ptr(keep)[0].value
-        rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
-                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
-        h = C.c_void_p()
-        st = BuildStats()
-        dp, _k1 = as_ptr(data)
-        rp, _k2 = as_ptr(rid)
-        check(lib().lb2_ivfhnswsq_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt),
-                                        C.c_int(_metric(distance_type)), C.byref(bp), rp, C.byref(h), C.byref(st)))
-        ix = cls(h, st)
-        ix._dt = dt
-        return ix
-
-    @classmethod
-    def from_parts(cls, centroids, bounds, part_ids, codes, row_ids=None, distance_type="l2", dtype=np.float32,
-                   bf16=False, graph=None):
-        """IvfSqIndex.from_parts plus `graph`: a dict as export()["graph"] returns (max_level, m, ef_construction,
-        levels, counts0, neighbors0, dists0, counts_up, neighbors_up, dists_up) over the rows in partition order."""
+    def _need_graph(cls, graph):
         if graph is None:
-            raise ValueError("IvfHnswSqIndex.from_parts needs graph= (the dict export()['graph'] returns)")
-        ix = super().from_parts(centroids, bounds, part_ids, codes, row_ids, distance_type, dtype, bf16)
+            raise ValueError(f"{cls.__name__}.from_parts needs graph= (the dict export()['graph'] returns)")
+
+    def _attach_graph(self, graph):
+        """lb2_index_load_hnsw_sq / _pq of a dict as export()["graph"] returns"""
         g = graph
         arr = {k: np.ascontiguousarray(g[k], dtype=t) for k, t in (
             ("levels", np.uint8), ("counts0", np.uint32), ("neighbors0", np.uint32), ("dists0", np.float32),
             ("counts_up", np.uint32), ("neighbors_up", np.uint32), ("dists_up", np.float32))}
         ptr = {k: C.c_void_p(v.ctypes.data) if v.size else None for k, v in arr.items()}
-        check(lib().lb2_index_load_hnsw_sq(ix._h, C.c_uint32(g["max_level"]), C.c_uint32(g["m"]),
-                                           C.c_uint32(g.get("ef_construction", 0)), ptr["levels"], ptr["counts0"],
-                                           ptr["neighbors0"], ptr["dists0"], ptr["counts_up"], ptr["neighbors_up"],
-                                           ptr["dists_up"]))
-        return ix
+        check(getattr(lib(), f"lb2_index_load_hnsw_{self._KIND}")(
+            self._h, C.c_uint32(g["max_level"]), C.c_uint32(g["m"]), C.c_uint32(g.get("ef_construction", 0)),
+            ptr["levels"], ptr["counts0"], ptr["neighbors0"], ptr["dists0"], ptr["counts_up"], ptr["neighbors_up"],
+            ptr["dists_up"]))
 
-    def export(self):
-        """IvfSqIndex.export plus "graph": the HNSW graphs in the device layout of include/lance_b200.h."""
-        out = super().export()
+    def export(self, *args):
+        """the parent kind's export plus "graph": the HNSW graphs in the device layout of include/lance_b200.h."""
+        out = super().export(*args)
         n = self.info()["num_rows"]
         ml, m, efc, nu = C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint64()
-        check(lib().lb2_index_hnsw_sq_info(self._h, C.byref(ml), C.byref(m), C.byref(efc), C.byref(nu)))
+        check(getattr(lib(), f"lb2_index_hnsw_{self._KIND}_info")(self._h, C.byref(ml), C.byref(m), C.byref(efc), C.byref(nu)))
         m, nu = m.value, nu.value
         g = dict(max_level=ml.value, m=m, ef_construction=efc.value, levels=np.empty(n, np.uint8),
                  counts0=np.empty(n, np.uint32), neighbors0=np.empty((n, 2 * m), np.uint32),
                  dists0=np.empty((n, 2 * m), np.float32), counts_up=np.empty(nu, np.uint32),
                  neighbors_up=np.empty((nu, m), np.uint32), dists_up=np.empty((nu, m), np.float32))
         ptr = {k: C.c_void_p(v.ctypes.data) if isinstance(v, np.ndarray) and v.size else None for k, v in g.items()}
-        check(lib().lb2_index_export_hnsw_sq(self._h, ptr["levels"], ptr["counts0"], ptr["neighbors0"], ptr["dists0"],
+        check(getattr(lib(), f"lb2_index_export_hnsw_{self._KIND}")(self._h, ptr["levels"], ptr["counts0"], ptr["neighbors0"], ptr["dists0"],
                                              ptr["counts_up"], ptr["neighbors_up"], ptr["dists_up"]))
         out["graph"] = g
         return out
@@ -1117,6 +1099,115 @@ class IvfHnswSqIndex(IvfSqIndex):
                          int(mask_max_len or 0), None, 0)
         return self._search_hnsw(queries, k, 0, ef, pp, allow_bitmap, refine_factor, vectors, lower_bound,
                                  upper_bound)
+
+
+
+class IvfHnswSqIndex(_HnswGraphs, IvfSqIndex):
+    """Device-resident IVFIndex<HNSW, ScalarQuantizer> (IVF_HNSW_SQ): IVF_SQ's partitions, bounds and codes with an
+    HNSW graph per partition over the codes (lance-index/src/vector/hnsw/builder.rs).  search, search_refine,
+    search_ex and search_probed take ef= (lb2_index_search_hnsw); the other search methods use k' + k' / 2."""
+
+    @classmethod
+    def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
+              centroids=None, row_ids=None, bf16=False, sq_params=None, hnsw_params=None):
+        """create_index(.., "IVF_HNSW_SQ"); the IVF stage, bounds and codes equal IvfSqIndex.build's with the same
+        arguments.  The graphs' level draws use `seed`."""
+        sq_params = sq_params or SQBuildParams()
+        hnsw_params = hnsw_params or HnswBuildParams()
+        data, dt = _typed(data, bf16)
+        n, d = data.shape
+        bp = _CHnswSqBuildParams()
+        lib().lb2_ivfhnswsq_build_params_default(C.byref(bp))
+        bp.sq.num_partitions = num_partitions
+        bp.sq.ivf.max_iters, bp.sq.ivf.sample_rate, bp.sq.ivf.seed, bp.sq.seed = max_iters, sample_rate, seed, seed
+        bp.sq.num_bits, bp.sq.sample_rate = sq_params.num_bits, sq_params.sample_rate
+        bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
+        keep = None
+        if centroids is not None:
+            keep = _f32(centroids)
+            bp.sq.ivf.init_centroids = as_ptr(keep)[0].value
+        rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
+                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
+        h = C.c_void_p()
+        st = BuildStats()
+        dp, _k1 = as_ptr(data)
+        rp, _k2 = as_ptr(rid)
+        check(lib().lb2_ivfhnswsq_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt),
+                                        C.c_int(_metric(distance_type)), C.byref(bp), rp, C.byref(h), C.byref(st)))
+        ix = cls(h, st)
+        ix._dt = dt
+        return ix
+
+    _KIND = "sq"
+
+    @classmethod
+    def from_parts(cls, centroids, bounds, part_ids, codes, row_ids=None, distance_type="l2", dtype=np.float32,
+                   bf16=False, graph=None):
+        """IvfSqIndex.from_parts plus `graph`: a dict as export()["graph"] returns (max_level, m, ef_construction,
+        levels, counts0, neighbors0, dists0, counts_up, neighbors_up, dists_up) over the rows in partition order."""
+        cls._need_graph(graph)
+        ix = super().from_parts(centroids, bounds, part_ids, codes, row_ids, distance_type, dtype, bf16)
+        ix._attach_graph(graph)
+        return ix
+
+
+class IvfHnswPqIndex(_HnswGraphs, IvfPqIndex):
+    """Device-resident IVFIndex<HNSW, ProductQuantizer> (IVF_HNSW_PQ): IVF_PQ's partitions, codebook and codes with an
+    HNSW graph per partition over the PQ storage (lance-index/src/vector/pq/storage.rs:600-1037).  A query scores a
+    node from the IVF_PQ scan's table; a node being inserted scores others from the table of its own decoded codes,
+    and the heuristic compares the decoded rows (include/lance_b200.h).  search, search_refine, search_ex and
+    search_probed take ef=; the other search methods use k' + k' / 2."""
+    _KIND = "pq"
+
+    @classmethod
+    def build(cls, data, distance_type="l2", params=None, hnsw_params=HnswBuildParams(), row_ids=None, bf16=False):
+        """create_index(.., "IVF_HNSW_PQ"); the IVF stage, codebook and codes equal IvfPqIndex.build's with the same
+        arguments.  The graphs' level draws use params.seed."""
+        params = params or IvfBuildParams()
+        data, dt = _typed(data, bf16)
+        n, d = data.shape
+        bp = _CHnswPqBuildParams()
+        lib().lb2_ivfhnswpq_build_params_default(C.byref(bp))
+        keep = _fill_build_params(bp.pq, params)
+        bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
+        rid = None if row_ids is None else (row_ids if isinstance(row_ids, DeviceArray)
+                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
+        h = C.c_void_p()
+        st = BuildStats()
+        dp, _k1 = as_ptr(data)
+        rp, _k2 = as_ptr(rid)
+        check(lib().lb2_ivfhnswpq_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt),
+                                        C.c_int(_metric(distance_type)), C.byref(bp), rp, C.byref(h), C.byref(st)))
+        del keep
+        ix = cls(h, st)
+        ix._dt = dt
+        return ix
+
+    @classmethod
+    def from_parts(cls, centroids, codebook, part_ids, codes, row_ids=None, distance_type="l2", num_bits=8,
+                   dtype=np.float32, bf16=False, graph=None):
+        """IvfPqIndex.from_parts plus `graph` (as export()["graph"] returns).  dtype / bf16: the column's element type
+        (bf16=True: uint16 bit patterns), which picks the heuristic's distance rule and the type of the queries."""
+        cls._need_graph(graph)
+        dt = BF16 if bf16 else _DTYPES[np.dtype(dtype)]
+        centroids, codebook = _model_arr(centroids, dt), _model_arr(codebook, dt)
+        k, d = centroids.shape
+        M = codebook.shape[0]
+        h = C.c_void_p()
+        check(lib().lb2_index_create(C.c_void_p(centroids.ctypes.data), C.c_uint32(k), C.c_uint32(d),
+                                     C.c_int(dt), C.c_int(_metric(distance_type)),
+                                     C.c_void_p(codebook.ctypes.data), C.c_uint32(M), C.c_uint32(num_bits),
+                                     C.byref(h)))
+        ix = cls(h)
+        ix._dt = dt
+        part_ids = np.ascontiguousarray(part_ids, dtype=np.uint32)
+        codes = np.ascontiguousarray(codes, dtype=np.uint8)
+        rid = None if row_ids is None else np.ascontiguousarray(row_ids, dtype=np.uint64)
+        rp, _k = as_ptr(rid)
+        check(lib().lb2_index_load(h, C.c_void_p(part_ids.ctypes.data), C.c_void_p(codes.ctypes.data), rp,
+                                   C.c_uint64(part_ids.size)))
+        ix._attach_graph(graph)
+        return ix
 
 
 # ---- lance-index::vector::bq (RaBitQ) -------------------------------------------------------------

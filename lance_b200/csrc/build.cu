@@ -336,6 +336,13 @@ void lb2_ivfhnswsq_build_params_default(lb2_ivfhnswsq_build_params* p) {
   p->ef_construction = 150;
 }
 
+void lb2_ivfhnswpq_build_params_default(lb2_ivfhnswpq_build_params* p) {
+  lb2_ivfpq_build_params_default(&p->pq);
+  p->max_level = 7;  // HnswBuildParams::default (hnsw/builder.rs:63-72)
+  p->m = 20;
+  p->ef_construction = 150;
+}
+
 void lb2_ivfrq_build_params_default(lb2_ivfrq_build_params* p) {
   p->num_partitions = 256;
   lb2_kmeans_params_default(&p->ivf);
@@ -693,35 +700,76 @@ lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   LB2_API_END
 }
 
-lb2_status lb2_ivfhnswsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
-                               const lb2_ivfhnswsq_build_params* params, const uint64_t* row_ids, lb2_index** out,
-                               lb2_build_stats* stats) {
-  LB2_API_BEGIN
-  LB2_REQUIRE(data && params && out, "null argument");
-  LB2_REQUIRE(params->max_level >= 1 && params->max_level <= 64, "IVF_HNSW_SQ: max_level must be in 1 .. 64, got %u",
-              params->max_level);
-  LB2_REQUIRE(params->m >= 1 && params->m <= 1024, "IVF_HNSW_SQ: m must be in 1 .. 1024, got %u", params->m);
-  LB2_REQUIRE(params->ef_construction >= 1, "IVF_HNSW_SQ: ef_construction must be at least 1");
-  // 1. the IVF stage, bounds and codes of IVF_SQ with the same arguments
-  lb2_index* sq = nullptr;
-  const lb2_status st = lb2_ivfsq_build(data, n, d, dtype, metric, &params->sq, row_ids, &sq, stats);
-  if (st != LB2_OK) return st;  // its message is already the last error
-  std::unique_ptr<lb2_index> ix(sq);
-  // 2. HNSW::index_vectors per partition over its codes (v3 IvfIndexBuilder with an HNSW sub-index)
+}  // extern "C"
+
+// the graph parameters of an HNSW build (hnsw/builder.rs:63-72)
+static void check_hnsw_params(const char* kind, uint32_t max_level, uint32_t m, uint32_t ef_construction) {
+  LB2_REQUIRE(max_level >= 1 && max_level <= 64, "%s: max_level must be in 1 .. 64, got %u", kind, max_level);
+  LB2_REQUIRE(m >= 1 && m <= 1024, "%s: m must be in 1 .. 1024, got %u", kind, m);
+  LB2_REQUIRE(ef_construction >= 1, "%s: ef_construction must be at least 1", kind);
+}
+
+// step 2 of an IVF_HNSW_* build: the graphs of `ix`, counted in stats->ms_total only
+template <class F>
+static void attach_graphs(lb2_index* ix, const char* kind, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                          lb2_build_stats* stats, F&& build) {
   EventSet ev(2);
   ev.record(0);
   {
     TagScope tg("hnsw_build");
     ix->hnsw.reset(new HnswGraph());
     HnswGraph& g = *ix->hnsw;
-    g.max_level = (int)params->max_level;
-    g.m = (int)params->m;
-    g.ef_construction = (int)params->ef_construction;
-    const float rf = (float)(ix->sq_upper - ix->sq_lower);
-    hnsw_build(g, ix->part_offsets.p, ix->K, ix->codes.p, (int)d, ix->metric, rf * rf, params->sq.seed);
+    g.kind = kind;
+    g.max_level = (int)max_level;
+    g.m = (int)m;
+    g.ef_construction = (int)ef_construction;
+    build(g);
   }
   ev.record(1);
   if (stats) stats->ms_total += ev.ms(0, 1);  // the graph build is counted in the total only
+}
+
+extern "C" {
+
+lb2_status lb2_ivfhnswsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                               const lb2_ivfhnswsq_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                               lb2_build_stats* stats) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(data && params && out, "null argument");
+  check_hnsw_params("IVF_HNSW_SQ", params->max_level, params->m, params->ef_construction);
+  // 1. the IVF stage, bounds and codes of IVF_SQ with the same arguments
+  lb2_index* sq = nullptr;
+  const lb2_status st = lb2_ivfsq_build(data, n, d, dtype, metric, &params->sq, row_ids, &sq, stats);
+  if (st != LB2_OK) return st;  // its message is already the last error
+  std::unique_ptr<lb2_index> ix(sq);
+  // 2. HNSW::index_vectors per partition over its codes (v3 IvfIndexBuilder with an HNSW sub-index)
+  attach_graphs(ix.get(), "IVF_HNSW_SQ", params->max_level, params->m, params->ef_construction, stats, [&](HnswGraph& g) {
+    const float rf = (float)(ix->sq_upper - ix->sq_lower);
+    hnsw_build(g, ix->part_offsets.p, ix->K, ix->codes.p, (int)d, ix->metric, rf * rf, params->sq.seed);
+  });
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_ivfhnswpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                               const lb2_ivfhnswpq_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                               lb2_build_stats* stats) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(data && params && out, "null argument");
+  check_hnsw_params("IVF_HNSW_PQ", params->max_level, params->m, params->ef_construction);
+  if (comm_nranks() > 1) fail(LB2_UNSUPPORTED, "IVF_HNSW_PQ: a build over more than one rank is not implemented");
+  // 1. the IVF stage, codebook and codes of IVF_PQ with the same arguments
+  lb2_index* pq = nullptr;
+  const lb2_status st = lb2_ivfpq_build(data, n, d, dtype, metric, &params->pq, row_ids, &pq, stats);
+  if (st != LB2_OK) return st;  // its message is already the last error
+  std::unique_ptr<lb2_index> ix(pq);
+  ix->slab_off.release();  // the skewed code copy serves only the IVF_PQ scan
+  ix->codes_skew.release();
+  // 2. HNSW::index_vectors per partition over its PQ storage (IvfIndexBuilder<HNSW, ProductQuantizer>)
+  attach_graphs(ix.get(), "IVF_HNSW_PQ", params->max_level, params->m, params->ef_construction, stats, [&](HnswGraph& g) {
+    hnsw_build_pq(g, ix->part_offsets.p, ix->K, ix->codes.p, ix->codebook.p, (int)d, ix->M, ix->nbits, ix->metric,
+                  dtype, params->pq.seed);
+  });
   *out = ix.release();
   LB2_API_END
 }

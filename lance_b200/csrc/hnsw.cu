@@ -1,19 +1,24 @@
-// hnsw.cu -- IVF_HNSW_SQ: an HNSW graph per partition over the partition's SQ codes, built and searched on the device
-// (lance-index/src/vector/hnsw/builder.rs, graph.rs, hnsw.rs, graph/builder.rs).
+// hnsw.cu -- IVF_HNSW_SQ and IVF_HNSW_PQ: an HNSW graph per partition over the partition's SQ or PQ codes, built and
+// searched on the device (lance-index/src/vector/hnsw/builder.rs, graph.rs, hnsw.rs, graph/builder.rs).
 //
 // Replaces  HNSW::index_vectors / HnswBuilder::insert      hnsw/builder.rs:386-507,742-775
 //           select_neighbors_heuristic                   hnsw.rs:60-88
 //           beam_search / greedy_search                  graph.rs:275-409
 //           HNSW::search / search_inner / flat_search    hnsw/builder.rs:164-280,678-739
 //
-// Every distance is the SQ row rule of sq.cuh (query-to-row and row-to-row alike, sq/storage.rs:387-444,
-// storage.rs:102-105): an integer sum times one constant, so the build is deterministic and bit-exact.
+// The engine is generic over a distance policy (SqDist, PqDist below), as the reference is over VectorStore: `key`
+// is the distance of the query (or of the inserting node) to a node, `between` the heuristic's dist_between.
+//  * SQ: both are the SQ row rule of sq.cuh (sq/storage.rs:387-444, storage.rs:102-105): an integer sum times one
+//    constant, so the build is deterministic and bit-exact.
+//  * PQ (pq/storage.rs:675-919): `key` sums a lookup table over the node's codes; the table is the residual query's
+//    at search time and, while a node is inserted, the table of the node's own decoded codes (dist_calculator_from_id);
+//    `between` is the full-width distance of the two decoded rows (dist_between).
 //
-// One warp owns one partition (build) or one (query, partition) slot (search).  Its heaps and visited bitset live in
-// a per-warp global scratch sized by the largest partition, so no partition is refused for its size.  Lane 0 runs
-// the reference's serial heap and list updates in the reference's order; the 32 lanes compute the distances of a
-// neighbour list or of a candidate's accepted neighbours, one row per lane.  Control decisions reach the other lanes through shared memory after a
-// __syncwarp.
+// One warp owns one partition (build) or one (query, partition) slot (search).  Its heaps, visited bitset and (PQ)
+// table live in a per-warp global scratch sized by the largest partition, so no partition is refused for its size.
+// Lane 0 runs the reference's serial heap and list updates in the reference's order; the 32 lanes compute the
+// distances of a neighbour list or of a candidate's accepted neighbours, one row per lane, and build a PQ table
+// together.  Control decisions reach the other lanes through shared memory after a __syncwarp.
 #include <algorithm>
 #include <vector>
 
@@ -21,7 +26,9 @@
 #include "exact.cuh"
 #include "hnsw.cuh"
 #include "ivf_search.cuh"
+#include "pq_lut.cuh"
 #include "probe.cuh"
+#include "row_distance.cuh"
 #include "sq.cuh"
 #include "topk.cuh"
 
@@ -54,26 +61,25 @@ __device__ __forceinline__ ListRef list_of(const GraphDev& g, uint64_t row, int 
   return {g.cntu + r, g.nbru + r * g.m, g.dstu + r * g.m};
 }
 
-// one partition as a warp sees it
-struct Part {
-  const uint8_t* codes;  // the partition's first code row
-  uint64_t off;          // its first storage position
-  uint32_t n;
-  int d;
-  float r2;
-};
-
-// per-warp scratch (u32 words): vis[words(nmax)], candidate heap ck / cid [nmax + 1], result heap rk / rid [E + 1],
-// batch bid / bk [B], list lid / lk / ord [LB], accepted aid / ak [B]
+// per-warp scratch (u32 words): PQ table tab[TW] and query / decoded row qv[QW] (none for SQ), vis[words(nmax)],
+// candidate heap ck / cid [nmax + 1], result heap rk / rid [E + 1], batch bid / bk [B], list lid / lk / ord [LB],
+// accepted aid / ak [B].  With a table the warp's share is a multiple of 4 words, so tab and qv stay 16-byte aligned.
 struct Scratch {
+  float *tab, *qv;
   uint32_t *vis, *ck, *cid, *rk, *rid, *bid, *bk, *lid, *lk, *ord, *aid, *ak;
 };
-__host__ __device__ inline size_t scratch_words(uint64_t nmax, uint32_t E, uint32_t B, uint32_t LB) {
-  return (nmax + 31) / 32 + 2 * (nmax + 1) + 2 * ((size_t)E + 1) + 4 * (size_t)B + 3 * (size_t)LB;
+__host__ __device__ inline size_t scratch_words(uint64_t nmax, uint32_t E, uint32_t B, uint32_t LB, uint32_t TW = 0,
+                                                uint32_t QW = 0) {
+  const size_t w = (size_t)TW + QW + (nmax + 31) / 32 + 2 * (nmax + 1) + 2 * ((size_t)E + 1) + 4 * (size_t)B +
+                   3 * (size_t)LB;
+  return TW ? (w + 3) & ~(size_t)3 : w;
 }
-__device__ inline Scratch scratch_at(uint32_t* base, uint64_t nmax, uint32_t E, uint32_t B, uint32_t LB) {
+__device__ inline Scratch scratch_at(uint32_t* base, uint64_t nmax, uint32_t E, uint32_t B, uint32_t LB,
+                                     uint32_t TW = 0, uint32_t QW = 0) {
   Scratch s;
-  s.vis = base;
+  s.tab = reinterpret_cast<float*>(base);
+  s.qv = s.tab + TW;
+  s.vis = base + TW + QW;
   s.ck = s.vis + (nmax + 31) / 32;
   s.cid = s.ck + nmax + 1;
   s.rk = s.cid + nmax + 1;
@@ -97,11 +103,114 @@ __device__ __forceinline__ uint32_t pair_key(const uint8_t* a, const uint8_t* b,
   return ukey_of(sq_distance<METRIC>(acc, r2));
 }
 
-// keys[j] = key(q, node ids[j]) for j < n, one node per lane; the ids must be visible to every lane
+// The distance policies.  A policy is bound to one partition (storage positions off .. off + n - 1) and provides
+//   node_ctx(i, s):       the context of inserting node i (all lanes call it; it may fill the warp's scratch)
+//   query_ctx(qi, p, s):  the context of query qi of the slab in probed partition p (all lanes)
+//   key(ctx, node):       the order key of the context's distance to a node (one lane)
+//   between(u, v):        the order key of dist_between(u, v), the heuristic's distance (one lane)
+
+// IVF_HNSW_SQ: every distance is the SQ row rule over d code bytes (sq/storage.rs:387-444, storage.rs:102-105)
 template <int METRIC>
-__device__ __forceinline__ void warp_keys(const Part& P, const uint8_t* q, const uint32_t* ids, uint32_t n,
+struct SqDist {
+  const uint8_t* base;    // the index's code rows [n][d]
+  const uint8_t* qcodes;  // the slab's query codes [qn][d] (search)
+  int d;
+  float r2;
+  const uint8_t* codes;  // the partition's first code row
+  uint64_t off;          // its first storage position
+  uint32_t n;
+  using Ctx = const uint8_t*;
+  static constexpr bool TABLE = false;  // no table or query rows in the scratch
+  __device__ __forceinline__ void bind(uint64_t o, uint32_t cnt) {
+    off = o;
+    n = cnt;
+    codes = base + o * d;
+  }
+  __device__ __forceinline__ Ctx node_ctx(uint32_t i, const Scratch&) const { return codes + (uint64_t)i * d; }
+  __device__ __forceinline__ Ctx query_ctx(uint64_t qi, uint32_t, const Scratch&) const { return qcodes + qi * d; }
+  __device__ __forceinline__ uint32_t key(Ctx q, uint32_t node) const {
+    return pair_key<METRIC>(q, codes + (uint64_t)node * d, d, r2);
+  }
+  __device__ __forceinline__ uint32_t between(uint32_t u, uint32_t v) const {
+    return pair_key<METRIC>(codes + (uint64_t)u * d, codes + (uint64_t)v * d, d, r2);
+  }
+};
+
+// IVF_HNSW_PQ over ProductQuantizationStorage (pq/storage.rs:600-1037); METRIC is L2 (also for cosine: the storage
+// carries L2, pq/storage.rs:465-468) or dot.
+//  * key: PQDistCalculator::distance (:891-919) on a table of M x 2^NBITS f32 entries in the warp's scratch: 8-bit the
+//    m-ascending sum (pq8_row_distance), 4-bit the byte-ordered sum of pair sums; dot subtracts M - 1.  The search
+//    table is the IVF_PQ scan's (the residual query under L2, the raw query under dot, ivf/v2.rs:316-332); the
+//    build table is the node's own decoded codes' (dist_calculator_from_id, :675-749), both from build_lut.
+//  * between: dist_between (:751-841): distance_type.func() over the two decoded full-width rows, with the element
+//    type's lane rule of row_distance.cuh (RULE: 16 lanes, or 32 lanes for 16-bit dot).
+template <int METRIC, int NBITS, int RULE>
+struct PqDist {
+  const uint8_t* base;       // the index's code rows [n][cw]
+  const float* codebook;     // [M][2^NBITS][ds]
+  const float* queries;      // the slab's queries [qn][d] (search; normalised under cosine)
+  const float* centroids;    // [K][d]
+  int d, M, ds, cw;
+  const uint8_t* codes;
+  uint64_t off;
+  uint32_t n;
+  using Ctx = const float*;  // the table
+  static constexpr bool TABLE = true;
+  __device__ __forceinline__ void bind(uint64_t o, uint32_t cnt) {
+    off = o;
+    n = cnt;
+    codes = base + o * cw;
+  }
+  // element e of a row's decoded vector (get_centroids / get_centroids_4bit: the codewords concatenated)
+  __device__ __forceinline__ float elem(const uint8_t* row, int e) const {
+    const int m = e / ds, t = e - m * ds;
+    const uint32_t c = NBITS == 8 ? __ldg(row + m) : (__ldg(row + (m >> 1)) >> ((m & 1) * 4)) & 0xF;
+    return __ldg(codebook + ((size_t)m * (1 << NBITS) + c) * ds + t);
+  }
+  __device__ __forceinline__ Ctx table_of_qv(const Scratch& s) const {
+    __syncwarp();
+    build_lut<METRIC, NBITS, 32>(s.tab, s.qv, codebook, M, ds, threadIdx.x & 31);
+    __syncwarp();
+    return s.tab;
+  }
+  __device__ __forceinline__ Ctx node_ctx(uint32_t i, const Scratch& s) const {
+    const uint8_t* row = codes + (uint64_t)i * cw;
+    for (int e = threadIdx.x & 31; e < d; e += 32) s.qv[e] = elem(row, e);
+    return table_of_qv(s);
+  }
+  __device__ __forceinline__ Ctx query_ctx(uint64_t qi, uint32_t p, const Scratch& s) const {
+    const float* q = queries + qi * d;
+    for (int t = threadIdx.x & 31; t < d; t += 32)
+      s.qv[t] = METRIC == METRIC_DOT ? q[t] : __fsub_rn(q[t], centroids[(size_t)p * d + t]);
+    return table_of_qv(s);
+  }
+  __device__ __forceinline__ uint32_t key(Ctx lut, uint32_t node) const {
+    const uint8_t* row = codes + (uint64_t)node * cw;
+    float dist = NBITS == 8 ? pq8_row_distance(lut, row, M) : pq4_pair_distance(lut, row, cw);
+    // storage.rs:917-918; a NaN passes through, as on x86 (pq_scan.cu does the same)
+    if (METRIC == METRIC_DOT && dist == dist) dist = __fsub_rn(dist, (float)M - 1.0f);
+    return ukey_of(dist);
+  }
+  __device__ __forceinline__ uint32_t between(uint32_t u, uint32_t v) const {
+    const uint8_t* ru = codes + (uint64_t)u * cw;
+    const uint8_t* rv = codes + (uint64_t)v * cw;
+    LaneAcc<RULE, METRIC> acc[16];  // the 16 lanes of the rule, walked one after the other; lane 0 takes the tail
+#pragma unroll
+    for (int l = 0; l < 16; ++l)
+      rule_walk<RULE>(d, l, [&](int e, auto part) {
+        constexpr int PART = decltype(part)::value;
+        if (PART != 2 || l == 0) acc[l].template step<PART>(elem(ru, e), elem(rv, e));
+      });
+    return ukey_of(fold_partials<RULE, METRIC>([&](int i) { return acc[i].a; }, [&](int i) { return acc[i].b; },
+                                               [](int) { return 0u; }, acc[0].s, 0.0f));
+  }
+};
+
+// keys[j] = key(q, node ids[j]) for j < n, one node per lane; the ids must be visible to every lane
+template <class Dist>
+__device__ __forceinline__ void warp_keys(const Dist& P, typename Dist::Ctx q, const uint32_t* ids, uint32_t n,
                                           uint32_t* keys) {
-  for (uint32_t j = threadIdx.x & 31; j < n; j += 32) keys[j] = pair_key<METRIC>(q, P.codes + (uint64_t)ids[j] * P.d, P.d, P.r2);
+  for (uint32_t j = threadIdx.x & 31; j < n; j += 32) keys[j] = P.key(q, ids[j]);
   __syncwarp();
 }
 
@@ -110,15 +219,15 @@ __device__ __forceinline__ bool allowed(const uint64_t* allow, uint64_t pos) {
 }
 
 // greedy_search (graph.rs:375-409): neighbours in list order, strictly closer (f32 `<`) moves on
-template <int METRIC>
-__device__ void greedy(const GraphDev& g, const Part& P, const uint8_t* q, int level, uint32_t& cur, uint32_t& ckey,
+template <class Dist>
+__device__ void greedy(const GraphDev& g, const Dist& P, typename Dist::Ctx q, int level, uint32_t& cur, uint32_t& ckey,
                        const Scratch& s) {
   __shared__ uint32_t sh_cur, sh_key, sh_go;
   const int lane = threadIdx.x & 31;
   for (;;) {
     const ListRef L = list_of(g, P.off + cur, level);
     const uint32_t n = *L.cnt;
-    warp_keys<METRIC>(P, q, L.ids, n, s.bk);
+    warp_keys(P, q, L.ids, n, s.bk);
     if (lane == 0) {
       uint32_t next = NONE;
       float cf = float_of(ckey);
@@ -147,8 +256,8 @@ __device__ void greedy(const GraphDev& g, const Part& P, const uint8_t* q, int l
 // beam_search (graph.rs:275-355) at `level` from (ep, ep_key) with `ef`; the bitmap (bits at off + node, nullable)
 // and the range [lo, hi) (signed total-order keys) filter the results, not the traversal.  `furthest` is read once
 // per expanded node.  Returns the number of results, left ascending (into_sorted_vec) at rk / rid.
-template <int METRIC>
-__device__ uint32_t beam_search(const GraphDev& g, const Part& P, const uint8_t* q, int level, uint32_t ep,
+template <class Dist>
+__device__ uint32_t beam_search(const GraphDev& g, const Dist& P, typename Dist::Ctx q, int level, uint32_t ep,
                                 uint32_t ep_key, uint32_t ef, const uint64_t* allow, int32_t lo, int32_t hi,
                                 const Scratch& s) {
   __shared__ uint32_t sh_go, sh_n;
@@ -192,7 +301,7 @@ __device__ uint32_t beam_search(const GraphDev& g, const Part& P, const uint8_t*
     const bool go = sh_go;
     const uint32_t n = sh_n;
     if (!go) break;
-    warp_keys<METRIC>(P, q, s.bid, n, s.bk);
+    warp_keys(P, q, s.bid, n, s.bk);
     if (lane == 0) {
       for (uint32_t j = 0; j < n; ++j) {
         const uint32_t key = s.bk[j], id = s.bid[j];
@@ -225,8 +334,8 @@ __device__ uint32_t beam_search(const GraphDev& g, const Part& P, const uint8_t*
 // m_max entries stay in push order, a longer list goes through select_neighbors_heuristic (hnsw.rs:60-88) with a
 // STABLE sort by distance in f32::total_cmp order (OrderedFloat's partial_cmp, graph.rs:68-82; the reference's
 // sort_unstable_by leaves tied candidates in an unspecified order).
-template <int METRIC>
-__device__ void prune_into(const Part& P, const uint32_t* ids, const uint32_t* keys, uint32_t c, uint32_t m_max,
+template <class Dist>
+__device__ void prune_into(const Dist& P, const uint32_t* ids, const uint32_t* keys, uint32_t c, uint32_t m_max,
                            const ListRef& dst, const Scratch& s) {
   __shared__ uint32_t sh_na;
   const int lane = threadIdx.x & 31;
@@ -258,9 +367,7 @@ __device__ void prune_into(const Part& P, const uint32_t* ids, const uint32_t* k
   for (uint32_t t = 0; t < c && na < m_max; ++t) {
     const uint32_t u = s.ord[t], uid = ids[u], ukey = keys[u];
     bool ok = true;
-    const uint8_t* urow = P.codes + (uint64_t)uid * P.d;
-    for (uint32_t j = lane; j < na; j += 32)
-      ok = ok && ukey < pair_key<METRIC>(urow, P.codes + (uint64_t)s.aid[j] * P.d, P.d, P.r2);
+    for (uint32_t j = lane; j < na; j += 32) ok = ok && ukey < P.between(uid, s.aid[j]);
     ok = __all_sync(0xffffffffu, ok);
     if (ok) {
       if (lane == 0) {
@@ -282,15 +389,16 @@ __device__ void prune_into(const Part& P, const uint32_t* ids, const uint32_t* k
 }
 
 // HNSW::index_vectors of partitions order[0 ..), taken largest first by a persistent grid of one-warp CTAs
-template <int METRIC>
+template <class Dist>
 __global__ void __launch_bounds__(32)
 hnsw_build_kernel(GraphDev g, const uint64_t* __restrict__ part_offsets, const uint32_t* __restrict__ order, int nparts,
-                  uint32_t* __restrict__ next, const uint8_t* __restrict__ codes, int d, float r2, uint32_t efc,
-                  int32_t lo, int32_t hi, uint32_t* __restrict__ scratch, uint64_t nmax, uint32_t E, uint32_t B,
-                  uint32_t LB) {
+                  uint32_t* __restrict__ next, const Dist proto, uint32_t efc, int32_t lo, int32_t hi,
+                  uint32_t* __restrict__ scratch, uint64_t nmax, uint32_t E, uint32_t B, uint32_t LB, uint32_t TW,
+                  uint32_t QW) {
   __shared__ uint32_t sh_part, sh_go, sh_n;
   const int lane = threadIdx.x & 31;
-  const Scratch s = scratch_at(scratch + blockIdx.x * scratch_words(nmax, E, B, LB), nmax, E, B, LB);
+  if (!Dist::TABLE) TW = QW = 0;
+  const Scratch s = scratch_at(scratch + blockIdx.x * scratch_words(nmax, E, B, LB, TW, QW), nmax, E, B, LB, TW, QW);
   for (;;) {
     if (lane == 0) sh_part = atomicAdd(next, 1u);
     __syncwarp();
@@ -298,23 +406,19 @@ hnsw_build_kernel(GraphDev g, const uint64_t* __restrict__ part_offsets, const u
     __syncwarp();
     if (t >= (uint32_t)nparts) return;
     const uint32_t p = order[t];
-    Part P;
-    P.off = part_offsets[p];
-    P.n = (uint32_t)(part_offsets[p + 1] - P.off);
-    P.codes = codes + P.off * d;
-    P.d = d;
-    P.r2 = r2;
+    Dist P = proto;
+    P.bind(part_offsets[p], (uint32_t)(part_offsets[p + 1] - part_offsets[p]));
     for (uint32_t i = 1; i < P.n; ++i) {  // HnswBuilder::insert (builder.rs:396-463)
-      const uint8_t* q = P.codes + (uint64_t)i * d;
+      const typename Dist::Ctx q = P.node_ctx(i, s);  // dist_calculator_from_id(node)
       const int target = (int)g.nlev[P.off + i] - 1;
-      uint32_t ep = 0, ekey = pair_key<METRIC>(q, P.codes, d, r2);
-      for (int level = g.max_level - 1; level > target; --level) greedy<METRIC>(g, P, q, level, ep, ekey, s);
+      uint32_t ep = 0, ekey = P.key(q, 0);
+      for (int level = g.max_level - 1; level > target; --level) greedy(g, P, q, level, ep, ekey, s);
       for (int level = target; level >= 0; --level) {
-        const uint32_t R = beam_search<METRIC>(g, P, q, level, ep, ekey, efc, nullptr, lo, hi, s);
+        const uint32_t R = beam_search(g, P, q, level, ep, ekey, efc, nullptr, lo, hi, s);
         ep = s.rid[0];
         ekey = s.rk[0];
         const uint32_t m_max = level == 0 ? 2 * g.m : g.m;
-        prune_into<METRIC>(P, s.rid, s.rk, R, m_max, list_of(g, P.off + i, level), s);
+        prune_into(P, s.rid, s.rk, R, m_max, list_of(g, P.off + i, level), s);
       }
       for (int level = 0; level <= target; ++level) {  // the back-links, level by level, in pruned-list order
         const uint32_t m_max = level == 0 ? 2 * g.m : g.m;
@@ -343,7 +447,7 @@ hnsw_build_kernel(GraphDev g, const uint64_t* __restrict__ part_offsets, const u
           const bool add = sh_go;
           const uint32_t c = sh_n;
           __syncwarp();
-          if (add) prune_into<METRIC>(P, s.lid, s.lk, c, m_max, other, s);
+          if (add) prune_into(P, s.lid, s.lk, c, m_max, other, s);
         }
       }
     }
@@ -352,31 +456,27 @@ hnsw_build_kernel(GraphDev g, const uint64_t* __restrict__ part_offsets, const u
 
 // HNSW::search of every slot: partition id >= K or an empty partition -> no rows; the prefilter's flat branch when
 // fewer than 10 % of the partition's rows are allowed (builder.rs:715-725), search_inner otherwise
-template <int METRIC>
+template <class Dist>
 __global__ void __launch_bounds__(32)
 hnsw_search_kernel(GraphDev g, uint64_t nslots, int np, const uint32_t* __restrict__ probe_ids,
-                   const uint64_t* __restrict__ offsets, const uint32_t* __restrict__ acnt,
-                   const uint8_t* __restrict__ qcodes, const uint8_t* __restrict__ codes, int d, float r2,
+                   const uint64_t* __restrict__ offsets, const uint32_t* __restrict__ acnt, const Dist proto,
                    const uint64_t* __restrict__ row_ids, uint32_t ef, int kc, ScanFilter flt,
                    float* __restrict__ cand_d, uint64_t* __restrict__ cand_id, uint32_t* __restrict__ cand_cnt,
-                   uint32_t* __restrict__ scratch, uint64_t nmax, uint32_t E, uint32_t B) {
+                   uint32_t* __restrict__ scratch, uint64_t nmax, uint32_t E, uint32_t B, uint32_t TW, uint32_t QW) {
   __shared__ uint32_t sh_n;
   const int lane = threadIdx.x & 31;
-  const Scratch s = scratch_at(scratch + blockIdx.x * scratch_words(nmax, E, B, 0), nmax, E, B, 0);
+  if (!Dist::TABLE) TW = QW = 0;
+  const Scratch s = scratch_at(scratch + blockIdx.x * scratch_words(nmax, E, B, 0, TW, QW), nmax, E, B, 0, TW, QW);
   for (uint64_t slot = blockIdx.x; slot < nslots; slot += gridDim.x) {
     const uint64_t qi = slot / np;
     const uint32_t p = probe_ids[slot];
-    Part P;
-    P.off = offsets[p];
-    P.n = (uint32_t)(offsets[p + 1] - P.off);
-    P.codes = codes + P.off * d;
-    P.d = d;
-    P.r2 = r2;
+    Dist P = proto;
+    P.bind(offsets[p], (uint32_t)(offsets[p + 1] - offsets[p]));
     if (P.n == 0) {  // an empty partition returns no rows (builder.rs:695-697)
       if (lane == 0) cand_cnt[slot] = 0;
       continue;
     }
-    const uint8_t* q = qcodes + qi * d;
+    const typename Dist::Ctx q = P.query_ctx(qi, p, s);  // dist_calculator(query)
     uint32_t R;
     if (flt.allow && acnt[p] < (uint32_t)((uint64_t)P.n * 10 / 100)) {
       // HNSW::flat_search (builder.rs:238-280): allowed rows in node order, kept when lower < d <= upper.  Lane 0 drives
@@ -385,7 +485,7 @@ hnsw_search_kernel(GraphDev g, uint64_t nslots, int np, const uint32_t* __restri
       uint32_t len = 0;
       for (uint32_t c0 = 0; c0 < P.n; c0 += 32) {
         const uint32_t j = c0 + lane;
-        if (j < P.n && allowed(flt.allow, P.off + j)) s.bk[lane] = pair_key<METRIC>(q, P.codes + (uint64_t)j * d, d, r2);
+        if (j < P.n && allowed(flt.allow, P.off + j)) s.bk[lane] = P.key(q, j);
         __syncwarp();
         if (lane == 0) {
           for (uint32_t t = 0; t < 32 && c0 + t < P.n; ++t) {
@@ -411,9 +511,9 @@ hnsw_search_kernel(GraphDev g, uint64_t nslots, int np, const uint32_t* __restri
       R = sh_n;
       __syncwarp();
     } else {  // search_inner (builder.rs:164-201): greedy descent to level 0 inclusive, then the beam search
-      uint32_t ep = 0, ekey = pair_key<METRIC>(q, P.codes, d, r2);
-      for (int level = g.max_level - 1; level >= 0; --level) greedy<METRIC>(g, P, q, level, ep, ekey, s);
-      R = beam_search<METRIC>(g, P, q, 0, ep, ekey, ef, flt.allow, flt.lo_key, flt.hi_key, s);
+      uint32_t ep = 0, ekey = P.key(q, 0);
+      for (int level = g.max_level - 1; level >= 0; --level) greedy(g, P, q, level, ep, ekey, s);
+      R = beam_search(g, P, q, 0, ep, ekey, ef, flt.allow, flt.lo_key, flt.hi_key, s);
       R = min(R, (uint32_t)kc);
     }
     for (uint32_t j = lane; j < R; j += 32) {
@@ -442,8 +542,11 @@ void hnsw_level_thresholds(int m, int max_level, uint64_t* thr) {
   }
 }
 
-void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, int d, int metric, float r2,
-                uint64_t seed) {
+// the levels and the empty lists of every partition's graph, then `launch(kernel, policy)` of the build kernel with
+// the policy's table and query words TW / QW in each warp's scratch
+template <class Launch>
+static void build_graphs(HnswGraph& g, const uint64_t* part_offsets, int K, uint64_t seed, uint32_t TW, uint32_t QW,
+                         Launch&& launch) {
   std::vector<uint64_t> off(K + 1);
   d2h(off.data(), part_offsets, (size_t)K + 1);
   sync_stream();
@@ -468,7 +571,7 @@ void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t
       nlev[off[p] + i] = (uint8_t)L;
       up_base[off[p] + i] = (uint32_t)n_up;
       n_up += (uint64_t)(L - 1);
-      LB2_REQUIRE(n_up < 0xffffffffull, "IVF_HNSW_SQ: more than 2^32 - 1 upper-level rows");
+      LB2_REQUIRE(n_up < 0xffffffffull, "%s: more than 2^32 - 1 upper-level rows", g.kind);
     }
   }
   std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
@@ -499,7 +602,7 @@ void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t
     return;
   }
   const uint32_t E = (uint32_t)g.ef_construction, B = 2 * (uint32_t)g.m + 1, LB = std::max(E, B);
-  const size_t words = scratch_words(nmax, E, B, LB);
+  const size_t words = scratch_words(nmax, E, B, LB, TW, QW);
   // one warp per partition, at most 32 per SM, and no more warps than 512 MB of scratch holds
   const size_t fit = std::max<size_t>(1, (512ull << 20) / (words * 4));
   const unsigned nct = (unsigned)std::min<size_t>({order.size(), (size_t)ctx().num_sms * 32, fit});
@@ -507,13 +610,66 @@ void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t
   h2d(dorder.p, order.data(), order.size());
   next.zero();
   const int32_t lo = key_of_host(-3.40282347e+38f), hi = key_of_host(3.40282347e+38f);  // f32::MIN, f32::MAX
-  auto launch = [&](auto kern) {
-    LB2_LAUNCH("hnsw_build", kern, nct, 32, 0, dev_view(g), part_offsets, dorder.p, (int)order.size(), next.p, codes,
-               d, r2, E, lo, hi, scratch.p, nmax, E, B, LB);
-  };
-  if (metric == METRIC_DOT) launch(hnsw_build_kernel<METRIC_DOT>);
-  else launch(hnsw_build_kernel<METRIC_L2>);  // cosine: L2 on the normalised vectors' codes
+  launch([&](auto kern, const auto& P) {
+    LB2_LAUNCH("hnsw_build", kern, nct, 32, 0, dev_view(g), part_offsets, dorder.p, (int)order.size(), next.p, P, E,
+               lo, hi, scratch.p, nmax, E, B, LB, TW, QW);
+  });
   sync_stream();
+}
+
+void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, int d, int metric, float r2,
+                uint64_t seed) {
+  build_graphs(g, part_offsets, K, seed, 0, 0, [&](auto go) {
+    auto with = [&](auto m) {
+      SqDist<decltype(m)::value> P{};
+      P.base = codes;
+      P.d = d;
+      P.r2 = r2;
+      go(hnsw_build_kernel<SqDist<decltype(m)::value>>, P);
+    };
+    if (metric == METRIC_DOT) with(std::integral_constant<int, METRIC_DOT>{});
+    else with(std::integral_constant<int, METRIC_L2>{});  // cosine: L2 on the normalised vectors' codes
+  });
+}
+
+// the PQ policy's template arguments: f(metric, nbits, rule) with std::integral_constants.  Cosine is L2 (the
+// storage's distance type, pq/storage.rs:465-468); dist_between of 16-bit rows under dot takes 32 lanes
+// (dot.rs:78-83,133), every other case 16.
+template <class F>
+static void dispatch_pq(int metric, int nbits, lb2_dtype dtype, F&& f) {
+  auto by_bits = [&](auto m, auto rule) {
+    if (nbits == 4) f(m, std::integral_constant<int, 4>{}, rule);
+    else f(m, std::integral_constant<int, 8>{}, rule);
+  };
+  if (metric == METRIC_DOT) {
+    if (dtype == LB2_F16 || dtype == LB2_BF16)
+      by_bits(std::integral_constant<int, METRIC_DOT>{}, std::integral_constant<int, RULE_DOT32>{});
+    else
+      by_bits(std::integral_constant<int, METRIC_DOT>{}, std::integral_constant<int, RULE_LANES16>{});
+  } else {
+    by_bits(std::integral_constant<int, METRIC_L2>{}, std::integral_constant<int, RULE_LANES16>{});
+  }
+}
+
+// the words of a PQ warp's table (M x 2^nbits) and of its query / decoded row (d, kept 16-byte aligned)
+static uint32_t pq_table_words(int M, int nbits) { return (uint32_t)M << nbits; }
+static uint32_t pq_query_words(int d) { return (uint32_t)(d + 3) & ~3u; }
+
+void hnsw_build_pq(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, const float* codebook,
+                   int d, int M, int nbits, int metric, lb2_dtype dtype, uint64_t seed) {
+  build_graphs(g, part_offsets, K, seed, pq_table_words(M, nbits), pq_query_words(d), [&](auto go) {
+    dispatch_pq(metric, nbits, dtype, [&](auto m, auto b, auto r) {
+      using Dist = PqDist<decltype(m)::value, decltype(b)::value, decltype(r)::value>;
+      Dist P{};
+      P.base = codes;
+      P.codebook = codebook;
+      P.d = d;
+      P.M = M;
+      P.ds = d / M;
+      P.cw = nbits == 4 ? M / 2 : M;
+      go(hnsw_build_kernel<Dist>, P);
+    });
+  });
 }
 
 // caller memory (host or device) -> host
@@ -526,10 +682,10 @@ static std::vector<T> fetch(const T* src, size_t count) {
 }
 
 // a list naming one node twice would be expanded once here and twice by beam_search's filter-then-process loop
-static void no_duplicates(const uint32_t* ids, uint32_t c, uint64_t row, int level) {
+static void no_duplicates(const char* kind, const uint32_t* ids, uint32_t c, uint64_t row, int level) {
   for (uint32_t a = 0; a < c; ++a)
     for (uint32_t b = a + 1; b < c; ++b)
-      LB2_REQUIRE(ids[a] != ids[b], "IVF_HNSW_SQ: row %llu lists node %u twice at level %d", (unsigned long long)row,
+      LB2_REQUIRE(ids[a] != ids[b], "%s: row %llu lists node %u twice at level %d", kind, (unsigned long long)row,
                   ids[a], level);
 }
 
@@ -547,11 +703,11 @@ void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t*
     for (uint64_t r = off[p]; r < off[p + 1]; ++r) {
       const int L = lv[r];
       LB2_REQUIRE(L >= 1 && L <= g.max_level && (r > off[p] || L == g.max_level),
-                  "IVF_HNSW_SQ: row %llu has %d levels (node 0 of a partition has max_level = %d, the others 1 .. %d)",
+                  "%s: row %llu has %d levels (node 0 of a partition has max_level = %d, the others 1 .. %d)", g.kind,
                   (unsigned long long)r, L, g.max_level, g.max_level);
       up_base[r] = (uint32_t)n_up;
       n_up += (uint64_t)(L - 1);
-      LB2_REQUIRE(n_up < 0xffffffffull, "IVF_HNSW_SQ: more than 2^32 - 1 upper-level rows");
+      LB2_REQUIRE(n_up < 0xffffffffull, "%s: more than 2^32 - 1 upper-level rows", g.kind);
     }
   }
   LB2_REQUIRE(n_up == 0 || (counts_up && nbr_up && dist_up), "null argument");
@@ -560,22 +716,22 @@ void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t*
   for (int p = 0; p < K; ++p) {  // every neighbour is a node of the partition that has the level
     const uint64_t a = off[p], np_ = off[p + 1] - a;
     for (uint64_t r = a; r < off[p + 1]; ++r) {
-      LB2_REQUIRE(c0[r] <= 2 * m, "IVF_HNSW_SQ: row %llu has %u level-0 neighbours (at most 2m = %llu)",
+      LB2_REQUIRE(c0[r] <= 2 * m, "%s: row %llu has %u level-0 neighbours (at most 2m = %llu)", g.kind,
                   (unsigned long long)r, c0[r], (unsigned long long)(2 * m));
       for (uint32_t j = 0; j < c0[r]; ++j)
-        LB2_REQUIRE(n0[r * 2 * m + j] < np_, "IVF_HNSW_SQ: row %llu links to node %u of a %llu-row partition",
+        LB2_REQUIRE(n0[r * 2 * m + j] < np_, "%s: row %llu links to node %u of a %llu-row partition", g.kind,
                     (unsigned long long)r, n0[r * 2 * m + j], (unsigned long long)np_);
-      no_duplicates(&n0[r * 2 * m], c0[r], r, 0);
+      no_duplicates(g.kind, &n0[r * 2 * m], c0[r], r, 0);
       for (int l = 1; l < lv[r]; ++l) {
         const uint64_t u = up_base[r] + (l - 1);
-        LB2_REQUIRE(cu[u] <= m, "IVF_HNSW_SQ: row %llu has %u neighbours at level %d (at most m = %llu)",
+        LB2_REQUIRE(cu[u] <= m, "%s: row %llu has %u neighbours at level %d (at most m = %llu)", g.kind,
                     (unsigned long long)r, cu[u], l, (unsigned long long)m);
         for (uint32_t j = 0; j < cu[u]; ++j) {
           const uint32_t id = nu[u * m + j];
-          LB2_REQUIRE(id < np_ && lv[a + id] > l, "IVF_HNSW_SQ: row %llu links at level %d to node %u, which lacks it",
+          LB2_REQUIRE(id < np_ && lv[a + id] > l, "%s: row %llu links at level %d to node %u, which lacks it", g.kind,
                       (unsigned long long)r, l, id);
         }
-        no_duplicates(&nu[u * m], cu[u], r, l);
+        no_duplicates(g.kind, &nu[u * m], cu[u], r, l);
       }
     }
   }
@@ -605,11 +761,14 @@ void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t*
   sync_stream();
 }
 
-void hnsw_search(const IvfSearch& s, const HnswGraph& g, const uint8_t* codes, float r2, const uint8_t* qcodes,
-                 uint32_t ef) {
+// HNSW::search of every probed partition with `launch(kernel, policy, scratch words)`; `bind(policy, slots)` points the
+// policy at the slab's queries
+template <class Launch>
+static void search_graphs(const IvfSearch& s, const HnswGraph& g, uint32_t ef, uint32_t TW, uint32_t QW,
+                          Launch&& launch) {
   const uint32_t kc = (uint32_t)s.k;
   if (ef == 0) ef = kc + kc / 2;
-  if (ef < kc) fail(LB2_INVALID_ARG, "IVF_HNSW_SQ: ef = %u must be greater than or equal to k = %u", ef, kc);
+  if (ef < kc) fail(LB2_INVALID_ARG, "%s: ef = %u must be greater than or equal to k = %u", g.kind, ef, kc);
   if (!ivf_search_begin(s, 0, "%zu", 0)) return;
   DevBuf<uint32_t> acnt;
   if (s.flt.allow) {  // `remained`: the allowed rows of each partition (builder.rs:715-718)
@@ -618,20 +777,53 @@ void hnsw_search(const IvfSearch& s, const HnswGraph& g, const uint8_t* codes, f
   }
   const uint64_t nmax = std::max<uint64_t>(g.max_part, 1);
   const uint32_t E = std::max(ef, kc), B = std::max<uint32_t>(2 * (uint32_t)g.m, 32);
-  const size_t words = scratch_words(nmax, E, B, 0);
+  const size_t words = scratch_words(nmax, E, B, 0, TW, QW);
   const uint64_t cap = std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)ctx().num_sms * 32, (256ull << 20) / (words * 4)));
   DevBuf<uint32_t> scratch(words * cap);
   run_ivf_search(s, [&](const ScanSlots& sl) {
     const uint64_t nslots = sl.qn * sl.np;
     if (nslots == 0) return;
     const unsigned nct = (unsigned)std::min<uint64_t>(nslots, cap);
-    auto launch = [&](auto kern) {
-      LB2_LAUNCH("hnsw_search", kern, nct, 32, 0, dev_view(g), nslots, sl.np, sl.probe_ids, sl.offsets, acnt.p,
-                 qcodes + sl.q0 * s.d, codes, s.d, r2, s.row_ids, ef, (int)kc, s.flt, sl.cand_d, sl.cand_id,
-                 sl.cand_cnt, scratch.p, nmax, E, B);
+    launch(sl, [&](auto kern, const auto& P) {
+      LB2_LAUNCH("hnsw_search", kern, nct, 32, 0, dev_view(g), nslots, sl.np, sl.probe_ids, sl.offsets, acnt.p, P,
+                 s.row_ids, ef, (int)kc, s.flt, sl.cand_d, sl.cand_id, sl.cand_cnt, scratch.p, nmax, E, B, TW, QW);
+    });
+  });
+}
+
+void hnsw_search(const IvfSearch& s, const HnswGraph& g, const uint8_t* codes, float r2, const uint8_t* qcodes,
+                 uint32_t ef) {
+  search_graphs(s, g, ef, 0, 0, [&](const ScanSlots& sl, auto go) {
+    auto with = [&](auto m) {
+      SqDist<decltype(m)::value> P{};
+      P.base = codes;
+      P.qcodes = qcodes + sl.q0 * s.d;
+      P.d = s.d;
+      P.r2 = r2;
+      go(hnsw_search_kernel<SqDist<decltype(m)::value>>, P);
     };
-    if (s.metric == METRIC_DOT) launch(hnsw_search_kernel<METRIC_DOT>);
-    else launch(hnsw_search_kernel<METRIC_L2>);
+    if (s.metric == METRIC_DOT) with(std::integral_constant<int, METRIC_DOT>{});
+    else with(std::integral_constant<int, METRIC_L2>{});
+  });
+}
+
+void hnsw_search_pq(const IvfSearch& s, const HnswGraph& g, const float* codebook, int M, int nbits,
+                    const uint8_t* codes, uint32_t ef) {
+  search_graphs(s, g, ef, pq_table_words(M, nbits), pq_query_words(s.d), [&](const ScanSlots& sl, auto go) {
+    // the search never calls `between`: one rule per (metric, nbits)
+    dispatch_pq(s.metric, nbits, LB2_F32, [&](auto m, auto b, auto r) {
+      using Dist = PqDist<decltype(m)::value, decltype(b)::value, decltype(r)::value>;
+      Dist P{};
+      P.base = codes;
+      P.codebook = codebook;
+      P.queries = s.queries + sl.q0 * s.d;
+      P.centroids = s.centroids;
+      P.d = s.d;
+      P.M = M;
+      P.ds = s.d / M;
+      P.cw = nbits == 4 ? M / 2 : M;
+      go(hnsw_search_kernel<Dist>, P);
+    });
   });
 }
 

@@ -1,5 +1,5 @@
-// hnsw.cuh -- the per-partition HNSW graphs of IVF_HNSW_SQ (lance-index/src/vector/hnsw/builder.rs) and their
-// device layout; internal interface of hnsw.cu
+// hnsw.cuh -- the per-partition HNSW graphs of IVF_HNSW_SQ and IVF_HNSW_PQ (lance-index/src/vector/hnsw/builder.rs)
+// and their device layout; internal interface of hnsw.cu
 #pragma once
 #include <stdint.h>
 
@@ -14,6 +14,7 @@ struct IvfSearch;
 // Lists keep the reference's order of level_neighbors_ranked (graph/builder.rs:33-48); the distances are those of
 // the ranked list.  Node 0 of every partition has max_level levels and is the entry point (builder.rs:354-376).
 struct HnswGraph {
+  const char* kind = "IVF_HNSW_SQ";  // the index kind's name in messages: IVF_HNSW_SQ or IVF_HNSW_PQ
   int max_level = 0, m = 0, ef_construction = 0;
   uint64_t max_part = 0;  // rows of the largest partition (scratch sizing)
   uint64_t n_up = 0;      // upper-level rows
@@ -39,6 +40,11 @@ inline uint32_t hnsw_level_draw(uint64_t seed, uint32_t p, uint32_t i) {
 // codes [n][d] in partition order, part_offsets on the device.  Fills g (its parameters set by the caller).
 void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, int d, int metric, float r2,
                 uint64_t seed);
+// the same over PQ codes [n][cw] (cw = M, or M / 2 for 4-bit codes) with the codebook [M][2^nbits][d / M]: a node's
+// descent, beam searches and lists use the table of its decoded codes, the heuristic the decoded rows' distance with
+// the rule of `dtype` (pq/storage.rs:675-841)
+void hnsw_build_pq(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, const float* codebook,
+                   int d, int M, int nbits, int metric, lb2_dtype dtype, uint64_t seed);
 // a graph from the caller's arrays in the layout above (host or device memory), checked against the partitions
 void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* levels, const uint32_t* counts0,
                const uint32_t* nbr0, const float* dist0, const uint32_t* counts_up, const uint32_t* nbr_up,
@@ -46,4 +52,7 @@ void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t*
 // HNSW::search (builder.rs:678-739) as the scan of every probed partition; ef = 0: k' + k' / 2 (builder.rs:563-573)
 void hnsw_search(const IvfSearch& s, const HnswGraph& g, const uint8_t* codes, float r2, const uint8_t* qcodes,
                  uint32_t ef);
+// the same over PQ codes: each slot's table is the IVF_PQ scan's table of the (residual) query
+void hnsw_search_pq(const IvfSearch& s, const HnswGraph& g, const float* codebook, int M, int nbits,
+                    const uint8_t* codes, uint32_t ef);
 }  // namespace lb2

@@ -324,8 +324,11 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
       break;
     }
     case IndexKind::PQ:
-      ivfpq_search(s, index->codebook.p, index->M, index->nbits, index->codes.p, index->slab_off.p,
-                   index->codes_skew.p);
+      if (index->hnsw)  // IVF_HNSW_PQ: the IVF_PQ scan's query tables, searched through each partition's graph
+        hnsw_search_pq(s, *index->hnsw, index->codebook.p, index->M, index->nbits, index->codes.p, ef);
+      else
+        ivfpq_search(s, index->codebook.p, index->M, index->nbits, index->codes.p, index->slab_off.p,
+                     index->codes_skew.p);
       break;
   }
   if (refine) {
@@ -527,6 +530,7 @@ lb2_status lb2_index_load(lb2_index* index, const uint32_t* part_ids, const uint
                           const uint64_t* row_ids, uint64_t n) {
   LB2_API_BEGIN
   LB2_REQUIRE(index && index->kind == IndexKind::PQ, "not an IVF_PQ index");
+  LB2_REQUIRE(!index->hnsw, "lb2_index_load: the index already has an HNSW graph over its rows");
   load_codes(index, part_ids, codes, row_ids, n, "index_load");
   LB2_API_END
 }
@@ -598,41 +602,40 @@ lb2_status lb2_index_export_sq(const lb2_index* index, void* centroids_out, doub
   LB2_API_END
 }
 
-lb2_status lb2_index_load_hnsw_sq(lb2_index* index, uint32_t max_level, uint32_t m, uint32_t ef_construction,
-                                  const uint8_t* levels, const uint32_t* counts0, const uint32_t* neighbors0,
-                                  const float* dists0, const uint32_t* counts_up, const uint32_t* neighbors_up,
-                                  const float* dists_up) {
-  LB2_API_BEGIN
-  LB2_REQUIRE(index && index->kind == IndexKind::SQ, "not an IVF_SQ index");
-  LB2_REQUIRE(max_level >= 1 && max_level <= 64 && m >= 1 && m <= 1024, "IVF_HNSW_SQ: max_level %u or m %u out of range",
+}  // extern "C"
+
+// lb2_index_load_hnsw_sq / _pq: a graph over the rows of an index of `kind`
+static void load_hnsw(lb2_index* index, IndexKind kind, const char* name, uint32_t max_level, uint32_t m,
+                      uint32_t ef_construction, const uint8_t* levels, const uint32_t* counts0,
+                      const uint32_t* neighbors0, const float* dists0, const uint32_t* counts_up,
+                      const uint32_t* neighbors_up, const float* dists_up) {
+  LB2_REQUIRE(index && index->kind == kind, "not an %s index", kind == IndexKind::SQ ? "IVF_SQ" : "IVF_PQ");
+  LB2_REQUIRE(max_level >= 1 && max_level <= 64 && m >= 1 && m <= 1024, "%s: max_level %u or m %u out of range", name,
               max_level, m);
   std::unique_ptr<HnswGraph> g(new HnswGraph());
+  g->kind = name;
   g->max_level = (int)max_level;
   g->m = (int)m;
   g->ef_construction = (int)ef_construction;
   hnsw_load(*g, index->part_offsets.p, index->K, levels, counts0, neighbors0, dists0, counts_up, neighbors_up, dists_up);
   index->hnsw = std::move(g);
-  LB2_API_END
 }
 
-lb2_status lb2_index_hnsw_sq_info(const lb2_index* index, uint32_t* max_level, uint32_t* m, uint32_t* ef_construction,
-                                  uint64_t* num_upper_rows) {
-  LB2_API_BEGIN
-  LB2_REQUIRE(index && index->hnsw, "not an IVF_HNSW_SQ index");
-  const HnswGraph& g = *index->hnsw;
+// lb2_index_hnsw_sq_info / _pq_info: the graph of an index of `kind`
+static const HnswGraph& graph_of(const lb2_index* index, IndexKind kind, const char* name) {
+  LB2_REQUIRE(index && index->hnsw && index->kind == kind, "not an %s index", name);
+  return *index->hnsw;
+}
+static void hnsw_info(const HnswGraph& g, uint32_t* max_level, uint32_t* m, uint32_t* ef_construction,
+                      uint64_t* num_upper_rows) {
   if (max_level) *max_level = (uint32_t)g.max_level;
   if (m) *m = (uint32_t)g.m;
   if (ef_construction) *ef_construction = (uint32_t)g.ef_construction;
   if (num_upper_rows) *num_upper_rows = g.n_up;
-  LB2_API_END
 }
-
-lb2_status lb2_index_export_hnsw_sq(const lb2_index* index, uint8_t* levels_out, uint32_t* counts0_out,
-                                    uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
-                                    uint32_t* neighbors_up_out, float* dists_up_out) {
-  LB2_API_BEGIN
-  LB2_REQUIRE(index && index->hnsw, "not an IVF_HNSW_SQ index");
-  const HnswGraph& g = *index->hnsw;
+static void export_hnsw(const lb2_index* index, const HnswGraph& g, uint8_t* levels_out, uint32_t* counts0_out,
+                        uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
+                        uint32_t* neighbors_up_out, float* dists_up_out) {
   const size_t n = index->n, nu = g.n_up, m = (size_t)g.m;
   cudaStream_t st = ctx().stream;
   auto out = [&](void* dst, const void* src, size_t bytes) {
@@ -646,6 +649,59 @@ lb2_status lb2_index_export_hnsw_sq(const lb2_index* index, uint8_t* levels_out,
   out(neighbors_up_out, g.nbru.p, 4 * nu * m);
   out(dists_up_out, g.dstu.p, 4 * nu * m);
   sync_stream();
+}
+
+extern "C" {
+
+lb2_status lb2_index_load_hnsw_sq(lb2_index* index, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                                  const uint8_t* levels, const uint32_t* counts0, const uint32_t* neighbors0,
+                                  const float* dists0, const uint32_t* counts_up, const uint32_t* neighbors_up,
+                                  const float* dists_up) {
+  LB2_API_BEGIN
+  load_hnsw(index, IndexKind::SQ, "IVF_HNSW_SQ", max_level, m, ef_construction, levels, counts0, neighbors0, dists0,
+            counts_up, neighbors_up, dists_up);
+  LB2_API_END
+}
+
+lb2_status lb2_index_load_hnsw_pq(lb2_index* index, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                                  const uint8_t* levels, const uint32_t* counts0, const uint32_t* neighbors0,
+                                  const float* dists0, const uint32_t* counts_up, const uint32_t* neighbors_up,
+                                  const float* dists_up) {
+  LB2_API_BEGIN
+  load_hnsw(index, IndexKind::PQ, "IVF_HNSW_PQ", max_level, m, ef_construction, levels, counts0, neighbors0, dists0,
+            counts_up, neighbors_up, dists_up);
+  LB2_API_END
+}
+
+lb2_status lb2_index_hnsw_sq_info(const lb2_index* index, uint32_t* max_level, uint32_t* m, uint32_t* ef_construction,
+                                  uint64_t* num_upper_rows) {
+  LB2_API_BEGIN
+  hnsw_info(graph_of(index, IndexKind::SQ, "IVF_HNSW_SQ"), max_level, m, ef_construction, num_upper_rows);
+  LB2_API_END
+}
+
+lb2_status lb2_index_hnsw_pq_info(const lb2_index* index, uint32_t* max_level, uint32_t* m, uint32_t* ef_construction,
+                                  uint64_t* num_upper_rows) {
+  LB2_API_BEGIN
+  hnsw_info(graph_of(index, IndexKind::PQ, "IVF_HNSW_PQ"), max_level, m, ef_construction, num_upper_rows);
+  LB2_API_END
+}
+
+lb2_status lb2_index_export_hnsw_sq(const lb2_index* index, uint8_t* levels_out, uint32_t* counts0_out,
+                                    uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
+                                    uint32_t* neighbors_up_out, float* dists_up_out) {
+  LB2_API_BEGIN
+  export_hnsw(index, graph_of(index, IndexKind::SQ, "IVF_HNSW_SQ"), levels_out, counts0_out, neighbors0_out,
+              dists0_out, counts_up_out, neighbors_up_out, dists_up_out);
+  LB2_API_END
+}
+
+lb2_status lb2_index_export_hnsw_pq(const lb2_index* index, uint8_t* levels_out, uint32_t* counts0_out,
+                                    uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
+                                    uint32_t* neighbors_up_out, float* dists_up_out) {
+  LB2_API_BEGIN
+  export_hnsw(index, graph_of(index, IndexKind::PQ, "IVF_HNSW_PQ"), levels_out, counts0_out, neighbors0_out,
+              dists0_out, counts_up_out, neighbors_up_out, dists_up_out);
   LB2_API_END
 }
 
@@ -767,7 +823,7 @@ lb2_status lb2_index_search_hnsw(lb2_index* index, const void* queries, uint64_t
                                  uint32_t* counts_out, uint32_t* nprobes_out) {
   LB2_API_BEGIN
   LB2_REQUIRE(sp && index, "null argument");
-  LB2_REQUIRE(index->hnsw, "not an IVF_HNSW_SQ index");
+  LB2_REQUIRE(index->hnsw, "not an IVF_HNSW_SQ or IVF_HNSW_PQ index");
   LB2_REQUIRE(!nprobes_out || pp, "nprobes_out needs probe parameters");
   if (pp) {
     ProbedSearch ps(sp, pp, nq, nprobes_out);
@@ -914,6 +970,7 @@ lb2_status lb2_index_update(const lb2_index* old, const void* new_centroids, uin
                             uint64_t n_add, const uint64_t* remove_row_ids, uint64_t n_remove, lb2_index** out) {
   LB2_API_BEGIN
   LB2_REQUIRE(old && out && old->kind == IndexKind::PQ, "lb2_index_update takes an IVF_PQ index");
+  if (old->hnsw) fail(LB2_UNSUPPORTED, "lb2_index_update: IVF_HNSW_PQ indexes are not implemented");
   LB2_REQUIRE(new_k > 0 && (new_centroids || new_k == (uint32_t)old->K), "a changed partition count needs new centroids");
   LB2_REQUIRE(n_add == 0 || (add_part_ids && add_codes && add_row_ids), "added rows need partition ids, codes and row ids");
   LB2_REQUIRE(n_remove == 0 || remove_row_ids, "null remove list");
@@ -956,7 +1013,7 @@ lb2_status lb2_index_repartition(const lb2_index* shard, lb2_index** owned_out) 
   LB2_API_BEGIN
   LB2_REQUIRE(shard && owned_out, "null argument");
   if (shard->kind == IndexKind::RQ) fail(LB2_UNSUPPORTED, "lb2_index_repartition: IVF_RQ indexes are not implemented");
-  if (shard->hnsw) fail(LB2_UNSUPPORTED, "lb2_index_repartition: IVF_HNSW_SQ indexes are not implemented");
+  if (shard->hnsw) fail(LB2_UNSUPPORTED, "lb2_index_repartition: %s indexes are not implemented", shard->hnsw->kind);
   Comm* cm = current_comm();
   const int G = cm ? cm->nranks : 1, me = cm ? cm->rank : 0;
   const int K = shard->K;

@@ -16,52 +16,11 @@
 #include "common.cuh"
 #include "exact.cuh"
 #include "ivf_search.cuh"
+#include "pq_lut.cuh"
 #include "scan.cuh"
 #include "topk.cuh"
 
 namespace lb2 {
-
-// LUT[m][c] = dist(q_m, cb[m][c])  (pq/distance.rs:38-56).  For the common sub-vector widths the
-// codeword is fetched with 128-bit loads and the reference-order sum is fully unrolled.
-template <int METRIC, int DS>
-__device__ __forceinline__ float lut_entry_fixed(const float* __restrict__ qm, const float* __restrict__ cw) {
-  float qv[DS], cv[DS];
-#pragma unroll
-  for (int t = 0; t < DS; t += 4) {
-    const float4 a = *reinterpret_cast<const float4*>(qm + t);
-    const float4 b = __ldg(reinterpret_cast<const float4*>(cw + t));
-    qv[t] = a.x; qv[t + 1] = a.y; qv[t + 2] = a.z; qv[t + 3] = a.w;
-    cv[t] = b.x; cv[t + 1] = b.y; cv[t + 2] = b.z; cv[t + 3] = b.w;
-  }
-  if (DS < 16) {  // tail-only path (l2.rs:69-79): plain left-to-right sum
-    float s = 0.0f;
-#pragma unroll
-    for (int t = 0; t < DS; ++t) s = f_add(s, term<METRIC>(qv[t], cv[t]));
-    return finish<METRIC>(f_add(s, 0.0f));
-  } else {        // DS == 16: one chunk of 16 lanes, summed lane 0..15
-    float t0 = 0.0f;
-#pragma unroll
-    for (int t = 0; t < 16; ++t) t0 = f_add(t0, f_add(0.0f, term<METRIC>(qv[t], cv[t])));
-    return finish<METRIC>(f_add(0.0f, t0));
-  }
-}
-template <int METRIC>
-__device__ __forceinline__ void build_lut_smem(float* lut, const float* qr, const float* __restrict__ codebook,
-                                               int M, int ds, int tid) {
-  if (ds == 8) {
-    for (int idx = tid; idx < M * 256; idx += 256)
-      lut[idx] = lut_entry_fixed<METRIC, 8>(qr + (idx >> 8) * 8, codebook + (size_t)idx * 8);
-  } else if (ds == 4) {
-    for (int idx = tid; idx < M * 256; idx += 256)
-      lut[idx] = lut_entry_fixed<METRIC, 4>(qr + (idx >> 8) * 4, codebook + (size_t)idx * 4);
-  } else if (ds == 16) {
-    for (int idx = tid; idx < M * 256; idx += 256)
-      lut[idx] = lut_entry_fixed<METRIC, 16>(qr + (idx >> 8) * 16, codebook + (size_t)idx * 16);
-  } else {
-    for (int idx = tid; idx < M * 256; idx += 256)
-      lut[idx] = dist_exact_thread<METRIC>(qr + (idx >> 8) * ds, codebook + (size_t)idx * ds, ds);
-  }
-}
 
 // ------------------------------------------------------------------------------------------------
 // the fused (residual query -> LUT -> code scan -> top-k) kernels: one CTA per (query, probed
@@ -84,34 +43,8 @@ __device__ __forceinline__ void stage_query_lut(float* lut, float* qr, const Sca
   for (int t = threadIdx.x; t < a.d; t += 256)
     qr[t] = METRIC == METRIC_DOT ? q[t] : __fsub_rn(q[t], a.centroids[(size_t)p * a.d + t]);
   __syncthreads();
-  if (NBITS == 8) {
-    build_lut_smem<METRIC>(lut, qr, a.codebook, a.M, a.ds, threadIdx.x);
-  } else {
-    for (int idx = threadIdx.x; idx < a.M * 16; idx += 256)
-      lut[idx] = dist_exact_thread<METRIC>(qr + (idx / 16) * a.ds, a.codebook + (size_t)idx * a.ds, a.ds);
-  }
+  build_lut<METRIC, NBITS>(lut, qr, a.codebook, a.M, a.ds, threadIdx.x);
   __syncthreads();
-}
-
-// one row's 8-bit ADC distance: the reference's m-ascending f32 sum of LUT[m][code[m]] (pq/distance.rs:109-144)
-__device__ __forceinline__ float pq8_row_distance(const float* lut, const uint8_t* __restrict__ rp, int M) {
-  float dist = 0.0f;
-  if ((M & 15) == 0) {
-    const uint4* rp4 = reinterpret_cast<const uint4*>(rp);
-    for (int c16 = 0; c16 < M / 16; ++c16) {
-      const uint4 v = __ldg(rp4 + c16);
-      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
-      const float* l0 = lut + c16 * 16 * 256;
-#pragma unroll
-      for (int aa = 0; aa < 4; ++aa)
-#pragma unroll
-        for (int bb = 0; bb < 4; ++bb)
-          dist = f_add(dist, l0[(aa * 4 + bb) * 256 + ((w[aa] >> (8 * bb)) & 0xff)]);
-    }
-  } else {
-    for (int m = 0; m < M; ++m) dist = f_add(dist, lut[m * 256 + rp[m]]);
-  }
-  return dist;
 }
 
 // The 4-bit quantisation range (qmax - qmin) / 255 and the dequantisation q * range + qmin as x86 (where the reference
