@@ -580,7 +580,50 @@ lb2_status lb2_index_hnsw_pq_info(const lb2_index* index, uint32_t* max_level, u
 lb2_status lb2_index_export_hnsw_pq(const lb2_index* index, uint8_t* levels_out, uint32_t* counts0_out,
                                     uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
                                     uint32_t* neighbors_up_out, float* dists_up_out);
-/* lb2_index_search_hnsw takes an IVF_HNSW_SQ or an IVF_HNSW_PQ index. */
+
+/* ---- IVF_HNSW_FLAT: IVFIndex<HNSW, FlatQuantizer> (rust/lance/src/index/vector.rs:473-493) -----------------------
+ * An IVF_FLAT index (same IVF stage, vectors and row ids for the same arguments) with an HNSW graph per partition over
+ * the partition's FlatFloatStorage (lance-index/src/vector/flat/storage.rs:31-185,345-410): the stored rows as they
+ * are, normalised under cosine by the IVF transformer, no residuals.  Levels, insertion order, tie handling, the graph
+ * layout, ef, the prefilter switch and the refusals are IVF_HNSW_SQ's (above).  The storage keeps the index's distance
+ * type, cosine included (builder.rs:841, flat/storage.rs:108-158,353-366), and every distance is the one
+ * lb2_index_search on IVF_FLAT computes for the pair: the column's stored element type (f32 / f16 / bf16; u8 held as
+ * f32) with 16 f32 lanes under L2 and dot, and under cosine 16 f32 FMA lanes for <q, y> and <y, y>, the xor tree and
+ * 1 - xy / |q| / sqrt(yy), |q| the query role's norm from the same 16 FMA lanes:
+ *  - query to node (search): the (normalised) query in the query role;
+ *  - node to node while node i is inserted (dist_calculator_from_id): node i in the query role; these are the
+ *    distances in the lists;
+ *  - the heuristic (hnsw.rs:82): dist_between(u, v) with the candidate u in the query role and the accepted neighbour
+ *    v as the row.  Cosine is not symmetric in its rounding, so the orientation is part of the definition.
+ * The graph crosses the ABI in IVF_HNSW_SQ's layout. */
+typedef struct {
+  lb2_ivfflat_build_params flat;
+  uint32_t max_level;       /* HnswBuildParams (hnsw/builder.rs:63-72): 7 */
+  uint32_t m;               /* 20; level 0 keeps up to 2m neighbours, the others m */
+  uint32_t ef_construction; /* 150 */
+} lb2_ivfhnswflat_build_params;
+void lb2_ivfhnswflat_build_params_default(lb2_ivfhnswflat_build_params* p);
+/* IvfIndexBuilder<HNSW, FlatQuantizer>::build: lb2_ivfflat_build, then every partition's graph on the device (one warp
+ * per partition, the largest partitions first); the level draws use params->flat.seed.  The graph stage is counted in
+ * stats->ms_total only.  A communicator of more than one rank is LB2_UNSUPPORTED. */
+lb2_status lb2_ivfhnswflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                                 const lb2_ivfhnswflat_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                                 lb2_build_stats* stats);
+/* attach a graph (host or device arrays in the IVF_HNSW_SQ layout) to an IVF_FLAT index made by lb2_index_create_flat +
+ * lb2_index_load_flat; the checks of lb2_index_load_hnsw_sq.  lb2_index_load_flat, lb2_index_update and
+ * lb2_index_repartition refuse an index that has a graph. */
+lb2_status lb2_index_load_hnsw_flat(lb2_index* index, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                                    const uint8_t* levels, const uint32_t* counts0, const uint32_t* neighbors0,
+                                    const float* dists0, const uint32_t* counts_up, const uint32_t* neighbors_up,
+                                    const float* dists_up);
+/* as lb2_index_hnsw_sq_info / lb2_index_export_hnsw_sq for an IVF_HNSW_FLAT index; lb2_index_export_flat exports its
+ * IVF_FLAT part */
+lb2_status lb2_index_hnsw_flat_info(const lb2_index* index, uint32_t* max_level, uint32_t* m,
+                                    uint32_t* ef_construction, uint64_t* num_upper_rows);
+lb2_status lb2_index_export_hnsw_flat(const lb2_index* index, uint8_t* levels_out, uint32_t* counts0_out,
+                                      uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
+                                      uint32_t* neighbors_up_out, float* dists_up_out);
+/* lb2_index_search_hnsw takes an IVF_HNSW_SQ, IVF_HNSW_PQ or IVF_HNSW_FLAT index. */
 
 /* ---- IVF_RQ: IVFIndex<FlatIndex, RabitQuantizer> (lance-index/src/vector/bq/) ------------------------------------
  * create_index(.., "IVF_RQ") builds an IvfIndexBuilder<FlatIndex, RabitQuantizer> (rust/lance/src/index/vector.rs:

@@ -14,7 +14,8 @@ import numpy as np
 from ._lib import (BF16, COSINE, DOT, F16, F32, L2, METRICS, U8, BuildParams, BuildStats, FlatBuildParams,
                    DeviceArray, KMeansParams as _CKMeansParams, LanceB200Error, PinnedArray,
                    PQParams as _CPQParams, RqBuildParams as _CRqBuildParams, SqBuildParams as _CSqBuildParams,
-                   HnswSqBuildParams as _CHnswSqBuildParams, HnswPqBuildParams as _CHnswPqBuildParams, as_ptr,
+                   HnswSqBuildParams as _CHnswSqBuildParams, HnswPqBuildParams as _CHnswPqBuildParams,
+                   HnswFlatBuildParams as _CHnswFlatBuildParams, as_ptr,
                    check, device_count, lib)
 
 __all__ = ["device_count", "DeviceArray", "PinnedArray", "LanceB200Error", "train_kmeans",
@@ -22,7 +23,7 @@ __all__ = ["device_count", "DeviceArray", "PinnedArray", "LanceB200Error", "trai
            "l2_distance_batch", "dot_distance_batch", "cosine_distance_batch", "PQBuildParams", "ProductQuantizer",
            "build_distance_table_l2", "compute_pq_distance", "flat_topk", "flat_search", "IvfPqIndex",
            "IvfBuildParams", "IvfFlatIndex", "SQBuildParams", "ScalarQuantizer", "IvfSqIndex", "HnswBuildParams",
-           "IvfHnswSqIndex", "IvfHnswPqIndex", "RQBuildParams",
+           "IvfHnswSqIndex", "IvfHnswPqIndex", "IvfHnswFlatIndex", "RQBuildParams",
            "RabitQuantizer", "IvfRqIndex", "launch_count", "profile"]
 
 
@@ -994,10 +995,10 @@ class HnswBuildParams:
 
 
 class _HnswGraphs:
-    """The graph half of IvfHnswSqIndex and IvfHnswPqIndex: attach, export and search with ef=.  search,
-    search_refine, search_ex and search_probed take ef= (lb2_index_search_hnsw); the other search methods use
+    """The graph half of IvfHnswSqIndex, IvfHnswPqIndex and IvfHnswFlatIndex: attach, export and search with ef=.
+    search, search_refine, search_ex and search_probed take ef= (lb2_index_search_hnsw); the other search methods use
     k' + k' / 2."""
-    _KIND = None   # "sq" or "pq": the suffix of the kind's C entry points
+    _KIND = None   # "sq", "pq" or "flat": the suffix of the kind's C entry points
 
     @classmethod
     def _need_graph(cls, graph):
@@ -1005,7 +1006,7 @@ class _HnswGraphs:
             raise ValueError(f"{cls.__name__}.from_parts needs graph= (the dict export()['graph'] returns)")
 
     def _attach_graph(self, graph):
-        """lb2_index_load_hnsw_sq / _pq of a dict as export()["graph"] returns"""
+        """lb2_index_load_hnsw_sq / _pq / _flat of a dict as export()["graph"] returns"""
         g = graph
         arr = {k: np.ascontiguousarray(g[k], dtype=t) for k, t in (
             ("levels", np.uint8), ("counts0", np.uint32), ("neighbors0", np.uint32), ("dists0", np.float32),
@@ -1206,6 +1207,55 @@ class IvfHnswPqIndex(_HnswGraphs, IvfPqIndex):
         rp, _k = as_ptr(rid)
         check(lib().lb2_index_load(h, C.c_void_p(part_ids.ctypes.data), C.c_void_p(codes.ctypes.data), rp,
                                    C.c_uint64(part_ids.size)))
+        ix._attach_graph(graph)
+        return ix
+
+
+class IvfHnswFlatIndex(_HnswGraphs, IvfFlatIndex):
+    """Device-resident IVFIndex<HNSW, FlatQuantizer> (IVF_HNSW_FLAT): IVF_FLAT's partitions, vectors and row ids with
+    an HNSW graph per partition over the stored rows (lance-index/src/vector/flat/storage.rs).  Every distance, cosine
+    included, is the one IVF_FLAT's scan computes for the pair; the heuristic's dist_between(u, v) puts the candidate
+    u in the query role (include/lance_b200.h).  search, search_refine, search_ex and search_probed take ef=; the
+    other search methods use k' + k' / 2."""
+    _KIND = "flat"
+
+    @classmethod
+    def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
+              centroids=None, row_ids=None, bf16=False, hnsw_params=None):
+        """create_index(.., "IVF_HNSW_FLAT"); the IVF stage, vectors and row ids equal IvfFlatIndex.build's with the
+        same arguments.  The graphs' level draws use `seed`.  bf16=True: uint16 bfloat16 bit patterns."""
+        hnsw_params = hnsw_params or HnswBuildParams()
+        data, dt = _typed(data, bf16)
+        n, d = data.shape
+        bp = _CHnswFlatBuildParams()
+        lib().lb2_ivfhnswflat_build_params_default(C.byref(bp))
+        f = bp.flat
+        f.num_partitions = num_partitions
+        f.ivf.max_iters, f.ivf.sample_rate, f.ivf.seed, f.seed = max_iters, sample_rate, seed, seed
+        bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
+        keep = None
+        if centroids is not None:
+            keep = _f32(centroids)
+            bp.flat.ivf.init_centroids = as_ptr(keep)[0].value
+        rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
+                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
+        h = C.c_void_p()
+        st = BuildStats()
+        dp, _k1 = as_ptr(data)
+        rp, _k2 = as_ptr(rid)
+        check(lib().lb2_ivfhnswflat_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt),
+                                          C.c_int(_metric(distance_type)), C.byref(bp), rp, C.byref(h), C.byref(st)))
+        ix = cls(h, st)
+        ix._dt = dt
+        return ix
+
+    @classmethod
+    def from_parts(cls, centroids, part_ids, vectors, row_ids=None, distance_type="l2", bf16=False, graph=None):
+        """IvfFlatIndex.from_parts plus `graph` (as export()["graph"] returns) over the rows in partition order.  The
+        centroids may also be f32 as export() returns them for a bf16 column (their bits are kept)."""
+        cls._need_graph(graph)
+        centroids = _model_arr(centroids, BF16 if bf16 else _typed(vectors)[1])
+        ix = super().from_parts(centroids, part_ids, vectors, row_ids, distance_type, bf16)
         ix._attach_graph(graph)
         return ix
 

@@ -63,6 +63,11 @@ class HnswPqBuildParams(C.Structure):
     _fields_ = [("pq", BuildParams), ("max_level", C.c_uint32), ("m", C.c_uint32), ("ef_construction", C.c_uint32)]
 
 
+class HnswFlatBuildParams(C.Structure):
+    """lb2_ivfhnswflat_build_params (include/lance_b200.h)."""
+    _fields_ = [("flat", FlatBuildParams), ("max_level", C.c_uint32), ("m", C.c_uint32), ("ef_construction", C.c_uint32)]
+
+
 class RqBuildParams(C.Structure):
     """lb2_ivfrq_build_params (include/lance_b200.h)."""
     _fields_ = [("num_partitions", C.c_uint32), ("ivf", KMeansParams), ("num_bits", C.c_uint32),
@@ -95,7 +100,8 @@ EXPORTS = [
     "lb2_ivfrq_build_params_default", "lb2_ivfrq_build", "lb2_index_create_rq", "lb2_index_load_rq",
     "lb2_index_export_rq", "lb2_index_search_probed", "lb2_flat_search", "lb2_index_search_combined",
     "lb2_ivfhnswpq_build_params_default", "lb2_ivfhnswpq_build", "lb2_index_load_hnsw_pq", "lb2_index_hnsw_pq_info",
-    "lb2_index_export_hnsw_pq",
+    "lb2_index_export_hnsw_pq", "lb2_ivfhnswflat_build_params_default", "lb2_ivfhnswflat_build",
+    "lb2_index_load_hnsw_flat", "lb2_index_hnsw_flat_info", "lb2_index_export_hnsw_flat",
 ]
 
 _lib = None
@@ -120,7 +126,8 @@ def lib():
                             "lb2_kmeans_params_default", "lb2_pq_params_default",
                             "lb2_ivfpq_build_params_default", "lb2_ivfflat_build_params_default",
                             "lb2_ivfsq_build_params_default", "lb2_ivfrq_build_params_default",
-                            "lb2_ivfhnswsq_build_params_default", "lb2_ivfhnswpq_build_params_default"):
+                            "lb2_ivfhnswsq_build_params_default", "lb2_ivfhnswpq_build_params_default",
+                            "lb2_ivfhnswflat_build_params_default"):
                 getattr(L, name).restype = C.c_int
         L.lb2_sq_encode.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_int, C.c_double, C.c_double, C.c_void_p]
         L.lb2_index_create_sq.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int, C.c_int, C.c_double,

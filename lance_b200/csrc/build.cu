@@ -343,6 +343,13 @@ void lb2_ivfhnswpq_build_params_default(lb2_ivfhnswpq_build_params* p) {
   p->ef_construction = 150;
 }
 
+void lb2_ivfhnswflat_build_params_default(lb2_ivfhnswflat_build_params* p) {
+  lb2_ivfflat_build_params_default(&p->flat);
+  p->max_level = 7;  // HnswBuildParams::default (hnsw/builder.rs:63-72)
+  p->m = 20;
+  p->ef_construction = 150;
+}
+
 void lb2_ivfrq_build_params_default(lb2_ivfrq_build_params* p) {
   p->num_partitions = 256;
   lb2_kmeans_params_default(&p->ivf);
@@ -770,6 +777,28 @@ lb2_status lb2_ivfhnswpq_build(const void* data, uint64_t n, uint32_t d, lb2_dty
     hnsw_build_pq(g, ix->part_offsets.p, ix->K, ix->codes.p, ix->codebook.p, (int)d, ix->M, ix->nbits, ix->metric,
                   dtype, params->pq.seed);
   });
+  *out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_ivfhnswflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                                 const lb2_ivfhnswflat_build_params* params, const uint64_t* row_ids, lb2_index** out,
+                                 lb2_build_stats* stats) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(data && params && out, "null argument");
+  check_hnsw_params("IVF_HNSW_FLAT", params->max_level, params->m, params->ef_construction);
+  if (comm_nranks() > 1) fail(LB2_UNSUPPORTED, "IVF_HNSW_FLAT: a build over more than one rank is not implemented");
+  // 1. the IVF stage, vectors and row ids of IVF_FLAT with the same arguments
+  lb2_index* flat = nullptr;
+  const lb2_status st = lb2_ivfflat_build(data, n, d, dtype, metric, &params->flat, row_ids, &flat, stats);
+  if (st != LB2_OK) return st;  // its message is already the last error
+  std::unique_ptr<lb2_index> ix(flat);
+  // 2. HNSW::index_vectors per partition over its FlatFloatStorage (IvfIndexBuilder<HNSW, FlatQuantizer>)
+  attach_graphs(ix.get(), "IVF_HNSW_FLAT", params->max_level, params->m, params->ef_construction, stats,
+                [&](HnswGraph& g) {
+                  hnsw_build_flat(g, ix->part_offsets.p, ix->K, ix->vectors.p, (int)ix->vdtype(), (int)d, ix->metric,
+                                  params->flat.seed);
+                });
   *out = ix.release();
   LB2_API_END
 }

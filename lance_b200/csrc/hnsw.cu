@@ -1,18 +1,21 @@
-// hnsw.cu -- IVF_HNSW_SQ and IVF_HNSW_PQ: an HNSW graph per partition over the partition's SQ or PQ codes, built and
-// searched on the device (lance-index/src/vector/hnsw/builder.rs, graph.rs, hnsw.rs, graph/builder.rs).
+// hnsw.cu -- IVF_HNSW_SQ, IVF_HNSW_PQ and IVF_HNSW_FLAT: an HNSW graph per partition over the partition's SQ codes, PQ
+// codes or raw vectors, built and searched on the device (lance-index/src/vector/hnsw/builder.rs, graph.rs, hnsw.rs,
+// graph/builder.rs).
 //
 // Replaces  HNSW::index_vectors / HnswBuilder::insert      hnsw/builder.rs:386-507,742-775
 //           select_neighbors_heuristic                   hnsw.rs:60-88
 //           beam_search / greedy_search                  graph.rs:275-409
 //           HNSW::search / search_inner / flat_search    hnsw/builder.rs:164-280,678-739
 //
-// The engine is generic over a distance policy (SqDist, PqDist below), as the reference is over VectorStore: `key`
-// is the distance of the query (or of the inserting node) to a node, `between` the heuristic's dist_between.
+// The engine is generic over a distance policy (SqDist, PqDist, FlatDist below), as the reference is over
+// VectorStore: `key` is the distance of the query (or of the inserting node) to a node, `between` the heuristic's
+// dist_between.
 //  * SQ: both are the SQ row rule of sq.cuh (sq/storage.rs:387-444, storage.rs:102-105): an integer sum times one
 //    constant, so the build is deterministic and bit-exact.
 //  * PQ (pq/storage.rs:675-919): `key` sums a lookup table over the node's codes; the table is the residual query's
 //    at search time and, while a node is inserted, the table of the node's own decoded codes (dist_calculator_from_id);
 //    `between` is the full-width distance of the two decoded rows (dist_between).
+//  * FLAT (flat/storage.rs:345-410): all three are the IVF_FLAT scan's rule on the stored rows, cosine included.
 //
 // One warp owns one partition (build) or one (query, partition) slot (search).  Its heaps, visited bitset and (PQ)
 // table live in a per-warp global scratch sized by the largest partition, so no partition is refused for its size.
@@ -61,9 +64,10 @@ __device__ __forceinline__ ListRef list_of(const GraphDev& g, uint64_t row, int 
   return {g.cntu + r, g.nbru + r * g.m, g.dstu + r * g.m};
 }
 
-// per-warp scratch (u32 words): PQ table tab[TW] and query / decoded row qv[QW] (none for SQ), vis[words(nmax)],
+// per-warp scratch (u32 words): PQ table tab[TW] (PQ only) and query / row qv[QW] (PQ and flat), vis[words(nmax)],
 // candidate heap ck / cid [nmax + 1], result heap rk / rid [E + 1], batch bid / bk [B], list lid / lk / ord [LB],
-// accepted aid / ak [B].  With a table the warp's share is a multiple of 4 words, so tab and qv stay 16-byte aligned.
+// accepted aid / ak [B].  With a table or a query buffer the warp's share is a multiple of 4 words, so tab and qv
+// stay 16-byte aligned (TW and QW are multiples of 4).
 struct Scratch {
   float *tab, *qv;
   uint32_t *vis, *ck, *cid, *rk, *rid, *bid, *bk, *lid, *lk, *ord, *aid, *ak;
@@ -72,7 +76,7 @@ __host__ __device__ inline size_t scratch_words(uint64_t nmax, uint32_t E, uint3
                                                 uint32_t QW = 0) {
   const size_t w = (size_t)TW + QW + (nmax + 31) / 32 + 2 * (nmax + 1) + 2 * ((size_t)E + 1) + 4 * (size_t)B +
                    3 * (size_t)LB;
-  return TW ? (w + 3) & ~(size_t)3 : w;
+  return TW || QW ? (w + 3) & ~(size_t)3 : w;
 }
 __device__ inline Scratch scratch_at(uint32_t* base, uint64_t nmax, uint32_t E, uint32_t B, uint32_t LB,
                                      uint32_t TW = 0, uint32_t QW = 0) {
@@ -120,7 +124,7 @@ struct SqDist {
   uint64_t off;          // its first storage position
   uint32_t n;
   using Ctx = const uint8_t*;
-  static constexpr bool TABLE = false;  // no table or query rows in the scratch
+  static constexpr bool TABLE = false, QUERY = false;  // no table or query rows in the scratch
   __device__ __forceinline__ void bind(uint64_t o, uint32_t cnt) {
     off = o;
     n = cnt;
@@ -155,7 +159,7 @@ struct PqDist {
   uint64_t off;
   uint32_t n;
   using Ctx = const float*;  // the table
-  static constexpr bool TABLE = true;
+  static constexpr bool TABLE = true, QUERY = true;
   __device__ __forceinline__ void bind(uint64_t o, uint32_t cnt) {
     off = o;
     n = cnt;
@@ -203,6 +207,173 @@ struct PqDist {
       });
     return ukey_of(fold_partials<RULE, METRIC>([&](int i) { return acc[i].a; }, [&](int i) { return acc[i].b; },
                                                [](int) { return 0u; }, acc[0].s, 0.0f));
+  }
+};
+
+// IVF_HNSW_FLAT's row access: 4 elements from a multiple of 4 as f32.  An IVF_FLAT row holds d % 4 == 0 elements, so
+// they are one aligned 16-byte (f32) or 8-byte (16-bit) load; a 16-bit row that starts on 16 bytes reads 8 at a time.
+struct ScratchRow {  // the query or inserting row in the warp's scratch: written by the warp, so not read through __ldg
+  const float* p;
+  __device__ __forceinline__ void get4(int e, float* o) const {
+    const float4 v = *reinterpret_cast<const float4*>(p + e);
+    o[0] = v.x, o[1] = v.y, o[2] = v.z, o[3] = v.w;
+  }
+  __device__ __forceinline__ void get16(int e, float* o) const {
+#pragma unroll
+    for (int t = 0; t < 16; t += 4) get4(e + t, o + t);
+  }
+};
+__device__ __forceinline__ void unpack2(uint32_t w, const __half*, float* o) {
+  o[0] = __half2float(__ushort_as_half((unsigned short)(w & 0xffffu)));
+  o[1] = __half2float(__ushort_as_half((unsigned short)(w >> 16)));
+}
+__device__ __forceinline__ void unpack2(uint32_t w, const __nv_bfloat16*, float* o) {
+  o[0] = __uint_as_float(w << 16);
+  o[1] = __uint_as_float(w & 0xffff0000u);
+}
+template <class T>
+struct StoredRow {  // a stored f16 / bf16 row
+  const T* p;
+  bool a16;  // the row starts on 16 bytes
+  __device__ __forceinline__ static StoredRow at(const T* r) {
+    return {r, (reinterpret_cast<uintptr_t>(r) & 15) == 0};
+  }
+  __device__ __forceinline__ void get4(int e, float* o) const {
+    const uint2 w = __ldg(reinterpret_cast<const uint2*>(p + e));
+    unpack2(w.x, p, o);
+    unpack2(w.y, p, o + 2);
+  }
+  __device__ __forceinline__ void get16(int e, float* o) const {
+    if (a16) {
+#pragma unroll
+      for (int t = 0; t < 16; t += 8) {
+        const uint4 w = __ldg(reinterpret_cast<const uint4*>(p + e + t));
+        unpack2(w.x, p, o + t);
+        unpack2(w.y, p, o + t + 2);
+        unpack2(w.z, p, o + t + 4);
+        unpack2(w.w, p, o + t + 6);
+      }
+    } else {
+#pragma unroll
+      for (int t = 0; t < 16; t += 4) get4(e + t, o + t);
+    }
+  }
+};
+template <>
+struct StoredRow<float> {
+  const float* p;
+  __device__ __forceinline__ static StoredRow at(const float* r) { return {r}; }
+  __device__ __forceinline__ void get4(int e, float* o) const {
+    const float4 v = __ldg(reinterpret_cast<const float4*>(p + e));
+    o[0] = v.x, o[1] = v.y, o[2] = v.z, o[3] = v.w;
+  }
+  __device__ __forceinline__ void get16(int e, float* o) const {
+#pragma unroll
+    for (int t = 0; t < 16; t += 4) get4(e + t, o + t);
+  }
+};
+
+// The IVF_FLAT scan's rule (scan_rule<METRIC>) of one (query role q, row v) pair on one lane.  The lane walks both rows
+// once, 16 elements at a time, into the rule's 16 LaneAccs in registers: element e goes to accumulator e % 16, as
+// lane e % 16 of a half-warp takes it in row_distance, and the 16-lane rule's d % 16 tail goes to the sequential sum,
+// so every accumulator sees its elements in the rule's order.  QNORM: q's norm is accumulated in the same walk
+// (norm_l2's 16 FMA lanes, xor tree, sqrt, as ivfflat_scan_kernel computes the query's); otherwise q_norm is used.
+template <int METRIC, bool QNORM, class QR, class VR>
+__device__ __forceinline__ float lane_pair_distance(const QR& q, const VR& v, int d, float q_norm) {
+  constexpr int RULE = scan_rule<METRIC>();
+  LaneAcc<RULE, METRIC> acc[16];
+  float qq[16];
+#pragma unroll
+  for (int l = 0; l < 16; ++l) qq[l] = 0.0f;
+  const int n16 = d & ~15;
+  for (int c = 0; c < n16; c += 16) {
+    float a[16], b[16];
+    q.get16(c, a);
+    v.get16(c, b);
+#pragma unroll
+    for (int l = 0; l < 16; ++l) {
+      acc[l].template step<0>(a[l], b[l]);
+      if (QNORM) qq[l] = fmaf(a[l], a[l], qq[l]);
+    }
+  }
+#pragma unroll
+  for (int g = 0; g < 3; ++g) {  // the d % 16 rest, 4 elements at a time
+    const int e = n16 + 4 * g;
+    if (e < d) {
+      float a[4], b[4];
+      q.get4(e, a);
+      v.get4(e, b);
+#pragma unroll
+      for (int t = 0; t < 4; ++t) {
+        if constexpr (RULE == RULE_COSINE) {
+          acc[4 * g + t].template step<0>(a[t], b[t]);
+          if (QNORM) qq[4 * g + t] = fmaf(a[t], a[t], qq[4 * g + t]);
+        } else {
+          acc[0].template step<2>(a[t], b[t]);
+        }
+      }
+    }
+  }
+  if (RULE == RULE_COSINE && QNORM) q_norm = sqrtf(tree16([&](int i) { return qq[i]; }));
+  return fold_partials<RULE, METRIC>([&](int i) { return acc[i].a; }, [&](int i) { return acc[i].b; },
+                                     [](int) { return 0u; }, acc[0].s, q_norm);
+}
+
+// IVF_HNSW_FLAT over FlatFloatStorage (flat/storage.rs:31-185,345-410): the stored rows as they are (normalised under
+// cosine by the IVF transformer), and every distance FlatDistanceCal's distance_type.func() with the index's own
+// type, cosine included (storage.rs:108-158, flat/storage.rs:353-366).  Each is the IVF_FLAT scan's rule for the
+// column type, on one lane, so a list distance is bit-identical to the distance IVF_FLAT's scan gives the pair:
+//  * key: the context (the query, or the inserting node's row, as f32 in qv, with its norm) to a node
+//    (dist_calculator / dist_calculator_from_id);
+//  * between: dist_between(u, v) with u in the query role (hnsw.rs:82, storage.rs:102-105): cosine rounds the two
+//    norms separately, so the orientation matters.
+template <int METRIC, class T>
+struct FlatDist {
+  const T* base;          // the index's vectors [n][d]
+  const float* queries;   // the slab's queries [qn][d] (search; normalised under cosine)
+  int d;
+  const T* rows;          // the partition's first row
+  uint64_t off;
+  uint32_t n;
+  struct Ctx {
+    const float* q;  // the row in qv
+    float norm;      // its norm (cosine)
+  };
+  static constexpr bool TABLE = false, QUERY = true;
+  __device__ __forceinline__ void bind(uint64_t o, uint32_t cnt) {
+    off = o;
+    n = cnt;
+    rows = base + o * d;
+  }
+  __device__ __forceinline__ StoredRow<T> row(uint32_t i) const { return StoredRow<T>::at(rows + (uint64_t)i * d); }
+  // the norm of the row in qv with ivfflat_scan_kernel's 16 FMA lanes, xor tree and sqrt (norm_l2.rs:106-130)
+  __device__ __forceinline__ Ctx ctx_of_qv(const Scratch& s) const {
+    __syncwarp();
+    float nrm = 0.0f;
+    if (METRIC == METRIC_COSINE) {
+      float a = 0.0f;
+      for (int e = threadIdx.x & 15; e < d; e += 16) a = fmaf(s.qv[e], s.qv[e], a);
+#pragma unroll
+      for (int o = 8; o >= 1; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o, 16);
+      nrm = sqrtf(a);
+    }
+    return {s.qv, nrm};
+  }
+  __device__ __forceinline__ Ctx node_ctx(uint32_t i, const Scratch& s) const {
+    const T* r = rows + (uint64_t)i * d;
+    for (int e = threadIdx.x & 31; e < d; e += 32) s.qv[e] = ldf<T>(r, e);
+    return ctx_of_qv(s);
+  }
+  __device__ __forceinline__ Ctx query_ctx(uint64_t qi, uint32_t, const Scratch& s) const {
+    const float* q = queries + qi * d;
+    for (int e = threadIdx.x & 31; e < d; e += 32) s.qv[e] = q[e];
+    return ctx_of_qv(s);
+  }
+  __device__ __forceinline__ uint32_t key(const Ctx& c, uint32_t node) const {
+    return ukey_of(lane_pair_distance<METRIC, false>(ScratchRow{c.q}, row(node), d, c.norm));
+  }
+  __device__ __forceinline__ uint32_t between(uint32_t u, uint32_t v) const {
+    return ukey_of(lane_pair_distance<METRIC, true>(row(u), row(v), d, 0.0f));
   }
 };
 
@@ -397,7 +568,8 @@ hnsw_build_kernel(GraphDev g, const uint64_t* __restrict__ part_offsets, const u
                   uint32_t QW) {
   __shared__ uint32_t sh_part, sh_go, sh_n;
   const int lane = threadIdx.x & 31;
-  if (!Dist::TABLE) TW = QW = 0;
+  if (!Dist::TABLE) TW = 0;
+  if (!Dist::QUERY) QW = 0;
   const Scratch s = scratch_at(scratch + blockIdx.x * scratch_words(nmax, E, B, LB, TW, QW), nmax, E, B, LB, TW, QW);
   for (;;) {
     if (lane == 0) sh_part = atomicAdd(next, 1u);
@@ -465,7 +637,8 @@ hnsw_search_kernel(GraphDev g, uint64_t nslots, int np, const uint32_t* __restri
                    uint32_t* __restrict__ scratch, uint64_t nmax, uint32_t E, uint32_t B, uint32_t TW, uint32_t QW) {
   __shared__ uint32_t sh_n;
   const int lane = threadIdx.x & 31;
-  if (!Dist::TABLE) TW = QW = 0;
+  if (!Dist::TABLE) TW = 0;
+  if (!Dist::QUERY) QW = 0;
   const Scratch s = scratch_at(scratch + blockIdx.x * scratch_words(nmax, E, B, 0, TW, QW), nmax, E, B, 0, TW, QW);
   for (uint64_t slot = blockIdx.x; slot < nslots; slot += gridDim.x) {
     const uint64_t qi = slot / np;
@@ -651,13 +824,27 @@ static void dispatch_pq(int metric, int nbits, lb2_dtype dtype, F&& f) {
   }
 }
 
-// the words of a PQ warp's table (M x 2^nbits) and of its query / decoded row (d, kept 16-byte aligned)
+// the words of a PQ warp's table (M x 2^nbits) and of a PQ or flat warp's query / row (d, kept 16-byte aligned)
 static uint32_t pq_table_words(int M, int nbits) { return (uint32_t)M << nbits; }
-static uint32_t pq_query_words(int d) { return (uint32_t)(d + 3) & ~3u; }
+static uint32_t query_words(int d) { return (uint32_t)(d + 3) & ~3u; }
+
+void hnsw_build_flat(HnswGraph& g, const uint64_t* part_offsets, int K, const void* vectors, int vdt, int d, int metric,
+                     uint64_t seed) {
+  build_graphs(g, part_offsets, K, seed, 0, query_words(d), [&](auto go) {
+    dispatch_metric_elem<false>(metric, vdt, [&](auto m, auto e) {
+      using T = typename decltype(e)::type;
+      using Dist = FlatDist<decltype(m)::value, T>;
+      Dist P{};
+      P.base = static_cast<const T*>(vectors);
+      P.d = d;
+      go(hnsw_build_kernel<Dist>, P);
+    });
+  });
+}
 
 void hnsw_build_pq(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, const float* codebook,
                    int d, int M, int nbits, int metric, lb2_dtype dtype, uint64_t seed) {
-  build_graphs(g, part_offsets, K, seed, pq_table_words(M, nbits), pq_query_words(d), [&](auto go) {
+  build_graphs(g, part_offsets, K, seed, pq_table_words(M, nbits), query_words(d), [&](auto go) {
     dispatch_pq(metric, nbits, dtype, [&](auto m, auto b, auto r) {
       using Dist = PqDist<decltype(m)::value, decltype(b)::value, decltype(r)::value>;
       Dist P{};
@@ -809,7 +996,7 @@ void hnsw_search(const IvfSearch& s, const HnswGraph& g, const uint8_t* codes, f
 
 void hnsw_search_pq(const IvfSearch& s, const HnswGraph& g, const float* codebook, int M, int nbits,
                     const uint8_t* codes, uint32_t ef) {
-  search_graphs(s, g, ef, pq_table_words(M, nbits), pq_query_words(s.d), [&](const ScanSlots& sl, auto go) {
+  search_graphs(s, g, ef, pq_table_words(M, nbits), query_words(s.d), [&](const ScanSlots& sl, auto go) {
     // the search never calls `between`: one rule per (metric, nbits)
     dispatch_pq(s.metric, nbits, LB2_F32, [&](auto m, auto b, auto r) {
       using Dist = PqDist<decltype(m)::value, decltype(b)::value, decltype(r)::value>;
@@ -822,6 +1009,20 @@ void hnsw_search_pq(const IvfSearch& s, const HnswGraph& g, const float* codeboo
       P.M = M;
       P.ds = s.d / M;
       P.cw = nbits == 4 ? M / 2 : M;
+      go(hnsw_search_kernel<Dist>, P);
+    });
+  });
+}
+
+void hnsw_search_flat(const IvfSearch& s, const HnswGraph& g, const void* vectors, int vdt, uint32_t ef) {
+  search_graphs(s, g, ef, 0, query_words(s.d), [&](const ScanSlots& sl, auto go) {
+    dispatch_metric_elem<false>(s.metric, vdt, [&](auto m, auto e) {
+      using T = typename decltype(e)::type;
+      using Dist = FlatDist<decltype(m)::value, T>;
+      Dist P{};
+      P.base = static_cast<const T*>(vectors);
+      P.queries = s.queries + sl.q0 * s.d;
+      P.d = s.d;
       go(hnsw_search_kernel<Dist>, P);
     });
   });

@@ -1,5 +1,5 @@
-// hnsw.cuh -- the per-partition HNSW graphs of IVF_HNSW_SQ and IVF_HNSW_PQ (lance-index/src/vector/hnsw/builder.rs)
-// and their device layout; internal interface of hnsw.cu
+// hnsw.cuh -- the per-partition HNSW graphs of IVF_HNSW_SQ, IVF_HNSW_PQ and IVF_HNSW_FLAT
+// (lance-index/src/vector/hnsw/builder.rs) and their device layout; internal interface of hnsw.cu
 #pragma once
 #include <stdint.h>
 
@@ -14,7 +14,7 @@ struct IvfSearch;
 // Lists keep the reference's order of level_neighbors_ranked (graph/builder.rs:33-48); the distances are those of
 // the ranked list.  Node 0 of every partition has max_level levels and is the entry point (builder.rs:354-376).
 struct HnswGraph {
-  const char* kind = "IVF_HNSW_SQ";  // the index kind's name in messages: IVF_HNSW_SQ or IVF_HNSW_PQ
+  const char* kind = "IVF_HNSW_SQ";  // the index kind's name in messages: IVF_HNSW_SQ, IVF_HNSW_PQ or IVF_HNSW_FLAT
   int max_level = 0, m = 0, ef_construction = 0;
   uint64_t max_part = 0;  // rows of the largest partition (scratch sizing)
   uint64_t n_up = 0;      // upper-level rows
@@ -45,6 +45,10 @@ void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t
 // the rule of `dtype` (pq/storage.rs:675-841)
 void hnsw_build_pq(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, const float* codebook,
                    int d, int M, int nbits, int metric, lb2_dtype dtype, uint64_t seed);
+// the same over IVF_FLAT's stored rows [n][d] in element type `vdt` (f32, f16 or bf16): every distance, cosine
+// included, is the IVF_FLAT scan's rule (flat/storage.rs:345-410)
+void hnsw_build_flat(HnswGraph& g, const uint64_t* part_offsets, int K, const void* vectors, int vdt, int d, int metric,
+                     uint64_t seed);
 // a graph from the caller's arrays in the layout above (host or device memory), checked against the partitions
 void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* levels, const uint32_t* counts0,
                const uint32_t* nbr0, const float* dist0, const uint32_t* counts_up, const uint32_t* nbr_up,
@@ -55,4 +59,6 @@ void hnsw_search(const IvfSearch& s, const HnswGraph& g, const uint8_t* codes, f
 // the same over PQ codes: each slot's table is the IVF_PQ scan's table of the (residual) query
 void hnsw_search_pq(const IvfSearch& s, const HnswGraph& g, const float* codebook, int M, int nbits,
                     const uint8_t* codes, uint32_t ef);
+// the same over IVF_FLAT's stored rows: each slot scores rows with the IVF_FLAT scan's rule for the (normalised) query
+void hnsw_search_flat(const IvfSearch& s, const HnswGraph& g, const void* vectors, int vdt, uint32_t ef);
 }  // namespace lb2

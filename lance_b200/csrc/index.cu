@@ -306,7 +306,10 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
   DevBuf<uint8_t> qcodes;
   switch (index->kind) {
     case IndexKind::FLAT:
-      ivfflat_search(s, index->vectors.p, (int)index->vdtype());
+      if (index->hnsw)  // IVF_HNSW_FLAT: the IVF_FLAT scan's distances, searched through each partition's graph
+        hnsw_search_flat(s, *index->hnsw, index->vectors.p, (int)index->vdtype(), ef);
+      else
+        ivfflat_search(s, index->vectors.p, (int)index->vdtype());
       break;
     case IndexKind::RQ:
       // the (normalised) query's residual to each probed centroid is rotated (v2.rs:316-332, bq/storage.rs:407-445)
@@ -539,6 +542,7 @@ lb2_status lb2_index_load_flat(lb2_index* index, const uint32_t* part_ids, const
                                const uint64_t* row_ids, uint64_t n) {
   LB2_API_BEGIN
   LB2_REQUIRE(index && index->kind == IndexKind::FLAT, "not an IVF_FLAT index");
+  LB2_REQUIRE(!index->hnsw, "lb2_index_load_flat: the IVF_HNSW_FLAT index already has an HNSW graph over its rows");
   LB2_REQUIRE(index->d % 4 == 0, "IVF_FLAT needs a dimension that is a multiple of 4");
   InArg<uint32_t> p(part_ids, n);
   InArg<uint64_t> r(row_ids, n);
@@ -604,12 +608,13 @@ lb2_status lb2_index_export_sq(const lb2_index* index, void* centroids_out, doub
 
 }  // extern "C"
 
-// lb2_index_load_hnsw_sq / _pq: a graph over the rows of an index of `kind`
+// lb2_index_load_hnsw_sq / _pq / _flat: a graph over the rows of an index of `kind`
 static void load_hnsw(lb2_index* index, IndexKind kind, const char* name, uint32_t max_level, uint32_t m,
                       uint32_t ef_construction, const uint8_t* levels, const uint32_t* counts0,
                       const uint32_t* neighbors0, const float* dists0, const uint32_t* counts_up,
                       const uint32_t* neighbors_up, const float* dists_up) {
-  LB2_REQUIRE(index && index->kind == kind, "not an %s index", kind == IndexKind::SQ ? "IVF_SQ" : "IVF_PQ");
+  LB2_REQUIRE(index && index->kind == kind, "not an %s index",
+              kind == IndexKind::SQ ? "IVF_SQ" : kind == IndexKind::PQ ? "IVF_PQ" : "IVF_FLAT");
   LB2_REQUIRE(max_level >= 1 && max_level <= 64 && m >= 1 && m <= 1024, "%s: max_level %u or m %u out of range", name,
               max_level, m);
   std::unique_ptr<HnswGraph> g(new HnswGraph());
@@ -673,6 +678,16 @@ lb2_status lb2_index_load_hnsw_pq(lb2_index* index, uint32_t max_level, uint32_t
   LB2_API_END
 }
 
+lb2_status lb2_index_load_hnsw_flat(lb2_index* index, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                                    const uint8_t* levels, const uint32_t* counts0, const uint32_t* neighbors0,
+                                    const float* dists0, const uint32_t* counts_up, const uint32_t* neighbors_up,
+                                    const float* dists_up) {
+  LB2_API_BEGIN
+  load_hnsw(index, IndexKind::FLAT, "IVF_HNSW_FLAT", max_level, m, ef_construction, levels, counts0, neighbors0,
+            dists0, counts_up, neighbors_up, dists_up);
+  LB2_API_END
+}
+
 lb2_status lb2_index_hnsw_sq_info(const lb2_index* index, uint32_t* max_level, uint32_t* m, uint32_t* ef_construction,
                                   uint64_t* num_upper_rows) {
   LB2_API_BEGIN
@@ -684,6 +699,13 @@ lb2_status lb2_index_hnsw_pq_info(const lb2_index* index, uint32_t* max_level, u
                                   uint64_t* num_upper_rows) {
   LB2_API_BEGIN
   hnsw_info(graph_of(index, IndexKind::PQ, "IVF_HNSW_PQ"), max_level, m, ef_construction, num_upper_rows);
+  LB2_API_END
+}
+
+lb2_status lb2_index_hnsw_flat_info(const lb2_index* index, uint32_t* max_level, uint32_t* m,
+                                    uint32_t* ef_construction, uint64_t* num_upper_rows) {
+  LB2_API_BEGIN
+  hnsw_info(graph_of(index, IndexKind::FLAT, "IVF_HNSW_FLAT"), max_level, m, ef_construction, num_upper_rows);
   LB2_API_END
 }
 
@@ -701,6 +723,15 @@ lb2_status lb2_index_export_hnsw_pq(const lb2_index* index, uint8_t* levels_out,
                                     uint32_t* neighbors_up_out, float* dists_up_out) {
   LB2_API_BEGIN
   export_hnsw(index, graph_of(index, IndexKind::PQ, "IVF_HNSW_PQ"), levels_out, counts0_out, neighbors0_out,
+              dists0_out, counts_up_out, neighbors_up_out, dists_up_out);
+  LB2_API_END
+}
+
+lb2_status lb2_index_export_hnsw_flat(const lb2_index* index, uint8_t* levels_out, uint32_t* counts0_out,
+                                      uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
+                                      uint32_t* neighbors_up_out, float* dists_up_out) {
+  LB2_API_BEGIN
+  export_hnsw(index, graph_of(index, IndexKind::FLAT, "IVF_HNSW_FLAT"), levels_out, counts0_out, neighbors0_out,
               dists0_out, counts_up_out, neighbors_up_out, dists_up_out);
   LB2_API_END
 }
@@ -823,7 +854,7 @@ lb2_status lb2_index_search_hnsw(lb2_index* index, const void* queries, uint64_t
                                  uint32_t* counts_out, uint32_t* nprobes_out) {
   LB2_API_BEGIN
   LB2_REQUIRE(sp && index, "null argument");
-  LB2_REQUIRE(index->hnsw, "not an IVF_HNSW_SQ or IVF_HNSW_PQ index");
+  LB2_REQUIRE(index->hnsw, "not an IVF_HNSW_SQ, IVF_HNSW_PQ or IVF_HNSW_FLAT index");
   LB2_REQUIRE(!nprobes_out || pp, "nprobes_out needs probe parameters");
   if (pp) {
     ProbedSearch ps(sp, pp, nq, nprobes_out);
@@ -969,6 +1000,8 @@ lb2_status lb2_index_update(const lb2_index* old, const void* new_centroids, uin
                             const uint32_t* add_part_ids, const uint8_t* add_codes, const uint64_t* add_row_ids,
                             uint64_t n_add, const uint64_t* remove_row_ids, uint64_t n_remove, lb2_index** out) {
   LB2_API_BEGIN
+  if (old && old->kind == IndexKind::FLAT && old->hnsw)
+    fail(LB2_UNSUPPORTED, "lb2_index_update: IVF_HNSW_FLAT indexes are not implemented");
   LB2_REQUIRE(old && out && old->kind == IndexKind::PQ, "lb2_index_update takes an IVF_PQ index");
   if (old->hnsw) fail(LB2_UNSUPPORTED, "lb2_index_update: IVF_HNSW_PQ indexes are not implemented");
   LB2_REQUIRE(new_k > 0 && (new_centroids || new_k == (uint32_t)old->K), "a changed partition count needs new centroids");

@@ -32,8 +32,8 @@ struct lb2_index {
   // d * nbits), with the per-row factors rq_add / rq_scale [n] and the rotation rq_rot [code_dim][code_dim]
   // (bq/storage.rs:110-121)
   lb2::DevBuf<float> rq_rot, rq_add, rq_scale;
-  // IVF_HNSW_SQ / IVF_HNSW_PQ: an IVF_SQ / IVF_PQ index with an HNSW graph per partition over its codes (hnsw.cuh),
-  // searched through the graphs instead of the flat scan
+  // IVF_HNSW_SQ / IVF_HNSW_PQ / IVF_HNSW_FLAT: an IVF_SQ / IVF_PQ / IVF_FLAT index with an HNSW graph per partition
+  // over its codes or vectors (hnsw.cuh), searched through the graphs instead of the partition scan
   std::unique_ptr<lb2::HnswGraph> hnsw;
   int code_dim() const { return d * nbits; }
   size_t codebook_len() const { return ((size_t)1 << nbits) * d; }
