@@ -508,7 +508,8 @@ lb2_status lb2_index_export_sq(const lb2_index* index, void* centroids_out, doub
  * The graph crosses the ABI in the device layout: levels[n] (levels per row), level 0 dense (counts0[n],
  * neighbors0 / dists0 [n][2m]) and the upper levels node by node in storage order: a row with L levels owns L - 1
  * consecutive upper rows, levels 1 .. L-1 (counts_up[r], neighbors_up / dists_up [r][m]).  Lists are in the order of
- * level_neighbors_ranked (graph/builder.rs:33-48); neighbour ids are partition-local. */
+ * level_neighbors_ranked (graph/builder.rs:33-48); neighbour ids are partition-local.  A built graph's slots past
+ * a list's count hold zeros. */
 typedef struct {
   lb2_ivfsq_build_params sq;
   uint32_t max_level;       /* HnswBuildParams (hnsw/builder.rs:63-72): 7 */

@@ -550,9 +550,14 @@ __device__ void prune_into(const Dist& P, const uint32_t* ids, const uint32_t* k
     __syncwarp();
   }
   if (lane == 0) {
+    const uint32_t old = *dst.cnt;  // a back-link prune can shorten the list: the slots it drops go back to zero
     for (uint32_t j = 0; j < na; ++j) {
       dst.ids[j] = s.aid[j];
       dst.dist[j] = float_of(s.ak[j]);
+    }
+    for (uint32_t j = na; j < old; ++j) {
+      dst.ids[j] = 0;
+      dst.dist[j] = 0.0f;
     }
     *dst.cnt = na;
   }
