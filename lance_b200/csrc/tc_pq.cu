@@ -13,9 +13,11 @@
 //     top-3 of  r.c - |c|^2/2  over the 128 codeword PAIRS (c, c ^ 1) of the row (tc_common.cuh: column units) and
 //     classifies the row against tau = 3*2^-10 (|r_m|^2 + max|c_m|^2) (with the norm floor of cert_tau) like
 //     tc_assign.cu: flag 0 certifies the two codewords of the best pair, flag 1 the four of the two best;
-//   * flag 0/1 rows are decided IN THE EPILOGUE: each certified codeword gets the reference-order f32 distance
-//     from the operands that are still in shared memory (sequential 8-term sum, l2.rs:69-79; strict-< / lowest
-//     index);
+//   * the top 3 of each (row, sub-space) are parked in shared memory, and once an item's sub-spaces have been
+//     through the tournament, one converged DECISION PASS per warp classifies its 16 rows x 4 sub-spaces (all
+//     32 lanes, two pairs per lane): each certified codeword of a flag 0/1 pair gets the reference-order f32
+//     distance from the operands still in shared memory (sequential 8-term sum, l2.rs:69-79; strict-< / lowest
+//     index), as four independent chains; the item's stage is released after that pass;
 //   * flag 2 (row, sub-space) pairs are appended to a list and finished by pq_fallback_kernel
 //     (half-warp per pair, exact scan of all 256 codewords).
 #include "assign.cuh"
@@ -38,10 +40,12 @@ constexpr int STREAM_STAGE_BYTES = A_STAGE_BYTES + B_CHUNK_BYTES + CNH_CHUNK_BYT
 
 // One TMA producer warpgroup and CONSUMERS warpgroups that take the work items in turns.  The epilogue is bound by
 // the ALU pipe (per 128 scores of a lane 64 pair maxima, 64 packs and about 210 min/max of the pair tournament,
-// against 128 adds on the FMA pipe), and a consumer warp stalls often (wgmma waits, the divergent decision code, barrier waits, the
-// shuffles of top3_finish); the resident variant runs four consumers (4 warps per scheduler) so that the others
-// fill those stalls.  The streamed ring (44 KB per stage) has no room for more than four stages, so the streamed
-// variant keeps two consumers.
+// against 128 adds on the FMA pipe), and a consumer warp stalls often (wgmma waits, barrier waits, the shuffles of
+// top3_finish); the resident variant runs four consumers (4 warps per scheduler) so that the others fill those
+// stalls.  The decisions of an item run as one converged pass after its tournaments, with no MMA in flight: run
+// under the next item's first MMA instead, the pass holds a second stage per consumer, and the ring's slack lost
+// that way cost more than the overlap won (65 536-row training calls on an H100).  The streamed ring (44 KB per stage) has no room for more than four stages, so the streamed variant keeps two
+// consumers.
 // ACC_SETS: 64-register accumulator sets of a consumer.  With two, the tournament of one 128-codeword half runs
 // while the MMA of the next is in flight; they do not fit the 112 registers of four consumers without spills,
 // so there one half is computed at a time and the other warpgroups fill the MMA latency.
@@ -61,14 +65,20 @@ struct Pipe {
                 "register file");
 };
 
-// RESIDENT: [B: nkc x 32 KB][A ring: STAGES x 8 KB][cnh: M x 1 KB]
-// STREAM:   [ring: STAGES x (A 8 KB | B chunk 32 KB | cnh slice 4 KB)]
+// The parked tournament results of one consumer warp: the top 3 of its 16 rows for the item's 4 sub-spaces, as
+// [sub-space j][rank][row] (row-minor: the decision pass's half-warps read sub-spaces j and j + 2, 48 words apart,
+// so that their 16 rows fall on distinct banks)
+constexpr int PARK_WARP_FLOATS = 4 * 3 * 16;  // 768 B
+constexpr uint32_t SMEM_OPTIN = 227 * 1024;   // H100: the opt-in dynamic shared memory of one block
+
+// RESIDENT: [B: nkc x 32 KB][A ring: STAGES x 8 KB][cnh: M x 1 KB][bars][cbm][misc][park: 4 CONSUMERS x 768 B]
+// STREAM:   [ring: STAGES x (A 8 KB | B chunk 32 KB | cnh slice 4 KB)][bars][cbm][misc][park]
 struct Layout {
-  uint32_t b_off, a_off, cnh_off, bar_off, cbm_off, misc_off, total;
+  uint32_t b_off, a_off, cnh_off, bar_off, cbm_off, misc_off, park_off, total;
   uint32_t stage_bytes;  // distance between two A stages
 };
-__host__ __device__ inline Layout layout(int nkc, int M, bool stream) {
-  Layout L;
+__host__ __device__ constexpr Layout layout(int nkc, int M, bool stream) {
+  Layout L{};
   if (stream) {
     L.b_off = A_STAGE_BYTES;                  // + s * stage_bytes
     L.a_off = 0;                              // + s * stage_bytes
@@ -85,9 +95,13 @@ __host__ __device__ inline Layout layout(int nkc, int M, bool stream) {
   static_assert((2 * Pipe<false>::STAGES + 1) * 8 <= 256 && (2 * Pipe<true>::STAGES + 1) * 8 <= 256, "barriers");
   L.cbm_off = L.bar_off + 256;              // max_c |c|^2 per sub-space
   L.misc_off = L.cbm_off + MAX_M * 4;
-  L.total = L.misc_off + MAX_M;  // one "active" byte per sub-space
+  L.park_off = L.misc_off + MAX_M;  // after one "active" byte per sub-space
+  L.total = L.park_off + (stream ? Pipe<true>::CONSUMERS : Pipe<false>::CONSUMERS) * 4 * PARK_WARP_FLOATS * 4;
   return L;
 }
+// the largest shape of each variant, with the 1 KB that aligning the base to 1024 may take (tc_pq_assign)
+static_assert(layout(MAX_M_RESIDENT / 4, MAX_M_RESIDENT, false).total + 1024 <= SMEM_OPTIN, "resident layout");
+static_assert(layout(MAX_M / 4, MAX_M, true).total + 1024 <= SMEM_OPTIN, "streamed layout");
 
 // 1-D bulk copy global -> shared with mbarrier completion (the streamed -|c|^2/2 slice)
 __device__ __forceinline__ void bulk_load_1d(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
@@ -183,14 +197,95 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
       }
     }
   } else {
-    // ===== consumers: per active sub-space two wgmmas (K = 8, one per 128-codeword half), top-3, exact re-rank =====
-    // Each half is its own wgmma group.  No MMA is in flight during the divergent decision code: the compiler
-    // would serialize every wgmma of the kernel otherwise.
+    // ===== consumers: per active sub-space two wgmmas (K = 8, one per 128-codeword half) and the top-3
+    // tournament; per item one converged decision pass (every lane works, fixed trip counts) =====
+    // Each half is its own wgmma group.
     setmaxnreg_inc<P::CONSUMER_REGS>();
     const uint32_t w = (threadIdx.x >> 7) - 1;
     if (!STREAM) mbar_wait(b_full, 0);
     const int h = lane & 1;      // lanes 0 / 1 of the quad finish rows r0 / r0 + 8
-    const int rl = frag_row(h);  // row inside the tile
+    const int wrow = 16 * (warp & 3);  // the warp's 16 rows inside the tile
+    float* park = reinterpret_cast<float*>(smem + L.park_off) + (warp - 4) * PARK_WARP_FLOATS;
+    // decision pass: lane l decides row wrow + (l & 15) for sub-spaces dj + 2 d, d = 0, 1
+    const int drow = lane & 15, dj = lane >> 4;
+    // The flags, exact re-ranks and outputs of the item (tile, kc) in stage s for the warp's 16 rows and the item's
+    // active sub-spaces, from the parked top 3; rn = |r_m|^2 of the lane's two pairs.  Releases the stage.
+    auto decide_item = [&](uint32_t tile, int kc, int s, const float (&rn)[2]) {
+      __syncwarp();  // the parked results of the other lanes
+      const uint32_t cm = chunk_mask(kc);
+      const uint8_t* atile = smem + L.a_off + s * L.stage_bytes;
+      const uint8_t* bt = smem + L.b_off + (STREAM ? s * L.stage_bytes : kc * B_CHUNK_BYTES);
+      const uint32_t row = tile * TM + wrow + drow;  // n < 2^32 (n * M < 2^32)
+      const bool in = row < n;
+      uint32_t code2 = 0;  // encode: the lane's two codes at their byte positions of the row's 4-code word
+#pragma unroll
+      for (int d = 0; d < 2; ++d) {
+        const int j = dj + 2 * d, m = kc * 4 + j;
+        const float* pk = park + j * 48 + drow;
+        const float m1 = pk[0], m2 = pk[16], m3 = pk[32];
+        const float tau = cert_tau(0.0029296875f, rn[d] + cbm_s[m]);
+        // flag 0 certifies pair 1, flag 1 pairs 1 and 2; two pairs with the same score bits are duplicated
+        // codewords: such rows keep their route through pq_fallback_kernel, which handles any multiplicity
+        // (tests/test_assignment_routes.py pins the routes)
+        const bool f0 = m1 - m2 > tau;
+        const bool f1 = !f0 && m1 - m3 > tau && ((__float_as_uint(m1) ^ __float_as_uint(m2)) >> 8) != 0;
+        const bool live = in && ((cm >> j) & 1u);
+        // the low byte is a PAIR of columns (2p, 2p + 1), p < 128
+        const uint32_t p1 = __float_as_uint(m1) & 0x7Fu, p2 = __float_as_uint(m2) & 0x7Fu;
+        const uint32_t plo = f0 ? p1 : min(p1, p2), phi = max(p1, p2);
+        // exact, reference-order distances of four columns as independent chains; in ascending column order the
+        // certified ones (two under flag 0, four under flag 1) are ranked by strict < (the lowest index wins a tie)
+        const float4 r0 = *swz(atile, wrow + drow, j * 2), r1 = *swz(atile, wrow + drow, j * 2 + 1);
+        const float rv[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
+        float v[4];
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const int ci = (int)(2 * (c < 2 ? plo : phi) + (c & 1));
+          const float4 c0v = *swz(bt, ci, j * 2), c1v = *swz(bt, ci, j * 2 + 1);
+          const float cv[8] = {c0v.x, c0v.y, c0v.z, c0v.w, c1v.x, c1v.y, c1v.z, c1v.w};
+          float sacc = 0.0f;
+#pragma unroll
+          for (int t = 0; t < 8; ++t) sacc = f_add(sacc, sq_diff(rv[t], cv[t]));
+          v[c] = f_add(sacc, 0.0f);
+        }
+        float bv = __int_as_float(0x7f800000);
+        uint32_t bi = 0xffffffffu;
+#pragma unroll
+        for (int c = 0; c < 4; ++c) {
+          const bool better_c = (c < 2 || !f0) && v[c] < bv;
+          bv = better_c ? v[c] : bv;
+          bi = better_c ? 2 * (c < 2 ? plo : phi) + (c & 1) : bi;
+        }
+        const bool ok = bi != 0xffffffffu, decided = live && (f0 || f1);
+        if (TRAIN) {
+          if (decided) {  // consecutive lanes: consecutive rows of one sub-space
+            ids[(uint64_t)m * n + row] = ok ? bi : 0u;
+            dists[(uint64_t)m * n + row] = ok ? bv : __int_as_float(0x7fc00000);
+            valid[(uint64_t)m * n + row] = ok ? 1 : 0;
+          }
+        } else {
+          // an undecided pair's byte is rewritten by pq_fallback_kernel
+          code2 |= (ok ? bi & 0xFFu : 0u) << (8 * j);
+        }
+        // undecided pairs join sub-space m's list: one atomic per half-warp (= sub-space), ranks by popc.  Their
+        // order inside the list is free: pq_fallback_kernel decides every listed pair on its own
+        const uint32_t und = (__ballot_sync(0xffffffffu, live && !f0 && !f1) >> (16 * dj)) & 0xFFFFu;
+        const int lead = und ? __ffs(und) - 1 : 0;
+        uint32_t base = 0;
+        if (und && drow == lead) base = atomicAdd(fb_count + m, (uint32_t)__popc(und));
+        base = __shfl_sync(0xffffffffu, base, 16 * dj + lead);
+        if ((und >> drow) & 1u) fb_pairs[(size_t)m * n + base + __popc(und & ((1u << drow) - 1))] = row;
+      }
+      if (!TRAIN) {
+        // the row's four codes as one aligned word (codes is [n][M], M % 4 == 0); encode has every sub-space active
+        const uint32_t word = code2 | __shfl_xor_sync(0xffffffffu, code2, 16);
+        const bool rv_ok = in && (row_valid ? row_valid[row] != 0 : true);
+        if (in && dj == 0) *reinterpret_cast<uint32_t*>(codes + row * (uint64_t)M + 4 * kc) = rv_ok ? word : 0u;
+      }
+      // this warp's pass has read the stage and the parked results
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty_bar(s));
+    };
     float acc[P::ACC_SETS][64];
     uint32_t k = 0;  // ring index of the items with an active sub-space
     for (uint64_t item = blockIdx.x; item < num_tiles * nkc; item += gridDim.x) {
@@ -203,87 +298,43 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
       const uint32_t ph = (k / STAGES) & 1;
       ++k;
       if (!mine) continue;
-      const uint64_t row = tile * TM + rl;
-      const bool decides = (lane & 3) < 2 && row < n;
-      // |r_m|^2 of the item's four sub-spaces (contiguous, 16-byte aligned: M % 4 == 0), fetched before the MMAs
-      float4 rn4 = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-      if (decides) rn4 = *reinterpret_cast<const float4*>(rn2 + row * M + 4 * kc);
+      // |r_m|^2 of the lane's two decision pairs, fetched before the MMAs
+      float rn[2] = {0.0f, 0.0f};
+      {
+        const uint64_t row = tile * TM + wrow + drow;
+        if (row < n) {
+          rn[0] = rn2[row * M + 4 * kc + dj];
+          rn[1] = rn2[row * M + 4 * kc + dj + 2];
+        }
+      }
       mbar_wait(full_bar(s), ph);
-      const uint8_t* atile = smem + L.a_off + s * L.stage_bytes;
       const uint8_t* bt = smem + L.b_off + (STREAM ? s * L.stage_bytes : kc * B_CHUNK_BYTES);
       const float* cn4 = reinterpret_cast<const float*>(smem + L.cnh_off + (STREAM ? s * L.stage_bytes : kc * CNH_CHUNK_BYTES));
-      const uint32_t a_addr = smem_u32(atile), b_addr = smem_u32(bt);
-      // flag, exact re-rank and outputs of the row for sub-space j, from its top 3 (mm); no MMA is in flight
-      auto decide = [&](int j, const float (&mm)[3]) {
-        const int m = kc * 4 + j;
-        if (decides) {
-          const float m1 = mm[0], m2 = mm[1], m3 = mm[2];
-          const float rn = j == 0 ? rn4.x : j == 1 ? rn4.y : j == 2 ? rn4.z : rn4.w;
-          const float cbm = cbm_s[m];
-          const float tau = cert_tau(0.0029296875f, rn + cbm);
-          uint32_t flag = 2;
-          if (m1 - m2 > tau) flag = 0;
-          // two pairs with the same score bits are duplicated codewords: such rows keep their route through
-          // pq_fallback_kernel, which handles any multiplicity (tests/test_assignment_routes.py pins the routes)
-          else if (m1 - m3 > tau && ((__float_as_uint(m1) ^ __float_as_uint(m2)) >> 8) != 0) flag = 1;
-          // the low byte is a PAIR of columns (2p, 2p + 1): flag 0 certifies pair 1, flag 1 pairs 1 and 2
-          const uint32_t p1 = __float_as_uint(m1) & 0xFFu, p2 = __float_as_uint(m2) & 0xFFu;
-          uint32_t best_idx = 0;
-          float best_val = 0.0f;
-          bool ok = true;
-          if (flag == 2) {
-            fb_pairs[(size_t)m * n + atomicAdd(fb_count + m, 1u)] = (uint32_t)row;  // per-sub-space list
-          } else {
-            // exact, reference-order distances of the certified columns, in ascending column order, from the
-            // operands still in shared memory
-            const float4 r0 = *swz(atile, rl, j * 2), r1 = *swz(atile, rl, j * 2 + 1);
-            const float rv[8] = {r0.x, r0.y, r0.z, r0.w, r1.x, r1.y, r1.z, r1.w};
-            float bv = __int_as_float(0x7f800000);
-            uint32_t bi = 0xffffffffu;
-            const uint32_t plo = flag == 0 ? p1 : min(p1, p2), phi = max(p1, p2);
-            const int ncand = flag == 0 ? 2 : 4;
-            for (int c = 0; c < ncand; ++c) {
-              const uint32_t ci = 2 * (c < 2 ? plo : phi) + (c & 1);
-              const float4 c0v = *swz(bt, (int)ci, j * 2), c1v = *swz(bt, (int)ci, j * 2 + 1);
-              const float cv[8] = {c0v.x, c0v.y, c0v.z, c0v.w, c1v.x, c1v.y, c1v.z, c1v.w};
-              float sacc = 0.0f;
-  #pragma unroll
-              for (int t = 0; t < 8; ++t) sacc = f_add(sacc, sq_diff(rv[t], cv[t]));
-              const float vv = f_add(sacc, 0.0f);
-              if (vv < bv) { bv = vv; bi = ci; }  // strict <: the lowest index wins a tie
-            }
-            ok = bi != 0xffffffffu;
-            best_idx = ok ? bi : 0u;
-            best_val = bv;
-          }
-          if (flag != 2) {
-            if (TRAIN) {
-              ids[(uint64_t)m * n + row] = best_idx;
-              dists[(uint64_t)m * n + row] = ok ? best_val : __int_as_float(0x7fc00000);
-              valid[(uint64_t)m * n + row] = ok ? 1 : 0;
-            } else {
-              const bool rv_ok = row_valid ? row_valid[row] != 0 : true;
-              codes[row * (uint64_t)M + m] = (ok && rv_ok) ? (uint8_t)best_idx : (uint8_t)0;
-            }
-          }
-        }
-      };
+      const uint32_t a_addr = smem_u32(smem + L.a_off + s * L.stage_bytes), b_addr = smem_u32(bt);
       // half `hf` of sub-space j into d: codewords 128 hf .. 128 hf + 127 are B rows 128 hf.. (128 B each)
       auto issue = [&](float* d, int j, int hf) {
-        __syncwarp();  // wgmma is warp-aligned: reconverge after the divergent re-rank and barrier polls
+        __syncwarp();  // wgmma is warp-aligned: reconverge after the barrier polls
         acc_fence<64>(d);
         wgmma_fence();
         wgmma_tf32_n128(d, make_desc(a_addr + j * 32), make_desc(b_addr + hf * (TN / 2) * 128 + j * 32), 0u);
         wgmma_commit();
       };
+      uint32_t rest = cm;
+      int j = __ffs(rest) - 1;
+      rest &= rest - 1;
+      issue(acc[0], j, 0);
+      if constexpr (P::ACC_SETS == 2) issue(acc[1], j, 1);
+      // the finished top 3 of sub-space j, row r0 + 8 (lane & 1): every lane of the quad holds it, and both lanes of
+      // a row store it (the same value; no divergent code while the next sub-space's MMA is in flight)
+      auto park_top3 = [&](int j, const float (&mm)[3]) {
+        float* pk = park + j * 48 + (lane >> 2) + 8 * h;
+        pk[0] = mm[0];
+        pk[16] = mm[1];
+        pk[32] = mm[2];
+      };
       if constexpr (P::ACC_SETS == 2) {
         // the tournament of half 0 runs while half 1 is in flight, and that of half 1 while the next sub-space's
         // half 0, issued into the registers just read, is
-        uint32_t rest = cm;
-        int j = __ffs(rest) - 1;
-        rest &= rest - 1;
-        issue(acc[0], j, 0);
-        issue(acc[1], j, 1);
         for (;;) {
           const int jn = rest ? __ffs(rest) - 1 : -1;  // next active sub-space of the item
           Tour tour;
@@ -301,7 +352,7 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
           float mm[3];
           top3_finish<UNIT>(tour, mm);
           wgmma_wait<0>();
-          decide(j, mm);
+          park_top3(j, mm);
           if (jn < 0) break;
           issue(acc[1], jn, 1);
           j = jn;
@@ -309,10 +360,8 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
         }
       } else {
         // one half at a time, into the same registers
-        for (uint32_t rest = cm; rest; rest &= rest - 1) {
-          const int j = __ffs(rest) - 1;
+        for (;;) {
           Tour tour;
-          issue(acc[0], j, 0);
           wgmma_wait<0>();
           acc_fence<64>(acc[0]);
           top3_half<0, UNIT>(acc[0], cn4 + j * TN, tour);
@@ -322,12 +371,15 @@ tc_pq_kernel(const __grid_constant__ CUtensorMap map_r, const __grid_constant__ 
           top3_half<1, UNIT>(acc[0], cn4 + j * TN, tour);
           float mm[3];
           top3_finish<UNIT>(tour, mm);
-          decide(j, mm);
+          park_top3(j, mm);
+          if (!rest) break;
+          j = __ffs(rest) - 1;
+          rest &= rest - 1;
+          issue(acc[0], j, 0);
         }
       }
-      // every MMA of the item has completed (wait_group 0 above) and this warp's re-ranks have read the stage
-      __syncwarp();
-      if (lane == 0) mbar_arrive(empty_bar(s));
+      // every MMA of the item has completed
+      decide_item((uint32_t)tile, kc, s, rn);
     }
   }
 }
@@ -529,6 +581,7 @@ void tc_pq_assign(const float* r, const float* rn2, uint64_t n, int d, int M, co
   const Layout L = layout(nkc, M, stream);
   const size_t smem = L.total + 1024;
   if (smem > ctx().smem_optin) fail(LB2_UNSUPPORTED, "tc_pq: shared memory");
+  LB2_REQUIRE(!(codes && active), "tc_pq: encode decides every sub-space");
   if (!prepared) tc_pq_prepare(codebook, M, d, ws);  // also resets the undecided-row lists
   if (ws->fb_pairs.n < n * M) ws->fb_pairs.alloc(n * M);
   const CUtensorMap map_r = make_map_2d(r, n, d, tc::TM);
@@ -570,7 +623,8 @@ void tc_pq_assign(const float* r, const float* rn2, uint64_t n, int d, int M, co
 void pq_encode_dev(const float* x, uint64_t n, int d, int M, int ds, const float* codebook, int metric,
                    const float* cent, const uint32_t* part, const uint8_t* row_valid, uint8_t* codes) {
   if (n == 0) return;
-  if (!tc_pq_supported(n, d, M, ds, 256, metric, x)) {
+  // (the filter stores a row's four codes of a chunk as one word)
+  if (!tc_pq_supported(n, d, M, ds, 256, metric, x) || (reinterpret_cast<uintptr_t>(codes) & 3) != 0) {
     small_d_assign_f32(x, n, d, M, ds, codebook, 256, metric, cent, part, row_valid, codes, nullptr,
                        nullptr, nullptr, nullptr);
     return;
