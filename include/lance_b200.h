@@ -370,6 +370,64 @@ lb2_status lb2_index_update(const lb2_index* old_index, const void* new_centroid
                             const uint32_t* part_map, const uint32_t* add_part_ids, const uint8_t* add_codes,
                             const uint64_t* add_row_ids, uint64_t n_add, const uint64_t* remove_row_ids,
                             uint64_t n_remove, lb2_index** out);
+/* ---- optimize / remap of every index kind ----------------------------------------------------------------------
+ * lb2_index_transform: IvfTransformer::transform with the index's own model (lance-index/src/vector/ivf.rs:149-328),
+ * the "new rows" half of shuffle_data during an optimize (rust/lance/src/index/vector/builder.rs:685-829).  vectors
+ * [n][d] in the index's element type; per row the partition id, the payload the kind stores ([n][row_bytes]) and
+ * valid (0 = a row the kind's build drops: KeepFiniteVectors, transform.rs:112-159).  The payload is exactly what the
+ * kind's build stores for the same row:
+ *   IVF_PQ   the codes of lb2_ivfpq_transform (row_bytes M, or M / 2 for 4-bit codes);
+ *   IVF_FLAT the row, normalised under cosine, in the stored element type (u8 columns held as f32; row_bytes d * 4
+ *            or d * 2);
+ *   IVF_SQ   scale_to_u8 of the (normalised) row with the index's bounds (sq.rs:263-277; row_bytes d);
+ *   IVF_RQ   the codes and factors of lb2_ivfrq_transform (row_bytes d * num_bits / 8).
+ * The graph kinds transform as their base kind does.  Every output may be NULL; add_out / scale_out must be NULL
+ * unless the index is IVF_RQ. */
+lb2_status lb2_index_transform(const lb2_index* index, const void* vectors, uint64_t n, uint32_t* part_out,
+                               uint8_t* payload_out, float* add_out, float* scale_out, uint8_t* valid_out);
+/* lb2_index_optimize: the merge of IvfIndexBuilder::build_partitions / take_partition_batches (builder.rs:685-935)
+ * composed with IvfIndexBuilder::remap (builder.rs:256-359), for every kind; returns a NEW index of the old one's
+ * kind.  In this order:
+ *   1. the old rows in storage order, minus the ids in remove_row_ids and the partitions part_map sends to
+ *      UINT32_MAX; the rest move to part_map[p] (nullable = identity);
+ *   2. the add list appended (payload as lb2_index_transform writes it; IVF_RQ: with its factors, required);
+ *   3. a stable grouping by partition: inside a partition the surviving old rows first, then the added rows in list
+ *      order (lb2_index_update's order);
+ *   4. the row-id mapping applied to every row, old and added, without changing the order (storage.remap,
+ *      pq/storage.rs:499-540, bq/storage.rs:661): an id mapped to UINT64_MAX (None) is dropped, an id mapped to a
+ *      value is rewritten, an id that is not in remap_old_ids is kept as it is.
+ * The model stays: codebook, SQ bounds and RQ rotation; new_centroids (in the model's element type) replaces the
+ * centroids, and new_k must equal the old k without them.  As with lb2_index_update the caller is responsible for the
+ * centroids: an old partition whose centroid changes must come back through the add list (removed from the old rows
+ * by part_map or remove_row_ids), because its PQ residual codes or RQ factors were computed against the old centroid.
+ * Graphs (IVF_HNSW_*): the new index has one per partition iff the old one has, with the old max_level, m and
+ * ef_construction.  A new partition whose rows are all the rows of one old partition q, in the same order, with none of
+ * q's rows removed or remapped to None and nothing added, keeps q's graph verbatim (every node id and distance depends
+ * only on the partition's payload sequence; the reference's rebuild, hnsw/builder.rs:777-785, gives the same graph
+ * up to its unseeded level draws).  Every other partition with at least 2 rows gets the graph of the kind's build over
+ * its new storage, its level draws keyed by (seed, new partition id, node).
+ * LB2_INVALID_ARG before the new index is made: remap_old_ids not strictly ascending, a part id or part_map entry at or
+ * above new_k, missing or extra RQ factors, a changed new_k without new_centroids, more than 2^32 - 1 rows.  Under a
+ * communicator the non-graph kinds merge each shard's rows (as lb2_index_update); the graph kinds return
+ * LB2_UNSUPPORTED with more than one rank. */
+typedef struct {
+  const void* new_centroids; /* [new_k][d], nullable */
+  uint32_t new_k;
+  const uint32_t* part_map;  /* [old k], nullable = identity; UINT32_MAX = drop the old partition's rows */
+  const uint32_t* add_part_ids;
+  const uint8_t* add_payload; /* [n_add][row_bytes], as lb2_index_transform writes it */
+  const float* add_rq_add;    /* IVF_RQ: required with n_add > 0; other kinds: must be NULL */
+  const float* add_rq_scale;
+  const uint64_t* add_row_ids;
+  uint64_t n_add;
+  const uint64_t* remove_row_ids; /* sorted ascending */
+  uint64_t n_remove;
+  const uint64_t* remap_old_ids; /* strictly ascending */
+  const uint64_t* remap_new_ids; /* UINT64_MAX = None: the row is dropped */
+  uint64_t n_remap;
+  uint64_t seed;                 /* the level draws of the graphs that are rebuilt */
+} lb2_optimize_params;
+lb2_status lb2_index_optimize(const lb2_index* old_index, const lb2_optimize_params* p, lb2_index** out);
 /* Asynchronous search (SURVEY 8b "Threading": `_async` variants taking a stream/event).  Same
  * arguments and results as lb2_index_search_ex, but the call only ENQUEUES the work on `cuda_stream`
  * (cudaStream_t; NULL = the calling thread's current library stream) and returns: probe selection, LUT

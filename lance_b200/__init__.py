@@ -775,6 +775,80 @@ class IvfPqIndex:
             out._dt = self._dt
         return out
 
+    def _payload_empty(self, n):
+        """an array for n rows of this kind's stored payload, as export() returns it"""
+        i = self.info()
+        return np.empty((n, i["num_sub_vectors"] // 2 if i["num_bits"] == 4 else i["num_sub_vectors"]), np.uint8)
+
+    def transform(self, vectors):
+        """lb2_index_transform: IvfTransformer::transform with this index's model -> dict of part_ids, payload (what
+        the kind stores for each row, as export() holds it), add_factors / scale_factors (IVF_RQ, else None) and valid
+        (False: the kind's build drops the row)."""
+        npdt = {F32: np.float32, F16: np.float16, U8: np.uint8, BF16: np.uint16}[getattr(self, "_dt", F32)]
+        if not isinstance(vectors, (DeviceArray, PinnedArray)):
+            vectors = np.ascontiguousarray(vectors, dtype=npdt)
+        n = vectors.shape[0]
+        rq = isinstance(self, IvfRqIndex)
+        part, valid, payload = np.empty(n, np.uint32), np.empty(n, np.uint8), self._payload_empty(n)
+        add, scale = (np.empty(n, np.float32), np.empty(n, np.float32)) if rq else (None, None)
+        vp, _k = as_ptr(vectors)
+        ptr = [as_ptr(a)[0] if a is not None and a.size else None for a in (part, payload, add, scale, valid)]
+        check(lib().lb2_index_transform(self._h, vp, C.c_uint64(n), *ptr))
+        return dict(part_ids=part, payload=payload, add_factors=add, scale_factors=scale, valid=valid.astype(bool))
+
+    def optimize(self, add_vectors=None, add_row_ids=None, add_part_ids=None, add_payload=None, add_factors=None,
+                 new_centroids=None, part_map=None, remove_row_ids=None, remap=None, seed=0):
+        """lb2_index_optimize: append, remove, re-map partitions and remap row ids into a NEW index of this class.
+        add_vectors: raw rows run through transform() first, rows it marks invalid dropped (KeepFiniteVectors);
+        otherwise add_part_ids / add_payload (/ add_factors = (add, scale) for IVF_RQ) as transform() returns them.
+        remap: {old id: new id or None} or (old ids, new ids) with UINT64_MAX for None.  seed: the level draws of the
+        graphs that are rebuilt (IVF_HNSW_*)."""
+        from ._lib import OptimizeParams
+        if add_vectors is not None:
+            if add_part_ids is not None or add_payload is not None or add_factors is not None:
+                raise ValueError("optimize: pass add_vectors or add_part_ids / add_payload / add_factors, not both")
+            t = self.transform(add_vectors)
+            ok = t["valid"]
+            add_part_ids, add_payload = t["part_ids"][ok], t["payload"][ok]
+            if t["add_factors"] is not None:
+                add_factors = (t["add_factors"][ok], t["scale_factors"][ok])
+            if add_row_ids is not None:
+                add_row_ids = np.asarray(add_row_ids, dtype=np.uint64)[ok]
+        info = self.info()
+        dt = getattr(self, "_dt", F32)
+        cent = None if new_centroids is None else _model_arr(new_centroids, dt)
+        new_k = info["num_partitions"] if cent is None else cent.shape[0]
+        pm = None if part_map is None else np.ascontiguousarray(part_map, dtype=np.uint32)
+        ap = None if add_part_ids is None else np.ascontiguousarray(add_part_ids, dtype=np.uint32)
+        ac = None if add_payload is None else np.ascontiguousarray(add_payload)
+        ar = None if add_row_ids is None else np.ascontiguousarray(add_row_ids, dtype=np.uint64)
+        fa = fs = None
+        if add_factors is not None:
+            fa, fs = (np.ascontiguousarray(f, dtype=np.float32) for f in add_factors)
+        rm = None if remove_row_ids is None else np.sort(np.ascontiguousarray(remove_row_ids, dtype=np.uint64))
+        ro = rn = None
+        if remap is not None:
+            if isinstance(remap, dict):
+                ro = np.fromiter(remap.keys(), np.uint64, len(remap))
+                rn = np.fromiter((0xFFFFFFFFFFFFFFFF if v is None else v for v in remap.values()), np.uint64, len(remap))
+                o = np.argsort(ro, kind="stable")
+                ro, rn = ro[o], rn[o]
+            else:
+                ro, rn = (np.ascontiguousarray(a, dtype=np.uint64) for a in remap)
+        keep = [cent, pm, ap, ac, fa, fs, ar, rm, ro, rn]
+        ptr = [as_ptr(x)[0] if x is not None and x.size else None for x in keep]
+        nz = lambda p: p.value if p is not None else None  # noqa: E731
+        n_add = 0 if ap is None else ap.size
+        p = OptimizeParams(nz(ptr[0]), new_k, nz(ptr[1]), nz(ptr[2]), nz(ptr[3]), nz(ptr[4]), nz(ptr[5]), nz(ptr[6]),
+                           n_add, nz(ptr[7]), 0 if rm is None else rm.size, nz(ptr[8]), nz(ptr[9]),
+                           0 if ro is None else ro.size, seed)
+        h = C.c_void_p()
+        check(lib().lb2_index_optimize(self._h, C.byref(p), C.byref(h)))
+        out = type(self)(h)
+        if hasattr(self, "_dt"):
+            out._dt = self._dt
+        return out
+
     def repartition(self):
         """lb2_index_repartition: row-sharded index -> the index of the partitions this rank owns (p % nranks == rank),
         by one device all-to-all; a copy without a communicator."""
@@ -865,6 +939,10 @@ class IvfFlatIndex(IvfPqIndex):
         vp, _k2 = as_ptr(vectors)
         check(lib().lb2_index_load_flat(h, C.c_void_p(part_ids.ctypes.data), vp, rp, C.c_uint64(part_ids.size)))
         return ix
+
+    def _payload_empty(self, n):
+        return np.empty((n, self.info()["dimension"]),
+                        {F32: np.float32, F16: np.float16, BF16: np.uint16, U8: np.float32}[getattr(self, "_dt", F32)])
 
     def export(self):
         i = self.info()
@@ -970,6 +1048,9 @@ class IvfSqIndex(IvfPqIndex):
         check(lib().lb2_index_load_sq(h, C.c_void_p(part_ids.ctypes.data), C.c_void_p(codes.ctypes.data), rp,
                                       C.c_uint64(part_ids.size)))
         return ix
+
+    def _payload_empty(self, n):
+        return np.empty((n, self.info()["dimension"]), np.uint8)
 
     def export(self):
         i = self.info()
@@ -1362,6 +1443,10 @@ class IvfRqIndex(IvfPqIndex):
                                       C.c_void_p(add.ctypes.data), C.c_void_p(scale.ctypes.data), rp,
                                       C.c_uint64(part_ids.size)))
         return ix
+
+    def _payload_empty(self, n):
+        i = self.info()
+        return np.empty((n, i["dimension"] * i["num_bits"] // 8), np.uint8)
 
     def export(self):
         i = self.info()

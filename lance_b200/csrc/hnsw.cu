@@ -720,14 +720,62 @@ void hnsw_level_thresholds(int m, int max_level, uint64_t* thr) {
   }
 }
 
+// One kept partition of a rebuilt graph: its level-0 block (rows, 2m per row) and its upper block (rows, m per row),
+// each contiguous in both layouts because nodes are in storage order and upper rows are compact.
+struct SpliceSpan {
+  uint64_t old_row, new_row, rows, old_up, new_up, up_rows;
+};
+
+// copies every kept partition's blocks from the old graph to their new offsets (blockIdx.x = the partition, the
+// y blocks and the threads stride over its words); neighbour ids are partition-local, so nothing is rewritten
+__global__ void hnsw_splice_kernel(const SpliceSpan* __restrict__ spans, int m, const uint32_t* __restrict__ cnt0,
+                                   const uint32_t* __restrict__ nbr0, const float* __restrict__ dst0,
+                                   const uint32_t* __restrict__ cntu, const uint32_t* __restrict__ nbru,
+                                   const float* __restrict__ dstu, uint32_t* __restrict__ ocnt0,
+                                   uint32_t* __restrict__ onbr0, float* __restrict__ odst0, uint32_t* __restrict__ ocntu,
+                                   uint32_t* __restrict__ onbru, float* __restrict__ odstu) {
+  const SpliceSpan sp = spans[blockIdx.x];
+  const uint64_t t0 = (uint64_t)blockIdx.y * blockDim.x + threadIdx.x, st = (uint64_t)gridDim.y * blockDim.x;
+  const uint64_t w0 = sp.rows * 2 * (uint64_t)m, wu = sp.up_rows * (uint64_t)m;
+  for (uint64_t i = t0; i < sp.rows; i += st) ocnt0[sp.new_row + i] = cnt0[sp.old_row + i];
+  for (uint64_t i = t0; i < w0; i += st) {
+    onbr0[sp.new_row * 2 * m + i] = nbr0[sp.old_row * 2 * m + i];
+    odst0[sp.new_row * 2 * m + i] = dst0[sp.old_row * 2 * m + i];
+  }
+  for (uint64_t i = t0; i < sp.up_rows; i += st) ocntu[sp.new_up + i] = cntu[sp.old_up + i];
+  for (uint64_t i = t0; i < wu; i += st) {
+    onbru[sp.new_up * m + i] = nbru[sp.old_up * m + i];
+    odstu[sp.new_up * m + i] = dstu[sp.old_up * m + i];
+  }
+}
+
 // the levels and the empty lists of every partition's graph, then `launch(kernel, policy)` of the build kernel with
-// the policy's table and query words TW / QW in each warp's scratch
+// the policy's table and query words TW / QW in each warp's scratch.  With `keep`, a kept partition's nodes take
+// their levels from the old graph (a loaded graph has no seed) and its lists are spliced in; only the other
+// partitions with at least 2 rows are built.  max_part and the upper rows are counted over the whole new layout.
 template <class Launch>
 static void build_graphs(HnswGraph& g, const uint64_t* part_offsets, int K, uint64_t seed, uint32_t TW, uint32_t QW,
-                         Launch&& launch) {
+                         const HnswKeep* keep, Launch&& launch) {
   std::vector<uint64_t> off(K + 1);
   d2h(off.data(), part_offsets, (size_t)K + 1);
+  std::vector<uint8_t> old_lev;
+  if (keep) {
+    LB2_REQUIRE(keep->old && keep->src.size() == (size_t)K && !keep->old_off.empty(), "%s: bad kept-graph table", g.kind);
+    old_lev.resize(keep->old_off.back());
+    if (!old_lev.empty()) d2h(old_lev.data(), keep->old->nlev.p, old_lev.size());
+  }
   sync_stream();
+  // the first upper row of every old node's partition: the old upper rows are compact in storage order
+  std::vector<uint64_t> old_up;
+  if (keep) {
+    const size_t ok = keep->old_off.size() - 1;
+    old_up.assign(ok + 1, 0);
+    for (size_t q = 0; q < ok; ++q) {
+      uint64_t u = 0;
+      for (uint64_t r = keep->old_off[q]; r < keep->old_off[q + 1]; ++r) u += old_lev[r] - 1;
+      old_up[q + 1] = old_up[q] + u;
+    }
+  }
   const uint64_t n = off[K];
   std::vector<uint64_t> thr(g.max_level);
   hnsw_level_thresholds(g.m, g.max_level, thr.data());
@@ -735,13 +783,22 @@ static void build_graphs(HnswGraph& g, const uint64_t* part_offsets, int K, uint
   std::vector<uint32_t> up_base(n);
   uint64_t n_up = 0, nmax = 0;
   std::vector<uint32_t> order;
+  std::vector<SpliceSpan> spans;
   for (int p = 0; p < K; ++p) {
     const uint64_t np_ = off[p + 1] - off[p];
     nmax = std::max(nmax, np_);
-    if (np_ >= 2) order.push_back((uint32_t)p);
+    const int64_t q = keep ? keep->src[p] : -1;
+    if (q >= 0) {
+      LB2_REQUIRE(keep->old_off[q + 1] - keep->old_off[q] == np_, "%s: kept partition %d changed size", g.kind, p);
+      if (np_) spans.push_back({keep->old_off[q], off[p], np_, old_up[q], n_up, old_up[q + 1] - old_up[q]});
+    } else if (np_ >= 2) {
+      order.push_back((uint32_t)p);
+    }
     for (uint64_t i = 0; i < np_; ++i) {
       int L = g.max_level;  // node 0: every level (builder.rs:368-370)
-      if (i > 0) {
+      if (q >= 0) {
+        L = old_lev[keep->old_off[q] + i];
+      } else if (i > 0) {
         const uint64_t u = hnsw_level_draw(seed, (uint32_t)p, (uint32_t)i);
         L = 1;
         for (int l = 1; l < g.max_level; ++l) L += u < thr[l] ? 1 : 0;
@@ -775,6 +832,15 @@ static void build_graphs(HnswGraph& g, const uint64_t* part_offsets, int K, uint
   g.dst0.zero();
   g.nbru.zero();
   g.dstu.zero();
+  if (!spans.empty()) {
+    DevBuf<SpliceSpan> dspans(spans.size());
+    h2d(dspans.p, spans.data(), spans.size());
+    const HnswGraph& o = *keep->old;
+    LB2_LAUNCH("hnsw_splice", hnsw_splice_kernel, dim3((unsigned)spans.size(), 8), 256, 0, (const SpliceSpan*)dspans.p,
+               g.m, o.cnt0.p, o.nbr0.p, o.dst0.p, o.cntu.p, o.nbru.p, o.dstu.p, g.cnt0.p, g.nbr0.p, g.dst0.p, g.cntu.p,
+               g.nbru.p, g.dstu.p);
+    sync_stream();  // dspans is freed on return
+  }
   if (order.empty()) {
     sync_stream();
     return;
@@ -796,8 +862,8 @@ static void build_graphs(HnswGraph& g, const uint64_t* part_offsets, int K, uint
 }
 
 void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, int d, int metric, float r2,
-                uint64_t seed) {
-  build_graphs(g, part_offsets, K, seed, 0, 0, [&](auto go) {
+                uint64_t seed, const HnswKeep* keep) {
+  build_graphs(g, part_offsets, K, seed, 0, 0, keep, [&](auto go) {
     auto with = [&](auto m) {
       SqDist<decltype(m)::value> P{};
       P.base = codes;
@@ -834,8 +900,8 @@ static uint32_t pq_table_words(int M, int nbits) { return (uint32_t)M << nbits; 
 static uint32_t query_words(int d) { return (uint32_t)(d + 3) & ~3u; }
 
 void hnsw_build_flat(HnswGraph& g, const uint64_t* part_offsets, int K, const void* vectors, int vdt, int d, int metric,
-                     uint64_t seed) {
-  build_graphs(g, part_offsets, K, seed, 0, query_words(d), [&](auto go) {
+                     uint64_t seed, const HnswKeep* keep) {
+  build_graphs(g, part_offsets, K, seed, 0, query_words(d), keep, [&](auto go) {
     dispatch_metric_elem<false>(metric, vdt, [&](auto m, auto e) {
       using T = typename decltype(e)::type;
       using Dist = FlatDist<decltype(m)::value, T>;
@@ -848,8 +914,8 @@ void hnsw_build_flat(HnswGraph& g, const uint64_t* part_offsets, int K, const vo
 }
 
 void hnsw_build_pq(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, const float* codebook,
-                   int d, int M, int nbits, int metric, lb2_dtype dtype, uint64_t seed) {
-  build_graphs(g, part_offsets, K, seed, pq_table_words(M, nbits), query_words(d), [&](auto go) {
+                   int d, int M, int nbits, int metric, lb2_dtype dtype, uint64_t seed, const HnswKeep* keep) {
+  build_graphs(g, part_offsets, K, seed, pq_table_words(M, nbits), query_words(d), keep, [&](auto go) {
     dispatch_pq(metric, nbits, dtype, [&](auto m, auto b, auto r) {
       using Dist = PqDist<decltype(m)::value, decltype(b)::value, decltype(r)::value>;
       Dist P{};

@@ -3,6 +3,8 @@
 #pragma once
 #include <stdint.h>
 
+#include <vector>
+
 #include "common.cuh"
 namespace lb2 {
 struct IvfSearch;
@@ -36,19 +38,29 @@ inline uint32_t hnsw_level_draw(uint64_t seed, uint32_t p, uint32_t i) {
   return (uint32_t)(x >> 32);
 }
 
+// The partitions of a rebuilt index whose graphs are kept from an older graph of the same parameters: new partition
+// p takes old partition src[p]'s graph verbatim when src[p] >= 0 (its rows are all of src[p]'s rows, in order; node
+// ids are partition-local, so levels, lists and distances carry over), and is built from its storage otherwise.
+struct HnswKeep {
+  const HnswGraph* old = nullptr;
+  std::vector<uint64_t> old_off;  // the old index's part_offsets [old K + 1]
+  std::vector<int64_t> src;       // [new K]: old partition id, or -1 = build this partition
+};
+
 // HNSW::index_vectors (builder.rs:742-775) of every partition, nodes inserted 1 .. n_p - 1 in ascending order;
-// codes [n][d] in partition order, part_offsets on the device.  Fills g (its parameters set by the caller).
+// codes [n][d] in partition order, part_offsets on the device.  Fills g (its parameters set by the caller).  With
+// `keep`, only the partitions keep->src marks -1 are built; the others are spliced from keep->old.
 void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, int d, int metric, float r2,
-                uint64_t seed);
+                uint64_t seed, const HnswKeep* keep = nullptr);
 // the same over PQ codes [n][cw] (cw = M, or M / 2 for 4-bit codes) with the codebook [M][2^nbits][d / M]: a node's
 // descent, beam searches and lists use the table of its decoded codes, the heuristic the decoded rows' distance with
 // the rule of `dtype` (pq/storage.rs:675-841)
 void hnsw_build_pq(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, const float* codebook,
-                   int d, int M, int nbits, int metric, lb2_dtype dtype, uint64_t seed);
+                   int d, int M, int nbits, int metric, lb2_dtype dtype, uint64_t seed, const HnswKeep* keep = nullptr);
 // the same over IVF_FLAT's stored rows [n][d] in element type `vdt` (f32, f16 or bf16): every distance, cosine
 // included, is the IVF_FLAT scan's rule (flat/storage.rs:345-410)
 void hnsw_build_flat(HnswGraph& g, const uint64_t* part_offsets, int K, const void* vectors, int vdt, int d, int metric,
-                     uint64_t seed);
+                     uint64_t seed, const HnswKeep* keep = nullptr);
 // a graph from the caller's arrays in the layout above (host or device memory), checked against the partitions
 void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* levels, const uint32_t* counts0,
                const uint32_t* nbr0, const float* dist0, const uint32_t* counts_up, const uint32_t* nbr_up,

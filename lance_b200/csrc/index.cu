@@ -127,14 +127,20 @@ static void build_skew(lb2_index* ix) {
   }
 }
 
+// vec16: M is a multiple of 16 and both payloads are 16-byte aligned (IVF_FLAT rows), copied 16 bytes at a time
 __global__ void group_kernel(const uint32_t* __restrict__ members, uint64_t n, int M,
                              const uint8_t* __restrict__ codes, const uint64_t* __restrict__ row_ids,
-                             uint8_t* __restrict__ codes_out, uint64_t* __restrict__ row_ids_out) {
+                             uint8_t* __restrict__ codes_out, uint64_t* __restrict__ row_ids_out, int vec16) {
   const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (g >= n) return;
   const uint32_t src = members[g];
   row_ids_out[g] = row_ids ? row_ids[src] : (uint64_t)src;
-  for (int m = 0; m < M; ++m) codes_out[g * M + m] = codes[(size_t)src * M + m];
+  if (vec16) {
+    for (int m = 0; m < M; m += 16)
+      *reinterpret_cast<uint4*>(codes_out + g * M + m) = *reinterpret_cast<const uint4*>(codes + (size_t)src * M + m);
+  } else {
+    for (int m = 0; m < M; ++m) codes_out[g * M + m] = codes[(size_t)src * M + m];
+  }
 }
 
 __global__ void gather_f32_kernel(const uint32_t* __restrict__ members, uint64_t n, const float* __restrict__ src,
@@ -148,11 +154,13 @@ void index_load_dev(lb2_index* ix, const uint32_t* part_ids, const uint8_t* code
   MemberSort ms;
   const uint64_t kept = member_sort_index(ms, ix, part_ids, valid, n);
   const int cb = (int)ix->row_bytes();
-  ix->codes.alloc(std::max<uint64_t>(1, kept * cb));
+  DevBuf<uint8_t>& out = ix->payload();
+  out.alloc(std::max<uint64_t>(1, kept * cb));
   ix->row_ids.alloc(std::max<uint64_t>(1, kept));
+  const int vec16 = cb % 16 == 0 && (reinterpret_cast<uintptr_t>(codes) & 15) == 0;
   if (kept)
     LB2_LAUNCH("group_by_partition", group_kernel, cdiv(kept, 256), 256, 0, ms.members.p, kept, cb, codes, row_ids,
-               ix->codes.p, ix->row_ids.p);
+               out.p, ix->row_ids.p, vec16);
   if (ix->kind == IndexKind::RQ) {
     ix->rq_add.alloc(std::max<uint64_t>(1, kept));
     ix->rq_scale.alloc(std::max<uint64_t>(1, kept));
@@ -163,7 +171,7 @@ void index_load_dev(lb2_index* ix, const uint32_t* part_ids, const uint8_t* code
     }
   }
   ix->n = kept;
-  build_skew(ix);
+  if (ix->kind == IndexKind::PQ) build_skew(ix);
   sync_stream();
 }
 
@@ -402,18 +410,21 @@ __global__ void repart_unpack_kernel(const uint64_t* __restrict__ seg_prefix /*[
   }
 }
 
-// ---- incremental update of an IVF_PQ index: the data path of optimize / split / join (SURVEY 8f-4) --------------
+// ---- the merge of optimize / split / join / remap, for every kind (SURVEY 8f-4) ------------------------------------
 // The reference turns an optimize step into per-partition AssignOp::Add / AssignOp::Remove lists against a new
 // centroid set (rust/lance/src/index/vector/builder.rs:1219-1333 split, :1476-1530 join, :1534-1650
 // build_assign_batch) and merges them with the existing partitions when it writes the index.  The decisions --
-// which partition to split or join, which rows to move -- stay on the host (they need the dataset); this entry
-// point is the merge: old rows keep their codes, follow `part_map`, removed row ids are dropped, added rows join
-// the end of their partitions.
+// which partition to split or join, which rows to move -- stay on the host (they need the dataset); index_merge is
+// the merge: old rows keep their payload, follow `part_map`, removed row ids are dropped, added rows join the end of
+// their partitions, and a compaction's row-id mapping is applied last.
+// One pass over the old rows (storage order): the new partition and keep flag of each, and the rows each old
+// partition loses (dropped[p], nullable: the graph kinds' change detection)
 __global__ void update_old_rows_kernel(const uint64_t* __restrict__ part_offsets, int K, uint64_t n,
                                        const uint32_t* __restrict__ part_map /*nullable*/,
                                        const uint64_t* __restrict__ row_ids, const uint64_t* __restrict__ removed,
                                        uint64_t n_removed, uint32_t new_k, uint32_t* __restrict__ part_out,
-                                       uint8_t* __restrict__ valid_out, uint32_t* __restrict__ bad) {
+                                       uint8_t* __restrict__ valid_out, uint32_t* __restrict__ bad,
+                                       uint32_t* __restrict__ dropped) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int p = segment_of(part_offsets, K, i);
@@ -423,6 +434,41 @@ __global__ void update_old_rows_kernel(const uint64_t* __restrict__ part_offsets
   if (keep && n_removed) keep = !sorted_contains(removed, n_removed, row_ids[i]);
   part_out[i] = keep ? np_ : 0u;
   valid_out[i] = keep ? 1 : 0;
+  if (!keep && dropped) atomicAdd(&dropped[p], 1u);
+}
+// bad = 1 when the remap's old ids are not strictly ascending
+__global__ void remap_order_kernel(const uint64_t* __restrict__ old_ids, uint64_t n, uint32_t* __restrict__ bad) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i + 1 < n && old_ids[i] >= old_ids[i + 1]) atomicOr(bad, 1u);
+}
+// storage.remap of every kept row (pq/storage.rs:499-540): one binary search into the sorted pairs; a row mapped to
+// UINT64_MAX (None) loses its keep flag (an old row of partition p counts in dropped[p], nullable), a row mapped to
+// a value takes it, a row not in the mapping is left as it is
+__global__ void remap_rows_kernel(uint64_t* __restrict__ row_ids, uint8_t* __restrict__ valid, uint64_t n,
+                                  const uint64_t* __restrict__ old_ids, const uint64_t* __restrict__ new_ids,
+                                  uint64_t n_remap, const uint64_t* __restrict__ part_offsets, int K, uint64_t n_old,
+                                  uint32_t* __restrict__ dropped) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || !valid[i]) return;
+  const uint64_t id = row_ids[i];
+  uint64_t lo = 0, hi = n_remap;
+  while (lo < hi) {
+    const uint64_t mid = (lo + hi) >> 1;
+    if (old_ids[mid] < id) lo = mid + 1; else hi = mid;
+  }
+  if (lo == n_remap || old_ids[lo] != id) return;
+  const uint64_t to = new_ids[lo];
+  if (to != ~0ull) {
+    row_ids[i] = to;
+    return;
+  }
+  valid[i] = 0;
+  if (dropped && i < n_old) atomicAdd(&dropped[segment_of(part_offsets, K, i)], 1u);
+}
+// rows per partition id
+__global__ void count_parts_kernel(const uint32_t* __restrict__ part, uint64_t n, uint32_t* __restrict__ counts) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) atomicAdd(&counts[part[i]], 1u);
 }
 __global__ void fill_u8_kernel(uint8_t* __restrict__ p, uint64_t n, uint8_t v) {
   const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -461,6 +507,142 @@ __global__ void transpose_codes_kernel(const uint8_t* __restrict__ codes, uint64
   const uint64_t j = g % n;
   const int m = (int)(g / n);
   out[g] = codes[j * cw + m];
+}
+
+// the kept graphs of a merge (lb2_optimize_params' rule): new partition p keeps old partition q's graph when q lost no
+// row, nothing was added to p, and p holds exactly q's rows (then no other old partition sent p a row)
+static HnswKeep kept_partitions(const lb2_index* old, const lb2_index* ix, const uint32_t* part_map,
+                                const uint32_t* dropped, const uint32_t* added) {
+  HnswKeep keep;
+  keep.old = old->hnsw.get();
+  const int ok = old->K, nk = ix->K;
+  keep.old_off.resize(ok + 1);
+  std::vector<uint64_t> noff(nk + 1);
+  std::vector<uint32_t> pm(part_map ? ok : 0), dr(ok), ad(nk);
+  d2h(keep.old_off.data(), old->part_offsets.p, (size_t)ok + 1);
+  d2h(noff.data(), ix->part_offsets.p, (size_t)nk + 1);
+  if (part_map) d2h(pm.data(), part_map, (size_t)ok);
+  d2h(dr.data(), dropped, (size_t)ok);
+  d2h(ad.data(), added, (size_t)nk);
+  sync_stream();
+  keep.src.assign(nk, -1);
+  for (int q = 0; q < ok; ++q) {
+    const uint32_t p = part_map ? pm[q] : (uint32_t)q;
+    const uint64_t rows = keep.old_off[q + 1] - keep.old_off[q];
+    if (p == 0xffffffffu || rows == 0 || dr[q] || ad[p] || noff[p + 1] - noff[p] != rows) continue;
+    keep.src[p] = q;
+  }
+  return keep;
+}
+
+// lb2_index_optimize's merge (and lb2_index_update's); `what` names the entry point in messages
+static std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_optimize_params& p, const char* what) {
+  const bool rq = old->kind == IndexKind::RQ;
+  const uint32_t new_k = p.new_k;
+  LB2_REQUIRE(new_k > 0 && (p.new_centroids || new_k == (uint32_t)old->K), "a changed partition count needs new centroids");
+  LB2_REQUIRE(p.n_add == 0 || (p.add_part_ids && p.add_payload && p.add_row_ids),
+              "%s: added rows need partition ids, payload and row ids", what);
+  if (rq)
+    LB2_REQUIRE(p.n_add == 0 || (p.add_rq_add && p.add_rq_scale), "%s: IVF_RQ rows need their add and scale factors",
+                what);
+  else
+    LB2_REQUIRE(!p.add_rq_add && !p.add_rq_scale, "%s: add and scale factors are for IVF_RQ indexes only", what);
+  LB2_REQUIRE(p.n_remove == 0 || p.remove_row_ids, "null remove list");
+  LB2_REQUIRE(p.n_remap == 0 || (p.remap_old_ids && p.remap_new_ids), "%s: null remap list", what);
+  if (old->hnsw && comm_nranks() > 1)
+    fail(LB2_UNSUPPORTED, "%s: %s indexes over more than one rank are not implemented", what, old->hnsw->kind);
+  const int rb = (int)old->row_bytes();
+  const uint64_t n_old = old->n, n_add = p.n_add, n_all = n_old + n_add;
+  LB2_REQUIRE(n_all < 0xffffffffull, "more than 2^32-1 rows per index shard");
+  std::unique_ptr<lb2_index> ix = make_index(old->kind, new_k, old->d, old->metric, old->dtype);
+  copy_model(old, ix.get(), p.new_centroids);
+  InArg<uint32_t> pm(p.part_map, p.part_map ? (size_t)old->K : 0), ap(p.add_part_ids, n_add);
+  InArg<uint8_t> ac(p.add_payload, (size_t)n_add * rb);
+  InArg<float> aa(p.add_rq_add, rq ? n_add : 0), as(p.add_rq_scale, rq ? n_add : 0);
+  InArg<uint64_t> ar(p.add_row_ids, n_add), rm(p.remove_row_ids, p.n_remove), ro(p.remap_old_ids, p.n_remap),
+      rn(p.remap_new_ids, p.n_remap);
+  if (n_add) check_part_ids(ap.get(), n_add, new_k, what);
+  // one row list: old rows in storage order, then the added rows (so a partition keeps its old rows first)
+  DevBuf<uint32_t> part(std::max<uint64_t>(1, n_all)), bad(2), dropped, added;
+  DevBuf<uint8_t> valid(std::max<uint64_t>(1, n_all)), payload(std::max<uint64_t>(1, n_all * rb));
+  DevBuf<uint64_t> rid(std::max<uint64_t>(1, n_all));
+  DevBuf<float> fa, fs;
+  bad.zero();
+  if (old->hnsw) {  // what the graph kinds need to find the unchanged partitions
+    dropped.alloc(old->K);
+    dropped.zero();
+    added.alloc(new_k);
+    added.zero();
+    if (n_add) LB2_LAUNCH("count_added", count_parts_kernel, cdiv(n_add, 256), 256, 0, ap.get(), n_add, added.p);
+  }
+  if (rq) {
+    fa.alloc(std::max<uint64_t>(1, n_all));
+    fs.alloc(std::max<uint64_t>(1, n_all));
+  }
+  if (p.n_remap > 1)
+    LB2_LAUNCH("remap_order", remap_order_kernel, cdiv(p.n_remap, 256), 256, 0, ro.get(), p.n_remap, bad.p + 1);
+  if (n_old) {
+    LB2_LAUNCH("update_old_rows", update_old_rows_kernel, cdiv(n_old, 256), 256, 0, old->part_offsets.p, old->K, n_old,
+               pm.get(), (const uint64_t*)old->row_ids.p, rm.get(), p.n_remove, new_k, part.p, valid.p, bad.p,
+               dropped.p);
+    d2d(payload.p, old->payload().p, (size_t)n_old * rb);
+    d2d(rid.p, old->row_ids.p, (size_t)n_old);
+    if (rq) {
+      d2d(fa.p, old->rq_add.p, (size_t)n_old);
+      d2d(fs.p, old->rq_scale.p, (size_t)n_old);
+    }
+  }
+  if (n_add) {
+    d2d(part.p + n_old, ap.get(), (size_t)n_add);
+    d2d(payload.p + n_old * rb, ac.get(), (size_t)n_add * rb);
+    d2d(rid.p + n_old, ar.get(), (size_t)n_add);
+    if (rq) {
+      d2d(fa.p + n_old, aa.get(), (size_t)n_add);
+      d2d(fs.p + n_old, as.get(), (size_t)n_add);
+    }
+    LB2_LAUNCH("fill_valid", fill_u8_kernel, cdiv(n_add, 256), 256, 0, valid.p + n_old, n_add, (uint8_t)1);
+  }
+  uint32_t hbad[2] = {0, 0};
+  d2h(hbad, bad.p, 2);
+  sync_stream();
+  if (hbad[0]) fail(LB2_INVALID_ARG, "%s: part_map sends a partition to %u, the new index has %u partitions", what, hbad[0], new_k);
+  if (hbad[1]) fail(LB2_INVALID_ARG, "%s: the remap's old row ids are not strictly ascending", what);
+  if (p.n_remap && n_all)
+    LB2_LAUNCH("remap_rows", remap_rows_kernel, cdiv(n_all, 256), 256, 0, rid.p, valid.p, n_all, ro.get(), rn.get(),
+               p.n_remap, old->part_offsets.p, old->K, n_old, dropped.p);
+  index_load_dev(ix.get(), part.p, payload.p, rid.p, n_all, valid.p, fa.p, fs.p);
+  if (old->hnsw) {
+    const HnswGraph& og = *old->hnsw;
+    const HnswKeep keep = kept_partitions(old, ix.get(), pm.get(), dropped.p, added.p);
+    ix->hnsw.reset(new HnswGraph());
+    HnswGraph& g = *ix->hnsw;
+    g.kind = og.kind;
+    g.max_level = og.max_level;
+    g.m = og.m;
+    g.ef_construction = og.ef_construction;
+    TagScope tg("hnsw_build");
+    switch (ix->kind) {
+      case IndexKind::SQ: {
+        const float rf = (float)(ix->sq_upper - ix->sq_lower);
+        hnsw_build(g, ix->part_offsets.p, ix->K, ix->codes.p, ix->d, ix->metric, rf * rf, p.seed, &keep);
+        break;
+      }
+      case IndexKind::PQ:
+        ix->slab_off.release();  // the skewed code copy serves only the IVF_PQ scan
+        ix->codes_skew.release();
+        hnsw_build_pq(g, ix->part_offsets.p, ix->K, ix->codes.p, ix->codebook.p, ix->d, ix->M, ix->nbits, ix->metric,
+                      ix->dtype, p.seed, &keep);
+        break;
+      case IndexKind::FLAT:
+        hnsw_build_flat(g, ix->part_offsets.p, ix->K, ix->vectors.p, (int)ix->vdtype(), ix->d, ix->metric, p.seed,
+                        &keep);
+        break;
+      case IndexKind::RQ:  // no IVF_RQ index has a graph
+        break;
+    }
+  }
+  sync_stream();
+  return ix;
 }
 
 }  // namespace lb2
@@ -1004,41 +1186,25 @@ lb2_status lb2_index_update(const lb2_index* old, const void* new_centroids, uin
     fail(LB2_UNSUPPORTED, "lb2_index_update: IVF_HNSW_FLAT indexes are not implemented");
   LB2_REQUIRE(old && out && old->kind == IndexKind::PQ, "lb2_index_update takes an IVF_PQ index");
   if (old->hnsw) fail(LB2_UNSUPPORTED, "lb2_index_update: IVF_HNSW_PQ indexes are not implemented");
-  LB2_REQUIRE(new_k > 0 && (new_centroids || new_k == (uint32_t)old->K), "a changed partition count needs new centroids");
   LB2_REQUIRE(n_add == 0 || (add_part_ids && add_codes && add_row_ids), "added rows need partition ids, codes and row ids");
-  LB2_REQUIRE(n_remove == 0 || remove_row_ids, "null remove list");
-  const int cbw = (int)old->row_bytes();
-  const uint64_t n_old = old->n, n_all = n_old + n_add;
-  LB2_REQUIRE(n_all < 0xffffffffull, "more than 2^32-1 rows per index shard");
-  std::unique_ptr<lb2_index> ix = make_index(old->kind, new_k, old->d, old->metric, old->dtype);
-  copy_model(old, ix.get(), new_centroids);
-  InArg<uint32_t> pm(part_map, part_map ? (size_t)old->K : 0), ap(add_part_ids, n_add);
-  InArg<uint8_t> ac(add_codes, (size_t)n_add * cbw);
-  InArg<uint64_t> ar(add_row_ids, n_add), rm(remove_row_ids, n_remove);
-  if (n_add) check_part_ids(ap.get(), n_add, new_k, "index_update");
-  // one row list: old rows in storage order, then the added rows (so a partition keeps its old rows first)
-  DevBuf<uint32_t> part(std::max<uint64_t>(1, n_all)), bad(1);
-  DevBuf<uint8_t> valid(std::max<uint64_t>(1, n_all)), codes(std::max<uint64_t>(1, n_all * cbw));
-  DevBuf<uint64_t> rid(std::max<uint64_t>(1, n_all));
-  bad.zero();
-  if (n_old) {
-    LB2_LAUNCH("update_old_rows", update_old_rows_kernel, cdiv(n_old, 256), 256, 0, old->part_offsets.p, old->K, n_old,
-               pm.get(), (const uint64_t*)old->row_ids.p, rm.get(), n_remove, new_k, part.p, valid.p, bad.p);
-    d2d(codes.p, old->codes.p, (size_t)n_old * cbw);
-    d2d(rid.p, old->row_ids.p, (size_t)n_old);
-  }
-  if (n_add) {
-    d2d(part.p + n_old, ap.get(), (size_t)n_add);
-    d2d(codes.p + n_old * cbw, ac.get(), (size_t)n_add * cbw);
-    d2d(rid.p + n_old, ar.get(), (size_t)n_add);
-    LB2_LAUNCH("fill_valid", fill_u8_kernel, cdiv(n_add, 256), 256, 0, valid.p + n_old, n_add, (uint8_t)1);
-  }
-  uint32_t hbad = 0;
-  d2h(&hbad, bad.p, 1);
-  sync_stream();
-  if (hbad) fail(LB2_INVALID_ARG, "index_update: part_map sends a partition to %u, the new index has %u partitions", hbad, new_k);
-  index_load_dev(ix.get(), part.p, codes.p, rid.p, n_all, valid.p);
-  *out = ix.release();
+  lb2_optimize_params p = {};
+  p.new_centroids = new_centroids;
+  p.new_k = new_k;
+  p.part_map = part_map;
+  p.add_part_ids = add_part_ids;
+  p.add_payload = add_codes;
+  p.add_row_ids = add_row_ids;
+  p.n_add = n_add;
+  p.remove_row_ids = remove_row_ids;
+  p.n_remove = n_remove;
+  *out = index_merge(old, p, "index_update").release();
+  LB2_API_END
+}
+
+lb2_status lb2_index_optimize(const lb2_index* old, const lb2_optimize_params* p, lb2_index** out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(old && p && out, "null argument");
+  *out = index_merge(old, *p, "index_optimize").release();
   LB2_API_END
 }
 

@@ -58,7 +58,8 @@ namespace lb2 {
 std::unique_ptr<lb2_index> make_index(IndexKind kind, uint32_t K, uint32_t d, int metric, lb2_dtype dtype);
 // a partition id >= K (a corrupted / mismatched shuffle file) would index device memory out of bounds
 void check_part_ids(const uint32_t* part_ids, uint64_t n, uint32_t K, const char* what);
-// rows with valid[r] == 0 are dropped; rq_add / rq_scale (IVF_RQ only): the rows' factors, grouped with their codes
+// stable grouping of n rows' payloads (row_bytes() each: codes, or IVF_FLAT's stored rows) by partition; rows with
+// valid[r] == 0 are dropped; rq_add / rq_scale (IVF_RQ only): the rows' factors, grouped with their codes
 void index_load_dev(lb2_index* ix, const uint32_t* part_ids, const uint8_t* codes, const uint64_t* row_ids,
                     uint64_t n, const uint8_t* valid = nullptr, const float* rq_add = nullptr,
                     const float* rq_scale = nullptr);
