@@ -405,9 +405,11 @@ lb2_status lb2_index_transform(const lb2_index* index, const void* vectors, uint
  * q's rows removed or remapped to None and nothing added, keeps q's graph verbatim (every node id and distance depends
  * only on the partition's payload sequence; the reference's rebuild, hnsw/builder.rs:777-785, gives the same graph
  * up to its unseeded level draws).  Every other partition with at least 2 rows gets the graph of the kind's build over
- * its new storage, its level draws keyed by (seed, new partition id, node).
- * LB2_INVALID_ARG before the new index is made: remap_old_ids not strictly ascending, a part id or part_map entry at or
- * above new_k, missing or extra RQ factors, a changed new_k without new_centroids, more than 2^32 - 1 rows.  Under a
+ * its new storage, its level draws keyed by (seed, new partition id, node), inserted in rounds of insert_batch (0: the
+ * B the old index was built with, 1 for a loaded graph); the new index records the B it used.  insert_batch above
+ * 65 536 is LB2_INVALID_ARG for a graph kind; the other kinds ignore it.
+ * LB2_INVALID_ARG before the new index is made: remap_old_ids not strictly ascending, a graph kind's insert_batch
+ * above 65 536, a part id or part_map entry at or above new_k, missing or extra RQ factors, a changed new_k without new_centroids, more than 2^32 - 1 rows.  Under a
  * communicator the non-graph kinds merge each shard's rows (as lb2_index_update); the graph kinds return
  * LB2_UNSUPPORTED with more than one rank. */
 typedef struct {
@@ -426,6 +428,7 @@ typedef struct {
   const uint64_t* remap_new_ids; /* UINT64_MAX = None: the row is dropped */
   uint64_t n_remap;
   uint64_t seed;                 /* the level draws of the graphs that are rebuilt */
+  uint32_t insert_batch;         /* B of the graphs that are rebuilt (IVF_HNSW_SQ's rounds); 0: the old index's B */
 } lb2_optimize_params;
 lb2_status lb2_index_optimize(const lb2_index* old_index, const lb2_optimize_params* p, lb2_index** out);
 /* Asynchronous search (SURVEY 8b "Threading": `_async` variants taking a stream/event).  Same
@@ -556,6 +559,21 @@ lb2_status lb2_index_export_sq(const lb2_index* index, void* centroids_out, doub
  * inserted 1 .. n_p - 1 in ascending order (the reference inserts in parallel); node 0 has max_level levels and is
  * the entry point (:354-376), node i >= 1 gets 1 + random_level() levels (:386-393) from a u32 draw keyed by (seed,
  * p, i) compared against floor(2^32 / m^l).  Ties in select_neighbors_heuristic (hnsw.rs:60-88) keep their order.
+ *
+ * Batched insertion (insert_batch = B >= 2; 0 and 1 insert one node at a time, as above): a deterministic stand-in
+ * for the reference's concurrent inserts.  The graph is a function of (data, seed, m, ef_construction, max_level, B)
+ * alone, whatever the number of warps in flight.  A partition with n_p >= 2 rows is built in rounds: the first round
+ * starts at s = 1, a round starting at s inserts nodes s .. e - 1 with e = min(n_p, s + min(B, s)), and the next
+ * round starts at e (rounds of 1, 2, 4, .. nodes until B, then B).  Each round has two phases:
+ *   1. every node i of the round runs insert's descent and beam searches (builder.rs:396-463) over the graph as it
+ *      stood at the start of the round, and its own lists are the pruned results, as in the serial build (no list
+ *      names a node of the round yet, so no node of the round reaches another);
+ *   2. the back-links, as if applied for i ascending, level 0 .. i's top level, entries in list order, each with the
+ *      serial rule (enter the target's list when closer than its LAST entry or the list is short, then prune).  Every
+ *      target is a node < s and a list takes at most one entry per node, so this is each target list taking its
+ *      entries in ascending i, distinct lists independently.
+ * Levels, level draws, the entry point and every distance and tie rule are the serial build's; with B = 1 every
+ * round holds one node and the graph is the serial graph byte for byte.
  * Searches go through lb2_index_search / _refine / _ex / _probed / _combined / _async / _sharded with the default ef
  * k' + k' / 2, k' = k * refine_factor (:563-573), or through lb2_index_search_hnsw with an explicit ef: each probed
  * partition is HNSW::search (builder.rs:678-739); ef < k' is LB2_INVALID_ARG (:687-692).  A prefilter that leaves fewer than
@@ -573,10 +591,12 @@ typedef struct {
   uint32_t max_level;       /* HnswBuildParams (hnsw/builder.rs:63-72): 7 */
   uint32_t m;               /* 20; level 0 keeps up to 2m neighbours, the others m */
   uint32_t ef_construction; /* 150 */
+  uint32_t insert_batch;    /* B of the batched insertion above: 0 or 1 serial (the default 1), at most 65 536 */
 } lb2_ivfhnswsq_build_params;
 void lb2_ivfhnswsq_build_params_default(lb2_ivfhnswsq_build_params* p);
-/* IvfIndexBuilder<HNSW, ScalarQuantizer>::build: lb2_ivfsq_build, then every partition's graph on the device (one
- * warp per partition, the largest partitions first); the level draws use params->sq.seed. */
+/* IvfIndexBuilder<HNSW, ScalarQuantizer>::build: lb2_ivfsq_build, then every partition's graph on the device (serial:
+ * one warp per partition, the largest partitions first; batched: one warp per inserting node, then one per
+ * back-linked list, all partitions advancing round by round); the level draws use params->sq.seed. */
 lb2_status lb2_ivfhnswsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
                                const lb2_ivfhnswsq_build_params* params, const uint64_t* row_ids, lb2_index** out,
                                lb2_build_stats* stats);
@@ -601,9 +621,9 @@ lb2_status lb2_index_search_hnsw(lb2_index* index, const void* queries, uint64_t
 
 /* ---- IVF_HNSW_PQ: IVFIndex<HNSW, ProductQuantizer> (rust/lance/src/index/vector.rs:494-520) ---------------------
  * An IVF_PQ index (same IVF stage, codebook and codes for the same arguments) with an HNSW graph per partition over
- * the partition's PQ storage (lance-index/src/vector/pq/storage.rs:600-1037).  Levels, insertion order, tie handling,
- * the graph layout, ef, the prefilter switch and the refusals are IVF_HNSW_SQ's (above); the distances are the PQ
- * storage's, and cosine is L2 on the normalised rows throughout (the storage carries L2, pq/storage.rs:465-468):
+ * the partition's PQ storage (lance-index/src/vector/pq/storage.rs:600-1037).  Levels, insertion order (batched
+ * rounds included), tie handling, the graph layout, ef, the prefilter switch and the refusals are IVF_HNSW_SQ's
+ * (above); the distances are the PQ storage's, and cosine is L2 on the normalised rows throughout (the storage carries L2, pq/storage.rs:465-468):
  *  - query to node (search): PQDistCalculator::distance (storage.rs:891-919) on the IVF_PQ scan's table of the
  *    query (its residual to the probed centroid under L2 / cosine, the raw query under dot): 8-bit codes the
  *    m-ascending f32 sum of table[m][code[m]], the distance of lb2_index_search on IVF_PQ; 4-bit codes the sum, in
@@ -619,10 +639,11 @@ typedef struct {
   uint32_t max_level;       /* HnswBuildParams (hnsw/builder.rs:63-72): 7 */
   uint32_t m;               /* 20; level 0 keeps up to 2m neighbours, the others m */
   uint32_t ef_construction; /* 150 */
+  uint32_t insert_batch;    /* as lb2_ivfhnswsq_build_params.insert_batch */
 } lb2_ivfhnswpq_build_params;
 void lb2_ivfhnswpq_build_params_default(lb2_ivfhnswpq_build_params* p);
 /* IvfIndexBuilder<HNSW, ProductQuantizer>::build (vector.rs:507-520): lb2_ivfpq_build, then every partition's graph on
- * the device (one warp per partition, the largest partitions first); the level draws use params->pq.seed.  The graph
+ * the device (as lb2_ivfhnswsq_build's, serial or batched); the level draws use params->pq.seed.  The graph
  * stage is counted in stats->ms_total only.  A communicator of more than one rank is LB2_UNSUPPORTED. */
 lb2_status lb2_ivfhnswpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
                                const lb2_ivfhnswpq_build_params* params, const uint64_t* row_ids, lb2_index** out,
@@ -660,10 +681,11 @@ typedef struct {
   uint32_t max_level;       /* HnswBuildParams (hnsw/builder.rs:63-72): 7 */
   uint32_t m;               /* 20; level 0 keeps up to 2m neighbours, the others m */
   uint32_t ef_construction; /* 150 */
+  uint32_t insert_batch;    /* as lb2_ivfhnswsq_build_params.insert_batch */
 } lb2_ivfhnswflat_build_params;
 void lb2_ivfhnswflat_build_params_default(lb2_ivfhnswflat_build_params* p);
-/* IvfIndexBuilder<HNSW, FlatQuantizer>::build: lb2_ivfflat_build, then every partition's graph on the device (one warp
- * per partition, the largest partitions first); the level draws use params->flat.seed.  The graph stage is counted in
+/* IvfIndexBuilder<HNSW, FlatQuantizer>::build: lb2_ivfflat_build, then every partition's graph on the device (as
+ * lb2_ivfhnswsq_build's, serial or batched); the level draws use params->flat.seed.  The graph stage is counted in
  * stats->ms_total only.  A communicator of more than one rank is LB2_UNSUPPORTED. */
 lb2_status lb2_ivfhnswflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
                                  const lb2_ivfhnswflat_build_params* params, const uint64_t* row_ids, lb2_index** out,

@@ -803,6 +803,11 @@ class IvfPqIndex:
         otherwise add_part_ids / add_payload (/ add_factors = (add, scale) for IVF_RQ) as transform() returns them.
         remap: {old id: new id or None} or (old ids, new ids) with UINT64_MAX for None.  seed: the level draws of the
         graphs that are rebuilt (IVF_HNSW_*)."""
+        return self._optimize(add_vectors, add_row_ids, add_part_ids, add_payload, add_factors, new_centroids, part_map,
+                              remove_row_ids, remap, seed, 0)
+
+    def _optimize(self, add_vectors, add_row_ids, add_part_ids, add_payload, add_factors, new_centroids, part_map,
+                  remove_row_ids, remap, seed, insert_batch):
         from ._lib import OptimizeParams
         if add_vectors is not None:
             if add_part_ids is not None or add_payload is not None or add_factors is not None:
@@ -841,7 +846,7 @@ class IvfPqIndex:
         n_add = 0 if ap is None else ap.size
         p = OptimizeParams(nz(ptr[0]), new_k, nz(ptr[1]), nz(ptr[2]), nz(ptr[3]), nz(ptr[4]), nz(ptr[5]), nz(ptr[6]),
                            n_add, nz(ptr[7]), 0 if rm is None else rm.size, nz(ptr[8]), nz(ptr[9]),
-                           0 if ro is None else ro.size, seed)
+                           0 if ro is None else ro.size, seed, insert_batch)
         h = C.c_void_p()
         check(lib().lb2_index_optimize(self._h, C.byref(p), C.byref(h)))
         out = type(self)(h)
@@ -1069,10 +1074,13 @@ class IvfSqIndex(IvfPqIndex):
 
 # ---- lance-index::vector::hnsw over SQ storage (IVF_HNSW_SQ) ---------------------------------------------
 class HnswBuildParams:
-    """lance_index::vector::hnsw::builder::HnswBuildParams (hnsw/builder.rs:47-72)."""
+    """lance_index::vector::hnsw::builder::HnswBuildParams (hnsw/builder.rs:47-72), plus insert_batch: B of the
+    batched build (include/lance_b200.h, IVF_HNSW_SQ): nodes are inserted in deterministic rounds of up to B
+    concurrent inserts (1, 2, 4, .. then B).  1 (or 0) is the serial build; at most 65536."""
 
-    def __init__(self, max_level=7, m=20, ef_construction=150):
+    def __init__(self, max_level=7, m=20, ef_construction=150, insert_batch=1):
         self.max_level, self.m, self.ef_construction = max_level, m, ef_construction
+        self.insert_batch = insert_batch
 
 
 class _HnswGraphs:
@@ -1114,6 +1122,13 @@ class _HnswGraphs:
                                              ptr["counts_up"], ptr["neighbors_up"], ptr["dists_up"]))
         out["graph"] = g
         return out
+
+    def optimize(self, add_vectors=None, add_row_ids=None, add_part_ids=None, add_payload=None, add_factors=None,
+                 new_centroids=None, part_map=None, remove_row_ids=None, remap=None, seed=0, insert_batch=None):
+        """the parent kind's optimize; insert_batch: B of the rebuilt partitions' graphs (None: the B this index was
+        built with, 1 for a loaded graph).  Kept partitions keep their graphs verbatim."""
+        return self._optimize(add_vectors, add_row_ids, add_part_ids, add_payload, add_factors, new_centroids, part_map,
+                              remove_row_ids, remap, seed, 0 if insert_batch is None else int(insert_batch))
 
     def _search_hnsw(self, queries, k, nprobes, ef, probe=None, allow_bitmap=None, refine_factor=0, vectors=None,
                      lower_bound=None, upper_bound=None):
@@ -1204,6 +1219,7 @@ class IvfHnswSqIndex(_HnswGraphs, IvfSqIndex):
         bp.sq.ivf.max_iters, bp.sq.ivf.sample_rate, bp.sq.ivf.seed, bp.sq.seed = max_iters, sample_rate, seed, seed
         bp.sq.num_bits, bp.sq.sample_rate = sq_params.num_bits, sq_params.sample_rate
         bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
+        bp.insert_batch = hnsw_params.insert_batch
         keep = None
         if centroids is not None:
             keep = _f32(centroids)
@@ -1252,6 +1268,7 @@ class IvfHnswPqIndex(_HnswGraphs, IvfPqIndex):
         lib().lb2_ivfhnswpq_build_params_default(C.byref(bp))
         keep = _fill_build_params(bp.pq, params)
         bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
+        bp.insert_batch = hnsw_params.insert_batch
         rid = None if row_ids is None else (row_ids if isinstance(row_ids, DeviceArray)
                                             else np.ascontiguousarray(row_ids, dtype=np.uint64))
         h = C.c_void_p()
@@ -1314,6 +1331,7 @@ class IvfHnswFlatIndex(_HnswGraphs, IvfFlatIndex):
         f.num_partitions = num_partitions
         f.ivf.max_iters, f.ivf.sample_rate, f.ivf.seed, f.seed = max_iters, sample_rate, seed, seed
         bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
+        bp.insert_batch = hnsw_params.insert_batch
         keep = None
         if centroids is not None:
             keep = _f32(centroids)

@@ -55,17 +55,20 @@ class SqBuildParams(C.Structure):
 
 class HnswSqBuildParams(C.Structure):
     """lb2_ivfhnswsq_build_params (include/lance_b200.h)."""
-    _fields_ = [("sq", SqBuildParams), ("max_level", C.c_uint32), ("m", C.c_uint32), ("ef_construction", C.c_uint32)]
+    _fields_ = [("sq", SqBuildParams), ("max_level", C.c_uint32), ("m", C.c_uint32), ("ef_construction", C.c_uint32),
+                ("insert_batch", C.c_uint32)]
 
 
 class HnswPqBuildParams(C.Structure):
     """lb2_ivfhnswpq_build_params (include/lance_b200.h)."""
-    _fields_ = [("pq", BuildParams), ("max_level", C.c_uint32), ("m", C.c_uint32), ("ef_construction", C.c_uint32)]
+    _fields_ = [("pq", BuildParams), ("max_level", C.c_uint32), ("m", C.c_uint32), ("ef_construction", C.c_uint32),
+                ("insert_batch", C.c_uint32)]
 
 
 class HnswFlatBuildParams(C.Structure):
     """lb2_ivfhnswflat_build_params (include/lance_b200.h)."""
-    _fields_ = [("flat", FlatBuildParams), ("max_level", C.c_uint32), ("m", C.c_uint32), ("ef_construction", C.c_uint32)]
+    _fields_ = [("flat", FlatBuildParams), ("max_level", C.c_uint32), ("m", C.c_uint32), ("ef_construction", C.c_uint32),
+                ("insert_batch", C.c_uint32)]
 
 
 class RqBuildParams(C.Structure):
@@ -80,7 +83,8 @@ class OptimizeParams(C.Structure):
                 ("add_part_ids", C.c_void_p), ("add_payload", C.c_void_p), ("add_rq_add", C.c_void_p),
                 ("add_rq_scale", C.c_void_p), ("add_row_ids", C.c_void_p), ("n_add", C.c_uint64),
                 ("remove_row_ids", C.c_void_p), ("n_remove", C.c_uint64), ("remap_old_ids", C.c_void_p),
-                ("remap_new_ids", C.c_void_p), ("n_remap", C.c_uint64), ("seed", C.c_uint64)]
+                ("remap_new_ids", C.c_void_p), ("n_remap", C.c_uint64), ("seed", C.c_uint64),
+                ("insert_batch", C.c_uint32)]
 
 
 class BuildStats(C.Structure):

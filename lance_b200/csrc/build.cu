@@ -334,6 +334,7 @@ void lb2_ivfhnswsq_build_params_default(lb2_ivfhnswsq_build_params* p) {
   p->max_level = 7;  // HnswBuildParams::default (hnsw/builder.rs:63-72)
   p->m = 20;
   p->ef_construction = 150;
+  p->insert_batch = 1;
 }
 
 void lb2_ivfhnswpq_build_params_default(lb2_ivfhnswpq_build_params* p) {
@@ -341,6 +342,7 @@ void lb2_ivfhnswpq_build_params_default(lb2_ivfhnswpq_build_params* p) {
   p->max_level = 7;  // HnswBuildParams::default (hnsw/builder.rs:63-72)
   p->m = 20;
   p->ef_construction = 150;
+  p->insert_batch = 1;
 }
 
 void lb2_ivfhnswflat_build_params_default(lb2_ivfhnswflat_build_params* p) {
@@ -348,6 +350,7 @@ void lb2_ivfhnswflat_build_params_default(lb2_ivfhnswflat_build_params* p) {
   p->max_level = 7;  // HnswBuildParams::default (hnsw/builder.rs:63-72)
   p->m = 20;
   p->ef_construction = 150;
+  p->insert_batch = 1;
 }
 
 void lb2_ivfrq_build_params_default(lb2_ivfrq_build_params* p) {
@@ -775,17 +778,19 @@ lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
 
 }  // extern "C"
 
-// the graph parameters of an HNSW build (hnsw/builder.rs:63-72)
-static void check_hnsw_params(const char* kind, uint32_t max_level, uint32_t m, uint32_t ef_construction) {
+// the graph parameters of an HNSW build (hnsw/builder.rs:63-72) and the batched insertion's B
+static void check_hnsw_params(const char* kind, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                              uint32_t insert_batch) {
   LB2_REQUIRE(max_level >= 1 && max_level <= 64, "%s: max_level must be in 1 .. 64, got %u", kind, max_level);
   LB2_REQUIRE(m >= 1 && m <= 1024, "%s: m must be in 1 .. 1024, got %u", kind, m);
   LB2_REQUIRE(ef_construction >= 1, "%s: ef_construction must be at least 1", kind);
+  LB2_REQUIRE(insert_batch <= 65536, "%s: insert_batch must be at most 65536, got %u", kind, insert_batch);
 }
 
 // step 2 of an IVF_HNSW_* build: the graphs of `ix`, counted in stats->ms_total only
 template <class F>
 static void attach_graphs(lb2_index* ix, const char* kind, uint32_t max_level, uint32_t m, uint32_t ef_construction,
-                          lb2_build_stats* stats, F&& build) {
+                          uint32_t insert_batch, lb2_build_stats* stats, F&& build) {
   EventSet ev(2);
   ev.record(0);
   {
@@ -796,6 +801,7 @@ static void attach_graphs(lb2_index* ix, const char* kind, uint32_t max_level, u
     g.max_level = (int)max_level;
     g.m = (int)m;
     g.ef_construction = (int)ef_construction;
+    g.insert_batch = std::max<uint32_t>(insert_batch, 1);
     build(g);
   }
   ev.record(1);
@@ -809,14 +815,15 @@ lb2_status lb2_ivfhnswsq_build(const void* data, uint64_t n, uint32_t d, lb2_dty
                                lb2_build_stats* stats) {
   LB2_API_BEGIN
   LB2_REQUIRE(data && params && out, "null argument");
-  check_hnsw_params("IVF_HNSW_SQ", params->max_level, params->m, params->ef_construction);
+  check_hnsw_params("IVF_HNSW_SQ", params->max_level, params->m, params->ef_construction, params->insert_batch);
   // 1. the IVF stage, bounds and codes of IVF_SQ with the same arguments
   lb2_index* sq = nullptr;
   const lb2_status st = lb2_ivfsq_build(data, n, d, dtype, metric, &params->sq, row_ids, &sq, stats);
   if (st != LB2_OK) return st;  // its message is already the last error
   std::unique_ptr<lb2_index> ix(sq);
   // 2. HNSW::index_vectors per partition over its codes (v3 IvfIndexBuilder with an HNSW sub-index)
-  attach_graphs(ix.get(), "IVF_HNSW_SQ", params->max_level, params->m, params->ef_construction, stats, [&](HnswGraph& g) {
+  attach_graphs(ix.get(), "IVF_HNSW_SQ", params->max_level, params->m, params->ef_construction,
+                params->insert_batch, stats, [&](HnswGraph& g) {
     const float rf = (float)(ix->sq_upper - ix->sq_lower);
     hnsw_build(g, ix->part_offsets.p, ix->K, ix->codes.p, (int)d, ix->metric, rf * rf, params->sq.seed);
   });
@@ -829,7 +836,7 @@ lb2_status lb2_ivfhnswpq_build(const void* data, uint64_t n, uint32_t d, lb2_dty
                                lb2_build_stats* stats) {
   LB2_API_BEGIN
   LB2_REQUIRE(data && params && out, "null argument");
-  check_hnsw_params("IVF_HNSW_PQ", params->max_level, params->m, params->ef_construction);
+  check_hnsw_params("IVF_HNSW_PQ", params->max_level, params->m, params->ef_construction, params->insert_batch);
   if (comm_nranks() > 1) fail(LB2_UNSUPPORTED, "IVF_HNSW_PQ: a build over more than one rank is not implemented");
   // 1. the IVF stage, codebook and codes of IVF_PQ with the same arguments
   lb2_index* pq = nullptr;
@@ -839,7 +846,8 @@ lb2_status lb2_ivfhnswpq_build(const void* data, uint64_t n, uint32_t d, lb2_dty
   ix->slab_off.release();  // the skewed code copy serves only the IVF_PQ scan
   ix->codes_skew.release();
   // 2. HNSW::index_vectors per partition over its PQ storage (IvfIndexBuilder<HNSW, ProductQuantizer>)
-  attach_graphs(ix.get(), "IVF_HNSW_PQ", params->max_level, params->m, params->ef_construction, stats, [&](HnswGraph& g) {
+  attach_graphs(ix.get(), "IVF_HNSW_PQ", params->max_level, params->m, params->ef_construction,
+                params->insert_batch, stats, [&](HnswGraph& g) {
     hnsw_build_pq(g, ix->part_offsets.p, ix->K, ix->codes.p, ix->codebook.p, (int)d, ix->M, ix->nbits, ix->metric,
                   dtype, params->pq.seed);
   });
@@ -852,7 +860,7 @@ lb2_status lb2_ivfhnswflat_build(const void* data, uint64_t n, uint32_t d, lb2_d
                                  lb2_build_stats* stats) {
   LB2_API_BEGIN
   LB2_REQUIRE(data && params && out, "null argument");
-  check_hnsw_params("IVF_HNSW_FLAT", params->max_level, params->m, params->ef_construction);
+  check_hnsw_params("IVF_HNSW_FLAT", params->max_level, params->m, params->ef_construction, params->insert_batch);
   if (comm_nranks() > 1) fail(LB2_UNSUPPORTED, "IVF_HNSW_FLAT: a build over more than one rank is not implemented");
   // 1. the IVF stage, vectors and row ids of IVF_FLAT with the same arguments
   lb2_index* flat = nullptr;
@@ -860,7 +868,8 @@ lb2_status lb2_ivfhnswflat_build(const void* data, uint64_t n, uint32_t d, lb2_d
   if (st != LB2_OK) return st;  // its message is already the last error
   std::unique_ptr<lb2_index> ix(flat);
   // 2. HNSW::index_vectors per partition over its FlatFloatStorage (IvfIndexBuilder<HNSW, FlatQuantizer>)
-  attach_graphs(ix.get(), "IVF_HNSW_FLAT", params->max_level, params->m, params->ef_construction, stats,
+  attach_graphs(ix.get(), "IVF_HNSW_FLAT", params->max_level, params->m, params->ef_construction,
+                params->insert_batch, stats,
                 [&](HnswGraph& g) {
                   hnsw_build_flat(g, ix->part_offsets.p, ix->K, ix->vectors.p, (int)ix->vdtype(), (int)d, ix->metric,
                                   params->flat.seed);

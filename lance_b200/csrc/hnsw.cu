@@ -17,12 +17,15 @@
 //    `between` is the full-width distance of the two decoded rows (dist_between).
 //  * FLAT (flat/storage.rs:345-410): all three are the IVF_FLAT scan's rule on the stored rows, cosine included.
 //
-// One warp owns one partition (build) or one (query, partition) slot (search).  Its heaps, visited bitset and (PQ)
-// table live in a per-warp global scratch sized by the largest partition, so no partition is refused for its size.
+// One warp owns one partition (serial build), one inserting node or one back-linked list (batched build, in rounds;
+// see the round kernels) or one (query, partition) slot (search).  Its heaps, visited bitset and (PQ) table live in a
+// per-warp global scratch sized by the largest partition, so no partition is refused for its size.
 // Lane 0 runs the reference's serial heap and list updates in the reference's order; the 32 lanes compute the
 // distances of a neighbour list or of a candidate's accepted neighbours, one row per lane, and build a PQ table
 // together.  Control decisions reach the other lanes through shared memory after a __syncwarp.
 #include <algorithm>
+#include <cstdlib>
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -564,14 +567,62 @@ __device__ void prune_into(const Dist& P, const uint32_t* ids, const uint32_t* k
   __syncwarp();
 }
 
-// HNSW::index_vectors of partitions order[0 ..), taken largest first by a persistent grid of one-warp CTAs
+// the search half of HnswBuilder::insert (builder.rs:396-463) of node i: the descent, a beam search per level of the
+// node from its target level down, and the node's own lists, the pruned results.  Reads the lists the searches reach,
+// writes only node i's.
+template <class Dist>
+__device__ void insert_search(const GraphDev& g, const Dist& P, uint32_t i, uint32_t efc, int32_t lo, int32_t hi,
+                              const Scratch& s) {
+  const typename Dist::Ctx q = P.node_ctx(i, s);  // dist_calculator_from_id(node)
+  const int target = (int)g.nlev[P.off + i] - 1;
+  uint32_t ep = 0, ekey = P.key(q, 0);
+  for (int level = g.max_level - 1; level > target; --level) greedy(g, P, q, level, ep, ekey, s);
+  for (int level = target; level >= 0; --level) {
+    const uint32_t R = beam_search(g, P, q, level, ep, ekey, efc, nullptr, lo, hi, s);
+    ep = s.rid[0];
+    ekey = s.rk[0];
+    const uint32_t m_max = level == 0 ? 2 * g.m : g.m;
+    prune_into(P, s.rid, s.rk, R, m_max, list_of(g, P.off + i, level), s);
+  }
+}
+
+// one back-link of insert (builder.rs:446-460): node i, at order key `ekey` in its own list, enters `other` when it is
+// closer than the LAST entry of a full list (GraphBuilderNode::cutoff, graph/builder.rs:50-57), then `other` is pruned
+template <class Dist>
+__device__ void back_link(const Dist& P, const ListRef& other, uint32_t i, uint32_t ekey, uint32_t m_max,
+                          const Scratch& s) {
+  __shared__ uint32_t sh_go, sh_n;
+  if ((threadIdx.x & 31) == 0) {
+    const uint32_t c2 = *other.cnt;
+    const uint32_t cutoff = c2 < m_max ? KEY_INF : ukey_of(other.dist[c2 - 1]);  // the LAST entry
+    const bool add = ekey < cutoff;
+    if (add) {
+      for (uint32_t j = 0; j < c2; ++j) {
+        s.lid[j] = other.ids[j];
+        s.lk[j] = ukey_of(other.dist[j]);
+      }
+      s.lid[c2] = i;
+      s.lk[c2] = ekey;
+    }
+    sh_go = add;
+    sh_n = c2 + 1;
+  }
+  __syncwarp();
+  const bool add = sh_go;
+  const uint32_t c = sh_n;
+  __syncwarp();
+  if (add) prune_into(P, s.lid, s.lk, c, m_max, other, s);
+}
+
+// HNSW::index_vectors of partitions order[0 ..), taken largest first by a persistent grid of one-warp CTAs, each
+// inserting its partition's nodes 1 .. n_p - 1 one after the other (insert_batch 1)
 template <class Dist>
 __global__ void __launch_bounds__(32)
 hnsw_build_kernel(GraphDev g, const uint64_t* __restrict__ part_offsets, const uint32_t* __restrict__ order, int nparts,
                   uint32_t* __restrict__ next, const Dist proto, uint32_t efc, int32_t lo, int32_t hi,
                   uint32_t* __restrict__ scratch, uint64_t nmax, uint32_t E, uint32_t B, uint32_t LB, uint32_t TW,
                   uint32_t QW) {
-  __shared__ uint32_t sh_part, sh_go, sh_n;
+  __shared__ uint32_t sh_part;
   const int lane = threadIdx.x & 31;
   if (!Dist::TABLE) TW = 0;
   if (!Dist::QUERY) QW = 0;
@@ -586,47 +637,137 @@ hnsw_build_kernel(GraphDev g, const uint64_t* __restrict__ part_offsets, const u
     Dist P = proto;
     P.bind(part_offsets[p], (uint32_t)(part_offsets[p + 1] - part_offsets[p]));
     for (uint32_t i = 1; i < P.n; ++i) {  // HnswBuilder::insert (builder.rs:396-463)
-      const typename Dist::Ctx q = P.node_ctx(i, s);  // dist_calculator_from_id(node)
+      insert_search(g, P, i, efc, lo, hi, s);
       const int target = (int)g.nlev[P.off + i] - 1;
-      uint32_t ep = 0, ekey = P.key(q, 0);
-      for (int level = g.max_level - 1; level > target; --level) greedy(g, P, q, level, ep, ekey, s);
-      for (int level = target; level >= 0; --level) {
-        const uint32_t R = beam_search(g, P, q, level, ep, ekey, efc, nullptr, lo, hi, s);
-        ep = s.rid[0];
-        ekey = s.rk[0];
-        const uint32_t m_max = level == 0 ? 2 * g.m : g.m;
-        prune_into(P, s.rid, s.rk, R, m_max, list_of(g, P.off + i, level), s);
-      }
       for (int level = 0; level <= target; ++level) {  // the back-links, level by level, in pruned-list order
         const uint32_t m_max = level == 0 ? 2 * g.m : g.m;
         const ListRef mine = list_of(g, P.off + i, level);
         const uint32_t cm = *mine.cnt;
-        for (uint32_t e = 0; e < cm; ++e) {
-          const uint32_t eid = mine.ids[e];
-          const ListRef other = list_of(g, P.off + eid, level);
-          if (lane == 0) {
-            const uint32_t ekey2 = ukey_of(mine.dist[e]);
-            const uint32_t c2 = *other.cnt;
-            const uint32_t cutoff = c2 < m_max ? KEY_INF : ukey_of(other.dist[c2 - 1]);  // the LAST entry
-            const bool add = ekey2 < cutoff;
-            if (add) {
-              for (uint32_t j = 0; j < c2; ++j) {
-                s.lid[j] = other.ids[j];
-                s.lk[j] = ukey_of(other.dist[j]);
-              }
-              s.lid[c2] = i;
-              s.lk[c2] = ekey2;
-            }
-            sh_go = add;
-            sh_n = c2 + 1;
-          }
-          __syncwarp();
-          const bool add = sh_go;
-          const uint32_t c = sh_n;
-          __syncwarp();
-          if (add) prune_into(P, s.lid, s.lk, c, m_max, other, s);
-        }
+        for (uint32_t e = 0; e < cm; ++e)
+          back_link(P, list_of(g, P.off + mine.ids[e], level), i, ukey_of(mine.dist[e]), m_max, s);
       }
+    }
+  }
+}
+
+// ---- the batched build (insert_batch B >= 2): rounds of concurrent inserts --------------------------------------
+// A round inserts nodes s0 .. s0 + W - 1 of every partition order[0 .. nparts) (each clipped to its rows), item t
+// being node s0 + t % W of partition order[t / W].  Phase 1 (hnsw_round_search_kernel) runs every item's
+// insert_search over the graph as the round found it: no list names a node of the round yet, so it reads lists of
+// nodes < s0 only and writes only the round's own lists.  Phase 2 applies the back-links as if the round's nodes
+// had linked back one after the other in ascending order: a list (j, level) receives at most one entry per node, and
+// lists are independent, so each target list takes its entries in ascending node order, distinct lists in parallel.
+// hnsw_round_link_kernel chains every back-link onto its target list (head[list] -> rec_next ...) and names each
+// target list once in `touched`; hnsw_round_apply_kernel gives each touched list to one warp, which orders the
+// chain by node and applies back_link entry by entry.
+
+struct RoundBufs {
+  uint32_t* counters;  // [0] the next phase-1 item, [1] records, [2] touched lists
+  uint32_t* head;      // [n + n_up] the last record of each list's chain, NONE when empty
+  uint32_t *rec_i, *rec_key, *rec_next;
+  uint32_t* touched;   // [3][..]: partition, node, level of each touched list
+};
+
+// the list number of (global row, level): level 0 by row, the upper levels after every level-0 list
+__device__ __forceinline__ uint64_t list_number(const GraphDev& g, uint64_t n, uint64_t row, int level) {
+  return level == 0 ? row : n + g.up_base[row] + (level - 1);
+}
+
+template <class Dist>
+__global__ void __launch_bounds__(32)
+hnsw_round_search_kernel(GraphDev g, const uint64_t* __restrict__ part_offsets, const uint32_t* __restrict__ order,
+                         uint32_t nparts, uint32_t s0, uint32_t W, RoundBufs rb, const Dist proto, uint32_t efc,
+                         int32_t lo, int32_t hi, uint32_t* __restrict__ scratch, uint64_t nmax, uint32_t E, uint32_t B,
+                         uint32_t LB, uint32_t TW, uint32_t QW) {
+  __shared__ uint32_t sh_t;
+  const int lane = threadIdx.x & 31;
+  if (!Dist::TABLE) TW = 0;
+  if (!Dist::QUERY) QW = 0;
+  const Scratch s = scratch_at(scratch + blockIdx.x * scratch_words(nmax, E, B, LB, TW, QW), nmax, E, B, LB, TW, QW);
+  const uint32_t items = nparts * W;
+  for (;;) {
+    if (lane == 0) sh_t = atomicAdd(rb.counters, 1u);
+    __syncwarp();
+    const uint32_t t = sh_t;
+    __syncwarp();
+    if (t >= items) return;
+    const uint32_t p = order[t / W], i = s0 + t % W;
+    Dist P = proto;
+    P.bind(part_offsets[p], (uint32_t)(part_offsets[p + 1] - part_offsets[p]));
+    if (i < P.n) insert_search(g, P, i, efc, lo, hi, s);
+  }
+}
+
+// one thread per item: every entry of the item's lists becomes a record on its target list's chain
+__global__ void hnsw_round_link_kernel(GraphDev g, uint64_t n, const uint64_t* __restrict__ part_offsets,
+                                       const uint32_t* __restrict__ order, uint32_t nparts, uint32_t s0, uint32_t W,
+                                       RoundBufs rb) {
+  const uint64_t t = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (uint64_t)nparts * W) return;
+  const uint32_t p = order[t / W], i = s0 + (uint32_t)(t % W);
+  const uint64_t off = part_offsets[p];
+  if (i >= part_offsets[p + 1] - off) return;
+  const int target = (int)g.nlev[off + i] - 1;
+  for (int level = 0; level <= target; ++level) {
+    const ListRef mine = list_of(g, off + i, level);
+    const uint32_t cm = *mine.cnt;
+    for (uint32_t e = 0; e < cm; ++e) {
+      const uint32_t eid = mine.ids[e];
+      const uint32_t r = atomicAdd(rb.counters + 1, 1u);
+      rb.rec_i[r] = i;
+      rb.rec_key[r] = ukey_of(mine.dist[e]);
+      const uint32_t prev = atomicExch(rb.head + list_number(g, n, off + eid, level), r);
+      rb.rec_next[r] = prev;
+      if (prev == NONE) {  // the first record of this list: name the list once
+        const uint32_t u = atomicAdd(rb.counters + 2, 1u);
+        rb.touched[3 * (uint64_t)u] = p;
+        rb.touched[3 * (uint64_t)u + 1] = eid;
+        rb.touched[3 * (uint64_t)u + 2] = (uint32_t)level;
+      }
+    }
+  }
+}
+
+// one warp per touched list: its chain ordered by node (each node appears once), then back_link in that order; the
+// list's chain head goes back to NONE for the next round
+template <class Dist>
+__global__ void __launch_bounds__(32)
+hnsw_round_apply_kernel(GraphDev g, uint64_t n, const uint64_t* __restrict__ part_offsets, RoundBufs rb,
+                        const Dist proto, uint32_t* __restrict__ scratch, uint64_t nmax, uint32_t E, uint32_t B,
+                        uint32_t LB, uint32_t TW, uint32_t QW) {
+  __shared__ uint32_t sh_c;
+  const int lane = threadIdx.x & 31;
+  if (!Dist::TABLE) TW = 0;
+  if (!Dist::QUERY) QW = 0;
+  const Scratch s = scratch_at(scratch + blockIdx.x * scratch_words(nmax, E, B, LB, TW, QW), nmax, E, B, LB, TW, QW);
+  const uint32_t nt = rb.counters[2];
+  for (uint32_t u = blockIdx.x; u < nt; u += gridDim.x) {
+    const uint32_t p = rb.touched[3 * (uint64_t)u], j = rb.touched[3 * (uint64_t)u + 1];
+    const int level = (int)rb.touched[3 * (uint64_t)u + 2];
+    Dist P = proto;
+    P.bind(part_offsets[p], (uint32_t)(part_offsets[p + 1] - part_offsets[p]));
+    const uint64_t ln = list_number(g, n, P.off + j, level);
+    if (lane == 0) {  // the chain, at most one record per node of the round (< n_p <= nmax), into ck
+      uint32_t c = 0;
+      for (uint32_t r = rb.head[ln]; r != NONE; r = rb.rec_next[r]) s.ck[c++] = r;
+      rb.head[ln] = NONE;
+      sh_c = c;
+    }
+    __syncwarp();
+    const uint32_t c = sh_c;
+    __syncwarp();
+    for (uint32_t a = lane; a < c; a += 32) {  // rank by node: the nodes are distinct, so the ranks are a permutation
+      const uint32_t ra = s.ck[a], ia = rb.rec_i[ra];
+      uint32_t rank = 0;
+      for (uint32_t b = 0; b < c; ++b) rank += rb.rec_i[s.ck[b]] < ia;
+      s.cid[rank] = ra;
+    }
+    __syncwarp();
+    const ListRef other = list_of(g, P.off + j, level);
+    const uint32_t m_max = level == 0 ? 2 * g.m : g.m;
+    for (uint32_t k = 0; k < c; ++k) {
+      const uint32_t r = s.cid[k];
+      back_link(P, other, rb.rec_i[r], rb.rec_key[r], m_max, s);
     }
   }
 }
@@ -847,16 +988,72 @@ static void build_graphs(HnswGraph& g, const uint64_t* part_offsets, int K, uint
   }
   const uint32_t E = (uint32_t)g.ef_construction, B = 2 * (uint32_t)g.m + 1, LB = std::max(E, B);
   const size_t words = scratch_words(nmax, E, B, LB, TW, QW);
-  // one warp per partition, at most 32 per SM, and no more warps than 512 MB of scratch holds
+  // one warp per work item, at most 32 per SM, and no more warps than 512 MB of scratch holds
   const size_t fit = std::max<size_t>(1, (512ull << 20) / (words * 4));
-  const unsigned nct = (unsigned)std::min<size_t>({order.size(), (size_t)ctx().num_sms * 32, fit});
-  DevBuf<uint32_t> scratch(words * nct), dorder(order.size()), next(1);
+  DevBuf<uint32_t> dorder(order.size());
   h2d(dorder.p, order.data(), order.size());
-  next.zero();
   const int32_t lo = key_of_host(-3.40282347e+38f), hi = key_of_host(3.40282347e+38f);  // f32::MIN, f32::MAX
-  launch([&](auto kern, const auto& P) {
-    LB2_LAUNCH("hnsw_build", kern, nct, 32, 0, dev_view(g), part_offsets, dorder.p, (int)order.size(), next.p, P, E,
-               lo, hi, scratch.p, nmax, E, B, LB, TW, QW);
+  const uint32_t batch = std::max<uint32_t>(g.insert_batch, 1);
+  // LB2_HNSW_ROUNDS=1: insert_batch 1 through the round driver too (the same graph; for timing it against the serial
+  // kernel).  Read on every call.
+  const char* env_rounds = getenv("LB2_HNSW_ROUNDS");
+  if (batch == 1 && !(env_rounds && *env_rounds && *env_rounds != '0')) {
+    const unsigned nct = (unsigned)std::min<size_t>({order.size(), (size_t)ctx().num_sms * 32, fit});
+    DevBuf<uint32_t> scratch(words * nct), next(1);
+    next.zero();
+    launch([&](const auto& P) {
+      using Dist = std::decay_t<decltype(P)>;
+      LB2_LAUNCH("hnsw_build", hnsw_build_kernel<Dist>, nct, 32, 0, dev_view(g), part_offsets, dorder.p,
+                 (int)order.size(), next.p, P, E, lo, hi, scratch.p, nmax, E, B, LB, TW, QW);
+    });
+    sync_stream();
+    return;
+  }
+  // The rounds: starting at s = 1, a round inserts nodes s .. s + min(batch, s) - 1 of every partition that has them,
+  // so rounds hold 1, 2, 4, .. nodes, then `batch`.  `order` is largest first, so a round's partitions are a prefix.
+  // Size the round buffers by the largest round: its items, and the entries its nodes' lists can hold.
+  struct Round {
+    uint32_t s0, W, nparts;
+  };
+  std::vector<Round> rounds;
+  uint64_t max_items = 0, max_recs = 0;
+  {
+    const uint64_t top = off[order[0] + 1] - off[order[0]];
+    uint32_t np_r = (uint32_t)order.size();
+    for (uint64_t s0 = 1; s0 < top;) {
+      const uint64_t W = std::min<uint64_t>(batch, s0);
+      while (np_r > 0 && off[order[np_r - 1] + 1] - off[order[np_r - 1]] <= s0) --np_r;
+      uint64_t recs = 0;
+      for (uint32_t t = 0; t < np_r; ++t) {
+        const uint64_t a = off[order[t]], np_ = off[order[t] + 1] - a;
+        for (uint64_t i = s0; i < std::min(np_, s0 + W); ++i) recs += 2 * (uint64_t)g.m + (uint64_t)g.m * (nlev[a + i] - 1);
+      }
+      rounds.push_back({(uint32_t)s0, (uint32_t)W, np_r});
+      max_items = std::max(max_items, (uint64_t)np_r * W);
+      max_recs = std::max(max_recs, recs);
+      s0 += W;
+    }
+  }
+  LB2_REQUIRE(max_items < 0xffffffffull && max_recs < 0xffffffffull, "%s: a round of more than 2^32 - 1 back-links",
+              g.kind);
+  const unsigned nct = (unsigned)std::min<size_t>({(size_t)max_items, (size_t)ctx().num_sms * 32, fit});
+  DevBuf<uint32_t> scratch(words * nct), counters(3), head(n + n_up), rec_i(max_recs), rec_key(max_recs),
+      rec_next(max_recs), touched(3 * max_recs);
+  LB2_CUDA(cudaMemsetAsync(head.p, 0xff, head.n * sizeof(uint32_t), ctx().stream));  // every chain empty (NONE)
+  const RoundBufs rb{counters.p, head.p, rec_i.p, rec_key.p, rec_next.p, touched.p};
+  launch([&](const auto& P) {
+    using Dist = std::decay_t<decltype(P)>;
+    for (const Round& r : rounds) {
+      const uint64_t items = (uint64_t)r.nparts * r.W;
+      counters.zero();
+      LB2_LAUNCH("hnsw_round_search", hnsw_round_search_kernel<Dist>, (unsigned)std::min<uint64_t>(items, nct), 32, 0,
+                 dev_view(g), part_offsets, dorder.p, r.nparts, r.s0, r.W, rb, P, E, lo, hi, scratch.p, nmax, E, B, LB,
+                 TW, QW);
+      LB2_LAUNCH("hnsw_round_link", hnsw_round_link_kernel, (unsigned)cdiv(items, 128), 128, 0, dev_view(g), n,
+                 part_offsets, dorder.p, r.nparts, r.s0, r.W, rb);
+      LB2_LAUNCH("hnsw_round_apply", hnsw_round_apply_kernel<Dist>, nct, 32, 0, dev_view(g), n, part_offsets, rb, P,
+                 scratch.p, nmax, E, B, LB, TW, QW);
+    }
   });
   sync_stream();
 }
@@ -869,7 +1066,7 @@ void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t
       P.base = codes;
       P.d = d;
       P.r2 = r2;
-      go(hnsw_build_kernel<SqDist<decltype(m)::value>>, P);
+      go(P);
     };
     if (metric == METRIC_DOT) with(std::integral_constant<int, METRIC_DOT>{});
     else with(std::integral_constant<int, METRIC_L2>{});  // cosine: L2 on the normalised vectors' codes
@@ -908,7 +1105,7 @@ void hnsw_build_flat(HnswGraph& g, const uint64_t* part_offsets, int K, const vo
       Dist P{};
       P.base = static_cast<const T*>(vectors);
       P.d = d;
-      go(hnsw_build_kernel<Dist>, P);
+      go(P);
     });
   });
 }
@@ -925,7 +1122,7 @@ void hnsw_build_pq(HnswGraph& g, const uint64_t* part_offsets, int K, const uint
       P.M = M;
       P.ds = d / M;
       P.cw = nbits == 4 ? M / 2 : M;
-      go(hnsw_build_kernel<Dist>, P);
+      go(P);
     });
   });
 }

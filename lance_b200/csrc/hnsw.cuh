@@ -18,7 +18,8 @@ struct IvfSearch;
 struct HnswGraph {
   const char* kind = "IVF_HNSW_SQ";  // the index kind's name in messages: IVF_HNSW_SQ, IVF_HNSW_PQ or IVF_HNSW_FLAT
   int max_level = 0, m = 0, ef_construction = 0;
-  uint64_t max_part = 0;  // rows of the largest partition (scratch sizing)
+  uint32_t insert_batch = 1;  // B of the batched build (1: serial; a loaded graph records 1)
+  uint64_t max_part = 0;      // rows of the largest partition (scratch sizing)
   uint64_t n_up = 0;      // upper-level rows
   DevBuf<uint8_t> nlev;
   DevBuf<uint32_t> up_base, cnt0, nbr0, cntu, nbru;
@@ -47,7 +48,8 @@ struct HnswKeep {
   std::vector<int64_t> src;       // [new K]: old partition id, or -1 = build this partition
 };
 
-// HNSW::index_vectors (builder.rs:742-775) of every partition, nodes inserted 1 .. n_p - 1 in ascending order;
+// HNSW::index_vectors (builder.rs:742-775) of every partition, nodes inserted 1 .. n_p - 1 in ascending order, or in
+// rounds of up to g.insert_batch concurrent inserts when it is above 1 (the round definition of include/lance_b200.h);
 // codes [n][d] in partition order, part_offsets on the device.  Fills g (its parameters set by the caller).  With
 // `keep`, only the partitions keep->src marks -1 are built; the others are spliced from keep->old.
 void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, int d, int metric, float r2,

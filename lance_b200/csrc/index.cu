@@ -551,6 +551,8 @@ static std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_op
   LB2_REQUIRE(p.n_remap == 0 || (p.remap_old_ids && p.remap_new_ids), "%s: null remap list", what);
   if (old->hnsw && comm_nranks() > 1)
     fail(LB2_UNSUPPORTED, "%s: %s indexes over more than one rank are not implemented", what, old->hnsw->kind);
+  if (old->hnsw)
+    LB2_REQUIRE(p.insert_batch <= 65536, "%s: insert_batch must be at most 65536, got %u", what, p.insert_batch);
   const int rb = (int)old->row_bytes();
   const uint64_t n_old = old->n, n_add = p.n_add, n_all = n_old + n_add;
   LB2_REQUIRE(n_all < 0xffffffffull, "more than 2^32-1 rows per index shard");
@@ -620,6 +622,7 @@ static std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_op
     g.max_level = og.max_level;
     g.m = og.m;
     g.ef_construction = og.ef_construction;
+    g.insert_batch = p.insert_batch ? p.insert_batch : og.insert_batch;
     TagScope tg("hnsw_build");
     switch (ix->kind) {
       case IndexKind::SQ: {
