@@ -137,7 +137,8 @@ lb2_status lb2_compute_residual(const void* centroids, uint32_t k, uint32_t d, l
 
 /* ---- product quantisation (lance-index/src/vector/pq*.rs) ------------------------------------ */
 typedef struct {
-  uint32_t num_sub_vectors; /* PQBuildParams (pq/builder.rs:27-59): 16 */
+  uint32_t num_sub_vectors; /* PQBuildParams (pq/builder.rs:27-59): 16; any divisor of d (every sub-vector width
+                               d / num_sub_vectors has an exact device route) */
   uint32_t num_bits;        /* 8 or 4 */
   uint32_t max_iters;       /* 50 */
   uint32_t kmeans_redos;    /* 1 (PQ k-means has no balance bias: any value equals one run, see redos above) */
@@ -148,7 +149,8 @@ typedef struct {
 void lb2_pq_params_default(lb2_pq_params* p);
 
 /* PQBuildParams::build(data, distance_type) -> ProductQuantizer (pq/builder.rs:162-194):
- * codebook_out is the flat [M][2^nbits][d/M] layout of pq/utils.rs:59-76; iters_out[M] nullable. */
+ * codebook_out is the flat [M][2^nbits][d/M] layout of pq/utils.rs:59-76; iters_out[M] nullable.  Every M that
+ * divides d trains on the device, at every sub-vector width d / M. */
 lb2_status lb2_pq_train(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype,
                         lb2_metric metric, const lb2_pq_params* params, void* codebook_out,
                         uint32_t* iters_out);
@@ -157,7 +159,8 @@ lb2_status lb2_pq_train(const void* data, uint64_t n, uint32_t d, lb2_dtype dtyp
  * ([num_centroids][d]) and `part_ids` are given the residual (residual.rs:161-205) is fused: codes of
  * v - centroids[part]; a part id >= num_centroids is LB2_INVALID_ARG.
  * codes_out is row-major [n][M] (8-bit) or [n][M/2] (4-bit: byte i = code[2i+1] << 4 | code[2i],
- * pq.rs:168-173; 16 codewords per sub-space, M even). */
+ * pq.rs:168-173; 16 codewords per sub-space, M even).  Every sub-vector width d / M is encoded exactly (the
+ * reference's 16-lane order from width 16 on). */
 lb2_status lb2_pq_encode(const void* codebook, uint32_t num_sub_vectors, uint32_t num_bits,
                          uint32_t d, lb2_dtype dtype, lb2_metric metric, const void* centroids,
                          uint32_t num_centroids, const uint32_t* part_ids, const void* vectors, uint64_t n,
@@ -227,7 +230,9 @@ lb2_status lb2_flat_search(const void* vectors, uint64_t n, uint32_t d, lb2_dtyp
  * `metric` is the index metric: it selects the partition assignment and whether residuals are taken
  * (not for dot, PQBuildParams::use_residual); the PQ codes are L2 codes in every case, because the
  * index builder trains its quantizer with DistanceType::L2 (rust/lance/src/index/vector/builder.rs:460).
- * valid_out[i] = 0 marks rows KeepFiniteVectors would drop (transform.rs:112-159). */
+ * valid_out[i] = 0 marks rows KeepFiniteVectors would drop (transform.rs:112-159).  Any num_sub_vectors that divides
+ * d, as lb2_pq_encode; so lb2_index_transform and lb2_index_optimize maintain IVF_PQ and IVF_HNSW_PQ indexes of every
+ * sub-vector width, reference-built ones included. */
 lb2_status lb2_ivfpq_transform(const void* centroids, uint32_t k, const void* codebook,
                                uint32_t num_sub_vectors, uint32_t num_bits, uint32_t d,
                                lb2_dtype dtype, lb2_metric metric, const void* vectors, uint64_t n,

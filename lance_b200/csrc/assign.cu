@@ -5,12 +5,16 @@
 //   compute_partitions_with_dists                   kmeans.rs:1275-1294
 //   compute_partition (PQ code assignment)          kmeans.rs:1350-1369, pq.rs:148-178
 //   l2_distance_batch / dot_distance_batch          lance-linalg/src/distance/l2.rs:194, dot.rs:164
-// Three kernels, all producing bit-identical distances to the reference's 16-lane scalar loops:
+// Four kernels, all producing bit-identical distances to the reference's 16-lane scalar loops:
 //   (a) assign_tile_kernel   d % 16 == 0, d <= 256: 64 rows x 64 centroids per tile, 4x4 per thread,
 //       lane-outer / chunk-inner so only two accumulators per pair are live;
 //   (b) small_d_kernel       d < 16 (PQ sub-vectors, tail-only path of l2.rs:69-79), batched over
 //       the M sub-spaces, optional fused residual (residual.rs:86-95), u8 codes or u32 ids out;
-//   (c) generic_kernel       any d: half-warp per centroid, lane l owns lane-accumulator l.
+//   (c) generic_kernel       any d: half-warp per centroid, lane l owns lane-accumulator l;
+//   (d) pq_wide_kernel       PQ sub-vectors of 16 <= ds <= 256: (a)'s tile and order plus the sequential
+//       tail, with (b)'s batching over the sub-spaces, fused residual and outputs.
+// pq_assign_f32 gives every PQ sub-vector width a route: (b) below 16, (d) up to 256, and wider sub-spaces
+// one at a time through assign_f32_ex on a contiguous copy.
 #include "assign.cuh"
 #include "common.cuh"
 #include "exact.cuh"
@@ -19,12 +23,15 @@
 namespace lb2 {
 
 // ------------------------------------------------------------------------------------------------
-// transposed, padded copy of the centroids: cT[e][Kp], pad columns = NaN (never win an argmin)
+// transposed, padded copy of the centroids: cT[e][Kp], pad columns = NaN (never win an argmin).
+// blockIdx.y selects one of a batch of such matrices (the M codebooks of a product quantizer)
 // ------------------------------------------------------------------------------------------------
 __global__ void transpose_pad_kernel(const float* __restrict__ c, int K, int d, int Kp,
                                      float* __restrict__ cT) {
   int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= d * Kp) return;
+  c += (size_t)blockIdx.y * K * d;
+  cT += (size_t)blockIdx.y * d * Kp;
   int e = idx / Kp, k = idx % Kp;
   cT[idx] = k < K ? c[(size_t)k * d + e] : __int_as_float(0x7fc00000);
 }
@@ -406,6 +413,166 @@ generic_kernel(const float* __restrict__ x, uint64_t n, int d, const float* __re
 }
 
 // ------------------------------------------------------------------------------------------------
+// (d) wide PQ kernel (16 <= ds <= 256: the reference's full order, l2.rs:57-91 / dot.rs:30-58, restated in
+//   dist_exact_thread): per (row, codeword) pair the 16 lane sums in chunk order, added in lane order (t), the
+//   tail ds & ~15 .. ds-1 summed left to right (s), then s + t.
+//   grid = (row tiles of 64, M), 4 rows x 4 codewords per thread as in (a): lane-outer / chunk-inner, so only the
+//   lane and total accumulators are live, then the tail.  The tile's rows (residuals when ivf_centroids is given)
+//   and 64-codeword tiles of cbT ([M][ds][Kp], NaN pad columns, transpose_pad_kernel) are staged in shared memory.
+//   Outputs, tie rule and row_valid as in (b).
+// ------------------------------------------------------------------------------------------------
+template <int METRIC, bool CODES>
+__global__ void __launch_bounds__(256)
+pq_wide_kernel(const float* __restrict__ x, uint64_t n, int ldx, int ds, const float* __restrict__ cbT, int Kp,
+               const float* __restrict__ ivf_centroids, const uint32_t* __restrict__ part_ids,
+               const uint8_t* __restrict__ row_valid, uint8_t* __restrict__ codes, int M,
+               uint32_t* __restrict__ ids, float* __restrict__ dists, uint8_t* __restrict__ valid,
+               const uint8_t* __restrict__ active) {
+  const int m = blockIdx.y;
+  if (active && !active[m]) return;
+  extern __shared__ float smem[];
+  const int ld = ds + 1;
+  float* xs = smem;            // [64][ds+1]
+  float* cs = smem + 64 * ld;  // [ds][64] (64 * ld floats: 16-byte aligned)
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const uint64_t row0 = (uint64_t)blockIdx.x * 64;
+  // scalar loads: neither the row stride nor m * ds need be a multiple of 4
+  for (int idx = tid; idx < 64 * ds; idx += 256) {
+    const int r = idx / ds, t = idx - r * ds;
+    float v = 0.0f;
+    if (row0 + r < n) {
+      v = x[(row0 + r) * (uint64_t)ldx + (uint64_t)m * ds + t];
+      if (ivf_centroids)  // residual.rs:93
+        v = __fsub_rn(v, ivf_centroids[(uint64_t)part_ids[row0 + r] * ldx + (uint64_t)m * ds + t]);
+    }
+    xs[r * ld + t] = v;
+  }
+  const float* cb = cbT + (size_t)m * ds * Kp;
+  const float* xrow = xs + (ty * 4) * ld;
+  const int nchunk = ds >> 4, n16 = ds & ~15;
+  float best_val[4];
+  uint32_t best_idx[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    best_val[i] = __int_as_float(0x7f800000);
+    best_idx[i] = 0xffffffffu;
+  }
+  for (int ct = 0; ct < Kp; ct += 64) {
+    __syncthreads();
+    for (int idx = tid; idx < ds * 16; idx += 256) {
+      const int e = idx >> 4, q = idx & 15;
+      *reinterpret_cast<float4*>(cs + e * 64 + q * 4) =
+          *reinterpret_cast<const float4*>(cb + (size_t)e * Kp + ct + q * 4);
+    }
+    __syncthreads();
+    float total[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) total[i][j] = 0.0f;
+    for (int l = 0; l < 16; ++l) {
+      float acc[4][4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = 0.0f;
+#pragma unroll 2
+      for (int c = 0; c < nchunk; ++c) {
+        const int e = c * 16 + l;
+        const float4 cv = *reinterpret_cast<const float4*>(cs + e * 64 + tx * 4);
+        float xv[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) xv[i] = xrow[i * ld + e];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          acc[i][0] = f_add(acc[i][0], term<METRIC>(xv[i], cv.x));
+          acc[i][1] = f_add(acc[i][1], term<METRIC>(xv[i], cv.y));
+          acc[i][2] = f_add(acc[i][2], term<METRIC>(xv[i], cv.z));
+          acc[i][3] = f_add(acc[i][3], term<METRIC>(xv[i], cv.w));
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) total[i][j] = f_add(total[i][j], acc[i][j]);
+    }
+    float s[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) s[i][j] = 0.0f;
+    for (int e = n16; e < ds; ++e) {
+      const float4 cv = *reinterpret_cast<const float4*>(cs + e * 64 + tx * 4);
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float xv = xrow[i * ld + e];
+        s[i][0] = f_add(s[i][0], term<METRIC>(xv, cv.x));
+        s[i][1] = f_add(s[i][1], term<METRIC>(xv, cv.y));
+        s[i][2] = f_add(s[i][2], term<METRIC>(xv, cv.z));
+        s[i][3] = f_add(s[i][3], term<METRIC>(xv, cv.w));
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const float v = finish<METRIC>(f_add(s[i][j], total[i][j]));
+        const uint32_t cidx = ct + tx * 4 + j;
+        if (v < best_val[i]) {  // ascending codewords, strict <: the first minimum; NaN never wins
+          best_val[i] = v;
+          best_idx[i] = cidx;
+        }
+      }
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+#pragma unroll
+    for (int off = 8; off >= 1; off >>= 1) {
+      float ov = __shfl_xor_sync(0xffffffffu, best_val[i], off);
+      uint32_t oi = __shfl_xor_sync(0xffffffffu, best_idx[i], off);
+      if (better(ov, oi, best_val[i], best_idx[i])) {
+        best_val[i] = ov; best_idx[i] = oi;
+      }
+    }
+    const uint64_t r = row0 + ty * 4 + i;
+    if (tx == 0 && r < n) {
+      const bool ok = best_idx[i] != 0xffffffffu;
+      if (CODES) {
+        const bool rv = row_valid ? row_valid[r] != 0 : true;
+        codes[r * (uint64_t)M + m] = (ok && rv) ? (uint8_t)best_idx[i] : (uint8_t)0;
+      } else {
+        ids[(uint64_t)m * n + r] = ok ? best_idx[i] : 0u;
+        if (dists) dists[(uint64_t)m * n + r] = ok ? best_val[i] : __int_as_float(0x7fc00000);
+        if (valid) valid[(uint64_t)m * n + r] = ok ? 1 : 0;
+      }
+    }
+  }
+}
+
+// sub-space m of rows [0, n) as contiguous [n][ds] rows (residuals when cent is given): the route for
+// sub-vectors wider than pq_wide_kernel's tile hands them to assign_f32_ex one sub-space at a time
+__global__ void pq_subspace_copy_kernel(const float* __restrict__ x, uint64_t n, int ldx, int ds, int m,
+                                        const float* __restrict__ cent, const uint32_t* __restrict__ part,
+                                        float* __restrict__ out) {
+  const uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (g >= n * ds) return;
+  const uint64_t r = g / ds;
+  const uint64_t col = (uint64_t)m * ds + g % ds;
+  const float v = x[r * ldx + col];
+  out[g] = cent ? __fsub_rn(v, cent[(uint64_t)part[r] * ldx + col]) : v;  // residual.rs:93
+}
+
+// sub-space m's codes from an assignment: pq.rs:165 `unwrap_or(0)`, zero for rows row_valid drops
+__global__ void pq_subspace_codes_kernel(const uint32_t* __restrict__ ids, const uint8_t* __restrict__ ok,
+                                         const uint8_t* __restrict__ row_valid, uint64_t n, int M, int m,
+                                         uint8_t* __restrict__ codes) {
+  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n) return;
+  const bool rv = row_valid ? row_valid[r] != 0 : true;
+  codes[r * M + m] = (ok[r] && rv) ? (uint8_t)ids[r] : (uint8_t)0;
+}
+
+// ------------------------------------------------------------------------------------------------
 // host dispatch
 // ------------------------------------------------------------------------------------------------
 template <int METRIC, bool WRITE_ALL>
@@ -567,13 +734,78 @@ static void small_d_launch(const float* x, uint64_t n, int ldx, int M, const flo
                codebook, Kc, ivf_centroids, part_ids, row_valid, codes, M, ids, dists, valid, active);
 }
 
-bool small_d_supported(int ds) { return ds == 1 || ds == 2 || ds == 4 || ds == 8 || ds == 12; }
+template <int METRIC>
+static void pq_wide_launch(const float* x, uint64_t n, int ldx, int M, int ds, const float* codebook, int Kc,
+                           const float* ivf_centroids, const uint32_t* part_ids, const uint8_t* row_valid,
+                           uint8_t* codes, uint32_t* ids, float* dists, uint8_t* valid, const uint8_t* active,
+                           PqAssignWorkspace& ws) {
+  const int Kp = (Kc + 63) / 64 * 64;
+  if (ws.cbT.n < (size_t)M * ds * Kp) ws.cbT.alloc((size_t)M * ds * Kp);
+  LB2_LAUNCH("pq_codebook_transpose", transpose_pad_kernel, dim3(cdiv((uint64_t)ds * Kp, 256), M), 256, 0, codebook,
+             Kc, ds, Kp, ws.cbT.p);
+  const size_t smem = sizeof(float) * (64 * (size_t)(ds + 1) + (size_t)ds * 64);
+  const dim3 grid(cdiv(n, 64), M);
+#define LB2_WIDE(CODESV)                                                                                    \
+  do {                                                                                                      \
+    set_smem(pq_wide_kernel<METRIC, CODESV>, smem);                                                         \
+    LB2_LAUNCH("pq_assign_wide", (pq_wide_kernel<METRIC, CODESV>), grid, 256, smem, x, n, ldx, ds, ws.cbT.p, \
+               Kp, ivf_centroids, part_ids, row_valid, codes, M, ids, dists, valid, active);               \
+  } while (0)
+  if (codes) LB2_WIDE(true); else LB2_WIDE(false);
+#undef LB2_WIDE
+}
 
-void small_d_assign_f32(const float* x, uint64_t n, int ldx, int M, int ds, const float* codebook,
-                        int Kc, int metric, const float* ivf_centroids, const uint32_t* part_ids,
-                        const uint8_t* row_valid, uint8_t* codes, uint32_t* ids, float* dists,
-                        uint8_t* valid, const uint8_t* active) {
+// sub-vectors wider than the wide kernel's tile: each sub-space's rows as a contiguous matrix through the exact IVF
+// assignment (tensor-core filter + exact re-rank where it applies), which computes the same reference-order
+// distances, keeps the same first minimum and marks a row without a finite winner with valid = 0
+static void pq_assign_by_subspace(const float* x, uint64_t n, int ldx, int M, int ds, const float* codebook, int Kc,
+                                  int metric, const float* ivf_centroids, const uint32_t* part_ids,
+                                  const uint8_t* row_valid, uint8_t* codes, uint32_t* ids, float* dists,
+                                  uint8_t* valid, const uint8_t* active, PqAssignWorkspace& ws) {
+  const uint64_t chunk = std::min<uint64_t>(n, std::max<uint64_t>(1ull << 16, (1ull << 28) / (uint64_t)ds));  // <= 1 GB
+  if (ws.sub.n < chunk * ds) ws.sub.alloc(chunk * ds);
+  if (codes && ws.ids.n < chunk) {
+    ws.ids.alloc(chunk);
+    ws.ok.alloc(chunk);
+  }
+  for (uint64_t r0 = 0; r0 < n; r0 += chunk) {
+    const uint64_t rows = std::min(chunk, n - r0);
+    for (int m = 0; m < M; ++m) {
+      LB2_LAUNCH("pq_subspace_copy", pq_subspace_copy_kernel, cdiv(rows * ds, 256), 256, 0, x + r0 * ldx, rows, ldx,
+                 ds, m, ivf_centroids, part_ids ? part_ids + r0 : nullptr, ws.sub.p);
+      ws.tc.norm_src = nullptr;  // the buffer holds another sub-space now: its cached row norms are stale
+      const float* cb = codebook + (size_t)m * Kc * ds;
+      if (codes) {
+        assign_f32_ex(ws.sub.p, rows, ds, cb, Kc, metric, nullptr, ws.ids.p, nullptr, ws.ok.p, nullptr, ws.tc);
+        LB2_LAUNCH("pq_subspace_codes", pq_subspace_codes_kernel, cdiv(rows, 256), 256, 0, ws.ids.p, ws.ok.p,
+                   row_valid ? row_valid + r0 : nullptr, rows, M, m, codes + r0 * M);
+      } else {
+        const uint64_t o = (uint64_t)m * n + r0;
+        assign_f32_ex(ws.sub.p, rows, ds, cb, Kc, metric, nullptr, ids + o, dists ? dists + o : nullptr,
+                      valid ? valid + o : nullptr, active ? active + m : nullptr, ws.tc);
+      }
+    }
+  }
+}
+
+void pq_assign_f32(const float* x, uint64_t n, int ldx, int M, int ds, const float* codebook, int Kc, int metric,
+                   const float* ivf_centroids, const uint32_t* part_ids, const uint8_t* row_valid, uint8_t* codes,
+                   uint32_t* ids, float* dists, uint8_t* valid, const uint8_t* active, PqAssignWorkspace* ws) {
   if (n == 0) return;
+  if (ds >= 16) {
+    PqAssignWorkspace local;  // stream-ordered frees: nothing to wait for on return
+    PqAssignWorkspace& w = ws ? *ws : local;
+    if (ds > PQ_WIDE_MAX_DS)
+      pq_assign_by_subspace(x, n, ldx, M, ds, codebook, Kc, metric, ivf_centroids, part_ids, row_valid, codes, ids,
+                            dists, valid, active, w);
+    else if (metric == METRIC_DOT)
+      pq_wide_launch<METRIC_DOT>(x, n, ldx, M, ds, codebook, Kc, ivf_centroids, part_ids, row_valid, codes, ids,
+                                 dists, valid, active, w);
+    else
+      pq_wide_launch<METRIC_L2>(x, n, ldx, M, ds, codebook, Kc, ivf_centroids, part_ids, row_valid, codes, ids,
+                                dists, valid, active, w);
+    return;
+  }
 #define LB2_SD(DSV)                                                                              \
   case DSV:                                                                                      \
     if (metric == METRIC_DOT)                                                                    \
@@ -584,9 +816,10 @@ void small_d_assign_f32(const float* x, uint64_t n, int ldx, int M, int ds, cons
                                      row_valid, codes, ids, dists, valid, active);               \
     break;
   switch (ds) {
-    LB2_SD(1) LB2_SD(2) LB2_SD(4) LB2_SD(8) LB2_SD(12)
+    LB2_SD(1) LB2_SD(2) LB2_SD(3) LB2_SD(4) LB2_SD(5) LB2_SD(6) LB2_SD(7) LB2_SD(8)
+    LB2_SD(9) LB2_SD(10) LB2_SD(11) LB2_SD(12) LB2_SD(13) LB2_SD(14) LB2_SD(15)
     default:
-      fail(LB2_UNSUPPORTED, "sub-vector width %d has no small-d kernel", ds);
+      fail(LB2_INVALID_ARG, "PQ sub-vector width %d", ds);
   }
 #undef LB2_SD
 }

@@ -32,8 +32,6 @@ void check_pq_shape(uint32_t d, uint32_t M, uint32_t nbits, PqUse use) {
     fail(LB2_INVALID_ARG, "PQ: num_bits must be 4 or 8, got %u", nbits);
   if (use == PqUse::TRAIN) return;
   LB2_REQUIRE(nbits == 8 || M % 2 == 0, "PQ: num_sub_vectors must be divisible by 2 for num_bits=4, but got %u", M);
-  if (use == PqUse::ENCODE && !small_d_supported((int)(d / M)))
-    fail(LB2_UNSUPPORTED, "PQ sub-vector width %d not supported yet", (int)(d / M));
 }
 
 // ProductQuantizer::transform_impl for either code width (pq.rs:116-191): 8-bit -> [n][M] through the
@@ -46,8 +44,8 @@ void pq_encode_any(const float* x, uint64_t n, int d, int M, int ds, const float
   }
   if (n == 0) return;
   DevBuf<uint8_t> wide((size_t)n * M);
-  small_d_assign_f32(x, n, d, M, ds, codebook, 16, metric, cent, part, row_valid, wide.p, nullptr, nullptr,
-                     nullptr, nullptr);
+  pq_assign_f32(x, n, d, M, ds, codebook, 16, metric, cent, part, row_valid, wide.p, nullptr, nullptr, nullptr,
+                nullptr);
   pack_nibbles(wide.p, n, M, codes);
   sync_stream();  // `wide` is freed on return
 }

@@ -9,9 +9,9 @@ __global__ void residual_kernel(const float* x, const float* __restrict__ cent, 
                                 uint64_t n, int d, float* out);
 
 // What a ProductQuantizer of M sub-vectors and num_bits codes needs: M divides d (pq/utils.rs:25) and num_bits is 4
-// or 8 (INDEX and ENCODE: M is even for 4-bit codes, pq.rs:132-140; ENCODE: the sub-vector width is one the encode
-// kernels implement -> LB2_UNSUPPORTED)
-enum class PqUse { TRAIN, INDEX, ENCODE };
+// or 8 (ENCODE, i.e. wherever codes exist: M is even for 4-bit codes, pq.rs:132-140).  Every sub-vector width has
+// an exact encode route (pq_assign_f32).
+enum class PqUse { TRAIN, ENCODE };
 void check_pq_shape(uint32_t d, uint32_t M, uint32_t nbits, PqUse use);
 void check_redos(uint32_t redos, float balance_factor);
 void pq_train_dev(const float* data, uint64_t n, int d, int metric, const lb2_pq_params* p, float* codebook,

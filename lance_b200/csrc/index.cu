@@ -659,7 +659,7 @@ lb2_status lb2_index_create(const void* centroids, uint32_t k, uint32_t d, lb2_d
                             uint32_t num_bits, lb2_index** out) {
   LB2_API_BEGIN
   LB2_REQUIRE(out && centroids && codebook, "null argument");
-  check_pq_shape(d, num_sub_vectors, num_bits, PqUse::INDEX);
+  check_pq_shape(d, num_sub_vectors, num_bits, PqUse::ENCODE);
   std::unique_ptr<lb2_index> ix = index_with_centroids(IndexKind::PQ, centroids, k, d, dtype, metric);
   ix->M = num_sub_vectors;
   ix->nbits = num_bits;

@@ -824,8 +824,6 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, c
   LB2_REQUIRE(n_global < 0xfffffffeull, "training sample too large");
   const size_t BK = (size_t)B * K;
   const bool small = B > 1;
-  if (small && !small_d_supported(ds))
-    fail(LB2_UNSUPPORTED, "PQ sub-vector width %d is not supported by the device trainer yet", ds);
 
   // ---- init (kmeans.rs:149-170; our rng): k distinct rows by a partial Fisher-Yates ------------
   std::vector<LloydState> h_states(B);
@@ -931,6 +929,7 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, c
   }
   TcWorkspace tcws;
   TcPqWorkspace pqws;
+  PqAssignWorkspace pqaws;  // the wide PQ routes' scratch, allocated by the eager first iteration
   DevBuf<float> rn2;
   const bool pq_tc = small && ldx == B * ds && tc_pq_supported(n, ldx, B, ds, K, p.metric, x);
   TcPqPrepArgs pq_prep;      // bm == nullptr unless the PQ tensor path is in use
@@ -953,8 +952,8 @@ void lloyd_train(const float* x, uint64_t n_in, int ldx, int B, int ds, int K, c
                    active_d.p, &pqws, /*prepared=*/pq_prepared);
       pq_prepared = true;
     } else {
-      small_d_assign_f32(x, n, ldx, B, ds, centroids, K, p.metric, nullptr, nullptr, nullptr, nullptr,
-                         ids.p, dists.p, valid.p, active_d.p);
+      pq_assign_f32(x, n, ldx, B, ds, centroids, K, p.metric, nullptr, nullptr, nullptr, nullptr, ids.p, dists.p,
+                    valid.p, active_d.p, &pqaws);
     }
     ms.run(ids.p, valid.p, n, K, B, active_d.p);
     // ds % 8 == 0 (and 16-byte aligned rows): warp-cooperative update, one warp per (b, cluster, 8 dims)

@@ -625,8 +625,8 @@ void pq_encode_dev(const float* x, uint64_t n, int d, int M, int ds, const float
   if (n == 0) return;
   // (the filter stores a row's four codes of a chunk as one word)
   if (!tc_pq_supported(n, d, M, ds, 256, metric, x) || (reinterpret_cast<uintptr_t>(codes) & 3) != 0) {
-    small_d_assign_f32(x, n, d, M, ds, codebook, 256, metric, cent, part, row_valid, codes, nullptr,
-                       nullptr, nullptr, nullptr);
+    pq_assign_f32(x, n, d, M, ds, codebook, 256, metric, cent, part, row_valid, codes, nullptr, nullptr, nullptr,
+                  nullptr);
     return;
   }
   TcPqWorkspace ws;

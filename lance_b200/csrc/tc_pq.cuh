@@ -47,7 +47,7 @@ bool tc_pq_supported(uint64_t n, int d, int M, int ds, int Kc, int metric, const
 void tc_pq_residual_norms(const float* x, const float* cent, const uint32_t* part, uint64_t n, int M,
                           float* r_out, float* rn2);
 // codes != NULL: u8 [n][M] (encode); else ids/dists/valid [M][n] (training). Bit-identical to
-// small_d_assign_f32 on the same inputs.
+// pq_assign_f32 on the same inputs.
 // prepared = the operands were already refreshed for this codebook (by the fused epilogue)
 void tc_pq_assign(const float* r, const float* rn2, uint64_t n, int d, int M, const float* codebook,
                   const uint8_t* row_valid, uint8_t* codes, uint32_t* ids, float* dists,
