@@ -356,13 +356,12 @@ lb2_status lb2_index_search_combined(lb2_index* index, const void* queries, uint
                                      const lb2_probe_params* pp /* nullable */, const lb2_unindexed_rows* u,
                                      uint64_t* row_ids_out, float* dists_out, uint32_t* counts_out,
                                      uint32_t* nprobes_out /* nullable; requires pp */);
-/* Incremental update: the device half of optimize_indices / split / join (SURVEY 8f-4).
+/* Incremental update of an IVF_PQ index (SURVEY 8f-4).
  * The reference expresses an optimize step as per-partition AssignOp::Add / AssignOp::Remove lists against a new
  * centroid set (rust/lance/src/index/vector/builder.rs:1219-1333 split_partition_impl, :1476-1530
- * join_partition_impl, :1534-1650 build_assign_batch) and merges them with the stored partitions.  The decisions
- * (should_split :1152, should_join :1343, assign_vectors :1690 -- built from lb2_kmeans_train(k = 2),
- * lb2_distance_batch and lb2_ivfpq_transform on the moved rows) stay with the host, which owns the dataset;
- * this call is the merge on the device and returns a NEW index:
+ * join_partition_impl, :1534-1650 build_assign_batch) and merges them with the stored partitions.  This call is that
+ * merge for lists the caller built (lb2_index_split / lb2_index_join below make the lists of a split or join
+ * themselves) and returns a NEW index:
  *   - new_centroids [new_k][d] in the model's element type (NULL = unchanged, then new_k must equal the old k);
  *   - part_map[old_k] (nullable = identity): new partition id of every old partition, UINT32_MAX = the partition's
  *     rows are dropped (split: the split partition's rows come back through the add list; join: ids after the
@@ -436,6 +435,82 @@ typedef struct {
   uint32_t insert_batch;         /* B of the graphs that are rebuilt (IVF_HNSW_SQ's rounds); 0: the old index's B */
 } lb2_optimize_params;
 lb2_status lb2_index_optimize(const lb2_index* old_index, const lb2_optimize_params* p, lb2_index** out);
+/* ---- partition split and join (optimize_indices / remap, rust/lance/src/index/vector/builder.rs:1152-1814) -------
+ * The host owns the dataset: it fetches a partition's raw rows by row id (load_partition_raw_vectors, :1118-1147);
+ * every other step is one of these calls.
+ * lb2_index_partition_to_split (should_split, :1152-1176): a partition's size is its stored rows plus the rows of
+ *   new_part_ids (the add list's partitions); the largest partition strictly above MAX_PARTITION_SIZE_FACTOR (4) x
+ *   target, the first of equal sizes.  lb2_index_partition_to_join (should_join, :1343-1394): a partition's size is
+ *   its rows the remap (strictly ascending old ids; UINT64_MAX = None) does not map to None; the smallest strictly
+ *   below MIN_PARTITION_SIZE_PERCENT (25) x target / 100, never with one partition.  target is
+ *   IndexType::target_partition_size (lance-index/src/lib.rs:284-295): 4096 for IVF_FLAT, 8192 for IVF_PQ, IVF_SQ and
+ *   IVF_RQ, 1 Mi for the graph kinds.  *part = UINT32_MAX when none qualifies.
+ * lb2_index_reassign_candidates (select_reassign_candidates_impl, :1788-1814): every centroid ranked by
+ *   lb2_distance_batch(c_part, centroids) under the index metric, the first min(65, K) by (distance, id), `part`
+ *   dropped, min(65, K) - 1 kept: ids[64], *count.  The host fetches these partitions' raw rows for a split.
+ * lb2_index_split (split_partition_impl, :1219-1333): returns a NEW index of K + 1 partitions.
+ *   - c1, c2: lb2_kmeans_train(k = 2) on the first 512 of the partition's raw rows (normalised under cosine, trained
+ *     with L2), max_iters 50, redos 1, tolerance 1e-4, no balance factor, seeded by opt.seed; c1 replaces centroid
+ *     `part`, c2 is centroid K.
+ *   - d0 / d1 / d2 = lb2_distance_batch(c, row) on the raw rows; candidate distances lb2_distance_batch(row, c) (the
+ *     orientation matters for cosine).  A row of the split partition (assign_vectors with deleted_original_partition,
+ *     :1690-1749) whose d0 <= d1 && d0 <= d2 goes to the first minimum over the candidates by total_cmp when that is
+ *     <= d1 and <= d2 (reassign_vectors, :1754-1785); every other row goes to c1 when d1 <= d2, else to c2.  A row of
+ *     a candidate partition stays when its d0 (to its own centroid) is <= d1 and <= d2, else it moves to c1 or c2 by
+ *     the same rule.  With K = 1 there are no candidates and such a row takes the c1 / c2 rule (the reference
+ *     unwraps an empty minimum there).
+ *   - the result is lb2_index_optimize of: the old rows without the split partition's and the moved rows; opt's add
+ *     list without its rows of `part` and the moved rows; then the moved rows in add-op order (the split rows in
+ *     ascending row id, then the candidate partitions in candidate order), with the payload of
+ *     lb2_index_transform under the new centroids -- IVF_PQ residuals to the decided partition, IVF_RQ codes and
+ *     factors from its nearest new centroid (ivf.rs:301-304) stored in the decided partition.
+ *   - one stated difference (DESIGN.md section 2): every row is placed once, at its decision; the reference's
+ *     build_partitions also keeps the split partition's old copies in partition `part`.
+ *   A split partition without raw rows changes nothing but opt (:1184-1189).  LB2_INVALID_ARG: a bad part, one raw
+ *   row, row ids not ascending within a group or candidate groups out of candidate order, a raw row that is not a row
+ *   (stored or in opt's add list) of the partition it is passed for, a raw row the transform would drop (a non-finite
+ *   element, a zero row under cosine; a moved row also when the new model's transform finds no finite distance to
+ *   any centroid, ivf.rs:166), an add list without its partition ids, payload or row ids, opt.new_centroids / part_map / remap set.  LB2_UNSUPPORTED: u8 columns (the reference's
+ *   arrow_batch_func cannot take u8 rows against its f32 centroids: l2.rs:205-266), more than one rank.
+ * lb2_index_join (join_partition_impl, :1476-1530): a NEW index of K - 1 partitions: centroid `part` deleted, every
+ *   raw row of `part` to the first minimum over its candidates (ids above `part` shift down by one), composed with the
+ *   removals and the remap as lb2_index_optimize applies them (to old and moved rows alike). */
+typedef struct {
+  uint32_t part;
+  const void* vectors;             /* [n][d] the partition's raw rows, the index's element type */
+  const uint64_t* row_ids;         /* [n] ascending */
+  uint64_t n;
+  const void* cand_vectors;        /* [n_cand][d] the candidate partitions' raw rows */
+  const uint64_t* cand_row_ids;    /* [n_cand] */
+  const uint32_t* cand_part_ids;   /* [n_cand] grouped in candidate order, ascending row ids within a group */
+  uint64_t n_cand;
+  lb2_optimize_params opt;         /* add list, removals, seed, insert_batch; new_centroids, part_map and the remap
+                                      NULL (the split's own), new_k ignored */
+  void* new_centroids_out;         /* nullable: [new k][d] in the model type */
+  uint32_t* dest_out;              /* nullable: [n + n_cand] new partition of each raw row, UINT32_MAX = stays */
+} lb2_split_params;
+typedef struct {
+  uint32_t part;
+  const void* vectors;             /* [n][d] the partition's raw rows */
+  const uint64_t* row_ids;         /* [n] ascending */
+  uint64_t n;
+  const uint64_t* remove_row_ids;  /* sorted ascending */
+  uint64_t n_remove;
+  const uint64_t* remap_old_ids;   /* strictly ascending */
+  const uint64_t* remap_new_ids;   /* UINT64_MAX = None */
+  uint64_t n_remap;
+  uint64_t seed;
+  uint32_t insert_batch;
+  uint32_t* dest_out;              /* nullable: [n] new partition of each raw row */
+} lb2_join_params;
+lb2_status lb2_index_partition_to_split(const lb2_index* index, const uint32_t* new_part_ids, uint64_t n_new,
+                                        uint32_t* part);
+lb2_status lb2_index_partition_to_join(const lb2_index* index, const uint64_t* remap_old_ids,
+                                       const uint64_t* remap_new_ids, uint64_t n_remap, uint32_t* part);
+lb2_status lb2_index_reassign_candidates(const lb2_index* index, uint32_t part, uint32_t* ids_out /*[64]*/,
+                                         uint32_t* count);
+lb2_status lb2_index_split(const lb2_index* old_index, const lb2_split_params* p, lb2_index** out);
+lb2_status lb2_index_join(const lb2_index* old_index, const lb2_join_params* p, lb2_index** out);
 /* Asynchronous search (SURVEY 8b "Threading": `_async` variants taking a stream/event).  Same
  * arguments and results as lb2_index_search_ex, but the call only ENQUEUES the work on `cuda_stream`
  * (cudaStream_t; NULL = the calling thread's current library stream) and returns: probe selection, LUT

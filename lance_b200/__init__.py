@@ -808,6 +808,34 @@ class IvfPqIndex:
 
     def _optimize(self, add_vectors, add_row_ids, add_part_ids, add_payload, add_factors, new_centroids, part_map,
                   remove_row_ids, remap, seed, insert_batch):
+        p, _keep = self._optimize_params(add_vectors, add_row_ids, add_part_ids, add_payload, add_factors,
+                                         new_centroids, part_map, remove_row_ids, remap, seed, insert_batch)
+        h = C.c_void_p()
+        check(lib().lb2_index_optimize(self._h, C.byref(p), C.byref(h)))
+        return self._like(h)
+
+    def _like(self, h):
+        """a new index of this class over handle h, with this index's element type"""
+        out = type(self)(h)
+        if hasattr(self, "_dt"):
+            out._dt = self._dt
+        return out
+
+    @staticmethod
+    def _remap_arrays(remap):
+        """{old id: new id or None} or (old ids, new ids) -> ascending (old ids, new ids), UINT64_MAX for None"""
+        if remap is None:
+            return None, None
+        if isinstance(remap, dict):
+            ro = np.fromiter(remap.keys(), np.uint64, len(remap))
+            rn = np.fromiter((0xFFFFFFFFFFFFFFFF if v is None else v for v in remap.values()), np.uint64, len(remap))
+            o = np.argsort(ro, kind="stable")
+            return ro[o], rn[o]
+        return tuple(np.ascontiguousarray(a, dtype=np.uint64) for a in remap)
+
+    def _optimize_params(self, add_vectors, add_row_ids, add_part_ids, add_payload, add_factors, new_centroids,
+                         part_map, remove_row_ids, remap, seed, insert_batch):
+        """lb2_optimize_params of optimize()'s arguments, and the arrays it points into (keep them alive)"""
         from ._lib import OptimizeParams
         if add_vectors is not None:
             if add_part_ids is not None or add_payload is not None or add_factors is not None:
@@ -831,15 +859,7 @@ class IvfPqIndex:
         if add_factors is not None:
             fa, fs = (np.ascontiguousarray(f, dtype=np.float32) for f in add_factors)
         rm = None if remove_row_ids is None else np.sort(np.ascontiguousarray(remove_row_ids, dtype=np.uint64))
-        ro = rn = None
-        if remap is not None:
-            if isinstance(remap, dict):
-                ro = np.fromiter(remap.keys(), np.uint64, len(remap))
-                rn = np.fromiter((0xFFFFFFFFFFFFFFFF if v is None else v for v in remap.values()), np.uint64, len(remap))
-                o = np.argsort(ro, kind="stable")
-                ro, rn = ro[o], rn[o]
-            else:
-                ro, rn = (np.ascontiguousarray(a, dtype=np.uint64) for a in remap)
+        ro, rn = self._remap_arrays(remap)
         keep = [cent, pm, ap, ac, fa, fs, ar, rm, ro, rn]
         ptr = [as_ptr(x)[0] if x is not None and x.size else None for x in keep]
         nz = lambda p: p.value if p is not None else None  # noqa: E731
@@ -847,12 +867,92 @@ class IvfPqIndex:
         p = OptimizeParams(nz(ptr[0]), new_k, nz(ptr[1]), nz(ptr[2]), nz(ptr[3]), nz(ptr[4]), nz(ptr[5]), nz(ptr[6]),
                            n_add, nz(ptr[7]), 0 if rm is None else rm.size, nz(ptr[8]), nz(ptr[9]),
                            0 if ro is None else ro.size, seed, insert_batch)
+        return p, keep
+
+    # ---- partition split and join (rust/lance/src/index/vector/builder.rs:1152-1814) ------------------------------
+    def partition_to_split(self, new_part_ids=None):
+        """lb2_index_partition_to_split (should_split): the partition to split, counting the add list's partition ids
+        new_part_ids with the stored rows, or None"""
+        a = None if new_part_ids is None else np.ascontiguousarray(new_part_ids, dtype=np.uint32)
+        part = C.c_uint32()
+        check(lib().lb2_index_partition_to_split(self._h, as_ptr(a)[0] if a is not None and a.size else None,
+                                                 C.c_uint64(0 if a is None else a.size), C.byref(part)))
+        return None if part.value == 0xFFFFFFFF else part.value
+
+    def partition_to_join(self, remap=None):
+        """lb2_index_partition_to_join (should_join): the partition to join, counting the rows the remap does not map
+        to None, or None"""
+        ro, rn = self._remap_arrays(remap)
+        n = 0 if ro is None else ro.size
+        part = C.c_uint32()
+        check(lib().lb2_index_partition_to_join(self._h, as_ptr(ro)[0] if n else None, as_ptr(rn)[0] if n else None,
+                                                C.c_uint64(n), C.byref(part)))
+        return None if part.value == 0xFFFFFFFF else part.value
+
+    def reassign_candidates(self, part):
+        """lb2_index_reassign_candidates (select_reassign_candidates): the partitions whose raw rows a split of `part`
+        reads, in candidate order"""
+        ids, cnt = np.empty(64, np.uint32), C.c_uint32()
+        check(lib().lb2_index_reassign_candidates(self._h, C.c_uint32(part), C.c_void_p(ids.ctypes.data), C.byref(cnt)))
+        return ids[:cnt.value].copy()
+
+    def _raw(self, vectors):
+        if isinstance(vectors, (DeviceArray, PinnedArray)):
+            return vectors
+        npdt = {F32: np.float32, F16: np.float16, U8: np.uint8, BF16: np.uint16}[getattr(self, "_dt", F32)]
+        d = self.info()["dimension"]
+        return np.ascontiguousarray(np.asarray(vectors).reshape(-1, d), dtype=npdt)
+
+    def split(self, part, vectors, row_ids, cand_vectors=None, cand_row_ids=None, cand_part_ids=None,
+              add_vectors=None, add_row_ids=None, add_part_ids=None, add_payload=None, add_factors=None,
+              remove_row_ids=None, seed=0):
+        """lb2_index_split: split partition `part` (vectors / row_ids: its raw rows, ascending ids) with the raw rows of
+        its reassign candidates (grouped in candidate order), composed with an optimize's add list and removals.
+        Returns (new index, dict(new_centroids, dest)): dest[i] the new partition of raw row i (the partition's rows,
+        then the candidates'), 0xFFFFFFFF for a candidate row that stays."""
+        return self._split(part, vectors, row_ids, cand_vectors, cand_row_ids, cand_part_ids, add_vectors, add_row_ids,
+                           add_part_ids, add_payload, add_factors, remove_row_ids, seed, 0)
+
+    def _split(self, part, vectors, row_ids, cand_vectors, cand_row_ids, cand_part_ids, add_vectors, add_row_ids,
+               add_part_ids, add_payload, add_factors, remove_row_ids, seed, insert_batch):
+        from ._lib import SplitParams
+        op, keep = self._optimize_params(add_vectors, add_row_ids, add_part_ids, add_payload, add_factors, None, None,
+                                         remove_row_ids, None, seed, insert_batch)
+        info = self.info()
+        d = info["dimension"]
+        v, r = self._raw(vectors), np.ascontiguousarray(row_ids, dtype=np.uint64)
+        if cand_vectors is None:
+            cv, cr, cp = self._raw(np.zeros((0, d))), np.zeros(0, np.uint64), np.zeros(0, np.uint32)
+        else:
+            cv, cr = self._raw(cand_vectors), np.ascontiguousarray(cand_row_ids, dtype=np.uint64)
+            cp = np.ascontiguousarray(cand_part_ids, dtype=np.uint32)
+        new_k = info["num_partitions"] + (1 if len(r) else 0)
+        cent = np.empty((new_k, d), _model_np(getattr(self, "_dt", F32)))
+        dest = np.empty(len(r) + len(cr), np.uint32)
+        pz = lambda a: as_ptr(a)[0] if a.shape[0] else None  # noqa: E731
+        sp = SplitParams(part, pz(v), pz(r), len(r), pz(cv), pz(cr), pz(cp), len(cr), op, pz(cent), pz(dest))
         h = C.c_void_p()
-        check(lib().lb2_index_optimize(self._h, C.byref(p), C.byref(h)))
-        out = type(self)(h)
-        if hasattr(self, "_dt"):
-            out._dt = self._dt
-        return out
+        check(lib().lb2_index_split(self._h, C.byref(sp), C.byref(h)))
+        del keep
+        return self._like(h), dict(new_centroids=cent, dest=dest)
+
+    def join(self, part, vectors, row_ids, remove_row_ids=None, remap=None, seed=0):
+        """lb2_index_join: delete partition `part` and send its raw rows (ascending ids) to their nearest reassign
+        candidate, composed with removals and a row-id remap.  Returns (new index, dest)."""
+        return self._join(part, vectors, row_ids, remove_row_ids, remap, seed, 0)
+
+    def _join(self, part, vectors, row_ids, remove_row_ids, remap, seed, insert_batch):
+        from ._lib import JoinParams
+        v, r = self._raw(vectors), np.ascontiguousarray(row_ids, dtype=np.uint64)
+        rm = None if remove_row_ids is None else np.sort(np.ascontiguousarray(remove_row_ids, dtype=np.uint64))
+        ro, rn = self._remap_arrays(remap)
+        dest = np.empty(len(r), np.uint32)
+        pz = lambda a: as_ptr(a)[0] if a is not None and a.shape[0] else None  # noqa: E731
+        jp = JoinParams(part, pz(v), pz(r), len(r), pz(rm), 0 if rm is None else rm.size, pz(ro), pz(rn),
+                        0 if ro is None else ro.size, seed, insert_batch, pz(dest))
+        h = C.c_void_p()
+        check(lib().lb2_index_join(self._h, C.byref(jp), C.byref(h)))
+        return self._like(h), dest
 
     def repartition(self):
         """lb2_index_repartition: row-sharded index -> the index of the partitions this rank owns (p % nranks == rank),
@@ -1129,6 +1229,19 @@ class _HnswGraphs:
         built with, 1 for a loaded graph).  Kept partitions keep their graphs verbatim."""
         return self._optimize(add_vectors, add_row_ids, add_part_ids, add_payload, add_factors, new_centroids, part_map,
                               remove_row_ids, remap, seed, 0 if insert_batch is None else int(insert_batch))
+
+    def split(self, part, vectors, row_ids, cand_vectors=None, cand_row_ids=None, cand_part_ids=None,
+              add_vectors=None, add_row_ids=None, add_part_ids=None, add_payload=None, add_factors=None,
+              remove_row_ids=None, seed=0, insert_batch=None):
+        """the parent kind's split; insert_batch as in optimize"""
+        return self._split(part, vectors, row_ids, cand_vectors, cand_row_ids, cand_part_ids, add_vectors, add_row_ids,
+                           add_part_ids, add_payload, add_factors, remove_row_ids, seed,
+                           0 if insert_batch is None else int(insert_batch))
+
+    def join(self, part, vectors, row_ids, remove_row_ids=None, remap=None, seed=0, insert_batch=None):
+        """the parent kind's join; insert_batch as in optimize"""
+        return self._join(part, vectors, row_ids, remove_row_ids, remap, seed,
+                          0 if insert_batch is None else int(insert_batch))
 
     def _search_hnsw(self, queries, k, nprobes, ef, probe=None, allow_bitmap=None, refine_factor=0, vectors=None,
                      lower_bound=None, upper_bound=None):

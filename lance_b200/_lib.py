@@ -87,6 +87,22 @@ class OptimizeParams(C.Structure):
                 ("insert_batch", C.c_uint32)]
 
 
+class SplitParams(C.Structure):
+    """lb2_split_params (include/lance_b200.h)."""
+    _fields_ = [("part", C.c_uint32), ("vectors", C.c_void_p), ("row_ids", C.c_void_p), ("n", C.c_uint64),
+                ("cand_vectors", C.c_void_p), ("cand_row_ids", C.c_void_p), ("cand_part_ids", C.c_void_p),
+                ("n_cand", C.c_uint64), ("opt", OptimizeParams), ("new_centroids_out", C.c_void_p),
+                ("dest_out", C.c_void_p)]
+
+
+class JoinParams(C.Structure):
+    """lb2_join_params (include/lance_b200.h)."""
+    _fields_ = [("part", C.c_uint32), ("vectors", C.c_void_p), ("row_ids", C.c_void_p), ("n", C.c_uint64),
+                ("remove_row_ids", C.c_void_p), ("n_remove", C.c_uint64), ("remap_old_ids", C.c_void_p),
+                ("remap_new_ids", C.c_void_p), ("n_remap", C.c_uint64), ("seed", C.c_uint64),
+                ("insert_batch", C.c_uint32), ("dest_out", C.c_void_p)]
+
+
 class BuildStats(C.Structure):
     _fields_ = [("ms_ivf_train", C.c_float), ("ms_pq_train", C.c_float), ("ms_transform", C.c_float),
                 ("ms_group", C.c_float), ("ms_total", C.c_float), ("ivf_iters", C.c_uint32),
@@ -108,6 +124,8 @@ EXPORTS = [
     "lb2_index_load_flat", "lb2_index_export_flat", "lb2_comm_unique_id", "lb2_comm_init", "lb2_comm_destroy",
     "lb2_comm_info", "lb2_index_search_sharded", "lb2_set_stream", "lb2_trim_memory", "lb2_index_search_async", "lb2_index_repartition", "lb2_index_update",
     "lb2_index_transform", "lb2_index_optimize",
+    "lb2_index_partition_to_split", "lb2_index_partition_to_join", "lb2_index_reassign_candidates", "lb2_index_split",
+    "lb2_index_join",
     "lb2_sq_train", "lb2_sq_encode", "lb2_ivfsq_build_params_default", "lb2_ivfsq_build", "lb2_index_create_sq",
     "lb2_index_load_sq", "lb2_index_export_sq", "lb2_ivfhnswsq_build_params_default", "lb2_ivfhnswsq_build",
     "lb2_index_load_hnsw_sq", "lb2_index_hnsw_sq_info", "lb2_index_export_hnsw_sq", "lb2_index_search_hnsw", "lb2_rq_rotation", "lb2_ivfrq_transform",

@@ -13,6 +13,7 @@
 #include "index.cuh"
 #include "ivf_search.cuh"
 #include "kmeans.cuh"
+#include "row_distance.cuh"
 #include "rq.cuh"
 #include "scan.cuh"
 #include "sq.cuh"
@@ -99,20 +100,9 @@ __global__ void cosine_f32_kernel(const float* __restrict__ from, const float* _
   const uint64_t w = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (w >= n) return;
-  float xx = 0.0f, xy = 0.0f, yy = 0.0f;
-  for (int e = lane; e < d; e += 32) {
-    const float x = from[e], y = to[w * d + e];
-    xx = fmaf(x, x, xx);
-    xy = fmaf(x, y, xy);
-    yy = fmaf(y, y, yy);
-  }
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) {
-    xx += __shfl_xor_sync(0xffffffffu, xx, o);
-    xy += __shfl_xor_sync(0xffffffffu, xy, o);
-    yy += __shfl_xor_sync(0xffffffffu, yy, o);
-  }
-  if (lane == 0) out[w] = 1.0f - xy / sqrtf(xx) / sqrtf(yy);
+  float xx, xy, yy;
+  cos32_sums(from, to + w * d, d, lane, xx, xy, yy);
+  if (lane == 0) out[w] = cos32_finish(xy, xx, yy);
 }
 
 }  // namespace lb2

@@ -297,6 +297,74 @@ static void rq_centroid_norms(int metric, const float* cent, int K, int d, DevBu
   rq_norm_sq_f32(cent, K, d, out.p);
 }
 
+// lb2_index_transform's rows (every output nullable).  given_part (nullable, device): the partition of every row is
+// given (a split's decisions, build_assign_batch's PART_ID column, builder.rs:1534-1650): IVF_PQ takes its residuals
+// to it; the other kinds store the same payload whatever the partition, and part_out still gets the nearest centroid.
+void index_transform_rows(const lb2_index* index, Source& src, const uint32_t* given_part, uint32_t* part_out,
+                          uint8_t* payload_out, float* add_out, float* scale_out, uint8_t* valid_out) {
+  const uint64_t n = src.n();
+  const bool rq = index->kind == IndexKind::RQ;
+  const int d = index->d, m = index->metric, K = index->K;
+  const size_t rb = index->row_bytes();
+  const float* cent = index->centroids.p;
+  // every output the chunk functions write is needed: the caller's NULLs get scratch
+  DevBuf<uint32_t> ptmp;
+  DevBuf<uint8_t> vtmp, ltmp;
+  DevBuf<float> atmp, stmp;
+  uint32_t* pp = part_out;
+  uint8_t *vp = valid_out, *lp = payload_out;
+  float *ap = add_out, *sp = scale_out;
+  if (!pp) { ptmp.alloc(std::max<uint64_t>(n, 1)); pp = ptmp.p; }
+  if (!vp) { vtmp.alloc(std::max<uint64_t>(n, 1)); vp = vtmp.p; }
+  if (!lp) { ltmp.alloc(std::max<uint64_t>(n * rb, 1)); lp = ltmp.p; }
+  if (rq && !ap) { atmp.alloc(std::max<uint64_t>(n, 1)); ap = atmp.p; }
+  if (rq && !sp) { stmp.alloc(std::max<uint64_t>(n, 1)); sp = stmp.p; }
+  if (n) {
+    src.start_resident_copy();
+    const int sdt = (int)src.dtype();
+    DevBuf<float> normbuf, cnorm;
+    RqWork w;
+    if (rq) rq_centroid_norms(m, cent, K, d, cnorm);
+    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
+      uint8_t* out = lp + r0 * rb;
+      switch (index->kind) {
+        case IndexKind::PQ:  // lb2_ivfpq_transform's rows
+          if (given_part) {
+            const float* xp = normalize_assign(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0, nullptr);
+            const bool dot = m == METRIC_DOT;
+            pq_encode_any(xp, rows, d, index->M, d / index->M, index->codebook.p, METRIC_L2, dot ? nullptr : cent,
+                          dot ? nullptr : given_part + r0, vp + r0, index->nbits, out);
+          } else {
+            transform_chunk(xf, xnat, sdt, rows, d, m, cent, K, index->codebook.p, index->M, index->nbits, normbuf,
+                            pp + r0, out, vp + r0);
+          }
+          break;
+        case IndexKind::RQ:  // lb2_ivfrq_transform's rows
+          rq_transform_chunk(xf, xnat, sdt, rows, d, m, cent, K, index->rq_rot.p, index->nbits, cnorm.p, w, pp + r0,
+                             vp + r0, out, ap + r0, sp + r0);
+          break;
+        case IndexKind::SQ: {  // lb2_ivfsq_build's codes
+          const float* xs = assign_flat_chunk(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0);
+          if (m == METRIC_COSINE) round_model(normbuf.p, (size_t)rows * d, index->dtype);
+          sq_encode_f32(xs, (uint64_t)rows * d, index->sq_lower, index->sq_upper, out);
+          break;
+        }
+        case IndexKind::FLAT: {  // index_load_flat_src's stored rows: (normalised) f32 in the stored element type
+          const float* xs = assign_flat_chunk(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0);
+          const lb2_dtype vdt = index->vdtype();
+          if (vdt == LB2_F32)
+            d2d(reinterpret_cast<float*>(out), xs, (size_t)rows * d);
+          else
+            LB2_LAUNCH("convert_from_f32", from_f32_kernel, cdiv(rows * d, 256), 256, 0, xs, (int)vdt, (size_t)rows * d,
+                       (void*)out);
+          break;
+        }
+      }
+    });
+  }
+  sync_stream();  // the scratch outputs are freed on return
+}
+
 }  // namespace lb2
 
 using namespace lb2;
@@ -433,60 +501,13 @@ lb2_status lb2_index_transform(const lb2_index* index, const void* vectors, uint
   LB2_REQUIRE(index && (vectors || n == 0), "null argument");
   const bool rq = index->kind == IndexKind::RQ;
   LB2_REQUIRE(rq || (!add_out && !scale_out), "lb2_index_transform: add and scale factors are for IVF_RQ indexes only");
-  const int d = index->d, m = index->metric, K = index->K;
   const size_t rb = index->row_bytes();
-  const float* cent = index->centroids.p;
   OutArg<uint32_t> po(part_out, n);
   OutArg<uint8_t> pl(payload_out, (size_t)n * rb), vo(valid_out, n);
   OutArg<float> ao(add_out, n), so(scale_out, n);
-  // every output the chunk functions write is needed: the caller's NULLs get scratch
-  DevBuf<uint32_t> ptmp;
-  DevBuf<uint8_t> vtmp, ltmp;
-  DevBuf<float> atmp, stmp;
-  uint32_t* pp = po.get();
-  uint8_t *vp = vo.get(), *lp = pl.get();
-  float *ap = ao.get(), *sp = so.get();
-  if (!pp) { ptmp.alloc(std::max<uint64_t>(n, 1)); pp = ptmp.p; }
-  if (!vp) { vtmp.alloc(std::max<uint64_t>(n, 1)); vp = vtmp.p; }
-  if (!lp) { ltmp.alloc(std::max<uint64_t>(n * rb, 1)); lp = ltmp.p; }
-  if (rq && !ap) { atmp.alloc(std::max<uint64_t>(n, 1)); ap = atmp.p; }
-  if (rq && !sp) { stmp.alloc(std::max<uint64_t>(n, 1)); sp = stmp.p; }
   if (n) {
-    Source src(vectors, n, d, index->dtype);
-    src.start_resident_copy();
-    const int sdt = (int)src.dtype();
-    DevBuf<float> normbuf, cnorm;
-    RqWork w;
-    if (rq) rq_centroid_norms(m, cent, K, d, cnorm);
-    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
-      uint8_t* out = lp + r0 * rb;
-      switch (index->kind) {
-        case IndexKind::PQ:  // lb2_ivfpq_transform's rows
-          transform_chunk(xf, xnat, sdt, rows, d, m, cent, K, index->codebook.p, index->M, index->nbits, normbuf,
-                          pp + r0, out, vp + r0);
-          break;
-        case IndexKind::RQ:  // lb2_ivfrq_transform's rows
-          rq_transform_chunk(xf, xnat, sdt, rows, d, m, cent, K, index->rq_rot.p, index->nbits, cnorm.p, w, pp + r0,
-                             vp + r0, out, ap + r0, sp + r0);
-          break;
-        case IndexKind::SQ: {  // lb2_ivfsq_build's codes
-          const float* xs = assign_flat_chunk(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0);
-          if (m == METRIC_COSINE) round_model(normbuf.p, (size_t)rows * d, index->dtype);
-          sq_encode_f32(xs, (uint64_t)rows * d, index->sq_lower, index->sq_upper, out);
-          break;
-        }
-        case IndexKind::FLAT: {  // index_load_flat_src's stored rows: (normalised) f32 in the stored element type
-          const float* xs = assign_flat_chunk(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0);
-          const lb2_dtype vdt = index->vdtype();
-          if (vdt == LB2_F32)
-            d2d(reinterpret_cast<float*>(out), xs, (size_t)rows * d);
-          else
-            LB2_LAUNCH("convert_from_f32", from_f32_kernel, cdiv(rows * d, 256), 256, 0, xs, (int)vdt, (size_t)rows * d,
-                       (void*)out);
-          break;
-        }
-      }
-    });
+    Source src(vectors, n, index->d, index->dtype);
+    index_transform_rows(index, src, nullptr, po.get(), pl.get(), ao.get(), so.get(), vo.get());
   }
   po.commit(); pl.commit(); vo.commit(); ao.commit(); so.commit();
   sync_stream();

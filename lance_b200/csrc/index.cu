@@ -40,7 +40,7 @@ static std::unique_ptr<lb2_index> index_with_centroids(IndexKind kind, const voi
 
 // the model of `from` in `to`, an index of the same kind from make_index: the centroids (or `new_centroids`, in the
 // model type of the index, when given), M, nbits, and the codebook, SQ bounds or RQ rotation as the kind has them
-static void copy_model(const lb2_index* from, lb2_index* to, const void* new_centroids = nullptr) {
+void copy_model(const lb2_index* from, lb2_index* to, const void* new_centroids) {
   const size_t kd = (size_t)to->K * to->d;
   if (new_centroids) {
     VecIn c(new_centroids, kd, model_dtype(to->dtype));
@@ -413,10 +413,9 @@ __global__ void repart_unpack_kernel(const uint64_t* __restrict__ seg_prefix /*[
 // ---- the merge of optimize / split / join / remap, for every kind (SURVEY 8f-4) ------------------------------------
 // The reference turns an optimize step into per-partition AssignOp::Add / AssignOp::Remove lists against a new
 // centroid set (rust/lance/src/index/vector/builder.rs:1219-1333 split, :1476-1530 join, :1534-1650
-// build_assign_batch) and merges them with the existing partitions when it writes the index.  The decisions --
-// which partition to split or join, which rows to move -- stay on the host (they need the dataset); index_merge is
-// the merge: old rows keep their payload, follow `part_map`, removed row ids are dropped, added rows join the end of
-// their partitions, and a compaction's row-id mapping is applied last.
+// build_assign_batch) and merges them with the existing partitions when it writes the index.  The decisions of a
+// split or join are split.cu's; index_merge is the merge: old rows keep their payload, follow `part_map`, removed row
+// ids are dropped, added rows join the end of their partitions, and a compaction's row-id mapping is applied last.
 // One pass over the old rows (storage order): the new partition and keep flag of each, and the rows each old
 // partition loses (dropped[p], nullable: the graph kinds' change detection)
 __global__ void update_old_rows_kernel(const uint64_t* __restrict__ part_offsets, int K, uint64_t n,
@@ -535,8 +534,17 @@ static HnswKeep kept_partitions(const lb2_index* old, const lb2_index* ix, const
   return keep;
 }
 
-// lb2_index_optimize's merge (and lb2_index_update's); `what` names the entry point in messages
-static std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_optimize_params& p, const char* what) {
+// rows per partition id among the rows with valid[i] != 0
+__global__ void count_valid_parts_kernel(const uint32_t* __restrict__ part, const uint8_t* __restrict__ valid,
+                                         uint64_t n, uint32_t* __restrict__ counts) {
+  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && valid[i]) atomicAdd(&counts[part[i]], 1u);
+}
+
+// lb2_index_optimize's merge (and lb2_index_update's, lb2_index_split's and lb2_index_join's); `what` names the entry
+// point in messages.  add_valid (nullable, device [n_add]): added rows with 0 are left out.
+std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_optimize_params& p, const char* what,
+                                       const uint8_t* add_valid) {
   const bool rq = old->kind == IndexKind::RQ;
   const uint32_t new_k = p.new_k;
   LB2_REQUIRE(new_k > 0 && (p.new_centroids || new_k == (uint32_t)old->K), "a changed partition count needs new centroids");
@@ -575,7 +583,10 @@ static std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_op
     dropped.zero();
     added.alloc(new_k);
     added.zero();
-    if (n_add) LB2_LAUNCH("count_added", count_parts_kernel, cdiv(n_add, 256), 256, 0, ap.get(), n_add, added.p);
+    if (n_add && add_valid)
+      LB2_LAUNCH("count_added", count_valid_parts_kernel, cdiv(n_add, 256), 256, 0, ap.get(), add_valid, n_add, added.p);
+    else if (n_add)
+      LB2_LAUNCH("count_added", count_parts_kernel, cdiv(n_add, 256), 256, 0, ap.get(), n_add, added.p);
   }
   if (rq) {
     fa.alloc(std::max<uint64_t>(1, n_all));
@@ -602,7 +613,10 @@ static std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_op
       d2d(fa.p + n_old, aa.get(), (size_t)n_add);
       d2d(fs.p + n_old, as.get(), (size_t)n_add);
     }
-    LB2_LAUNCH("fill_valid", fill_u8_kernel, cdiv(n_add, 256), 256, 0, valid.p + n_old, n_add, (uint8_t)1);
+    if (add_valid)
+      d2d(valid.p + n_old, add_valid, (size_t)n_add);
+    else
+      LB2_LAUNCH("fill_valid", fill_u8_kernel, cdiv(n_add, 256), 256, 0, valid.p + n_old, n_add, (uint8_t)1);
   }
   uint32_t hbad[2] = {0, 0};
   d2h(hbad, bad.p, 2);

@@ -67,4 +67,11 @@ void index_load_dev(lb2_index* ix, const uint32_t* part_ids, const uint8_t* code
 void index_load_flat_src(lb2_index* ix, const uint32_t* part_ids, Source& src, const uint64_t* row_ids,
                          const uint8_t* valid, bool normalize);
 
+// the model of `from` in `to`, an index of the same kind from make_index: the centroids (or new_centroids, in the
+// model type of the index), M, nbits, and the codebook, SQ bounds or RQ rotation
+void copy_model(const lb2_index* from, lb2_index* to, const void* new_centroids = nullptr);
+// lb2_index_optimize's merge into a new index; add_valid (nullable, device [n_add]): added rows with 0 are left out
+std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_optimize_params& p, const char* what,
+                                       const uint8_t* add_valid = nullptr);
+
 }  // namespace lb2

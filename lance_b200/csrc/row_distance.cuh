@@ -170,6 +170,70 @@ __device__ __forceinline__ float row_distance(const float* __restrict__ q, const
   }
 }
 
+// lb2_distance_batch's cosine (cosine_distance_batch, cosine.rs:143-174,266-290) over one warp: lane l owns elements
+// l, l + 32, .. and accumulates <x, y> with FMA; the 32 partials are folded with the xor tree (offsets 16 .. 1).
+// <x, x> is cos32_sum(x, x).  The distance of `from` to `to` is cos32_finish(<from, to>, <from, from>, <to, to>).
+template <class T, class U>
+__device__ __forceinline__ float cos32_sum(const T* __restrict__ x, const U* __restrict__ y, int d, int lane) {
+  float s = 0.0f;
+  for (int e = lane; e < d; e += 32) s = fmaf(ldf<T>(x, e), ldf<U>(y, e), s);
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  return s;
+}
+// <x, x>, <x, y> and <y, y> as three cos32_sum would give them, in one pass over x and y
+template <class T, class U>
+__device__ __forceinline__ void cos32_sums(const T* __restrict__ x, const U* __restrict__ y, int d, int lane,
+                                           float& xx, float& xy, float& yy) {
+  xx = 0.0f, xy = 0.0f, yy = 0.0f;
+  for (int e = lane; e < d; e += 32) {
+    const float a = ldf<T>(x, e), b = ldf<U>(y, e);
+    xx = fmaf(a, a, xx);
+    xy = fmaf(a, b, xy);
+    yy = fmaf(b, b, yy);
+  }
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) {
+    xx += __shfl_xor_sync(0xffffffffu, xx, o);
+    xy += __shfl_xor_sync(0xffffffffu, xy, o);
+    yy += __shfl_xor_sync(0xffffffffu, yy, o);
+  }
+}
+// cos32_sum's value computed by one thread: the 32 lane partials in registers, folded as the xor tree folds them onto
+// lane 0 (at offset o, partial i < o takes partial i + o; f32 addition is commutative)
+__device__ __forceinline__ float cos32_sum_thread(const float* __restrict__ x, const float* __restrict__ y, int d) {
+  float v[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) v[i] = 0.0f;
+  for (int c = 0; c < d; c += 32) {
+#pragma unroll
+    for (int i = 0; i < 32; ++i)
+      if (c + i < d) v[i] = fmaf(x[c + i], y[c + i], v[i]);
+  }
+#pragma unroll
+  for (int o = 16; o >= 1; o >>= 1) {
+#pragma unroll
+    for (int i = 0; i < o; ++i) v[i] = v[i] + v[i + o];
+  }
+  return v[0];
+}
+__device__ __forceinline__ float cos32_finish(float xy, float from_sq, float to_sq) {
+  return 1.0f - xy / sqrtf(from_sq) / sqrtf(to_sq);
+}
+
+// One pair by one thread: the 16 lanes of the rule as 16 LaneAcc in registers, folded as fold_partials folds them (the
+// value row_distance leaves on its lanes).  Not for cosine, whose per-row form is the xor tree of row_distance.
+template <int RULE, int METRIC, class T>
+__device__ __forceinline__ float thread_distance(const float* __restrict__ q, const T* __restrict__ v, int d) {
+  static_assert(RULE != RULE_COSINE, "thread_distance: cosine folds with the xor tree");
+  LaneAcc<RULE, METRIC> acc[16];
+#pragma unroll
+  for (int l = 0; l < 16; ++l)
+    rule_walk<RULE>(d, l, [&](int e, auto part) { acc[l].template step<decltype(part)::value>(q[e], ldf<T>(v, e)); });
+  return fold_partials<RULE, METRIC>([&](int i) { return acc[i].a; }, [&](int i) { return acc[i].b; },
+                                     [&](int i) { return acc[i].u; }, acc[0].s, 0.0f);
+}
+
 // the IVF_FLAT scan: FlatDistanceCal::distance_all (flat/storage.rs:397-403)
 template <int METRIC, class T = float>
 __device__ __forceinline__ float flat_row_distance(const float* __restrict__ q, const T* __restrict__ v, int d, int l,
