@@ -115,3 +115,103 @@ def join_decisions(dist, centroids, part, rows):
     cands = select_reassign_candidates([dist(centroids[part], c) for c in centroids], part)
     return np.array(cands, np.uint32), join_destinations([[dist(r, centroids[c]) for c in cands] for r in rows], cands,
                                                          part)
+
+
+# ---- the per-pair distance rules in numpy f32, to show that a case tells rules apart ---------------------------------
+# Every operation rounds to f32 (numpy float32 arithmetic, no FMA).  x, y: f32 arrays [..., d] holding the elements'
+# exact f32 values; the result is dist(x, y) per leading index.
+def _terms(x, y, metric):
+    x, y = np.asarray(x, np.float32), np.asarray(y, np.float32)
+    if metric == "dot":
+        return x * y
+    t = x - y
+    return t * t
+
+
+def rule_sum(x, y, metric, lanes=16, tail="first", fold=None):
+    """lanes f32 accumulators, lane l owning elements l, l + lanes, ...; tail="first": the d % lanes tail summed
+    sequentially first and added last (the reference's dot_scalar / l2 shape), tail="lanes": the tail walked into the
+    lanes like any other element; fold: the order the lanes are folded in (default 0 .. lanes - 1).  dot: 1 - sum."""
+    t = _terms(x, y, metric)
+    d = t.shape[-1]
+    n = d // lanes * lanes
+    s = np.zeros(t.shape[:-1], np.float32)
+    acc = np.zeros(t.shape[:-1] + (lanes,), np.float32)
+    for c in range(0, n, lanes):
+        acc += t[..., c:c + lanes]
+    if tail == "first":
+        for e in range(n, d):
+            s += t[..., e]
+    else:
+        for e in range(n, d):
+            acc[..., e - n] += t[..., e]
+    tot = np.zeros(t.shape[:-1], np.float32)
+    for lane in (range(lanes) if fold is None else fold):
+        tot += acc[..., lane]
+    out = s + tot
+    return np.float32(1) - out if metric == "dot" else out
+
+
+def lanes16(x, y, metric):
+    """LANES16: l2 / dot of f32 rows and 16-bit l2 (l2.rs:57-91, dot.rs:30-58 with 16 lanes)"""
+    return rule_sum(x, y, metric, 16)
+
+
+def dot32(x, y, metric="dot"):
+    """DOT32: 16-bit dot, dot_scalar::<T, f32, 32> (dot.rs:30-58)"""
+    return rule_sum(x, y, metric, 32)
+
+
+def tail_in_lanes(x, y, metric):
+    """wrong: 16 lanes with the tail walked into the lanes"""
+    return rule_sum(x, y, metric, 16, tail="lanes")
+
+
+def dot32_b_first(x, y, metric="dot"):
+    """wrong: DOT32 with accumulators 16..31 folded before 0..15"""
+    return rule_sum(x, y, metric, 32, fold=list(range(16, 32)) + list(range(16)))
+
+
+def batch_rule(metric, dt):
+    """lb2_distance_batch's rule for l2 / dot: DOT32 for 16-bit dot, LANES16 otherwise"""
+    return dot32 if metric == "dot" and dt != "f32" else lanes16
+
+
+def matrix(rule, metric):
+    """D(A, B)[i, j] = rule(A[i], B[j]) (A in the `from` role)"""
+    return lambda A, B: rule(np.asarray(A, np.float32)[:, None, :], np.asarray(B, np.float32)[None, :, :], metric)
+
+
+def decisions(D, centroids, part, rows, c12=None, cand_rows=None, cand_parts=None, Dc=None):
+    """split_decisions (c12 = (c1, c2)) or join_decisions over matrix distances D(from_rows, to_rows) -> (candidates,
+    destinations); Dc: the distances of the candidate scan, dist(row, candidate centroid) (default D)"""
+    Dc = Dc or D
+    centroids = np.asarray(centroids, np.float32)
+    rows = np.asarray(rows, np.float32)
+    k = len(centroids)
+    cands = select_reassign_candidates(D(centroids[part:part + 1], centroids)[0], part)
+    cid = np.asarray(cands, np.int64)
+
+    def first_min(rs):
+        dc = Dc(rs, centroids[cid])
+        j = np.argmin(_total_key(dc), axis=1)
+        return cid[j], dc[np.arange(len(rs)), j]
+    if c12 is None:
+        ids, _ = first_min(rows)
+        return cands, np.where(ids < part, ids, ids - 1).astype(np.uint32)
+    c1, c2 = (np.asarray(c, np.float32) for c in c12)
+    d0, d1, d2 = D(np.stack([centroids[part], c1, c2]), rows)
+    out = np.where(d1 <= d2, part, k).astype(np.int64)
+    want = (d0 <= d1) & (d0 <= d2)
+    if len(cands) and want.any():
+        ids, best = first_min(rows[want])
+        take = (best <= d1[want]) & (best <= d2[want])
+        out[want] = np.where(take, ids, out[want])
+    dest = [out]
+    cand_rows = np.asarray(cand_rows, np.float32).reshape(-1, centroids.shape[1])
+    for q in cands:
+        rq = cand_rows[np.asarray(cand_parts) == q]
+        e0 = D(centroids[q:q + 1], rq)[0]
+        e1, e2 = D(np.stack([c1, c2]), rq)
+        dest.append(np.where((e0 <= e1) & (e0 <= e2), STAYS, np.where(e1 <= e2, part, k)))
+    return cands, np.concatenate(dest).astype(np.uint32)

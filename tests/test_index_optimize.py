@@ -170,14 +170,14 @@ def _t_rows(kind, t, row_ids):
     return r, t["part_ids"][ok]
 
 
-def _graph_of(kind, e, metric, seed):
-    """the restatement's graph over an export's storage"""
+def _graph_of(kind, e, metric, seed, dt="f32"):
+    """the restatement's graph over an export's storage (dt: the column's element type)"""
     kw = dict(m=HNSW["m"], max_level=HNSW["max_level"], efc=HNSW["ef_construction"], seed=seed)
     if kind == "hnsw_sq":
         return hr.build(e["codes"], e["part_offsets"], e["bounds"], "dot" if metric == "dot" else "l2", **kw)
     if kind == "hnsw_pq":
-        return pr.build(e["codes"], e["part_offsets"], e["codebook"], 8, metric, "f32", **kw)
-    return hf.build(e["vectors"], e["part_offsets"], metric, "f32", **kw)
+        return pr.build(e["codes"], e["part_offsets"], e["codebook"], 8, metric, dt, **kw)
+    return hf.build(e["vectors"], e["part_offsets"], metric, dt, **kw)
 
 
 def _assert_graph_equal(a, b):
@@ -187,7 +187,7 @@ def _assert_graph_equal(a, b):
         assert np.array_equal(np.asarray(a[k]).view(np.uint8), np.asarray(b[k]).view(np.uint8)), k
 
 
-def _check_merge(kind, old, new, old_e, offs, rows, src, metric, seed):
+def _check_merge(kind, old, new, old_e, offs, rows, src, metric, seed, dt="f32"):
     """new's export against the restated storage (and graphs)"""
     e = new.export()
     assert np.array_equal(e["part_offsets"], offs)
@@ -197,7 +197,7 @@ def _check_merge(kind, old, new, old_e, offs, rows, src, metric, seed):
         assert np.array_equal(e["add_factors"].view(np.uint32), rows["add"].view(np.uint32))
         assert np.array_equal(e["scale_factors"].view(np.uint32), rows["scale"].view(np.uint32))
     if kind in GRAPH:
-        want = assemble(offs, src, _graph_of(kind, e, metric, seed), old_e["graph"], old_e["part_offsets"])
+        want = assemble(offs, src, _graph_of(kind, e, metric, seed, dt), old_e["graph"], old_e["part_offsets"])
         _assert_graph_equal(e["graph"], want)
     return e
 
