@@ -539,6 +539,80 @@ lb2_status lb2_index_export(const lb2_index* index, void* centroids_out, void* c
  * *num_rows_out.  tests/: the bytes equal the reference's own fixture test_data/v0.27.1/pq_in_schema. */
 lb2_status lb2_index_export_partition(const lb2_index* index, uint32_t partition, uint8_t* codes_transposed_out,
                                       uint64_t* row_ids_out, uint64_t* num_rows_out);
+/* ---- a whole index in the reference's storage layout (every kind) ----------------------------------------------
+ * The columns merge_partitions writes (rust/lance/src/index/vector/builder.rs:938-1079): each partition's storage
+ * batch is written on its own, so `auxiliary.idx` (and for the graph kinds `index.idx`) holds the partitions back to
+ * back, partition 0 first, with part_lengths[p] rows (an empty partition adds none).  Here every column is that
+ * concatenation.  Row-wise columns, per partition in storage order:
+ *   _rowid            u64 [num_rows] (ROW_ID_FIELD).
+ *   payload [num_bytes], num_bytes = num_rows x the kind's bytes per row:
+ *     IVF_PQ, IVF_HNSW_PQ     `__pq_code` with "transposed": true (pq/storage.rs:52-67,430-450): each partition's
+ *                             codes column-major [code bytes per row][n_p], the bytes lb2_index_export_partition gives.
+ *     IVF_SQ, IVF_HNSW_SQ     `__sq_code` [n_p][d] (sq/storage.rs:38-45,280-300).
+ *     IVF_FLAT, IVF_HNSW_FLAT `flat` rows [n_p][d] in the stored element type, f32 / f16 / bf16 (flat/storage.rs:27,
+ *                             109-120).  u8 columns: LB2_INVALID_ARG both ways.  The reference's u8 flat storage is
+ *                             its binary Hamming storage (FlatBinStorage, flat/storage.rs:190-300), while this library
+ *                             holds u8 rows as f32 under L2 / cosine / dot, so no stored column matches them.
+ *     IVF_RQ                  `__rabit_code` packed (RabitQuantizationMetadata::packed, bq/storage.rs:48-55): the
+ *                             packing restarts at every partition, because try_from_batch packs each partition's
+ *                             batch on its own (bq/storage.rs:607-640) and merge_partitions writes each partition's
+ *                             storage separately.  In a partition of n_p rows of cl = code_dim / 8 bytes, with
+ *                             nb = n_p / 32 full blocks (pack_codes, bq/storage.rs:477-543): byte b*32*cl + i*32 + j,
+ *                             j < 16, is (c[32b + PERM0[j]][i] & 15) | (c[32b + PERM0[j] + 16][i] & 15) << 4, and
+ *                             byte b*32*cl + i*32 + 16 + j the same of the high nibbles (>> 4); PERM0 = 0, 8, 1, 9,
+ *                             .. 7, 15 (lance-linalg/src/simd/dist_table.rs:10).  The last n_p % 32 rows follow
+ *                             transposed, [cl][n_p % 32].  unpack_codes (:546-600) is the inverse.
+ *   add_factors, scale_factors  f32 [num_rows]: IVF_RQ's `__add_factors` / `__scale_factors`; NULL for other kinds.
+ * Graph kinds, also (HNSW::to_batch / HNSW::load, hnsw/builder.rs:579-640,788-833; the `lance:hnsw` metadata list
+ * of hnsw/index.rs:57-110 gives each partition's HnswMetadata {entry_point, params, level_offsets}, :283-303):
+ *   max_level, m, ef_construction   HnswBuildParams of every partition (params).
+ *   entry_point       u32 [K]: 0 -- node 0 of every non-empty partition is the entry point (:354-376) and the
+ *                     device search starts there; anything else is LB2_INVALID_ARG.
+ *   level_offsets     u64 [K][max_level + 1]: partition-local, 0 first; level l's rows are level_offsets[p][l] ..
+ *                     level_offsets[p][l + 1] - 1 of the partition's batch.
+ *   vector_id         u32 [num_graph_rows] `__vector_id`: for each partition, for each level 0 .. max_level - 1, the
+ *                     nodes that have the level, ascending (partition-local ids).  num_graph_rows = num_rows + the
+ *                     upper-level rows of the device layout (lb2_index_hnsw_*_info).
+ *   list_offsets      u64 [num_graph_rows + 1]: the Arrow list offsets of `__neighbors` and `_distance`, over the
+ *                     concatenation (a partition's own offsets are its slice minus its first entry); 0 first,
+ *                     num_edges last.
+ *   neighbors         u32 [num_edges] `__neighbors`, distances f32 [num_edges] `_distance`: each row's list in the
+ *                     order of level_neighbors_ranked, which the device layout keeps (graph/builder.rs:33-48).
+ *   An empty partition has no rows and level_offsets all 0.  HNSW::load gives every node all levels; a loaded graph
+ *   gives a node the levels whose batches hold it, which searches the same (no list names a node above its levels).
+ * lb2_index_export_storage: out->num_partitions, num_rows, num_bytes, max_level, m, ef_construction,
+ *   num_graph_rows and num_edges are set (max_level = 0 without a graph); each non-NULL buffer is written.  Call
+ *   with NULL buffers first to size them.  Buffers are host or device memory.
+ * lb2_index_load_storage: loads into a handle made by the kind's lb2_index_create* call (or one that already holds
+ *   rows; the content is replaced, graph included).  max_level = 0 loads no graph; max_level >= 1 attaches one, as
+ *   lb2_index_load_hnsw_* does, to an IVF_SQ, IVF_PQ or IVF_FLAT handle.  Every input is checked before the handle
+ *   changes; LB2_INVALID_ARG, the handle as it was, for: num_partitions other than the index's; a part length above
+ *   num_rows, or part_lengths not summing to num_rows; num_bytes other than num_rows x bytes per row; IVF_RQ without
+ *   factors or other kinds with them; list offsets that descend or do not run from 0 to num_edges; a vector_id at or
+ *   above n_p, or not ascending within its level; level_offsets that do not start at 0 and ascend by at most n_p per
+ *   level, whose level 0 is not every row of the partition, or that do not add up to num_graph_rows; a node present
+ *   at level l but absent at l - 1; more than 2m neighbours at level 0 or more than m above; a neighbour that is not
+ *   a node of its partition at that level, or is named twice in a list; a non-empty partition whose node 0 lacks a
+ *   level (lb2_index_load_hnsw_sq's check); an entry_point other than 0. */
+typedef struct {
+  uint32_t num_partitions;  /* K */
+  uint64_t num_rows, num_bytes;
+  uint64_t* part_lengths;   /* [K] */
+  uint64_t* row_ids;        /* _rowid */
+  uint8_t* payload;         /* __pq_code / __sq_code / flat / __rabit_code values */
+  float* add_factors;
+  float* scale_factors;
+  uint32_t max_level, m, ef_construction;
+  uint64_t num_graph_rows, num_edges;
+  uint32_t* entry_point;
+  uint64_t* level_offsets;
+  uint32_t* vector_id;
+  uint64_t* list_offsets;
+  uint32_t* neighbors;
+  float* distances;
+} lb2_index_storage;
+lb2_status lb2_index_export_storage(const lb2_index* index, lb2_index_storage* out);
+lb2_status lb2_index_load_storage(lb2_index* index, const lb2_index_storage* storage);
 lb2_status lb2_index_destroy(lb2_index* index);
 
 /* IvfIndexBuilder::build (rust/lance/src/index/vector/builder.rs:236): sample -> train IVF ->

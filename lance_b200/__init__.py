@@ -15,7 +15,7 @@ from ._lib import (BF16, COSINE, DOT, F16, F32, L2, METRICS, U8, BuildParams, Bu
                    DeviceArray, KMeansParams as _CKMeansParams, LanceB200Error, PinnedArray,
                    PQParams as _CPQParams, RqBuildParams as _CRqBuildParams, SqBuildParams as _CSqBuildParams,
                    HnswSqBuildParams as _CHnswSqBuildParams, HnswPqBuildParams as _CHnswPqBuildParams,
-                   HnswFlatBuildParams as _CHnswFlatBuildParams, as_ptr,
+                   HnswFlatBuildParams as _CHnswFlatBuildParams, IndexStorage as _CIndexStorage, as_ptr,
                    check, device_count, lib)
 
 __all__ = ["device_count", "DeviceArray", "PinnedArray", "LanceB200Error", "train_kmeans",
@@ -796,6 +796,90 @@ class IvfPqIndex:
         check(lib().lb2_index_transform(self._h, vp, C.c_uint64(n), *ptr))
         return dict(part_ids=part, payload=payload, add_factors=add, scale_factors=scale, valid=valid.astype(bool))
 
+    # the name of the kind's payload column in the reference's storage
+    _STORAGE_COLUMN = "__pq_code"
+
+    def export_storage(self):
+        """lb2_index_export_storage: the whole index in the reference's storage layout, every partition's batch back
+        to back (include/lance_b200.h, lb2_index_storage).  A dict of numpy arrays keyed by the reference's column
+        names -- "_rowid", the payload column ("__pq_code" transposed per partition, "__sq_code", "flat" or the packed
+        "__rabit_code", each [num_rows][bytes or elements per row] as the FixedSizeList values), IVF_RQ's
+        "__add_factors" / "__scale_factors" -- plus "part_lengths".  A graph kind adds its HNSW metadata
+        ("max_level", "m", "ef_construction", "entry_point" [K], "level_offsets" [K][max_level + 1]) and the level
+        batches: "__vector_id", "list_offsets" (the Arrow list offsets over all partitions), "__neighbors",
+        "_distance"."""
+        st = _CIndexStorage()
+        check(lib().lb2_index_export_storage(self._h, C.byref(st)))
+        K, n, L, rows, e = st.num_partitions, st.num_rows, st.max_level, st.num_graph_rows, st.num_edges
+        out = {"part_lengths": np.empty(K, np.uint64), "_rowid": np.empty(n, np.uint64),
+               self._STORAGE_COLUMN: self._payload_empty(n)}
+        if isinstance(self, IvfRqIndex):
+            out["__add_factors"], out["__scale_factors"] = np.empty(n, np.float32), np.empty(n, np.float32)
+        if L:
+            out.update({"max_level": L, "m": st.m, "ef_construction": st.ef_construction,
+                        "entry_point": np.empty(K, np.uint32), "level_offsets": np.empty((K, L + 1), np.uint64),
+                        "__vector_id": np.empty(rows, np.uint32), "list_offsets": np.empty(rows + 1, np.uint64),
+                        "__neighbors": np.empty(e, np.uint32), "_distance": np.empty(e, np.float32)})
+        ptr = lambda k: C.c_void_p(out[k].ctypes.data) if k in out and out[k].size else None  # noqa: E731
+        st.part_lengths, st.row_ids, st.payload = ptr("part_lengths"), ptr("_rowid"), ptr(self._STORAGE_COLUMN)
+        st.add_factors, st.scale_factors = ptr("__add_factors"), ptr("__scale_factors")
+        st.entry_point, st.level_offsets, st.vector_id = ptr("entry_point"), ptr("level_offsets"), ptr("__vector_id")
+        st.list_offsets, st.neighbors, st.distances = ptr("list_offsets"), ptr("__neighbors"), ptr("_distance")
+        check(lib().lb2_index_export_storage(self._h, C.byref(st)))
+        return out
+
+    @classmethod
+    def _check_storage_class(cls, storage):
+        """the graph columns are present exactly for the graph classes (IvfHnsw*Index)"""
+        graph, hnsw = "level_offsets" in storage, issubclass(cls, _HnswGraphs)
+        if graph != hnsw:
+            raise ValueError(f"{cls.__name__}.from_storage: " + (
+                "the storage has no HNSW graph columns (level_offsets, __vector_id, ...)" if hnsw else
+                "the storage has HNSW graph columns: open it with the IvfHnsw*Index class of this kind"))
+
+    def _load_storage(self, storage):
+        """lb2_index_load_storage of a dict as export_storage returns it (a graph when it has "level_offsets")"""
+        s = storage
+        a = {"part_lengths": np.ascontiguousarray(s["part_lengths"], dtype=np.uint64),
+             "_rowid": np.ascontiguousarray(s["_rowid"], dtype=np.uint64),
+             "payload": np.ascontiguousarray(s[self._STORAGE_COLUMN])}
+        for k in ("__add_factors", "__scale_factors", "_distance"):
+            if k in s:
+                a[k] = np.ascontiguousarray(s[k], dtype=np.float32)
+        for k in ("entry_point", "__vector_id", "__neighbors"):
+            if k in s:
+                a[k] = np.ascontiguousarray(s[k], dtype=np.uint32)
+        for k in ("level_offsets", "list_offsets"):
+            if k in s:
+                a[k] = np.ascontiguousarray(s[k], dtype=np.uint64)
+        ptr = lambda k: C.c_void_p(a[k].ctypes.data) if k in a and a[k].size else None  # noqa: E731
+        graph = "level_offsets" in a
+        st = _CIndexStorage(a["part_lengths"].size, a["_rowid"].size, a["payload"].nbytes, ptr("part_lengths"),
+                            ptr("_rowid"), ptr("payload"), ptr("__add_factors"), ptr("__scale_factors"),
+                            int(s["max_level"]) if graph else 0, int(s["m"]) if graph else 0,
+                            int(s.get("ef_construction", 0)) if graph else 0,
+                            a["__vector_id"].size if graph else 0, a["__neighbors"].size if graph else 0,
+                            ptr("entry_point"), ptr("level_offsets"), ptr("__vector_id"), ptr("list_offsets"),
+                            ptr("__neighbors"), ptr("_distance"))
+        check(lib().lb2_index_load_storage(self._h, C.byref(st)))
+
+    @classmethod
+    def from_storage(cls, centroids, codebook, storage, distance_type="l2", num_bits=8, dtype=np.float32, bf16=False):
+        """Open an index from its model and its storage columns (a dict as export_storage returns; with the HNSW
+        metadata and level batches for IvfHnswPqIndex).  dtype / bf16: the column's element type."""
+        cls._check_storage_class(storage)
+        dt = BF16 if bf16 else _DTYPES[np.dtype(dtype)]
+        centroids, codebook = _model_arr(centroids, dt), _model_arr(codebook, dt)
+        k, d = centroids.shape
+        h = C.c_void_p()
+        check(lib().lb2_index_create(C.c_void_p(centroids.ctypes.data), C.c_uint32(k), C.c_uint32(d), C.c_int(dt),
+                                     C.c_int(_metric(distance_type)), C.c_void_p(codebook.ctypes.data),
+                                     C.c_uint32(codebook.shape[0]), C.c_uint32(num_bits), C.byref(h)))
+        ix = cls(h)
+        ix._dt = dt
+        ix._load_storage(storage)
+        return ix
+
     def optimize(self, add_vectors=None, add_row_ids=None, add_part_ids=None, add_payload=None, add_factors=None,
                  new_centroids=None, part_map=None, remove_row_ids=None, remap=None, seed=0):
         """lb2_index_optimize: append, remove, re-map partitions and remap row ids into a NEW index of this class.
@@ -1045,6 +1129,24 @@ class IvfFlatIndex(IvfPqIndex):
         check(lib().lb2_index_load_flat(h, C.c_void_p(part_ids.ctypes.data), vp, rp, C.c_uint64(part_ids.size)))
         return ix
 
+    _STORAGE_COLUMN = "flat"
+
+    @classmethod
+    def from_storage(cls, centroids, storage, distance_type="l2", dtype=np.float32, bf16=False):
+        """Open an index from its centroids (the model type of the column) and its storage columns, as
+        IvfPqIndex.from_storage.  dtype / bf16: the element type of the stored rows."""
+        cls._check_storage_class(storage)
+        dt = BF16 if bf16 else _DTYPES[np.dtype(dtype)]
+        centroids = _model_arr(centroids, dt)
+        k, d = centroids.shape
+        h = C.c_void_p()
+        check(lib().lb2_index_create_flat(C.c_void_p(centroids.ctypes.data), C.c_uint32(k), C.c_uint32(d),
+                                          C.c_int(dt), C.c_int(_metric(distance_type)), C.byref(h)))
+        ix = cls(h)
+        ix._dt = dt
+        ix._load_storage(storage)
+        return ix
+
     def _payload_empty(self, n):
         return np.empty((n, self.info()["dimension"]),
                         {F32: np.float32, F16: np.float16, BF16: np.uint16, U8: np.float32}[getattr(self, "_dt", F32)])
@@ -1139,7 +1241,7 @@ class IvfSqIndex(IvfPqIndex):
         output (partition ids, codes [n][d], row ids).  dtype / bf16: the element type of the queries and of the
         raw column used by refine (bf16=True: uint16 bit patterns)."""
         dt = BF16 if bf16 else _DTYPES[np.dtype(dtype)]
-        centroids = np.ascontiguousarray(centroids, dtype=_model_np(dt))
+        centroids = _model_arr(centroids, dt)
         k, d = centroids.shape
         h = C.c_void_p()
         check(lib().lb2_index_create_sq(C.c_void_p(centroids.ctypes.data), k, d, dt, _metric(distance_type),
@@ -1152,6 +1254,24 @@ class IvfSqIndex(IvfPqIndex):
         rp, _k = as_ptr(rid)
         check(lib().lb2_index_load_sq(h, C.c_void_p(part_ids.ctypes.data), C.c_void_p(codes.ctypes.data), rp,
                                       C.c_uint64(part_ids.size)))
+        return ix
+
+    _STORAGE_COLUMN = "__sq_code"
+
+    @classmethod
+    def from_storage(cls, centroids, bounds, storage, distance_type="l2", dtype=np.float32, bf16=False):
+        """Open an index from its centroids, the `lance:sq` bounds and its storage columns, as
+        IvfPqIndex.from_storage."""
+        cls._check_storage_class(storage)
+        dt = BF16 if bf16 else _DTYPES[np.dtype(dtype)]
+        centroids = _model_arr(centroids, dt)
+        k, d = centroids.shape
+        h = C.c_void_p()
+        check(lib().lb2_index_create_sq(C.c_void_p(centroids.ctypes.data), k, d, dt, _metric(distance_type),
+                                        float(bounds[0]), float(bounds[1]), C.byref(h)))
+        ix = cls(h)
+        ix._dt = dt
+        ix._load_storage(storage)
         return ix
 
     def _payload_empty(self, n):
@@ -1573,6 +1693,26 @@ class IvfRqIndex(IvfPqIndex):
         check(lib().lb2_index_load_rq(h, C.c_void_p(part_ids.ctypes.data), C.c_void_p(codes.ctypes.data),
                                       C.c_void_p(add.ctypes.data), C.c_void_p(scale.ctypes.data), rp,
                                       C.c_uint64(part_ids.size)))
+        return ix
+
+    _STORAGE_COLUMN = "__rabit_code"
+
+    @classmethod
+    def from_storage(cls, centroids, rotation, storage, distance_type="l2", num_bits=1, dtype=np.float32):
+        """Open an index from its centroids, the `lance:rabit` rotation and its storage columns (the packed
+        "__rabit_code", "__add_factors", "__scale_factors"), as IvfPqIndex.from_storage."""
+        cls._check_storage_class(storage)
+        dt = _DTYPES[np.dtype(dtype)]
+        centroids = np.ascontiguousarray(centroids, dtype=_model_np(dt))
+        rotation = np.ascontiguousarray(rotation, dtype=_model_np(dt))
+        k, d = centroids.shape
+        h = C.c_void_p()
+        check(lib().lb2_index_create_rq(C.c_void_p(centroids.ctypes.data), C.c_uint32(k), C.c_uint32(d), C.c_int(dt),
+                                        C.c_int(_metric(distance_type)), C.c_void_p(rotation.ctypes.data),
+                                        C.c_uint32(num_bits), C.byref(h)))
+        ix = cls(h)
+        ix._dt = dt
+        ix._load_storage(storage)
         return ix
 
     def _payload_empty(self, n):

@@ -103,6 +103,17 @@ class JoinParams(C.Structure):
                 ("insert_batch", C.c_uint32), ("dest_out", C.c_void_p)]
 
 
+class IndexStorage(C.Structure):
+    """lb2_index_storage (include/lance_b200.h)."""
+    _fields_ = [("num_partitions", C.c_uint32), ("num_rows", C.c_uint64), ("num_bytes", C.c_uint64),
+                ("part_lengths", C.c_void_p), ("row_ids", C.c_void_p), ("payload", C.c_void_p),
+                ("add_factors", C.c_void_p), ("scale_factors", C.c_void_p), ("max_level", C.c_uint32),
+                ("m", C.c_uint32), ("ef_construction", C.c_uint32), ("num_graph_rows", C.c_uint64),
+                ("num_edges", C.c_uint64), ("entry_point", C.c_void_p), ("level_offsets", C.c_void_p),
+                ("vector_id", C.c_void_p), ("list_offsets", C.c_void_p), ("neighbors", C.c_void_p),
+                ("distances", C.c_void_p)]
+
+
 class BuildStats(C.Structure):
     _fields_ = [("ms_ivf_train", C.c_float), ("ms_pq_train", C.c_float), ("ms_transform", C.c_float),
                 ("ms_group", C.c_float), ("ms_total", C.c_float), ("ivf_iters", C.c_uint32),
@@ -134,6 +145,7 @@ EXPORTS = [
     "lb2_ivfhnswpq_build_params_default", "lb2_ivfhnswpq_build", "lb2_index_load_hnsw_pq", "lb2_index_hnsw_pq_info",
     "lb2_index_export_hnsw_pq", "lb2_ivfhnswflat_build_params_default", "lb2_ivfhnswflat_build",
     "lb2_index_load_hnsw_flat", "lb2_index_hnsw_flat_info", "lb2_index_export_hnsw_flat",
+    "lb2_index_export_storage", "lb2_index_load_storage",
 ]
 
 _lib = None

@@ -254,6 +254,17 @@ __device__ __forceinline__ bool sorted_contains(const uint64_t* __restrict__ a, 
   return lo < n && a[lo] == v;
 }
 
+// the last p < n with offsets[p] <= i (offsets ascending from offsets[0] <= i): the segment holding i, empty
+// segments skipped
+__device__ __forceinline__ int segment_of(const uint64_t* __restrict__ offsets, int n, uint64_t i) {
+  int lo = 0, hi = n;
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (offsets[mid] <= i) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+
 // our reproducible rng (the reference's is unseeded: kmeans.rs:181,645)
 struct SplitMix64 {
   uint64_t s;

@@ -67,6 +67,20 @@ void hnsw_build_flat(HnswGraph& g, const uint64_t* part_offsets, int K, const vo
 void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* levels, const uint32_t* counts0,
                const uint32_t* nbr0, const float* dist0, const uint32_t* counts_up, const uint32_t* nbr_up,
                const float* dist_up);
+// out[0] = 0, out[i + 1] = in[0] + .. + in[i] for i < n, on the device (out has n + 1 entries)
+void scan_u64(const uint64_t* in, uint64_t n, uint64_t* out);
+// The graphs in the reference's storage layout (HNSW::to_batch / HNSW::load, builder.rs:579-640,788-833), every
+// partition's level batches back to back (include/lance_b200.h, lb2_index_storage).  hnsw_storage_edges: the number
+// of list entries.  hnsw_to_storage: every output a device pointer or NULL; level_offsets [K][max_level + 1],
+// vector_id [rows], list_offsets [rows + 1] (global), neighbors / distances [edges], rows = n + g.n_up.
+uint64_t hnsw_storage_edges(const HnswGraph& g, uint64_t n);
+void hnsw_to_storage(const HnswGraph& g, const uint64_t* part_offsets, int K, uint64_t n, uint64_t* level_offsets,
+                     uint32_t* vector_id, uint64_t* list_offsets, uint32_t* neighbors, float* distances);
+// the inverse into g (max_level, m, ef_construction, kind set by the caller; device inputs): the storage checks on the
+// device, then hnsw_load of the dense layout.  LB2_INVALID_ARG on malformed input, before g is filled.
+void hnsw_from_storage(HnswGraph& g, const uint64_t* part_offsets, int K, uint64_t n, const uint32_t* entry_point,
+                       const uint64_t* level_offsets, const uint32_t* vector_id, const uint64_t* list_offsets,
+                       const uint32_t* neighbors, const float* distances, uint64_t rows, uint64_t edges);
 // HNSW::search (builder.rs:678-739) as the scan of every probed partition; ef = 0: k' + k' / 2 (builder.rs:563-573)
 void hnsw_search(const IvfSearch& s, const HnswGraph& g, const uint8_t* codes, float r2, const uint8_t* qcodes,
                  uint32_t ef);
