@@ -798,33 +798,42 @@ lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
 }  // extern "C"
 
 // the graph parameters of an HNSW build (hnsw/builder.rs:63-72) and the batched insertion's B
-static void check_hnsw_params(const char* kind, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+static void check_hnsw_params(IndexKind kind, uint32_t max_level, uint32_t m, uint32_t ef_construction,
                               uint32_t insert_batch) {
-  LB2_REQUIRE(max_level >= 1 && max_level <= 64, "%s: max_level must be in 1 .. 64, got %u", kind, max_level);
-  LB2_REQUIRE(m >= 1 && m <= 1024, "%s: m must be in 1 .. 1024, got %u", kind, m);
-  LB2_REQUIRE(ef_construction >= 1, "%s: ef_construction must be at least 1", kind);
-  LB2_REQUIRE(insert_batch <= 65536, "%s: insert_batch must be at most 65536, got %u", kind, insert_batch);
+  const char* name = hnsw_kind_name(kind);
+  LB2_REQUIRE(max_level >= 1 && max_level <= 64, "%s: max_level must be in 1 .. 64, got %u", name, max_level);
+  LB2_REQUIRE(m >= 1 && m <= 1024, "%s: m must be in 1 .. 1024, got %u", name, m);
+  LB2_REQUIRE(ef_construction >= 1, "%s: ef_construction must be at least 1", name);
+  LB2_REQUIRE(insert_batch <= 65536, "%s: insert_batch must be at most 65536, got %u", name, insert_batch);
 }
 
-// step 2 of an IVF_HNSW_* build: the graphs of `ix`, counted in stats->ms_total only
-template <class F>
-static void attach_graphs(lb2_index* ix, const char* kind, uint32_t max_level, uint32_t m, uint32_t ef_construction,
-                          uint32_t insert_batch, lb2_build_stats* stats, F&& build) {
+// an IVF_HNSW_* build: 1. build_base, the IVF_SQ, IVF_PQ or IVF_FLAT build with the same arguments (params->*base),
+// gives the IVF stage, the model and the payload; 2. HNSW::index_vectors per partition over its storage (v3
+// IvfIndexBuilder with an HNSW sub-index), counted in stats->ms_total only.  Only IVF_HNSW_SQ builds over more than
+// one rank.
+template <class P, class BP>
+static lb2_status build_hnsw(IndexKind kind, BP P::*base,
+                             lb2_status (*build_base)(const void*, uint64_t, uint32_t, lb2_dtype, lb2_metric, const BP*,
+                                                      const uint64_t*, lb2_index**, lb2_build_stats*),
+                             const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                             const P* params, const uint64_t* row_ids, lb2_index** out, lb2_build_stats* stats) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(data && params && out, "null argument");
+  check_hnsw_params(kind, params->max_level, params->m, params->ef_construction, params->insert_batch);
+  if (kind != IndexKind::SQ && comm_nranks() > 1)
+    fail(LB2_UNSUPPORTED, "%s: a build over more than one rank is not implemented", hnsw_kind_name(kind));
+  lb2_index* built = nullptr;
+  const lb2_status st = build_base(data, n, d, dtype, metric, &(params->*base), row_ids, &built, stats);
+  if (st != LB2_OK) return st;  // its message is already the last error
+  std::unique_ptr<lb2_index> ix(built);
   EventSet ev(2);
   ev.record(0);
-  {
-    TagScope tg("hnsw_build");
-    ix->hnsw.reset(new HnswGraph());
-    HnswGraph& g = *ix->hnsw;
-    g.kind = kind;
-    g.max_level = (int)max_level;
-    g.m = (int)m;
-    g.ef_construction = (int)ef_construction;
-    g.insert_batch = std::max<uint32_t>(insert_batch, 1);
-    build(g);
-  }
+  attach_graph(ix.get(), params->max_level, params->m, params->ef_construction, params->insert_batch,
+               (params->*base).seed);
   ev.record(1);
-  if (stats) stats->ms_total += ev.ms(0, 1);  // the graph build is counted in the total only
+  if (stats) stats->ms_total += ev.ms(0, 1);
+  *out = ix.release();
+  LB2_API_END
 }
 
 extern "C" {
@@ -832,69 +841,22 @@ extern "C" {
 lb2_status lb2_ivfhnswsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
                                const lb2_ivfhnswsq_build_params* params, const uint64_t* row_ids, lb2_index** out,
                                lb2_build_stats* stats) {
-  LB2_API_BEGIN
-  LB2_REQUIRE(data && params && out, "null argument");
-  check_hnsw_params("IVF_HNSW_SQ", params->max_level, params->m, params->ef_construction, params->insert_batch);
-  // 1. the IVF stage, bounds and codes of IVF_SQ with the same arguments
-  lb2_index* sq = nullptr;
-  const lb2_status st = lb2_ivfsq_build(data, n, d, dtype, metric, &params->sq, row_ids, &sq, stats);
-  if (st != LB2_OK) return st;  // its message is already the last error
-  std::unique_ptr<lb2_index> ix(sq);
-  // 2. HNSW::index_vectors per partition over its codes (v3 IvfIndexBuilder with an HNSW sub-index)
-  attach_graphs(ix.get(), "IVF_HNSW_SQ", params->max_level, params->m, params->ef_construction,
-                params->insert_batch, stats, [&](HnswGraph& g) {
-    const float rf = (float)(ix->sq_upper - ix->sq_lower);
-    hnsw_build(g, ix->part_offsets.p, ix->K, ix->codes.p, (int)d, ix->metric, rf * rf, params->sq.seed);
-  });
-  *out = ix.release();
-  LB2_API_END
+  return build_hnsw(IndexKind::SQ, &lb2_ivfhnswsq_build_params::sq, lb2_ivfsq_build, data, n, d, dtype, metric,
+                    params, row_ids, out, stats);
 }
 
 lb2_status lb2_ivfhnswpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
                                const lb2_ivfhnswpq_build_params* params, const uint64_t* row_ids, lb2_index** out,
                                lb2_build_stats* stats) {
-  LB2_API_BEGIN
-  LB2_REQUIRE(data && params && out, "null argument");
-  check_hnsw_params("IVF_HNSW_PQ", params->max_level, params->m, params->ef_construction, params->insert_batch);
-  if (comm_nranks() > 1) fail(LB2_UNSUPPORTED, "IVF_HNSW_PQ: a build over more than one rank is not implemented");
-  // 1. the IVF stage, codebook and codes of IVF_PQ with the same arguments
-  lb2_index* pq = nullptr;
-  const lb2_status st = lb2_ivfpq_build(data, n, d, dtype, metric, &params->pq, row_ids, &pq, stats);
-  if (st != LB2_OK) return st;  // its message is already the last error
-  std::unique_ptr<lb2_index> ix(pq);
-  ix->slab_off.release();  // the skewed code copy serves only the IVF_PQ scan
-  ix->codes_skew.release();
-  // 2. HNSW::index_vectors per partition over its PQ storage (IvfIndexBuilder<HNSW, ProductQuantizer>)
-  attach_graphs(ix.get(), "IVF_HNSW_PQ", params->max_level, params->m, params->ef_construction,
-                params->insert_batch, stats, [&](HnswGraph& g) {
-    hnsw_build_pq(g, ix->part_offsets.p, ix->K, ix->codes.p, ix->codebook.p, (int)d, ix->M, ix->nbits, ix->metric,
-                  dtype, params->pq.seed);
-  });
-  *out = ix.release();
-  LB2_API_END
+  return build_hnsw(IndexKind::PQ, &lb2_ivfhnswpq_build_params::pq, lb2_ivfpq_build, data, n, d, dtype, metric,
+                    params, row_ids, out, stats);
 }
 
 lb2_status lb2_ivfhnswflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
                                  const lb2_ivfhnswflat_build_params* params, const uint64_t* row_ids, lb2_index** out,
                                  lb2_build_stats* stats) {
-  LB2_API_BEGIN
-  LB2_REQUIRE(data && params && out, "null argument");
-  check_hnsw_params("IVF_HNSW_FLAT", params->max_level, params->m, params->ef_construction, params->insert_batch);
-  if (comm_nranks() > 1) fail(LB2_UNSUPPORTED, "IVF_HNSW_FLAT: a build over more than one rank is not implemented");
-  // 1. the IVF stage, vectors and row ids of IVF_FLAT with the same arguments
-  lb2_index* flat = nullptr;
-  const lb2_status st = lb2_ivfflat_build(data, n, d, dtype, metric, &params->flat, row_ids, &flat, stats);
-  if (st != LB2_OK) return st;  // its message is already the last error
-  std::unique_ptr<lb2_index> ix(flat);
-  // 2. HNSW::index_vectors per partition over its FlatFloatStorage (IvfIndexBuilder<HNSW, FlatQuantizer>)
-  attach_graphs(ix.get(), "IVF_HNSW_FLAT", params->max_level, params->m, params->ef_construction,
-                params->insert_batch, stats,
-                [&](HnswGraph& g) {
-                  hnsw_build_flat(g, ix->part_offsets.p, ix->K, ix->vectors.p, (int)ix->vdtype(), (int)d, ix->metric,
-                                  params->flat.seed);
-                });
-  *out = ix.release();
-  LB2_API_END
+  return build_hnsw(IndexKind::FLAT, &lb2_ivfhnswflat_build_params::flat, lb2_ivfflat_build, data, n, d, dtype,
+                    metric, params, row_ids, out, stats);
 }
 
 }  // extern "C"

@@ -7,8 +7,8 @@
 //           beam_search / greedy_search                  graph.rs:275-409
 //           HNSW::search / search_inner / flat_search    hnsw/builder.rs:164-280,678-739
 //
-// The engine is generic over a distance policy (SqDist, PqDist, FlatDist below), as the reference is over
-// VectorStore: `key` is the distance of the query (or of the inserting node) to a node, `between` the heuristic's
+// The engine is generic over a distance policy (SqDist, PqDist, FlatDist below; with_policy picks an index's), as the
+// reference is over VectorStore: `key` is the distance of the query (or of the inserting node) to a node, `between` the heuristic's
 // dist_between.
 //  * SQ: both are the SQ row rule of sq.cuh (sq/storage.rs:387-444, storage.rs:102-105): an integer sum times one
 //    constant, so the build is deterministic and bit-exact.
@@ -31,6 +31,7 @@
 #include "common.cuh"
 #include "exact.cuh"
 #include "hnsw.cuh"
+#include "index.cuh"
 #include "ivf_search.cuh"
 #include "pq_lut.cuh"
 #include "probe.cuh"
@@ -47,25 +48,6 @@ constexpr uint32_t NONE = 0xffffffffu;
 
 __device__ __forceinline__ uint32_t ukey_of(float f) { return (uint32_t)total_order_key(f) ^ 0x80000000u; }
 __device__ __forceinline__ float float_of(uint32_t uk) { return key_to_float((int32_t)(uk ^ 0x80000000u)); }
-
-struct GraphDev {
-  const uint8_t* nlev;
-  const uint32_t* up_base;
-  uint32_t *cnt0, *nbr0, *cntu, *nbru;
-  float *dst0, *dstu;
-  int m, max_level;
-};
-struct ListRef {
-  uint32_t* cnt;
-  uint32_t* ids;
-  float* dist;
-};
-// the list of global row `row` at `level`
-__device__ __forceinline__ ListRef list_of(const GraphDev& g, uint64_t row, int level) {
-  if (level == 0) return {g.cnt0 + row, g.nbr0 + row * 2 * g.m, g.dst0 + row * 2 * g.m};
-  const uint64_t r = (uint64_t)g.up_base[row] + (level - 1);
-  return {g.cntu + r, g.nbru + r * g.m, g.dstu + r * g.m};
-}
 
 // per-warp scratch (u32 words): PQ table tab[TW] (PQ only) and query / row qv[QW] (PQ and flat), vis[words(nmax)],
 // candidate heap ck / cid [nmax + 1], result heap rk / rid [E + 1], batch bid / bk [B], list lid / lk / ord [LB],
@@ -133,6 +115,7 @@ struct SqDist {
     n = cnt;
     codes = base + o * d;
   }
+  void at_slab(uint64_t q0) { qcodes += q0 * d; }  // a search's queries from query q0 on
   __device__ __forceinline__ Ctx node_ctx(uint32_t i, const Scratch&) const { return codes + (uint64_t)i * d; }
   __device__ __forceinline__ Ctx query_ctx(uint64_t qi, uint32_t, const Scratch&) const { return qcodes + qi * d; }
   __device__ __forceinline__ uint32_t key(Ctx q, uint32_t node) const {
@@ -168,6 +151,7 @@ struct PqDist {
     n = cnt;
     codes = base + o * cw;
   }
+  void at_slab(uint64_t q0) { queries += q0 * d; }
   // element e of a row's decoded vector (get_centroids / get_centroids_4bit: the codewords concatenated)
   __device__ __forceinline__ float elem(const uint8_t* row, int e) const {
     const int m = e / ds, t = e - m * ds;
@@ -348,6 +332,7 @@ struct FlatDist {
     n = cnt;
     rows = base + o * d;
   }
+  void at_slab(uint64_t q0) { queries += q0 * d; }
   __device__ __forceinline__ StoredRow<T> row(uint32_t i) const { return StoredRow<T>::at(rows + (uint64_t)i * d); }
   // the norm of the row in qv with ivfflat_scan_kernel's 16 FMA lanes, xor tree and sqrt (norm_l2.rs:106-130)
   __device__ __forceinline__ Ctx ctx_of_qv(const Scratch& s) const {
@@ -844,10 +829,6 @@ hnsw_search_kernel(GraphDev g, uint64_t nslots, int np, const uint32_t* __restri
   }
 }
 
-GraphDev dev_view(const HnswGraph& g) {
-  return GraphDev{g.nlev.p, g.up_base.p, g.cnt0.p, g.nbr0.p, g.cntu.p, g.nbru.p, g.dst0.p, g.dstu.p, g.m, g.max_level};
-}
-
 int32_t key_of_host(float f) { return host_total_key(f); }
 
 }  // namespace
@@ -890,13 +871,28 @@ __global__ void hnsw_splice_kernel(const SpliceSpan* __restrict__ spans, int m, 
   }
 }
 
-// the levels and the empty lists of every partition's graph, then `launch(kernel, policy)` of the build kernel with
-// the policy's table and query words TW / QW in each warp's scratch.  With `keep`, a kept partition's nodes take
-// their levels from the old graph (a loaded graph has no seed) and its lists are spliced in; only the other
-// partitions with at least 2 rows are built.  max_part and the upper rows are counted over the whole new layout.
-template <class Launch>
-static void build_graphs(HnswGraph& g, const uint64_t* part_offsets, int K, uint64_t seed, uint32_t TW, uint32_t QW,
-                         const HnswKeep* keep, Launch&& launch) {
+// the buffers of the layout for n rows, n_up upper rows and a largest partition of nmax rows (each at least 1 entry)
+static void alloc_layout(HnswGraph& g, uint64_t n, uint64_t n_up, uint64_t nmax) {
+  const uint64_t m = (uint64_t)g.m;
+  g.max_part = nmax;
+  g.n_up = n_up;
+  g.nlev.alloc(std::max<uint64_t>(n, 1));
+  g.up_base.alloc(std::max<uint64_t>(n, 1));
+  g.cnt0.alloc(std::max<uint64_t>(n, 1));
+  g.nbr0.alloc(std::max<uint64_t>(n * 2 * m, 1));
+  g.dst0.alloc(std::max<uint64_t>(n * 2 * m, 1));
+  g.cntu.alloc(std::max<uint64_t>(n_up, 1));
+  g.nbru.alloc(std::max<uint64_t>(n_up * m, 1));
+  g.dstu.alloc(std::max<uint64_t>(n_up * m, 1));
+}
+
+// the levels and the empty lists of every partition's graph, then the build kernels with policy P and its table and
+// query words TW / QW in each warp's scratch.  With `keep`, a kept partition's nodes take their levels from the old
+// graph (a loaded graph has no seed) and its lists are spliced in; only the other partitions with at least 2 rows are
+// built.  max_part and the upper rows are counted over the whole new layout.
+template <class Dist>
+static void build_graphs(HnswGraph& g, const uint64_t* part_offsets, int K, uint64_t seed, const HnswKeep* keep,
+                         const Dist& P, uint32_t TW, uint32_t QW) {
   std::vector<uint64_t> off(K + 1);
   d2h(off.data(), part_offsets, (size_t)K + 1);
   std::vector<uint8_t> old_lev;
@@ -953,16 +949,7 @@ static void build_graphs(HnswGraph& g, const uint64_t* part_offsets, int K, uint
   std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
     return off[a + 1] - off[a] > off[b + 1] - off[b];
   });
-  g.max_part = nmax;
-  g.n_up = n_up;
-  g.nlev.alloc(std::max<uint64_t>(n, 1));
-  g.up_base.alloc(std::max<uint64_t>(n, 1));
-  g.cnt0.alloc(std::max<uint64_t>(n, 1));
-  g.nbr0.alloc(std::max<uint64_t>(n * 2 * g.m, 1));
-  g.dst0.alloc(std::max<uint64_t>(n * 2 * g.m, 1));
-  g.cntu.alloc(std::max<uint64_t>(n_up, 1));
-  g.nbru.alloc(std::max<uint64_t>(n_up * g.m, 1));
-  g.dstu.alloc(std::max<uint64_t>(n_up * g.m, 1));
+  alloc_layout(g, n, n_up, nmax);
   if (n) {
     h2d(g.nlev.p, nlev.data(), n);
     h2d(g.up_base.p, up_base.data(), n);
@@ -1001,11 +988,8 @@ static void build_graphs(HnswGraph& g, const uint64_t* part_offsets, int K, uint
     const unsigned nct = (unsigned)std::min<size_t>({order.size(), (size_t)ctx().num_sms * 32, fit});
     DevBuf<uint32_t> scratch(words * nct), next(1);
     next.zero();
-    launch([&](const auto& P) {
-      using Dist = std::decay_t<decltype(P)>;
-      LB2_LAUNCH("hnsw_build", hnsw_build_kernel<Dist>, nct, 32, 0, dev_view(g), part_offsets, dorder.p,
-                 (int)order.size(), next.p, P, E, lo, hi, scratch.p, nmax, E, B, LB, TW, QW);
-    });
+    LB2_LAUNCH("hnsw_build", hnsw_build_kernel<Dist>, nct, 32, 0, dev_view(g), part_offsets, dorder.p,
+               (int)order.size(), next.p, P, E, lo, hi, scratch.p, nmax, E, B, LB, TW, QW);
     sync_stream();
     return;
   }
@@ -1041,89 +1025,95 @@ static void build_graphs(HnswGraph& g, const uint64_t* part_offsets, int K, uint
       rec_next(max_recs), touched(3 * max_recs);
   LB2_CUDA(cudaMemsetAsync(head.p, 0xff, head.n * sizeof(uint32_t), ctx().stream));  // every chain empty (NONE)
   const RoundBufs rb{counters.p, head.p, rec_i.p, rec_key.p, rec_next.p, touched.p};
-  launch([&](const auto& P) {
-    using Dist = std::decay_t<decltype(P)>;
-    for (const Round& r : rounds) {
-      const uint64_t items = (uint64_t)r.nparts * r.W;
-      counters.zero();
-      LB2_LAUNCH("hnsw_round_search", hnsw_round_search_kernel<Dist>, (unsigned)std::min<uint64_t>(items, nct), 32, 0,
-                 dev_view(g), part_offsets, dorder.p, r.nparts, r.s0, r.W, rb, P, E, lo, hi, scratch.p, nmax, E, B, LB,
-                 TW, QW);
-      LB2_LAUNCH("hnsw_round_link", hnsw_round_link_kernel, (unsigned)cdiv(items, 128), 128, 0, dev_view(g), n,
-                 part_offsets, dorder.p, r.nparts, r.s0, r.W, rb);
-      LB2_LAUNCH("hnsw_round_apply", hnsw_round_apply_kernel<Dist>, nct, 32, 0, dev_view(g), n, part_offsets, rb, P,
-                 scratch.p, nmax, E, B, LB, TW, QW);
-    }
-  });
-  sync_stream();
-}
-
-void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, int d, int metric, float r2,
-                uint64_t seed, const HnswKeep* keep) {
-  build_graphs(g, part_offsets, K, seed, 0, 0, keep, [&](auto go) {
-    auto with = [&](auto m) {
-      SqDist<decltype(m)::value> P{};
-      P.base = codes;
-      P.d = d;
-      P.r2 = r2;
-      go(P);
-    };
-    if (metric == METRIC_DOT) with(std::integral_constant<int, METRIC_DOT>{});
-    else with(std::integral_constant<int, METRIC_L2>{});  // cosine: L2 on the normalised vectors' codes
-  });
-}
-
-// the PQ policy's template arguments: f(metric, nbits, rule) with std::integral_constants.  Cosine is L2 (the
-// storage's distance type, pq/storage.rs:465-468); dist_between of 16-bit rows under dot takes 32 lanes
-// (dot.rs:78-83,133), every other case 16.
-template <class F>
-static void dispatch_pq(int metric, int nbits, lb2_dtype dtype, F&& f) {
-  auto by_bits = [&](auto m, auto rule) {
-    if (nbits == 4) f(m, std::integral_constant<int, 4>{}, rule);
-    else f(m, std::integral_constant<int, 8>{}, rule);
-  };
-  if (metric == METRIC_DOT) {
-    if (dtype == LB2_F16 || dtype == LB2_BF16)
-      by_bits(std::integral_constant<int, METRIC_DOT>{}, std::integral_constant<int, RULE_DOT32>{});
-    else
-      by_bits(std::integral_constant<int, METRIC_DOT>{}, std::integral_constant<int, RULE_LANES16>{});
-  } else {
-    by_bits(std::integral_constant<int, METRIC_L2>{}, std::integral_constant<int, RULE_LANES16>{});
+  for (const Round& r : rounds) {
+    const uint64_t items = (uint64_t)r.nparts * r.W;
+    counters.zero();
+    LB2_LAUNCH("hnsw_round_search", hnsw_round_search_kernel<Dist>, (unsigned)std::min<uint64_t>(items, nct), 32, 0,
+               dev_view(g), part_offsets, dorder.p, r.nparts, r.s0, r.W, rb, P, E, lo, hi, scratch.p, nmax, E, B, LB,
+               TW, QW);
+    LB2_LAUNCH("hnsw_round_link", hnsw_round_link_kernel, (unsigned)cdiv(items, 128), 128, 0, dev_view(g), n,
+               part_offsets, dorder.p, r.nparts, r.s0, r.W, rb);
+    LB2_LAUNCH("hnsw_round_apply", hnsw_round_apply_kernel<Dist>, nct, 32, 0, dev_view(g), n, part_offsets, rb, P,
+               scratch.p, nmax, E, B, LB, TW, QW);
   }
+  sync_stream();
 }
 
 // the words of a PQ warp's table (M x 2^nbits) and of a PQ or flat warp's query / row (d, kept 16-byte aligned)
 static uint32_t pq_table_words(int M, int nbits) { return (uint32_t)M << nbits; }
 static uint32_t query_words(int d) { return (uint32_t)(d + 3) & ~3u; }
 
-void hnsw_build_flat(HnswGraph& g, const uint64_t* part_offsets, int K, const void* vectors, int vdt, int d, int metric,
-                     uint64_t seed, const HnswKeep* keep) {
-  build_graphs(g, part_offsets, K, seed, 0, query_words(d), keep, [&](auto go) {
-    dispatch_metric_elem<false>(metric, vdt, [&](auto m, auto e) {
-      using T = typename decltype(e)::type;
-      using Dist = FlatDist<decltype(m)::value, T>;
-      Dist P{};
-      P.base = static_cast<const T*>(vectors);
-      P.d = d;
-      go(P);
-    });
-  });
+// The distance policy of ix's graphs, the one place it is chosen: f(P, TW, QW) with P over ix's payload and model and
+// TW / QW its table and query words in each warp's scratch.  s: the search (nullptr: the build), whose P holds its
+// queries (f32, normalised under cosine) and the SQ query codes `qcodes` from query 0 on (at_slab moves them).
+//  * SQ: r2 = (upper - lower)^2 (inverse_scalar_dist, sq.rs:279-287); cosine is L2 on the normalised vectors' codes.
+//  * PQ: cosine is L2 (the storage's distance type, pq/storage.rs:465-468); dist_between of 16-bit rows under dot
+//    takes 32 lanes (dot.rs:78-83,133), every other case 16.  The search never calls `between`, so it takes the f32
+//    rule: one rule per (metric, nbits).
+//  * FLAT: every distance, cosine included, is the IVF_FLAT scan's rule for the metric and the stored element type.
+template <class F>
+static void with_policy(const lb2_index& ix, const IvfSearch* s, const uint8_t* qcodes, F&& f) {
+  const int d = ix.d, M = ix.M, nbits = ix.nbits;
+  const float* queries = s ? s->queries : nullptr;
+  switch (ix.kind) {
+    case IndexKind::SQ: {
+      const float rf = (float)(ix.sq_upper - ix.sq_lower);
+      auto go = [&](auto m) {
+        SqDist<decltype(m)::value> P{};
+        P.base = ix.codes.p;
+        P.qcodes = qcodes;
+        P.d = d;
+        P.r2 = rf * rf;
+        f(P, 0u, 0u);
+      };
+      if (ix.metric == METRIC_DOT) go(std::integral_constant<int, METRIC_DOT>{});
+      else go(std::integral_constant<int, METRIC_L2>{});
+      break;
+    }
+    case IndexKind::PQ: {
+      auto go = [&](auto m, auto rule) {
+        auto with_bits = [&](auto b) {
+          PqDist<decltype(m)::value, decltype(b)::value, decltype(rule)::value> P{};
+          P.base = ix.codes.p;
+          P.codebook = ix.codebook.p;
+          P.queries = queries;
+          P.centroids = ix.centroids.p;
+          P.d = d;
+          P.M = M;
+          P.ds = d / M;
+          P.cw = nbits == 4 ? M / 2 : M;
+          f(P, pq_table_words(M, nbits), query_words(d));
+        };
+        if (nbits == 4) with_bits(std::integral_constant<int, 4>{});
+        else with_bits(std::integral_constant<int, 8>{});
+      };
+      const lb2_dtype rule_dtype = s ? LB2_F32 : ix.dtype;
+      if (ix.metric != METRIC_DOT)
+        go(std::integral_constant<int, METRIC_L2>{}, std::integral_constant<int, RULE_LANES16>{});
+      else if (rule_dtype == LB2_F16 || rule_dtype == LB2_BF16)
+        go(std::integral_constant<int, METRIC_DOT>{}, std::integral_constant<int, RULE_DOT32>{});
+      else
+        go(std::integral_constant<int, METRIC_DOT>{}, std::integral_constant<int, RULE_LANES16>{});
+      break;
+    }
+    case IndexKind::FLAT:
+      dispatch_metric_elem<false>(ix.metric, (int)ix.vdtype(), [&](auto m, auto e) {
+        using T = typename decltype(e)::type;
+        FlatDist<decltype(m)::value, T> P{};
+        P.base = reinterpret_cast<const T*>(ix.vectors.p);
+        P.queries = queries;
+        P.d = d;
+        f(P, 0u, query_words(d));
+      });
+      break;
+    case IndexKind::RQ:  // no IVF_RQ index has a graph
+      break;
+  }
 }
 
-void hnsw_build_pq(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, const float* codebook,
-                   int d, int M, int nbits, int metric, lb2_dtype dtype, uint64_t seed, const HnswKeep* keep) {
-  build_graphs(g, part_offsets, K, seed, pq_table_words(M, nbits), query_words(d), keep, [&](auto go) {
-    dispatch_pq(metric, nbits, dtype, [&](auto m, auto b, auto r) {
-      using Dist = PqDist<decltype(m)::value, decltype(b)::value, decltype(r)::value>;
-      Dist P{};
-      P.base = codes;
-      P.codebook = codebook;
-      P.d = d;
-      P.M = M;
-      P.ds = d / M;
-      P.cw = nbits == 4 ? M / 2 : M;
-      go(P);
-    });
+void hnsw_build(HnswGraph& g, const lb2_index& ix, uint64_t seed, const HnswKeep* keep) {
+  with_policy(ix, nullptr, nullptr, [&](const auto& P, uint32_t TW, uint32_t QW) {
+    build_graphs(g, ix.part_offsets.p, ix.K, seed, keep, P, TW, QW);
   });
 }
 
@@ -1190,16 +1180,7 @@ void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t*
       }
     }
   }
-  g.max_part = nmax;
-  g.n_up = n_up;
-  g.nlev.alloc(std::max<uint64_t>(n, 1));
-  g.up_base.alloc(std::max<uint64_t>(n, 1));
-  g.cnt0.alloc(std::max<uint64_t>(n, 1));
-  g.nbr0.alloc(std::max<uint64_t>(n * 2 * m, 1));
-  g.dst0.alloc(std::max<uint64_t>(n * 2 * m, 1));
-  g.cntu.alloc(std::max<uint64_t>(n_up, 1));
-  g.nbru.alloc(std::max<uint64_t>(n_up * m, 1));
-  g.dstu.alloc(std::max<uint64_t>(n_up * m, 1));
+  alloc_layout(g, n, n_up, nmax);
   cudaStream_t st = ctx().stream;
   if (n) {
     h2d(g.nlev.p, lv.data(), n);
@@ -1216,11 +1197,11 @@ void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t*
   sync_stream();
 }
 
-// HNSW::search of every probed partition with `launch(kernel, policy, scratch words)`; `bind(policy, slots)` points the
-// policy at the slab's queries
-template <class Launch>
-static void search_graphs(const IvfSearch& s, const HnswGraph& g, uint32_t ef, uint32_t TW, uint32_t QW,
-                          Launch&& launch) {
+// HNSW::search of every probed partition with policy P0 (its queries from the search's first on) and its table and
+// query words TW / QW in each warp's scratch
+template <class Dist>
+static void search_graphs(const IvfSearch& s, const HnswGraph& g, uint32_t ef, const Dist& P0, uint32_t TW,
+                          uint32_t QW) {
   const uint32_t kc = (uint32_t)s.k;
   if (ef == 0) ef = kc + kc / 2;
   if (ef < kc) fail(LB2_INVALID_ARG, "%s: ef = %u must be greater than or equal to k = %u", g.kind, ef, kc);
@@ -1239,408 +1220,18 @@ static void search_graphs(const IvfSearch& s, const HnswGraph& g, uint32_t ef, u
     const uint64_t nslots = sl.qn * sl.np;
     if (nslots == 0) return;
     const unsigned nct = (unsigned)std::min<uint64_t>(nslots, cap);
-    launch(sl, [&](auto kern, const auto& P) {
-      LB2_LAUNCH("hnsw_search", kern, nct, 32, 0, dev_view(g), nslots, sl.np, sl.probe_ids, sl.offsets, acnt.p, P,
-                 s.row_ids, ef, (int)kc, s.flt, sl.cand_d, sl.cand_id, sl.cand_cnt, scratch.p, nmax, E, B, TW, QW);
-    });
+    Dist P = P0;
+    P.at_slab(sl.q0);
+    LB2_LAUNCH("hnsw_search", hnsw_search_kernel<Dist>, nct, 32, 0, dev_view(g), nslots, sl.np, sl.probe_ids,
+               sl.offsets, acnt.p, P, s.row_ids, ef, (int)kc, s.flt, sl.cand_d, sl.cand_id, sl.cand_cnt, scratch.p,
+               nmax, E, B, TW, QW);
   });
 }
 
-void hnsw_search(const IvfSearch& s, const HnswGraph& g, const uint8_t* codes, float r2, const uint8_t* qcodes,
-                 uint32_t ef) {
-  search_graphs(s, g, ef, 0, 0, [&](const ScanSlots& sl, auto go) {
-    auto with = [&](auto m) {
-      SqDist<decltype(m)::value> P{};
-      P.base = codes;
-      P.qcodes = qcodes + sl.q0 * s.d;
-      P.d = s.d;
-      P.r2 = r2;
-      go(hnsw_search_kernel<SqDist<decltype(m)::value>>, P);
-    };
-    if (s.metric == METRIC_DOT) with(std::integral_constant<int, METRIC_DOT>{});
-    else with(std::integral_constant<int, METRIC_L2>{});
+void hnsw_search(const IvfSearch& s, const lb2_index& ix, const uint8_t* sq_query_codes, uint32_t ef) {
+  with_policy(ix, &s, sq_query_codes, [&](const auto& P, uint32_t TW, uint32_t QW) {
+    search_graphs(s, *ix.hnsw, ef, P, TW, QW);
   });
-}
-
-void hnsw_search_pq(const IvfSearch& s, const HnswGraph& g, const float* codebook, int M, int nbits,
-                    const uint8_t* codes, uint32_t ef) {
-  search_graphs(s, g, ef, pq_table_words(M, nbits), query_words(s.d), [&](const ScanSlots& sl, auto go) {
-    // the search never calls `between`: one rule per (metric, nbits)
-    dispatch_pq(s.metric, nbits, LB2_F32, [&](auto m, auto b, auto r) {
-      using Dist = PqDist<decltype(m)::value, decltype(b)::value, decltype(r)::value>;
-      Dist P{};
-      P.base = codes;
-      P.codebook = codebook;
-      P.queries = s.queries + sl.q0 * s.d;
-      P.centroids = s.centroids;
-      P.d = s.d;
-      P.M = M;
-      P.ds = s.d / M;
-      P.cw = nbits == 4 ? M / 2 : M;
-      go(hnsw_search_kernel<Dist>, P);
-    });
-  });
-}
-
-void hnsw_search_flat(const IvfSearch& s, const HnswGraph& g, const void* vectors, int vdt, uint32_t ef) {
-  search_graphs(s, g, ef, 0, query_words(s.d), [&](const ScanSlots& sl, auto go) {
-    dispatch_metric_elem<false>(s.metric, vdt, [&](auto m, auto e) {
-      using T = typename decltype(e)::type;
-      using Dist = FlatDist<decltype(m)::value, T>;
-      Dist P{};
-      P.base = static_cast<const T*>(vectors);
-      P.queries = s.queries + sl.q0 * s.d;
-      P.d = s.d;
-      go(hnsw_search_kernel<Dist>, P);
-    });
-  });
-}
-
-// ---- the reference's storage layout of the graphs (HNSW::to_batch / HNSW::load, builder.rs:283-303,579-640,788-833)
-// One record batch per partition: level 0 .. max_level - 1, a row per node that has the level, ascending node id.
-
-// out[0] = 0, out[i + 1] = in[0] + .. + in[i]: a block-local scan of 1024-element tiles, the tile sums scanned by one
-// block, then added back
-__device__ __forceinline__ uint64_t block_exclusive_scan(uint64_t v, uint64_t* warp_sums, uint64_t* total) {
-  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  uint64_t x = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint64_t y = __shfl_up_sync(0xffffffffu, x, o);
-    if (lane >= o) x += y;
-  }
-  if (lane == 31) warp_sums[w] = x;
-  __syncthreads();
-  uint64_t before = 0, all = 0;
-  for (int i = 0; i < nw; ++i) {
-    if (i < w) before += warp_sums[i];
-    all += warp_sums[i];
-  }
-  __syncthreads();
-  *total = all;
-  return before + x - v;
-}
-
-__global__ void scan_tiles_kernel(const uint64_t* __restrict__ in, uint64_t n, uint64_t* __restrict__ tile_sums) {
-  __shared__ uint64_t ws[32];
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  uint64_t t;
-  block_exclusive_scan(i < n ? in[i] : 0, ws, &t);
-  if (threadIdx.x == 0) tile_sums[blockIdx.x] = t;
-}
-
-__global__ void scan_sums_kernel(uint64_t* __restrict__ sums, uint64_t nt) {
-  __shared__ uint64_t ws[32];
-  uint64_t carry = 0;
-  for (uint64_t b = 0; b < nt; b += blockDim.x) {
-    const uint64_t i = b + threadIdx.x;
-    const uint64_t v = i < nt ? sums[i] : 0;
-    uint64_t t;
-    const uint64_t e = block_exclusive_scan(v, ws, &t);
-    if (i < nt) sums[i] = carry + e;
-    carry += t;
-  }
-  if (threadIdx.x == 0) sums[nt] = carry;
-}
-
-__global__ void scan_apply_kernel(const uint64_t* __restrict__ in, uint64_t n, const uint64_t* __restrict__ tile_sums,
-                                  uint64_t* __restrict__ out) {
-  __shared__ uint64_t ws[32];
-  const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  uint64_t t;
-  const uint64_t e = block_exclusive_scan(i < n ? in[i] : 0, ws, &t);
-  if (i < n) out[i] = tile_sums[blockIdx.x] + e;
-  if (i == 0) out[n] = tile_sums[gridDim.x];
-}
-
-void scan_u64(const uint64_t* in, uint64_t n, uint64_t* out) {
-  if (n == 0) {
-    LB2_CUDA(cudaMemsetAsync(out, 0, sizeof(uint64_t), ctx().stream));
-    return;
-  }
-  const uint64_t nt = cdiv(n, 1024);
-  DevBuf<uint64_t> sums(nt + 1);
-  LB2_LAUNCH("storage_scan", scan_tiles_kernel, (unsigned)nt, 1024, 0, in, n, sums.p);
-  LB2_LAUNCH("storage_scan", scan_sums_kernel, 1, 1024, 0, sums.p, nt);
-  LB2_LAUNCH("storage_scan", scan_apply_kernel, (unsigned)nt, 1024, 0, in, n, sums.p, out);
-}
-
-// per partition: level_offsets (lo[p][l + 1] - lo[p][l] = nodes with more than l levels) and its batch's rows
-__global__ void graph_level_offsets_kernel(const uint8_t* __restrict__ nlev, const uint64_t* __restrict__ off, int L,
-                                           uint64_t* __restrict__ lo, uint64_t* __restrict__ rows) {
-  __shared__ unsigned long long hist[64];
-  const int p = blockIdx.x;
-  for (int l = threadIdx.x; l < L; l += blockDim.x) hist[l] = 0;
-  __syncthreads();
-  for (uint64_t r = off[p] + threadIdx.x; r < off[p + 1]; r += blockDim.x) atomicAdd(&hist[nlev[r] - 1], 1ull);
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    uint64_t at_least = 0;  // nodes with more than l levels, from the top down
-    for (int l = L - 1; l >= 0; --l) {
-      at_least += hist[l];
-      hist[l] = at_least;
-    }
-    uint64_t acc = 0;
-    uint64_t* o = lo + (uint64_t)p * (L + 1);
-    for (int l = 0; l < L; ++l) {
-      o[l] = acc;
-      acc += hist[l];
-    }
-    o[L] = acc;
-    rows[p] = acc;
-  }
-}
-
-// per partition, in tiles of nodes: the rank of each (node, level) among the level's nodes -> its row of the batches
-// (gb[p] + lo[p][l] + rank): the node id, the list length and where the list lives in the dense layout
-__global__ void graph_rows_kernel(GraphDev g, const uint64_t* __restrict__ off, const uint64_t* __restrict__ gb,
-                                  const uint64_t* __restrict__ lo, uint64_t n, uint32_t* __restrict__ vid,
-                                  uint64_t* __restrict__ len, uint64_t* __restrict__ slot) {
-  __shared__ uint64_t ws[32];
-  __shared__ uint64_t run[64];
-  const int p = blockIdx.x, L = g.max_level;
-  const uint64_t o = off[p], np = off[p + 1] - o;
-  const uint64_t* lp = lo + (uint64_t)p * (L + 1);
-  for (int l = threadIdx.x; l < L; l += blockDim.x) run[l] = 0;
-  __syncthreads();
-  for (uint64_t base = 0; base < np; base += blockDim.x) {
-    const uint64_t i = base + threadIdx.x;
-    const int lv = i < np ? g.nlev[o + i] : 0;
-    for (int l = 0; l < L; ++l) {
-      uint64_t t;
-      // run[l] is read only after the scan's barriers: thread 0 wrote it after the previous tile's last barrier, and
-      // with max_level 1 no other barrier lies between that write and this read
-      const uint64_t e = block_exclusive_scan(lv > l ? 1 : 0, ws, &t);
-      const uint64_t rank = run[l] + e;
-      if (lv > l) {
-        const uint64_t gr = gb[p] + lp[l] + rank, r = o + i;
-        vid[gr] = (uint32_t)i;
-        len[gr] = *list_of(g, r, l).cnt;
-        slot[gr] = l == 0 ? r : n + g.up_base[r] + (l - 1);
-      }
-      __syncthreads();
-      if (threadIdx.x == 0) run[l] += t;
-    }
-  }
-}
-
-// one warp per batch row: its list, in ranked order, from the dense layout to the concatenated list values
-__global__ void graph_edges_out_kernel(GraphDev g, uint64_t rows, const uint64_t* __restrict__ slot, uint64_t n,
-                                       const uint64_t* __restrict__ loff, uint32_t* __restrict__ nbr,
-                                       float* __restrict__ dst) {
-  const uint64_t gr = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (gr >= rows) return;
-  const uint64_t s = slot[gr], a = loff[gr], c = loff[gr + 1] - a;
-  const uint32_t* sn = s < n ? g.nbr0 + s * 2 * g.m : g.nbru + (s - n) * g.m;
-  const float* sd = s < n ? g.dst0 + s * 2 * g.m : g.dstu + (s - n) * g.m;
-  for (uint64_t j = lane; j < c; j += 32) {
-    if (nbr) nbr[a + j] = sn[j];
-    if (dst) dst[a + j] = sd[j];
-  }
-}
-
-__global__ void sum_counts_kernel(const uint32_t* __restrict__ a, uint64_t n, unsigned long long* __restrict__ out) {
-  unsigned long long s = 0;
-  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) s += a[i];
-#pragma unroll
-  for (int o = 16; o >= 1; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-  if ((threadIdx.x & 31) == 0 && s) atomicAdd(out, s);
-}
-
-uint64_t hnsw_storage_edges(const HnswGraph& g, uint64_t n) {
-  DevBuf<unsigned long long> e(1);
-  e.zero();
-  const unsigned grid = (unsigned)std::max<uint64_t>(1, std::min<uint64_t>(cdiv(std::max(n, g.n_up), 256), 1024));
-  if (n) LB2_LAUNCH("hnsw_to_storage", sum_counts_kernel, grid, 256, 0, g.cnt0.p, n, e.p);
-  if (g.n_up) LB2_LAUNCH("hnsw_to_storage", sum_counts_kernel, grid, 256, 0, g.cntu.p, g.n_up, e.p);
-  unsigned long long h = 0;
-  d2h(&h, e.p, 1);
-  sync_stream();
-  return h;
-}
-
-void hnsw_to_storage(const HnswGraph& g, const uint64_t* part_offsets, int K, uint64_t n, uint64_t* level_offsets,
-                     uint32_t* vector_id, uint64_t* list_offsets, uint32_t* neighbors, float* distances) {
-  const int L = g.max_level;
-  const uint64_t rows = n + g.n_up;
-  DevBuf<uint64_t> lo((size_t)K * (L + 1)), prow(K), gb(K + 1), len(std::max<uint64_t>(rows, 1)),
-      slot(std::max<uint64_t>(rows, 1)), loff(rows + 1);
-  DevBuf<uint32_t> vid(std::max<uint64_t>(rows, 1));
-  LB2_LAUNCH("hnsw_to_storage", graph_level_offsets_kernel, K, 256, 0, g.nlev.p, part_offsets, L, lo.p, prow.p);
-  scan_u64(prow.p, K, gb.p);
-  if (rows) LB2_LAUNCH("hnsw_to_storage", graph_rows_kernel, K, 1024, 0, dev_view(g), part_offsets, gb.p, lo.p, n,
-                       vid.p, len.p, slot.p);
-  scan_u64(len.p, rows, loff.p);
-  if (rows && (neighbors || distances))
-    LB2_LAUNCH("hnsw_to_storage", graph_edges_out_kernel, cdiv(rows * 32, 256), 256, 0, dev_view(g), rows, slot.p, n,
-               loff.p, neighbors, distances);
-  cudaStream_t st = ctx().stream;
-  if (level_offsets) LB2_CUDA(cudaMemcpyAsync(level_offsets, lo.p, 8 * lo.n, cudaMemcpyDeviceToDevice, st));
-  if (vector_id && rows) LB2_CUDA(cudaMemcpyAsync(vector_id, vid.p, 4 * rows, cudaMemcpyDeviceToDevice, st));
-  if (list_offsets) LB2_CUDA(cudaMemcpyAsync(list_offsets, loff.p, 8 * (rows + 1), cudaMemcpyDeviceToDevice, st));
-  sync_stream();
-}
-
-// the checks of hnsw_from_storage, in the order they are reported
-enum : uint32_t {
-  SE_LEVEL_OFFSETS = 1, SE_LEVEL0, SE_ENTRY, SE_VECTOR_ID, SE_ASCENDING, SE_LIST_OFFSETS, SE_DEGREE, SE_GAP
-};
-__device__ __forceinline__ void storage_error(uint64_t* err, uint32_t code, uint64_t where) {
-  if (atomicCAS(reinterpret_cast<unsigned long long*>(err), 0ull, (unsigned long long)code) == 0) err[1] = where;
-}
-
-// per partition: level_offsets start at 0 and ascend by at most n_p per level, level 0 holds every row of the
-// partition, the entry point is node 0; rows[p] = the batch's rows
-__global__ void storage_check_parts_kernel(const uint64_t* __restrict__ off, int K, int L, const uint64_t* __restrict__ lo,
-                                           const uint32_t* __restrict__ entry, uint64_t* __restrict__ rows,
-                                           uint64_t* __restrict__ err) {
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= K) return;
-  const uint64_t* o = lo + (uint64_t)p * (L + 1);
-  const uint64_t np = off[p + 1] - off[p];
-  bool mono = o[0] == 0;
-  for (int l = 0; l < L; ++l) mono = mono && o[l + 1] >= o[l] && o[l + 1] - o[l] <= np;
-  if (!mono) storage_error(err, SE_LEVEL_OFFSETS, p);
-  else if (o[1] != np) storage_error(err, SE_LEVEL0, p);
-  if (entry[p] != 0) storage_error(err, SE_ENTRY, p);
-  rows[p] = mono ? o[L] : 0;
-}
-
-// the partition p and level l of batch row gr, and its position i in the level
-struct BatchRow {
-  int p, l;
-  uint64_t i;
-};
-__device__ __forceinline__ BatchRow batch_row(const uint64_t* gb, int K, const uint64_t* lo, int L, uint64_t gr) {
-  BatchRow b;
-  b.p = segment_of(gb, K, gr);
-  const uint64_t* o = lo + (uint64_t)b.p * (L + 1);
-  const uint64_t t = gr - gb[b.p];
-  b.l = segment_of(o, L, t);
-  b.i = t - o[b.l];
-  return b;
-}
-
-// one thread per batch row: the id is a node of the partition, ascending in its level; the list offsets ascend and
-// the list fits the level's degree; the node's level mask gains bit l
-__global__ void storage_check_rows_kernel(const uint64_t* __restrict__ off, int K, const uint64_t* __restrict__ gb,
-                                          const uint64_t* __restrict__ lo, int L, int m, uint64_t rows,
-                                          const uint32_t* __restrict__ vid, const uint64_t* __restrict__ loff,
-                                          unsigned long long* __restrict__ mask, uint64_t* __restrict__ err) {
-  const uint64_t gr = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (gr >= rows) return;
-  const BatchRow b = batch_row(gb, K, lo, L, gr);
-  const uint64_t np = off[b.p + 1] - off[b.p];
-  const uint32_t v = vid[gr];
-  if (v >= np) { storage_error(err, SE_VECTOR_ID, gr); return; }
-  if (b.i > 0 && vid[gr - 1] >= v) { storage_error(err, SE_ASCENDING, gr); return; }
-  if (loff[gr + 1] < loff[gr]) { storage_error(err, SE_LIST_OFFSETS, gr); return; }
-  if (loff[gr + 1] - loff[gr] > (uint64_t)(b.l == 0 ? 2 * m : m)) { storage_error(err, SE_DEGREE, gr); return; }
-  atomicOr(&mask[off[b.p] + v], 1ull << b.l);
-}
-
-// one thread per node: its levels are 0 .. L - 1 without a gap -> nlev, and its L - 1 upper rows
-__global__ void storage_node_levels_kernel(const unsigned long long* __restrict__ mask, uint64_t n,
-                                           uint8_t* __restrict__ nlev, uint64_t* __restrict__ nup,
-                                           uint64_t* __restrict__ err) {
-  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n) return;
-  const unsigned long long k = mask[r];
-  if (k == 0 || (k & (k + 1)) != 0) storage_error(err, SE_GAP, r);
-  const int L = __popcll(k);
-  nlev[r] = (uint8_t)L;
-  nup[r] = L ? L - 1 : 0;
-}
-
-// one warp per batch row: its list into the dense layout (level 0 row r, upper row up[r] + l - 1)
-__global__ void storage_edges_in_kernel(const uint64_t* __restrict__ off, int K, const uint64_t* __restrict__ gb,
-                                        const uint64_t* __restrict__ lo, int L, int m, uint64_t rows,
-                                        const uint32_t* __restrict__ vid, const uint64_t* __restrict__ loff,
-                                        const uint32_t* __restrict__ nbr, const float* __restrict__ dst,
-                                        const uint64_t* __restrict__ up, uint32_t* __restrict__ cnt0,
-                                        uint32_t* __restrict__ nbr0, float* __restrict__ dst0,
-                                        uint32_t* __restrict__ cntu, uint32_t* __restrict__ nbru,
-                                        float* __restrict__ dstu) {
-  const uint64_t gr = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int lane = threadIdx.x & 31;
-  if (gr >= rows) return;
-  const BatchRow b = batch_row(gb, K, lo, L, gr);
-  const uint64_t r = off[b.p] + vid[gr], a = loff[gr], c = loff[gr + 1] - a;
-  uint32_t* on;
-  float* od;
-  if (b.l == 0) {
-    on = nbr0 + r * 2 * m;
-    od = dst0 + r * 2 * m;
-    if (lane == 0) cnt0[r] = (uint32_t)c;
-  } else {
-    const uint64_t u = up[r] + (b.l - 1);
-    on = nbru + u * m;
-    od = dstu + u * m;
-    if (lane == 0) cntu[u] = (uint32_t)c;
-  }
-  for (uint64_t j = lane; j < c; j += 32) {
-    on[j] = nbr[a + j];
-    od[j] = dst[a + j];
-  }
-}
-
-void hnsw_from_storage(HnswGraph& g, const uint64_t* part_offsets, int K, uint64_t n, const uint32_t* entry_point,
-                       const uint64_t* level_offsets, const uint32_t* vector_id, const uint64_t* list_offsets,
-                       const uint32_t* neighbors, const float* distances, uint64_t rows, uint64_t edges) {
-  const int L = g.max_level, m = g.m;
-  DevBuf<uint64_t> err(2), prow(K), gb(K + 1), nup(std::max<uint64_t>(n, 1)), up(n + 1);
-  err.zero();
-  LB2_LAUNCH("hnsw_from_storage", storage_check_parts_kernel, cdiv(K, 256), 256, 0, part_offsets, K, L, level_offsets,
-             entry_point, prow.p, err.p);
-  scan_u64(prow.p, K, gb.p);
-  uint64_t h[3], e[2];
-  d2h(h, gb.p + K, 1);
-  d2h(h + 1, list_offsets, 1);
-  d2h(h + 2, list_offsets + rows, 1);
-  d2h(e, err.p, 2);
-  sync_stream();
-  auto report = [&](uint64_t code, uint64_t at) {
-    switch (code) {
-      case SE_LEVEL_OFFSETS: fail(LB2_INVALID_ARG, "%s: level_offsets of partition %llu do not start at 0 and ascend by at most the partition's rows per level", g.kind, (unsigned long long)at);
-      case SE_LEVEL0: fail(LB2_INVALID_ARG, "%s: level 0 of partition %llu does not hold every row of the partition", g.kind, (unsigned long long)at);
-      case SE_ENTRY: fail(LB2_INVALID_ARG, "%s: the entry point of partition %llu is not node 0", g.kind, (unsigned long long)at);
-      case SE_VECTOR_ID: fail(LB2_INVALID_ARG, "%s: __vector_id of batch row %llu is not a node of its partition", g.kind, (unsigned long long)at);
-      case SE_ASCENDING: fail(LB2_INVALID_ARG, "%s: __vector_id of batch row %llu does not ascend within its level", g.kind, (unsigned long long)at);
-      case SE_LIST_OFFSETS: fail(LB2_INVALID_ARG, "%s: the list offsets of batch row %llu descend", g.kind, (unsigned long long)at);
-      case SE_DEGREE: fail(LB2_INVALID_ARG, "%s: batch row %llu has more neighbours than its level allows (2m at level 0, m above)", g.kind, (unsigned long long)at);
-      case SE_GAP: fail(LB2_INVALID_ARG, "%s: row %llu is present at a level but absent at the level below", g.kind, (unsigned long long)at);
-    }
-  };
-  report(e[0], e[1]);
-  LB2_REQUIRE(h[0] == rows, "%s: level_offsets give %llu batch rows, the storage has %llu", g.kind,
-              (unsigned long long)h[0], (unsigned long long)rows);
-  LB2_REQUIRE(h[1] == 0 && h[2] == edges, "%s: the list offsets run from %llu to %llu, not from 0 to the %llu edges",
-              g.kind, (unsigned long long)h[1], (unsigned long long)h[2], (unsigned long long)edges);
-  DevBuf<unsigned long long> mask(std::max<uint64_t>(n, 1));
-  DevBuf<uint8_t> nlev(std::max<uint64_t>(n, 1));
-  mask.zero();
-  if (rows)
-    LB2_LAUNCH("hnsw_from_storage", storage_check_rows_kernel, cdiv(rows, 256), 256, 0, part_offsets, K, gb.p,
-               level_offsets, L, m, rows, vector_id, list_offsets, mask.p, err.p);
-  if (n) LB2_LAUNCH("hnsw_from_storage", storage_node_levels_kernel, cdiv(n, 256), 256, 0, mask.p, n, nlev.p, nup.p, err.p);
-  d2h(e, err.p, 2);
-  sync_stream();
-  report(e[0], e[1]);
-  scan_u64(nup.p, n, up.p);
-  uint64_t n_up = 0;
-  d2h(&n_up, up.p + n, 1);
-  sync_stream();
-  DevBuf<uint32_t> cnt0(std::max<uint64_t>(n, 1)), nbr0(std::max<uint64_t>(n * 2 * m, 1)),
-      cntu(std::max<uint64_t>(n_up, 1)), nbru(std::max<uint64_t>(n_up * m, 1));
-  DevBuf<float> dst0(std::max<uint64_t>(n * 2 * m, 1)), dstu(std::max<uint64_t>(n_up * m, 1));
-  cnt0.zero(); nbr0.zero(); dst0.zero(); cntu.zero(); nbru.zero(); dstu.zero();
-  if (rows)
-    LB2_LAUNCH("hnsw_from_storage", storage_edges_in_kernel, cdiv(rows * 32, 256), 256, 0, part_offsets, K, gb.p,
-               level_offsets, L, m, rows, vector_id, list_offsets, neighbors, distances, up.p, cnt0.p, nbr0.p, dst0.p,
-               cntu.p, nbru.p, dstu.p);
-  // the neighbour checks and the attachment are lb2_index_load_hnsw_*'s
-  hnsw_load(g, part_offsets, K, nlev.p, cnt0.p, nbr0.p, dst0.p, cntu.p, nbru.p, dstu.p);
 }
 
 }  // namespace lb2

@@ -6,6 +6,7 @@
 #include <vector>
 
 #include "common.cuh"
+struct lb2_index;
 namespace lb2 {
 struct IvfSearch;
 
@@ -16,7 +17,7 @@ struct IvfSearch;
 // Lists keep the reference's order of level_neighbors_ranked (graph/builder.rs:33-48); the distances are those of
 // the ranked list.  Node 0 of every partition has max_level levels and is the entry point (builder.rs:354-376).
 struct HnswGraph {
-  const char* kind = "IVF_HNSW_SQ";  // the index kind's name in messages: IVF_HNSW_SQ, IVF_HNSW_PQ or IVF_HNSW_FLAT
+  const char* kind = nullptr;  // the index kind's name in messages (hnsw_kind_name)
   int max_level = 0, m = 0, ef_construction = 0;
   uint32_t insert_batch = 1;  // B of the batched build (1: serial; a loaded graph records 1)
   uint64_t max_part = 0;      // rows of the largest partition (scratch sizing)
@@ -25,6 +26,29 @@ struct HnswGraph {
   DevBuf<uint32_t> up_base, cnt0, nbr0, cntu, nbru;
   DevBuf<float> dst0, dstu;
 };
+
+// the layout as the kernels see it
+struct GraphDev {
+  const uint8_t* nlev;
+  const uint32_t* up_base;
+  uint32_t *cnt0, *nbr0, *cntu, *nbru;
+  float *dst0, *dstu;
+  int m, max_level;
+};
+inline GraphDev dev_view(const HnswGraph& g) {
+  return GraphDev{g.nlev.p, g.up_base.p, g.cnt0.p, g.nbr0.p, g.cntu.p, g.nbru.p, g.dst0.p, g.dstu.p, g.m, g.max_level};
+}
+struct ListRef {
+  uint32_t* cnt;
+  uint32_t* ids;
+  float* dist;
+};
+// the list of global row `row` at `level`
+__device__ __forceinline__ ListRef list_of(const GraphDev& g, uint64_t row, int level) {
+  if (level == 0) return {g.cnt0 + row, g.nbr0 + row * 2 * g.m, g.dst0 + row * 2 * g.m};
+  const uint64_t r = (uint64_t)g.up_base[row] + (level - 1);
+  return {g.cntu + r, g.nbru + r * g.m, g.dstu + r * g.m};
+}
 
 // The level thresholds of random_level (builder.rs:386-393): node i >= 1 of a partition gets 1 + #{l in 1 ..
 // max_level - 1 : u < thr[l]} levels, u the u32 draw of hnsw_level_draw; thr[l] = floor(2^32 / m^l), so P(level >= l)
@@ -48,45 +72,18 @@ struct HnswKeep {
   std::vector<int64_t> src;       // [new K]: old partition id, or -1 = build this partition
 };
 
-// HNSW::index_vectors (builder.rs:742-775) of every partition, nodes inserted 1 .. n_p - 1 in ascending order, or in
-// rounds of up to g.insert_batch concurrent inserts when it is above 1 (the round definition of include/lance_b200.h);
-// codes [n][d] in partition order, part_offsets on the device.  Fills g (its parameters set by the caller).  With
-// `keep`, only the partitions keep->src marks -1 are built; the others are spliced from keep->old.
-void hnsw_build(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, int d, int metric, float r2,
-                uint64_t seed, const HnswKeep* keep = nullptr);
-// the same over PQ codes [n][cw] (cw = M, or M / 2 for 4-bit codes) with the codebook [M][2^nbits][d / M]: a node's
-// descent, beam searches and lists use the table of its decoded codes, the heuristic the decoded rows' distance with
-// the rule of `dtype` (pq/storage.rs:675-841)
-void hnsw_build_pq(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* codes, const float* codebook,
-                   int d, int M, int nbits, int metric, lb2_dtype dtype, uint64_t seed, const HnswKeep* keep = nullptr);
-// the same over IVF_FLAT's stored rows [n][d] in element type `vdt` (f32, f16 or bf16): every distance, cosine
-// included, is the IVF_FLAT scan's rule (flat/storage.rs:345-410)
-void hnsw_build_flat(HnswGraph& g, const uint64_t* part_offsets, int K, const void* vectors, int vdt, int d, int metric,
-                     uint64_t seed, const HnswKeep* keep = nullptr);
+// HNSW::index_vectors (builder.rs:742-775) of every partition of ix over its payload (codes or rows in partition
+// order), nodes inserted 1 .. n_p - 1 in ascending order, or in rounds of up to g.insert_batch concurrent inserts when
+// it is above 1 (the round definition of include/lance_b200.h), with the distances of ix's kind (hnsw.cu: SqDist,
+// PqDist, FlatDist).  Fills g (its parameters set by the caller).  With `keep`, only the partitions keep->src marks -1
+// are built; the others are spliced from keep->old.
+void hnsw_build(HnswGraph& g, const lb2_index& ix, uint64_t seed, const HnswKeep* keep = nullptr);
 // a graph from the caller's arrays in the layout above (host or device memory), checked against the partitions
 void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* levels, const uint32_t* counts0,
                const uint32_t* nbr0, const float* dist0, const uint32_t* counts_up, const uint32_t* nbr_up,
                const float* dist_up);
-// out[0] = 0, out[i + 1] = in[0] + .. + in[i] for i < n, on the device (out has n + 1 entries)
-void scan_u64(const uint64_t* in, uint64_t n, uint64_t* out);
-// The graphs in the reference's storage layout (HNSW::to_batch / HNSW::load, builder.rs:579-640,788-833), every
-// partition's level batches back to back (include/lance_b200.h, lb2_index_storage).  hnsw_storage_edges: the number
-// of list entries.  hnsw_to_storage: every output a device pointer or NULL; level_offsets [K][max_level + 1],
-// vector_id [rows], list_offsets [rows + 1] (global), neighbors / distances [edges], rows = n + g.n_up.
-uint64_t hnsw_storage_edges(const HnswGraph& g, uint64_t n);
-void hnsw_to_storage(const HnswGraph& g, const uint64_t* part_offsets, int K, uint64_t n, uint64_t* level_offsets,
-                     uint32_t* vector_id, uint64_t* list_offsets, uint32_t* neighbors, float* distances);
-// the inverse into g (max_level, m, ef_construction, kind set by the caller; device inputs): the storage checks on the
-// device, then hnsw_load of the dense layout.  LB2_INVALID_ARG on malformed input, before g is filled.
-void hnsw_from_storage(HnswGraph& g, const uint64_t* part_offsets, int K, uint64_t n, const uint32_t* entry_point,
-                       const uint64_t* level_offsets, const uint32_t* vector_id, const uint64_t* list_offsets,
-                       const uint32_t* neighbors, const float* distances, uint64_t rows, uint64_t edges);
-// HNSW::search (builder.rs:678-739) as the scan of every probed partition; ef = 0: k' + k' / 2 (builder.rs:563-573)
-void hnsw_search(const IvfSearch& s, const HnswGraph& g, const uint8_t* codes, float r2, const uint8_t* qcodes,
-                 uint32_t ef);
-// the same over PQ codes: each slot's table is the IVF_PQ scan's table of the (residual) query
-void hnsw_search_pq(const IvfSearch& s, const HnswGraph& g, const float* codebook, int M, int nbits,
-                    const uint8_t* codes, uint32_t ef);
-// the same over IVF_FLAT's stored rows: each slot scores rows with the IVF_FLAT scan's rule for the (normalised) query
-void hnsw_search_flat(const IvfSearch& s, const HnswGraph& g, const void* vectors, int vdt, uint32_t ef);
+// HNSW::search (builder.rs:678-739) as the scan of every probed partition, through ix's graphs with the distances of
+// ix's kind: the IVF_SQ scan's on sq_query_codes (s's queries encoded, IVF_HNSW_SQ only), the IVF_PQ scan's tables or
+// the IVF_FLAT scan's rule.  ef = 0: k' + k' / 2 (builder.rs:563-573)
+void hnsw_search(const IvfSearch& s, const lb2_index& ix, const uint8_t* sq_query_codes, uint32_t ef);
 }  // namespace lb2

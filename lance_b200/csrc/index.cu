@@ -1,6 +1,8 @@
 // index.cu -- the device-resident index: creation, loads and exports of every kind, the grouping of rows by
-// partition, search dispatch, incremental update and the partition exchange of a row-sharded index.
+// partition, the attachment of HNSW graphs, search dispatch, incremental update and the partition exchange of a
+// row-sharded index.
 #include <algorithm>
+#include <cstring>
 #include <memory>
 
 #include "build.cuh"
@@ -312,35 +314,32 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
   const IvfSearch s{index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->row_ids.p, qp, nq,
                     (int)kc, (int)nprobes, si, sd, sc, flt, pr};
   DevBuf<uint8_t> qcodes;
-  switch (index->kind) {
-    case IndexKind::FLAT:
-      if (index->hnsw)  // IVF_HNSW_FLAT: the IVF_FLAT scan's distances, searched through each partition's graph
-        hnsw_search_flat(s, *index->hnsw, index->vectors.p, (int)index->vdtype(), ef);
-      else
+  if (index->kind == IndexKind::SQ) {
+    // the (normalised) query is encoded with the index's bounds, not turned into a residual (sq/storage.rs:404-430)
+    qcodes.alloc(std::max<uint64_t>(1, nq * d));
+    sq_encode_f32(qp, nq * d, index->sq_lower, index->sq_upper, qcodes.p);
+  }
+  if (index->hnsw) {  // IVF_HNSW_*: the kind's scan distances, searched through each partition's graph
+    hnsw_search(s, *index, qcodes.p, ef);
+  } else {
+    switch (index->kind) {
+      case IndexKind::FLAT:
         ivfflat_search(s, index->vectors.p, (int)index->vdtype());
-      break;
-    case IndexKind::RQ:
-      // the (normalised) query's residual to each probed centroid is rotated (v2.rs:316-332, bq/storage.rs:407-445)
-      ivfrq_search(s, index->rq_rot.p, index->code_dim(), index->codes.p, index->rq_add.p, index->rq_scale.p);
-      break;
-    case IndexKind::SQ: {
-      // the (normalised) query is encoded with the index's bounds, not turned into a residual (sq/storage.rs:404-430)
-      qcodes.alloc(std::max<uint64_t>(1, nq * d));
-      sq_encode_f32(qp, nq * d, index->sq_lower, index->sq_upper, qcodes.p);
-      const float rf = (float)(index->sq_upper - index->sq_lower);  // inverse_scalar_dist (sq.rs:279-287)
-      if (index->hnsw)  // IVF_HNSW_SQ: the same query codes, searched through each partition's graph
-        hnsw_search(s, *index->hnsw, index->codes.p, rf * rf, qcodes.p, ef);
-      else
+        break;
+      case IndexKind::RQ:
+        // the (normalised) query's residual to each probed centroid is rotated (v2.rs:316-332, bq/storage.rs:407-445)
+        ivfrq_search(s, index->rq_rot.p, index->code_dim(), index->codes.p, index->rq_add.p, index->rq_scale.p);
+        break;
+      case IndexKind::SQ: {
+        const float rf = (float)(index->sq_upper - index->sq_lower);  // inverse_scalar_dist (sq.rs:279-287)
         ivfsq_search(s, index->codes.p, rf * rf, qcodes.p);
-      break;
-    }
-    case IndexKind::PQ:
-      if (index->hnsw)  // IVF_HNSW_PQ: the IVF_PQ scan's query tables, searched through each partition's graph
-        hnsw_search_pq(s, *index->hnsw, index->codebook.p, index->M, index->nbits, index->codes.p, ef);
-      else
+        break;
+      }
+      case IndexKind::PQ:
         ivfpq_search(s, index->codebook.p, index->M, index->nbits, index->codes.p, index->slab_off.p,
                      index->codes_skew.p);
-      break;
+        break;
+    }
   }
   if (refine) {
     // exact re-rank with the true metric on the ORIGINAL (un-normalised) query, as flat_knn does; the
@@ -489,27 +488,6 @@ static void row_mask_f32(const uint64_t* row_ids, uint64_t n, const uint64_t* al
              has_allow ? 1 : 0, block, n_block, has_block ? 1 : 0, reinterpret_cast<uint32_t*>(bitmap));
 }
 
-// row-major codes [n_p][cw] of the partitions off[0 .. K] -> the reference's storage layout, each partition
-// column-major [cw][n_p] (pq/storage.rs:430-450), or back (to_rows); `in` and `out` start at partition 0's first byte
-__global__ void transpose_codes_kernel(const uint8_t* __restrict__ in, const uint64_t* __restrict__ off, int K, int cw,
-                                       uint64_t total, int to_rows, uint8_t* __restrict__ out) {
-  for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (uint64_t)gridDim.x * blockDim.x) {
-    const uint64_t o0 = off[0], G = o0 * cw + g;
-    const int p = segment_of(off, K, G / cw);
-    const uint64_t o = off[p], n = off[p + 1] - o, l = G - o * cw;
-    const uint64_t row = (o - o0 + l % n) * cw + l / n;
-    if (to_rows) out[row] = in[g];
-    else out[g] = in[row];
-  }
-}
-static void transpose_codes(const uint8_t* in, const uint64_t* off, int K, int cw, uint64_t rows, bool to_rows,
-                            uint8_t* out) {
-  const uint64_t total = rows * cw;
-  if (total)
-    LB2_LAUNCH("transpose_codes", transpose_codes_kernel, (unsigned)std::min<uint64_t>(cdiv(total, 256), 64ull * ctx().num_sms),
-               256, 0, in, off, K, cw, total, to_rows ? 1 : 0, out);
-}
-
 // the kept graphs of a merge (lb2_optimize_params' rule): new partition p keeps old partition q's graph when q lost no
 // row, nothing was added to p, and p holds exactly q's rows (then no other old partition sent p a row)
 static HnswKeep kept_partitions(const lb2_index* old, const lb2_index* ix, const uint32_t* part_map,
@@ -632,33 +610,8 @@ std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_optimize_
   if (old->hnsw) {
     const HnswGraph& og = *old->hnsw;
     const HnswKeep keep = kept_partitions(old, ix.get(), pm.get(), dropped.p, added.p);
-    ix->hnsw.reset(new HnswGraph());
-    HnswGraph& g = *ix->hnsw;
-    g.kind = og.kind;
-    g.max_level = og.max_level;
-    g.m = og.m;
-    g.ef_construction = og.ef_construction;
-    g.insert_batch = p.insert_batch ? p.insert_batch : og.insert_batch;
-    TagScope tg("hnsw_build");
-    switch (ix->kind) {
-      case IndexKind::SQ: {
-        const float rf = (float)(ix->sq_upper - ix->sq_lower);
-        hnsw_build(g, ix->part_offsets.p, ix->K, ix->codes.p, ix->d, ix->metric, rf * rf, p.seed, &keep);
-        break;
-      }
-      case IndexKind::PQ:
-        ix->slab_off.release();  // the skewed code copy serves only the IVF_PQ scan
-        ix->codes_skew.release();
-        hnsw_build_pq(g, ix->part_offsets.p, ix->K, ix->codes.p, ix->codebook.p, ix->d, ix->M, ix->nbits, ix->metric,
-                      ix->dtype, p.seed, &keep);
-        break;
-      case IndexKind::FLAT:
-        hnsw_build_flat(g, ix->part_offsets.p, ix->K, ix->vectors.p, (int)ix->vdtype(), ix->d, ix->metric, p.seed,
-                        &keep);
-        break;
-      case IndexKind::RQ:  // no IVF_RQ index has a graph
-        break;
-    }
+    attach_graph(ix.get(), og.max_level, og.m, og.ef_construction, p.insert_batch ? p.insert_batch : og.insert_batch,
+                 p.seed, &keep);
   }
   sync_stream();
   return ix;
@@ -809,27 +762,51 @@ lb2_status lb2_index_export_sq(const lb2_index* index, void* centroids_out, doub
 
 }  // extern "C"
 
-// lb2_index_load_hnsw_sq / _pq / _flat: a graph over the rows of an index of `kind`
-static void load_hnsw(lb2_index* index, IndexKind kind, const char* name, uint32_t max_level, uint32_t m,
-                      uint32_t ef_construction, const uint8_t* levels, const uint32_t* counts0,
-                      const uint32_t* neighbors0, const float* dists0, const uint32_t* counts_up,
-                      const uint32_t* neighbors_up, const float* dists_up) {
-  LB2_REQUIRE(index && index->kind == kind, "not an %s index",
-              kind == IndexKind::SQ ? "IVF_SQ" : kind == IndexKind::PQ ? "IVF_PQ" : "IVF_FLAT");
-  LB2_REQUIRE(max_level >= 1 && max_level <= 64 && m >= 1 && m <= 1024, "%s: max_level %u or m %u out of range", name,
-              max_level, m);
+namespace lb2 {
+
+const char* hnsw_kind_name(IndexKind kind) {
+  return kind == IndexKind::SQ ? "IVF_HNSW_SQ" : kind == IndexKind::PQ ? "IVF_HNSW_PQ" : "IVF_HNSW_FLAT";
+}
+
+std::unique_ptr<HnswGraph> new_graph(IndexKind kind, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                                     uint32_t insert_batch) {
+  LB2_REQUIRE(max_level >= 1 && max_level <= 64 && m >= 1 && m <= 1024, "%s: max_level %u or m %u out of range",
+              hnsw_kind_name(kind), max_level, m);
   std::unique_ptr<HnswGraph> g(new HnswGraph());
-  g->kind = name;
+  g->kind = hnsw_kind_name(kind);
   g->max_level = (int)max_level;
   g->m = (int)m;
   g->ef_construction = (int)ef_construction;
+  g->insert_batch = std::max<uint32_t>(insert_batch, 1);
+  return g;
+}
+
+void attach_graph(lb2_index* ix, uint32_t max_level, uint32_t m, uint32_t ef_construction, uint32_t insert_batch,
+                  uint64_t seed, const HnswKeep* keep) {
+  TagScope tg("hnsw_build");
+  std::unique_ptr<HnswGraph> g = new_graph(ix->kind, max_level, m, ef_construction, insert_batch);
+  ix->slab_off.release();  // the skewed code copy serves only the IVF_PQ scan
+  ix->codes_skew.release();
+  hnsw_build(*g, *ix, seed, keep);
+  ix->hnsw = std::move(g);
+}
+
+}  // namespace lb2
+
+// lb2_index_load_hnsw_sq / _pq / _flat: a graph over the rows of an index of `kind`
+static void load_hnsw(lb2_index* index, IndexKind kind, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                      const uint8_t* levels, const uint32_t* counts0, const uint32_t* neighbors0, const float* dists0,
+                      const uint32_t* counts_up, const uint32_t* neighbors_up, const float* dists_up) {
+  // the refusal names the index kind, IVF_SQ, IVF_PQ or IVF_FLAT: the graph kind's name past "IVF_HNSW_"
+  LB2_REQUIRE(index && index->kind == kind, "not an IVF_%s index", hnsw_kind_name(kind) + strlen("IVF_HNSW_"));
+  std::unique_ptr<HnswGraph> g = new_graph(kind, max_level, m, ef_construction);
   hnsw_load(*g, index->part_offsets.p, index->K, levels, counts0, neighbors0, dists0, counts_up, neighbors_up, dists_up);
   index->hnsw = std::move(g);
 }
 
-// lb2_index_hnsw_sq_info / _pq_info: the graph of an index of `kind`
-static const HnswGraph& graph_of(const lb2_index* index, IndexKind kind, const char* name) {
-  LB2_REQUIRE(index && index->hnsw && index->kind == kind, "not an %s index", name);
+// lb2_index_hnsw_*_info / lb2_index_export_hnsw_*: the graph of an index of `kind`
+static const HnswGraph& graph_of(const lb2_index* index, IndexKind kind) {
+  LB2_REQUIRE(index && index->hnsw && index->kind == kind, "not an %s index", hnsw_kind_name(kind));
   return *index->hnsw;
 }
 static void hnsw_info(const HnswGraph& g, uint32_t* max_level, uint32_t* m, uint32_t* ef_construction,
@@ -864,7 +841,7 @@ lb2_status lb2_index_load_hnsw_sq(lb2_index* index, uint32_t max_level, uint32_t
                                   const float* dists0, const uint32_t* counts_up, const uint32_t* neighbors_up,
                                   const float* dists_up) {
   LB2_API_BEGIN
-  load_hnsw(index, IndexKind::SQ, "IVF_HNSW_SQ", max_level, m, ef_construction, levels, counts0, neighbors0, dists0,
+  load_hnsw(index, IndexKind::SQ, max_level, m, ef_construction, levels, counts0, neighbors0, dists0,
             counts_up, neighbors_up, dists_up);
   LB2_API_END
 }
@@ -874,7 +851,7 @@ lb2_status lb2_index_load_hnsw_pq(lb2_index* index, uint32_t max_level, uint32_t
                                   const float* dists0, const uint32_t* counts_up, const uint32_t* neighbors_up,
                                   const float* dists_up) {
   LB2_API_BEGIN
-  load_hnsw(index, IndexKind::PQ, "IVF_HNSW_PQ", max_level, m, ef_construction, levels, counts0, neighbors0, dists0,
+  load_hnsw(index, IndexKind::PQ, max_level, m, ef_construction, levels, counts0, neighbors0, dists0,
             counts_up, neighbors_up, dists_up);
   LB2_API_END
 }
@@ -884,7 +861,7 @@ lb2_status lb2_index_load_hnsw_flat(lb2_index* index, uint32_t max_level, uint32
                                     const float* dists0, const uint32_t* counts_up, const uint32_t* neighbors_up,
                                     const float* dists_up) {
   LB2_API_BEGIN
-  load_hnsw(index, IndexKind::FLAT, "IVF_HNSW_FLAT", max_level, m, ef_construction, levels, counts0, neighbors0,
+  load_hnsw(index, IndexKind::FLAT, max_level, m, ef_construction, levels, counts0, neighbors0,
             dists0, counts_up, neighbors_up, dists_up);
   LB2_API_END
 }
@@ -892,21 +869,21 @@ lb2_status lb2_index_load_hnsw_flat(lb2_index* index, uint32_t max_level, uint32
 lb2_status lb2_index_hnsw_sq_info(const lb2_index* index, uint32_t* max_level, uint32_t* m, uint32_t* ef_construction,
                                   uint64_t* num_upper_rows) {
   LB2_API_BEGIN
-  hnsw_info(graph_of(index, IndexKind::SQ, "IVF_HNSW_SQ"), max_level, m, ef_construction, num_upper_rows);
+  hnsw_info(graph_of(index, IndexKind::SQ), max_level, m, ef_construction, num_upper_rows);
   LB2_API_END
 }
 
 lb2_status lb2_index_hnsw_pq_info(const lb2_index* index, uint32_t* max_level, uint32_t* m, uint32_t* ef_construction,
                                   uint64_t* num_upper_rows) {
   LB2_API_BEGIN
-  hnsw_info(graph_of(index, IndexKind::PQ, "IVF_HNSW_PQ"), max_level, m, ef_construction, num_upper_rows);
+  hnsw_info(graph_of(index, IndexKind::PQ), max_level, m, ef_construction, num_upper_rows);
   LB2_API_END
 }
 
 lb2_status lb2_index_hnsw_flat_info(const lb2_index* index, uint32_t* max_level, uint32_t* m,
                                     uint32_t* ef_construction, uint64_t* num_upper_rows) {
   LB2_API_BEGIN
-  hnsw_info(graph_of(index, IndexKind::FLAT, "IVF_HNSW_FLAT"), max_level, m, ef_construction, num_upper_rows);
+  hnsw_info(graph_of(index, IndexKind::FLAT), max_level, m, ef_construction, num_upper_rows);
   LB2_API_END
 }
 
@@ -914,7 +891,7 @@ lb2_status lb2_index_export_hnsw_sq(const lb2_index* index, uint8_t* levels_out,
                                     uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
                                     uint32_t* neighbors_up_out, float* dists_up_out) {
   LB2_API_BEGIN
-  export_hnsw(index, graph_of(index, IndexKind::SQ, "IVF_HNSW_SQ"), levels_out, counts0_out, neighbors0_out,
+  export_hnsw(index, graph_of(index, IndexKind::SQ), levels_out, counts0_out, neighbors0_out,
               dists0_out, counts_up_out, neighbors_up_out, dists_up_out);
   LB2_API_END
 }
@@ -923,7 +900,7 @@ lb2_status lb2_index_export_hnsw_pq(const lb2_index* index, uint8_t* levels_out,
                                     uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
                                     uint32_t* neighbors_up_out, float* dists_up_out) {
   LB2_API_BEGIN
-  export_hnsw(index, graph_of(index, IndexKind::PQ, "IVF_HNSW_PQ"), levels_out, counts0_out, neighbors0_out,
+  export_hnsw(index, graph_of(index, IndexKind::PQ), levels_out, counts0_out, neighbors0_out,
               dists0_out, counts_up_out, neighbors_up_out, dists_up_out);
   LB2_API_END
 }
@@ -932,7 +909,7 @@ lb2_status lb2_index_export_hnsw_flat(const lb2_index* index, uint8_t* levels_ou
                                       uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
                                       uint32_t* neighbors_up_out, float* dists_up_out) {
   LB2_API_BEGIN
-  export_hnsw(index, graph_of(index, IndexKind::FLAT, "IVF_HNSW_FLAT"), levels_out, counts0_out, neighbors0_out,
+  export_hnsw(index, graph_of(index, IndexKind::FLAT), levels_out, counts0_out, neighbors0_out,
               dists0_out, counts_up_out, neighbors_up_out, dists_up_out);
   LB2_API_END
 }
@@ -950,190 +927,6 @@ lb2_status lb2_index_export_rq(const lb2_index* index, void* centroids_out, void
   if (add_out && n) LB2_CUDA(cudaMemcpyAsync(add_out, index->rq_add.p, sizeof(float) * n, cudaMemcpyDefault, s));
   if (scale_out && n) LB2_CUDA(cudaMemcpyAsync(scale_out, index->rq_scale.p, sizeof(float) * n, cudaMemcpyDefault, s));
   sync_stream();
-  LB2_API_END
-}
-
-lb2_status lb2_index_export_partition(const lb2_index* index, uint32_t partition, uint8_t* codes_transposed_out,
-                                      uint64_t* row_ids_out, uint64_t* num_rows_out) {
-  LB2_API_BEGIN
-  LB2_REQUIRE(index && index->kind == IndexKind::PQ, "not an IVF_PQ index");
-  LB2_REQUIRE(partition < (uint32_t)index->K, "partition %u out of range (the index has %d)", partition, index->K);
-  uint64_t off[2];
-  d2h(off, index->part_offsets.p + partition, 2);
-  sync_stream();
-  const uint64_t np = off[1] - off[0];
-  const int cw = (int)index->row_bytes();
-  if (num_rows_out) *num_rows_out = np;
-  if (np && codes_transposed_out) {
-    OutArg<uint8_t> o(codes_transposed_out, (size_t)np * cw);
-    transpose_codes(index->codes.p + off[0] * cw, index->part_offsets.p + partition, 1, cw, np, false, o.get());
-    o.commit();
-  }
-  if (np && row_ids_out)
-    LB2_CUDA(cudaMemcpyAsync(row_ids_out, index->row_ids.p + off[0], sizeof(uint64_t) * np, cudaMemcpyDefault, ctx().stream));
-  sync_stream();
-  LB2_API_END
-}
-
-}  // extern "C"
-
-__global__ void part_lengths_kernel(const uint64_t* __restrict__ off, int K, uint64_t* __restrict__ len) {
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p < K) len[p] = off[p + 1] - off[p];
-}
-// a length above n would let the u64 sum of the lengths wrap to n with offsets that are not ascending
-__global__ void lengths_above_kernel(const uint64_t* __restrict__ len, int K, uint64_t n, uint32_t* __restrict__ bad) {
-  const int p = blockIdx.x * blockDim.x + threadIdx.x;
-  if (p < K && len[p] > n) atomicMax(bad, (uint32_t)p + 1);
-}
-__global__ void part_ids_kernel(const uint64_t* __restrict__ off, int K, uint64_t n, uint32_t* __restrict__ part) {
-  const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r < n) part[r] = (uint32_t)segment_of(off, K, r);
-}
-
-static const char* graph_kind_name(IndexKind kind) {
-  return kind == IndexKind::SQ ? "IVF_HNSW_SQ" : kind == IndexKind::PQ ? "IVF_HNSW_PQ" : "IVF_HNSW_FLAT";
-}
-// u8 IVF_FLAT rows are held as f32; the reference's u8 flat storage is the Hamming one (include/lance_b200.h)
-static void storage_kind_check(const lb2_index* index, const char* what) {
-  LB2_REQUIRE(!(index->kind == IndexKind::FLAT && index->dtype == LB2_U8),
-              "%s: an IVF_FLAT index over u8 rows has no storage layout (the reference stores u8 columns only in its "
-              "binary Hamming storage)", what);
-}
-
-extern "C" {
-
-lb2_status lb2_index_export_storage(const lb2_index* index, lb2_index_storage* out) {
-  LB2_API_BEGIN
-  LB2_REQUIRE(index && out, "null argument");
-  storage_kind_check(index, "index_export_storage");
-  const uint64_t n = index->n;
-  const int K = index->K;
-  const size_t rb = index->row_bytes();
-  const HnswGraph* g = index->hnsw.get();
-  out->num_partitions = (uint32_t)K;
-  out->num_rows = n;
-  out->num_bytes = n * rb;
-  out->max_level = g ? (uint32_t)g->max_level : 0;
-  out->m = g ? (uint32_t)g->m : 0;
-  out->ef_construction = g ? (uint32_t)g->ef_construction : 0;
-  out->num_graph_rows = g ? n + g->n_up : 0;
-  out->num_edges = g ? hnsw_storage_edges(*g, n) : 0;
-  cudaStream_t s = ctx().stream;
-  const uint64_t* off = index->part_offsets.p;
-  OutArg<uint64_t> len(out->part_lengths, K);
-  if (len.get()) LB2_LAUNCH("storage_export", part_lengths_kernel, cdiv(K, 256), 256, 0, off, K, len.get());
-  len.commit();
-  if (out->row_ids && n)
-    LB2_CUDA(cudaMemcpyAsync(out->row_ids, index->row_ids.p, sizeof(uint64_t) * n, cudaMemcpyDefault, s));
-  OutArg<uint8_t> pay(out->payload, n * rb);
-  if (pay.get()) {
-    if (index->kind == IndexKind::PQ) transpose_codes(index->codes.p, off, K, (int)rb, n, false, pay.get());
-    else if (index->kind == IndexKind::RQ) rq_pack(index->codes.p, off, K, n, (int)rb, pay.get(), false);
-    else d2d(pay.get(), index->payload().p, n * rb);
-  }
-  pay.commit();
-  if (index->kind == IndexKind::RQ && n) {
-    if (out->add_factors)
-      LB2_CUDA(cudaMemcpyAsync(out->add_factors, index->rq_add.p, sizeof(float) * n, cudaMemcpyDefault, s));
-    if (out->scale_factors)
-      LB2_CUDA(cudaMemcpyAsync(out->scale_factors, index->rq_scale.p, sizeof(float) * n, cudaMemcpyDefault, s));
-  }
-  if (g) {
-    const uint64_t rows = out->num_graph_rows, e = out->num_edges;
-    OutArg<uint32_t> ep(out->entry_point, K);
-    if (ep.get()) LB2_CUDA(cudaMemsetAsync(ep.get(), 0, sizeof(uint32_t) * K, s));
-    ep.commit();
-    OutArg<uint64_t> lo(out->level_offsets, (size_t)K * (g->max_level + 1)), lof(out->list_offsets, rows + 1);
-    OutArg<uint32_t> vid(out->vector_id, rows), nbr(out->neighbors, e);
-    OutArg<float> dst(out->distances, e);
-    if (lo.get() || vid.get() || lof.get() || nbr.get() || dst.get())
-      hnsw_to_storage(*g, off, K, n, lo.get(), vid.get(), lof.get(), nbr.get(), dst.get());
-    lo.commit(); lof.commit(); vid.commit(); nbr.commit(); dst.commit();
-    sync_stream();
-  }
-  sync_stream();
-  LB2_API_END
-}
-
-lb2_status lb2_index_load_storage(lb2_index* index, const lb2_index_storage* st) {
-  LB2_API_BEGIN
-  LB2_REQUIRE(index && st, "null argument");
-  storage_kind_check(index, "index_load_storage");
-  const int K = index->K;
-  const uint64_t n = st->num_rows;
-  const size_t rb = index->row_bytes();
-  const bool rq = index->kind == IndexKind::RQ;
-  LB2_REQUIRE(st->num_partitions == (uint32_t)K, "index_load_storage: %u partitions, the index has %d",
-              st->num_partitions, K);
-  LB2_REQUIRE(n < 0xffffffffull, "more than 2^32-1 rows per index shard");
-  LB2_REQUIRE(st->num_bytes == n * rb, "index_load_storage: %llu payload bytes, %llu rows of %zu bytes need %llu",
-              (unsigned long long)st->num_bytes, (unsigned long long)n, rb, (unsigned long long)(n * rb));
-  LB2_REQUIRE(st->part_lengths && (n == 0 || (st->payload && st->row_ids)), "null argument");
-  LB2_REQUIRE(rq ? n == 0 || (st->add_factors && st->scale_factors) : !st->add_factors && !st->scale_factors,
-              "index_load_storage: add / scale factors are IVF_RQ's columns, required there and only there");
-  LB2_REQUIRE(st->max_level == 0 || !rq, "index_load_storage: IVF_RQ has no graph");
-  if (index->kind == IndexKind::FLAT)
-    LB2_REQUIRE(index->d % 4 == 0, "IVF_FLAT needs a dimension that is a multiple of 4");
-  InArg<uint64_t> len(st->part_lengths, K);
-  std::unique_ptr<lb2_index> ix = make_index(index->kind, K, index->d, index->metric, index->dtype);
-  copy_model(index, ix.get());
-  DevBuf<uint64_t> off(K + 1);
-  DevBuf<uint32_t> bad(1);
-  bad.zero();
-  LB2_LAUNCH("storage_load", lengths_above_kernel, cdiv(K, 256), 256, 0, len.get(), K, n, bad.p);
-  scan_u64(len.get(), K, off.p);
-  uint64_t total = 0;
-  uint32_t above = 0;
-  d2h(&total, off.p + K, 1);
-  d2h(&above, bad.p, 1);
-  sync_stream();
-  LB2_REQUIRE(above == 0, "index_load_storage: part_lengths[%u] is above num_rows %llu", above - 1,
-              (unsigned long long)n);
-  LB2_REQUIRE(total == n, "index_load_storage: part_lengths sum to %llu, num_rows is %llu", (unsigned long long)total,
-              (unsigned long long)n);
-  // the rows in partition order with their partition ids: the loads' own grouping keeps that order
-  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
-  if (n) LB2_LAUNCH("storage_load", part_ids_kernel, cdiv(n, 256), 256, 0, off.p, K, n, part.p);
-  InArg<uint64_t> rid(st->row_ids, n);
-  if (index->kind == IndexKind::FLAT) {
-    Source src(st->payload, n, index->d, index->dtype);
-    src.start_resident_copy();
-    index_load_flat_src(ix.get(), part.p, src, rid.get(), nullptr, /*normalize=*/false);
-  } else {
-    InArg<uint8_t> pay(st->payload, n * rb);
-    InArg<float> a(st->add_factors, n), sc(st->scale_factors, n);
-    DevBuf<uint8_t> rows;
-    const uint8_t* codes = pay.get();
-    if (index->kind != IndexKind::SQ && n) {
-      rows.alloc(n * rb);
-      if (rq) rq_pack(pay.get(), off.p, K, n, (int)rb, rows.p, true);
-      else transpose_codes(pay.get(), off.p, K, (int)rb, n, true, rows.p);
-      codes = rows.p;
-    }
-    index_load_dev(ix.get(), part.p, codes, rid.get(), n, nullptr, a.get(), sc.get());
-  }
-  if (st->max_level) {
-    const uint64_t rows = st->num_graph_rows, e = st->num_edges;
-    LB2_REQUIRE(st->max_level <= 64 && st->m >= 1 && st->m <= 1024, "%s: max_level %u or m %u out of range",
-                graph_kind_name(index->kind), st->max_level, st->m);
-    LB2_REQUIRE(st->entry_point && st->level_offsets && st->list_offsets && (rows == 0 || st->vector_id) &&
-                    (e == 0 || (st->neighbors && st->distances)),
-                "null argument");
-    std::unique_ptr<HnswGraph> g(new HnswGraph());
-    g->kind = graph_kind_name(index->kind);
-    g->max_level = (int)st->max_level;
-    g->m = (int)st->m;
-    g->ef_construction = (int)st->ef_construction;
-    InArg<uint32_t> ep(st->entry_point, K), vid(st->vector_id, rows), nbr(st->neighbors, e);
-    InArg<uint64_t> lo(st->level_offsets, (size_t)K * (st->max_level + 1)), lof(st->list_offsets, rows + 1);
-    InArg<float> dst(st->distances, e);
-    hnsw_from_storage(*g, ix->part_offsets.p, K, n, ep.get(), lo.get(), vid.get(), lof.get(), nbr.get(), dst.get(),
-                      rows, e);
-    ix->hnsw = std::move(g);
-  }
-  sync_stream();
-  *index = std::move(*ix);
   LB2_API_END
 }
 

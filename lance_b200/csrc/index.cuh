@@ -70,6 +70,16 @@ void index_load_flat_src(lb2_index* ix, const uint32_t* part_ids, Source& src, c
 // the model of `from` in `to`, an index of the same kind from make_index: the centroids (or new_centroids, in the
 // model type of the index), M, nbits, and the codebook, SQ bounds or RQ rotation
 void copy_model(const lb2_index* from, lb2_index* to, const void* new_centroids = nullptr);
+// the name of the graph kind over an index of `kind` in messages: IVF_HNSW_SQ, IVF_HNSW_PQ or IVF_HNSW_FLAT
+const char* hnsw_kind_name(IndexKind kind);
+// an empty graph of these parameters (hnsw/builder.rs:63-72; max_level and m range-checked) over an index of `kind`;
+// insert_batch 0 or 1 is the serial build, and what a loaded graph records
+std::unique_ptr<HnswGraph> new_graph(IndexKind kind, uint32_t max_level, uint32_t m, uint32_t ef_construction,
+                                     uint32_t insert_batch = 1);
+// the graphs of ix built (hnsw_build, under the hnsw_build tag; `keep`: the partitions spliced from an older graph)
+// and attached; an IVF_PQ index's skewed code copy is released, as only the IVF_PQ scan reads it
+void attach_graph(lb2_index* ix, uint32_t max_level, uint32_t m, uint32_t ef_construction, uint32_t insert_batch,
+                  uint64_t seed, const HnswKeep* keep = nullptr);
 // lb2_index_optimize's merge into a new index; add_valid (nullable, device [n_add]): added rows with 0 are left out
 std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_optimize_params& p, const char* what,
                                        const uint8_t* add_valid = nullptr);

@@ -5,7 +5,6 @@
 //           codes_res_dot_dists                  bq/builder.rs:100-141 (the per-row |rot| sum)
 //           RQTransformer::transform             bq/transform.rs:70-220 (add / scale factors)
 //           RabitDistCalculator                  bq/storage.rs:160-445 (the partition scan of a search)
-//           pack_codes / unpack_codes            bq/storage.rs:477-601 (the stored `__rabit_code` layout)
 //
 // Exactness: the reference rotates data rows with an ndarray GEMM whose summation order is unspecified.  Here the
 // rotation of a row is defined as the query side's rotation, the 16-lane f32 `dot` (dot.rs:30-58, the order of
@@ -445,66 +444,6 @@ void ivfrq_search(const IvfSearch& s, const float* rotation, int code_dim, const
                  sl.cand_d + a * np * k, sl.cand_id + a * np * k, sl.cand_cnt + a * np, s.flt);
     }
   });
-}
-
-// pack_codes / unpack_codes (bq/storage.rs:477-601), restarted at every partition.  Byte g of the packed column
-// belongs to the partition of row g / cl (a partition's packed bytes are its own rows' bytes); inside it, with nb
-// full 32-row blocks, byte b * 32 * cl + i * 32 + j (j < 16) holds the low nibbles of byte i of rows 32b + PERM0[j]
-// (bits 0..3) and 32b + PERM0[j] + 16 (bits 4..7), byte j + 16 their high nibbles; the n_p % 32 tail rows follow
-// column-major [cl][tail].  PERM0[j] = j / 2 + (j % 2) * 8 (lance-linalg/src/simd/dist_table.rs:10).
-// One thread per output byte: every byte is written once and read from at most two input bytes.
-__global__ void rq_pack_kernel(const uint8_t* __restrict__ codes, const uint64_t* __restrict__ off, int K, int cl,
-                               uint64_t total, uint8_t* __restrict__ packed) {
-  for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (uint64_t)gridDim.x * blockDim.x) {
-    const int p = segment_of(off, K, g / cl);
-    const uint64_t o = off[p], np = off[p + 1] - o, full = np / 32 * 32;
-    const uint64_t l = g - o * cl;  // byte within the partition
-    const uint8_t* c = codes + o * cl;
-    uint8_t v;
-    if (l < full * cl) {
-      const uint64_t b = l / (32ull * cl);
-      const int i = (int)(l / 32 % cl), j = (int)(l % 32), jj = j & 15;
-      const uint64_t r0 = b * 32 + (jj >> 1) + (jj & 1) * 8;  // PERM0[jj]
-      const int sh = j < 16 ? 0 : 4;
-      v = (uint8_t)(((c[r0 * cl + i] >> sh) & 0xF) | (((c[(r0 + 16) * cl + i] >> sh) & 0xF) << 4));
-    } else {
-      const uint64_t t = l - full * cl, rem = np - full;
-      v = c[(full + t % rem) * cl + t / rem];
-    }
-    packed[g] = v;
-  }
-}
-
-// the inverse: byte g of the row-major codes from the packed column
-__global__ void rq_unpack_kernel(const uint8_t* __restrict__ packed, const uint64_t* __restrict__ off, int K, int cl,
-                                 uint64_t total, uint8_t* __restrict__ codes) {
-  for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < total; g += (uint64_t)gridDim.x * blockDim.x) {
-    const uint64_t row = g / cl;
-    const int i = (int)(g % cl);
-    const int p = segment_of(off, K, row);
-    const uint64_t o = off[p], np = off[p + 1] - o, full = np / 32 * 32, r = row - o;
-    const uint8_t* c = packed + o * cl;
-    uint8_t v;
-    if (r < full) {
-      const uint64_t base = r / 32 * 32 * cl + (uint64_t)i * 32;
-      const int t = (int)(r % 32), h = t >> 4, u = t & 15;
-      const int j = (u & 7) * 2 + (u >> 3);  // PERM0[j] == u
-      const int sh = h ? 4 : 0;
-      v = (uint8_t)(((c[base + j] >> sh) & 0xF) | (((c[base + j + 16] >> sh) & 0xF) << 4));
-    } else {
-      const uint64_t rem = np - full;
-      v = c[full * cl + (uint64_t)i * rem + (r - full)];
-    }
-    codes[g] = v;
-  }
-}
-
-void rq_pack(const uint8_t* codes, const uint64_t* part_offsets, int K, uint64_t n, int cl, uint8_t* packed, bool unpack) {
-  const uint64_t total = n * cl;
-  if (!total) return;
-  const unsigned grid = (unsigned)std::min<uint64_t>(cdiv(total, 256), 64ull * ctx().num_sms);
-  if (unpack) LB2_LAUNCH("rq_unpack", rq_unpack_kernel, grid, 256, 0, codes, part_offsets, K, cl, total, packed);
-  else LB2_LAUNCH("rq_pack", rq_pack_kernel, grid, 256, 0, codes, part_offsets, K, cl, total, packed);
 }
 
 }  // namespace lb2

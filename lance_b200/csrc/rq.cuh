@@ -19,9 +19,6 @@ void rq_norm_sq_f32(const float* x, uint64_t m, int d, float* out);
 void rq_encode_f32(const float* rot, const float* residual, const float* dist_v_c, const uint32_t* part,
                    const float* cnorm_sq, const uint8_t* valid, uint64_t m, int d, int num_bits, int metric,
                    uint8_t* codes, float* add, float* scale);
-// pack_codes (unpack = false) or unpack_codes (unpack = true) of every partition of the part_offsets [K + 1] (device)
-// at once: n rows of cl = code_dim / 8 bytes, `in` and `out` in partition order (bq/storage.rs:477-601)
-void rq_pack(const uint8_t* in, const uint64_t* part_offsets, int K, uint64_t n, int cl, uint8_t* out, bool unpack);
 // IVF_RQ: rotation [code_dim][code_dim]; codes [n][code_dim / 8] and the add / scale factors [n] in partition order;
 // s.queries: f32 (normalised for cosine).  rq_scan_fits: the scan's tables and a k-slot fit shared memory.
 struct IvfSearch;
