@@ -109,6 +109,12 @@ typedef struct {
   uint64_t seed;           /* the reference is unseeded (kmeans.rs:645); we are reproducible */
   const void* init_centroids; /* KMeanInit::Incremental (k x d, same dtype) or NULL = random rows */
   lb2_metric metric;       /* L2 or DOT (cosine callers normalise first, as the reference does) */
+  uint32_t partition_index;       /* lb2_partition_index_mode of a build's full pass (below): EXACT (the default),
+                                     AUTO or HNSW.  A build whose mode resolves to the graph assigns every row
+                                     through lb2_partition_index_* over its trained centroids, and the index keeps
+                                     the rule (lb2_index_set_partition_index).  lb2_kmeans_train refuses any other
+                                     value than EXACT with LB2_INVALID_ARG: training never uses the graph. */
+  uint32_t partition_index_batch; /* the graph's insert_batch: 0 or 1 serial (the default), B >= 2 in rounds */
 } lb2_kmeans_params;
 void lb2_kmeans_params_default(lb2_kmeans_params* p);
 
@@ -134,6 +140,77 @@ lb2_status lb2_find_partitions(const void* centroids, uint32_t k, uint32_t d, lb
 lb2_status lb2_compute_residual(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype,
                                 const void* vectors, uint64_t n, const uint32_t* part_ids,
                                 void* out);
+
+/* ---- partition index: an HNSW graph over the centroids (lance-index/src/vector/utils.rs:26-108) --------------------
+ * PartitionTransformer::new (ivf/transform.rs:48-68) asks SimpleIndex::may_train_index for a graph over the centroids,
+ * and transform (:112-124) then assigns each row by one graph search instead of the exact scan.  The modes are the
+ * values of LANCE_USE_HNSW_SPEEDUP_INDEXING (utils.rs:26-44): EXACT = "disabled", AUTO = unset (or any other value),
+ * HNSW = "enabled".  EXACT is this library's default everywhere. */
+typedef enum {
+  LB2_PARTITION_INDEX_EXACT = 0, /* never the graph */
+  LB2_PARTITION_INDEX_AUTO = 1,  /* the graph when k * d >= 1 000 000 (centroids.len() of the flat values array) */
+  LB2_PARTITION_INDEX_HNSW = 2   /* always the graph */
+} lb2_partition_index_mode;
+typedef struct lb2_partition_index lb2_partition_index;
+/* may_train_index's decision (utils.rs:67-91), on the host only: *uses_graph_out = 1 when `mode` resolves to the
+ * graph for a k x d model whose columns have element type `dtype`.  Only an f32 model has a graph (utils.rs:83-90);
+ * u8 columns have f32 models and follow f32, f16 / bf16 models are always exact. */
+lb2_status lb2_partition_index_uses_graph(uint64_t k, uint32_t d, lb2_dtype dtype, lb2_partition_index_mode mode,
+                                          int* uses_graph_out);
+/* SimpleIndex::try_new (utils.rs:53-59): HNSW::index_vectors (hnsw/builder.rs:742-775) over FlatFloatStorage of the
+ * k centroids (f32, [k][d]; node i is centroid i) under L2 or dot, with HnswBuildParams::default() (max_level 7),
+ * ef_construction 15 and m 12.  *out = NULL whenever the mode resolves to the exact scan, as may_train_index returns
+ * None.  The graph is IVF_HNSW_FLAT's graph of one partition holding the centroids, bit for bit: its distances are
+ * the f32 16-lane rule (below), the level of node i >= 1 comes from the counter-based draw of (seed, partition 0,
+ * node i) (the reference's rayon build and unseeded levels are not reproducible), and insert_batch B >= 2 builds in
+ * IVF_HNSW_SQ's deterministic rounds (0 or 1: the serial build).  Cosine -> LB2_INVALID_ARG (the IVF transformer
+ * normalises first and assigns under L2, ivf.rs:149-166: normalise and pass L2); d % 4 != 0 or a communicator of more
+ * than one rank with a mode that resolves to the graph -> LB2_UNSUPPORTED. */
+lb2_status lb2_partition_index_build(const void* centroids, uint32_t k, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                                     lb2_partition_index_mode mode, uint64_t seed, uint32_t insert_batch,
+                                     lb2_partition_index** out);
+/* PartitionTransformer::transform's partition step (ivf/transform.rs:112-124).  pi == NULL is the exact scan:
+ * lb2_compute_partitions with the same arguments.  Otherwise SimpleIndex::search (utils.rs:93-108) of every row:
+ * search_basic (hnsw/builder.rs:164-235) with k = 1, ef = 15, no bounds and no prefilter (entry node 0, greedy_search
+ * at every level from max_level - 1 down to 0, beam_search at level 0), part_out[i] / dist_out[i] the first result.
+ * The distance is the f32 16-lane rule of lb2_compute_partitions (l2.rs / dot.rs with LANES = 16), so dist_out is the
+ * reference's CENTROID_DIST for the row and partition.  k, d and the metric must be pi's; the graph reads its own copy
+ * of the centroids, so `centroids` is only read when pi == NULL.  Rows are f32 or u8 (held as f32), on the host
+ * (streamed in chunks, LB2_CHUNK_ROWS / LB2_MAX_RESIDENT_MB) or the device.  valid_out[i] = 0, part_out[i] = 0 and
+ * dist_out[i] = NaN for
+ *  - a row with a NaN or infinite element: KeepFiniteVectors drops it before the partition step (ivf.rs:149-166);
+ *  - a finite row whose search keeps no result: beam_search admits f32::MIN <= dist < f32::MAX only (graph.rs:
+ *    290-291), so a row whose every distance it meets overflows has none, and the reference's `res[0]` panics
+ *    (utils.rs:106).  The exact scan drops such a row too (kmeans.rs:1187-1246 returns None).
+ * Every other row is valid, with the graph's answer. */
+lb2_status lb2_partition_index_assign(const lb2_partition_index* pi, const void* centroids, uint32_t k, uint32_t d,
+                                      lb2_dtype dtype, lb2_metric metric, const void* vectors, uint64_t n,
+                                      uint32_t* part_out, float* dist_out, uint8_t* valid_out);
+/* the graph's shape (each output nullable), and the graph in the layout of lb2_index_export_hnsw_flat for one
+ * partition of k rows: levels[k], counts0[k], neighbors0 / dists0 [k][2m], counts_up / neighbors_up / dists_up over
+ * the num_upper_rows upper-level rows ([.][m]); unused list slots are zero */
+lb2_status lb2_partition_index_info(const lb2_partition_index* pi, uint32_t* k, uint32_t* d, uint32_t* max_level,
+                                    uint32_t* m, uint32_t* ef_construction, uint64_t* num_upper_rows);
+lb2_status lb2_partition_index_export(const lb2_partition_index* pi, uint8_t* levels_out, uint32_t* counts0_out,
+                                      uint32_t* neighbors0_out, float* dists0_out, uint32_t* counts_up_out,
+                                      uint32_t* neighbors_up_out, float* dists_up_out);
+lb2_status lb2_partition_index_destroy(lb2_partition_index* pi); /* NULL is a no-op */
+/* Builds: lb2_kmeans_params.partition_index selects the rule of the full pass of every build that takes the params
+ * (IVF_PQ, IVF_FLAT, IVF_SQ, IVF_RQ and the three IVF_HNSW kinds); the graph is built over the trained centroids
+ * (under L2 for a cosine index, whose rows are normalised first; dot for dot) with level seed
+ * seed ^ 0x7061727469646978 ("partidix"; `seed` the build's seed) and insert_batch partition_index_batch.  Each
+ * row's partition, CENTROID_DIST (IVF_RQ's dist_v_c and factors) and residual (IVF_PQ's codes) follow the graph's
+ * answer; rows without one are dropped, as the exact scan drops its None rows.  EXACT builds are unchanged. */
+/* The partition rule of an index handle: the mode, the graph's level seed and insert_batch, and the graph over the
+ * index's centroids when the mode resolves to one for the index's column type (the rule and refusals of
+ * lb2_partition_index_build; cosine indexes use L2 on normalised rows).  It serves lb2_index_transform, the
+ * nearest-new-centroid transform of IVF_RQ rows in lb2_index_split (ivf.rs:301-304), and every index that
+ * lb2_index_optimize / _split / _join / _update return, which inherit the rule and build the graph over their own
+ * centroids.  Builds set it from their parameters; an index opened with lb2_index_create* / _load* /
+ * _load_storage starts EXACT (LANCE_USE_HNSW_SPEEDUP_INDEXING's mapping is the caller's: see INTEGRATION.md).
+ * EXACT drops the graph.  lb2_index_load_storage keeps the rule. */
+lb2_status lb2_index_set_partition_index(lb2_index* index, lb2_partition_index_mode mode, uint64_t seed,
+                                         uint32_t insert_batch);
 
 /* ---- product quantisation (lance-index/src/vector/pq*.rs) ------------------------------------ */
 typedef struct {

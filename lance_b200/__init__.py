@@ -24,7 +24,7 @@ __all__ = ["device_count", "DeviceArray", "PinnedArray", "LanceB200Error", "trai
            "build_distance_table_l2", "compute_pq_distance", "flat_topk", "flat_search", "IvfPqIndex",
            "IvfBuildParams", "IvfFlatIndex", "SQBuildParams", "ScalarQuantizer", "IvfSqIndex", "HnswBuildParams",
            "IvfHnswSqIndex", "IvfHnswPqIndex", "IvfHnswFlatIndex", "RQBuildParams",
-           "RabitQuantizer", "IvfRqIndex", "launch_count", "profile"]
+           "RabitQuantizer", "IvfRqIndex", "PartitionIndex", "launch_count", "profile"]
 
 
 def _metric(m):
@@ -269,6 +269,98 @@ def compute_residual(centroids, vectors, partitions, bf16=False):
     return out
 
 
+# ---- lance-index::vector::utils: SimpleIndex, the HNSW graph over the centroids ----------------------------
+PARTITION_INDEX_MODES = {"exact": 0, "auto": 1, "hnsw": 2}
+
+
+def _pi_mode(mode):
+    if mode not in PARTITION_INDEX_MODES:
+        raise ValueError(f"partition index mode {mode!r}: one of {sorted(PARTITION_INDEX_MODES)}")
+    return PARTITION_INDEX_MODES[mode]
+
+
+class PartitionIndex:
+    """SimpleIndex (lance-index/src/vector/utils.rs:26-108): an HNSW graph over the IVF centroids that assigns each row
+    by one graph search (k = 1, ef = 15) instead of the exact scan.  mode is LANCE_USE_HNSW_SPEEDUP_INDEXING's value:
+    "exact" (disabled, the default), "auto" (unset: the graph when k * d >= 1 000 000) or "hnsw" (enabled).  Only f32
+    models have a graph (u8 columns have f32 models); f16 / bf16 models, like "exact", assign by the exact scan
+    (compute_partitions).  Cosine columns are normalised by the caller and assigned under "l2"."""
+
+    def __init__(self, handle, centroids, dtype, distance_type):
+        self._h, self._centroids, self._dt, self.distance_type = handle, centroids, dtype, distance_type
+
+    @staticmethod
+    def uses_graph(k, d, mode="auto", dtype=np.float32, bf16=False):
+        """may_train_index's decision (utils.rs:67-91) for a k x d model over columns of `dtype`; host only"""
+        dt = BF16 if bf16 else _DTYPES[np.dtype(dtype)]
+        out = C.c_int()
+        check(lib().lb2_partition_index_uses_graph(C.c_uint64(k), C.c_uint32(d), C.c_int(dt), C.c_int(_pi_mode(mode)),
+                                                   C.byref(out)))
+        return bool(out.value)
+
+    @classmethod
+    def build(cls, centroids, distance_type="l2", mode="hnsw", seed=0, insert_batch=1, dtype=np.float32, bf16=False):
+        """lb2_partition_index_build over the model `centroids` [k][d] of a column of element type `dtype` (bf16=True:
+        a bf16 column, uint16 bit patterns).  The graph (when the mode resolves to it) levels nodes with seed and is
+        built serially (insert_batch 1) or in rounds of insert_batch concurrent inserts."""
+        dt = BF16 if bf16 else _DTYPES[np.dtype(dtype)]
+        centroids = np.ascontiguousarray(centroids, dtype=_model_np(dt))
+        k, d = centroids.shape
+        h = C.c_void_p()
+        check(lib().lb2_partition_index_build(C.c_void_p(centroids.ctypes.data), C.c_uint32(k), C.c_uint32(d),
+                                              C.c_int(dt), C.c_int(_metric(distance_type)), C.c_int(_pi_mode(mode)),
+                                              C.c_uint64(seed), C.c_uint32(insert_batch), C.byref(h)))
+        return cls(h if h.value else None, centroids, dt, distance_type)
+
+    @property
+    def has_graph(self):
+        return self._h is not None
+
+    def assign(self, vectors):
+        """lb2_partition_index_assign -> (part_ids u32[n], dists f32[n], valid bool[n]); without a graph this is
+        compute_partitions.  vectors: the column's rows (numpy, DeviceArray or PinnedArray), in its element type."""
+        vectors, dt = _typed(vectors, self._dt == BF16)
+        k, d = self._centroids.shape
+        n = vectors.shape[0]
+        part = np.empty(n, np.uint32)
+        dist = np.empty(n, np.float32)
+        valid = np.empty(n, np.uint8)
+        vp, _keep = as_ptr(vectors)
+        check(lib().lb2_partition_index_assign(self._h, C.c_void_p(self._centroids.ctypes.data), C.c_uint32(k),
+                                               C.c_uint32(d), C.c_int(dt), C.c_int(_metric(self.distance_type)), vp,
+                                               C.c_uint64(n), C.c_void_p(part.ctypes.data),
+                                               C.c_void_p(dist.ctypes.data), C.c_void_p(valid.ctypes.data)))
+        return part, dist, valid.astype(bool)
+
+    def export(self):
+        """the graph in IvfHnswFlatIndex.export()["graph"]'s layout (one partition of k rows), or None without one"""
+        if self._h is None:
+            return None
+        k, d, ml, m, efc, nu = (C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint32(), C.c_uint64())
+        check(lib().lb2_partition_index_info(self._h, C.byref(k), C.byref(d), C.byref(ml), C.byref(m), C.byref(efc),
+                                             C.byref(nu)))
+        n, m, nu = k.value, m.value, nu.value
+        g = dict(max_level=ml.value, m=m, ef_construction=efc.value, levels=np.empty(n, np.uint8),
+                 counts0=np.empty(n, np.uint32), neighbors0=np.empty((n, 2 * m), np.uint32),
+                 dists0=np.empty((n, 2 * m), np.float32), counts_up=np.empty(nu, np.uint32),
+                 neighbors_up=np.empty((nu, m), np.uint32), dists_up=np.empty((nu, m), np.float32))
+        ptr = {key: C.c_void_p(v.ctypes.data) if isinstance(v, np.ndarray) and v.size else None for key, v in g.items()}
+        check(lib().lb2_partition_index_export(self._h, ptr["levels"], ptr["counts0"], ptr["neighbors0"],
+                                               ptr["dists0"], ptr["counts_up"], ptr["neighbors_up"], ptr["dists_up"]))
+        return g
+
+    def close(self):
+        if self._h is not None:
+            lib().lb2_partition_index_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 # ---- lance-index::vector::pq -----------------------------------------------------------------
 class PQBuildParams:
     """lance_index::vector::pq::builder::PQBuildParams (pq/builder.rs:27-59)."""
@@ -447,16 +539,20 @@ class IvfBuildParams:
 
     def __init__(self, num_partitions=256, num_sub_vectors=16, num_bits=8, max_iters=50,
                  sample_rate=256, pq_max_iters=50, pq_sample_rate=256, seed=0, centroids=None,
-                 codebook=None):
+                 codebook=None, partition_index="exact", partition_index_batch=1):
         self.num_partitions, self.num_sub_vectors, self.num_bits = num_partitions, num_sub_vectors, num_bits
         self.max_iters, self.sample_rate, self.pq_max_iters = max_iters, sample_rate, pq_max_iters
         self.pq_sample_rate, self.seed, self.centroids, self.codebook = pq_sample_rate, seed, centroids, codebook
+        # how the full pass assigns rows (PartitionIndex's modes: "exact", "auto", "hnsw") and the graph's insert_batch
+        self.partition_index, self.partition_index_batch = partition_index, partition_index_batch
 
 
 def _fill_build_params(bp, params):
     """lb2_ivfpq_build_params from IvfBuildParams; returns the arrays bp points into (keep them alive)"""
     bp.num_partitions = params.num_partitions
     bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed = params.max_iters, params.sample_rate, params.seed
+    bp.ivf.partition_index = _pi_mode(getattr(params, "partition_index", "exact"))
+    bp.ivf.partition_index_batch = getattr(params, "partition_index_batch", 1)
     bp.pq.num_sub_vectors, bp.pq.num_bits = params.num_sub_vectors, params.num_bits
     bp.pq.max_iters, bp.pq.sample_rate, bp.pq.seed = params.pq_max_iters, params.pq_sample_rate, params.seed + 1000
     bp.seed = params.seed
@@ -1069,6 +1165,14 @@ class IvfPqIndex:
         check(lib().lb2_index_search_sharded(self._h, qp, C.c_uint64(nq), C.byref(sp), ip, dp, None))
         return ids, dists
 
+    def set_partition_index(self, mode, seed=0, insert_batch=1):
+        """lb2_index_set_partition_index: how this index assigns rows it transforms (transform, IVF_RQ's split) and
+        the rule the indexes optimize / split / join return inherit.  mode as PartitionIndex's ("exact", "auto",
+        "hnsw": LANCE_USE_HNSW_SPEEDUP_INDEXING's disabled / unset / enabled); the graph over this index's centroids
+        draws its levels from seed and is built with insert_batch."""
+        check(lib().lb2_index_set_partition_index(self._h, C.c_int(_pi_mode(mode)), C.c_uint64(seed),
+                                                  C.c_uint32(insert_batch)))
+
     def close(self):
         if self._h:
             lib().lb2_index_destroy(self._h)
@@ -1087,7 +1191,7 @@ class IvfFlatIndex(IvfPqIndex):
 
     @classmethod
     def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
-              centroids=None, row_ids=None, bf16=False):
+              centroids=None, row_ids=None, partition_index="exact", partition_index_batch=1, bf16=False):
         """bf16=True: `data` is a uint16 array holding bfloat16 bit patterns (numpy has no bf16 dtype)."""
         data, dt = _typed(data, bf16)
         n, d = data.shape
@@ -1095,6 +1199,8 @@ class IvfFlatIndex(IvfPqIndex):
         lib().lb2_ivfflat_build_params_default(C.byref(bp))
         bp.num_partitions = num_partitions
         bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed, bp.seed = max_iters, sample_rate, seed, seed
+        bp.ivf.partition_index = _pi_mode(partition_index)
+        bp.ivf.partition_index_batch = partition_index_batch
         keep = None
         if centroids is not None:
             keep = _f32(centroids)
@@ -1207,7 +1313,7 @@ class IvfSqIndex(IvfPqIndex):
 
     @classmethod
     def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
-              centroids=None, row_ids=None, bf16=False, sq_params=None):
+              centroids=None, row_ids=None, partition_index="exact", partition_index_batch=1, bf16=False, sq_params=None):
         """create_index(.., "IVF_SQ"); the IVF stage equals IvfFlatIndex.build's with the same arguments.
         bf16=True: `data` is a uint16 array holding bfloat16 bit patterns."""
         sq_params = sq_params or SQBuildParams()
@@ -1217,6 +1323,8 @@ class IvfSqIndex(IvfPqIndex):
         lib().lb2_ivfsq_build_params_default(C.byref(bp))
         bp.num_partitions = num_partitions
         bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed, bp.seed = max_iters, sample_rate, seed, seed
+        bp.ivf.partition_index = _pi_mode(partition_index)
+        bp.ivf.partition_index_batch = partition_index_batch
         bp.num_bits, bp.sample_rate = sq_params.num_bits, sq_params.sample_rate
         keep = None
         if centroids is not None:
@@ -1439,7 +1547,7 @@ class IvfHnswSqIndex(_HnswGraphs, IvfSqIndex):
 
     @classmethod
     def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
-              centroids=None, row_ids=None, bf16=False, sq_params=None, hnsw_params=None):
+              centroids=None, row_ids=None, partition_index="exact", partition_index_batch=1, bf16=False, sq_params=None, hnsw_params=None):
         """create_index(.., "IVF_HNSW_SQ"); the IVF stage, bounds and codes equal IvfSqIndex.build's with the same
         arguments.  The graphs' level draws use `seed`."""
         sq_params = sq_params or SQBuildParams()
@@ -1450,6 +1558,8 @@ class IvfHnswSqIndex(_HnswGraphs, IvfSqIndex):
         lib().lb2_ivfhnswsq_build_params_default(C.byref(bp))
         bp.sq.num_partitions = num_partitions
         bp.sq.ivf.max_iters, bp.sq.ivf.sample_rate, bp.sq.ivf.seed, bp.sq.seed = max_iters, sample_rate, seed, seed
+        bp.sq.ivf.partition_index = _pi_mode(partition_index)
+        bp.sq.ivf.partition_index_batch = partition_index_batch
         bp.sq.num_bits, bp.sq.sample_rate = sq_params.num_bits, sq_params.sample_rate
         bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
         bp.insert_batch = hnsw_params.insert_batch
@@ -1552,7 +1662,7 @@ class IvfHnswFlatIndex(_HnswGraphs, IvfFlatIndex):
 
     @classmethod
     def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
-              centroids=None, row_ids=None, bf16=False, hnsw_params=None):
+              centroids=None, row_ids=None, partition_index="exact", partition_index_batch=1, bf16=False, hnsw_params=None):
         """create_index(.., "IVF_HNSW_FLAT"); the IVF stage, vectors and row ids equal IvfFlatIndex.build's with the
         same arguments.  The graphs' level draws use `seed`.  bf16=True: uint16 bfloat16 bit patterns."""
         hnsw_params = hnsw_params or HnswBuildParams()
@@ -1563,6 +1673,8 @@ class IvfHnswFlatIndex(_HnswGraphs, IvfFlatIndex):
         f = bp.flat
         f.num_partitions = num_partitions
         f.ivf.max_iters, f.ivf.sample_rate, f.ivf.seed, f.seed = max_iters, sample_rate, seed, seed
+        f.ivf.partition_index = _pi_mode(partition_index)
+        f.ivf.partition_index_batch = partition_index_batch
         bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
         bp.insert_batch = hnsw_params.insert_batch
         keep = None
@@ -1642,7 +1754,7 @@ class IvfRqIndex(IvfPqIndex):
 
     @classmethod
     def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
-              centroids=None, row_ids=None, rq_params=None):
+              centroids=None, row_ids=None, partition_index="exact", partition_index_batch=1, rq_params=None):
         """create_index(.., "IVF_RQ"); the IVF stage equals IvfFlatIndex.build's with the same arguments, the
         rotation is drawn from seed + 1.  f32 columns."""
         rq_params = rq_params or RQBuildParams()
@@ -1652,6 +1764,8 @@ class IvfRqIndex(IvfPqIndex):
         lib().lb2_ivfrq_build_params_default(C.byref(bp))
         bp.num_partitions = num_partitions
         bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed, bp.seed = max_iters, sample_rate, seed, seed
+        bp.ivf.partition_index = _pi_mode(partition_index)
+        bp.ivf.partition_index_batch = partition_index_batch
         bp.num_bits = rq_params.num_bits
         keep = None
         if centroids is not None:

@@ -29,7 +29,7 @@ class KMeansParams(C.Structure):
     _fields_ = [("max_iters", C.c_uint32), ("tolerance", C.c_double), ("redos", C.c_uint32),
                 ("balance_factor", C.c_float), ("hierarchical_k", C.c_uint32),
                 ("sample_rate", C.c_uint64), ("seed", C.c_uint64), ("init_centroids", C.c_void_p),
-                ("metric", C.c_int)]
+                ("metric", C.c_int), ("partition_index", C.c_uint32), ("partition_index_batch", C.c_uint32)]
 
 
 class PQParams(C.Structure):
@@ -146,6 +146,9 @@ EXPORTS = [
     "lb2_index_export_hnsw_pq", "lb2_ivfhnswflat_build_params_default", "lb2_ivfhnswflat_build",
     "lb2_index_load_hnsw_flat", "lb2_index_hnsw_flat_info", "lb2_index_export_hnsw_flat",
     "lb2_index_export_storage", "lb2_index_load_storage",
+    "lb2_partition_index_uses_graph", "lb2_partition_index_build", "lb2_partition_index_assign",
+    "lb2_partition_index_info", "lb2_partition_index_export", "lb2_partition_index_destroy",
+    "lb2_index_set_partition_index",
 ]
 
 _lib = None

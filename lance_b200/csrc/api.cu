@@ -255,6 +255,8 @@ void lb2_kmeans_params_default(lb2_kmeans_params* p) {
   p->seed = 0;
   p->init_centroids = nullptr;
   p->metric = LB2_L2;
+  p->partition_index = LB2_PARTITION_INDEX_EXACT;
+  p->partition_index_batch = 1;
 }
 void lb2_pq_params_default(lb2_pq_params* p) {
   p->num_sub_vectors = 16;
@@ -315,6 +317,8 @@ lb2_status lb2_kmeans_train(const void* data, uint64_t n, uint32_t d, lb2_dtype 
   LB2_API_BEGIN
   LB2_REQUIRE(params && data && centroids_out, "null argument");
   check_redos(params->redos, params->balance_factor);
+  if (params->partition_index != LB2_PARTITION_INDEX_EXACT)
+    fail(LB2_INVALID_ARG, "KMeans: training never assigns through a partition index (partition_index must be EXACT)");
   const int m = metric_of(params->metric);
   if (m == METRIC_COSINE)
     fail(LB2_INVALID_ARG, "KMeans: cosine is trained as L2 on normalised vectors (normalise first)");

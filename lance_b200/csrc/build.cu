@@ -184,6 +184,12 @@ static void train_ivf_stage(Source& src, lb2_index* ix, const lb2_kmeans_params&
 
 // the stage times of a build from its events: start, IVF trained, [quantizer trained,] transformed, grouped (IVF_FLAT
 // has no quantizer stage: 4 events, ms_pq_train 0)
+// the build's partition rule from its IVF parameters (lb2_kmeans_params.partition_index): recorded on ix, with the
+// graph over the trained centroids when the mode resolves to one; the graph's levels draw from partition_index_seed
+static void attach_partition_index(lb2_index* ix, const lb2_kmeans_params& kp, uint64_t seed) {
+  set_partition_index(ix, kp.partition_index, partition_index_seed(seed), kp.partition_index_batch);
+}
+
 static void fill_stats(lb2_build_stats* stats, const EventSet& ev, const std::vector<double>& loss,
                        const std::vector<uint32_t>& iters, const std::vector<uint32_t>& pq_iters = {}) {
   if (!stats) return;
@@ -201,10 +207,10 @@ static void fill_stats(lb2_build_stats* stats, const EventSet& ev, const std::ve
 
 // IvfTransformer's partition step over one chunk of rows (ivf.rs:158-166): normalised first under cosine, then
 // assigned (by dot or L2) from f32, or from the rows' own type (xnat / dtype, for_each_chunk) when not normalised.
-// Returns the chunk as the index sees it.
+// Returns the chunk as the index sees it.  pi (nullable): the index's partition index, which assigns instead.
 static const float* normalize_assign(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
                                      const float* cent, int K, DevBuf<float>& normbuf, uint32_t* part, uint8_t* valid,
-                                     float* dist) {
+                                     float* dist, const lb2_partition_index* pi = nullptr) {
   const float* xp = xf;
   if (m == METRIC_COSINE) {
     if (normbuf.n < (size_t)rows * d) normbuf.alloc((size_t)rows * d);
@@ -212,7 +218,10 @@ static const float* normalize_assign(const float* xf, const void* xnat, int dtyp
     xp = normbuf.p;
     xnat = nullptr;
   }
-  assign_f32(xp, rows, d, cent, K, m == METRIC_DOT ? METRIC_DOT : METRIC_L2, nullptr, part, dist, valid, xnat, dtype);
+  if (pi)  // the partition index over these centroids (PartitionTransformer's graph arm, ivf/transform.rs:112-124)
+    partition_index_assign(*pi, xp, rows, part, dist, valid);
+  else
+    assign_f32(xp, rows, d, cent, K, m == METRIC_DOT ? METRIC_DOT : METRIC_L2, nullptr, part, dist, valid, xnat, dtype);
   return xp;
 }
 
@@ -223,8 +232,8 @@ static const float* normalize_assign(const float* xf, const void* xnat, int dtyp
 // assignment, whether residuals are taken (not for dot, PQBuildParams::use_residual) and the query-time table.
 static void transform_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m, const float* cent,
                             int K, const float* codebook, int M, int nbits, DevBuf<float>& normbuf, uint32_t* part,
-                            uint8_t* codes, uint8_t* valid) {
-  const float* xp = normalize_assign(xf, xnat, dtype, rows, d, m, cent, K, normbuf, part, valid, nullptr);
+                            uint8_t* codes, uint8_t* valid, const lb2_partition_index* pi = nullptr) {
+  const float* xp = normalize_assign(xf, xnat, dtype, rows, d, m, cent, K, normbuf, part, valid, nullptr, pi);
   const bool dot = m == METRIC_DOT;
   pq_encode_any(xp, rows, d, M, d / M, codebook, METRIC_L2, dot ? nullptr : cent, dot ? nullptr : part, valid, nbits,
                 codes);
@@ -237,8 +246,9 @@ static void transform_chunk(const float* xf, const void* xnat, int dtype, uint64
 // distance, so the elements are checked.
 static const float* assign_flat_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
                                       const float* cent, int K, DevBuf<float>& normbuf, uint32_t* part,
-                                      uint8_t* valid, float* dist = nullptr) {
-  const float* xp = normalize_assign(xf, xnat, dtype, rows, d, m, cent, K, normbuf, part, valid, dist);
+                                      uint8_t* valid, float* dist = nullptr,
+                                      const lb2_partition_index* pi = nullptr) {
+  const float* xp = normalize_assign(xf, xnat, dtype, rows, d, m, cent, K, normbuf, part, valid, dist, pi);
   if (m == METRIC_DOT && rows)
     LB2_LAUNCH("drop_nonfinite_rows", finite_rows_kernel, cdiv(rows * 32, 256), 256, 0, xp, rows, d, valid, 1);
   return xp;
@@ -274,13 +284,14 @@ struct RqWork {
 };
 static void rq_transform_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
                                const float* cent, int K, const float* rotation, int num_bits, const float* cnorm,
-                               RqWork& w, uint32_t* part, uint8_t* valid, uint8_t* codes, float* add, float* scale) {
+                               RqWork& w, uint32_t* part, uint8_t* valid, uint8_t* codes, float* add, float* scale,
+                               const lb2_partition_index* pi = nullptr) {
   const int cd = d * num_bits;
   const uint64_t sub = std::min<uint64_t>(rows, std::max<uint64_t>(1, (1ull << 28) / (uint64_t)cd));
   if (w.dist.n < rows) w.dist.alloc(rows);
   if (w.res.n < rows * d) w.res.alloc(rows * d);
   if (w.rot.n < sub * cd) w.rot.alloc(sub * cd);
-  const float* xs = assign_flat_chunk(xf, xnat, dtype, rows, d, m, cent, K, w.normbuf, part, valid, w.dist.p);
+  const float* xs = assign_flat_chunk(xf, xnat, dtype, rows, d, m, cent, K, w.normbuf, part, valid, w.dist.p, pi);
   rq_residual_f32(xs, rows, d, cent, part, valid, w.res.p);
   for (uint64_t r0 = 0; r0 < rows; r0 += sub) {
     const uint64_t rs = std::min(sub, rows - r0);
@@ -307,6 +318,7 @@ void index_transform_rows(const lb2_index* index, Source& src, const uint32_t* g
   const int d = index->d, m = index->metric, K = index->K;
   const size_t rb = index->row_bytes();
   const float* cent = index->centroids.p;
+  const lb2_partition_index* pi = index->pidx.get();  // the index's partition rule (null: the exact scan)
   // every output the chunk functions write is needed: the caller's NULLs get scratch
   DevBuf<uint32_t> ptmp;
   DevBuf<uint8_t> vtmp, ltmp;
@@ -330,27 +342,27 @@ void index_transform_rows(const lb2_index* index, Source& src, const uint32_t* g
       switch (index->kind) {
         case IndexKind::PQ:  // lb2_ivfpq_transform's rows
           if (given_part) {
-            const float* xp = normalize_assign(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0, nullptr);
+            const float* xp = normalize_assign(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0, nullptr, pi);
             const bool dot = m == METRIC_DOT;
             pq_encode_any(xp, rows, d, index->M, d / index->M, index->codebook.p, METRIC_L2, dot ? nullptr : cent,
                           dot ? nullptr : given_part + r0, vp + r0, index->nbits, out);
           } else {
             transform_chunk(xf, xnat, sdt, rows, d, m, cent, K, index->codebook.p, index->M, index->nbits, normbuf,
-                            pp + r0, out, vp + r0);
+                            pp + r0, out, vp + r0, pi);
           }
           break;
         case IndexKind::RQ:  // lb2_ivfrq_transform's rows
           rq_transform_chunk(xf, xnat, sdt, rows, d, m, cent, K, index->rq_rot.p, index->nbits, cnorm.p, w, pp + r0,
-                             vp + r0, out, ap + r0, sp + r0);
+                             vp + r0, out, ap + r0, sp + r0, pi);
           break;
         case IndexKind::SQ: {  // lb2_ivfsq_build's codes
-          const float* xs = assign_flat_chunk(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0);
+          const float* xs = assign_flat_chunk(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0, nullptr, pi);
           if (m == METRIC_COSINE) round_model(normbuf.p, (size_t)rows * d, index->dtype);
           sq_encode_f32(xs, (uint64_t)rows * d, index->sq_lower, index->sq_upper, out);
           break;
         }
         case IndexKind::FLAT: {  // index_load_flat_src's stored rows: (normalised) f32 in the stored element type
-          const float* xs = assign_flat_chunk(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0);
+          const float* xs = assign_flat_chunk(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0, nullptr, pi);
           const lb2_dtype vdt = index->vdtype();
           if (vdt == LB2_F32)
             d2d(reinterpret_cast<float*>(out), xs, (size_t)rows * d);
@@ -536,10 +548,11 @@ lb2_status lb2_ivfflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype
   DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1));
   {
     TagScope tg("transform");
+    attach_partition_index(ix.get(), params->ivf, params->seed);
     DevBuf<float> normbuf;
     for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
       assign_flat_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, normbuf, part.p + r0,
-                        valid.p + r0);
+                        valid.p + r0, nullptr, ix->pidx.get());
     });
   }
   ev.record(2);
@@ -594,10 +607,11 @@ lb2_status lb2_ivfsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1)), codes(std::max<uint64_t>(1, (uint64_t)n * d));
   {
     TagScope tg("transform");
+    attach_partition_index(ix.get(), params->ivf, params->seed);
     DevBuf<float> normbuf;
     for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
       const float* xs = assign_flat_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, normbuf,
-                                          part.p + r0, valid.p + r0);
+                                          part.p + r0, valid.p + r0, nullptr, ix->pidx.get());
       if (m == METRIC_COSINE) round_model(normbuf.p, (size_t)rows * d, dtype);  // as IVF_FLAT stores them
       sq_encode_f32(xs, (uint64_t)rows * d, ix->sq_lower, ix->sq_upper, codes.p + r0 * d);
     });
@@ -651,10 +665,12 @@ lb2_status lb2_ivfrq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   {
     TagScope tg("transform");
     rq_centroid_norms(m, ix->centroids.p, K, (int)d, cnorm);
+    attach_partition_index(ix.get(), params->ivf, params->seed);
     RqWork w;
     for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
       rq_transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, ix->rq_rot.p, ix->nbits,
-                         cnorm.p, w, part.p + r0, valid.p + r0, codes.p + r0 * (cd / 8), add.p + r0, scale.p + r0);
+                         cnorm.p, w, part.p + r0, valid.p + r0, codes.p + r0 * (cd / 8), add.p + r0, scale.p + r0,
+                         ix->pidx.get());
     });
   }
   ev.record(3);
@@ -774,10 +790,11 @@ lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   DevBuf<uint8_t> codes(std::max<uint64_t>(1, (size_t)n * cw)), valid(std::max<uint64_t>(n, 1));
   {
     TagScope tg("transform");
+    attach_partition_index(ix.get(), params->ivf, params->seed);
     DevBuf<float> normbuf;
     for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
       transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, ix->codebook.p, M, nbits, normbuf,
-                      part.p + r0, codes.p + r0 * cw, valid.p + r0);
+                      part.p + r0, codes.p + r0 * cw, valid.p + r0, ix->pidx.get());
     });
   }
   ev.record(3);

@@ -1117,6 +1117,21 @@ void hnsw_build(HnswGraph& g, const lb2_index& ix, uint64_t seed, const HnswKeep
   });
 }
 
+void hnsw_build_rows(HnswGraph& g, const float* rows, uint64_t n, int d, int metric, uint64_t seed) {
+  LB2_REQUIRE(d % 4 == 0, "%s: the graph's rows need a dimension that is a multiple of 4, d = %d", g.kind, d);
+  const uint64_t off[2] = {0, n};
+  DevBuf<uint64_t> doff(2);
+  h2d(doff.p, off, 2);
+  auto go = [&](auto m) {
+    FlatDist<decltype(m)::value, float> P{};
+    P.base = rows;
+    P.d = d;
+    build_graphs(g, doff.p, 1, seed, nullptr, P, 0u, query_words(d));
+  };
+  if (metric == METRIC_DOT) go(std::integral_constant<int, METRIC_DOT>{});
+  else go(std::integral_constant<int, METRIC_L2>{});
+}
+
 // caller memory (host or device) -> host
 template <class T>
 static std::vector<T> fetch(const T* src, size_t count) {

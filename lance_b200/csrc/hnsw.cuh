@@ -78,6 +78,9 @@ struct HnswKeep {
 // PqDist, FlatDist).  Fills g (its parameters set by the caller).  With `keep`, only the partitions keep->src marks -1
 // are built; the others are spliced from keep->old.
 void hnsw_build(HnswGraph& g, const lb2_index& ix, uint64_t seed, const HnswKeep* keep = nullptr);
+// the same build over one partition of n f32 rows on the device (d % 4 == 0), with IVF_HNSW_FLAT's f32 distances
+// under L2 (METRIC_L2) or dot (METRIC_DOT): the graph over the centroids of a partition index (partition_index.cu)
+void hnsw_build_rows(HnswGraph& g, const float* rows, uint64_t n, int d, int metric, uint64_t seed);
 // a graph from the caller's arrays in the layout above (host or device memory), checked against the partitions
 void hnsw_load(HnswGraph& g, const uint64_t* part_offsets, int K, const uint8_t* levels, const uint32_t* counts0,
                const uint32_t* nbr0, const float* dist0, const uint32_t* counts_up, const uint32_t* nbr_up,

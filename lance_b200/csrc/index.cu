@@ -607,6 +607,7 @@ std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_optimize_
     LB2_LAUNCH("remap_rows", remap_rows_kernel, cdiv(n_all, 256), 256, 0, rid.p, valid.p, n_all, ro.get(), rn.get(),
                p.n_remap, old->part_offsets.p, old->K, n_old, dropped.p);
   index_load_dev(ix.get(), part.p, payload.p, rid.p, n_all, valid.p, fa.p, fs.p);
+  set_partition_index(ix.get(), old->pi_mode, old->pi_seed, old->pi_batch);  // the rule, over the new centroids
   if (old->hnsw) {
     const HnswGraph& og = *old->hnsw;
     const HnswKeep keep = kept_partitions(old, ix.get(), pm.get(), dropped.p, added.p);
@@ -779,6 +780,16 @@ std::unique_ptr<HnswGraph> new_graph(IndexKind kind, uint32_t max_level, uint32_
   g->ef_construction = (int)ef_construction;
   g->insert_batch = std::max<uint32_t>(insert_batch, 1);
   return g;
+}
+
+void set_partition_index(lb2_index* ix, uint32_t mode, uint64_t seed, uint32_t insert_batch) {
+  PartitionIndexPtr pi = partition_index_make(ix->centroids.p, (uint32_t)ix->K, (uint32_t)ix->d, ix->dtype,
+                                              ix->metric == METRIC_DOT ? METRIC_DOT : METRIC_L2, mode, seed,
+                                              insert_batch);
+  ix->pi_mode = mode;
+  ix->pi_seed = seed;
+  ix->pi_batch = std::max<uint32_t>(insert_batch, 1);
+  ix->pidx = std::move(pi);
 }
 
 void attach_graph(lb2_index* ix, uint32_t max_level, uint32_t m, uint32_t ef_construction, uint32_t insert_batch,
@@ -1281,6 +1292,14 @@ lb2_status lb2_index_repartition(const lb2_index* shard, lb2_index** owned_out) 
   build_skew(ix.get());
   sync_stream();
   *owned_out = ix.release();
+  LB2_API_END
+}
+
+lb2_status lb2_index_set_partition_index(lb2_index* index, lb2_partition_index_mode mode, uint64_t seed,
+                                         uint32_t insert_batch) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index, "null argument");
+  set_partition_index(index, (uint32_t)mode, seed, insert_batch);
   LB2_API_END
 }
 

@@ -3,6 +3,7 @@
 #include <memory>
 
 #include "hnsw.cuh"
+#include "partition_index.cuh"
 #include "staging.cuh"
 
 namespace lb2 {
@@ -35,6 +36,13 @@ struct lb2_index {
   // IVF_HNSW_SQ / IVF_HNSW_PQ / IVF_HNSW_FLAT: an IVF_SQ / IVF_PQ / IVF_FLAT index with an HNSW graph per partition
   // over its codes or vectors (hnsw.cuh), searched through the graphs instead of the partition scan
   std::unique_ptr<lb2::HnswGraph> hnsw;
+  // how rows are assigned to partitions (lb2_partition_index_mode, partition_index.cuh): the mode, the graph's level
+  // seed and insert_batch, and the graph over the centroids when the mode resolves to one (null: the exact scan).
+  // lb2_index_transform, IVF_RQ's split transform and the indexes optimize / split / join return follow it.
+  uint32_t pi_mode = LB2_PARTITION_INDEX_EXACT;
+  uint64_t pi_seed = 0;
+  uint32_t pi_batch = 1;
+  lb2::PartitionIndexPtr pidx;
   int code_dim() const { return d * nbits; }
   size_t codebook_len() const { return ((size_t)1 << nbits) * d; }
   // a row's payload in partition order: IVF_FLAT's vectors, the codes of every other kind
@@ -80,6 +88,9 @@ std::unique_ptr<HnswGraph> new_graph(IndexKind kind, uint32_t max_level, uint32_
 // and attached; an IVF_PQ index's skewed code copy is released, as only the IVF_PQ scan reads it
 void attach_graph(lb2_index* ix, uint32_t max_level, uint32_t m, uint32_t ef_construction, uint32_t insert_batch,
                   uint64_t seed, const HnswKeep* keep = nullptr);
+// ix's partition rule: mode, level seed and insert_batch recorded, and the graph over ix's centroids built when the
+// mode resolves to one (lb2_index_set_partition_index, the builds, and the indexes optimize / split / join return)
+void set_partition_index(lb2_index* ix, uint32_t mode, uint64_t seed, uint32_t insert_batch);
 // lb2_index_optimize's merge into a new index; add_valid (nullable, device [n_add]): added rows with 0 are left out
 std::unique_ptr<lb2_index> index_merge(const lb2_index* old, const lb2_optimize_params& p, const char* what,
                                        const uint8_t* add_valid = nullptr);

@@ -815,6 +815,8 @@ lb2_status lb2_index_split(const lb2_index* old, const lb2_split_params* sp, lb2
   DevBuf<uint8_t> newc_model = model_centroids(newc.p, (size_t)new_k * d, dt);
   std::unique_ptr<lb2_index> model = make_index(old->kind, new_k, d, old->metric, dt);
   copy_model(old, model.get(), newc_model.p);
+  if (old->kind == IndexKind::RQ)  // IVF_RQ's moved rows take their nearest new centroid by the index's rule
+    set_partition_index(model.get(), old->pi_mode, old->pi_seed, old->pi_batch);
   const std::vector<uint32_t> cands = reassign_candidates(old, part);
   Moved mv;
   decide_and_transform(old, what, part, c012.p, cands, va.get(), ia.get(), n_a, vb.get(), ib.get(), pb.get(), n_b,
@@ -942,6 +944,8 @@ lb2_status lb2_index_join(const lb2_index* old, const lb2_join_params* jp, lb2_i
   if (n_a) {
     std::unique_ptr<lb2_index> model = make_index(old->kind, new_k, d, old->metric, dt);
     copy_model(old, model.get(), newc_model.p);
+    if (old->kind == IndexKind::RQ)  // IVF_RQ's moved rows take their nearest new centroid by the index's rule
+      set_partition_index(model.get(), old->pi_mode, old->pi_seed, old->pi_batch);
     const std::vector<uint32_t> cands = reassign_candidates(old, part);
     decide_and_transform(old, what, part, nullptr, cands, va.get(), ia.get(), n_a, nullptr, nullptr, nullptr, 0,
                          nullptr, nullptr, 0, true, model.get(), mv);

@@ -621,6 +621,10 @@ lb2_status lb2_index_load_storage(lb2_index* index, const lb2_index_storage* st)
     ix->hnsw = std::move(g);
   }
   sync_stream();
+  ix->pi_mode = index->pi_mode;  // the centroids are unchanged, so the partition rule and its graph carry over
+  ix->pi_seed = index->pi_seed;
+  ix->pi_batch = index->pi_batch;
+  ix->pidx = std::move(index->pidx);
   *index = std::move(*ix);
   LB2_API_END
 }
