@@ -547,20 +547,49 @@ class IvfBuildParams:
         self.partition_index, self.partition_index_batch = partition_index, partition_index_batch
 
 
+def _ivf_fields(bp, num_partitions, max_iters, sample_rate, seed, centroids, partition_index, partition_index_batch):
+    """the IVF fields of a build's parameters (num_partitions, ivf, seed); returns the centroid array bp points into
+    (keep it alive across the build)"""
+    bp.num_partitions = num_partitions
+    bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed, bp.seed = max_iters, sample_rate, seed, seed
+    bp.ivf.partition_index = _pi_mode(partition_index)
+    bp.ivf.partition_index_batch = partition_index_batch
+    if centroids is None:
+        return None
+    keep = _f32(centroids)
+    bp.ivf.init_centroids = as_ptr(keep)[0].value
+    return keep
+
+
+def _hnsw_fields(bp, hnsw_params):
+    """the graph fields of an IVF_HNSW_* build's parameters"""
+    hnsw_params = hnsw_params or HnswBuildParams()
+    bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
+    bp.insert_batch = hnsw_params.insert_batch
+
+
+def _build(cls, build_fn, bp, data, distance_type, row_ids, bf16=False):
+    """cls(handle, stats) of the C build `build_fn` of `data` with the parameters bp"""
+    data, dt = _typed(data, bf16)
+    n, d = data.shape
+    rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
+                                        else np.ascontiguousarray(row_ids, dtype=np.uint64))
+    h, st = C.c_void_p(), BuildStats()
+    dp, _k1 = as_ptr(data)
+    rp, _k2 = as_ptr(rid)
+    check(build_fn(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt), C.c_int(_metric(distance_type)), C.byref(bp), rp,
+                   C.byref(h), C.byref(st)))
+    ix = cls(h, st)
+    ix._dt = dt
+    return ix
+
+
 def _fill_build_params(bp, params):
     """lb2_ivfpq_build_params from IvfBuildParams; returns the arrays bp points into (keep them alive)"""
-    bp.num_partitions = params.num_partitions
-    bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed = params.max_iters, params.sample_rate, params.seed
-    bp.ivf.partition_index = _pi_mode(getattr(params, "partition_index", "exact"))
-    bp.ivf.partition_index_batch = getattr(params, "partition_index_batch", 1)
+    keep = [_ivf_fields(bp, params.num_partitions, params.max_iters, params.sample_rate, params.seed, params.centroids,
+                        getattr(params, "partition_index", "exact"), getattr(params, "partition_index_batch", 1))]
     bp.pq.num_sub_vectors, bp.pq.num_bits = params.num_sub_vectors, params.num_bits
     bp.pq.max_iters, bp.pq.sample_rate, bp.pq.seed = params.pq_max_iters, params.pq_sample_rate, params.seed + 1000
-    bp.seed = params.seed
-    keep = []
-    if params.centroids is not None:
-        c = _f32(params.centroids)
-        keep.append(c)
-        bp.ivf.init_centroids = as_ptr(c)[0].value
     if params.codebook is not None:
         c = _f32(params.codebook)
         keep.append(c)
@@ -579,24 +608,10 @@ class IvfPqIndex:
     def build(cls, data, distance_type="l2", params=None, row_ids=None, bf16=False):
         """IvfIndexBuilder::build (builder.rs:236): create_index("IVF_PQ").
         bf16=True: `data` is a uint16 array holding bfloat16 bit patterns (numpy has no bf16 dtype)."""
-        params = params or IvfBuildParams()
-        data, dt = _typed(data, bf16)
-        n, d = data.shape
         bp = BuildParams()
         lib().lb2_ivfpq_build_params_default(C.byref(bp))
-        keep = _fill_build_params(bp, params)
-        rid = None if row_ids is None else (row_ids if isinstance(row_ids, DeviceArray)
-                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
-        h = C.c_void_p()
-        st = BuildStats()
-        dp, _k1 = as_ptr(data)
-        rp, _k2 = as_ptr(rid)
-        check(lib().lb2_ivfpq_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt),
-                                    C.c_int(_metric(distance_type)), C.byref(bp), rp, C.byref(h),
-                                    C.byref(st)))
-        ix = cls(h, st)
-        ix._dt = dt
-        return ix
+        keep = _fill_build_params(bp, params or IvfBuildParams())  # noqa: F841 (alive across the build)
+        return _build(cls, lib().lb2_ivfpq_build, bp, data, distance_type, row_ids, bf16)
 
     @classmethod
     def from_parts(cls, centroids, codebook, part_ids, codes, row_ids=None, distance_type="l2", num_bits=8):
@@ -1193,29 +1208,11 @@ class IvfFlatIndex(IvfPqIndex):
     def build(cls, data, distance_type="l2", num_partitions=256, max_iters=50, sample_rate=256, seed=0,
               centroids=None, row_ids=None, partition_index="exact", partition_index_batch=1, bf16=False):
         """bf16=True: `data` is a uint16 array holding bfloat16 bit patterns (numpy has no bf16 dtype)."""
-        data, dt = _typed(data, bf16)
-        n, d = data.shape
         bp = FlatBuildParams()
         lib().lb2_ivfflat_build_params_default(C.byref(bp))
-        bp.num_partitions = num_partitions
-        bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed, bp.seed = max_iters, sample_rate, seed, seed
-        bp.ivf.partition_index = _pi_mode(partition_index)
-        bp.ivf.partition_index_batch = partition_index_batch
-        keep = None
-        if centroids is not None:
-            keep = _f32(centroids)
-            bp.ivf.init_centroids = as_ptr(keep)[0].value
-        rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
-                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
-        h = C.c_void_p()
-        st = BuildStats()
-        dp, _k1 = as_ptr(data)
-        rp, _k2 = as_ptr(rid)
-        check(lib().lb2_ivfflat_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt),
-                                      C.c_int(_metric(distance_type)), C.byref(bp), rp, C.byref(h), C.byref(st)))
-        ix = cls(h, st)
-        ix._dt = dt
-        return ix
+        keep = _ivf_fields(bp, num_partitions, max_iters, sample_rate, seed, centroids,  # noqa: F841
+                           partition_index, partition_index_batch)
+        return _build(cls, lib().lb2_ivfflat_build, bp, data, distance_type, row_ids, bf16)
 
     @classmethod
     def from_parts(cls, centroids, part_ids, vectors, row_ids=None, distance_type="l2", bf16=False):
@@ -1317,30 +1314,12 @@ class IvfSqIndex(IvfPqIndex):
         """create_index(.., "IVF_SQ"); the IVF stage equals IvfFlatIndex.build's with the same arguments.
         bf16=True: `data` is a uint16 array holding bfloat16 bit patterns."""
         sq_params = sq_params or SQBuildParams()
-        data, dt = _typed(data, bf16)
-        n, d = data.shape
         bp = _CSqBuildParams()
         lib().lb2_ivfsq_build_params_default(C.byref(bp))
-        bp.num_partitions = num_partitions
-        bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed, bp.seed = max_iters, sample_rate, seed, seed
-        bp.ivf.partition_index = _pi_mode(partition_index)
-        bp.ivf.partition_index_batch = partition_index_batch
+        keep = _ivf_fields(bp, num_partitions, max_iters, sample_rate, seed, centroids,  # noqa: F841
+                           partition_index, partition_index_batch)
         bp.num_bits, bp.sample_rate = sq_params.num_bits, sq_params.sample_rate
-        keep = None
-        if centroids is not None:
-            keep = _f32(centroids)
-            bp.ivf.init_centroids = as_ptr(keep)[0].value
-        rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
-                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
-        h = C.c_void_p()
-        st = BuildStats()
-        dp, _k1 = as_ptr(data)
-        rp, _k2 = as_ptr(rid)
-        check(lib().lb2_ivfsq_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt), C.c_int(_metric(distance_type)),
-                                    C.byref(bp), rp, C.byref(h), C.byref(st)))
-        ix = cls(h, st)
-        ix._dt = dt
-        return ix
+        return _build(cls, lib().lb2_ivfsq_build, bp, data, distance_type, row_ids, bf16)
 
     @classmethod
     def from_parts(cls, centroids, bounds, part_ids, codes, row_ids=None, distance_type="l2", dtype=np.float32,
@@ -1551,33 +1530,13 @@ class IvfHnswSqIndex(_HnswGraphs, IvfSqIndex):
         """create_index(.., "IVF_HNSW_SQ"); the IVF stage, bounds and codes equal IvfSqIndex.build's with the same
         arguments.  The graphs' level draws use `seed`."""
         sq_params = sq_params or SQBuildParams()
-        hnsw_params = hnsw_params or HnswBuildParams()
-        data, dt = _typed(data, bf16)
-        n, d = data.shape
         bp = _CHnswSqBuildParams()
         lib().lb2_ivfhnswsq_build_params_default(C.byref(bp))
-        bp.sq.num_partitions = num_partitions
-        bp.sq.ivf.max_iters, bp.sq.ivf.sample_rate, bp.sq.ivf.seed, bp.sq.seed = max_iters, sample_rate, seed, seed
-        bp.sq.ivf.partition_index = _pi_mode(partition_index)
-        bp.sq.ivf.partition_index_batch = partition_index_batch
+        keep = _ivf_fields(bp.sq, num_partitions, max_iters, sample_rate, seed, centroids,  # noqa: F841
+                           partition_index, partition_index_batch)
         bp.sq.num_bits, bp.sq.sample_rate = sq_params.num_bits, sq_params.sample_rate
-        bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
-        bp.insert_batch = hnsw_params.insert_batch
-        keep = None
-        if centroids is not None:
-            keep = _f32(centroids)
-            bp.sq.ivf.init_centroids = as_ptr(keep)[0].value
-        rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
-                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
-        h = C.c_void_p()
-        st = BuildStats()
-        dp, _k1 = as_ptr(data)
-        rp, _k2 = as_ptr(rid)
-        check(lib().lb2_ivfhnswsq_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt),
-                                        C.c_int(_metric(distance_type)), C.byref(bp), rp, C.byref(h), C.byref(st)))
-        ix = cls(h, st)
-        ix._dt = dt
-        return ix
+        _hnsw_fields(bp, hnsw_params)
+        return _build(cls, lib().lb2_ivfhnswsq_build, bp, data, distance_type, row_ids, bf16)
 
     _KIND = "sq"
 
@@ -1604,26 +1563,11 @@ class IvfHnswPqIndex(_HnswGraphs, IvfPqIndex):
     def build(cls, data, distance_type="l2", params=None, hnsw_params=HnswBuildParams(), row_ids=None, bf16=False):
         """create_index(.., "IVF_HNSW_PQ"); the IVF stage, codebook and codes equal IvfPqIndex.build's with the same
         arguments.  The graphs' level draws use params.seed."""
-        params = params or IvfBuildParams()
-        data, dt = _typed(data, bf16)
-        n, d = data.shape
         bp = _CHnswPqBuildParams()
         lib().lb2_ivfhnswpq_build_params_default(C.byref(bp))
-        keep = _fill_build_params(bp.pq, params)
-        bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
-        bp.insert_batch = hnsw_params.insert_batch
-        rid = None if row_ids is None else (row_ids if isinstance(row_ids, DeviceArray)
-                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
-        h = C.c_void_p()
-        st = BuildStats()
-        dp, _k1 = as_ptr(data)
-        rp, _k2 = as_ptr(rid)
-        check(lib().lb2_ivfhnswpq_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt),
-                                        C.c_int(_metric(distance_type)), C.byref(bp), rp, C.byref(h), C.byref(st)))
-        del keep
-        ix = cls(h, st)
-        ix._dt = dt
-        return ix
+        keep = _fill_build_params(bp.pq, params or IvfBuildParams())  # noqa: F841 (alive across the build)
+        _hnsw_fields(bp, hnsw_params)
+        return _build(cls, lib().lb2_ivfhnswpq_build, bp, data, distance_type, row_ids, bf16)
 
     @classmethod
     def from_parts(cls, centroids, codebook, part_ids, codes, row_ids=None, distance_type="l2", num_bits=8,
@@ -1665,33 +1609,12 @@ class IvfHnswFlatIndex(_HnswGraphs, IvfFlatIndex):
               centroids=None, row_ids=None, partition_index="exact", partition_index_batch=1, bf16=False, hnsw_params=None):
         """create_index(.., "IVF_HNSW_FLAT"); the IVF stage, vectors and row ids equal IvfFlatIndex.build's with the
         same arguments.  The graphs' level draws use `seed`.  bf16=True: uint16 bfloat16 bit patterns."""
-        hnsw_params = hnsw_params or HnswBuildParams()
-        data, dt = _typed(data, bf16)
-        n, d = data.shape
         bp = _CHnswFlatBuildParams()
         lib().lb2_ivfhnswflat_build_params_default(C.byref(bp))
-        f = bp.flat
-        f.num_partitions = num_partitions
-        f.ivf.max_iters, f.ivf.sample_rate, f.ivf.seed, f.seed = max_iters, sample_rate, seed, seed
-        f.ivf.partition_index = _pi_mode(partition_index)
-        f.ivf.partition_index_batch = partition_index_batch
-        bp.max_level, bp.m, bp.ef_construction = hnsw_params.max_level, hnsw_params.m, hnsw_params.ef_construction
-        bp.insert_batch = hnsw_params.insert_batch
-        keep = None
-        if centroids is not None:
-            keep = _f32(centroids)
-            bp.flat.ivf.init_centroids = as_ptr(keep)[0].value
-        rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
-                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
-        h = C.c_void_p()
-        st = BuildStats()
-        dp, _k1 = as_ptr(data)
-        rp, _k2 = as_ptr(rid)
-        check(lib().lb2_ivfhnswflat_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt),
-                                          C.c_int(_metric(distance_type)), C.byref(bp), rp, C.byref(h), C.byref(st)))
-        ix = cls(h, st)
-        ix._dt = dt
-        return ix
+        keep = _ivf_fields(bp.flat, num_partitions, max_iters, sample_rate, seed, centroids,  # noqa: F841
+                           partition_index, partition_index_batch)
+        _hnsw_fields(bp, hnsw_params)
+        return _build(cls, lib().lb2_ivfhnswflat_build, bp, data, distance_type, row_ids, bf16)
 
     @classmethod
     def from_parts(cls, centroids, part_ids, vectors, row_ids=None, distance_type="l2", bf16=False, graph=None):
@@ -1757,31 +1680,12 @@ class IvfRqIndex(IvfPqIndex):
               centroids=None, row_ids=None, partition_index="exact", partition_index_batch=1, rq_params=None):
         """create_index(.., "IVF_RQ"); the IVF stage equals IvfFlatIndex.build's with the same arguments, the
         rotation is drawn from seed + 1.  f32 columns."""
-        rq_params = rq_params or RQBuildParams()
-        data, dt = _typed(data)
-        n, d = data.shape
         bp = _CRqBuildParams()
         lib().lb2_ivfrq_build_params_default(C.byref(bp))
-        bp.num_partitions = num_partitions
-        bp.ivf.max_iters, bp.ivf.sample_rate, bp.ivf.seed, bp.seed = max_iters, sample_rate, seed, seed
-        bp.ivf.partition_index = _pi_mode(partition_index)
-        bp.ivf.partition_index_batch = partition_index_batch
-        bp.num_bits = rq_params.num_bits
-        keep = None
-        if centroids is not None:
-            keep = _f32(centroids)
-            bp.ivf.init_centroids = as_ptr(keep)[0].value
-        rid = None if row_ids is None else (row_ids if isinstance(row_ids, (DeviceArray, PinnedArray))
-                                            else np.ascontiguousarray(row_ids, dtype=np.uint64))
-        h = C.c_void_p()
-        st = BuildStats()
-        dp, _k1 = as_ptr(data)
-        rp, _k2 = as_ptr(rid)
-        check(lib().lb2_ivfrq_build(dp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt), C.c_int(_metric(distance_type)),
-                                    C.byref(bp), rp, C.byref(h), C.byref(st)))
-        ix = cls(h, st)
-        ix._dt = dt
-        return ix
+        keep = _ivf_fields(bp, num_partitions, max_iters, sample_rate, seed, centroids,  # noqa: F841
+                           partition_index, partition_index_batch)
+        bp.num_bits = (rq_params or RQBuildParams()).num_bits
+        return _build(cls, lib().lb2_ivfrq_build, bp, data, distance_type, row_ids)
 
     @classmethod
     def from_parts(cls, centroids, rotation, part_ids, codes, add_factors, scale_factors, row_ids=None,

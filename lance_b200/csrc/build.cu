@@ -152,7 +152,7 @@ void train_ivf(const float* xs, uint64_t s, int d, int K, int am, const lb2_kmea
 }
 }  // namespace
 
-// The IVF stage of every build, in two halves so that IVF_PQ can gather its own sample in between:
+// The IVF stage of every build, in two halves so that IVF_PQ can gather its own sample in between (build_index):
 // (a) the IVF training sample's rows (ivf.rs:1237-1241), to be gathered with gather_finite_sample (rows that are not
 // finite dropped, normalised first under cosine);
 static std::vector<uint64_t> ivf_sample_rows(uint64_t n, int K, const lb2_kmeans_params& kp, uint64_t seed) {
@@ -171,46 +171,13 @@ static void train_ivf_model(const float* sample, uint64_t s, lb2_index* ix, cons
             iters);
   round_model(ix->centroids.p, (size_t)K * d, ix->dtype);
 }
-// both halves, with the bulk copy started in between (IVF_FLAT, IVF_SQ, IVF_RQ)
-static void train_ivf_stage(Source& src, lb2_index* ix, const lb2_kmeans_params& kp, uint64_t seed,
-                            std::vector<double>* loss, std::vector<uint32_t>* iters) {
-  TagScope tg("ivf_train");
-  std::vector<uint64_t> rows = ivf_sample_rows(src.n(), ix->K, kp, seed);
-  DevBuf<float> sample;
-  const uint64_t s = gather_finite_sample(src, rows, ix->metric == METRIC_COSINE, sample);
-  src.start_resident_copy();  // host rows: the bulk copy runs on its own stream while the centroids train
-  train_ivf_model(sample.p, s, ix, kp, loss, iters);
-}
-
-// the stage times of a build from its events: start, IVF trained, [quantizer trained,] transformed, grouped (IVF_FLAT
-// has no quantizer stage: 4 events, ms_pq_train 0)
-// the build's partition rule from its IVF parameters (lb2_kmeans_params.partition_index): recorded on ix, with the
-// graph over the trained centroids when the mode resolves to one; the graph's levels draw from partition_index_seed
-static void attach_partition_index(lb2_index* ix, const lb2_kmeans_params& kp, uint64_t seed) {
-  set_partition_index(ix, kp.partition_index, partition_index_seed(seed), kp.partition_index_batch);
-}
-
-static void fill_stats(lb2_build_stats* stats, const EventSet& ev, const std::vector<double>& loss,
-                       const std::vector<uint32_t>& iters, const std::vector<uint32_t>& pq_iters = {}) {
-  if (!stats) return;
-  memset(stats, 0, sizeof(*stats));
-  const int q = (int)ev.ev.size() - 4;
-  stats->ms_ivf_train = ev.ms(0, 1);
-  if (q) stats->ms_pq_train = ev.ms(1, 2);
-  stats->ms_transform = ev.ms(1 + q, 2 + q);
-  stats->ms_group = ev.ms(2 + q, 3 + q);
-  stats->ms_total = ev.ms(0, 3 + q);
-  stats->ivf_iters = iters.empty() ? 0 : iters[0];
-  for (auto v : pq_iters) stats->pq_iters_max = std::max(stats->pq_iters_max, v);
-  stats->ivf_loss = loss.empty() ? 0.0 : loss[0];
-}
-
 // IvfTransformer's partition step over one chunk of rows (ivf.rs:158-166): normalised first under cosine, then
-// assigned (by dot or L2) from f32, or from the rows' own type (xnat / dtype, for_each_chunk) when not normalised.
-// Returns the chunk as the index sees it.  pi (nullable): the index's partition index, which assigns instead.
-static const float* normalize_assign(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
-                                     const float* cent, int K, DevBuf<float>& normbuf, uint32_t* part, uint8_t* valid,
-                                     float* dist, const lb2_partition_index* pi = nullptr) {
+// assigned through the index's partition rule -- its partition index when it has one (PartitionTransformer's graph
+// arm, ivf/transform.rs:112-124), else the exact scan (by dot or L2) from f32, or from the rows' own type (xnat /
+// dtype, for_each_chunk) when not normalised.  Returns the chunk as the index sees it.
+static const float* normalize_assign(const lb2_index& ix, const float* xf, const void* xnat, int dtype, uint64_t rows,
+                                     DevBuf<float>& normbuf, uint32_t* part, uint8_t* valid, float* dist) {
+  const int d = ix.d, m = ix.metric;
   const float* xp = xf;
   if (m == METRIC_COSINE) {
     if (normbuf.n < (size_t)rows * d) normbuf.alloc((size_t)rows * d);
@@ -218,10 +185,11 @@ static const float* normalize_assign(const float* xf, const void* xnat, int dtyp
     xp = normbuf.p;
     xnat = nullptr;
   }
-  if (pi)  // the partition index over these centroids (PartitionTransformer's graph arm, ivf/transform.rs:112-124)
-    partition_index_assign(*pi, xp, rows, part, dist, valid);
+  if (ix.pidx)
+    partition_index_assign(*ix.pidx, xp, rows, part, dist, valid);
   else
-    assign_f32(xp, rows, d, cent, K, m == METRIC_DOT ? METRIC_DOT : METRIC_L2, nullptr, part, dist, valid, xnat, dtype);
+    assign_f32(xp, rows, d, ix.centroids.p, ix.K, m == METRIC_DOT ? METRIC_DOT : METRIC_L2, nullptr, part, dist, valid,
+               xnat, dtype);
   return xp;
 }
 
@@ -230,13 +198,14 @@ static const float* normalize_assign(const float* xf, const void* xnat, int dtyp
 // trained -- and therefore encodes -- with L2 whatever the index metric is: Q::build(&training_data,
 // DistanceType::L2, ..) (rust/lance/src/index/vector/builder.rs:460); the index metric only decides the partition
 // assignment, whether residuals are taken (not for dot, PQBuildParams::use_residual) and the query-time table.
-static void transform_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m, const float* cent,
-                            int K, const float* codebook, int M, int nbits, DevBuf<float>& normbuf, uint32_t* part,
-                            uint8_t* codes, uint8_t* valid, const lb2_partition_index* pi = nullptr) {
-  const float* xp = normalize_assign(xf, xnat, dtype, rows, d, m, cent, K, normbuf, part, valid, nullptr, pi);
-  const bool dot = m == METRIC_DOT;
-  pq_encode_any(xp, rows, d, M, d / M, codebook, METRIC_L2, dot ? nullptr : cent, dot ? nullptr : part, valid, nbits,
-                codes);
+// res_part (nullable): the partitions the residuals are taken to instead of the assigned ones.
+static void transform_chunk(const lb2_index& ix, const float* xf, const void* xnat, int dtype, uint64_t rows,
+                            DevBuf<float>& normbuf, uint32_t* part, uint8_t* codes, uint8_t* valid,
+                            const uint32_t* res_part) {
+  const float* xp = normalize_assign(ix, xf, xnat, dtype, rows, normbuf, part, valid, nullptr);
+  const bool dot = ix.metric == METRIC_DOT;
+  pq_encode_any(xp, rows, ix.d, ix.M, ix.d / ix.M, ix.codebook.p, METRIC_L2, dot ? nullptr : ix.centroids.p,
+                dot ? nullptr : (res_part ? res_part : part), valid, ix.nbits, codes);
 }
 
 // partition assignment of one chunk of rows (IVF_FLAT / IVF_SQ / IVF_RQ transform); returns the chunk as f32 as the
@@ -244,13 +213,11 @@ static void transform_chunk(const float* xf, const void* xnat, int dtype, uint64
 // (KeepFiniteVectors precedes the partition transform, ivf.rs:166, 256, 299).  Under L2 and cosine such a row has
 // no finite distance and the assignment already drops it; under dot a +-inf element can still give a -inf best
 // distance, so the elements are checked.
-static const float* assign_flat_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
-                                      const float* cent, int K, DevBuf<float>& normbuf, uint32_t* part,
-                                      uint8_t* valid, float* dist = nullptr,
-                                      const lb2_partition_index* pi = nullptr) {
-  const float* xp = normalize_assign(xf, xnat, dtype, rows, d, m, cent, K, normbuf, part, valid, dist, pi);
-  if (m == METRIC_DOT && rows)
-    LB2_LAUNCH("drop_nonfinite_rows", finite_rows_kernel, cdiv(rows * 32, 256), 256, 0, xp, rows, d, valid, 1);
+static const float* assign_flat_chunk(const lb2_index& ix, const float* xf, const void* xnat, int dtype, uint64_t rows,
+                                      DevBuf<float>& normbuf, uint32_t* part, uint8_t* valid, float* dist) {
+  const float* xp = normalize_assign(ix, xf, xnat, dtype, rows, normbuf, part, valid, dist);
+  if (ix.metric == METRIC_DOT && rows)
+    LB2_LAUNCH("drop_nonfinite_rows", finite_rows_kernel, cdiv(rows * 32, 256), 256, 0, xp, rows, ix.d, valid, 1);
   return xp;
 }
 
@@ -278,103 +245,320 @@ void rq_check(uint32_t d, lb2_dtype dtype, uint32_t num_bits) {
 // IVF_RQ transform of one chunk (IvfTransformer::with_rq, ivf.rs:281-328): [normalise] -> partition and dist_v_c ->
 // residual -> rotation -> sign codes and factors.  Cosine is L2 on the normalised rows from there on.
 // The row chunk is bounded by d (Source::rows_per_chunk), the rotated rows by code_dim = d * num_bits: they are
-// rotated and encoded in sub-chunks of at most 2^28 / code_dim rows (1 GB of f32).
+// rotated and encoded in sub-chunks of at most 2^28 / code_dim rows (1 GB of f32).  cnorm: |c|^2 per centroid
+// (norm_squared_fsl, RQTransformer::new, bq/transform.rs:42-59), dot only.
 struct RqWork {
-  DevBuf<float> normbuf, dist, res, rot;
+  DevBuf<float> normbuf, dist, res, rot, cnorm;
 };
-static void rq_transform_chunk(const float* xf, const void* xnat, int dtype, uint64_t rows, int d, int m,
-                               const float* cent, int K, const float* rotation, int num_bits, const float* cnorm,
-                               RqWork& w, uint32_t* part, uint8_t* valid, uint8_t* codes, float* add, float* scale,
-                               const lb2_partition_index* pi = nullptr) {
-  const int cd = d * num_bits;
+static void rq_transform_chunk(const lb2_index& ix, const float* xf, const void* xnat, int dtype, uint64_t rows,
+                               RqWork& w, uint32_t* part, uint8_t* valid, uint8_t* codes, float* add, float* scale) {
+  const int d = ix.d, cd = ix.code_dim();
   const uint64_t sub = std::min<uint64_t>(rows, std::max<uint64_t>(1, (1ull << 28) / (uint64_t)cd));
   if (w.dist.n < rows) w.dist.alloc(rows);
   if (w.res.n < rows * d) w.res.alloc(rows * d);
   if (w.rot.n < sub * cd) w.rot.alloc(sub * cd);
-  const float* xs = assign_flat_chunk(xf, xnat, dtype, rows, d, m, cent, K, w.normbuf, part, valid, w.dist.p, pi);
-  rq_residual_f32(xs, rows, d, cent, part, valid, w.res.p);
+  const float* xs = assign_flat_chunk(ix, xf, xnat, dtype, rows, w.normbuf, part, valid, w.dist.p);
+  rq_residual_f32(xs, rows, d, ix.centroids.p, part, valid, w.res.p);
   for (uint64_t r0 = 0; r0 < rows; r0 += sub) {
     const uint64_t rs = std::min(sub, rows - r0);
-    rq_rotate_f32(rotation, cd, d, w.res.p + r0 * d, rs, w.rot.p);
-    rq_encode_f32(w.rot.p, w.res.p + r0 * d, w.dist.p + r0, part + r0, cnorm, valid + r0, rs, d, num_bits,
-                  m == METRIC_DOT ? METRIC_DOT : METRIC_L2, codes + r0 * (cd / 8), add + r0, scale + r0);
+    rq_rotate_f32(ix.rq_rot.p, cd, d, w.res.p + r0 * d, rs, w.rot.p);
+    rq_encode_f32(w.rot.p, w.res.p + r0 * d, w.dist.p + r0, part + r0, w.cnorm.p, valid + r0, rs, d, ix.nbits,
+                  ix.metric == METRIC_DOT ? METRIC_DOT : METRIC_L2, codes + r0 * (cd / 8), add + r0, scale + r0);
   }
 }
 
-// |c|^2 per centroid (norm_squared_fsl, RQTransformer::new, bq/transform.rs:42-59): dot only
-static void rq_centroid_norms(int metric, const float* cent, int K, int d, DevBuf<float>& out) {
-  if (metric != METRIC_DOT) return;
-  out.alloc(K);
-  rq_norm_sq_f32(cent, K, d, out.p);
-}
-
-// lb2_index_transform's rows (every output nullable).  given_part (nullable, device): the partition of every row is
-// given (a split's decisions, build_assign_batch's PART_ID column, builder.rs:1534-1650): IVF_PQ takes its residuals
-// to it; the other kinds store the same payload whatever the partition, and part_out still gets the nearest centroid.
+// The transform of every row of `src` with the model and partition rule of `index`, chunk by chunk: the builds' full
+// pass, lb2_index_transform, the stand-alone IVF_PQ / IVF_RQ transforms and a split's moved rows.  Every output is
+// nullable: a NULL part_out, valid_out, add_out / scale_out (IVF_RQ) or payload_out gets scratch, except IVF_FLAT's
+// payload, whose stored rows are then not converted (a build groups them from `src` again, index_load_flat_src).
+// Synchronises only when it allocated scratch.  given_part (nullable, device): the partition of every row is given
+// (a split's decisions, build_assign_batch's PART_ID column, builder.rs:1534-1650): IVF_PQ takes its residuals to it;
+// the other kinds store the same payload whatever the partition, and part_out still gets the assigned partition.
 void index_transform_rows(const lb2_index* index, Source& src, const uint32_t* given_part, uint32_t* part_out,
                           uint8_t* payload_out, float* add_out, float* scale_out, uint8_t* valid_out) {
   const uint64_t n = src.n();
   const bool rq = index->kind == IndexKind::RQ;
-  const int d = index->d, m = index->metric, K = index->K;
+  const int d = index->d;
   const size_t rb = index->row_bytes();
-  const float* cent = index->centroids.p;
-  const lb2_partition_index* pi = index->pidx.get();  // the index's partition rule (null: the exact scan)
-  // every output the chunk functions write is needed: the caller's NULLs get scratch
   DevBuf<uint32_t> ptmp;
   DevBuf<uint8_t> vtmp, ltmp;
   DevBuf<float> atmp, stmp;
-  uint32_t* pp = part_out;
-  uint8_t *vp = valid_out, *lp = payload_out;
-  float *ap = add_out, *sp = scale_out;
-  if (!pp) { ptmp.alloc(std::max<uint64_t>(n, 1)); pp = ptmp.p; }
-  if (!vp) { vtmp.alloc(std::max<uint64_t>(n, 1)); vp = vtmp.p; }
-  if (!lp) { ltmp.alloc(std::max<uint64_t>(n * rb, 1)); lp = ltmp.p; }
-  if (rq && !ap) { atmp.alloc(std::max<uint64_t>(n, 1)); ap = atmp.p; }
-  if (rq && !sp) { stmp.alloc(std::max<uint64_t>(n, 1)); sp = stmp.p; }
+  bool scratch = false;
+  auto need = [&](auto& buf, auto*& p, uint64_t count) {
+    if (p) return;
+    buf.alloc(std::max<uint64_t>(count, 1));
+    p = buf.p;
+    scratch = true;
+  };
+  need(ptmp, part_out, n);
+  need(vtmp, valid_out, n);
+  if (index->kind != IndexKind::FLAT) need(ltmp, payload_out, n * rb);
+  if (rq) {
+    need(atmp, add_out, n);
+    need(stmp, scale_out, n);
+  }
   if (n) {
     src.start_resident_copy();
     const int sdt = (int)src.dtype();
-    DevBuf<float> normbuf, cnorm;
     RqWork w;
-    if (rq) rq_centroid_norms(m, cent, K, d, cnorm);
+    if (rq && index->metric == METRIC_DOT) {
+      w.cnorm.alloc(index->K);
+      rq_norm_sq_f32(index->centroids.p, index->K, d, w.cnorm.p);
+    }
     for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
-      uint8_t* out = lp + r0 * rb;
+      uint32_t* part = part_out + r0;
+      uint8_t* valid = valid_out + r0;
       switch (index->kind) {
-        case IndexKind::PQ:  // lb2_ivfpq_transform's rows
-          if (given_part) {
-            const float* xp = normalize_assign(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0, nullptr, pi);
-            const bool dot = m == METRIC_DOT;
-            pq_encode_any(xp, rows, d, index->M, d / index->M, index->codebook.p, METRIC_L2, dot ? nullptr : cent,
-                          dot ? nullptr : given_part + r0, vp + r0, index->nbits, out);
-          } else {
-            transform_chunk(xf, xnat, sdt, rows, d, m, cent, K, index->codebook.p, index->M, index->nbits, normbuf,
-                            pp + r0, out, vp + r0, pi);
-          }
+        case IndexKind::PQ:
+          transform_chunk(*index, xf, xnat, sdt, rows, w.normbuf, part, payload_out + r0 * rb, valid,
+                          given_part ? given_part + r0 : nullptr);
           break;
-        case IndexKind::RQ:  // lb2_ivfrq_transform's rows
-          rq_transform_chunk(xf, xnat, sdt, rows, d, m, cent, K, index->rq_rot.p, index->nbits, cnorm.p, w, pp + r0,
-                             vp + r0, out, ap + r0, sp + r0, pi);
+        case IndexKind::RQ:
+          rq_transform_chunk(*index, xf, xnat, sdt, rows, w, part, valid, payload_out + r0 * rb, add_out + r0,
+                             scale_out + r0);
           break;
-        case IndexKind::SQ: {  // lb2_ivfsq_build's codes
-          const float* xs = assign_flat_chunk(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0, nullptr, pi);
-          if (m == METRIC_COSINE) round_model(normbuf.p, (size_t)rows * d, index->dtype);
-          sq_encode_f32(xs, (uint64_t)rows * d, index->sq_lower, index->sq_upper, out);
+        case IndexKind::SQ: {  // the SQ codes of the stored vectors themselves
+          const float* xs = assign_flat_chunk(*index, xf, xnat, sdt, rows, w.normbuf, part, valid, nullptr);
+          if (index->metric == METRIC_COSINE)  // as IVF_FLAT stores them
+            round_model(w.normbuf.p, (size_t)rows * d, index->dtype);
+          sq_encode_f32(xs, (uint64_t)rows * d, index->sq_lower, index->sq_upper, payload_out + r0 * rb);
           break;
         }
         case IndexKind::FLAT: {  // index_load_flat_src's stored rows: (normalised) f32 in the stored element type
-          const float* xs = assign_flat_chunk(xf, xnat, sdt, rows, d, m, cent, K, normbuf, pp + r0, vp + r0, nullptr, pi);
+          const float* xs = assign_flat_chunk(*index, xf, xnat, sdt, rows, w.normbuf, part, valid, nullptr);
+          if (!payload_out) break;
           const lb2_dtype vdt = index->vdtype();
           if (vdt == LB2_F32)
-            d2d(reinterpret_cast<float*>(out), xs, (size_t)rows * d);
+            d2d(reinterpret_cast<float*>(payload_out + r0 * rb), xs, (size_t)rows * d);
           else
             LB2_LAUNCH("convert_from_f32", from_f32_kernel, cdiv(rows * d, 256), 256, 0, xs, (int)vdt, (size_t)rows * d,
-                       (void*)out);
+                       (void*)(payload_out + r0 * rb));
           break;
         }
       }
     });
   }
-  sync_stream();  // the scratch outputs are freed on return
+  if (scratch) sync_stream();  // the scratch outputs are freed on return
+}
+
+// IVF_PQ's IVF stage, gathering its own sample before the bulk copy starts.  Staging (class Source): device rows are used in place.  Host rows:
+// both training samples (<= K * 256 and 65 536 rows) are gathered straight out of the caller's memory (zero-copy
+// reads over PCIe when it is pinned), then the matrix is copied ONCE, in its own element type, on a second stream
+// while both trainings run; the per-row pass waits for it and converts one chunk of rows at a time.  A matrix too
+// large for that is streamed chunk by chunk during the per-row pass instead (double buffered).  No whole-matrix f32
+// copy exists.  Returns the PQ sample (256*2^nbits rows, builder.rs:410-421; normalised for cosine, rows that are
+// not finite dropped, builder.rs:436) in sample_pq.
+static uint64_t stage_ivf_pq(Source& src, lb2_index* ix, const lb2_kmeans_params& kp, const lb2_pq_params& pq,
+                             uint64_t seed, DevBuf<float>& sample_pq, std::vector<double>* loss,
+                             std::vector<uint32_t>* iters) {
+  const uint64_t n = src.n();
+  const int m = ix->metric, d = ix->d;
+  const uint64_t nranks = comm_nranks();  // sharded build: this rank's rows
+  const uint64_t s_pq0 = std::min<uint64_t>(n, (pq.sample_rate * ((uint64_t)1 << ix->nbits) + nranks - 1) / nranks);
+  DevBuf<float> sample_ivf;
+  uint64_t s_ivf = 0, s_pq = 0;
+  std::vector<uint64_t> rows_pq;
+  bool pq_deferred = false;
+  // LB2_TRACE_BUILD=1: host wall-clock stamps of the staging steps on stderr (diagnostics; adds synchronisations)
+  static const bool trace = getenv("LB2_TRACE_BUILD") && *getenv("LB2_TRACE_BUILD");
+  const auto tr0 = std::chrono::steady_clock::now();
+  auto stamp = [&](const char* what) {
+    if (!trace) return;
+    sync_stream();
+    fprintf(stderr, "[lb2 build] %-22s +%.3f ms\n", what,
+            std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tr0).count());
+  };
+  {
+    std::vector<uint64_t> rows = ivf_sample_rows(n, ix->K, kp, seed);
+    stamp("sample_rows(ivf)");
+    s_ivf = gather_finite_sample(src, rows, m == METRIC_COSINE, sample_ivf);
+    stamp("gather(ivf sample)");
+    rows_pq = sample_rows(n, s_pq0, seed + 1);
+    // the PQ sample is not needed before the IVF model exists: from pinned f32 rows it is gathered on the copy
+    // stream (in front of the bulk copy) while the IVF training runs; otherwise here
+    if (m != METRIC_COSINE && !trace && !rows_pq.empty()) {
+      sample_pq.alloc(rows_pq.size() * (uint64_t)d);
+      pq_deferred = src.gather_f32_async(rows_pq, sample_pq.p);
+    }
+    if (!pq_deferred) {
+      s_pq = gather_finite_sample(src, rows_pq, m == METRIC_COSINE, sample_pq);
+      stamp("gather(pq sample)");
+    }
+  }
+  src.start_resident_copy();
+  if (trace) fprintf(stderr, "[lb2 build] %-22s +%.3f ms (host, no sync)\n", "bulk copy issued",
+                     std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tr0).count());
+  train_ivf_model(sample_ivf.p, s_ivf, ix, kp, loss, iters);
+  stamp("ivf trained");
+  if (pq_deferred) {
+    if (src.finish_async_sample()) {
+      s_pq = rows_pq.size();
+    } else {  // rare: some sampled rows are not finite -> the synchronous path drops them and gathers again
+      s_pq = gather_finite_sample(src, rows_pq, false, sample_pq);
+    }
+  }
+  return s_pq;
+}
+
+// a build's quantizer parameters: nbits (IVF_SQ, IVF_RQ, IVF_PQ), the IVF_SQ bounds' sample_rate, IVF_PQ's parameters
+struct QuantizerParams {
+  uint32_t nbits = 0;
+  uint64_t sample_rate = 0;
+  const lb2_pq_params* pq = nullptr;
+};
+
+// IvfIndexBuilder::build (builder.rs:236) of every kind, its arguments checked: 1. the IVF stage; 2. the quantizer
+// (none for IVF_FLAT); 3. every row transformed through the index's partition rule; 4. the kept rows grouped by
+// partition.  stats: the time between the stages' events.
+static void build_index(IndexKind kind, const void* data, uint64_t n, uint32_t d, lb2_dtype dtype, int m, uint32_t K,
+                        const lb2_kmeans_params& kp, uint64_t seed, const QuantizerParams& q, const uint64_t* row_ids,
+                        lb2_index** out, lb2_build_stats* stats) {
+  const bool flat = kind == IndexKind::FLAT;
+  const int q1 = flat ? 0 : 1;  // the quantizer stage's event
+  EventSet ev(4 + q1);
+  ev.record(0);
+  // (declared before `src`: on an error path ~Source waits for the copy stream, which may still be writing IVF_PQ's
+  // deferred sample, before the buffer goes back to the pool)
+  DevBuf<float> sample_pq;
+  Source src(data, n, (int)d, dtype);
+  std::unique_ptr<lb2_index> ix = make_index(kind, K, d, m, dtype);
+  ix->nbits = (int)q.nbits;
+  std::vector<double> loss;
+  std::vector<uint32_t> iters, pq_iters;
+  // 1. IVF: the same sample, seed and training for every kind
+  uint64_t s_pq = 0;
+  if (kind == IndexKind::PQ) {
+    ix->M = q.pq->num_sub_vectors;
+    ix->codebook.alloc(ix->codebook_len());
+    s_pq = stage_ivf_pq(src, ix.get(), kp, *q.pq, seed, sample_pq, &loss, &iters);
+  } else {
+    TagScope tg("ivf_train");
+    std::vector<uint64_t> rows = ivf_sample_rows(n, K, kp, seed);
+    DevBuf<float> sample;
+    const uint64_t s = gather_finite_sample(src, rows, m == METRIC_COSINE, sample);
+    src.start_resident_copy();  // host rows: the bulk copy runs on its own stream while the centroids train
+    train_ivf_model(sample.p, s, ix.get(), kp, &loss, &iters);
+  }
+  ev.record(1);
+  // 2. the quantizer
+  switch (kind) {
+    case IndexKind::FLAT:
+      break;
+    case IndexKind::SQ: {
+      // ScalarQuantizer::build (sq.rs:152-182) on sample_rate * 2^num_bits rows (builder.rs:410-421), normalised under
+      // cosine, rows that are not finite dropped (builder.rs:436), no residuals (quantizer.rs:52).  The bounds are
+      // taken over the values the index stores: normalised, in the column's element type.
+      TagScope tg("sq_train");
+      std::vector<uint64_t> rows = sample_rows(n, std::min<uint64_t>(n, q.sample_rate * 256), seed + 1);
+      DevBuf<float> sample;
+      const uint64_t s = gather_finite_sample(src, rows, m == METRIC_COSINE, sample);
+      round_model(sample.p, (size_t)s * d, dtype);
+      sq_bounds_f32(sample.p, (uint64_t)s * d, &ix->sq_lower, &ix->sq_upper);
+      break;
+    }
+    case IndexKind::RQ: {  // RabitQuantizer::new (bq/builder.rs:52-70): the rotation, from seed + 1
+      TagScope tg("rq_train");
+      const int cd = ix->code_dim();
+      ix->rq_rot.alloc((size_t)cd * cd);
+      rq_rotation_f32(cd, seed + 1, ix->rq_rot.p);
+      break;
+    }
+    case IndexKind::PQ: {  // residuals of its sample w.r.t. the IVF centroids (builder.rs:439-450)
+      TagScope tg("pq_train");
+      if (m != METRIC_DOT && s_pq) {
+        DevBuf<uint32_t> part(s_pq);
+        assign_f32(sample_pq.p, s_pq, d, ix->centroids.p, K, METRIC_L2, nullptr, part.p, nullptr, nullptr);
+        LB2_LAUNCH("residual", residual_kernel, cdiv(s_pq * d, 256), 256, 0, sample_pq.p, ix->centroids.p, part.p, s_pq,
+                   (int)d, sample_pq.p);
+      }
+      VecIn cb_init(q.pq->codebook, ix->codebook_len(), model_dtype(dtype));
+      lb2_pq_params pqp = *q.pq;
+      pqp.codebook = cb_init.get();
+      // always L2 k-means (builder.rs:460: Q::build(&training_data, DistanceType::L2, ..)); for a dot index the sample
+      // is the raw vectors (no residual), for L2 / cosine the residuals computed above
+      pq_train_dev(sample_pq.p, s_pq, d, METRIC_L2, &pqp, ix->codebook.p, &pq_iters);
+      round_model(ix->codebook.p, ix->codebook_len(), dtype);
+      sample_pq.release();
+      break;
+    }
+  }
+  if (q1) ev.record(2);
+  // 3. transform (ivf.rs:188-328): IVF_FLAT keeps the partitions only, index_load_flat_src gathers its rows again
+  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
+  DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1)), payload;
+  DevBuf<float> add, scale;
+  if (!flat) payload.alloc(std::max<uint64_t>(1, n * ix->row_bytes()));
+  if (kind == IndexKind::RQ) {
+    add.alloc(std::max<uint64_t>(n, 1));
+    scale.alloc(std::max<uint64_t>(n, 1));
+  }
+  {
+    TagScope tg("transform");
+    set_partition_index(ix.get(), kp.partition_index, partition_index_seed(seed), kp.partition_index_batch);
+    index_transform_rows(ix.get(), src, nullptr, part.p, payload.p, add.p, scale.p, valid.p);
+  }
+  ev.record(2 + q1);
+  {
+    // 4. group the kept rows by partition (shuffle + build_partitions, builder.rs:501-937); rows the transform marked
+    //    invalid are dropped, as KeepFiniteVectors does (transform.rs:112-159)
+    TagScope tg("group");
+    InArg<uint64_t> rid(row_ids, n);
+    if (flat)  // the stored vectors are the normalised ones when the metric is cosine
+      index_load_flat_src(ix.get(), part.p, src, rid.get(), valid.p, m == METRIC_COSINE);
+    else
+      index_load_dev(ix.get(), part.p, payload.p, rid.get(), n, valid.p, add.p, scale.p);
+  }
+  ev.record(3 + q1);
+  sync_stream();
+  if (stats) {
+    memset(stats, 0, sizeof(*stats));
+    stats->ms_ivf_train = ev.ms(0, 1);
+    if (q1) stats->ms_pq_train = ev.ms(1, 2);
+    stats->ms_transform = ev.ms(1 + q1, 2 + q1);
+    stats->ms_group = ev.ms(2 + q1, 3 + q1);
+    stats->ms_total = ev.ms(0, 3 + q1);
+    stats->ivf_iters = iters.empty() ? 0 : iters[0];
+    for (auto v : pq_iters) stats->pq_iters_max = std::max(stats->pq_iters_max, v);
+    stats->ivf_loss = loss.empty() ? 0.0 : loss[0];
+  }
+  *out = ix.release();
+}
+
+// the defaults of every build's IVF fields (IvfBuildParams, ivf/builder.rs:62-78; balance factor 1,
+// rust/lance/src/index/vector/ivf.rs:1858) and of an HNSW build's graph (HnswBuildParams::default,
+// hnsw/builder.rs:63-72, inserted serially)
+template <class P>
+static void ivf_defaults(P* p) {
+  p->num_partitions = 256;
+  lb2_kmeans_params_default(&p->ivf);
+  p->ivf.balance_factor = 1.0f;
+  p->seed = 0;
+}
+template <class P>
+static void hnsw_defaults(P* p) {
+  p->max_level = 7;
+  p->m = 20;
+  p->ef_construction = 150;
+  p->insert_batch = 1;
+}
+
+// lb2_index_transform's rows into the caller's buffers (host or device, each nullable)
+static void transform_into(const lb2_index* ix, const void* vectors, uint64_t n, uint32_t* part_out,
+                           uint8_t* payload_out, float* add_out, float* scale_out, uint8_t* valid_out) {
+  OutArg<uint32_t> po(part_out, n);
+  OutArg<uint8_t> pl(payload_out, (size_t)n * ix->row_bytes()), vo(valid_out, n);
+  OutArg<float> ao(add_out, n), so(scale_out, n);
+  if (n) {
+    Source src(vectors, n, ix->d, ix->dtype);
+    index_transform_rows(ix, src, nullptr, po.get(), pl.get(), ao.get(), so.get(), vo.get());
+  }
+  po.commit(); pl.commit(); vo.commit(); ao.commit(); so.commit();
+  sync_stream();
+}
+// the stand-alone transforms run on a handle holding the caller's model as it is (never rounded to the column's type)
+static void copy_in(float* to, const void* from, size_t count, lb2_dtype dt) {
+  VecIn v(from, count, dt);
+  d2d(to, v.get(), count);
 }
 
 }  // namespace lb2
@@ -384,59 +568,36 @@ using namespace lb2;
 extern "C" {
 
 void lb2_ivfpq_build_params_default(lb2_ivfpq_build_params* p) {
-  p->num_partitions = 256;
-  lb2_kmeans_params_default(&p->ivf);
-  p->ivf.balance_factor = 1.0f;  // rust/lance/src/index/vector/ivf.rs:1858
+  ivf_defaults(p);
   lb2_pq_params_default(&p->pq);
-  p->seed = 0;
 }
 
-void lb2_ivfflat_build_params_default(lb2_ivfflat_build_params* p) {
-  p->num_partitions = 256;
-  lb2_kmeans_params_default(&p->ivf);
-  p->ivf.balance_factor = 1.0f;
-  p->seed = 0;
-}
+void lb2_ivfflat_build_params_default(lb2_ivfflat_build_params* p) { ivf_defaults(p); }
 
 void lb2_ivfsq_build_params_default(lb2_ivfsq_build_params* p) {
-  p->num_partitions = 256;
-  lb2_kmeans_params_default(&p->ivf);
-  p->ivf.balance_factor = 1.0f;
+  ivf_defaults(p);
   p->num_bits = 8;
   p->sample_rate = 256;
-  p->seed = 0;
 }
 
 void lb2_ivfhnswsq_build_params_default(lb2_ivfhnswsq_build_params* p) {
   lb2_ivfsq_build_params_default(&p->sq);
-  p->max_level = 7;  // HnswBuildParams::default (hnsw/builder.rs:63-72)
-  p->m = 20;
-  p->ef_construction = 150;
-  p->insert_batch = 1;
+  hnsw_defaults(p);
 }
 
 void lb2_ivfhnswpq_build_params_default(lb2_ivfhnswpq_build_params* p) {
   lb2_ivfpq_build_params_default(&p->pq);
-  p->max_level = 7;  // HnswBuildParams::default (hnsw/builder.rs:63-72)
-  p->m = 20;
-  p->ef_construction = 150;
-  p->insert_batch = 1;
+  hnsw_defaults(p);
 }
 
 void lb2_ivfhnswflat_build_params_default(lb2_ivfhnswflat_build_params* p) {
   lb2_ivfflat_build_params_default(&p->flat);
-  p->max_level = 7;  // HnswBuildParams::default (hnsw/builder.rs:63-72)
-  p->m = 20;
-  p->ef_construction = 150;
-  p->insert_batch = 1;
+  hnsw_defaults(p);
 }
 
 void lb2_ivfrq_build_params_default(lb2_ivfrq_build_params* p) {
-  p->num_partitions = 256;
-  lb2_kmeans_params_default(&p->ivf);
-  p->ivf.balance_factor = 1.0f;
+  ivf_defaults(p);
   p->num_bits = 1;
-  p->seed = 0;
 }
 
 lb2_status lb2_ivfpq_transform(const void* centroids, uint32_t k, const void* codebook,
@@ -445,26 +606,13 @@ lb2_status lb2_ivfpq_transform(const void* centroids, uint32_t k, const void* co
                                uint32_t* part_out, uint8_t* codes_out, uint8_t* valid_out) {
   LB2_API_BEGIN
   check_pq_shape(d, num_sub_vectors, num_bits, PqUse::ENCODE);
-  const int M = num_sub_vectors;
-  const int m = metric_of(metric);
-  VecIn c(centroids, (size_t)k * d, model_dtype(dtype)), cb(codebook, ((size_t)1 << num_bits) * d, model_dtype(dtype));
-  const size_t cw = num_bits == 4 ? M / 2 : M;
-  OutArg<uint32_t> p(part_out, n);
-  OutArg<uint8_t> co(codes_out, (size_t)n * cw), v(valid_out, n);
-  DevBuf<uint8_t> vtmp;
-  uint8_t* vp = v.get();
-  if (!vp) { vtmp.alloc(std::max<uint64_t>(n, 1)); vp = vtmp.p; }
-  if (n) {
-    Source src(vectors, n, (int)d, dtype);
-    src.start_resident_copy();
-    DevBuf<float> normbuf;
-    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
-      transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, c.get(), (int)k, cb.get(), M, (int)num_bits, normbuf,
-                      p.get() + r0, co.get() + r0 * cw, vp + r0);
-    });
-  }
-  p.commit(); co.commit(); v.commit();
-  sync_stream();
+  std::unique_ptr<lb2_index> ix = make_index(IndexKind::PQ, k, d, metric_of(metric), dtype);
+  ix->M = (int)num_sub_vectors;
+  ix->nbits = (int)num_bits;
+  ix->codebook.alloc(ix->codebook_len());
+  copy_in(ix->centroids.p, centroids, (size_t)k * d, model_dtype(dtype));
+  copy_in(ix->codebook.p, codebook, ix->codebook_len(), model_dtype(dtype));
+  transform_into(ix.get(), vectors, n, part_out, codes_out, nullptr, nullptr, valid_out);
   LB2_API_END
 }
 
@@ -474,36 +622,13 @@ lb2_status lb2_ivfrq_transform(const void* centroids, uint32_t k, const void* ro
   LB2_API_BEGIN
   LB2_REQUIRE(centroids && rotation && (vectors || n == 0) && k > 0, "null argument");
   rq_check(d, dtype, num_bits);
-  const int m = metric_of(metric);
-  const uint64_t cd = (uint64_t)d * num_bits;
-  VecIn c(centroids, (size_t)k * d, dtype), r(rotation, cd * cd, dtype);
-  DevBuf<float> cnorm;
-  rq_centroid_norms(m, c.get(), (int)k, (int)d, cnorm);
-  OutArg<uint32_t> p(part_out, n);
-  OutArg<uint8_t> co(codes_out, (size_t)(n * cd / 8)), v(valid_out, n);
-  OutArg<float> ao(add_out, n), so(scale_out, n);
-  DevBuf<uint32_t> ptmp;
-  DevBuf<uint8_t> vtmp, ctmp;
-  DevBuf<float> atmp, stmp;
-  uint32_t* pp = p.get();
-  uint8_t *vp = v.get(), *cp = co.get();
-  float *ap = ao.get(), *sp = so.get();
-  if (!pp) { ptmp.alloc(std::max<uint64_t>(n, 1)); pp = ptmp.p; }
-  if (!vp) { vtmp.alloc(std::max<uint64_t>(n, 1)); vp = vtmp.p; }
-  if (!cp) { ctmp.alloc(std::max<uint64_t>(n * cd / 8, 1)); cp = ctmp.p; }
-  if (!ap) { atmp.alloc(std::max<uint64_t>(n, 1)); ap = atmp.p; }
-  if (!sp) { stmp.alloc(std::max<uint64_t>(n, 1)); sp = stmp.p; }
-  if (n) {
-    Source src(vectors, n, (int)d, dtype);
-    src.start_resident_copy();
-    RqWork w;
-    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
-      rq_transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, c.get(), (int)k, r.get(),
-                         (int)num_bits, cnorm.p, w, pp + r0, vp + r0, cp + r0 * (cd / 8), ap + r0, sp + r0);
-    });
-  }
-  p.commit(); co.commit(); v.commit(); ao.commit(); so.commit();
-  sync_stream();
+  std::unique_ptr<lb2_index> ix = make_index(IndexKind::RQ, k, d, metric_of(metric), dtype);
+  ix->nbits = (int)num_bits;
+  const uint64_t cd = ix->code_dim();
+  ix->rq_rot.alloc(cd * cd);
+  copy_in(ix->centroids.p, centroids, (size_t)k * d, dtype);
+  copy_in(ix->rq_rot.p, rotation, cd * cd, dtype);
+  transform_into(ix.get(), vectors, n, part_out, codes_out, add_out, scale_out, valid_out);
   LB2_API_END
 }
 
@@ -511,18 +636,8 @@ lb2_status lb2_index_transform(const lb2_index* index, const void* vectors, uint
                                uint8_t* payload_out, float* add_out, float* scale_out, uint8_t* valid_out) {
   LB2_API_BEGIN
   LB2_REQUIRE(index && (vectors || n == 0), "null argument");
-  const bool rq = index->kind == IndexKind::RQ;
-  LB2_REQUIRE(rq || (!add_out && !scale_out), "lb2_index_transform: add and scale factors are for IVF_RQ indexes only");
-  const size_t rb = index->row_bytes();
-  OutArg<uint32_t> po(part_out, n);
-  OutArg<uint8_t> pl(payload_out, (size_t)n * rb), vo(valid_out, n);
-  OutArg<float> ao(add_out, n), so(scale_out, n);
-  if (n) {
-    Source src(vectors, n, index->d, index->dtype);
-    index_transform_rows(index, src, nullptr, po.get(), pl.get(), ao.get(), so.get(), vo.get());
-  }
-  po.commit(); pl.commit(); vo.commit(); ao.commit(); so.commit();
-  sync_stream();
+  LB2_REQUIRE(index->kind == IndexKind::RQ || (!add_out && !scale_out), "lb2_index_transform: add and scale factors are for IVF_RQ indexes only");
+  transform_into(index, vectors, n, part_out, payload_out, add_out, scale_out, valid_out);
   LB2_API_END
 }
 
@@ -536,35 +651,7 @@ lb2_status lb2_ivfflat_build(const void* data, uint64_t n, uint32_t d, lb2_dtype
   const int K = params->num_partitions;
   LB2_REQUIRE(K > 0 && (comm_nranks() > 1 || n >= (uint64_t)K), "KMeans: can not train %d centroids with %llu vectors", K,
               (unsigned long long)n);
-  EventSet ev(4);
-  ev.record(0);
-  Source src(data, n, (int)d, dtype);
-  std::unique_ptr<lb2_index> ix = make_index(IndexKind::FLAT, K, d, m, dtype);
-  std::vector<double> loss;
-  std::vector<uint32_t> iters;
-  train_ivf_stage(src, ix.get(), params->ivf, params->seed, &loss, &iters);
-  ev.record(1);
-  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
-  DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1));
-  {
-    TagScope tg("transform");
-    attach_partition_index(ix.get(), params->ivf, params->seed);
-    DevBuf<float> normbuf;
-    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
-      assign_flat_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, normbuf, part.p + r0,
-                        valid.p + r0, nullptr, ix->pidx.get());
-    });
-  }
-  ev.record(2);
-  InArg<uint64_t> rid(row_ids, n);
-  {
-    TagScope tg("group");  // the stored vectors are the normalised ones when the metric is cosine
-    index_load_flat_src(ix.get(), part.p, src, rid.get(), valid.p, m == METRIC_COSINE);
-  }
-  ev.record(3);
-  sync_stream();
-  fill_stats(stats, ev, loss, iters);
-  *out = ix.release();
+  build_index(IndexKind::FLAT, data, n, d, dtype, m, K, params->ivf, params->seed, {}, row_ids, out, stats);
   LB2_API_END
 }
 
@@ -580,52 +667,8 @@ lb2_status lb2_ivfsq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   const int m = metric_of(metric);
   const int K = params->num_partitions;
   LB2_REQUIRE(K > 0 && n >= (uint64_t)K, "KMeans: can not train %d centroids with %llu vectors", K, (unsigned long long)n);
-  EventSet ev(5);
-  ev.record(0);
-  Source src(data, n, (int)d, dtype);
-  std::unique_ptr<lb2_index> ix = make_index(IndexKind::SQ, K, d, m, dtype);
-  ix->nbits = 8;
-  std::vector<double> loss;
-  std::vector<uint32_t> iters;
-  // 1. IVF: the same stage as lb2_ivfflat_build (same sample, seed, training)
-  train_ivf_stage(src, ix.get(), params->ivf, params->seed, &loss, &iters);
-  ev.record(1);
-  // 2. ScalarQuantizer::build (sq.rs:152-182) on sample_rate * 2^num_bits rows (builder.rs:410-421), normalised
-  //    under cosine, rows that are not finite dropped (builder.rs:436), no residuals (quantizer.rs:52).  The bounds
-  //    are taken over the values the index stores: normalised, in the column's element type.
-  {
-    TagScope tg("sq_train");
-    std::vector<uint64_t> rows = sample_rows(n, std::min<uint64_t>(n, params->sample_rate * 256), params->seed + 1);
-    DevBuf<float> sample;
-    const uint64_t s = gather_finite_sample(src, rows, m == METRIC_COSINE, sample);
-    round_model(sample.p, (size_t)s * d, dtype);
-    sq_bounds_f32(sample.p, (uint64_t)s * d, &ix->sq_lower, &ix->sq_upper);
-  }
-  ev.record(2);
-  // 3. transform (ivf.rs:238-279): partition, then the SQ codes of the stored vectors themselves
-  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
-  DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1)), codes(std::max<uint64_t>(1, (uint64_t)n * d));
-  {
-    TagScope tg("transform");
-    attach_partition_index(ix.get(), params->ivf, params->seed);
-    DevBuf<float> normbuf;
-    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
-      const float* xs = assign_flat_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, normbuf,
-                                          part.p + r0, valid.p + r0, nullptr, ix->pidx.get());
-      if (m == METRIC_COSINE) round_model(normbuf.p, (size_t)rows * d, dtype);  // as IVF_FLAT stores them
-      sq_encode_f32(xs, (uint64_t)rows * d, ix->sq_lower, ix->sq_upper, codes.p + r0 * d);
-    });
-  }
-  ev.record(3);
-  {
-    TagScope tg("group");
-    InArg<uint64_t> rid(row_ids, n);
-    index_load_dev(ix.get(), part.p, codes.p, rid.get(), n, valid.p);
-  }
-  ev.record(4);
-  sync_stream();
-  fill_stats(stats, ev, loss, iters);
-  *out = ix.release();
+  build_index(IndexKind::SQ, data, n, d, dtype, m, K, params->ivf, params->seed, {params->num_bits, params->sample_rate},
+              row_ids, out, stats);
   LB2_API_END
 }
 
@@ -640,49 +683,8 @@ lb2_status lb2_ivfrq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   const int m = metric_of(metric);
   const int K = params->num_partitions;
   LB2_REQUIRE(K > 0 && n >= (uint64_t)K, "KMeans: can not train %d centroids with %llu vectors", K, (unsigned long long)n);
-  EventSet ev(5);
-  ev.record(0);
-  Source src(data, n, (int)d, dtype);
-  std::unique_ptr<lb2_index> ix = make_index(IndexKind::RQ, K, d, m, dtype);
-  ix->nbits = (int)params->num_bits;
-  const int cd = ix->code_dim();
-  std::vector<double> loss;
-  std::vector<uint32_t> iters;
-  // 1. IVF: the same stage as lb2_ivfflat_build (same sample, seed, training)
-  train_ivf_stage(src, ix.get(), params->ivf, params->seed, &loss, &iters);
-  ev.record(1);
-  // 2. RabitQuantizer::new (bq/builder.rs:52-70): the rotation, from seed + 1
-  {
-    TagScope tg("rq_train");
-    ix->rq_rot.alloc((size_t)cd * cd);
-    rq_rotation_f32(cd, params->seed + 1, ix->rq_rot.p);
-  }
-  ev.record(2);
-  // 3. transform (ivf.rs:281-328) of every row
-  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
-  DevBuf<uint8_t> valid(std::max<uint64_t>(n, 1)), codes(std::max<uint64_t>(1, n * (cd / 8)));
-  DevBuf<float> add(std::max<uint64_t>(n, 1)), scale(std::max<uint64_t>(n, 1)), cnorm;
-  {
-    TagScope tg("transform");
-    rq_centroid_norms(m, ix->centroids.p, K, (int)d, cnorm);
-    attach_partition_index(ix.get(), params->ivf, params->seed);
-    RqWork w;
-    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
-      rq_transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, ix->rq_rot.p, ix->nbits,
-                         cnorm.p, w, part.p + r0, valid.p + r0, codes.p + r0 * (cd / 8), add.p + r0, scale.p + r0,
-                         ix->pidx.get());
-    });
-  }
-  ev.record(3);
-  {
-    TagScope tg("group");
-    InArg<uint64_t> rid(row_ids, n);
-    index_load_dev(ix.get(), part.p, codes.p, rid.get(), n, valid.p, add.p, scale.p);
-  }
-  ev.record(4);
-  sync_stream();
-  fill_stats(stats, ev, loss, iters);
-  *out = ix.release();
+  build_index(IndexKind::RQ, data, n, d, dtype, m, K, params->ivf, params->seed, {params->num_bits}, row_ids, out,
+              stats);
   LB2_API_END
 }
 
@@ -692,123 +694,12 @@ lb2_status lb2_ivfpq_build(const void* data, uint64_t n, uint32_t d, lb2_dtype d
   LB2_API_BEGIN
   LB2_REQUIRE(data && params && out, "null argument");
   const int m = metric_of(metric);
-  const int K = params->num_partitions, M = params->pq.num_sub_vectors;
-  const uint64_t nranks = comm_nranks();  // sharded build: this rank's rows
-  LB2_REQUIRE(K > 0 && (nranks > 1 || n >= (uint64_t)K), "KMeans: can not train %d centroids with %llu vectors", K,
+  const int K = params->num_partitions;
+  LB2_REQUIRE(K > 0 && (comm_nranks() > 1 || n >= (uint64_t)K), "KMeans: can not train %d centroids with %llu vectors", K,
               (unsigned long long)n);
-  check_pq_shape(d, M, params->pq.num_bits, PqUse::ENCODE);
-  const int nbits = (int)params->pq.num_bits;
-  EventSet ev(5);
-  ev.record(0);
-
-  // Staging (class Source).  Device rows: used in place.  Host rows: both training samples (<= K * 256 and
-  // 65 536 rows) are gathered straight out of the caller's memory (zero-copy reads over PCIe when it is pinned),
-  // then the matrix is copied ONCE, in its own element type, on a second stream while both trainings run; the
-  // per-row pass waits for it and converts one chunk of rows at a time.  A matrix too large for that is streamed
-  // chunk by chunk during the per-row pass instead (double buffered).  No whole-matrix f32 copy exists.
-  // (declared before `src`: on an error path ~Source waits for the copy stream, which may still be writing the PQ
-  // sample, before these buffers go back to the pool)
-  DevBuf<float> sample_ivf, sample_pq;
-  Source src(data, n, (int)d, dtype);
-
-  std::unique_ptr<lb2_index> ix = make_index(IndexKind::PQ, K, d, m, dtype);
-  ix->M = M;
-  ix->nbits = nbits;
-  ix->codebook.alloc(ix->codebook_len());
-  std::vector<double> ivf_loss;
-  std::vector<uint32_t> ivf_iters, pq_iters;
-  // 0. both training samples are gathered first (IVF: K*sample_rate rows, rust/lance/src/index/
-  //    vector/ivf.rs:1237-1241; PQ: 256*2^nbits rows, builder.rs:410-421), normalised for cosine; rows that are
-  //    not finite are dropped from them (builder.rs:436); then the bulk copy starts
-  const uint64_t s_pq0 = std::min<uint64_t>(n, (params->pq.sample_rate * ((uint64_t)1 << nbits) + nranks - 1) / nranks);
-  uint64_t s_ivf = 0, s_pq = 0;
-  std::vector<uint64_t> rows_pq;
-  bool pq_deferred = false;
-  // LB2_TRACE_BUILD=1: host wall-clock stamps of the staging steps on stderr (diagnostics; adds synchronisations)
-  static const bool trace = getenv("LB2_TRACE_BUILD") && *getenv("LB2_TRACE_BUILD");
-  const auto tr0 = std::chrono::steady_clock::now();
-  auto stamp = [&](const char* what) {
-    if (!trace) return;
-    sync_stream();
-    fprintf(stderr, "[lb2 build] %-22s +%.3f ms\n", what,
-            std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tr0).count());
-  };
-  {
-    std::vector<uint64_t> rows = ivf_sample_rows(n, K, params->ivf, params->seed);
-    stamp("sample_rows(ivf)");
-    s_ivf = gather_finite_sample(src, rows, m == METRIC_COSINE, sample_ivf);
-    stamp("gather(ivf sample)");
-    rows_pq = sample_rows(n, s_pq0, params->seed + 1);
-    // the PQ sample is not needed before the IVF model exists: from pinned f32 rows it is gathered on the copy
-    // stream (in front of the bulk copy) while the IVF training runs; otherwise here
-    if (m != METRIC_COSINE && !trace && !rows_pq.empty()) {
-      sample_pq.alloc(rows_pq.size() * (uint64_t)d);
-      pq_deferred = src.gather_f32_async(rows_pq, sample_pq.p);
-    }
-    if (!pq_deferred) {
-      s_pq = gather_finite_sample(src, rows_pq, m == METRIC_COSINE, sample_pq);
-      stamp("gather(pq sample)");
-    }
-  }
-  src.start_resident_copy();
-  if (trace) fprintf(stderr, "[lb2 build] %-22s +%.3f ms (host, no sync)\n", "bulk copy issued",
-                     std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - tr0).count());
-  // 1. IVF
-  train_ivf_model(sample_ivf.p, s_ivf, ix.get(), params->ivf, &ivf_loss, &ivf_iters);
-  stamp("ivf trained");
-  if (pq_deferred) {
-    if (src.finish_async_sample()) {
-      s_pq = rows_pq.size();
-    } else {  // rare: some sampled rows are not finite -> the synchronous path drops them and gathers again
-      s_pq = gather_finite_sample(src, rows_pq, false, sample_pq);
-    }
-  }
-  sample_ivf.release();
-  ev.record(1);
-  // 2. PQ: residuals of its sample w.r.t. the IVF centroids (builder.rs:439-450)
-  {
-    TagScope tg("pq_train");
-    if (m != METRIC_DOT && s_pq) {
-      DevBuf<uint32_t> part(s_pq);
-      assign_f32(sample_pq.p, s_pq, d, ix->centroids.p, K, METRIC_L2, nullptr, part.p, nullptr, nullptr);
-      LB2_LAUNCH("residual", residual_kernel, cdiv(s_pq * d, 256), 256, 0, sample_pq.p, ix->centroids.p,
-                 part.p, s_pq, (int)d, sample_pq.p);
-    }
-    VecIn cb_init(params->pq.codebook, ix->codebook_len(), model_dtype(dtype));
-    lb2_pq_params pqp = params->pq;
-    pqp.codebook = cb_init.get();
-    // always L2 k-means (builder.rs:460: Q::build(&training_data, DistanceType::L2, ..)); for a dot index
-    // the sample is the raw vectors (no residual), for L2 / cosine the residuals computed above
-    pq_train_dev(sample_pq.p, s_pq, d, METRIC_L2, &pqp, ix->codebook.p, &pq_iters);
-    round_model(ix->codebook.p, ix->codebook_len(), dtype);
-  }
-  sample_pq.release();
-  ev.record(2);
-  // 3. transform every row (lance-index/src/vector/ivf.rs:357: partition -> residual -> PQ), chunk by chunk
-  const size_t cw = ix->row_bytes();
-  DevBuf<uint32_t> part(std::max<uint64_t>(n, 1));
-  DevBuf<uint8_t> codes(std::max<uint64_t>(1, (size_t)n * cw)), valid(std::max<uint64_t>(n, 1));
-  {
-    TagScope tg("transform");
-    attach_partition_index(ix.get(), params->ivf, params->seed);
-    DevBuf<float> normbuf;
-    for_each_chunk(src, [&](const float* xf, const void* xnat, uint64_t r0, uint64_t rows) {
-      transform_chunk(xf, xnat, (int)src.dtype(), rows, (int)d, m, ix->centroids.p, K, ix->codebook.p, M, nbits, normbuf,
-                      part.p + r0, codes.p + r0 * cw, valid.p + r0, ix->pidx.get());
-    });
-  }
-  ev.record(3);
-  {
-    // 4. group the kept rows by partition (shuffle + build_partitions, builder.rs:501-937); rows the
-    //    transform marked invalid are dropped, as KeepFiniteVectors does (transform.rs:112-159)
-    TagScope tg("group");
-    InArg<uint64_t> rid(row_ids, n);
-    index_load_dev(ix.get(), part.p, codes.p, rid.get(), n, valid.p);
-  }
-  ev.record(4);
-  sync_stream();
-  fill_stats(stats, ev, ivf_loss, ivf_iters, pq_iters);
-  *out = ix.release();
+  check_pq_shape(d, params->pq.num_sub_vectors, params->pq.num_bits, PqUse::ENCODE);
+  build_index(IndexKind::PQ, data, n, d, dtype, m, K, params->ivf, params->seed, {params->pq.num_bits, 0, &params->pq},
+              row_ids, out, stats);
   LB2_API_END
 }
 

@@ -22,8 +22,9 @@ void pq_encode_any(const float* x, uint64_t n, int d, int M, int ds, const float
                    const float* cent, const uint32_t* part, const uint8_t* row_valid, int nbits, uint8_t* codes);
 void sq_check_dim(uint32_t d);
 void rq_check(uint32_t d, lb2_dtype dtype, uint32_t num_bits);
-// lb2_index_transform's rows of `src` with the model of `index` (every output nullable, device); given_part (nullable):
-// the rows' partitions are given, and IVF_PQ takes its residuals to them
+// the transform of every row of `src` with the model and partition rule of `index`, for the builds, the stand-alone
+// transforms and a split (every output nullable, device; IVF_FLAT's NULL payload is not written; synchronises only
+// for scratch); given_part (nullable): the rows' partitions are given, and IVF_PQ takes its residuals to them
 void index_transform_rows(const lb2_index* index, Source& src, const uint32_t* given_part, uint32_t* part_out,
                           uint8_t* payload_out, float* add_out, float* scale_out, uint8_t* valid_out);
 

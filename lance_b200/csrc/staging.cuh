@@ -225,8 +225,10 @@ class Source {
   }
   // Host rows that fit: one bulk copy in the NATIVE type on a second stream (call after the sample gathers --
   // zero-copy reads get no PCIe bandwidth while the copy engine streams).  Otherwise chunks are staged on demand.
+  // Decided once: a later call does nothing.
   void start_resident_copy() {
-    if (dev_native_ || n_ == 0) return;
+    if (dev_native_ || n_ == 0 || copy_decided_) return;
+    copy_decided_ = true;
     const size_t bytes = (size_t)n_ * d_ * es_;
     acquire_cache();  // (a second Source alive on the same thread falls back to private resources)
     // LB2_MAX_RESIDENT_MB=m: a matrix of more than m MB is streamed (0 = always); read on every call, and
@@ -381,6 +383,7 @@ class Source {
   cudaStream_t copy_stream_ = nullptr;
   cudaEvent_t copied_ = nullptr, slot_ready_[2] = {nullptr, nullptr}, slot_free_[2] = {nullptr, nullptr};
   bool bulk_pending_ = false;
+  bool copy_decided_ = false;       // start_resident_copy() has run
   uint64_t calls_ = 0;
 };
 

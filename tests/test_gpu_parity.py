@@ -337,15 +337,19 @@ def test_index_4bit_build_search_matches_oracle(metric):
 
 
 # ---- prefilter: PreFilter / RowIdMask (prefilter.rs:27-51, flat/index.rs:129-165) --------------
-@pytest.mark.parametrize("kind", ["pq", "flat"])
+@pytest.mark.parametrize("kind", ["pq", "flat", "pq_pinned_ids"])
 def test_index_search_with_row_mask_matches_oracle(kind):
     rng = np.random.default_rng(115)
     n, d, K, M = 24000, 64, 24, 8
     data = synth.gaussian_mixture(n, d, n_components=K, seed=115)
     rid = (rng.permutation(n).astype(np.uint64) * 3 + 7)          # sparse, shuffled row ids
+    pin = None
+    if kind == "pq_pinned_ids":                                    # the same row ids from pinned host memory
+        kind, pin = "pq", lb.PinnedArray(rid.shape, np.uint64)
+        pin.array[...] = rid
     if kind == "pq":
         ix = lb.IvfPqIndex.build(data, "l2", lb.IvfBuildParams(num_partitions=K, num_sub_vectors=M, max_iters=8,
-                                                               pq_max_iters=6), row_ids=rid)
+                                                               pq_max_iters=6), row_ids=rid if pin is None else pin)
     else:
         ix = lb.IvfFlatIndex.build(data, "l2", num_partitions=K, max_iters=8, row_ids=rid)
     parts = ix.export()
