@@ -406,6 +406,44 @@ lb2_status lb2_index_search_probed(lb2_index* index, const void* queries, uint64
                                    const lb2_search_params* sp /* nprobes must be 0 */,
                                    const lb2_probe_params* pp, uint64_t* row_ids_out, float* dists_out,
                                    uint32_t* counts_out, uint32_t* nprobes_out /* nullable, [nq] */);
+/* A batch of queries with their own parameters, as separate nearest() plans reach the index (each its own Query,
+ * lance-index/src/vector.rs:72-116, and its own PreFilter mask, prefilter.rs:27-51), searched in one device pass.
+ * Row q of the output is bit for bit what the single-parameter call returns for query q alone with q's parameters
+ * and filter: lb2_index_search_ex for a fixed nprobes (nprobes_out[q] = min(nprobes, K)),
+ * lb2_index_search_probed for nprobes = 0 (its minimum / maximum nprobes, the filter's max_len and mask_ids, and
+ * late_width), and lb2_index_search_hnsw when ef is set on an IVF_HNSW_* index.  Rows are [nq][k_stride]; slots
+ * k_q .. k_stride - 1 hold UINT64_MAX / +inf.  counts_out [nq] and nprobes_out [nq] are nullable.  Filters are
+ * staged once each and shared by every query that names them; refine_vectors / num_vectors are the raw column of
+ * every query with refine_factor > 0 (as lb2_search_params); late_width is the probe rule's (>= 1).
+ * Every query's own k, probes, refine factor, range, filter and ef reach the scan kernels from a per-query table on
+ * the device, so the number of kernel launches depends on the routes the batch needs, not on how many parameter
+ * sets or filters it holds.
+ * Refused before anything is launched or written: a query its own call would refuse (that call's status; the
+ * message names the query), and with LB2_INVALID_ARG: k_stride below the largest k, a filter index that is neither
+ * below num_filters nor UINT32_MAX, ef on a non-HNSW index, refine_factor > 0 without refine_vectors, late_width 0.
+ * LB2_UNSUPPORTED: a thread whose communicator has more than one rank. */
+typedef struct {
+  const uint64_t* allow_bitmap; /* storage positions, as lb2_index_row_mask builds it; host or device */
+  uint32_t has_max_len;         /* RowIdMask::max_len(): used by minimum / maximum nprobes queries only */
+  uint64_t max_len;
+  const uint64_t* mask_ids;     /* ditto; NULL = not iterable */
+  uint64_t num_mask_ids;
+} lb2_query_filter;
+typedef struct {
+  uint32_t k;                                /* >= 1 */
+  uint32_t nprobes;                          /* > 0: fixed probes (search_ex); 0: minimum / maximum below */
+  uint32_t minimum_nprobes, maximum_nprobes; /* as lb2_probe_params */
+  uint32_t refine_factor;                    /* 0 = no refine */
+  uint32_t filter;                           /* index into filters[], UINT32_MAX = no prefilter */
+  uint32_t ef;                               /* IVF_HNSW_* only; 0 = k' + k' / 2 */
+  uint32_t has_lower_bound, has_upper_bound;
+  float lower_bound, upper_bound;
+} lb2_query_params;
+lb2_status lb2_index_search_batch(lb2_index* index, const void* queries, uint64_t nq,
+                                  const lb2_query_params* params /* [nq] */, const lb2_query_filter* filters,
+                                  uint32_t num_filters, const void* refine_vectors, uint64_t num_vectors,
+                                  uint32_t late_width, uint32_t k_stride, uint64_t* row_ids_out /* [nq][k_stride] */,
+                                  float* dists_out, uint32_t* counts_out, uint32_t* nprobes_out);
 /* knn_combined (rust/lance/src/dataset/scanner.rs:2946-3027): a nearest() query on an index that does not yet cover
  * every row of its table.  The reference takes the raw vectors of the ANN rows and re-scores them exactly, runs a
  * flat KNN with the index metric over the unindexed rows (with the query's prefilter), and sorts the union by

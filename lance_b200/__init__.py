@@ -795,6 +795,105 @@ class IvfPqIndex:
                                             as_ptr(dists)[0], as_ptr(counts)[0], as_ptr(nprobes)[0]))
         return ids, dists, counts, nprobes
 
+    def search_batch(self, queries, k, nprobes=None, minimum_nprobes=None, maximum_nprobes=None, refine_factor=0,
+                     vectors=None, filters=None, filter_of=None, lower_bound=None, upper_bound=None, ef=None,
+                     late_width=1, out=None):
+        """lb2_index_search_batch: every query with its own parameters, in one device pass.  Row q equals search_ex
+        (or, with ef, the HNSW kinds' search_ex with ef) of query q alone with its own parameters and filter.
+        Every per-query argument is a scalar or an [nq] array: k, nprobes, refine_factor, filter_of (index into
+        `filters`, -1 = none), lower_bound / upper_bound (NaN or None = no bound), ef (0 or None = k' + k' / 2).
+        `filters` is a list of allow bitmaps (as row_mask builds them) or (bitmap, max_len, mask_ids) tuples.
+        A query with nprobes 0 (or every query when nprobes is None) runs the probe rule with its own minimum_nprobes
+        (default 1) and maximum_nprobes (None or 0 = every partition), equal to search_probed; a filter tuple's
+        max_len and mask_ids and late_width serve those queries.
+        Returns (ids, dists, counts, nprobes): ids / dists [nq][max k] (or `out`'s arrays and their row length)."""
+        from ._lib import QueryFilter, QueryParams
+        dt = getattr(self, "_dt", F32)
+        npdt = {F32: np.float32, F16: np.float16, U8: np.uint8, BF16: np.uint16}[dt]
+        if not isinstance(queries, (DeviceArray, PinnedArray)):
+            queries = np.ascontiguousarray(queries, dtype=npdt)
+        if vectors is not None and not isinstance(vectors, (DeviceArray, PinnedArray)):
+            vectors = np.ascontiguousarray(vectors, dtype=npdt)
+        nq = int(queries.shape[0])
+
+        def per_query(name, v, dtype, default):
+            a = np.asarray(default if v is None else v, dtype=dtype)
+            if a.ndim == 0:
+                return np.full(nq, a, dtype)
+            if a.shape != (nq,):
+                raise ValueError(f"search_batch: {name} must be a scalar or an array of {nq} values, got shape {a.shape}")
+            return a
+
+        ks = per_query("k", k, np.int64, 0)
+        if nq and (ks < 1).any():
+            raise ValueError("search_batch: every k must be at least 1")
+        nps = per_query("nprobes", nprobes, np.int64, 0)
+        mins = per_query("minimum_nprobes", minimum_nprobes, np.int64, 1)
+        maxs = per_query("maximum_nprobes", maximum_nprobes, np.int64, 0)
+        if (nps < 0).any():
+            raise ValueError("search_batch: nprobes must not be negative (0: minimum / maximum nprobes)")
+        ruled = nps == 0
+        if (mins[ruled] < 1).any() or (maxs[ruled] < 0).any():
+            raise ValueError("search_batch: minimum_nprobes must be at least 1 and maximum_nprobes not negative")
+        mins, maxs = np.where(ruled, mins, 0), np.where(ruled, maxs, 0)
+        rfs = per_query("refine_factor", refine_factor, np.int64, 0)
+        if (rfs < 0).any():
+            raise ValueError("search_batch: refine_factor must not be negative")
+        if (rfs > 0).any() and vectors is None:
+            raise ValueError("search_batch: refine_factor > 0 needs vectors")
+        filters = list(filters or [])
+        fof = per_query("filter_of", filter_of, np.int64, -1)
+        if ((fof < -1) | (fof >= len(filters))).any():
+            raise ValueError(f"search_batch: filter_of must be -1 or below the {len(filters)} filters")
+        lows = per_query("lower_bound", lower_bound, np.float32, np.nan)
+        ups = per_query("upper_bound", upper_bound, np.float32, np.nan)
+        efs = per_query("ef", ef, np.int64, 0)
+        if (efs < 0).any():
+            raise ValueError("search_batch: ef must not be negative")
+        kmax = int(ks.max()) if nq else 1
+        if out is None:
+            ids, dists = np.empty((nq, kmax), np.uint64), np.empty((nq, kmax), np.float32)
+        else:
+            ids, dists = out
+        k_stride = int(ids.shape[1]) if len(ids.shape) == 2 else kmax
+        if tuple(ids.shape) != (nq, k_stride) or tuple(dists.shape) != (nq, k_stride) or k_stride < kmax:
+            raise ValueError(f"search_batch: out arrays must be [{nq}][>= {kmax}], got {ids.shape} and {dists.shape}")
+        counts, probes = np.empty(nq, np.uint32), np.empty(nq, np.uint32)
+        keep = []
+        cf = (QueryFilter * max(1, len(filters)))()
+        for i, f in enumerate(filters):
+            bm, max_len, mask_ids = (f if isinstance(f, tuple) else (f, None, None))
+            if bm is not None and not isinstance(bm, (DeviceArray, PinnedArray)):
+                bm = np.ascontiguousarray(bm, dtype=np.uint64)
+            if mask_ids is not None and not isinstance(mask_ids, (DeviceArray, PinnedArray)):
+                mask_ids = np.ascontiguousarray(np.sort(np.asarray(mask_ids, dtype=np.uint64)))
+            bp, kb = as_ptr(bm)
+            mp, km = as_ptr(mask_ids)
+            if mask_ids is not None and mp.value is None:  # an empty numpy array has no buffer address to pass
+                km = np.zeros(1, np.uint64)
+                mp = C.c_void_p(km.ctypes.data)
+            keep += [bm, mask_ids, kb, km]
+            cf[i] = QueryFilter(bp.value if bp is not None else None, int(max_len is not None), int(max_len or 0),
+                                mp.value if mp is not None else None, 0 if mask_ids is None else int(mask_ids.shape[0]))
+        # the lb2_query_params array, filled column by column (same layout as QueryParams)
+        cp = np.zeros(max(1, nq), np.dtype({"names": [f for f, _ in QueryParams._fields_],
+                                            "formats": [np.float32 if t is C.c_float else np.uint32
+                                                        for _, t in QueryParams._fields_]}))
+        for name, col in (("k", ks), ("nprobes", nps), ("minimum_nprobes", mins), ("maximum_nprobes", maxs),
+                          ("refine_factor", rfs), ("ef", efs)):
+            cp[name][:nq] = col
+        cp["filter"][:nq] = np.where(fof < 0, 0xFFFFFFFF, fof)
+        cp["has_lower_bound"][:nq], cp["has_upper_bound"][:nq] = ~np.isnan(lows), ~np.isnan(ups)
+        cp["lower_bound"][:nq], cp["upper_bound"][:nq] = np.nan_to_num(lows, nan=0.0), np.nan_to_num(ups, nan=0.0)
+        assert cp.dtype.itemsize == C.sizeof(QueryParams)
+        qp, _k1 = as_ptr(queries)
+        vp, _k0 = as_ptr(vectors)
+        check(lib().lb2_index_search_batch(self._h, qp, C.c_uint64(nq), C.c_void_p(cp.ctypes.data), cf, C.c_uint32(len(filters)), vp,
+                                           C.c_uint64(0 if vectors is None else vectors.shape[0]),
+                                           C.c_uint32(late_width), C.c_uint32(k_stride), as_ptr(ids)[0],
+                                           as_ptr(dists)[0], as_ptr(counts)[0], as_ptr(probes)[0]))
+        return ids, dists, counts, probes
+
     def search_combined(self, queries, k, vectors, unindexed_vectors, unindexed_row_ids, nprobes=None,
                         minimum_nprobes=None, maximum_nprobes=None, late_width=1, refine_factor=0, allow_bitmap=None,
                         unindexed_allow_bitmap=None, mask_ids=None, mask_max_len=None, lower_bound=None,

@@ -148,7 +148,7 @@ EXPORTS = [
     "lb2_index_export_storage", "lb2_index_load_storage",
     "lb2_partition_index_uses_graph", "lb2_partition_index_build", "lb2_partition_index_assign",
     "lb2_partition_index_info", "lb2_partition_index_export", "lb2_partition_index_destroy",
-    "lb2_index_set_partition_index",
+    "lb2_index_set_partition_index", "lb2_index_search_batch",
 ]
 
 _lib = None
@@ -208,6 +208,20 @@ class ProbeParams(C.Structure):
     _fields_ = [("minimum_nprobes", C.c_uint32), ("maximum_nprobes", C.c_uint32), ("late_width", C.c_uint32),
                 ("has_max_len", C.c_uint32), ("max_len", C.c_uint64), ("mask_ids", C.c_void_p),
                 ("num_mask_ids", C.c_uint64)]
+
+
+class QueryFilter(C.Structure):
+    """lb2_query_filter (include/lance_b200.h)."""
+    _fields_ = [("allow_bitmap", C.c_void_p), ("has_max_len", C.c_uint32), ("max_len", C.c_uint64),
+                ("mask_ids", C.c_void_p), ("num_mask_ids", C.c_uint64)]
+
+
+class QueryParams(C.Structure):
+    """lb2_query_params (include/lance_b200.h)."""
+    _fields_ = [("k", C.c_uint32), ("nprobes", C.c_uint32), ("minimum_nprobes", C.c_uint32),
+                ("maximum_nprobes", C.c_uint32), ("refine_factor", C.c_uint32), ("filter", C.c_uint32),
+                ("ef", C.c_uint32), ("has_lower_bound", C.c_uint32), ("has_upper_bound", C.c_uint32),
+                ("lower_bound", C.c_float), ("upper_bound", C.c_float)]
 
 
 class FlatSearchParams(C.Structure):

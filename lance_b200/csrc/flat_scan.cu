@@ -30,10 +30,9 @@ ivfflat_scan_kernel(const float* __restrict__ queries, int d, const uint32_t* __
                     int np, const uint64_t* __restrict__ part_offsets,
                     const T* __restrict__ vectors, const uint64_t* __restrict__ row_ids, int k,
                     float* __restrict__ cand_d, uint64_t* __restrict__ cand_id,
-                    uint32_t* __restrict__ cand_cnt, const ScanFilter flt) {
+                    uint32_t* __restrict__ cand_cnt, const ScanFilter flt0, const QueryParam* __restrict__ qp) {
   extern __shared__ float smem[];
   float* qs = smem;                          // [d]
-  const SlotSmem s(qs + d, k + 1);
   __shared__ float s_qnorm;
   const int tid = threadIdx.x, l = tid & 15;
   const unsigned hmask = 0xffffu << (16 * ((tid >> 4) & 1));
@@ -41,6 +40,9 @@ ivfflat_scan_kernel(const float* __restrict__ queries, int d, const uint32_t* __
   uint32_t p, n_p;
   uint64_t off;
   if (!slot_partition(probe_ids, np, part_offsets, cand_cnt, qi, slot, p, off, n_p)) return;
+  const int kq = query_k(qp, qi, k);  // k: the lists' stride
+  const ScanFilter flt = query_filter(qp, qi, flt0);
+  const SlotSmem s(qs + d, kq + 1);
   for (int t = tid; t < d; t += 256) qs[t] = queries[qi * d + t];
   __syncthreads();
   if (METRIC == METRIC_COSINE && tid < 32) {  // norm_l2(query): 16 lanes + sqrt (norm_l2.rs:106-130)
@@ -58,7 +60,7 @@ ivfflat_scan_kernel(const float* __restrict__ queries, int d, const uint32_t* __
       if (l == 0) s.ukey[j] = (uint32_t)total_order_key(dist) ^ 0x80000000u;
     }
   };
-  const uint32_t cnt = slot_topk(s, n_p, k, flt, off, false, fill);
+  const uint32_t cnt = slot_topk(s, n_p, kq, flt, off, false, fill);
   write_slot(s, cnt, slot, k, off, row_ids, cand_d, cand_id, cand_cnt);
 }
 
@@ -103,7 +105,7 @@ void ivfflat_search(const IvfSearch& s, const void* vectors, int vdt) {
       set_smem(kern, smem);
       LB2_LAUNCH("flat_scan", kern, dim3(sl.np, (unsigned)sl.qn), 256, smem, s.queries + sl.q0 * d, d, sl.probe_ids,
                  sl.np, sl.offsets, reinterpret_cast<const T*>(vectors), s.row_ids, k, sl.cand_d, sl.cand_id,
-                 sl.cand_cnt, s.flt);
+                 sl.cand_cnt, s.flt, s.qp_at(sl.q0));
     });
   });
 }
@@ -112,12 +114,14 @@ void ivfflat_search(const IvfSearch& s, const void* vectors, int vdt) {
 // refine: exact distances of k' = k * refine_factor candidates from the raw vectors, then the k
 // best by (distance, row id)  (scanner.rs:2884-2905, flat.rs:95-148)
 // ------------------------------------------------------------------------------------------------
-template <int METRIC, class T>
+// BATCH: per-query values from qo (refine_batch_f32); the single-parameter refine is compiled without them
+template <int METRIC, class T, bool BATCH>
 __global__ void __launch_bounds__(256)
 refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ vectors,
               uint64_t num_vectors, const uint64_t* __restrict__ cand_id, const uint32_t* __restrict__ cand_cnt,
               int kc, int k, uint64_t* __restrict__ out_id, float* __restrict__ out_d,
-              uint32_t* __restrict__ out_cnt, int has_lower, float lower, int has_upper, float upper) {
+              uint32_t* __restrict__ out_cnt, int has_lower, float lower, int has_upper, float upper,
+              const float* __restrict__ cand_d, const QueryOut* __restrict__ qo, int k_stride) {
   extern __shared__ float smem[];
   float* qs = smem;       // [d]
   float* cd = qs + d;     // [kc]
@@ -125,7 +129,23 @@ refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ ve
   const size_t qi = blockIdx.x;
   const int tid = threadIdx.x, l = tid & 15;
   const unsigned hmask = 0xffffu << (16 * ((tid >> 4) & 1));
-  const uint32_t cnt = min(cand_cnt[qi], (uint32_t)kc);
+  const uint64_t* ids = cand_id + qi * kc;
+  if constexpr (BATCH) {  // a batch: this query's own k' (kc is the lists' stride), k, range; output rows of k_stride
+    const QueryOut& o = qo[qi];
+    has_lower = o.has_lower; lower = o.lower; has_upper = o.has_upper; upper = o.upper;
+    if (!o.refine) {  // the merged list is the result: its first k, ascending already
+      const uint32_t r = min(cand_cnt[qi], (uint32_t)o.k);
+      for (int e = tid; e < k_stride; e += 256) {
+        out_id[qi * k_stride + e] = (uint32_t)e < r ? ids[e] : ~0ull;
+        out_d[qi * k_stride + e] = (uint32_t)e < r ? cand_d[qi * kc + e] : __int_as_float(0x7f800000);
+      }
+      if (tid == 0 && out_cnt) out_cnt[qi] = r;
+      return;
+    }
+  }
+  const int kcq = BATCH ? qo[qi].kc : kc, os = BATCH ? k_stride : k;
+  if constexpr (BATCH) k = qo[qi].k;
+  const uint32_t cnt = min(cand_cnt[qi], (uint32_t)kcq);
   for (int t = tid; t < d; t += 256) qs[t] = queries[qi * d + t];
   __syncthreads();
   if (METRIC == METRIC_COSINE && tid < 32) {
@@ -137,7 +157,6 @@ refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ ve
   }
   __syncthreads();
   const float qn = METRIC == METRIC_COSINE ? s_qnorm : 0.0f;
-  const uint64_t* ids = cand_id + qi * kc;
   for (uint32_t c = tid >> 4; c < cnt; c += 16) {
     const uint64_t id = ids[c];
     float dist = __int_as_float(0x7fc00000);
@@ -156,12 +175,12 @@ refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ ve
         return passes(cd[c]);
       },
       [&](uint32_t r, uint32_t c, int32_t, uint64_t id) {
-        out_id[qi * k + r] = id;
-        out_d[qi * k + r] = cd[c];
+        out_id[qi * os + r] = id;
+        out_d[qi * os + r] = cd[c];
       });
-  for (uint32_t e = r + tid; e < (uint32_t)k; e += 256) {
-    out_id[qi * k + e] = ~0ull;
-    out_d[qi * k + e] = __int_as_float(0x7f800000);
+  for (uint32_t e = r + tid; e < (uint32_t)os; e += 256) {
+    out_id[qi * os + e] = ~0ull;
+    out_d[qi * os + e] = __int_as_float(0x7f800000);
   }
   if (tid == 0 && out_cnt) out_cnt[qi] = r;
 }
@@ -174,10 +193,25 @@ void refine_f32(const float* queries, uint64_t nq, int d, int metric, const void
   const size_t smem = sizeof(float) * ((size_t)d + kc);
   dispatch_metric_elem<true>(metric, vdt, [&](auto m, auto e) {
     using T = typename decltype(e)::type;
-    auto kern = refine_kernel<decltype(m)::value, T>;
+    auto kern = refine_kernel<decltype(m)::value, T, false>;
     set_smem(kern, smem);
     LB2_LAUNCH("refine", kern, (unsigned)nq, 256, smem, queries, d, reinterpret_cast<const T*>(vectors), num_vectors,
-               cand_id, cand_cnt, kc, k, out_id, out_d, out_cnt, has_lower, lower, has_upper, upper);
+               cand_id, cand_cnt, kc, k, out_id, out_d, out_cnt, has_lower, lower, has_upper, upper,
+               (const float*)nullptr, (const QueryOut*)nullptr, k);
+  });
+}
+
+void refine_batch_f32(const float* queries, uint64_t nq, int d, int metric, const void* vectors, int vdt,
+                      uint64_t num_vectors, const float* cand_d, const uint64_t* cand_id, const uint32_t* cand_cnt,
+                      int kc, const QueryOut* qo, int k_stride, uint64_t* out_id, float* out_d, uint32_t* out_cnt) {
+  if (nq == 0) return;
+  const size_t smem = sizeof(float) * ((size_t)d + kc);
+  dispatch_metric_elem<true>(metric, vdt, [&](auto m, auto e) {
+    using T = typename decltype(e)::type;
+    auto kern = refine_kernel<decltype(m)::value, T, true>;
+    set_smem(kern, smem);
+    LB2_LAUNCH("refine", kern, (unsigned)nq, 256, smem, queries, d, reinterpret_cast<const T*>(vectors), num_vectors,
+               cand_id, cand_cnt, kc, k_stride, out_id, out_d, out_cnt, 0, 0.0f, 0, 0.0f, cand_d, qo, k_stride);
   });
 }
 

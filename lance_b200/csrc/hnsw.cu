@@ -763,9 +763,10 @@ template <class Dist>
 __global__ void __launch_bounds__(32)
 hnsw_search_kernel(GraphDev g, uint64_t nslots, int np, const uint32_t* __restrict__ probe_ids,
                    const uint64_t* __restrict__ offsets, const uint32_t* __restrict__ acnt, const Dist proto,
-                   const uint64_t* __restrict__ row_ids, uint32_t ef, int kc, ScanFilter flt,
+                   const uint64_t* __restrict__ row_ids, uint32_t ef0, int kc, ScanFilter flt0,
                    float* __restrict__ cand_d, uint64_t* __restrict__ cand_id, uint32_t* __restrict__ cand_cnt,
-                   uint32_t* __restrict__ scratch, uint64_t nmax, uint32_t E, uint32_t B, uint32_t TW, uint32_t QW) {
+                   uint32_t* __restrict__ scratch, uint64_t nmax, uint32_t E, uint32_t B, uint32_t TW, uint32_t QW,
+                   const QueryParam* __restrict__ qp) {
   __shared__ uint32_t sh_n;
   const int lane = threadIdx.x & 31;
   if (!Dist::TABLE) TW = 0;
@@ -774,6 +775,11 @@ hnsw_search_kernel(GraphDev g, uint64_t nslots, int np, const uint32_t* __restri
   for (uint64_t slot = blockIdx.x; slot < nslots; slot += gridDim.x) {
     const uint64_t qi = slot / np;
     const uint32_t p = probe_ids[slot];
+    // the query's own k', ef, filter and allowed-row counts with per-query values (kc is then the lists' stride)
+    const int kq = qp ? qp[qi].k : kc;
+    const uint32_t ef = qp ? qp[qi].ef : ef0;
+    const ScanFilter flt = qp ? qp[qi].flt : flt0;
+    const uint32_t* __restrict__ ac = qp ? qp[qi].acnt : acnt;
     Dist P = proto;
     P.bind(offsets[p], (uint32_t)(offsets[p + 1] - offsets[p]));
     if (P.n == 0) {  // an empty partition returns no rows (builder.rs:695-697)
@@ -782,7 +788,7 @@ hnsw_search_kernel(GraphDev g, uint64_t nslots, int np, const uint32_t* __restri
     }
     const typename Dist::Ctx q = P.query_ctx(qi, p, s);  // dist_calculator(query)
     uint32_t R;
-    if (flt.allow && acnt[p] < (uint32_t)((uint64_t)P.n * 10 / 100)) {
+    if (flt.allow && ac[p] < (uint32_t)((uint64_t)P.n * 10 / 100)) {
       // HNSW::flat_search (builder.rs:238-280): allowed rows in node order, kept when lower < d <= upper.  Lane 0 drives
       // the reference's heap over the partition's rows, 32 distances at a time; this branch only runs when fewer than
       // 10 % of the rows are allowed.
@@ -797,7 +803,7 @@ hnsw_search_kernel(GraphDev g, uint64_t nslots, int np, const uint32_t* __restri
             const uint32_t key = s.bk[t];
             const int32_t sk = (int32_t)(key ^ 0x80000000u);
             if (sk <= flt.lo_key || sk > flt.hi_key) continue;
-            if (len < (uint32_t)kc) {
+            if (len < (uint32_t)kq) {
               rheap_push(s.rk, s.rid, len, key, c0 + t);
             } else if (key < s.rk[0]) {
               rheap_pop(s.rk, s.rid, len);
@@ -818,7 +824,7 @@ hnsw_search_kernel(GraphDev g, uint64_t nslots, int np, const uint32_t* __restri
       uint32_t ep = 0, ekey = P.key(q, 0);
       for (int level = g.max_level - 1; level >= 0; --level) greedy(g, P, q, level, ep, ekey, s);
       R = beam_search(g, P, q, 0, ep, ekey, ef, flt.allow, flt.lo_key, flt.hi_key, s);
-      R = min(R, (uint32_t)kc);
+      R = min(R, (uint32_t)kq);
     }
     for (uint32_t j = lane; j < R; j += 32) {
       cand_d[slot * kc + j] = float_of(s.rk[j]);
@@ -1219,10 +1225,11 @@ static void search_graphs(const IvfSearch& s, const HnswGraph& g, uint32_t ef, c
                           uint32_t QW) {
   const uint32_t kc = (uint32_t)s.k;
   if (ef == 0) ef = kc + kc / 2;
-  if (ef < kc) fail(LB2_INVALID_ARG, "%s: ef = %u must be greater than or equal to k = %u", g.kind, ef, kc);
+  // per-query values: every query's ef was resolved and checked by the caller, ef is the largest
+  if (ef < kc && !s.qp) fail(LB2_INVALID_ARG, "%s: ef = %u must be greater than or equal to k = %u", g.kind, ef, kc);
   if (!ivf_search_begin(s, 0, "%zu", 0)) return;
   DevBuf<uint32_t> acnt;
-  if (s.flt.allow) {  // `remained`: the allowed rows of each partition (builder.rs:715-718)
+  if (s.flt.allow && !s.qp) {  // `remained`: the allowed rows of each partition (builder.rs:715-718)
     acnt.alloc(s.K);
     partition_counts(s.part_offsets, s.K, s.flt.allow, 0xffffffffu, acnt.p);
   }
@@ -1239,7 +1246,7 @@ static void search_graphs(const IvfSearch& s, const HnswGraph& g, uint32_t ef, c
     P.at_slab(sl.q0);
     LB2_LAUNCH("hnsw_search", hnsw_search_kernel<Dist>, nct, 32, 0, dev_view(g), nslots, sl.np, sl.probe_ids,
                sl.offsets, acnt.p, P, s.row_ids, ef, (int)kc, s.flt, sl.cand_d, sl.cand_id, sl.cand_cnt, scratch.p,
-               nmax, E, B, TW, QW);
+               nmax, E, B, TW, QW, s.qp_at(sl.q0));
   });
 }
 

@@ -274,6 +274,27 @@ static void export_common(const lb2_index* index, void* centroids_out, uint64_t*
     LB2_CUDA(cudaMemcpyAsync(row_ids_out, index->row_ids.p, sizeof(uint64_t) * index->n, cudaMemcpyDefault, s));
 }
 
+static void search_kind(lb2_index* index, const IvfSearch& s, uint32_t ef);
+
+// the queries of every lb2_index_search*: the index's element type -> f32 (q), normalised under cosine (knn.rs:497-499;
+// get() is the search's view)
+namespace {
+struct SearchQueries {
+  VecIn q;
+  DevBuf<float> qn;
+  const float* p;
+  SearchQueries(const lb2_index* index, const void* queries, uint64_t nq)
+      : q(queries, (size_t)nq * index->d, index->dtype), p(q.get()) {
+    if (index->metric == METRIC_COSINE) {
+      qn.alloc((size_t)nq * index->d);
+      normalize_rows(p, nq, index->d, qn.p);
+      p = qn.p;
+    }
+  }
+  const float* get() const { return p; }
+};
+}  // namespace
+
 // one implementation behind every lb2_index_search* (pr: the probe rule of lb2_index_search_probed; ef: the graph
 // search's ef of lb2_index_search_hnsw, 0 for k' + k' / 2)
 static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq, const lb2_search_params& sp,
@@ -285,14 +306,8 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
   const uint64_t kc = refine ? (uint64_t)k * sp.refine_factor : k;
   if (kc > 1024) fail(LB2_UNSUPPORTED, "k * refine_factor = %llu > 1024 is not implemented", (unsigned long long)kc);
   const int d = index->d;
-  VecIn q(queries, (size_t)nq * d, index->dtype);
+  const SearchQueries q(index, queries, nq);
   const float* qp = q.get();
-  DevBuf<float> qn;
-  if (index->metric == METRIC_COSINE) {  // knn.rs:497-499
-    qn.alloc((size_t)nq * d);
-    normalize_rows(qp, nq, d, qn.p);
-    qp = qn.p;
-  }
   InArg<uint64_t> allow(sp.allow_bitmap, sp.allow_bitmap ? (size_t)((index->n + 63) / 64) : 0);
   OutArg<uint64_t> oi(row_ids_out, (size_t)nq * k);
   OutArg<float> od(dists_out, (size_t)nq * k);
@@ -313,11 +328,28 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
                                     sp.has_upper_bound != 0, sp.upper_bound);
   const IvfSearch s{index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->row_ids.p, qp, nq,
                     (int)kc, (int)nprobes, si, sd, sc, flt, pr};
+  search_kind(index, s, ef);
+  if (refine) {
+    // exact re-rank with the true metric on the ORIGINAL (un-normalised) query, as flat_knn does; the
+    // plan then filters `_distance >= lower AND _distance < upper` on the exact distances (scanner.rs:3342-3377)
+    InArg<uint8_t> v(sp.refine_vectors, (size_t)sp.num_vectors * d * dtype_size(index->dtype));  // raw column, native type
+    refine_f32(q.q.get(), nq, d, index->metric, v.get(), (int)index->dtype, sp.num_vectors, cid.p, ccnt.p, (int)kc, (int)k,
+               oi.get(), od.get(), oc.get(), sp.has_lower_bound != 0, sp.lower_bound, sp.has_upper_bound != 0,
+               sp.upper_bound);
+  }
+  oi.commit(); od.commit(); oc.commit();
+  if (!ctx().async_call) sync_stream();
+}
+
+// the scan of the index's kind over the search s (ef: IVF_HNSW_*'s graph search ef, 0 for k' + k' / 2)
+static void search_kind(lb2_index* index, const IvfSearch& s, uint32_t ef) {
+  const uint64_t nq = s.nq;
+  const int d = s.d;
   DevBuf<uint8_t> qcodes;
   if (index->kind == IndexKind::SQ) {
     // the (normalised) query is encoded with the index's bounds, not turned into a residual (sq/storage.rs:404-430)
     qcodes.alloc(std::max<uint64_t>(1, nq * d));
-    sq_encode_f32(qp, nq * d, index->sq_lower, index->sq_upper, qcodes.p);
+    sq_encode_f32(s.queries, nq * d, index->sq_lower, index->sq_upper, qcodes.p);
   }
   if (index->hnsw) {  // IVF_HNSW_*: the kind's scan distances, searched through each partition's graph
     hnsw_search(s, *index, qcodes.p, ef);
@@ -341,16 +373,6 @@ static void index_search_impl(lb2_index* index, const void* queries, uint64_t nq
         break;
     }
   }
-  if (refine) {
-    // exact re-rank with the true metric on the ORIGINAL (un-normalised) query, as flat_knn does; the
-    // plan then filters `_distance >= lower AND _distance < upper` on the exact distances (scanner.rs:3342-3377)
-    InArg<uint8_t> v(sp.refine_vectors, (size_t)sp.num_vectors * d * dtype_size(index->dtype));  // raw column, native type
-    refine_f32(q.get(), nq, d, index->metric, v.get(), (int)index->dtype, sp.num_vectors, cid.p, ccnt.p, (int)kc, (int)k,
-               oi.get(), od.get(), oc.get(), sp.has_lower_bound != 0, sp.lower_bound, sp.has_upper_bound != 0,
-               sp.upper_bound);
-  }
-  oi.commit(); od.commit(); oc.commit();
-  if (!ctx().async_call) sync_stream();
 }
 
 // ---- partition ownership: device all-to-all (SURVEY 8e "partition build", 8f-4) ---------------------------------
@@ -1031,6 +1053,163 @@ lb2_status lb2_index_search_hnsw(lb2_index* index, const void* queries, uint64_t
     LB2_REQUIRE(sp->refine_factor == 0 || sp->refine_vectors, "refine_factor > 0 needs refine_vectors");
     index_search_impl(index, queries, nq, *sp, row_ids_out, dists_out, counts_out, nullptr, ef);
   }
+  sync_stream();
+  LB2_API_END
+}
+
+// A batch of queries with their own parameters in one pass (include/lance_b200.h).  Every query's own call is
+// checked first, so a refusal writes nothing.  The filters are staged once; each query's k', filter, range and ef
+// go to the device as one QueryParam per query for the scan kernels and one QueryOut per query for the finish
+// (refine or copy to rows of k_stride).  The lists are as long as the batch's largest k' and the probe grid as wide
+// as its largest nprobes; a query's other slots probe the empty partition.  A batch with minimum / maximum nprobes
+// queries runs the probe rule for every query, each with its own QueryProbe: a fixed nprobes p is minimum = maximum =
+// p, which lb2_index_search_probed defines to equal lb2_index_search_ex.
+lb2_status lb2_index_search_batch(lb2_index* index, const void* queries, uint64_t nq, const lb2_query_params* params,
+                                  const lb2_query_filter* filters, uint32_t num_filters, const void* refine_vectors,
+                                  uint64_t num_vectors, uint32_t late_width, uint32_t k_stride, uint64_t* row_ids_out,
+                                  float* dists_out, uint32_t* counts_out, uint32_t* nprobes_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index, "null index");
+  LB2_REQUIRE(nq == 0 || (queries && params), "null queries or params");
+  LB2_REQUIRE(num_filters == 0 || filters, "null filters");
+  LB2_REQUIRE(late_width >= 1, "late_width must be at least 1");
+  const uint32_t K = (uint32_t)index->K;
+  uint32_t kmax = 0, kcmax = 0, npmax = 0, efmax = 0, Lmax = 0;
+  bool any_refine = false, any_filter = false, any_range = false, any_probed = false;
+  for (uint64_t q = 0; q < nq; ++q) {
+    const lb2_query_params& p = params[q];
+    const unsigned long long qi = (unsigned long long)q;
+    LB2_REQUIRE(p.k > 0, "query %llu: k must be positive", qi);
+    LB2_REQUIRE(p.filter < num_filters || p.filter == UINT32_MAX, "query %llu: filter %u is not below num_filters %u",
+                qi, p.filter, num_filters);
+    LB2_REQUIRE(p.ef == 0 || index->hnsw, "query %llu: ef is set on an index without HNSW graphs", qi);
+    LB2_REQUIRE(p.refine_factor == 0 || refine_vectors, "query %llu: refine_factor > 0 needs refine_vectors", qi);
+    if (p.nprobes == 0) {  // lb2_index_search_probed's checks
+      LB2_REQUIRE(p.minimum_nprobes >= 1, "query %llu: minimum_nprobes must be at least 1", qi);
+      LB2_REQUIRE(p.maximum_nprobes == 0 || p.maximum_nprobes >= p.minimum_nprobes,
+                  "query %llu: maximum_nprobes %u is below minimum_nprobes %u", qi, p.maximum_nprobes,
+                  p.minimum_nprobes);
+      LB2_REQUIRE(p.filter == UINT32_MAX || filters[p.filter].allow_bitmap ||
+                      (!filters[p.filter].has_max_len && !filters[p.filter].mask_ids),
+                  "query %llu: max_len and mask_ids need an allow bitmap", qi);
+      any_probed = true;
+    }
+    const uint64_t kc = (uint64_t)p.k * std::max<uint32_t>(1, p.refine_factor);
+    if (kc > 1024)
+      fail(LB2_UNSUPPORTED, "query %llu: k * refine_factor = %llu > 1024 is not implemented", qi, (unsigned long long)kc);
+    const uint32_t ef = p.ef ? p.ef : (uint32_t)(kc + kc / 2);
+    if (index->hnsw && ef < kc)
+      fail(LB2_INVALID_ARG, "query %llu: %s: ef = %u must be greater than or equal to k = %u", qi, index->hnsw->kind, ef,
+           (uint32_t)kc);
+    kmax = std::max(kmax, p.k);
+    kcmax = std::max(kcmax, (uint32_t)kc);
+    npmax = std::max(npmax, std::min(p.nprobes, K));
+    const uint32_t mx = p.nprobes ? p.nprobes : p.maximum_nprobes;
+    Lmax = std::max(Lmax, mx ? std::min(mx, K) : K);
+    efmax = std::max(efmax, ef);
+    any_refine |= p.refine_factor > 0;
+    any_filter |= p.filter != UINT32_MAX || p.has_lower_bound || p.has_upper_bound;
+    any_range |= p.has_lower_bound || p.has_upper_bound;
+  }
+  LB2_REQUIRE(k_stride >= kmax, "k_stride %u is below the largest k %u", k_stride, kmax);
+  if (current_comm() && current_comm()->nranks > 1)
+    fail(LB2_UNSUPPORTED, "a batch search on a row-sharded index is not implemented");
+  if (nq == 0) {
+    sync_stream();
+    return LB2_OK;
+  }
+  const int d = index->d;
+  const SearchQueries q(index, queries, nq);
+  // the filters, staged once each (with the probe rule also their allow lists' ids), and their allowed rows per
+  // partition in one launch: IVF_HNSW_*'s `remained`, and the probe rule's c_p (row num_filters: no prefilter)
+  const size_t words = (size_t)((index->n + 63) / 64);
+  std::vector<InArg<uint64_t>> allow(num_filters), ids(num_filters);
+  std::vector<const uint64_t*> allow_h(num_filters + 1, nullptr), ids_h(num_filters, nullptr);
+  DevBuf<uint64_t> no_ids(1);  // an iterable, empty allow list
+  for (uint32_t f = 0; f < num_filters; ++f) {
+    allow[f].set(filters[f].allow_bitmap, filters[f].allow_bitmap ? words : 0);
+    allow_h[f] = allow[f].get();
+    if (any_probed && filters[f].mask_ids) {
+      ids[f].set(filters[f].mask_ids, filters[f].num_mask_ids);
+      ids_h[f] = ids[f].get() ? ids[f].get() : no_ids.p;
+    }
+  }
+  DevBuf<uint32_t> acnt;
+  if ((index->hnsw && num_filters) || any_probed) {
+    DevBuf<const uint64_t*> tab(num_filters + 1);
+    h2d(tab.p, allow_h.data(), num_filters + 1);
+    acnt.alloc((size_t)(num_filters + 1) * K);
+    partition_counts_table(index->part_offsets.p, (int)K, tab.p, (int)num_filters + 1, acnt.p);
+  }
+  std::vector<QueryProbe> qpr_h(any_probed ? nq : 0);
+  bool any_iterable = false;
+  std::vector<QueryParam> qp_h(nq);
+  std::vector<QueryOut> qo_h(nq);
+  std::vector<uint32_t> qnp_h(nq);
+  for (uint64_t i = 0; i < nq; ++i) {
+    const lb2_query_params& p = params[i];
+    const bool filtered = p.filter != UINT32_MAX && allow_h[p.filter];
+    const int kc = (int)p.k * (int)std::max<uint32_t>(1, p.refine_factor);
+    qp_h[i].flt = make_filter(filtered ? allow_h[p.filter] : nullptr, p.has_lower_bound != 0, p.lower_bound,
+                              p.has_upper_bound != 0, p.upper_bound);
+    qp_h[i].k = kc;
+    qp_h[i].ef = p.ef ? p.ef : (uint32_t)(kc + kc / 2);
+    qp_h[i].acnt = filtered && acnt.p ? acnt.p + (size_t)p.filter * K : nullptr;
+    qo_h[i] = QueryOut{kc, (int)p.k, p.refine_factor > 0, (int)(p.has_lower_bound != 0), (int)(p.has_upper_bound != 0),
+                       p.lower_bound, p.upper_bound};
+    qnp_h[i] = std::min(p.nprobes, K);
+    if (any_probed) {  // a fixed nprobes p: minimum = maximum = p, no shortcut
+      const uint32_t f = p.filter == UINT32_MAX ? num_filters : p.filter;
+      const bool probed = p.nprobes == 0;
+      const uint32_t mx = probed ? p.maximum_nprobes : p.nprobes;
+      const uint64_t* mids = probed && f < num_filters ? ids_h[f] : nullptr;
+      qpr_h[i] = QueryProbe{probed ? p.minimum_nprobes : p.nprobes, mx ? std::min(mx, K) : K, p.k, (uint32_t)kc,
+                            p.has_lower_bound || p.has_upper_bound, probed && f < num_filters && filters[f].has_max_len, probed && f < num_filters ?
+                            filters[f].max_len : 0, mids, mids ? filters[f].num_mask_ids : 0,
+                            acnt.p + (size_t)(allow_h[f] ? f : num_filters) * K};
+      any_iterable |= mids != nullptr;
+    }
+  }
+  DevBuf<QueryParam> qp(nq);
+  DevBuf<QueryOut> qo(nq);
+  DevBuf<uint32_t> qnp(nq);
+  h2d(qp.p, qp_h.data(), nq);
+  h2d(qo.p, qo_h.data(), nq);
+  h2d(qnp.p, qnp_h.data(), nq);
+  DevBuf<QueryProbe> qpr(qpr_h.size());
+  if (any_probed) h2d(qpr.p, qpr_h.data(), nq);
+  OutArg<uint64_t> oi(row_ids_out, (size_t)nq * k_stride);
+  OutArg<float> od(dists_out, (size_t)nq * k_stride);
+  OutArg<uint32_t> oc(counts_out, nq);
+  OutArg<uint32_t> onp(nprobes_out, nq);
+  DevBuf<uint64_t> cid((size_t)nq * kcmax);
+  DevBuf<float> cdist((size_t)nq * kcmax);
+  DevBuf<uint32_t> ccnt(nq);
+  {
+    TagScope tg("search");
+    IvfSearch s{index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->row_ids.p, q.get(), nq,
+                (int)kcmax, (int)npmax, cid.p, cdist.p, ccnt.p, ScanFilter{}, nullptr};
+    s.qp = qp.p;
+    s.qp_host = qp_h.data();
+    s.qnp = qnp.p;
+    s.any_filter = any_filter;
+    s.any_range = any_range;
+    ProbeRule pr;
+    if (any_probed) {
+      pr.max_np = Lmax;
+      pr.late_width = late_width;
+      pr.mask_ids = any_iterable ? no_ids.p : nullptr;  // non-null: lists get a shortcut slot
+      pr.nprobes_out = onp.get();
+      pr.qpr = qpr.p;
+      s.pr = &pr;
+    }
+    search_kind(index, s, efmax);
+    InArg<uint8_t> v(any_refine ? refine_vectors : nullptr, (size_t)num_vectors * d * dtype_size(index->dtype));
+    refine_batch_f32(q.q.get(), nq, d, index->metric, v.get(), (int)index->dtype, num_vectors, cdist.p, cid.p, ccnt.p,
+                     (int)kcmax, qo.p, (int)k_stride, oi.get(), od.get(), oc.get());
+  }
+  if (onp.get() && !any_probed) h2d(onp.get(), qnp_h.data(), nq);
+  oi.commit(); od.commit(); oc.commit(); onp.commit();
   sync_stream();
   LB2_API_END
 }

@@ -49,7 +49,7 @@ __global__ void __launch_bounds__(256)
 merge_rank_kernel(const float* __restrict__ cand_d, const uint64_t* __restrict__ cand_id,
                   const uint32_t* __restrict__ cand_cnt, int np, int k, size_t stride_p_d, size_t stride_p_id,
                   size_t stride_q, size_t cnt_stride_p, size_t cnt_stride_q, int nl, uint64_t* __restrict__ out_id,
-                  float* __restrict__ out_d, uint32_t* __restrict__ out_cnt) {
+                  float* __restrict__ out_d, uint32_t* __restrict__ out_cnt, const QueryParam* __restrict__ qp) {
   extern __shared__ __align__(16) unsigned char mr_smem[];
   const int total = np * k;
   uint64_t* s_id = reinterpret_cast<uint64_t*>(mr_smem);             // [total]
@@ -59,6 +59,7 @@ merge_rank_kernel(const float* __restrict__ cand_d, const uint64_t* __restrict__
   const int ng = nl > np ? (nl + np - 1) / np : 1;
   const size_t q = qi / ng;
   const int first = (int)(qi % ng) * np;
+  const int kq = qp ? qp[q].k : k;  // the query's own output length; the lists' stride stays k
   const int tid = threadIdx.x;
   if (tid == 0) s_valid = 0;
   __syncthreads();
@@ -81,12 +82,12 @@ merge_rank_kernel(const float* __restrict__ cand_d, const uint64_t* __restrict__
       const int32_t kj = s_key[j];
       rank += (kj < key || (kj == key && s_id[j] < id)) ? 1 : 0;
     }
-    if (rank < k) {
+    if (rank < kq) {
       out_id[qi * k + rank] = id;
       out_d[qi * k + rank] = key_to_float(key);
     }
   }
-  const int r = min((uint32_t)k, s_valid);
+  const int r = min((uint32_t)kq, s_valid);
   for (int e = r + tid; e < k; e += 256) {
     out_id[qi * k + e] = ~0ull;
     out_d[qi * k + e] = __int_as_float(0x7f800000);
@@ -98,14 +99,14 @@ __global__ void __launch_bounds__(128)
 merge_kernel(const float* __restrict__ cand_d, const uint64_t* __restrict__ cand_id,
              const uint32_t* __restrict__ cand_cnt, int np, int k, size_t stride_p_d, size_t stride_p_id,
              size_t stride_q, size_t cnt_stride_p, size_t cnt_stride_q, int nl, uint64_t* __restrict__ out_id,
-             float* __restrict__ out_d, uint32_t* __restrict__ out_cnt) {
+             float* __restrict__ out_d, uint32_t* __restrict__ out_cnt, const QueryParam* __restrict__ qp) {
   const size_t qi = blockIdx.x;
   const int ng = nl > np ? (nl + np - 1) / np : 1;
   const size_t q = qi / ng;
   const int first = (int)(qi % ng) * np;
   const int tid = threadIdx.x;
   const int r = (int)emit_ascending<128>(
-      k, np * k,
+      qp ? qp[q].k : k, np * k,
       [&](uint32_t c, int32_t& key, uint64_t& id) {
         const int pi = first + c / k, e = c % k;
         if (pi >= nl || (uint32_t)e >= cand_cnt[pi * cnt_stride_p + q * cnt_stride_q]) return false;
@@ -134,17 +135,18 @@ void find_partitions_f32(const float* centroids, int K, int d, int metric, const
 
 void merge_lists(const char* name, uint64_t nq, const float* cand_d, const uint64_t* cand_id, const uint32_t* cand_cnt,
                  int np, int k, size_t stride_p_d, size_t stride_p_id, size_t stride_q, size_t cnt_stride_p,
-                 size_t cnt_stride_q, uint64_t* out_ids, float* out_dists, uint32_t* out_counts, int nl) {
+                 size_t cnt_stride_q, uint64_t* out_ids, float* out_dists, uint32_t* out_counts, int nl,
+                 const QueryParam* qp) {
   if (nq == 0) return;
   if (nl < np) nl = np;
   const uint64_t blocks = nq * (uint64_t)(nl > np ? (nl + np - 1) / np : 1);
   const size_t total = (size_t)np * k;
   if (total <= (size_t)MERGE_RANK_MAX) {
     LB2_LAUNCH(name, merge_rank_kernel, (unsigned)blocks, 256, total * 12, cand_d, cand_id, cand_cnt, np, k, stride_p_d,
-               stride_p_id, stride_q, cnt_stride_p, cnt_stride_q, nl, out_ids, out_dists, out_counts);
+               stride_p_id, stride_q, cnt_stride_p, cnt_stride_q, nl, out_ids, out_dists, out_counts, qp);
   } else {
     LB2_LAUNCH(name, merge_kernel, (unsigned)blocks, 128, 0, cand_d, cand_id, cand_cnt, np, k, stride_p_d, stride_p_id,
-               stride_q, cnt_stride_p, cnt_stride_q, nl, out_ids, out_dists, out_counts);
+               stride_q, cnt_stride_p, cnt_stride_q, nl, out_ids, out_dists, out_counts, qp);
   }
 }
 
@@ -177,20 +179,50 @@ void merge_list_tree(const char* name, uint64_t nq, const float* cand_d, const u
 // partitions are found with L2 on the (normalised) vectors for cosine (ivf.rs:149-185)
 static int probe_metric(int metric) { return metric == METRIC_DOT ? METRIC_DOT : METRIC_L2; }
 
+// part_offsets with one more, empty, partition K: the probe id of a slot that searches nothing
+static void ext_offsets(const uint64_t* part_offsets, int K, DevBuf<uint64_t>& ext) {
+  ext.alloc((size_t)K + 2);
+  d2d(ext.p, part_offsets, (size_t)K + 1);
+  d2d(ext.p + K + 1, part_offsets + K, 1);
+}
+
 // The IVF query skeleton: the np nearest partitions of every query, one candidate list of <= k per (query, probe)
-// slot, the lists merged per query.
+// slot, the lists merged per query.  With per-query probe counts (s.qnp) np is the largest: a query's first qnp[q]
+// of its np nearest are its own nearest qnp[q], and its other slots probe the empty partition K; a batch holds its
+// candidate lists in sub-slabs of about 256 MB (scan, then merge, per sub-slab).
 static void ivf_search(const IvfSearch& s, int np, ScanRef scan) {
   const uint64_t nq = s.nq;
   const int k = s.k;
-  DevBuf<uint32_t> pids((size_t)nq * np), cand_cnt((size_t)nq * np);
-  DevBuf<float> pd((size_t)nq * np), cand_d((size_t)nq * np * k);
-  DevBuf<uint64_t> cand_id((size_t)nq * np * k);
+  const uint64_t per_q = (uint64_t)np * k * 12 + 4ull * np;
+  const uint64_t sub = s.qp ? std::max<uint64_t>(1, std::min<uint64_t>(nq, (256ull << 20) / per_q)) : nq;
+  DevBuf<uint32_t> pids((size_t)nq * np), cand_cnt((size_t)sub * np);
+  DevBuf<float> pd((size_t)nq * np), cand_d((size_t)sub * np * k);
+  DevBuf<uint64_t> cand_id((size_t)sub * np * k);
   find_partitions_f32(s.centroids, s.K, s.d, probe_metric(s.metric), s.queries, nq, np, pids.p, pd.p);
-  for (uint64_t q0 = 0; q0 < nq; q0 += SEARCH_SLAB)
-    scan({q0, std::min<uint64_t>(SEARCH_SLAB, nq - q0), np, s.part_offsets, pids.p + q0 * np, pd.p + q0 * np,
-          cand_d.p + q0 * np * k, cand_id.p + q0 * np * k, cand_cnt.p + q0 * np});
-  merge_lists("merge_topk", nq, cand_d.p, cand_id.p, cand_cnt.p, np, k, (size_t)k, (size_t)k, (size_t)np * k, (size_t)1,
-              (size_t)np, s.out_ids, s.out_dists, s.out_counts);
+  const uint64_t* offsets = s.part_offsets;
+  DevBuf<uint64_t> ext;
+  DevBuf<uint32_t> own_ids;
+  DevBuf<float> own_pd;
+  if (s.qnp) {
+    ext_offsets(s.part_offsets, s.K, ext);
+    own_ids.alloc((size_t)nq * np);
+    own_pd.alloc((size_t)nq * np);
+    gather_probes(nq, np, pids.p, pd.p, s.qnp, np, (uint32_t)s.K, own_ids.p, own_pd.p);
+    std::swap(pids, own_ids);
+    std::swap(pd, own_pd);
+    offsets = ext.p;
+  }
+  for (uint64_t a = 0; a < nq; a += sub) {
+    const uint64_t b = std::min(sub, nq - a);
+    for (uint64_t q0 = a; q0 < a + b; q0 += SEARCH_SLAB) {
+      const uint64_t c = q0 - a;  // the query's place in the sub-slab's lists
+      scan({q0, std::min<uint64_t>(SEARCH_SLAB, a + b - q0), np, offsets, pids.p + q0 * np, pd.p + q0 * np,
+            cand_d.p + c * np * k, cand_id.p + c * np * k, cand_cnt.p + c * np});
+    }
+    merge_lists("merge_topk", b, cand_d.p, cand_id.p, cand_cnt.p, np, k, (size_t)k, (size_t)k, (size_t)np * k,
+                (size_t)1, (size_t)np, s.out_ids + a * k, s.out_dists + a * k, s.out_counts ? s.out_counts + a : nullptr,
+                0, s.qp_at(a));
+  }
 }
 
 // The same skeleton with a per-query probe count (probe.cu): per slab of queries every centroid distance is ranked
@@ -206,13 +238,14 @@ static void ivf_search_probed(const IvfSearch& s, ScanRef scan) {
   const int K = s.K, d = s.d, kc = s.k;
   if (nq == 0) return;
   const int L = pr.max_np ? (int)std::min<uint32_t>(pr.max_np, (uint32_t)K) : K;
-  const bool by_scan = s.flt.range != 0;
+  // a batch scans every query's L partitions first when any of its queries has a range; the cutoff then takes a
+  // ranged query's c_p from its list counts and every other query's from its prefilter's counts, as its own call does
+  const bool by_scan = s.pr->qpr ? s.any_range : s.flt.range != 0;
   const int extra = pr.mask_ids ? 1 : 0;
-  DevBuf<uint64_t> ext_offsets((size_t)K + 2);
-  d2d(ext_offsets.p, s.part_offsets, (size_t)K + 1);
-  d2d(ext_offsets.p + K + 1, s.part_offsets + K, 1);
+  DevBuf<uint64_t> ext;
+  ext_offsets(s.part_offsets, K, ext);
   DevBuf<uint32_t> cpart;
-  if (!by_scan) {
+  if (!by_scan && !pr.qpr) {
     cpart.alloc(K);
     partition_counts(s.part_offsets, K, s.flt.allow, (uint32_t)kc, cpart.p);
   }
@@ -226,10 +259,11 @@ static void ivf_search_probed(const IvfSearch& s, ScanRef scan) {
     centroid_distances(s.queries + q0 * d, qn, d, s.centroids, K, probe_metric(s.metric), all.p);
     rank_probes(all.p, qn, K, L, pids.p, pd.p);
     uint32_t* nprobes_out = pr.nprobes_out ? pr.nprobes_out + q0 : nullptr;
+    const QueryProbe* qpr = pr.qpr ? pr.qpr + q0 : nullptr;
     int np = L;
     if (!by_scan) {
       nmax.zero();
-      probe_cutoff(pr, qn, L, pids.p, pd.p, cpart.p, nullptr, 0, nsearch.p, shortcut.p, nmax.p, nprobes_out);
+      probe_cutoff(pr, qn, L, pids.p, pd.p, cpart.p, nullptr, 0, nsearch.p, shortcut.p, nmax.p, nprobes_out, qpr);
       uint32_t h = 0;
       d2h(&h, nmax.p, 1);
       sync_stream();
@@ -238,7 +272,7 @@ static void ivf_search_probed(const IvfSearch& s, ScanRef scan) {
     const int nl = np + extra;  // slots per query
     DevBuf<uint32_t> sp((size_t)qn * nl);
     DevBuf<float> spd((size_t)qn * nl);
-    gather_probes(qn, L, pids.p, pd.p, by_scan ? nullptr : nsearch.p, nl, (uint32_t)K, sp.p, spd.p);
+    gather_probes(qn, L, pids.p, pd.p, by_scan ? nullptr : nsearch.p, nl, (uint32_t)K, sp.p, spd.p, qpr);
     const uint64_t per_q = (uint64_t)nl * kc * 12 + 4 * (uint64_t)nl;
     const uint64_t sub = std::max<uint64_t>(1, std::min<uint64_t>(qn, (256ull << 20) / per_q));
     DevBuf<float> cd(sub * nl * kc);
@@ -246,14 +280,16 @@ static void ivf_search_probed(const IvfSearch& s, ScanRef scan) {
     DevBuf<uint32_t> ccnt(sub * nl);
     for (uint64_t a = 0; a < qn; a += sub) {
       const uint64_t b = std::min(sub, qn - a);
-      scan({q0 + a, b, nl, ext_offsets.p, sp.p + a * nl, spd.p + a * nl, cd.p, cid.p, ccnt.p});
+      scan({q0 + a, b, nl, ext.p, sp.p + a * nl, spd.p + a * nl, cd.p, cid.p, ccnt.p});
       if (by_scan)
         probe_cutoff(pr, b, L, pids.p + a * L, pd.p + a * L, nullptr, ccnt.p, nl, nsearch.p + a, shortcut.p + a,
-                     nmax.p, nprobes_out ? nprobes_out + a : nullptr);
-      if (extra) shortcut_lists(b, shortcut.p + a, pr.mask_ids, pr.num_mask_ids, nl, kc, cd.p, cid.p, ccnt.p);
+                     nmax.p, nprobes_out ? nprobes_out + a : nullptr, qpr ? qpr + a : nullptr);
+      if (extra)
+        shortcut_lists(b, shortcut.p + a, pr.mask_ids, pr.num_mask_ids, nl, kc, cd.p, cid.p, ccnt.p,
+                       qpr ? qpr + a : nullptr);
       merge_lists("merge_topk", b, cd.p, cid.p, ccnt.p, nl, kc, (size_t)kc, (size_t)kc, (size_t)nl * kc, (size_t)1,
                   (size_t)nl, s.out_ids + (q0 + a) * kc, s.out_dists + (q0 + a) * kc,
-                  s.out_counts ? s.out_counts + q0 + a : nullptr);
+                  s.out_counts ? s.out_counts + q0 + a : nullptr, 0, s.qp_at(q0 + a));
     }
   }
 }

@@ -30,15 +30,33 @@ inline ScanFilter make_filter(const uint64_t* allow, int has_lower, float lower,
   return f;
 }
 
+// One query of a batch whose queries differ in their parameters (lb2_index_search_batch), on the device.  A scan
+// kernel reads its slot's query here; a search without the array gives every query IvfSearch::k and ::flt.
+struct QueryParam {
+  ScanFilter flt;        // the query's prefilter (device bitmap, nullable) and range
+  int k;                 // k' = k * max(1, refine_factor): the query's list length (<= IvfSearch::k, the list stride)
+  uint32_t ef;           // IVF_HNSW_*: the graph search's ef, >= k'
+  const uint32_t* acnt;  // IVF_HNSW_*: allowed rows per partition under the query's prefilter (null: no prefilter)
+};
+
 // One search of an IVF index, whatever its kind: the coarse model, the partition layout, the queries (f32,
 // normalised for cosine), what to return and where.  pr (nullable): search with the probe rule instead of nprobes
 // (k is then k * refine_factor, pr->k the query's k).
+// qp (nullable, device [nq]): per-query k' and filter; k is then the largest k', nprobes the largest probe count,
+// qnp (device [nq]) each query's own min(nprobes, K), and `filtering` tells whether any query filters.  The merge
+// writes query q's k'_q best at out[q * k], padded to k.  With per-query probe rules (pr->qpr) any_range tells whether
+// any query has a range, and the candidate lists are held in sub-slabs of about 256 MB.
 struct IvfSearch {
   const float* centroids; int K, d, metric;
   const uint64_t* part_offsets; const uint64_t* row_ids;
   const float* queries; uint64_t nq; int k; int nprobes;
   uint64_t* out_ids; float* out_dists; uint32_t* out_counts;
   ScanFilter flt; const ProbeRule* pr;
+  const QueryParam* qp = nullptr; const uint32_t* qnp = nullptr; bool any_filter = false, any_range = false;
+  const QueryParam* qp_host = nullptr;  // the same table on the host (route choices), with qp
+  bool filtering() const { return qp ? any_filter : (flt.allow != nullptr || flt.range != 0); }
+  // the per-query values of the queries from q0 on (null without them)
+  const QueryParam* qp_at(uint64_t q0) const { return qp ? qp + q0 : nullptr; }
 };
 
 // What a scan is asked to fill: the candidate lists of queries [q0, q0 + qn) (at most SEARCH_SLAB of them: the
@@ -76,9 +94,11 @@ void find_partitions_f32(const float* centroids, int K, int d, int metric, const
 // (~0, +inf).  List pi of query q: distances at cand_d[pi * stride_p_d + q * stride_q], ids likewise, count at
 // cand_cnt[pi * cnt_stride_p + q * cnt_stride_q].  nl > np: the query's nl lists are merged in groups of np
 // (output row q * ceil(nl / np) + group).
+// qp (nullable, nl == np): query q keeps its own qp[q].k best (<= k), padded to k.
 void merge_lists(const char* name, uint64_t nq, const float* cand_d, const uint64_t* cand_id, const uint32_t* cand_cnt,
                  int np, int k, size_t stride_p_d, size_t stride_p_id, size_t stride_q, size_t cnt_stride_p,
-                 size_t cnt_stride_q, uint64_t* out_ids, float* out_dists, uint32_t* out_counts, int nl = 0);
+                 size_t cnt_stride_q, uint64_t* out_ids, float* out_dists, uint32_t* out_counts, int nl = 0,
+                 const QueryParam* qp = nullptr);
 // [nq][nl][k] lists (counts [nq][nl]) -> [nq][k], any nl >= 1, by rank-counting merges only
 void merge_list_tree(const char* name, uint64_t nq, const float* cand_d, const uint64_t* cand_id,
                      const uint32_t* cand_cnt, int nl, int k, uint64_t* out_ids, float* out_dists,

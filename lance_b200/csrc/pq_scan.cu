@@ -12,6 +12,7 @@
 // position) pairs.
 #include <algorithm>
 #include <type_traits>
+#include <vector>
 
 #include "common.cuh"
 #include "exact.cuh"
@@ -34,6 +35,10 @@ struct ScanArgs {
   const uint32_t* probe_ids; int np; const uint64_t* part_offsets; const uint8_t* codes;
   const uint64_t* row_ids; int k; float* cand_d; uint64_t* cand_id; uint32_t* cand_cnt;
   ScanFilter flt;
+  const QueryParam* qp;  // per-query k' and filter of the slab's queries (k is then the lists' stride), or null
+  // the (slab-relative) queries a launch covers, one route's group of a batch: grid row / slot group g is query
+  // qlist[g]; null: every query of the slab
+  const uint32_t* qlist = nullptr;
 };
 
 // the residual query of partition p (v2.rs:316-332) and its LUT, in shared memory (256 threads)
@@ -95,16 +100,19 @@ __device__ __forceinline__ void pq4_quantize(const float* lut, int M, uint64_t f
   __syncthreads();
 }
 
-template <int METRIC, int NBITS>
+// BATCH: the slot's query's k' and filter come from a.qp; the single-parameter scan is compiled without the lookup
+template <int METRIC, int NBITS, bool BATCH>
 __device__ void radix_slot(const ScanArgs& a, size_t slot, bool replay) {
   extern __shared__ float smem[];
-  const int M = a.M, d = a.d, k = a.k, np = a.np;
+  const int M = a.M, d = a.d, np = a.np;
   float* lut = smem;                         // [M*16] (4-bit) or [M*256] (8-bit)
   float* qr = lut + M * (NBITS == 4 ? 16 : 256);  // [d]
-  const SlotSmem s(qr + d, k + 1);
   const int tid = threadIdx.x;
   const int pi = (int)(slot % np);
   const size_t qi = slot / np;
+  const int k = BATCH ? a.qp[qi].k : a.k;  // a.k: the lists' stride
+  const ScanFilter& flt = BATCH ? a.qp[qi].flt : a.flt;
+  const SlotSmem s(qr + d, k + 1);
   const uint32_t p = a.probe_ids[qi * np + pi];
   const uint64_t off = a.part_offsets[p];
   const uint32_t n_p = (uint32_t)(a.part_offsets[p + 1] - off);
@@ -133,7 +141,7 @@ __device__ void radix_slot(const ScanArgs& a, size_t slot, bool replay) {
     }
     return dist;
   };
-  if (NBITS == 4 && a.flt.allow == nullptr)  // the selection's (still unused) key buffer is the scratch
+  if (NBITS == 4 && flt.allow == nullptr)  // the selection's (still unused) key buffer is the scratch
     pq4_quantize(lut, M, flat_num, exact4, qt, s_q, reinterpret_cast<int32_t*>(s.ukey),
                  reinterpret_cast<float*>(s.ukey + 256));
   auto fill = [&](uint32_t c0, uint32_t clen) {
@@ -141,7 +149,7 @@ __device__ void radix_slot(const ScanArgs& a, size_t slot, bool replay) {
       const uint32_t row = c0 + j;
       float dist;
       if constexpr (NBITS == 4) {
-        if (a.flt.allow != nullptr || row < flat_num || row >= n_p - rem16) {
+        if (flt.allow != nullptr || row < flat_num || row >= n_p - rem16) {
           dist = exact4(row);
         } else {
           const uint8_t* rp = pc + (size_t)row * cw;
@@ -161,24 +169,24 @@ __device__ void radix_slot(const ScanArgs& a, size_t slot, bool replay) {
       s.ukey[j] = (uint32_t)total_order_key(dist) ^ 0x80000000u;
     }
   };
-  const uint32_t cnt = slot_topk(s, n_p, k, a.flt, off, replay, fill);
-  write_slot(s, cnt, slot, k, off, a.row_ids, a.cand_d, a.cand_id, a.cand_cnt);
+  const uint32_t cnt = slot_topk(s, n_p, k, flt, off, replay, fill);
+  write_slot(s, cnt, slot, a.k, off, a.row_ids, a.cand_d, a.cand_id, a.cand_cnt);
 }
 
 // grid (np, nq): one CTA per slot; or, with a replay list (slots the fast kernel could not settle because of
 // ties at the k-th distance), a small persistent grid that replays the listed slots
-template <int METRIC, int NBITS>
+template <int METRIC, int NBITS, bool BATCH = false>
 __global__ void __launch_bounds__(256)
 ivfpq_scan_radix_kernel(const ScanArgs a, const uint32_t* __restrict__ rlist, const uint32_t* __restrict__ rcount) {
   if (rlist) {
     const uint32_t cnt = *rcount;
     for (uint32_t i = blockIdx.x; i < cnt; i += gridDim.x) {
-      radix_slot<METRIC, NBITS>(a, rlist[i], true);
+      radix_slot<METRIC, NBITS, BATCH>(a, rlist[i], true);
       __syncthreads();
     }
     return;
   }
-  radix_slot<METRIC, NBITS>(a, (size_t)blockIdx.y * a.np + blockIdx.x, false);
+  radix_slot<METRIC, NBITS, BATCH>(a, (size_t)(a.qlist ? a.qlist[blockIdx.y] : blockIdx.y) * a.np + blockIdx.x, false);
 }
 
 // ---- warp-wide sorting network on packed (key, position) words -------------------------------------
@@ -196,10 +204,10 @@ __device__ __forceinline__ uint32_t cand_pos(uint64_t c) { return (uint32_t)c; }
 // k-th and the (k+1)-th share a key, more rows tie at the k-th distance than fit: which of them the reference's
 // BinaryHeap keeps depends on its sift order, so the slot goes on the replay list (ivfpq_scan_radix_kernel in list
 // mode restates that loop); so does a slot the kernel could not settle (replay).  Otherwise the first min(nw, k).
-__device__ __forceinline__ void fast_slot_epilogue(const ScanArgs& a, uint32_t slot, uint64_t off, const uint64_t* win,
-                                                   uint32_t nw, bool replay, int t, int nt, uint32_t* rlist,
-                                                   uint32_t* rcount) {
-  const int k = a.k;
+// k: the slot's query's k' (the lists' stride is a.k)
+__device__ __forceinline__ void fast_slot_epilogue(const ScanArgs& a, int k, uint32_t slot, uint64_t off,
+                                                   const uint64_t* win, uint32_t nw, bool replay, int t, int nt,
+                                                   uint32_t* rlist, uint32_t* rcount) {
   if (!replay && nw == (uint32_t)k + 1) {
     replay = cand_key(win[k]) == cand_key(win[k - 1]);
     nw = k;
@@ -212,8 +220,8 @@ __device__ __forceinline__ void fast_slot_epilogue(const ScanArgs& a, uint32_t s
     return;
   }
   for (uint32_t i = t; i < nw; i += nt) {
-    a.cand_d[(size_t)slot * k + i] = key_to_float(cand_key(win[i]));
-    a.cand_id[(size_t)slot * k + i] = a.row_ids[off + cand_pos(win[i])];
+    a.cand_d[(size_t)slot * a.k + i] = key_to_float(cand_key(win[i]));
+    a.cand_id[(size_t)slot * a.k + i] = a.row_ids[off + cand_pos(win[i])];
   }
   if (t == 0) a.cand_cnt[slot] = nw;
 }
@@ -265,9 +273,7 @@ __global__ void __launch_bounds__(256, 6)
 ivfpq_scan_kernel(const ScanArgs a, uint32_t* __restrict__ rlist, uint32_t* __restrict__ rcount) {
   constexpr int RPT = SCAN_CHUNK / 256;  // rows per thread and chunk (16)
   extern __shared__ float smem[];
-  const int M = a.M, k = a.k, np = a.np;
-  const int kk = k + 1;  // <= SCAN_KFAST: one more than asked for, to expose ties that overflow the k-th place
-  const uint64_t* __restrict__ allow = a.flt.allow;
+  const int M = a.M, np = a.np;
   float* lut = smem;          // [M*256]
   float* qr = lut + M * 256;  // [d]
   __shared__ uint64_t wl[8][SCAN_WLIST];                 // per-warp compacted candidates
@@ -278,7 +284,11 @@ ivfpq_scan_kernel(const ScanArgs a, uint32_t* __restrict__ rlist, uint32_t* __re
   size_t qi, slot;
   uint32_t p, n_p;
   uint64_t off;
-  if (!slot_partition(a.probe_ids, np, a.part_offsets, a.cand_cnt, qi, slot, p, off, n_p)) return;
+  if (!slot_partition(a.probe_ids, np, a.part_offsets, a.cand_cnt, qi, slot, p, off, n_p, a.qlist)) return;
+  const int k = query_k(a.qp, qi, a.k);  // a.k: the lists' stride
+  const int kk = k + 1;  // <= SCAN_KFAST: one more than asked for, to expose ties that overflow the k-th place
+  const ScanFilter flt = query_filter(a.qp, qi, a.flt);
+  const uint64_t* __restrict__ allow = flt.allow;
   if (tid == 0) s_nw = 0;
   stage_query_lut<METRIC, 8>(lut, qr, a, qi, p);
 
@@ -299,7 +309,7 @@ ivfpq_scan_kernel(const ScanArgs a, uint32_t* __restrict__ rlist, uint32_t* __re
         float dist = pq8_row_distance(lut, pc + (size_t)(c0 + j) * M, M);
         if (METRIC == METRIC_DOT) dist = __fsub_rn(dist, dot_fix);  // pq/storage.rs:957-958
         const int32_t kv = total_order_key(dist);
-        if (!FILTER || key_in_range(a.flt, kv)) {
+        if (!FILTER || key_in_range(flt, kv)) {
           if (FILTER) livemask |= 1u << u;
           key[u] = kv;
           const uint64_t c = pack_cand(kv, c0 + j);
@@ -351,7 +361,7 @@ ivfpq_scan_kernel(const ScanArgs a, uint32_t* __restrict__ rlist, uint32_t* __re
     }
     __syncthreads();
   }
-  fast_slot_epilogue(a, (uint32_t)slot, off, car, s_nw, false, tid, 256, rlist, rcount);
+  fast_slot_epilogue(a, k, (uint32_t)slot, off, car, s_nw, false, tid, 256, rlist, rcount);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -487,9 +497,7 @@ __global__ void __launch_bounds__(512, 1)
 ivfpq_scan_skew_kernel(const ScanArgs a, const uint64_t* __restrict__ slab_off, const uint8_t* __restrict__ skew,
                        uint32_t nslots, uint32_t* __restrict__ rlist, uint32_t* __restrict__ rcount) {
   extern __shared__ __align__(16) unsigned char sk_smem[];
-  const int d = a.d, k = a.k, np = a.np;
-  const int kk = k + 1;  // one more than asked for, to expose ties that overflow the k-th place
-  const uint64_t* __restrict__ allow = a.flt.allow;
+  const int d = a.d, np = a.np;
   // NTEAM = 2: teams of 8 warps, two LUT copies (no bank conflicts).  NTEAM = 4: teams of 4 warps, ONE copy each
   // (lanes l and l + 16 share a bank: two wavefronts per request) -- twice as many independent teams to fill the
   // issue slots a team leaves empty at its barriers and in its low-parallelism phases.
@@ -504,8 +512,9 @@ ivfpq_scan_skew_kernel(const ScanArgs a, const uint64_t* __restrict__ slab_off, 
   const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(sk_smem);
   if (sbase > SKEW_MAX_BASE) {  // never seen (the runtime reserves 1 KB: sbase = 0x400); the exact replay takes every slot
     for (uint32_t slot = blockIdx.x * 512 + tid; slot < nslots; slot += gridDim.x * 512) {
-      rlist[atomicAdd(rcount, 1u)] = slot;
-      a.cand_cnt[slot] = 0;
+      const uint32_t rs = a.qlist ? a.qlist[slot / np] * np + slot % np : slot;
+      rlist[atomicAdd(rcount, 1u)] = rs;
+      a.cand_cnt[rs] = 0;
     }
     return;
   }
@@ -550,19 +559,26 @@ ivfpq_scan_skew_kernel(const ScanArgs a, const uint64_t* __restrict__ slab_off, 
   // slot metadata is a chain of dependent global loads (probe id -> partition offsets -> slab offset): it is
   // fetched one slot ahead, and the first code unit of a slot is requested before its LUT is built
   const uint32_t stride = gridDim.x * NTEAM;
+  // slot v of the launch is slot real(v) of the slab (a group's queries: qlist)
+  auto real = [&](uint32_t v) -> uint32_t { return a.qlist ? a.qlist[v / np] * np + v % np : v; };
   uint32_t slot = blockIdx.x * NTEAM + team;
-  uint32_t p_n = slot < nslots ? a.probe_ids[slot] : 0u;
+  uint32_t p_n = slot < nslots ? a.probe_ids[real(slot)] : 0u;
   uint64_t off_n = a.part_offsets[p_n], end_n = a.part_offsets[p_n + 1], so_n = slab_off[p_n];
   for (; slot < nslots; slot += stride) {
-    const size_t qi = slot / np;
+    const uint32_t rs = real(slot);
+    const size_t qi = rs / np;
+    const int k = query_k(a.qp, qi, a.k);  // a.k: the lists' stride
+    const int kk = k + 1;  // one more than asked for, to expose ties that overflow the k-th place
+    const ScanFilter flt = query_filter(a.qp, qi, a.flt);
+    const uint64_t* __restrict__ allow = flt.allow;
     const uint32_t p = p_n;
     const uint64_t off = off_n;
     const uint32_t n_p = (uint32_t)(end_n - off_n);
     const uint8_t* sp = skew + so_n * SKEW_SLAB_BYTES;
-    p_n = slot + stride < nslots ? a.probe_ids[slot + stride] : 0u;
+    p_n = slot + stride < nslots ? a.probe_ids[real(slot + stride)] : 0u;
     if (n_p == 0) {
       off_n = a.part_offsets[p_n]; end_n = a.part_offsets[p_n + 1]; so_n = slab_off[p_n];
-      if (ttid == 0) a.cand_cnt[slot] = 0;
+      if (ttid == 0) a.cand_cnt[rs] = 0;
       continue;
     }
     const uint4* up0 = reinterpret_cast<const uint4*>(sp + (size_t)warp * SKEW_SLAB_BYTES) + lane;
@@ -644,7 +660,7 @@ ivfpq_scan_skew_kernel(const ScanArgs a, const uint64_t* __restrict__ slab_off, 
           if (FILTER) {
             const int ri = r - sh;
             const uint32_t j = wbase + lane + 32 * ri;
-            live = ri >= 0 && ri < 16 && j < clen && row_allowed(allow, off + c0 + j) && key_in_range(a.flt, kv);
+            live = ri >= 0 && ri < 16 && j < clen && row_allowed(allow, off + c0 + j) && key_in_range(flt, kv);
           } else {
             live = ((livemask >> r) & 1u) != 0;
           }
@@ -710,7 +726,7 @@ ivfpq_scan_skew_kernel(const ScanArgs a, const uint64_t* __restrict__ slab_off, 
       }
       team_sync<TT>(team);
     }
-    fast_slot_epilogue(a, slot, off, car + par * SCAN_KFAST, nw, replay, ttid, TT, rlist, rcount);
+    fast_slot_epilogue(a, k, rs, off, car + par * SCAN_KFAST, nw, replay, ttid, TT, rlist, rcount);
   }
 }
 
@@ -749,13 +765,24 @@ static int scan_mode_env() {
   return !e ? 0 : (!strcmp(e, "classic") ? 1 : (!strcmp(e, "skew") ? 2 : 0));
 }
 
+// the radix kernel, with per-query values when the search has them
+template <int METRIC, int NBITS>
+static void radix_launch(const char* name, dim3 grid, size_t smem, const ScanArgs& a, const uint32_t* rlist,
+                         const uint32_t* rcount) {
+  auto go = [&](auto kern) {
+    set_smem(kern, smem);
+    LB2_LAUNCH(name, kern, grid, 256, smem, a, rlist, rcount);
+  };
+  if (a.qp) go(ivfpq_scan_radix_kernel<METRIC, NBITS, true>);
+  else go(ivfpq_scan_radix_kernel<METRIC, NBITS, false>);
+}
+
+// one launch of the fast 8-bit scan (k' + 1 <= SCAN_KFAST) over grid (probes, queries); ties go to rlist
 template <int METRIC>
-static void scan_launch(int nbits, dim3 grid, size_t smem, const ScanArgs& a, uint32_t* rlist, uint32_t* rcount,
+static void fast_launch(dim3 grid, const ScanArgs& a, bool filtering, uint32_t* rlist, uint32_t* rcount,
                         const uint64_t* slab_off, const uint8_t* skew) {
-  const bool filtering = a.flt.allow != nullptr || a.flt.range;
-  if (nbits == 8 && a.k + 1 <= SCAN_KFAST) {
+  {
     const size_t smem_fast = sizeof(float) * ((size_t)a.M * 256 + a.d);
-    LB2_CUDA(cudaMemsetAsync(rcount, 0, sizeof(uint32_t), ctx().stream));
     const uint64_t nslots = (uint64_t)grid.x * grid.y;
     const bool skew_ok = skew && a.M == 16 && a.ds == 8 && (reinterpret_cast<uintptr_t>(a.queries) & 15) == 0 &&
                          (size_t)SKEW_SMEM_BYTES <= ctx().smem_optin;
@@ -783,22 +810,53 @@ static void scan_launch(int nbits, dim3 grid, size_t smem, const ScanArgs& a, ui
       set_smem(ivfpq_scan_kernel<METRIC, false>, smem_fast);
       LB2_LAUNCH("pq_scan", (ivfpq_scan_kernel<METRIC, false>), grid, 256, smem_fast, a, rlist, rcount);
     }
-    // slots with ties beyond the k-th place (rare): the reference's heap loop, restated
-    set_smem((ivfpq_scan_radix_kernel<METRIC, 8>), smem);
-    const unsigned rgrid = (unsigned)std::min<uint64_t>((uint64_t)grid.x * grid.y, 4 * (uint64_t)ctx().num_sms);
-    LB2_LAUNCH("pq_scan_tie_replay", (ivfpq_scan_radix_kernel<METRIC, 8>), rgrid, 256, smem, a,
-               (const uint32_t*)rlist, (const uint32_t*)rcount);
+  }
+}
+
+// slots with ties beyond the k-th place (rare): the reference's heap loop, restated, over the listed slots
+template <int METRIC>
+static void tie_replay(uint64_t nslots, size_t smem, ScanArgs a, const uint32_t* rlist, const uint32_t* rcount) {
+  a.qlist = nullptr;  // the list holds slots of the slab
+  const unsigned rgrid = (unsigned)std::min<uint64_t>(nslots, 4 * (uint64_t)ctx().num_sms);
+  radix_launch<METRIC, 8>("pq_scan_tie_replay", rgrid, smem, a, rlist, rcount);
+}
+
+template <int METRIC>
+static void scan_launch(int nbits, dim3 grid, size_t smem, const ScanArgs& a, bool filtering, uint32_t* rlist,
+                        uint32_t* rcount, const uint64_t* slab_off, const uint8_t* skew) {
+  if (nbits == 8 && a.k + 1 <= SCAN_KFAST) {
+    LB2_CUDA(cudaMemsetAsync(rcount, 0, sizeof(uint32_t), ctx().stream));
+    fast_launch<METRIC>(grid, a, filtering, rlist, rcount, slab_off, skew);
+    tie_replay<METRIC>((uint64_t)grid.x * grid.y, smem, a, rlist, rcount);
     return;
   }
-  if (nbits == 4) {
-    set_smem((ivfpq_scan_radix_kernel<METRIC, 4>), smem);
-    LB2_LAUNCH("pq_scan", (ivfpq_scan_radix_kernel<METRIC, 4>), grid, 256, smem, a, (const uint32_t*)nullptr,
-               (const uint32_t*)nullptr);
-    return;
+  if (nbits == 4)
+    radix_launch<METRIC, 4>("pq_scan", grid, smem, a, nullptr, nullptr);
+  else
+    radix_launch<METRIC, 8>("pq_scan", grid, smem, a, nullptr, nullptr);
+}
+
+// A batch's slab (queries with their own k' and filter): its queries in route groups -- the fast kernel without and
+// with the filter test (k' + 1 <= SCAN_KFAST, 8-bit), the radix kernel for the others -- and one launch per group
+// present, each over its own queries (qlist), then one tie replay for both fast groups.  groups[r] lists route r's
+// slab-relative queries on the host, glist holds them on the device in that order.
+template <int METRIC>
+static void scan_launch_groups(int np, size_t smem, ScanArgs a, const std::vector<uint32_t>* groups,
+                               const uint32_t* glist, uint32_t* rlist, uint32_t* rcount, const uint64_t* slab_off,
+                               const uint8_t* skew) {
+  const size_t nfast = groups[0].size() + groups[1].size();
+  if (nfast) LB2_CUDA(cudaMemsetAsync(rcount, 0, sizeof(uint32_t), ctx().stream));
+  size_t at = 0;
+  for (int r = 0; r < 3; ++r) {
+    const size_t n = groups[r].size();
+    if (!n) continue;
+    a.qlist = glist + at;
+    at += n;
+    const dim3 g((unsigned)np, (unsigned)n);
+    if (r < 2) fast_launch<METRIC>(g, a, r == 1, rlist, rcount, slab_off, skew);
+    else radix_launch<METRIC, 8>("pq_scan", g, smem, a, nullptr, nullptr);
   }
-  set_smem((ivfpq_scan_radix_kernel<METRIC, 8>), smem);
-  LB2_LAUNCH("pq_scan", (ivfpq_scan_radix_kernel<METRIC, 8>), grid, 256, smem, a, (const uint32_t*)nullptr,
-             (const uint32_t*)nullptr);
+  if (nfast) tie_replay<METRIC>((uint64_t)nfast * np, smem, a, rlist, rcount);
 }
 
 // the skewed copy of an index's codes (see ivfpq_scan_skew_kernel); sizes: slab_off u64[K + 1],
@@ -821,15 +879,18 @@ void ivfpq_search(const IvfSearch& s, const float* codebook, int M, int nbits, c
   const int np = s.nprobes < s.K ? s.nprobes : s.K;
   const size_t smem = sizeof(float) * ((size_t)M * (nbits == 4 ? 16 : 256) + d) + slot_smem_bytes(k);
   // every kernel the scan may launch must fit: the radix kernel (the scan itself, or the tie replay of the fast
-  // 8-bit kernels) and, for k + 1 <= SCAN_KFAST, the classic fast kernel with its LUT and larger static lists
+  // 8-bit kernels) and, for k + 1 <= SCAN_KFAST (a batch: any query's k'), the classic fast kernel with its LUT and
+  // larger static lists
+  bool any_fast = k + 1 <= SCAN_KFAST;
+  for (uint64_t q = 0; s.qp_host && q < s.nq && !any_fast; ++q) any_fast = s.qp_host[q].k + 1 <= SCAN_KFAST;
   size_t need = 0;
   auto need_of = [&](auto m) {
     constexpr int METRIC = decltype(m)::value;
     need = nbits == 4 ? smem_with_static(ivfpq_scan_radix_kernel<METRIC, 4>, smem)
                       : smem_with_static(ivfpq_scan_radix_kernel<METRIC, 8>, smem);
-    if (nbits == 8 && k + 1 <= SCAN_KFAST) {
+    if (nbits == 8 && any_fast) {
       const size_t fast = sizeof(float) * ((size_t)M * 256 + d);
-      const bool filtering = s.flt.allow != nullptr || s.flt.range;
+      const bool filtering = s.filtering();
       need = std::max(need, filtering ? smem_with_static(ivfpq_scan_kernel<METRIC, true>, fast)
                                       : smem_with_static(ivfpq_scan_kernel<METRIC, false>, fast));
     }
@@ -837,16 +898,33 @@ void ivfpq_search(const IvfSearch& s, const float* codebook, int M, int nbits, c
   if (metric == METRIC_DOT) need_of(std::integral_constant<int, METRIC_DOT>{});
   else need_of(std::integral_constant<int, METRIC_L2>{});
   if (!ivf_search_begin(s, need, "LUT and top-k scratch of %zu bytes exceed shared memory", need)) return;
-  DevBuf<uint32_t> rlist((size_t)std::min<uint64_t>(s.nq, SEARCH_SLAB) * np), rcount(1);
+  DevBuf<uint32_t> rlist((size_t)std::min<uint64_t>(s.nq, SEARCH_SLAB) * np), rcount(1), glist;
   run_ivf_search(s, [&](const ScanSlots& sl) {
     if (rlist.n < sl.qn * sl.np) rlist.alloc(sl.qn * sl.np);
     const ScanArgs a{s.queries + sl.q0 * d, d, s.centroids, codebook, M, d / M, sl.probe_ids, sl.np, sl.offsets, codes,
-                     s.row_ids, k, sl.cand_d, sl.cand_id, sl.cand_cnt, s.flt};
+                     s.row_ids, k, sl.cand_d, sl.cand_id, sl.cand_cnt, s.flt, s.qp_at(sl.q0)};
+    if (s.qp_host && nbits == 8) {  // a batch: route groups (fast unfiltered, fast filtered, radix), one launch each
+      std::vector<uint32_t> groups[3];
+      for (uint32_t q = 0; q < (uint32_t)sl.qn; ++q) {
+        const QueryParam& p = s.qp_host[sl.q0 + q];
+        groups[p.k + 1 > SCAN_KFAST ? 2 : (p.flt.allow || p.flt.range ? 1 : 0)].push_back(q);
+      }
+      std::vector<uint32_t> all(groups[0]);
+      all.insert(all.end(), groups[1].begin(), groups[1].end());
+      all.insert(all.end(), groups[2].begin(), groups[2].end());
+      if (glist.n < all.size()) glist.alloc(all.size());
+      h2d(glist.p, all.data(), all.size());
+      if (metric == METRIC_DOT)
+        scan_launch_groups<METRIC_DOT>(sl.np, smem, a, groups, glist.p, rlist.p, rcount.p, slab_off, skew);
+      else
+        scan_launch_groups<METRIC_L2>(sl.np, smem, a, groups, glist.p, rlist.p, rcount.p, slab_off, skew);
+      return;
+    }
     const dim3 g(sl.np, (unsigned)sl.qn);
     if (metric == METRIC_DOT)
-      scan_launch<METRIC_DOT>(nbits, g, smem, a, rlist.p, rcount.p, slab_off, skew);
+      scan_launch<METRIC_DOT>(nbits, g, smem, a, s.filtering(), rlist.p, rcount.p, slab_off, skew);
     else
-      scan_launch<METRIC_L2>(nbits, g, smem, a, rlist.p, rcount.p, slab_off, skew);
+      scan_launch<METRIC_L2>(nbits, g, smem, a, s.filtering(), rlist.p, rcount.p, slab_off, skew);
   });
 }
 

@@ -106,12 +106,17 @@ void rank_probes(const float* dists, uint64_t nq, int K, int L, uint32_t* ids, f
   }
 }
 
-// one warp per partition: the allow bitmap's popcount over the partition's storage range
+// one warp per partition: the allow bitmap's popcount over the partition's storage range; with a table of bitmaps
+// (allows) grid row y counts bitmap y into c[y * K ..]
 __global__ void __launch_bounds__(256)
-partition_counts_kernel(const uint64_t* __restrict__ off, int K, const uint64_t* __restrict__ allow, uint32_t kc,
-                        uint32_t* __restrict__ c) {
+partition_counts_kernel(const uint64_t* __restrict__ off, int K, const uint64_t* __restrict__ allow,
+                        const uint64_t* const* __restrict__ allows, uint32_t kc, uint32_t* __restrict__ c) {
   const int p = (int)((blockIdx.x * 256 + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (p >= K) return;
+  if (allows) {
+    allow = allows[blockIdx.y];
+    c += (size_t)blockIdx.y * K;
+  }
   const uint64_t a = off[p], b = off[p + 1];
   uint64_t cnt = 0;
   if (!allow) {
@@ -131,7 +136,13 @@ partition_counts_kernel(const uint64_t* __restrict__ off, int K, const uint64_t*
 void partition_counts(const uint64_t* part_offsets, int K, const uint64_t* allow, uint32_t kc, uint32_t* c) {
   if (K == 0) return;
   LB2_LAUNCH("partition_counts", partition_counts_kernel, cdiv((uint64_t)K * 32, 256), 256, 0, part_offsets, K, allow,
-             kc, c);
+             (const uint64_t* const*)nullptr, kc, c);
+}
+
+void partition_counts_table(const uint64_t* part_offsets, int K, const uint64_t* const* allows, int nf, uint32_t* c) {
+  if (K == 0 || nf == 0) return;
+  LB2_LAUNCH("partition_counts", partition_counts_kernel, dim3(cdiv((uint64_t)K * 32, 256), (unsigned)nf), 256, 0,
+             part_offsets, K, (const uint64_t*)nullptr, allows, 0xffffffffu, c);
 }
 
 // early_pruning (knn.rs:1117-1130): Rust's slice::partition_point(|d| d <= d0 * f), i.e. binary_search_by as
@@ -158,14 +169,30 @@ struct CutoffArgs {
 
 // one thread per query
 __global__ void __launch_bounds__(128)
-probe_cutoff_kernel(const CutoffArgs a, uint64_t nq, int L, const uint32_t* __restrict__ pids,
+probe_cutoff_kernel(const CutoffArgs a0, uint64_t nq, int L, const uint32_t* __restrict__ pids,
                     const float* __restrict__ pd, const uint32_t* __restrict__ cpart, uint32_t* __restrict__ cslot,
                     int slot_stride, uint32_t* __restrict__ nsearch, uint32_t* __restrict__ shortcut,
-                    uint32_t* __restrict__ nmax, uint32_t* __restrict__ nprobes_out) {
+                    uint32_t* __restrict__ nmax, uint32_t* __restrict__ nprobes_out,
+                    const QueryProbe* __restrict__ qpr) {
   const uint64_t q = (uint64_t)blockIdx.x * 128 + threadIdx.x;
   if (q >= nq) return;
-  auto c = [&](uint32_t t) -> uint64_t { return cpart ? cpart[pids[q * L + t]] : cslot[q * slot_stride + t]; };
-  const uint32_t Lu = (uint32_t)L, k = a.k;
+  CutoffArgs a = a0;
+  uint32_t Lu = (uint32_t)L, kc = 0xffffffffu;
+  if (qpr) {  // a batch: the query's own rule, and its own filter's counts capped by its own k'
+    const QueryProbe& r = qpr[q];
+    a.min_np = r.min_np;
+    a.k = r.k;
+    a.has_max_len = r.has_max_len;
+    a.iterable = r.mask_ids != nullptr;
+    a.max_len = r.max_len;
+    Lu = r.L;
+    kc = r.kc;
+    if (!cslot || !r.ranged) cpart = r.cpart;
+  }
+  auto c = [&](uint32_t t) -> uint64_t {
+    return cpart ? min(kc, cpart[pids[q * L + t]]) : cslot[q * slot_stride + t];
+  };
+  const uint32_t k = a.k;
   // adjust_probes (knn.rs:1108-1115) then initial_search's min(partitions.len())
   const uint32_t min_np = min(max(a.min_np, early_pruning(pd + q * L, Lu, k)), Lu);
   uint64_t sum0 = 0;
@@ -191,42 +218,44 @@ probe_cutoff_kernel(const CutoffArgs a, uint64_t nq, int L, const uint32_t* __re
   shortcut[q] = sc;
   atomicMax(nmax, n);
   if (nprobes_out) nprobes_out[q] = n;
-  if (!cpart)
+  if (cslot)  // the lists past the cutoff were scanned ahead of it: emptied
     for (uint32_t t = n; t < Lu; ++t) cslot[q * slot_stride + t] = 0;
 }
 
 void probe_cutoff(const ProbeRule& r, uint64_t nq, int L, const uint32_t* pids, const float* pd, const uint32_t* cpart,
                   uint32_t* cslot, int slot_stride, uint32_t* nsearch, uint32_t* shortcut, uint32_t* nmax,
-                  uint32_t* nprobes_out) {
+                  uint32_t* nprobes_out, const QueryProbe* qpr) {
   if (nq == 0) return;
   const CutoffArgs a{r.min_np, r.late_width, r.k, r.has_max_len, r.mask_ids != nullptr, r.max_len};
   LB2_LAUNCH("probe_cutoff", probe_cutoff_kernel, cdiv(nq, 128), 128, 0, a, nq, L, pids, pd, cpart, cslot, slot_stride,
-             nsearch, shortcut, nmax, nprobes_out);
+             nsearch, shortcut, nmax, nprobes_out, qpr);
 }
 
 __global__ void gather_probes_kernel(uint64_t nq, int L, const uint32_t* __restrict__ pids, const float* __restrict__ pd,
                                      const uint32_t* __restrict__ nsearch, int nl, uint32_t sentinel,
-                                     uint32_t* __restrict__ out_ids, float* __restrict__ out_pd) {
+                                     uint32_t* __restrict__ out_ids, float* __restrict__ out_pd,
+                                     const QueryProbe* __restrict__ qpr) {
   const uint64_t g = (uint64_t)blockIdx.x * 256 + threadIdx.x;
   if (g >= nq * nl) return;
   const uint64_t q = g / nl;
-  const uint32_t t = (uint32_t)(g % nl), n = nsearch ? nsearch[q] : (uint32_t)L;
+  const uint32_t t = (uint32_t)(g % nl), n = nsearch ? nsearch[q] : (qpr ? qpr[q].L : (uint32_t)L);
   const bool live = t < n && t < (uint32_t)L;
   out_ids[g] = live ? pids[q * L + t] : sentinel;
   out_pd[g] = live ? pd[q * L + t] : 0.0f;
 }
 
 void gather_probes(uint64_t nq, int L, const uint32_t* pids, const float* pd, const uint32_t* nsearch, int nl,
-                   uint32_t sentinel, uint32_t* out_ids, float* out_pd) {
+                   uint32_t sentinel, uint32_t* out_ids, float* out_pd, const QueryProbe* qpr) {
   if (nq == 0 || nl == 0) return;
   LB2_LAUNCH("gather_probes", gather_probes_kernel, cdiv(nq * nl, 256), 256, 0, nq, L, pids, pd, nsearch, nl, sentinel,
-             out_ids, out_pd);
+             out_ids, out_pd, qpr);
 }
 
 // one block per query.  The query's lists hold found0 < max_len <= k <= 1024 rows when it takes the shortcut.
 __global__ void __launch_bounds__(128)
 shortcut_kernel(const uint32_t* __restrict__ shortcut, const uint64_t* __restrict__ mask_ids, uint64_t nmask, int nl,
-                int kc, float* __restrict__ cand_d, uint64_t* __restrict__ cand_id, uint32_t* __restrict__ cand_cnt) {
+                int kc, float* __restrict__ cand_d, uint64_t* __restrict__ cand_id, uint32_t* __restrict__ cand_cnt,
+                const QueryProbe* __restrict__ qpr) {
   __shared__ uint64_t found[1024];
   __shared__ uint32_t s_nf, s_out, s_wsum[4];
   const uint64_t q = blockIdx.x;
@@ -236,13 +265,19 @@ shortcut_kernel(const uint32_t* __restrict__ shortcut, const uint64_t* __restric
     if (tid == 0) cand_cnt[list] = 0;
     return;
   }
+  const int stride = kc;  // a batch: the query's own ids and k'; the lists' stride stays kc
+  if (qpr) {
+    mask_ids = qpr[q].mask_ids;
+    nmask = qpr[q].num_mask_ids;
+    kc = (int)qpr[q].kc;
+  }
   if (tid == 0) { s_nf = 0; s_out = 0; }
   __syncthreads();
   for (int t = 0; t < nl - 1; ++t) {
     const uint32_t cnt = cand_cnt[q * nl + t];
     for (uint32_t e = tid; e < cnt; e += 128) {
       const uint32_t at = atomicAdd(&s_nf, 1u);
-      if (at < 1024) found[at] = cand_id[(q * nl + t) * kc + e];
+      if (at < 1024) found[at] = cand_id[(q * nl + t) * stride + e];
     }
   }
   __syncthreads();
@@ -264,8 +299,8 @@ shortcut_kernel(const uint32_t* __restrict__ shortcut, const uint64_t* __restric
     uint32_t pos = out0 + __popc(bal & ((1u << lane) - 1));
     for (int w = 0; w < warp; ++w) pos += s_wsum[w];
     if (keep && pos < (uint32_t)kc) {
-      cand_id[list * kc + pos] = id;
-      cand_d[list * kc + pos] = __int_as_float(0x7f800000);
+      cand_id[list * stride + pos] = id;
+      cand_d[list * stride + pos] = __int_as_float(0x7f800000);
     }
     __syncthreads();
     if (tid == 0) s_out = min((uint32_t)kc, out0 + s_wsum[0] + s_wsum[1] + s_wsum[2] + s_wsum[3]);
@@ -275,10 +310,10 @@ shortcut_kernel(const uint32_t* __restrict__ shortcut, const uint64_t* __restric
 }
 
 void shortcut_lists(uint64_t nq, const uint32_t* shortcut, const uint64_t* mask_ids, uint64_t num_mask_ids, int nl,
-                    int kc, float* cand_d, uint64_t* cand_id, uint32_t* cand_cnt) {
+                    int kc, float* cand_d, uint64_t* cand_id, uint32_t* cand_cnt, const QueryProbe* qpr) {
   if (nq == 0) return;
   LB2_LAUNCH("probe_shortcut", shortcut_kernel, (unsigned)nq, 128, 0, shortcut, mask_ids, num_mask_ids, nl, kc, cand_d,
-             cand_id, cand_cnt);
+             cand_id, cand_cnt, qpr);
 }
 
 }  // namespace lb2

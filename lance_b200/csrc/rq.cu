@@ -309,12 +309,11 @@ ivfrq_scan_kernel(const float* __restrict__ rq, int code_dim, float sqrt_d, int 
                   const uint64_t* __restrict__ part_offsets, const uint8_t* __restrict__ codes,
                   const float* __restrict__ add, const float* __restrict__ scale, const uint64_t* __restrict__ row_ids,
                   int k, float* __restrict__ cand_d, uint64_t* __restrict__ cand_id, uint32_t* __restrict__ cand_cnt,
-                  const ScanFilter flt) {
+                  const ScanFilter flt0, const QueryParam* __restrict__ qp) {
   extern __shared__ float rq_smem[];
   const int nt = code_dim >> 2;  // sub-tables of 16 entries
   float* tab = rq_smem;                                      // [nt * 16] f32
   uint8_t* qt = reinterpret_cast<uint8_t*>(tab + nt * 16);  // [nt * 16] u8 (code_dim % 8 == 0: 4-byte aligned end)
-  const SlotSmem s(qt + nt * 16, k + 1);
   __shared__ int32_t s_mn, s_mx;
   __shared__ float s_sum_q;
   const int tid = threadIdx.x;
@@ -322,6 +321,9 @@ ivfrq_scan_kernel(const float* __restrict__ rq, int code_dim, float sqrt_d, int 
   uint32_t p, n_p;
   uint64_t off;
   if (!slot_partition(probe_ids, np, part_offsets, cand_cnt, qi, slot, p, off, n_p)) return;
+  const int kq = query_k(qp, qi, k);  // k: the lists' stride
+  const ScanFilter flt = query_filter(qp, qi, flt0);
+  const SlotSmem s(qt + nt * 16, kq + 1);
   const float* r = rq + slot * (size_t)code_dim;
   if (tid == 0) { s_mn = 0x7fffffff; s_mx = (int32_t)0x80000000; }
   for (int st = tid; st < nt; st += 256) {
@@ -397,7 +399,7 @@ ivfrq_scan_kernel(const float* __restrict__ rq, int code_dim, float sqrt_d, int 
       s.ukey[j] = (uint32_t)total_order_key(out) ^ 0x80000000u;
     }
   };
-  const uint32_t cnt = slot_topk(s, n_p, k, flt, off, false, fill);
+  const uint32_t cnt = slot_topk(s, n_p, kq, flt, off, false, fill);
   write_slot(s, cnt, slot, k, off, row_ids, cand_d, cand_id, cand_cnt);
 }
 
@@ -441,7 +443,7 @@ void ivfrq_search(const IvfSearch& s, const float* rotation, int code_dim, const
       rq_rotate_f32(rotation, code_dim, d, res.p, b * np, rot.p);
       LB2_LAUNCH("rq_scan", ivfrq_scan_kernel, dim3(np, (unsigned)b), 256, smem, rot.p, code_dim, sqrt_d, q_minus_one,
                  sl.probe_ids + a * np, sl.probe_dists + a * np, np, sl.offsets, codes, add, scale, s.row_ids, k,
-                 sl.cand_d + a * np * k, sl.cand_id + a * np * k, sl.cand_cnt + a * np, s.flt);
+                 sl.cand_d + a * np * k, sl.cand_id + a * np * k, sl.cand_cnt + a * np, s.flt, s.qp_at(sl.q0 + a));
     }
   });
 }

@@ -28,6 +28,16 @@ void refine_f32(const float* queries, uint64_t nq, int d, int metric, const void
                 uint64_t num_vectors, const uint64_t* cand_id, const uint32_t* cand_cnt, int kc, int k,
                 uint64_t* out_id, float* out_d, uint32_t* out_cnt, int has_lower = 0, float lower = 0.0f,
                 int has_upper = 0, float upper = 0.0f);
+// the finish of a batch with per-query values (lb2_index_search_batch), one block per query: query q's merged
+// candidates (cand_* [nq][kc], its own k' = qo[q].kc of them at most) -> its k = qo[q].k results in rows of k_stride,
+// re-ranked by exact distance within its range when qo[q].refine (refine_f32), else its first k as they are
+struct QueryOut {
+  int kc, k, refine, has_lower, has_upper;
+  float lower, upper;
+};
+void refine_batch_f32(const float* queries, uint64_t nq, int d, int metric, const void* vectors, int vdt,
+                      uint64_t num_vectors, const float* cand_d, const uint64_t* cand_id, const uint32_t* cand_cnt,
+                      int kc, const QueryOut* qo, int k_stride, uint64_t* out_id, float* out_d, uint32_t* out_cnt);
 void flat_topk_f32(const float* dists, const uint64_t* row_ids, uint64_t n, int k, const ScanFilter& flt,
                    uint64_t* out_id, float* out_d, uint32_t* out_cnt);
 // lb2_distance_batch with the reference's per-type rule: u8 L2 / dot (exact integer sums) and f16 / bf16 dot

@@ -95,17 +95,19 @@ __global__ void __maxnreg__(128)  // 256 threads; under __launch_bounds__(256) p
 ivfsq_scan_kernel(const uint8_t* __restrict__ qcodes, int d, float r2, const uint32_t* __restrict__ probe_ids, int np,
                   const uint64_t* __restrict__ part_offsets, const uint8_t* __restrict__ codes,
                   const uint64_t* __restrict__ row_ids, int k, float* __restrict__ cand_d, uint64_t* __restrict__ cand_id,
-                  uint32_t* __restrict__ cand_cnt, const ScanFilter flt) {
+                  uint32_t* __restrict__ cand_cnt, const ScanFilter flt0, const QueryParam* __restrict__ qp) {
   extern __shared__ uint4 sq_smem[];
   const int nw = d >> 2;                                   // 4-byte words per row
   uint32_t* qw = reinterpret_cast<uint32_t*>(sq_smem);     // the query's codes, [nw] words (16-byte aligned)
-  const SlotSmem s(qw + ((nw + 3) & ~3), k + 1);
   const int tid = threadIdx.x, l = tid & 7;
   const unsigned gmask = 0xffu << (8 * ((tid >> 3) & 3));  // the row's 8 lanes
   size_t qi, slot;
   uint32_t p, n_p;
   uint64_t off;
   if (!slot_partition(probe_ids, np, part_offsets, cand_cnt, qi, slot, p, off, n_p)) return;
+  const int kq = query_k(qp, qi, k);  // k: the lists' stride
+  const ScanFilter flt = query_filter(qp, qi, flt0);
+  const SlotSmem s(qw + ((nw + 3) & ~3), kq + 1);
   const uint32_t* qsrc = reinterpret_cast<const uint32_t*>(qcodes + qi * (size_t)d);  // d % 4 == 0: word aligned
   for (int t = tid; t < nw; t += 256) qw[t] = qsrc[t];
   __syncthreads();
@@ -134,7 +136,7 @@ ivfsq_scan_kernel(const uint8_t* __restrict__ qcodes, int d, float r2, const uin
       }
     }
   };
-  const uint32_t cnt = slot_topk(s, n_p, k, flt, off, false, fill);
+  const uint32_t cnt = slot_topk(s, n_p, kq, flt, off, false, fill);
   write_slot(s, cnt, slot, k, off, row_ids, cand_d, cand_id, cand_cnt);
 }
 
@@ -156,7 +158,8 @@ void ivfsq_search(const IvfSearch& s, const uint8_t* codes, float r2, const uint
     with_kernel([&](auto kern) {
       set_smem(kern, smem);
       LB2_LAUNCH("sq_scan", kern, dim3(sl.np, (unsigned)sl.qn), 256, smem, qcodes + sl.q0 * d, d, r2, sl.probe_ids,
-                 sl.np, sl.offsets, codes, s.row_ids, k, sl.cand_d, sl.cand_id, sl.cand_cnt, s.flt);
+                 sl.np, sl.offsets, codes, s.row_ids, k, sl.cand_d, sl.cand_id, sl.cand_cnt, s.flt,
+                 s.qp_at(sl.q0));
     });
   });
 }

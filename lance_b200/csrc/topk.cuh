@@ -431,12 +431,14 @@ __device__ __forceinline__ void write_slot(const SlotSmem& s, uint32_t cnt, size
   if (threadIdx.x == 0) cand_cnt[slot] = cnt;
 }
 
-// the partition slot (query blockIdx.y, probe blockIdx.x) scans: false, with an empty candidate list, when it has no rows
+// the partition slot (query blockIdx.y, or qlist[blockIdx.y] for a grid over a group of queries; probe blockIdx.x)
+// scans: false, with an empty candidate list, when it has no rows
 __device__ __forceinline__ bool slot_partition(const uint32_t* __restrict__ probe_ids, int np,
                                                const uint64_t* __restrict__ part_offsets, uint32_t* __restrict__ cand_cnt,
-                                               size_t& qi, size_t& slot, uint32_t& p, uint64_t& off, uint32_t& n_p) {
+                                               size_t& qi, size_t& slot, uint32_t& p, uint64_t& off, uint32_t& n_p,
+                                               const uint32_t* __restrict__ qlist = nullptr) {
   const int pi = blockIdx.x;
-  qi = blockIdx.y;
+  qi = qlist ? qlist[blockIdx.y] : blockIdx.y;
   p = probe_ids[qi * np + pi];
   off = part_offsets[p];
   n_p = (uint32_t)(part_offsets[p + 1] - off);
@@ -446,6 +448,12 @@ __device__ __forceinline__ bool slot_partition(const uint32_t* __restrict__ prob
     return false;
   }
   return true;
+}
+
+// the k' and the filter of query qi (slab-relative): its own with per-query values (qp, of the slab), else the search's
+__device__ __forceinline__ int query_k(const QueryParam* __restrict__ qp, size_t qi, int k) { return qp ? qp[qi].k : k; }
+__device__ __forceinline__ ScanFilter query_filter(const QueryParam* __restrict__ qp, size_t qi, const ScanFilter& f) {
+  return qp ? qp[qi].flt : f;
 }
 
 }  // namespace lb2
