@@ -444,6 +444,49 @@ lb2_status lb2_index_search_batch(lb2_index* index, const void* queries, uint64_
                                   uint32_t num_filters, const void* refine_vectors, uint64_t num_vectors,
                                   uint32_t late_width, uint32_t k_stride, uint64_t* row_ids_out /* [nq][k_stride] */,
                                   float* dists_out, uint32_t* counts_out, uint32_t* nprobes_out);
+/* A refined batch over rows the caller takes, as the reference plans a refined query: the ANN node returns _rowid
+ * candidates, the scanner takes their vectors (self.take(ann_node, vector_projection)) and runs flat_knn over only
+ * those rows (rust/lance/src/dataset/scanner.rs:2884-2905).  Row ids are Lance _rowid values (fragment << 32 |
+ * offset, or stable row ids), so the raw column is never indexed by them; lb2_index_search_batch's refine_vectors
+ * is a dense column indexed by row id and cannot serve such a table.
+ *
+ * lb2_index_search_candidates: the index half.  Row q of cand_ids_out / cand_dists_out [nq][kc_stride] is exactly the
+ * list lb2_index_search_batch re-ranks for query q: k'_q = k_q * max(1, refine_factor_q) entries (k_q without
+ * refine), index distances in the merge's order, probe-rule shortcut rows at +inf included; slots from
+ * cand_counts_out[q] on hold UINT64_MAX / +inf.  nprobes_out (nullable) is lb2_index_search_batch's.  k and
+ * refine_factor stay separate, since the probe rule uses k as well as k' (early pruning, found0, the stop test):
+ * a query with k' and refine factor 0 is not the same list.  With distinct_ids_out (capacity nq * kc_stride),
+ * *num_distinct_out = m receives the number of distinct row ids over every valid slot of the batch, distinct_ids_out
+ * those ids ascending (entries m.. hold UINT64_MAX), and positions_out [nq][kc_stride] the index of each slot's id in
+ * that list (UINT64_MAX for an unused slot), so each row is taken once, in row-address order.  The three go
+ * together, each host or device.  Refused as lb2_index_search_batch refuses, except that refine_factor > 0 needs no
+ * vectors, and with LB2_INVALID_ARG kc_stride below the largest k'. */
+lb2_status lb2_index_search_candidates(lb2_index* index, const void* queries, uint64_t nq,
+                                       const lb2_query_params* params /* [nq] */, const lb2_query_filter* filters,
+                                       uint32_t num_filters, uint32_t late_width, uint32_t kc_stride,
+                                       uint64_t* cand_ids_out /* [nq][kc_stride] */, float* cand_dists_out,
+                                       uint32_t* cand_counts_out, uint32_t* nprobes_out /* nullable */,
+                                       uint64_t* distinct_ids_out /* nullable, capacity nq * kc_stride */,
+                                       uint64_t* num_distinct_out,
+                                       uint64_t* positions_out /* [nq][kc_stride]; required iff distinct_ids_out */);
+/* lb2_index_refine_taken: the exact re-rank, flat_knn over the taken rows (scanner.rs:2884-2905, flat.rs:95-148) with
+ * the arithmetic of lb2_index_search_batch's refine: the index's true metric on the original (not normalised) query
+ * in the index's element type, the k best by (distance, row id) under the f32 total order, then the query's range
+ * (scanner.rs:3342-3377).  Of params[q] only k, refine_factor and the bounds are read.  Candidate c of query q is
+ * the row taken[positions[q][c]] ([m][d], the index's element type; host pageable, pinned or device) with row id
+ * cand_ids[q][c]; a position >= m scores NaN (sorted last), as a row id past num_vectors does there.  A query with
+ * refine factor 0 returns the first k of its list as they are.  So candidates, a take of distinct_ids, and this
+ * call equal lb2_index_search_batch with the column as refine_vectors bit for bit.  Rows are [nq][k_stride], slots
+ * k_q.. UINT64_MAX / +inf; counts_out is nullable.  Only the m taken rows cross to the device; host rows past
+ * 512 MB are staged in query slabs, each slab's own rows at a time.
+ * LB2_INVALID_ARG: k == 0, k' above kc_stride, k_stride below the largest k, positions NULL with a refine query,
+ * taken NULL with m > 0.  LB2_UNSUPPORTED: k' > 1024. */
+lb2_status lb2_index_refine_taken(lb2_index* index, const void* queries /* [nq][d], the index's element type */,
+                                  uint64_t nq, const lb2_query_params* params, uint32_t kc_stride,
+                                  const uint64_t* cand_ids, const float* cand_dists, const uint32_t* cand_counts,
+                                  const void* taken /* [m][d], the index's element type */, uint64_t m,
+                                  const uint64_t* positions /* [nq][kc_stride] */, uint32_t k_stride,
+                                  uint64_t* row_ids_out /* [nq][k_stride] */, float* dists_out, uint32_t* counts_out);
 /* knn_combined (rust/lance/src/dataset/scanner.rs:2946-3027): a nearest() query on an index that does not yet cover
  * every row of its table.  The reference takes the raw vectors of the ANN rows and re-scores them exactly, runs a
  * flat KNN with the index metric over the unindexed rows (with the query's prefilter), and sorts the union by

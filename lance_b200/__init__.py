@@ -807,49 +807,13 @@ class IvfPqIndex:
         (default 1) and maximum_nprobes (None or 0 = every partition), equal to search_probed; a filter tuple's
         max_len and mask_ids and late_width serve those queries.
         Returns (ids, dists, counts, nprobes): ids / dists [nq][max k] (or `out`'s arrays and their row length)."""
-        from ._lib import QueryFilter, QueryParams
-        dt = getattr(self, "_dt", F32)
-        npdt = {F32: np.float32, F16: np.float16, U8: np.uint8, BF16: np.uint16}[dt]
-        if not isinstance(queries, (DeviceArray, PinnedArray)):
-            queries = np.ascontiguousarray(queries, dtype=npdt)
         if vectors is not None and not isinstance(vectors, (DeviceArray, PinnedArray)):
-            vectors = np.ascontiguousarray(vectors, dtype=npdt)
-        nq = int(queries.shape[0])
-
-        def per_query(name, v, dtype, default):
-            a = np.asarray(default if v is None else v, dtype=dtype)
-            if a.ndim == 0:
-                return np.full(nq, a, dtype)
-            if a.shape != (nq,):
-                raise ValueError(f"search_batch: {name} must be a scalar or an array of {nq} values, got shape {a.shape}")
-            return a
-
-        ks = per_query("k", k, np.int64, 0)
-        if nq and (ks < 1).any():
-            raise ValueError("search_batch: every k must be at least 1")
-        nps = per_query("nprobes", nprobes, np.int64, 0)
-        mins = per_query("minimum_nprobes", minimum_nprobes, np.int64, 1)
-        maxs = per_query("maximum_nprobes", maximum_nprobes, np.int64, 0)
-        if (nps < 0).any():
-            raise ValueError("search_batch: nprobes must not be negative (0: minimum / maximum nprobes)")
-        ruled = nps == 0
-        if (mins[ruled] < 1).any() or (maxs[ruled] < 0).any():
-            raise ValueError("search_batch: minimum_nprobes must be at least 1 and maximum_nprobes not negative")
-        mins, maxs = np.where(ruled, mins, 0), np.where(ruled, maxs, 0)
-        rfs = per_query("refine_factor", refine_factor, np.int64, 0)
-        if (rfs < 0).any():
-            raise ValueError("search_batch: refine_factor must not be negative")
+            vectors = np.ascontiguousarray(vectors, dtype=self._npdt())
+        queries, nq, ks, rfs, cp, cf, nf, _keep = self._batch_params(
+            "search_batch", queries, k, nprobes, minimum_nprobes, maximum_nprobes, refine_factor, filters, filter_of,
+            lower_bound, upper_bound, ef)
         if (rfs > 0).any() and vectors is None:
             raise ValueError("search_batch: refine_factor > 0 needs vectors")
-        filters = list(filters or [])
-        fof = per_query("filter_of", filter_of, np.int64, -1)
-        if ((fof < -1) | (fof >= len(filters))).any():
-            raise ValueError(f"search_batch: filter_of must be -1 or below the {len(filters)} filters")
-        lows = per_query("lower_bound", lower_bound, np.float32, np.nan)
-        ups = per_query("upper_bound", upper_bound, np.float32, np.nan)
-        efs = per_query("ef", ef, np.int64, 0)
-        if (efs < 0).any():
-            raise ValueError("search_batch: ef must not be negative")
         kmax = int(ks.max()) if nq else 1
         if out is None:
             ids, dists = np.empty((nq, kmax), np.uint64), np.empty((nq, kmax), np.float32)
@@ -859,6 +823,58 @@ class IvfPqIndex:
         if tuple(ids.shape) != (nq, k_stride) or tuple(dists.shape) != (nq, k_stride) or k_stride < kmax:
             raise ValueError(f"search_batch: out arrays must be [{nq}][>= {kmax}], got {ids.shape} and {dists.shape}")
         counts, probes = np.empty(nq, np.uint32), np.empty(nq, np.uint32)
+        qp, _k1 = as_ptr(queries)
+        vp, _k0 = as_ptr(vectors)
+        check(lib().lb2_index_search_batch(self._h, qp, C.c_uint64(nq), C.c_void_p(cp.ctypes.data), cf, C.c_uint32(nf), vp,
+                                           C.c_uint64(0 if vectors is None else vectors.shape[0]),
+                                           C.c_uint32(late_width), C.c_uint32(k_stride), as_ptr(ids)[0],
+                                           as_ptr(dists)[0], as_ptr(counts)[0], as_ptr(probes)[0]))
+        return ids, dists, counts, probes
+
+    def _npdt(self):
+        return {F32: np.float32, F16: np.float16, U8: np.uint8, BF16: np.uint16}[getattr(self, "_dt", F32)]
+
+    def _batch_params(self, name, queries, k, nprobes=None, minimum_nprobes=None, maximum_nprobes=None,
+                      refine_factor=0, filters=None, filter_of=None, lower_bound=None, upper_bound=None, ef=None):
+        """the checked per-query arguments of a batch call: (queries, nq, ks, rfs, the lb2_query_params array, the
+        lb2_query_filter array, the number of filters, keepalive)"""
+        from ._lib import QueryFilter, QueryParams
+        if not isinstance(queries, (DeviceArray, PinnedArray)):
+            queries = np.ascontiguousarray(queries, dtype=self._npdt())
+        nq = int(queries.shape[0])
+
+        def per_query(what, v, dtype, default):
+            a = np.asarray(default if v is None else v, dtype=dtype)
+            if a.ndim == 0:
+                return np.full(nq, a, dtype)
+            if a.shape != (nq,):
+                raise ValueError(f"{name}: {what} must be a scalar or an array of {nq} values, got shape {a.shape}")
+            return a
+
+        ks = per_query("k", k, np.int64, 0)
+        if nq and (ks < 1).any():
+            raise ValueError(f"{name}: every k must be at least 1")
+        nps = per_query("nprobes", nprobes, np.int64, 0)
+        mins = per_query("minimum_nprobes", minimum_nprobes, np.int64, 1)
+        maxs = per_query("maximum_nprobes", maximum_nprobes, np.int64, 0)
+        if (nps < 0).any():
+            raise ValueError(f"{name}: nprobes must not be negative (0: minimum / maximum nprobes)")
+        ruled = nps == 0
+        if (mins[ruled] < 1).any() or (maxs[ruled] < 0).any():
+            raise ValueError(f"{name}: minimum_nprobes must be at least 1 and maximum_nprobes not negative")
+        mins, maxs = np.where(ruled, mins, 0), np.where(ruled, maxs, 0)
+        rfs = per_query("refine_factor", refine_factor, np.int64, 0)
+        if (rfs < 0).any():
+            raise ValueError(f"{name}: refine_factor must not be negative")
+        filters = list(filters or [])
+        fof = per_query("filter_of", filter_of, np.int64, -1)
+        if ((fof < -1) | (fof >= len(filters))).any():
+            raise ValueError(f"{name}: filter_of must be -1 or below the {len(filters)} filters")
+        lows = per_query("lower_bound", lower_bound, np.float32, np.nan)
+        ups = per_query("upper_bound", upper_bound, np.float32, np.nan)
+        efs = per_query("ef", ef, np.int64, 0)
+        if (efs < 0).any():
+            raise ValueError(f"{name}: ef must not be negative")
         keep = []
         cf = (QueryFilter * max(1, len(filters)))()
         for i, f in enumerate(filters):
@@ -879,20 +895,78 @@ class IvfPqIndex:
         cp = np.zeros(max(1, nq), np.dtype({"names": [f for f, _ in QueryParams._fields_],
                                             "formats": [np.float32 if t is C.c_float else np.uint32
                                                         for _, t in QueryParams._fields_]}))
-        for name, col in (("k", ks), ("nprobes", nps), ("minimum_nprobes", mins), ("maximum_nprobes", maxs),
-                          ("refine_factor", rfs), ("ef", efs)):
-            cp[name][:nq] = col
+        for field, col in (("k", ks), ("nprobes", nps), ("minimum_nprobes", mins), ("maximum_nprobes", maxs),
+                           ("refine_factor", rfs), ("ef", efs)):
+            cp[field][:nq] = col
         cp["filter"][:nq] = np.where(fof < 0, 0xFFFFFFFF, fof)
         cp["has_lower_bound"][:nq], cp["has_upper_bound"][:nq] = ~np.isnan(lows), ~np.isnan(ups)
         cp["lower_bound"][:nq], cp["upper_bound"][:nq] = np.nan_to_num(lows, nan=0.0), np.nan_to_num(ups, nan=0.0)
         assert cp.dtype.itemsize == C.sizeof(QueryParams)
-        qp, _k1 = as_ptr(queries)
-        vp, _k0 = as_ptr(vectors)
-        check(lib().lb2_index_search_batch(self._h, qp, C.c_uint64(nq), C.c_void_p(cp.ctypes.data), cf, C.c_uint32(len(filters)), vp,
-                                           C.c_uint64(0 if vectors is None else vectors.shape[0]),
-                                           C.c_uint32(late_width), C.c_uint32(k_stride), as_ptr(ids)[0],
-                                           as_ptr(dists)[0], as_ptr(counts)[0], as_ptr(probes)[0]))
-        return ids, dists, counts, probes
+        return queries, nq, ks, rfs, cp, cf, len(filters), keep
+
+    def search_candidates(self, queries, k, nprobes=None, minimum_nprobes=None, maximum_nprobes=None,
+                          refine_factor=0, filters=None, filter_of=None, lower_bound=None, upper_bound=None, ef=None,
+                          late_width=1, distinct=False, kc_stride=None):
+        """lb2_index_search_candidates: the index half of a refined batch.  Takes search_batch's per-query arguments
+        (no vectors).  Row q of ids / dists [nq][kc_stride] (default: the largest k * max(1, refine_factor)) is the
+        list search_batch re-ranks for query q, counts[q] entries long; unused slots hold UINT64_MAX / +inf.
+        Returns (ids, dists, counts, nprobes), and with distinct=True also (distinct_ids, positions): the batch's
+        ascending distinct row ids and, per slot, the index of its id in them (UINT64_MAX for an unused slot).
+        Take the rows of distinct_ids and pass them to refine_taken."""
+        queries, nq, ks, rfs, cp, cf, nf, _keep = self._batch_params(
+            "search_candidates", queries, k, nprobes, minimum_nprobes, maximum_nprobes, refine_factor, filters,
+            filter_of, lower_bound, upper_bound, ef)
+        kcmax = int((ks * np.maximum(rfs, 1)).max()) if nq else 1
+        kc_stride = kcmax if kc_stride is None else int(kc_stride)
+        ids, dists = np.empty((nq, kc_stride), np.uint64), np.empty((nq, kc_stride), np.float32)
+        counts, probes = np.empty(nq, np.uint32), np.empty(nq, np.uint32)
+        uniq = np.empty(max(1, nq * kc_stride), np.uint64) if distinct else None
+        pos = np.empty((nq, kc_stride), np.uint64) if distinct else None
+        m = np.zeros(1, np.uint64)
+        check(lib().lb2_index_search_candidates(self._h, as_ptr(queries)[0], C.c_uint64(nq), C.c_void_p(cp.ctypes.data),
+                                                cf, C.c_uint32(nf), C.c_uint32(late_width), C.c_uint32(kc_stride),
+                                                as_ptr(ids)[0], as_ptr(dists)[0], as_ptr(counts)[0], as_ptr(probes)[0],
+                                                as_ptr(uniq)[0], as_ptr(m if distinct else None)[0], as_ptr(pos)[0]))
+        if not distinct:
+            return ids, dists, counts, probes
+        return ids, dists, counts, probes, uniq[:int(m[0])].copy(), pos
+
+    def refine_taken(self, queries, candidates, taken, positions, k, refine_factor=0, lower_bound=None,
+                     upper_bound=None, out=None):
+        """lb2_index_refine_taken: the exact re-rank of the rows the caller took.  `candidates` = (ids, dists,
+        counts) of search_candidates; `taken` [m][d] (numpy, PinnedArray or DeviceArray, the index's element type)
+        holds the rows of its distinct_ids, and `positions` is its positions array.  k, refine_factor and the
+        bounds are search_candidates' per-query values.  Equal to search_batch with the column as `vectors`.
+        Returns (ids, dists, counts): ids / dists [nq][max k] (or `out`'s arrays and their row length)."""
+        cid, cd, cc = candidates
+        queries, nq, ks, _rfs, cp, _cf, _nf, _keep = self._batch_params(
+            "refine_taken", queries, k, 1, None, None, refine_factor, None, None, lower_bound, upper_bound, None)
+        cid = cid if isinstance(cid, DeviceArray) else np.ascontiguousarray(cid, np.uint64)
+        cd = cd if isinstance(cd, DeviceArray) else np.ascontiguousarray(cd, np.float32)
+        cc = cc if isinstance(cc, DeviceArray) else np.ascontiguousarray(cc, np.uint32)
+        if tuple(cid.shape[:1]) != (nq,) or len(cid.shape) != 2 or tuple(cd.shape) != tuple(cid.shape):
+            raise ValueError(f"refine_taken: candidate arrays must be [{nq}][kc_stride], got {cid.shape} and {cd.shape}")
+        kc_stride = int(cid.shape[1])
+        if positions is not None and not isinstance(positions, DeviceArray):
+            positions = np.ascontiguousarray(positions, np.uint64)
+        if positions is not None and tuple(positions.shape) != tuple(cid.shape):
+            raise ValueError(f"refine_taken: positions must be [{nq}][{kc_stride}], got {positions.shape}")
+        if not isinstance(taken, (DeviceArray, PinnedArray)):
+            taken = np.ascontiguousarray(taken, dtype=self._npdt())
+        kmax = int(ks.max()) if nq else 1
+        if out is None:
+            ids, dists = np.empty((nq, kmax), np.uint64), np.empty((nq, kmax), np.float32)
+        else:
+            ids, dists = out
+        k_stride = int(ids.shape[1]) if len(ids.shape) == 2 else kmax
+        if tuple(ids.shape) != (nq, k_stride) or tuple(dists.shape) != (nq, k_stride) or k_stride < kmax:
+            raise ValueError(f"refine_taken: out arrays must be [{nq}][>= {kmax}], got {ids.shape} and {dists.shape}")
+        counts = np.empty(nq, np.uint32)
+        check(lib().lb2_index_refine_taken(self._h, as_ptr(queries)[0], C.c_uint64(nq), C.c_void_p(cp.ctypes.data),
+                                           C.c_uint32(kc_stride), as_ptr(cid)[0], as_ptr(cd)[0], as_ptr(cc)[0],
+                                           as_ptr(taken)[0], C.c_uint64(int(taken.shape[0])), as_ptr(positions)[0],
+                                           C.c_uint32(k_stride), as_ptr(ids)[0], as_ptr(dists)[0], as_ptr(counts)[0]))
+        return ids, dists, counts
 
     def search_combined(self, queries, k, vectors, unindexed_vectors, unindexed_row_ids, nprobes=None,
                         minimum_nprobes=None, maximum_nprobes=None, late_width=1, refine_factor=0, allow_bitmap=None,

@@ -148,7 +148,8 @@ EXPORTS = [
     "lb2_index_export_storage", "lb2_index_load_storage",
     "lb2_partition_index_uses_graph", "lb2_partition_index_build", "lb2_partition_index_assign",
     "lb2_partition_index_info", "lb2_partition_index_export", "lb2_partition_index_destroy",
-    "lb2_index_set_partition_index", "lb2_index_search_batch",
+    "lb2_index_set_partition_index", "lb2_index_search_batch", "lb2_index_search_candidates",
+    "lb2_index_refine_taken",
 ]
 
 _lib = None
@@ -180,6 +181,12 @@ def lib():
         L.lb2_index_create_sq.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_int, C.c_int, C.c_double,
                                           C.c_double, C.POINTER(C.c_void_p)]
         L.lb2_rq_rotation.argtypes = [C.c_uint32, C.c_uint64, C.c_void_p]
+        L.lb2_index_search_candidates.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                                  C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.lb2_index_refine_taken.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32,
+                                             C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 

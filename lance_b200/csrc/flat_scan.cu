@@ -114,14 +114,34 @@ void ivfflat_search(const IvfSearch& s, const void* vectors, int vdt) {
 // refine: exact distances of k' = k * refine_factor candidates from the raw vectors, then the k
 // best by (distance, row id)  (scanner.rs:2884-2905, flat.rs:95-148)
 // ------------------------------------------------------------------------------------------------
+// Where the refine kernel reads candidate c's row: null scores NaN, as a row the column does not hold.
+// ColumnRows: by row id from the dense column (lb2_index_search_ex / _batch's refine_vectors).
+template <class T>
+struct ColumnRows {
+  const T* v;
+  uint64_t n;
+  __device__ const T* row(size_t, uint32_t, uint64_t id, int d) const { return id < n ? v + id * (uint64_t)d : nullptr; }
+};
+// TakenRows: by the candidate's position in the rows the caller took (lb2_index_refine_taken), [nq][stride]
+template <class T>
+struct TakenRows {
+  const T* v;
+  uint64_t m;
+  const uint64_t* pos;
+  int stride;
+  __device__ const T* row(size_t qi, uint32_t c, uint64_t, int d) const {
+    const uint64_t p = pos[qi * stride + c];
+    return p < m ? v + p * (uint64_t)d : nullptr;
+  }
+};
+
 // BATCH: per-query values from qo (refine_batch_f32); the single-parameter refine is compiled without them
-template <int METRIC, class T, bool BATCH>
+template <int METRIC, class T, bool BATCH, class Rows>
 __global__ void __launch_bounds__(256)
-refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ vectors,
-              uint64_t num_vectors, const uint64_t* __restrict__ cand_id, const uint32_t* __restrict__ cand_cnt,
-              int kc, int k, uint64_t* __restrict__ out_id, float* __restrict__ out_d,
-              uint32_t* __restrict__ out_cnt, int has_lower, float lower, int has_upper, float upper,
-              const float* __restrict__ cand_d, const QueryOut* __restrict__ qo, int k_stride) {
+refine_kernel(const float* __restrict__ queries, int d, const Rows rows, const uint64_t* __restrict__ cand_id,
+              const uint32_t* __restrict__ cand_cnt, int kc, int k, uint64_t* __restrict__ out_id,
+              float* __restrict__ out_d, uint32_t* __restrict__ out_cnt, int has_lower, float lower, int has_upper,
+              float upper, const float* __restrict__ cand_d, const QueryOut* __restrict__ qo, int k_stride) {
   extern __shared__ float smem[];
   float* qs = smem;       // [d]
   float* cd = qs + d;     // [kc]
@@ -158,9 +178,9 @@ refine_kernel(const float* __restrict__ queries, int d, const T* __restrict__ ve
   __syncthreads();
   const float qn = METRIC == METRIC_COSINE ? s_qnorm : 0.0f;
   for (uint32_t c = tid >> 4; c < cnt; c += 16) {
-    const uint64_t id = ids[c];
+    const T* row = rows.row(qi, c, ids[c], d);
     float dist = __int_as_float(0x7fc00000);
-    if (id < num_vectors) dist = refine_row_distance<METRIC, T>(qs, vectors + id * (uint64_t)d, d, l, hmask, qn);
+    if (row) dist = refine_row_distance<METRIC, T>(qs, row, d, l, hmask, qn);
     if (l == 0) cd[c] = dist;
   }
   __syncthreads();
@@ -193,26 +213,55 @@ void refine_f32(const float* queries, uint64_t nq, int d, int metric, const void
   const size_t smem = sizeof(float) * ((size_t)d + kc);
   dispatch_metric_elem<true>(metric, vdt, [&](auto m, auto e) {
     using T = typename decltype(e)::type;
-    auto kern = refine_kernel<decltype(m)::value, T, false>;
+    auto kern = refine_kernel<decltype(m)::value, T, false, ColumnRows<T>>;
     set_smem(kern, smem);
-    LB2_LAUNCH("refine", kern, (unsigned)nq, 256, smem, queries, d, reinterpret_cast<const T*>(vectors), num_vectors,
-               cand_id, cand_cnt, kc, k, out_id, out_d, out_cnt, has_lower, lower, has_upper, upper,
-               (const float*)nullptr, (const QueryOut*)nullptr, k);
+    LB2_LAUNCH("refine", kern, (unsigned)nq, 256, smem, queries, d,
+               ColumnRows<T>{reinterpret_cast<const T*>(vectors), num_vectors}, cand_id, cand_cnt, kc, k, out_id,
+               out_d, out_cnt, has_lower, lower, has_upper, upper, (const float*)nullptr, (const QueryOut*)nullptr, k);
   });
 }
 
 void refine_batch_f32(const float* queries, uint64_t nq, int d, int metric, const void* vectors, int vdt,
                       uint64_t num_vectors, const float* cand_d, const uint64_t* cand_id, const uint32_t* cand_cnt,
-                      int kc, const QueryOut* qo, int k_stride, uint64_t* out_id, float* out_d, uint32_t* out_cnt) {
+                      int kc, const QueryOut* qo, int k_stride, uint64_t* out_id, float* out_d, uint32_t* out_cnt,
+                      const uint64_t* positions) {
   if (nq == 0) return;
   const size_t smem = sizeof(float) * ((size_t)d + kc);
   dispatch_metric_elem<true>(metric, vdt, [&](auto m, auto e) {
     using T = typename decltype(e)::type;
-    auto kern = refine_kernel<decltype(m)::value, T, true>;
-    set_smem(kern, smem);
-    LB2_LAUNCH("refine", kern, (unsigned)nq, 256, smem, queries, d, reinterpret_cast<const T*>(vectors), num_vectors,
-               cand_id, cand_cnt, kc, k_stride, out_id, out_d, out_cnt, 0, 0.0f, 0, 0.0f, cand_d, qo, k_stride);
+    auto launch = [&](auto kern, auto rows) {
+      set_smem(kern, smem);
+      LB2_LAUNCH("refine", kern, (unsigned)nq, 256, smem, queries, d, rows, cand_id, cand_cnt, kc, k_stride, out_id,
+                 out_d, out_cnt, 0, 0.0f, 0, 0.0f, cand_d, qo, k_stride);
+    };
+    const T* v = reinterpret_cast<const T*>(vectors);
+    if (positions)
+      launch(refine_kernel<decltype(m)::value, T, true, TakenRows<T>>, TakenRows<T>{v, num_vectors, positions, kc});
+    else
+      launch(refine_kernel<decltype(m)::value, T, true, ColumnRows<T>>, ColumnRows<T>{v, num_vectors});
   });
+}
+
+// lb2_index_search_candidates' rows: query q's merged list (stride kc, its own k' = qo[q].kc entries at most) into
+// a row of `stride`, unused slots UINT64_MAX / +inf
+__global__ void candidate_rows_kernel(const uint64_t* __restrict__ cid, const float* __restrict__ cdist,
+                                      const uint32_t* __restrict__ ccnt, int kc, const QueryOut* __restrict__ qo,
+                                      int stride, uint64_t* __restrict__ out_id, float* __restrict__ out_d,
+                                      uint32_t* __restrict__ out_cnt) {
+  const size_t qi = blockIdx.x;
+  const uint32_t r = min(ccnt[qi], (uint32_t)qo[qi].kc);
+  for (int e = threadIdx.x; e < stride; e += blockDim.x) {
+    out_id[qi * stride + e] = (uint32_t)e < r ? cid[qi * kc + e] : ~0ull;
+    out_d[qi * stride + e] = (uint32_t)e < r ? cdist[qi * kc + e] : __int_as_float(0x7f800000);
+  }
+  if (threadIdx.x == 0) out_cnt[qi] = r;
+}
+
+void candidate_rows(const uint64_t* cid, const float* cdist, const uint32_t* ccnt, uint64_t nq, int kc,
+                    const QueryOut* qo, int stride, uint64_t* out_id, float* out_d, uint32_t* out_cnt) {
+  if (nq == 0) return;
+  LB2_LAUNCH("candidate_rows", candidate_rows_kernel, (unsigned)nq, 256, 0, cid, cdist, ccnt, kc, qo, stride, out_id,
+             out_d, out_cnt);
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -1064,54 +1064,158 @@ lb2_status lb2_index_search_hnsw(lb2_index* index, const void* queries, uint64_t
 // as its largest nprobes; a query's other slots probe the empty partition.  A batch with minimum / maximum nprobes
 // queries runs the probe rule for every query, each with its own QueryProbe: a fixed nprobes p is minimum = maximum =
 // p, which lb2_index_search_probed defines to equal lb2_index_search_ex.
+// lb2_index_search_batch and lb2_index_search_candidates share everything up to the merged candidate lists:
+// BatchPlan checks the batch (have_vectors: refine_factor > 0 is allowed), BatchSearch runs it.
+namespace {
+struct BatchPlan {
+  uint32_t kmax = 0, kcmax = 0, npmax = 0, efmax = 0, Lmax = 0;
+  bool any_refine = false, any_filter = false, any_range = false, any_probed = false;
+  BatchPlan(const lb2_index* index, const void* queries, uint64_t nq, const lb2_query_params* params,
+            const lb2_query_filter* filters, uint32_t num_filters, uint32_t late_width, bool have_vectors) {
+    LB2_REQUIRE(index, "null index");
+    LB2_REQUIRE(nq == 0 || (queries && params), "null queries or params");
+    LB2_REQUIRE(num_filters == 0 || filters, "null filters");
+    LB2_REQUIRE(late_width >= 1, "late_width must be at least 1");
+    const uint32_t K = (uint32_t)index->K;
+    for (uint64_t q = 0; q < nq; ++q) {
+      const lb2_query_params& p = params[q];
+      const unsigned long long qi = (unsigned long long)q;
+      LB2_REQUIRE(p.k > 0, "query %llu: k must be positive", qi);
+      LB2_REQUIRE(p.filter < num_filters || p.filter == UINT32_MAX, "query %llu: filter %u is not below num_filters %u",
+                  qi, p.filter, num_filters);
+      LB2_REQUIRE(p.ef == 0 || index->hnsw, "query %llu: ef is set on an index without HNSW graphs", qi);
+      LB2_REQUIRE(p.refine_factor == 0 || have_vectors, "query %llu: refine_factor > 0 needs refine_vectors", qi);
+      if (p.nprobes == 0) {  // lb2_index_search_probed's checks
+        LB2_REQUIRE(p.minimum_nprobes >= 1, "query %llu: minimum_nprobes must be at least 1", qi);
+        LB2_REQUIRE(p.maximum_nprobes == 0 || p.maximum_nprobes >= p.minimum_nprobes,
+                    "query %llu: maximum_nprobes %u is below minimum_nprobes %u", qi, p.maximum_nprobes,
+                    p.minimum_nprobes);
+        LB2_REQUIRE(p.filter == UINT32_MAX || filters[p.filter].allow_bitmap ||
+                        (!filters[p.filter].has_max_len && !filters[p.filter].mask_ids),
+                    "query %llu: max_len and mask_ids need an allow bitmap", qi);
+        any_probed = true;
+      }
+      const uint64_t kc = (uint64_t)p.k * std::max<uint32_t>(1, p.refine_factor);
+      if (kc > 1024)
+        fail(LB2_UNSUPPORTED, "query %llu: k * refine_factor = %llu > 1024 is not implemented", qi, (unsigned long long)kc);
+      const uint32_t ef = p.ef ? p.ef : (uint32_t)(kc + kc / 2);
+      if (index->hnsw && ef < kc)
+        fail(LB2_INVALID_ARG, "query %llu: %s: ef = %u must be greater than or equal to k = %u", qi, index->hnsw->kind,
+             ef, (uint32_t)kc);
+      kmax = std::max(kmax, p.k);
+      kcmax = std::max(kcmax, (uint32_t)kc);
+      npmax = std::max(npmax, std::min(p.nprobes, K));
+      const uint32_t mx = p.nprobes ? p.nprobes : p.maximum_nprobes;
+      Lmax = std::max(Lmax, mx ? std::min(mx, K) : K);
+      efmax = std::max(efmax, ef);
+      any_refine |= p.refine_factor > 0;
+      any_filter |= p.filter != UINT32_MAX || p.has_lower_bound || p.has_upper_bound;
+      any_range |= p.has_lower_bound || p.has_upper_bound;
+    }
+  }
+};
+
+// the batch's scan up to the merged lists: cid / cdist [nq][kcmax], ccnt [nq], each query's QueryOut in qo; nprobes
+// (device, nullable) receives nprobes_out.  nq > 0.
+struct BatchSearch {
+  const SearchQueries q;
+  DevBuf<uint64_t> cid;
+  DevBuf<float> cdist;
+  DevBuf<uint32_t> ccnt;
+  DevBuf<QueryOut> qo;
+  std::vector<uint32_t> qnp_h;
+  BatchSearch(lb2_index* index, const void* queries, uint64_t nq, const lb2_query_params* params,
+              const lb2_query_filter* filters, uint32_t num_filters, uint32_t late_width, const BatchPlan& b,
+              uint32_t* nprobes)
+      : q(index, queries, nq), cid((size_t)nq * b.kcmax), cdist((size_t)nq * b.kcmax), ccnt(nq), qo(nq), qnp_h(nq) {
+    const uint32_t K = (uint32_t)index->K;
+    const int d = index->d;
+    // the filters, staged once each (with the probe rule also their allow lists' ids), and their allowed rows per
+    // partition in one launch: IVF_HNSW_*'s `remained`, and the probe rule's c_p (row num_filters: no prefilter)
+    const size_t words = (size_t)((index->n + 63) / 64);
+    std::vector<InArg<uint64_t>> allow(num_filters), ids(num_filters);
+    std::vector<const uint64_t*> allow_h(num_filters + 1, nullptr), ids_h(num_filters, nullptr);
+    DevBuf<uint64_t> no_ids(1);  // an iterable, empty allow list
+    for (uint32_t f = 0; f < num_filters; ++f) {
+      allow[f].set(filters[f].allow_bitmap, filters[f].allow_bitmap ? words : 0);
+      allow_h[f] = allow[f].get();
+      if (b.any_probed && filters[f].mask_ids) {
+        ids[f].set(filters[f].mask_ids, filters[f].num_mask_ids);
+        ids_h[f] = ids[f].get() ? ids[f].get() : no_ids.p;
+      }
+    }
+    DevBuf<uint32_t> acnt;
+    if ((index->hnsw && num_filters) || b.any_probed) {
+      DevBuf<const uint64_t*> tab(num_filters + 1);
+      h2d(tab.p, allow_h.data(), num_filters + 1);
+      acnt.alloc((size_t)(num_filters + 1) * K);
+      partition_counts_table(index->part_offsets.p, (int)K, tab.p, (int)num_filters + 1, acnt.p);
+    }
+    std::vector<QueryProbe> qpr_h(b.any_probed ? nq : 0);
+    bool any_iterable = false;
+    std::vector<QueryParam> qp_h(nq);
+    std::vector<QueryOut> qo_h(nq);
+    for (uint64_t i = 0; i < nq; ++i) {
+      const lb2_query_params& p = params[i];
+      const bool filtered = p.filter != UINT32_MAX && allow_h[p.filter];
+      const int kc = (int)p.k * (int)std::max<uint32_t>(1, p.refine_factor);
+      qp_h[i].flt = make_filter(filtered ? allow_h[p.filter] : nullptr, p.has_lower_bound != 0, p.lower_bound,
+                                p.has_upper_bound != 0, p.upper_bound);
+      qp_h[i].k = kc;
+      qp_h[i].ef = p.ef ? p.ef : (uint32_t)(kc + kc / 2);
+      qp_h[i].acnt = filtered && acnt.p ? acnt.p + (size_t)p.filter * K : nullptr;
+      qo_h[i] = QueryOut{kc, (int)p.k, p.refine_factor > 0, (int)(p.has_lower_bound != 0),
+                         (int)(p.has_upper_bound != 0), p.lower_bound, p.upper_bound};
+      qnp_h[i] = std::min(p.nprobes, K);
+      if (b.any_probed) {  // a fixed nprobes p: minimum = maximum = p, no shortcut
+        const uint32_t f = p.filter == UINT32_MAX ? num_filters : p.filter;
+        const bool probed = p.nprobes == 0;
+        const uint32_t mx = probed ? p.maximum_nprobes : p.nprobes;
+        const uint64_t* mids = probed && f < num_filters ? ids_h[f] : nullptr;
+        qpr_h[i] = QueryProbe{probed ? p.minimum_nprobes : p.nprobes, mx ? std::min(mx, K) : K, p.k, (uint32_t)kc,
+                              p.has_lower_bound || p.has_upper_bound, probed && f < num_filters && filters[f].has_max_len,
+                              probed && f < num_filters ? filters[f].max_len : 0, mids,
+                              mids ? filters[f].num_mask_ids : 0, acnt.p + (size_t)(allow_h[f] ? f : num_filters) * K};
+        any_iterable |= mids != nullptr;
+      }
+    }
+    DevBuf<QueryParam> qp(nq);
+    DevBuf<uint32_t> qnp(nq);
+    h2d(qp.p, qp_h.data(), nq);
+    h2d(qo.p, qo_h.data(), nq);
+    h2d(qnp.p, qnp_h.data(), nq);
+    DevBuf<QueryProbe> qpr(qpr_h.size());
+    if (b.any_probed) h2d(qpr.p, qpr_h.data(), nq);
+    TagScope tg("search");
+    IvfSearch s{index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->row_ids.p, q.get(), nq,
+                (int)b.kcmax, (int)b.npmax, cid.p, cdist.p, ccnt.p, ScanFilter{}, nullptr};
+    s.qp = qp.p;
+    s.qp_host = qp_h.data();
+    s.qnp = qnp.p;
+    s.any_filter = b.any_filter;
+    s.any_range = b.any_range;
+    ProbeRule pr;
+    if (b.any_probed) {
+      pr.max_np = b.Lmax;
+      pr.late_width = late_width;
+      pr.mask_ids = any_iterable ? no_ids.p : nullptr;  // non-null: lists get a shortcut slot
+      pr.nprobes_out = nprobes;
+      pr.qpr = qpr.p;
+      s.pr = &pr;
+    }
+    search_kind(index, s, b.efmax);
+    if (nprobes && !b.any_probed) h2d(nprobes, qnp_h.data(), nq);
+  }
+};
+}  // namespace
+
 lb2_status lb2_index_search_batch(lb2_index* index, const void* queries, uint64_t nq, const lb2_query_params* params,
                                   const lb2_query_filter* filters, uint32_t num_filters, const void* refine_vectors,
                                   uint64_t num_vectors, uint32_t late_width, uint32_t k_stride, uint64_t* row_ids_out,
                                   float* dists_out, uint32_t* counts_out, uint32_t* nprobes_out) {
   LB2_API_BEGIN
-  LB2_REQUIRE(index, "null index");
-  LB2_REQUIRE(nq == 0 || (queries && params), "null queries or params");
-  LB2_REQUIRE(num_filters == 0 || filters, "null filters");
-  LB2_REQUIRE(late_width >= 1, "late_width must be at least 1");
-  const uint32_t K = (uint32_t)index->K;
-  uint32_t kmax = 0, kcmax = 0, npmax = 0, efmax = 0, Lmax = 0;
-  bool any_refine = false, any_filter = false, any_range = false, any_probed = false;
-  for (uint64_t q = 0; q < nq; ++q) {
-    const lb2_query_params& p = params[q];
-    const unsigned long long qi = (unsigned long long)q;
-    LB2_REQUIRE(p.k > 0, "query %llu: k must be positive", qi);
-    LB2_REQUIRE(p.filter < num_filters || p.filter == UINT32_MAX, "query %llu: filter %u is not below num_filters %u",
-                qi, p.filter, num_filters);
-    LB2_REQUIRE(p.ef == 0 || index->hnsw, "query %llu: ef is set on an index without HNSW graphs", qi);
-    LB2_REQUIRE(p.refine_factor == 0 || refine_vectors, "query %llu: refine_factor > 0 needs refine_vectors", qi);
-    if (p.nprobes == 0) {  // lb2_index_search_probed's checks
-      LB2_REQUIRE(p.minimum_nprobes >= 1, "query %llu: minimum_nprobes must be at least 1", qi);
-      LB2_REQUIRE(p.maximum_nprobes == 0 || p.maximum_nprobes >= p.minimum_nprobes,
-                  "query %llu: maximum_nprobes %u is below minimum_nprobes %u", qi, p.maximum_nprobes,
-                  p.minimum_nprobes);
-      LB2_REQUIRE(p.filter == UINT32_MAX || filters[p.filter].allow_bitmap ||
-                      (!filters[p.filter].has_max_len && !filters[p.filter].mask_ids),
-                  "query %llu: max_len and mask_ids need an allow bitmap", qi);
-      any_probed = true;
-    }
-    const uint64_t kc = (uint64_t)p.k * std::max<uint32_t>(1, p.refine_factor);
-    if (kc > 1024)
-      fail(LB2_UNSUPPORTED, "query %llu: k * refine_factor = %llu > 1024 is not implemented", qi, (unsigned long long)kc);
-    const uint32_t ef = p.ef ? p.ef : (uint32_t)(kc + kc / 2);
-    if (index->hnsw && ef < kc)
-      fail(LB2_INVALID_ARG, "query %llu: %s: ef = %u must be greater than or equal to k = %u", qi, index->hnsw->kind, ef,
-           (uint32_t)kc);
-    kmax = std::max(kmax, p.k);
-    kcmax = std::max(kcmax, (uint32_t)kc);
-    npmax = std::max(npmax, std::min(p.nprobes, K));
-    const uint32_t mx = p.nprobes ? p.nprobes : p.maximum_nprobes;
-    Lmax = std::max(Lmax, mx ? std::min(mx, K) : K);
-    efmax = std::max(efmax, ef);
-    any_refine |= p.refine_factor > 0;
-    any_filter |= p.filter != UINT32_MAX || p.has_lower_bound || p.has_upper_bound;
-    any_range |= p.has_lower_bound || p.has_upper_bound;
-  }
-  LB2_REQUIRE(k_stride >= kmax, "k_stride %u is below the largest k %u", k_stride, kmax);
+  const BatchPlan b(index, queries, nq, params, filters, num_filters, late_width, refine_vectors != nullptr);
+  LB2_REQUIRE(k_stride >= b.kmax, "k_stride %u is below the largest k %u", k_stride, b.kmax);
   if (current_comm() && current_comm()->nranks > 1)
     fail(LB2_UNSUPPORTED, "a batch search on a row-sharded index is not implemented");
   if (nq == 0) {
@@ -1119,97 +1223,160 @@ lb2_status lb2_index_search_batch(lb2_index* index, const void* queries, uint64_
     return LB2_OK;
   }
   const int d = index->d;
-  const SearchQueries q(index, queries, nq);
-  // the filters, staged once each (with the probe rule also their allow lists' ids), and their allowed rows per
-  // partition in one launch: IVF_HNSW_*'s `remained`, and the probe rule's c_p (row num_filters: no prefilter)
-  const size_t words = (size_t)((index->n + 63) / 64);
-  std::vector<InArg<uint64_t>> allow(num_filters), ids(num_filters);
-  std::vector<const uint64_t*> allow_h(num_filters + 1, nullptr), ids_h(num_filters, nullptr);
-  DevBuf<uint64_t> no_ids(1);  // an iterable, empty allow list
-  for (uint32_t f = 0; f < num_filters; ++f) {
-    allow[f].set(filters[f].allow_bitmap, filters[f].allow_bitmap ? words : 0);
-    allow_h[f] = allow[f].get();
-    if (any_probed && filters[f].mask_ids) {
-      ids[f].set(filters[f].mask_ids, filters[f].num_mask_ids);
-      ids_h[f] = ids[f].get() ? ids[f].get() : no_ids.p;
-    }
-  }
-  DevBuf<uint32_t> acnt;
-  if ((index->hnsw && num_filters) || any_probed) {
-    DevBuf<const uint64_t*> tab(num_filters + 1);
-    h2d(tab.p, allow_h.data(), num_filters + 1);
-    acnt.alloc((size_t)(num_filters + 1) * K);
-    partition_counts_table(index->part_offsets.p, (int)K, tab.p, (int)num_filters + 1, acnt.p);
-  }
-  std::vector<QueryProbe> qpr_h(any_probed ? nq : 0);
-  bool any_iterable = false;
-  std::vector<QueryParam> qp_h(nq);
-  std::vector<QueryOut> qo_h(nq);
-  std::vector<uint32_t> qnp_h(nq);
-  for (uint64_t i = 0; i < nq; ++i) {
-    const lb2_query_params& p = params[i];
-    const bool filtered = p.filter != UINT32_MAX && allow_h[p.filter];
-    const int kc = (int)p.k * (int)std::max<uint32_t>(1, p.refine_factor);
-    qp_h[i].flt = make_filter(filtered ? allow_h[p.filter] : nullptr, p.has_lower_bound != 0, p.lower_bound,
-                              p.has_upper_bound != 0, p.upper_bound);
-    qp_h[i].k = kc;
-    qp_h[i].ef = p.ef ? p.ef : (uint32_t)(kc + kc / 2);
-    qp_h[i].acnt = filtered && acnt.p ? acnt.p + (size_t)p.filter * K : nullptr;
-    qo_h[i] = QueryOut{kc, (int)p.k, p.refine_factor > 0, (int)(p.has_lower_bound != 0), (int)(p.has_upper_bound != 0),
-                       p.lower_bound, p.upper_bound};
-    qnp_h[i] = std::min(p.nprobes, K);
-    if (any_probed) {  // a fixed nprobes p: minimum = maximum = p, no shortcut
-      const uint32_t f = p.filter == UINT32_MAX ? num_filters : p.filter;
-      const bool probed = p.nprobes == 0;
-      const uint32_t mx = probed ? p.maximum_nprobes : p.nprobes;
-      const uint64_t* mids = probed && f < num_filters ? ids_h[f] : nullptr;
-      qpr_h[i] = QueryProbe{probed ? p.minimum_nprobes : p.nprobes, mx ? std::min(mx, K) : K, p.k, (uint32_t)kc,
-                            p.has_lower_bound || p.has_upper_bound, probed && f < num_filters && filters[f].has_max_len, probed && f < num_filters ?
-                            filters[f].max_len : 0, mids, mids ? filters[f].num_mask_ids : 0,
-                            acnt.p + (size_t)(allow_h[f] ? f : num_filters) * K};
-      any_iterable |= mids != nullptr;
-    }
-  }
-  DevBuf<QueryParam> qp(nq);
-  DevBuf<QueryOut> qo(nq);
-  DevBuf<uint32_t> qnp(nq);
-  h2d(qp.p, qp_h.data(), nq);
-  h2d(qo.p, qo_h.data(), nq);
-  h2d(qnp.p, qnp_h.data(), nq);
-  DevBuf<QueryProbe> qpr(qpr_h.size());
-  if (any_probed) h2d(qpr.p, qpr_h.data(), nq);
   OutArg<uint64_t> oi(row_ids_out, (size_t)nq * k_stride);
   OutArg<float> od(dists_out, (size_t)nq * k_stride);
   OutArg<uint32_t> oc(counts_out, nq);
   OutArg<uint32_t> onp(nprobes_out, nq);
-  DevBuf<uint64_t> cid((size_t)nq * kcmax);
-  DevBuf<float> cdist((size_t)nq * kcmax);
-  DevBuf<uint32_t> ccnt(nq);
+  BatchSearch bs(index, queries, nq, params, filters, num_filters, late_width, b, onp.get());
   {
     TagScope tg("search");
-    IvfSearch s{index->centroids.p, index->K, d, index->metric, index->part_offsets.p, index->row_ids.p, q.get(), nq,
-                (int)kcmax, (int)npmax, cid.p, cdist.p, ccnt.p, ScanFilter{}, nullptr};
-    s.qp = qp.p;
-    s.qp_host = qp_h.data();
-    s.qnp = qnp.p;
-    s.any_filter = any_filter;
-    s.any_range = any_range;
-    ProbeRule pr;
-    if (any_probed) {
-      pr.max_np = Lmax;
-      pr.late_width = late_width;
-      pr.mask_ids = any_iterable ? no_ids.p : nullptr;  // non-null: lists get a shortcut slot
-      pr.nprobes_out = onp.get();
-      pr.qpr = qpr.p;
-      s.pr = &pr;
-    }
-    search_kind(index, s, efmax);
-    InArg<uint8_t> v(any_refine ? refine_vectors : nullptr, (size_t)num_vectors * d * dtype_size(index->dtype));
-    refine_batch_f32(q.q.get(), nq, d, index->metric, v.get(), (int)index->dtype, num_vectors, cdist.p, cid.p, ccnt.p,
-                     (int)kcmax, qo.p, (int)k_stride, oi.get(), od.get(), oc.get());
+    InArg<uint8_t> v(b.any_refine ? refine_vectors : nullptr, (size_t)num_vectors * d * dtype_size(index->dtype));
+    refine_batch_f32(bs.q.q.get(), nq, d, index->metric, v.get(), (int)index->dtype, num_vectors, bs.cdist.p,
+                     bs.cid.p, bs.ccnt.p, (int)b.kcmax, bs.qo.p, (int)k_stride, oi.get(), od.get(), oc.get());
   }
-  if (onp.get() && !any_probed) h2d(onp.get(), qnp_h.data(), nq);
   oi.commit(); od.commit(); oc.commit(); onp.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+// The index half of a refined batch (include/lance_b200.h): BatchSearch's merged lists, each query's k' of them, into
+// rows of kc_stride, and optionally the batch's distinct row ids with every slot's position among them.
+lb2_status lb2_index_search_candidates(lb2_index* index, const void* queries, uint64_t nq,
+                                       const lb2_query_params* params, const lb2_query_filter* filters,
+                                       uint32_t num_filters, uint32_t late_width, uint32_t kc_stride,
+                                       uint64_t* cand_ids_out, float* cand_dists_out, uint32_t* cand_counts_out,
+                                       uint32_t* nprobes_out, uint64_t* distinct_ids_out, uint64_t* num_distinct_out,
+                                       uint64_t* positions_out) {
+  LB2_API_BEGIN
+  const BatchPlan b(index, queries, nq, params, filters, num_filters, late_width, true);
+  LB2_REQUIRE(kc_stride >= b.kcmax, "kc_stride %u is below the largest k * max(1, refine_factor) %u", kc_stride,
+              b.kcmax);
+  LB2_REQUIRE(nq == 0 || (cand_ids_out && cand_dists_out && cand_counts_out), "null candidate outputs");
+  LB2_REQUIRE(!distinct_ids_out == !positions_out && !distinct_ids_out == !num_distinct_out,
+              "distinct_ids_out, num_distinct_out and positions_out go together");
+  if (current_comm() && current_comm()->nranks > 1)
+    fail(LB2_UNSUPPORTED, "a batch search on a row-sharded index is not implemented");
+  const size_t slots = (size_t)nq * kc_stride;
+  OutArg<uint64_t> om(num_distinct_out, 1);
+  if (nq == 0) {
+    if (om.get()) LB2_CUDA(cudaMemsetAsync(om.get(), 0, sizeof(uint64_t), ctx().stream));
+    om.commit();
+    sync_stream();
+    return LB2_OK;
+  }
+  OutArg<uint64_t> oi(cand_ids_out, slots);
+  OutArg<float> od(cand_dists_out, slots);
+  OutArg<uint32_t> oc(cand_counts_out, nq);
+  OutArg<uint32_t> onp(nprobes_out, nq);
+  OutArg<uint64_t> odi(distinct_ids_out, slots), opos(positions_out, slots);
+  BatchSearch bs(index, queries, nq, params, filters, num_filters, late_width, b, onp.get());
+  {
+    TagScope tg("search");
+    candidate_rows(bs.cid.p, bs.cdist.p, bs.ccnt.p, nq, (int)b.kcmax, bs.qo.p, (int)kc_stride, oi.get(), od.get(),
+                   oc.get());
+    if (odi.get()) distinct_ids(oi.get(), slots, odi.get(), om.get(), opos.get());
+  }
+  oi.commit(); od.commit(); oc.commit(); onp.commit(); odi.commit(); om.commit(); opos.commit();
+  sync_stream();
+  LB2_API_END
+}
+
+// taken rows in host memory up to this size cross to the device in one copy; a larger batch is staged in query slabs,
+// each slab's own taken rows gathered into a pinned buffer of this size
+static constexpr size_t kTakenStageBytes = (size_t)512 << 20;
+namespace {
+struct PinnedHostBuf {
+  void* p = nullptr;
+  explicit PinnedHostBuf(size_t bytes) { LB2_CUDA(cudaMallocHost(&p, bytes ? bytes : 1)); }
+  PinnedHostBuf(const PinnedHostBuf&) = delete;
+  PinnedHostBuf& operator=(const PinnedHostBuf&) = delete;
+  ~PinnedHostBuf() { cudaFreeHost(p); }
+};
+}  // namespace
+
+// The exact re-rank of the rows the caller took (include/lance_b200.h): refine_batch_f32 with the taken rows as its
+// row source, so it is lb2_index_search_batch's refine arithmetic with a row found by position instead of row id.
+lb2_status lb2_index_refine_taken(lb2_index* index, const void* queries, uint64_t nq, const lb2_query_params* params,
+                                  uint32_t kc_stride, const uint64_t* cand_ids, const float* cand_dists,
+                                  const uint32_t* cand_counts, const void* taken, uint64_t m, const uint64_t* positions,
+                                  uint32_t k_stride, uint64_t* row_ids_out, float* dists_out, uint32_t* counts_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index, "null index");
+  LB2_REQUIRE(nq == 0 || (queries && params && cand_ids && cand_dists && cand_counts), "null queries, params or candidates");
+  uint32_t kmax = 0;
+  bool any_refine = false;
+  std::vector<QueryOut> qo_h(nq);
+  for (uint64_t q = 0; q < nq; ++q) {
+    const lb2_query_params& p = params[q];
+    const unsigned long long qi = (unsigned long long)q;
+    LB2_REQUIRE(p.k > 0, "query %llu: k must be positive", qi);
+    const uint64_t kc = (uint64_t)p.k * std::max<uint32_t>(1, p.refine_factor);
+    if (kc > 1024)
+      fail(LB2_UNSUPPORTED, "query %llu: k * refine_factor = %llu > 1024 is not implemented", qi, (unsigned long long)kc);
+    LB2_REQUIRE(kc <= kc_stride, "query %llu: k * max(1, refine_factor) = %llu is above kc_stride %u", qi,
+                (unsigned long long)kc, kc_stride);
+    kmax = std::max(kmax, p.k);
+    any_refine |= p.refine_factor > 0;
+    qo_h[q] = QueryOut{(int)kc, (int)p.k, p.refine_factor > 0, (int)(p.has_lower_bound != 0),
+                       (int)(p.has_upper_bound != 0), p.lower_bound, p.upper_bound};
+  }
+  LB2_REQUIRE(k_stride >= kmax, "k_stride %u is below the largest k %u", k_stride, kmax);
+  LB2_REQUIRE(!any_refine || positions, "refine_factor > 0 needs positions");
+  LB2_REQUIRE(!any_refine || m == 0 || taken, "null taken rows");
+  if (nq == 0) {
+    sync_stream();
+    return LB2_OK;
+  }
+  const int d = index->d;
+  const size_t row_bytes = (size_t)d * dtype_size(index->dtype), slots = (size_t)nq * kc_stride;
+  VecIn q(queries, (size_t)nq * d, index->dtype);  // the original query, as the refine of a search takes it
+  DevBuf<QueryOut> qo(nq);
+  h2d(qo.p, qo_h.data(), nq);
+  InArg<uint64_t> ci(cand_ids, slots);
+  InArg<float> cd(cand_dists, slots);
+  InArg<uint32_t> cc(cand_counts, nq);
+  OutArg<uint64_t> oi(row_ids_out, (size_t)nq * k_stride);
+  OutArg<float> od(dists_out, (size_t)nq * k_stride);
+  OutArg<uint32_t> oc(counts_out, nq);
+  TagScope tg("search");
+  auto refine = [&](uint64_t q0, uint64_t n, const void* rows, uint64_t nrows, const uint64_t* pos) {
+    refine_batch_f32(q.get() + q0 * d, n, d, index->metric, rows, (int)index->dtype, nrows, cd.get() + q0 * kc_stride,
+                     ci.get() + q0 * kc_stride, cc.get() + q0, (int)kc_stride, qo.p + q0, (int)k_stride,
+                     oi.get() + q0 * k_stride, od.get() + q0 * k_stride, oc.get() ? oc.get() + q0 : nullptr, pos);
+  };
+  if (!any_refine) {
+    refine(0, nq, nullptr, 0, nullptr);
+  } else if (m * row_bytes <= kTakenStageBytes || is_device_ptr(taken)) {
+    InArg<uint8_t> t(taken, m * row_bytes);
+    InArg<uint64_t> pos(positions, slots);
+    refine(0, nq, t.get(), m, pos.get());
+  } else {
+    // query slabs: each slab's distinct positions (on the device, positions >= m left out so they still score NaN),
+    // its rows gathered on the host into the pinned buffer, its positions renumbered into that buffer
+    const size_t stage_rows = std::max<size_t>(kc_stride, kTakenStageBytes / row_bytes);
+    const uint64_t slab = std::max<uint64_t>(1, stage_rows / kc_stride);
+    InArg<uint64_t> pos(positions, slots);
+    PinnedHostBuf stage(stage_rows * row_bytes), sel((size_t)slab * kc_stride * sizeof(uint64_t));
+    DevBuf<uint8_t> rows(stage_rows * row_bytes);
+    DevBuf<uint64_t> ldist((size_t)slab * kc_stride), lpos((size_t)slab * kc_stride), lm(1);
+    const uint8_t* src = static_cast<const uint8_t*>(taken);
+    uint8_t* dst = static_cast<uint8_t*>(stage.p);
+    const uint64_t* local = static_cast<const uint64_t*>(sel.p);
+    for (uint64_t q0 = 0; q0 < nq; q0 += slab) {
+      const uint64_t n = std::min<uint64_t>(slab, nq - q0);
+      distinct_ids(pos.get() + q0 * kc_stride, n * kc_stride, ldist.p, lm.p, lpos.p, m);
+      uint64_t nl = 0;
+      d2h(&nl, lm.p, 1);
+      sync_stream();  // (also: the previous slab has read the staging buffer)
+      d2h(static_cast<uint64_t*>(sel.p), ldist.p, nl);
+      sync_stream();
+      for (uint64_t r = 0; r < nl; ++r) memcpy(dst + r * row_bytes, src + local[r] * row_bytes, row_bytes);
+      h2d(rows.p, dst, nl * row_bytes);
+      refine(q0, n, rows.p, nl, lpos.p);
+    }
+    sync_stream();  // before the pinned buffer is released
+  }
+  oi.commit(); od.commit(); oc.commit();
   sync_stream();
   LB2_API_END
 }

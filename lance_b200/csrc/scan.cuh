@@ -37,7 +37,18 @@ struct QueryOut {
 };
 void refine_batch_f32(const float* queries, uint64_t nq, int d, int metric, const void* vectors, int vdt,
                       uint64_t num_vectors, const float* cand_d, const uint64_t* cand_id, const uint32_t* cand_cnt,
-                      int kc, const QueryOut* qo, int k_stride, uint64_t* out_id, float* out_d, uint32_t* out_cnt);
+                      int kc, const QueryOut* qo, int k_stride, uint64_t* out_id, float* out_d, uint32_t* out_cnt,
+                      const uint64_t* positions = nullptr);
+// positions [nq][kc] (lb2_index_refine_taken): candidate c of query q is row positions[q][c] of the num_vectors rows
+// in `vectors`, not row cand_id[q][c]; the same kernel, only the row source differs
+void candidate_rows(const uint64_t* cid, const float* cdist, const uint32_t* ccnt, uint64_t nq, int kc,
+                    const QueryOut* qo, int stride, uint64_t* out_id, float* out_d, uint32_t* out_cnt);
+// ---- distinct.cu ----
+// the ascending distinct values of ids[0, n) below limit into distinct (capacity n; the rest UINT64_MAX), their
+// count m into *num_distinct (device), and positions[i] = the index of ids[i] in that list (UINT64_MAX for a value
+// at or above limit)
+void distinct_ids(const uint64_t* ids, uint64_t n, uint64_t* distinct, uint64_t* num_distinct, uint64_t* positions,
+                  uint64_t limit = ~0ull);
 void flat_topk_f32(const float* dists, const uint64_t* row_ids, uint64_t n, int k, const ScanFilter& flt,
                    uint64_t* out_id, float* out_d, uint32_t* out_cnt);
 // lb2_distance_batch with the reference's per-type rule: u8 L2 / dot (exact integer sums) and f16 / bf16 dot
