@@ -301,6 +301,29 @@ lb2_status lb2_flat_search(const void* vectors, uint64_t n, uint32_t d, lb2_dtyp
                            const uint64_t* row_ids /* NULL = 0..n; must be distinct */, const void* queries,
                            uint64_t nq, const lb2_flat_search_params* p, uint64_t* row_ids_out, float* dists_out,
                            uint32_t* counts_out);
+/* flat_knn for a batch of queries that differ in k, range and prefilter, as separate nearest() plans without an index
+ * (use_index(false), tables without an index, ground truth with per-query filters: scanner.rs:2912-2941) reach the
+ * column.  Row q of the outputs is bit for bit lb2_flat_search of query q alone with its own k, range and bitmap
+ * (filter_bitmaps[params[q].filter], or no bitmap for UINT32_MAX): ids, distance bits and counts.  Rows are
+ * [nq][k_stride]; slots k_q .. k_stride - 1 hold UINT64_MAX / +inf; counts_out is nullable.  Each bitmap ((n+63)/64
+ * words, host or device, a NULL entry admits every row) is staged once however many queries name it.  Every query's
+ * k and filter reach the scan kernel from a per-query table on the device, so the number of kernel launches depends
+ * on n, nq and the chunking of host rows, not on how many distinct (k, range, filter) sets the batch holds.
+ * Refused before anything is written: what lb2_flat_search refuses for any query (the message names the query), and
+ * with LB2_INVALID_ARG k_stride below the largest k, and a filter index that is neither below num_filters nor
+ * UINT32_MAX. */
+typedef struct {
+  uint32_t k;                          /* 1..1024 */
+  uint32_t filter;                     /* index into filter_bitmaps[], UINT32_MAX = no filter */
+  uint32_t has_lower_bound, has_upper_bound;
+  float lower_bound, upper_bound;
+} lb2_flat_query_params;
+lb2_status lb2_flat_search_batch(const void* vectors, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                                 const uint64_t* row_ids /* NULL = 0..n; must be distinct */, const void* queries,
+                                 uint64_t nq, const lb2_flat_query_params* params /* [nq] */,
+                                 const uint64_t* const* filter_bitmaps /* [num_filters] */, uint32_t num_filters,
+                                 uint32_t k_stride, uint64_t* row_ids_out /* [nq][k_stride] */, float* dists_out,
+                                 uint32_t* counts_out);
 
 /* IvfTransformer::transform for IVF_PQ (lance-index/src/vector/ivf.rs:188-236,357): for a batch,
  * [normalise if cosine] -> partition id -> residual -> PQ code, in one pass over the vectors.
@@ -514,6 +537,33 @@ lb2_status lb2_index_search_combined(lb2_index* index, const void* queries, uint
                                      const lb2_probe_params* pp /* nullable */, const lb2_unindexed_rows* u,
                                      uint64_t* row_ids_out, float* dists_out, uint32_t* counts_out,
                                      uint32_t* nprobes_out /* nullable; requires pp */);
+/* knn_combined for a mixed batch (scanner.rs:2946-3027): lb2_index_search_batch's per-query parameters over an index
+ * that does not cover every row, in one call.  Row q is what lb2_index_search_combined defines for query q alone:
+ *   1. the index half: lb2_index_search_batch's search of q (its probes, range, filter and ef) with refine factor
+ *      max(1, refine_factor_q) against refine_vectors;
+ *   2. the flat half: lb2_flat_search_batch over u's rows with the index metric, k_q and q's range on the original
+ *      (not normalised) query, admitting the rows of u->filter_bitmaps[filter_q] (u->rows.allow_bitmap for a query
+ *      without a filter);
+ *   3. the two lists merged by (distance, row id), first k_q.
+ * For a query without ef, row q and nprobes_out[q] equal lb2_index_search_combined of q alone bit for bit (with a
+ * fixed nprobes, or with the probe rule and the filter's max_len and mask_ids for nprobes 0).  A query with ef
+ * (IVF_HNSW_*) equals the merge of lb2_index_search_batch (ef, refine factor max(1, rf)) and lb2_flat_search.  The
+ * unindexed rows are read once for the whole batch.  Rows are [nq][k_stride], slots k_q.. UINT64_MAX / +inf;
+ * counts_out and nprobes_out are nullable.
+ * Refused before anything is written: what lb2_index_search_batch and lb2_flat_search_batch refuse, and with
+ * LB2_INVALID_ARG refine_vectors NULL, u or u->rows.row_ids NULL, u->rows.vectors NULL with n > 0, and
+ * u->filter_bitmaps NULL with num_filters > 0.  LB2_UNSUPPORTED: a thread whose communicator has more than one
+ * rank. */
+typedef struct {
+  lb2_unindexed_rows rows;                /* the unindexed rows; rows.allow_bitmap serves queries without a filter */
+  const uint64_t* const* filter_bitmaps;  /* [num_filters]: validity AND filter f over these rows; NULL entry = all */
+} lb2_unindexed_batch;
+lb2_status lb2_index_search_combined_batch(lb2_index* index, const void* queries, uint64_t nq,
+                                           const lb2_query_params* params /* [nq] */, const lb2_query_filter* filters,
+                                           uint32_t num_filters, const void* refine_vectors, uint64_t num_vectors,
+                                           uint32_t late_width, const lb2_unindexed_batch* u, uint32_t k_stride,
+                                           uint64_t* row_ids_out /* [nq][k_stride] */, float* dists_out,
+                                           uint32_t* counts_out, uint32_t* nprobes_out);
 /* Incremental update of an IVF_PQ index (SURVEY 8f-4).
  * The reference expresses an optimize step as per-partition AssignOp::Add / AssignOp::Remove lists against a new
  * centroid set (rust/lance/src/index/vector/builder.rs:1219-1333 split_partition_impl, :1476-1530

@@ -21,7 +21,7 @@ from ._lib import (BF16, COSINE, DOT, F16, F32, L2, METRICS, U8, BuildParams, Bu
 __all__ = ["device_count", "DeviceArray", "PinnedArray", "LanceB200Error", "train_kmeans",
            "compute_partitions", "kmeans_find_partitions", "compute_residual", "normalize_fsl",
            "l2_distance_batch", "dot_distance_batch", "cosine_distance_batch", "PQBuildParams", "ProductQuantizer",
-           "build_distance_table_l2", "compute_pq_distance", "flat_topk", "flat_search", "IvfPqIndex",
+           "build_distance_table_l2", "compute_pq_distance", "flat_topk", "flat_search", "flat_search_batch", "IvfPqIndex",
            "IvfBuildParams", "IvfFlatIndex", "SQBuildParams", "ScalarQuantizer", "IvfSqIndex", "HnswBuildParams",
            "IvfHnswSqIndex", "IvfHnswPqIndex", "IvfHnswFlatIndex", "RQBuildParams",
            "RabitQuantizer", "IvfRqIndex", "PartitionIndex", "launch_count", "profile"]
@@ -510,6 +510,86 @@ def flat_search(vectors, queries, k, distance_type="l2", row_ids=None, allow_bit
                          int(upper_bound is not None), float(lower_bound or 0.0), float(upper_bound or 0.0))
     check(lib().lb2_flat_search(vp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt), C.c_int(_metric(distance_type)), rp,
                                 qp, C.c_uint64(nq), C.byref(p), as_ptr(ids)[0], as_ptr(dists)[0], as_ptr(counts)[0]))
+    return ids, dists, counts
+
+
+def _per_query(name, what, v, nq, dtype, default):
+    """a per-query argument: a scalar broadcast to [nq], or an [nq] array"""
+    a = np.asarray(default if v is None else v, dtype=dtype)
+    if a.ndim == 0:
+        return np.full(nq, a, dtype)
+    if a.shape != (nq,):
+        raise ValueError(f"{name}: {what} must be a scalar or an array of {nq} values, got shape {a.shape}")
+    return a
+
+
+def _out_rows(name, out, nq, kmax):
+    """(ids, dists, k_stride): `out`'s arrays, or new [nq][kmax] ones"""
+    if out is None:
+        ids, dists = np.empty((nq, kmax), np.uint64), np.empty((nq, kmax), np.float32)
+    else:
+        ids, dists = out
+    k_stride = int(ids.shape[1]) if len(ids.shape) == 2 else kmax
+    if tuple(ids.shape) != (nq, k_stride) or tuple(dists.shape) != (nq, k_stride) or k_stride < kmax:
+        raise ValueError(f"{name}: out arrays must be [{nq}][>= {kmax}], got {ids.shape} and {dists.shape}")
+    return ids, dists, k_stride
+
+
+def _bitmap_table(bitmaps, keep):
+    """a C array of bitmap pointers (NULL for a None entry), with what it points at appended to keep"""
+    table = (C.c_void_p * max(1, len(bitmaps)))()
+    for i, b in enumerate(bitmaps):
+        bp, kb = as_ptr(_bitmap(b))
+        if bp is not None and bp.value is None:  # an empty numpy array has no buffer address to pass
+            kb = np.zeros(1, np.uint64)
+            bp = C.c_void_p(kb.ctypes.data)
+        keep += [b, kb]
+        table[i] = bp.value if bp is not None else None
+    return table
+
+
+def flat_search_batch(vectors, queries, k, distance_type="l2", row_ids=None, filters=None, filter_of=None,
+                      lower_bound=None, upper_bound=None, out=None, bf16=False):
+    """lb2_flat_search_batch: flat_search where every query has its own k, range and filter, in one call.  Row q
+    equals flat_search of query q alone with k[q], filters[filter_of[q]] as its allow bitmap (-1 = none) and its
+    bounds (NaN or None = no bound).  Every per-query argument is a scalar or an [nq] array; `filters` is a list of
+    allow bitmaps over the n rows ((n + 63) // 64 uint64 words; None admits every row).  Returns (ids, dists,
+    counts): ids / dists [nq][max k] (or `out`'s arrays and their row length); unused slots hold (2**64 - 1, +inf)."""
+    from ._lib import FlatQueryParams
+    vectors, dt = _typed(vectors, bf16)
+    if not isinstance(queries, (DeviceArray, PinnedArray)):
+        queries = np.ascontiguousarray(queries, dtype=vectors.dtype)
+    n, d = vectors.shape
+    nq = int(queries.shape[0])
+    name = "flat_search_batch"
+    ks = _per_query(name, "k", k, nq, np.int64, 0)
+    if nq and (ks < 1).any():
+        raise ValueError(f"{name}: every k must be at least 1")
+    filters = list(filters or [])
+    fof = _per_query(name, "filter_of", filter_of, nq, np.int64, -1)
+    if ((fof < -1) | (fof >= len(filters))).any():
+        raise ValueError(f"{name}: filter_of must be -1 or below the {len(filters)} filters")
+    lows = _per_query(name, "lower_bound", lower_bound, nq, np.float32, np.nan)
+    ups = _per_query(name, "upper_bound", upper_bound, nq, np.float32, np.nan)
+    ids, dists, k_stride = _out_rows(name, out, nq, int(ks.max()) if nq else 1)
+    cp = np.zeros(max(1, nq), np.dtype({"names": [f for f, _ in FlatQueryParams._fields_],
+                                        "formats": [np.float32 if t is C.c_float else np.uint32
+                                                    for _, t in FlatQueryParams._fields_]}))
+    assert cp.dtype.itemsize == C.sizeof(FlatQueryParams)
+    cp["k"][:nq] = ks
+    cp["filter"][:nq] = np.where(fof < 0, 0xFFFFFFFF, fof)
+    cp["has_lower_bound"][:nq], cp["has_upper_bound"][:nq] = ~np.isnan(lows), ~np.isnan(ups)
+    cp["lower_bound"][:nq], cp["upper_bound"][:nq] = np.nan_to_num(lows, nan=0.0), np.nan_to_num(ups, nan=0.0)
+    keep = []
+    table = _bitmap_table(filters, keep)
+    counts = np.empty(nq, np.uint32)
+    vp, _k0 = as_ptr(vectors)
+    qp, _k1 = as_ptr(queries)
+    rp, _k2 = as_ptr(_row_ids(row_ids))
+    check(lib().lb2_flat_search_batch(vp, C.c_uint64(n), C.c_uint32(d), C.c_int(dt), C.c_int(_metric(distance_type)),
+                                      rp, qp, C.c_uint64(nq), C.c_void_p(cp.ctypes.data), table,
+                                      C.c_uint32(len(filters)), C.c_uint32(k_stride), as_ptr(ids)[0],
+                                      as_ptr(dists)[0], as_ptr(counts)[0]))
     return ids, dists, counts
 
 
@@ -1020,6 +1100,54 @@ class IvfPqIndex:
                                               C.byref(pp) if pp is not None else None, C.byref(u), as_ptr(ids)[0],
                                               as_ptr(dists)[0], as_ptr(counts)[0], as_ptr(nprobes_out)[0]))
         return ids, dists, counts, nprobes_out
+
+    def search_combined_batch(self, queries, k, vectors, unindexed_vectors, unindexed_row_ids, nprobes=None,
+                              minimum_nprobes=None, maximum_nprobes=None, refine_factor=0, filters=None,
+                              filter_of=None, unindexed_allow_bitmap=None, unindexed_filters=None, lower_bound=None,
+                              upper_bound=None, ef=None, late_width=1, out=None):
+        """lb2_index_search_combined_batch: knn_combined (search_combined) for a batch whose queries differ in their
+        parameters, in one call.  Takes search_batch's per-query arguments; `vectors` is the indexed column (row id =
+        row number) and the index half runs with refine factor max(1, refine_factor).  The unindexed rows
+        (`unindexed_vectors` with their `unindexed_row_ids`) are searched flat: a query without a filter admits the
+        rows of `unindexed_allow_bitmap` (None: all), a query with filter f those of unindexed_filters[f] (one bitmap
+        per filter, validity AND the filter over the unindexed rows; None admits every row).  Row q equals
+        search_combined of query q alone.  Returns (ids, dists, counts, nprobes): ids / dists [nq][max k] (or
+        `out`'s arrays and their row length)."""
+        from ._lib import UnindexedBatch, UnindexedRows
+        name = "search_combined_batch"
+        if vectors is None:
+            raise ValueError(f"{name}: the index's rows are re-scored exactly: vectors is required")
+        if not isinstance(vectors, (DeviceArray, PinnedArray)):
+            vectors = np.ascontiguousarray(vectors, dtype=self._npdt())
+        if not isinstance(unindexed_vectors, (DeviceArray, PinnedArray)):
+            unindexed_vectors = np.ascontiguousarray(unindexed_vectors, dtype=self._npdt())
+        queries, nq, ks, _rfs, cp, cf, nf, keep = self._batch_params(
+            name, queries, k, nprobes, minimum_nprobes, maximum_nprobes, refine_factor, filters, filter_of,
+            lower_bound, upper_bound, ef)
+        ufilters = list(unindexed_filters) if unindexed_filters is not None else ([] if nf == 0 else None)
+        if ufilters is None or len(ufilters) != nf:
+            raise ValueError(f"{name}: unindexed_filters must hold one bitmap (or None) for each of the {nf} filters")
+        if unindexed_row_ids is None:
+            raise ValueError(f"{name}: unindexed_row_ids is required")
+        ids, dists, k_stride = _out_rows(name, out, nq, int(ks.max()) if nq else 1)
+        counts, probes = np.empty(nq, np.uint32), np.empty(nq, np.uint32)
+        table = _bitmap_table(ufilters, keep)
+        urp, _k4 = as_ptr(_row_ids(unindexed_row_ids))
+        if urp.value is None:  # no unindexed rows: any valid address stands for the empty list
+            _k4 = np.zeros(1, np.uint64)
+            urp = C.c_void_p(_k4.ctypes.data)
+        uvp, _k3 = as_ptr(unindexed_vectors)
+        ubp, _k5 = as_ptr(_bitmap(unindexed_allow_bitmap))
+        u = UnindexedBatch(UnindexedRows(uvp.value, unindexed_vectors.shape[0], urp.value,
+                                         ubp.value if ubp is not None else None), C.cast(table, C.c_void_p))
+        qp, _k1 = as_ptr(queries)
+        vp, _k0 = as_ptr(vectors)
+        check(lib().lb2_index_search_combined_batch(self._h, qp, C.c_uint64(nq), C.c_void_p(cp.ctypes.data), cf,
+                                                    C.c_uint32(nf), vp, C.c_uint64(vectors.shape[0]),
+                                                    C.c_uint32(late_width), C.byref(u), C.c_uint32(k_stride),
+                                                    as_ptr(ids)[0], as_ptr(dists)[0], as_ptr(counts)[0],
+                                                    as_ptr(probes)[0]))
+        return ids, dists, counts, probes
 
     def search_async(self, queries, out, k=10, nprobes=1, cuda_stream=None, done_event=None, allow_bitmap=None,
                      lower_bound=None, upper_bound=None):

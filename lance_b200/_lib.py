@@ -149,7 +149,7 @@ EXPORTS = [
     "lb2_partition_index_uses_graph", "lb2_partition_index_build", "lb2_partition_index_assign",
     "lb2_partition_index_info", "lb2_partition_index_export", "lb2_partition_index_destroy",
     "lb2_index_set_partition_index", "lb2_index_search_batch", "lb2_index_search_candidates",
-    "lb2_index_refine_taken",
+    "lb2_index_refine_taken", "lb2_flat_search_batch", "lb2_index_search_combined_batch",
 ]
 
 _lib = None
@@ -187,6 +187,12 @@ def lib():
         L.lb2_index_refine_taken.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32, C.c_void_p,
                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint32,
                                              C.c_void_p, C.c_void_p, C.c_void_p]
+        L.lb2_flat_search_batch.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_int, C.c_int, C.c_void_p,
+                                            C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32,
+                                            C.c_void_p, C.c_void_p, C.c_void_p]
+        L.lb2_index_search_combined_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                                      C.c_uint32, C.c_void_p, C.c_uint64, C.c_uint32, C.c_void_p,
+                                                      C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         _lib = L
     return _lib
 
@@ -240,6 +246,17 @@ class FlatSearchParams(C.Structure):
 class UnindexedRows(C.Structure):
     """lb2_unindexed_rows (include/lance_b200.h)."""
     _fields_ = [("vectors", C.c_void_p), ("n", C.c_uint64), ("row_ids", C.c_void_p), ("allow_bitmap", C.c_void_p)]
+
+
+class FlatQueryParams(C.Structure):
+    """lb2_flat_query_params (include/lance_b200.h)."""
+    _fields_ = [("k", C.c_uint32), ("filter", C.c_uint32), ("has_lower_bound", C.c_uint32),
+                ("has_upper_bound", C.c_uint32), ("lower_bound", C.c_float), ("upper_bound", C.c_float)]
+
+
+class UnindexedBatch(C.Structure):
+    """lb2_unindexed_batch (include/lance_b200.h)."""
+    _fields_ = [("rows", UnindexedRows), ("filter_bitmaps", C.c_void_p)]
 
 
 class DeviceArray:

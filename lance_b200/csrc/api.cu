@@ -543,6 +543,53 @@ lb2_status lb2_flat_search(const void* vectors, uint64_t n, uint32_t d, lb2_dtyp
   LB2_API_END
 }
 
+// Every query is checked first, so a refusal writes nothing; each bitmap is staged once.
+lb2_status lb2_flat_search_batch(const void* vectors, uint64_t n, uint32_t d, lb2_dtype dtype, lb2_metric metric,
+                                 const uint64_t* row_ids, const void* queries, uint64_t nq,
+                                 const lb2_flat_query_params* params, const uint64_t* const* filter_bitmaps,
+                                 uint32_t num_filters, uint32_t k_stride, uint64_t* row_ids_out, float* dists_out,
+                                 uint32_t* counts_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(d > 0, "dimension must be positive");
+  LB2_REQUIRE(dtype >= LB2_F32 && dtype <= LB2_U8, "unknown element type %d", (int)dtype);
+  LB2_REQUIRE((n == 0 || vectors) && (nq == 0 || (queries && params && row_ids_out && dists_out)), "null argument");
+  LB2_REQUIRE(num_filters == 0 || filter_bitmaps, "null filter_bitmaps");
+  const int m = metric_of(metric);
+  uint32_t kmax = 0;
+  for (uint64_t q = 0; q < nq; ++q) {
+    const lb2_flat_query_params& p = params[q];
+    const unsigned long long qi = (unsigned long long)q;
+    LB2_REQUIRE(p.k > 0, "query %llu: k must be positive", qi);
+    if (p.k > 1024) fail(LB2_UNSUPPORTED, "query %llu: k = %u > 1024 is not implemented", qi, p.k);
+    LB2_REQUIRE(p.filter < num_filters || p.filter == UINT32_MAX, "query %llu: filter %u is not below num_filters %u",
+                qi, p.filter, num_filters);
+    kmax = std::max(kmax, p.k);
+  }
+  LB2_REQUIRE(k_stride >= kmax, "k_stride %u is below the largest k %u", k_stride, kmax);
+  flat_search_batch_check((int)d, dtype, m, (int)std::max<uint32_t>(kmax, 1));
+  if (nq == 0) {
+    sync_stream();
+    return LB2_OK;
+  }
+  VecIn q(queries, (size_t)nq * d, dtype);
+  InArg<uint64_t> rid(row_ids, n);
+  std::vector<InArg<uint64_t>> bm(num_filters);
+  std::vector<const uint64_t*> bm_dev(num_filters);
+  for (uint32_t f = 0; f < num_filters; ++f) {
+    bm[f].set(filter_bitmaps[f], filter_bitmaps[f] ? (size_t)((n + 63) / 64) : 0);
+    bm_dev[f] = bm[f].get();
+  }
+  const std::vector<FlatQuery> fq = flat_queries(params, nq, bm_dev, nullptr);
+  OutArg<uint64_t> oi(row_ids_out, (size_t)nq * k_stride);
+  OutArg<float> od(dists_out, (size_t)nq * k_stride);
+  OutArg<uint32_t> oc(counts_out, nq);
+  flat_search_batch(q.get(), nq, (int)d, m, vectors, n, dtype, rid.get(), fq.data(), (int)k_stride, oi.get(), od.get(),
+                    oc.get());
+  oi.commit(); od.commit(); oc.commit();
+  sync_stream();
+  LB2_API_END
+}
+
 lb2_status lb2_comm_info(int* rank, int* nranks) {
   LB2_API_BEGIN
   Comm* c = current_comm();

@@ -2,7 +2,7 @@
 // pair by the refine plan's per-element-type rule (row_distance.cuh), the rows a bitmap and a [lower, upper) range
 // admit, and the k smallest (distance, row id) pairs of every query.
 //
-// Replaces  flat_knn                             rust/lance/src/dataset/scanner.rs:3336-3411
+// Replaces  flat_knn                             rust/lance/src/dataset/scanner.rs:3336-3411, 2912-2941
 //           compute_distance                     lance-index/src/vector/flat.rs:94-150
 //           SortExec(_distance, _rowid).fetch(k) scanner.rs:3450-3466
 //
@@ -15,14 +15,21 @@
 // (merge-path ranks: position in its own run + count of the other run before it), the list living in the output
 // candidate array.  The per-query top-k by (distance, row id) is contained in the union of the CTAs' lists, which
 // merge_list_tree (ivf_search.cu) merges per query.
+//
+// flat_search_batch runs the same scan for queries that differ in k, range and bitmap: the batch kernel loads its
+// tile's entries of a per-query table into shared memory, and each folded (query, row) pair reads its own query's
+// bitmap bit, bounds and k-th threshold; a query's list is cut at its own k.  The launches are those of a uniform
+// batch of the largest k.
 #include <algorithm>
 #include <memory>
+#include <vector>
 
 #include "common.cuh"
 #include "exact.cuh"
 #include "flat_search.cuh"
 #include "ivf_search.cuh"
 #include "row_distance.cuh"
+#include "scan.cuh"
 #include "staging.cuh"
 #include "topk.cuh"
 
@@ -120,11 +127,14 @@ __device__ __forceinline__ void fs_merge(int k, float* wd, uint64_t* wi, const i
 
 // grid (query tiles, row ranges of rows_per_cta rows); rows [0, n) of this launch are rows [r0, r0 + n) of the column.
 // The list of query q and row range y is list list0 + y of the nl lists per query of cand_* ([nq][nl][k]).
-template <int METRIC, class T>
-__global__ void __launch_bounds__(256)
-flat_search_scan_kernel(const float* __restrict__ queries, uint64_t nq, int d, const T* __restrict__ rows, uint64_t n,
-                        uint64_t r0, uint64_t rows_per_cta, const uint64_t* __restrict__ row_ids, const FlatFilter flt,
-                        int k, int nl, int list0, float* cand_d, uint64_t* cand_id, uint32_t* __restrict__ cand_cnt) {
+// BATCH: every query's own k (<= k, the lists' stride) and filter from s_fq, the tile's entries of the FlatQuery table
+// (flat_search_batch_scan_kernel); the single-parameter kernel is compiled without them.
+template <int METRIC, class T, bool BATCH>
+__device__ __forceinline__ void fs_scan(const float* __restrict__ queries, uint64_t nq, int d, const T* __restrict__ rows,
+                                        uint64_t n, uint64_t r0, uint64_t rows_per_cta,
+                                        const uint64_t* __restrict__ row_ids, const FlatFilter flt, int k, int nl,
+                                        int list0, float* cand_d, uint64_t* cand_id, uint32_t* __restrict__ cand_cnt,
+                                        const FlatQuery* s_fq) {
   constexpr int RULE = refine_rule<METRIC, T>();
   extern __shared__ __align__(16) unsigned char fs_smem[];
   const int qstride = fs_qstride(d);
@@ -197,44 +207,78 @@ flat_search_scan_kernel(const float* __restrict__ queries, uint64_t nq, int d, c
                                                    METRIC == METRIC_COSINE ? s_qnorm[fq] : 0.0f);
     const uint64_t r = r0 + t0 + fr;  // the row's position in the column
     // LanceFilterExec(_distance >= lower AND _distance < upper) and the caller's bitmap (scanner.rs:3342-3377)
-    if (fq < nqt && fr < nr && row_allowed(flt.allow, r) && (!flt.has_lower || dist >= flt.lower) &&
-        (!flt.has_upper || dist < flt.upper)) {
-      const int32_t key = total_order_key(dist);
-      const uint64_t id = row_ids ? row_ids[r] : r;
-      if (s_wcnt[fq] < (uint32_t)k || ki_less(key, id, s_wkey[fq], s_wid[fq])) {
-        const uint32_t at = atomicAdd(&s_pcnt[fq], 1u);
-        pkey[fq * FS_P + at] = key;
-        pid[fq * FS_P + at] = id;
+    auto offer = [&](const FlatFilter& f, int kq) {
+      if (fq < nqt && fr < nr && row_allowed(f.allow, r) && (!f.has_lower || dist >= f.lower) &&
+          (!f.has_upper || dist < f.upper)) {
+        const int32_t key = total_order_key(dist);
+        const uint64_t id = row_ids ? row_ids[r] : r;
+        if (s_wcnt[fq] < (uint32_t)kq || ki_less(key, id, s_wkey[fq], s_wid[fq])) {
+          const uint32_t at = atomicAdd(&s_pcnt[fq], 1u);
+          pkey[fq * FS_P + at] = key;
+          pid[fq * FS_P + at] = id;
+        }
       }
-    }
+    };
+    if constexpr (BATCH) offer(s_fq[fq].flt, s_fq[fq].k);
+    else offer(flt, k);
     __syncthreads();
     for (int qi = 0; qi < nqt; ++qi)  // a buffer that might not take the next tile's rows is merged
       if (s_pcnt[qi] > FS_P - FS_R)
-        fs_merge(k, list_d(qi), list_id(qi), pkey + qi * FS_P, pid + qi * FS_P, s_pcnt, s_wcnt, s_wkey, s_wid, qi);
+        fs_merge(BATCH ? s_fq[qi].k : k, list_d(qi), list_id(qi), pkey + qi * FS_P, pid + qi * FS_P, s_pcnt, s_wcnt,
+                 s_wkey, s_wid, qi);
   }
   for (int qi = 0; qi < nqt; ++qi)
     if (s_pcnt[qi] > 0)
-      fs_merge(k, list_d(qi), list_id(qi), pkey + qi * FS_P, pid + qi * FS_P, s_pcnt, s_wcnt, s_wkey, s_wid, qi);
+      fs_merge(BATCH ? s_fq[qi].k : k, list_d(qi), list_id(qi), pkey + qi * FS_P, pid + qi * FS_P, s_pcnt, s_wcnt,
+               s_wkey, s_wid, qi);
   if (tid < nqt) cand_cnt[(q0 + tid) * nl + list] = s_wcnt[tid];
 }
 
-template <class F>
+template <int METRIC, class T>
+__global__ void __launch_bounds__(256)
+flat_search_scan_kernel(const float* __restrict__ queries, uint64_t nq, int d, const T* __restrict__ rows, uint64_t n,
+                        uint64_t r0, uint64_t rows_per_cta, const uint64_t* __restrict__ row_ids, const FlatFilter flt,
+                        int k, int nl, int list0, float* cand_d, uint64_t* cand_id, uint32_t* __restrict__ cand_cnt) {
+  fs_scan<METRIC, T, false>(queries, nq, d, rows, n, r0, rows_per_cta, row_ids, flt, k, nl, list0, cand_d, cand_id,
+                            cand_cnt, nullptr);
+}
+
+// the batch version: query q's k and filter are fq[q] (flat_search_batch); k is the lists' stride, the largest k
+template <int METRIC, class T>
+__global__ void __launch_bounds__(256)
+flat_search_batch_scan_kernel(const float* __restrict__ queries, uint64_t nq, int d, const T* __restrict__ rows,
+                              uint64_t n, uint64_t r0, uint64_t rows_per_cta, const uint64_t* __restrict__ row_ids,
+                              const FlatQuery* __restrict__ fq, int k, int nl, int list0, float* cand_d,
+                              uint64_t* cand_id, uint32_t* __restrict__ cand_cnt) {
+  __shared__ FlatQuery s_fq[FS_Q];
+  const uint64_t q0 = (uint64_t)blockIdx.x * FS_Q;
+  if (threadIdx.x < FS_Q) s_fq[threadIdx.x] = q0 + threadIdx.x < nq ? fq[q0 + threadIdx.x] : FlatQuery{};
+  // (fs_scan's first barrier orders these writes before any read)
+  fs_scan<METRIC, T, true>(queries, nq, d, rows, n, r0, rows_per_cta, row_ids, FlatFilter{}, k, nl, list0, cand_d,
+                           cand_id, cand_cnt, s_fq);
+}
+
+template <bool BATCH, class F>
 static void with_scan_kernel(int metric, lb2_dtype dt, F&& f) {
   dispatch_metric_elem<true>(metric, (int)dt, [&](auto m, auto e) {
     using T = typename decltype(e)::type;
-    f(flat_search_scan_kernel<decltype(m)::value, T>, T{});
+    if constexpr (BATCH) f(flat_search_batch_scan_kernel<decltype(m)::value, T>, T{});
+    else f(flat_search_scan_kernel<decltype(m)::value, T>, T{});
   });
 }
 
-void flat_search_check(int d, lb2_dtype dt, int metric, int k) {
+template <bool BATCH>
+static void scan_check(int d, lb2_dtype dt, int metric, int k) {
   if (k > 1024) fail(LB2_UNSUPPORTED, "k = %d > 1024 is not implemented", k);
   const size_t dyn = fs_smem_bytes(d, dtype_size(dt));
   size_t need = 0;
-  with_scan_kernel(metric, dt, [&](auto kern, auto) { need = smem_with_static(kern, dyn); });
+  with_scan_kernel<BATCH>(metric, dt, [&](auto kern, auto) { need = smem_with_static(kern, dyn); });
   if (need > ctx().smem_optin)
     fail(LB2_UNSUPPORTED, "dimension %d: the flat search's tile of %d queries and %d rows needs %zu bytes of shared "
          "memory, the device has %zu", d, FS_Q, FS_R, need, ctx().smem_optin);
 }
+void flat_search_check(int d, lb2_dtype dt, int metric, int k) { scan_check<false>(d, dt, metric, k); }
+void flat_search_batch_check(int d, lb2_dtype dt, int metric, int kmax) { scan_check<true>(d, dt, metric, kmax); }
 
 // row ranges per launch over `rows` rows for nqt query tiles: enough CTAs for four per SM, each at least FS_MIN_ROWS
 static int fs_ranges(uint64_t rows, uint64_t nqt) {
@@ -242,12 +286,13 @@ static int fs_ranges(uint64_t rows, uint64_t nqt) {
   return (int)std::max<uint64_t>(1, std::min<uint64_t>(want, rows / FS_MIN_ROWS));
 }
 
-void flat_search(const float* queries, uint64_t nq, int d, int metric, const void* vectors, uint64_t n, lb2_dtype dt,
-                 const uint64_t* row_ids, const FlatFilter& flt, int k, uint64_t* out_ids, float* out_dists,
-                 uint32_t* out_counts) {
-  flat_search_check(d, dt, metric, k);
-  if (nq == 0) return;
-  TagScope tg("flat_search");
+// The scan of both entry points: query slabs whose candidate lists (stride k) hold at most about 256 MB, a launch per
+// staged chunk of host rows (one for device rows), and each slab's lists merged by merge_list_tree into [qn][k] at
+// out_ids + s0 * k (merged(s0, qn) runs after each slab's merge).  fq (device, BATCH only): the per-query table.
+template <bool BATCH, class Merged>
+static void fs_run(const float* queries, uint64_t nq, int d, int metric, const void* vectors, uint64_t n, lb2_dtype dt,
+                   const uint64_t* row_ids, const FlatFilter& flt, const FlatQuery* fq, int k, uint64_t* out_ids,
+                   float* out_dists, uint32_t* out_counts, Merged&& merged) {
   const size_t dyn = fs_smem_bytes(d, dtype_size(dt));
   std::unique_ptr<Source> src;
   const void* nat = nullptr;
@@ -277,11 +322,15 @@ void flat_search(const float* queries, uint64_t nq, int d, int metric, const voi
     auto scan = [&](const void* rows, uint64_t r0, uint64_t cnt) {
       const int nr = fs_ranges(cnt, nqt);
       const uint64_t per = (cdiv(cnt, nr) + FS_R - 1) / FS_R * FS_R;
-      with_scan_kernel(metric, dt, [&](auto kern, auto t) {
+      with_scan_kernel<BATCH>(metric, dt, [&](auto kern, auto t) {
         using T = decltype(t);
         set_smem(kern, dyn);
-        LB2_LAUNCH("scan", kern, dim3((unsigned)nqt, (unsigned)nr), 256, dyn, queries + s0 * d, qn, d,
-                   static_cast<const T*>(rows), cnt, r0, per, row_ids, flt, k, nl, list0, cd.p, cid.p, ccnt.p);
+        if constexpr (BATCH)
+          LB2_LAUNCH("scan", kern, dim3((unsigned)nqt, (unsigned)nr), 256, dyn, queries + s0 * d, qn, d,
+                     static_cast<const T*>(rows), cnt, r0, per, row_ids, fq + s0, k, nl, list0, cd.p, cid.p, ccnt.p);
+        else
+          LB2_LAUNCH("scan", kern, dim3((unsigned)nqt, (unsigned)nr), 256, dyn, queries + s0 * d, qn, d,
+                     static_cast<const T*>(rows), cnt, r0, per, row_ids, flt, k, nl, list0, cd.p, cid.p, ccnt.p);
       });
       list0 += nr;
     };
@@ -291,7 +340,48 @@ void flat_search(const float* queries, uint64_t nq, int d, int metric, const voi
     });
     merge_list_tree("merge", qn, cd.p, cid.p, ccnt.p, nl, k, out_ids + s0 * k, out_dists + s0 * k,
                     out_counts ? out_counts + s0 : nullptr);
+    merged(s0, qn);
   }
+}
+
+void flat_search(const float* queries, uint64_t nq, int d, int metric, const void* vectors, uint64_t n, lb2_dtype dt,
+                 const uint64_t* row_ids, const FlatFilter& flt, int k, uint64_t* out_ids, float* out_dists,
+                 uint32_t* out_counts) {
+  flat_search_check(d, dt, metric, k);
+  if (nq == 0) return;
+  TagScope tg("flat_search");
+  fs_run<false>(queries, nq, d, metric, vectors, n, dt, row_ids, flt, nullptr, k, out_ids, out_dists, out_counts,
+                [](uint64_t, uint64_t) {});
+}
+
+// Each slab's lists are merged to the slab's largest k (every list holds at most its own query's k, so the first k_q
+// of query q's merged row are its top k_q), then cut to k_q into rows of k_stride by candidate_rows.
+void flat_search_batch(const float* queries, uint64_t nq, int d, int metric, const void* vectors, uint64_t n,
+                       lb2_dtype dt, const uint64_t* row_ids, const FlatQuery* fq_host, int k_stride,
+                       uint64_t* out_ids, float* out_dists, uint32_t* out_counts) {
+  int kmax = 1;
+  for (uint64_t q = 0; q < nq; ++q) kmax = std::max(kmax, fq_host[q].k);
+  flat_search_batch_check(d, dt, metric, kmax);
+  if (nq == 0) return;
+  TagScope tg("flat_search");
+  DevBuf<FlatQuery> fq(nq);
+  h2d(fq.p, fq_host, nq);
+  std::vector<QueryOut> qo_h(nq);
+  for (uint64_t q = 0; q < nq; ++q) qo_h[q] = QueryOut{fq_host[q].k, fq_host[q].k, 0, 0, 0, 0.0f, 0.0f};
+  DevBuf<QueryOut> qo(nq);
+  h2d(qo.p, qo_h.data(), nq);
+  DevBuf<uint64_t> mi(nq * kmax);
+  DevBuf<float> md(nq * kmax);
+  DevBuf<uint32_t> mc(nq), oc;
+  if (!out_counts) {
+    oc.alloc(nq);
+    out_counts = oc.p;
+  }
+  fs_run<true>(queries, nq, d, metric, vectors, n, dt, row_ids, FlatFilter{}, fq.p, kmax, mi.p, md.p, mc.p,
+               [&](uint64_t s0, uint64_t qn) {
+                 candidate_rows(mi.p + s0 * kmax, md.p + s0 * kmax, mc.p + s0, qn, kmax, qo.p + s0, k_stride,
+                                out_ids + s0 * k_stride, out_dists + s0 * k_stride, out_counts + s0);
+               });
 }
 
 }  // namespace lb2

@@ -1431,6 +1431,79 @@ lb2_status lb2_index_search_combined(lb2_index* index, const void* queries, uint
   LB2_API_END
 }
 
+// knn_combined for a mixed batch (include/lance_b200.h): BatchSearch and refine_batch_f32 with every refine factor
+// raised to max(1, rf), flat_search_batch over the unindexed rows, and merge_lists with each query's own k.  Both
+// halves are rows of k_stride, so the merge writes the output rows directly.
+lb2_status lb2_index_search_combined_batch(lb2_index* index, const void* queries, uint64_t nq,
+                                           const lb2_query_params* params, const lb2_query_filter* filters,
+                                           uint32_t num_filters, const void* refine_vectors, uint64_t num_vectors,
+                                           uint32_t late_width, const lb2_unindexed_batch* u, uint32_t k_stride,
+                                           uint64_t* row_ids_out, float* dists_out, uint32_t* counts_out,
+                                           uint32_t* nprobes_out) {
+  LB2_API_BEGIN
+  LB2_REQUIRE(index, "null index");
+  LB2_REQUIRE(nq == 0 || params, "null queries or params");
+  LB2_REQUIRE(refine_vectors, "the combined search re-scores the index's rows exactly: refine_vectors is required");
+  std::vector<lb2_query_params> ip(params, params + nq);
+  for (lb2_query_params& p : ip) p.refine_factor = std::max<uint32_t>(1, p.refine_factor);
+  const BatchPlan b(index, queries, nq, ip.data(), filters, num_filters, late_width, true);
+  LB2_REQUIRE(k_stride >= b.kmax, "k_stride %u is below the largest k %u", k_stride, b.kmax);
+  LB2_REQUIRE(u && u->rows.row_ids, "the unindexed rows and their row ids are required");
+  LB2_REQUIRE(u->rows.n == 0 || u->rows.vectors, "null unindexed vectors");
+  LB2_REQUIRE(num_filters == 0 || u->filter_bitmaps, "null unindexed filter_bitmaps");
+  if (current_comm() && current_comm()->nranks > 1)
+    fail(LB2_UNSUPPORTED, "a combined search on a row-sharded index is not implemented");
+  const int d = index->d;
+  flat_search_batch_check(d, index->dtype, index->metric, (int)std::max<uint32_t>(1, b.kmax));
+  if (nq == 0) {
+    sync_stream();
+    return LB2_OK;
+  }
+  const size_t nk = (size_t)nq * k_stride;
+  OutArg<uint64_t> oi(row_ids_out, nk);
+  OutArg<float> od(dists_out, nk);
+  OutArg<uint32_t> oc(counts_out, nq);
+  OutArg<uint32_t> onp(nprobes_out, nq);
+  DevBuf<uint64_t> ids(2 * nk);
+  DevBuf<float> dists(2 * nk);
+  DevBuf<uint32_t> cnts(2 * nq);
+  // the index's rows, refined so that their distances are exact (scanner.rs:2884-2905)
+  BatchSearch bs(index, queries, nq, ip.data(), filters, num_filters, late_width, b, onp.get());
+  {
+    TagScope tg("search");
+    InArg<uint8_t> v(refine_vectors, (size_t)num_vectors * d * dtype_size(index->dtype));
+    refine_batch_f32(bs.q.q.get(), nq, d, index->metric, v.get(), (int)index->dtype, num_vectors, bs.cdist.p,
+                     bs.cid.p, bs.ccnt.p, (int)b.kcmax, bs.qo.p, (int)k_stride, ids.p, dists.p, cnts.p);
+  }
+  // the unindexed rows: flat_knn with the index metric on the original query, each query with its own bitmap
+  // (scanner.rs:2993-3013)
+  const lb2_unindexed_rows& r = u->rows;
+  const size_t words = (size_t)((r.n + 63) / 64);
+  InArg<uint64_t> rid(r.row_ids, r.n), allow(r.allow_bitmap, r.allow_bitmap ? words : 0);
+  std::vector<InArg<uint64_t>> bm(num_filters);
+  std::vector<const uint64_t*> bm_dev(num_filters);
+  for (uint32_t f = 0; f < num_filters; ++f) {
+    bm[f].set(u->filter_bitmaps[f], u->filter_bitmaps[f] ? words : 0);
+    bm_dev[f] = bm[f].get();
+  }
+  const std::vector<FlatQuery> fq = flat_queries(params, nq, bm_dev, allow.get());
+  flat_search_batch(bs.q.q.get(), nq, d, index->metric, r.vectors, r.n, index->dtype, rid.get(), fq.data(),
+                    (int)k_stride, ids.p + nk, dists.p + nk, cnts.p + nq);
+  // the union by (_distance, _rowid), first k_q
+  std::vector<QueryParam> qp_h(nq);
+  for (uint64_t q = 0; q < nq; ++q) qp_h[q].k = (int)params[q].k;
+  DevBuf<QueryParam> qp(nq);
+  h2d(qp.p, qp_h.data(), nq);
+  {
+    TagScope tg("search");
+    merge_lists("merge_combined", nq, dists.p, ids.p, cnts.p, 2, (int)k_stride, nk, nk, (size_t)k_stride, nq, 1,
+                oi.get(), od.get(), oc.get(), 2, qp.p);
+  }
+  oi.commit(); od.commit(); oc.commit(); onp.commit();
+  sync_stream();
+  LB2_API_END
+}
+
 // RAII: route the thread's work to the caller's stream for one asynchronous call
 namespace {
 struct AsyncScope {
