@@ -20,7 +20,10 @@
  *   - Calls are blocking (results are complete on return).  All entry points are thread-safe;
  *     each calling thread uses the CUDA device selected by lb2_set_device() on that thread and its
  *     own CUDA stream, so concurrent callers (the reference searches up to ncpu-2 partitions at a
- *     time, rust/lance/src/io/exec/knn.rs:881) overlap on the device.
+ *     time, rust/lance/src/io/exec/knn.rs:881) overlap on the device.  Calls that only read a handle
+ *     (searches, transform, export, optimize / split / join into a new handle) may share it across
+ *     threads; a call that changes or frees a handle (lb2_index_set_partition_index, the _load* calls,
+ *     lb2_index_destroy, lb2_partition_index_destroy) needs exclusive access to it.
  *   - Stream variants: lb2_set_stream() orders every later call of the thread on a caller-owned
  *     cudaStream_t; lb2_index_search_async() enqueues a whole search and returns without waiting.
  */

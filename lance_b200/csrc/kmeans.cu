@@ -148,17 +148,26 @@ class SplitWorkers {
     return *w;
   }
   int threads() const { return nthreads_; }
-  void submit(std::function<void()> f) {
+  // The pool is shared by every thread that trains at once, so each caller counts only its own tasks: a wave waits
+  // for its tasks, not for a queue that another training keeps filling.
+  struct Wave {
+    int pending = 0;
+  };
+  void submit(Wave& w, std::function<void()> f) {
     {
       std::lock_guard<std::mutex> lk(m_);
-      q_.push_back(std::move(f));
-      ++pending_;
+      ++w.pending;
+      q_.push_back([this, &w, f = std::move(f)] {
+        f();
+        std::lock_guard<std::mutex> lk(m_);
+        if (--w.pending == 0) done_.notify_all();
+      });
     }
     cv_.notify_one();
   }
-  void wait() {
+  void wait(Wave& w) {
     std::unique_lock<std::mutex> lk(m_);
-    done_.wait(lk, [&] { return pending_ == 0; });
+    done_.wait(lk, [&] { return w.pending == 0; });
   }
 
  private:
@@ -177,17 +186,12 @@ class SplitWorkers {
         q_.pop_front();
       }
       f();
-      {
-        std::lock_guard<std::mutex> lk(m_);
-        if (--pending_ == 0) done_.notify_all();
-      }
     }
   }
   int nthreads_ = 0;
   std::mutex m_;
   std::condition_variable cv_, done_;
   std::deque<std::function<void()>> q_;
-  int pending_ = 0;
 };
 }  // namespace
 
@@ -297,11 +301,12 @@ void hierarchical_train(const float* x, uint64_t n, int d, int K, const LloydPar
       sync_stream();  // the row lists written by earlier commits are visible to the workers' streams
       const bool prof_on = me.profiling;
       const std::string tag = me.tag;
+      SplitWorkers::Wave tasks;
       for (size_t w = 1; w < wave.size(); ++w) {
         SplitOut* o = outs[w].get();
         const HCluster c = wave[w];
         const int cck = wck[w];
-        workers->submit([=, &idx]() {
+        workers->submit(tasks, [=, &idx]() {
           try {
             lb2_set_device(device);
             Ctx& wc = ctx();
@@ -324,7 +329,7 @@ void hierarchical_train(const float* x, uint64_t n, int d, int K, const LloydPar
       } catch (...) {
         outs[0]->err = std::current_exception();
       }
-      if (wave.size() > 1) workers->wait();
+      if (wave.size() > 1) workers->wait(tasks);
       for (size_t w = 0; w < wave.size(); ++w) {
         if (outs[w]->err) std::rethrow_exception(outs[w]->err);
         me.launches += outs[w]->launches;

@@ -625,15 +625,17 @@ __global__ void forward_overflow_kernel(const uint32_t* __restrict__ list, const
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
+// Shared by every host thread: the first calls of the tensor-core filter may come from several threads at once, so
+// the pointer is a function-local static initialised once (C++ makes that thread-safe).  A failed lookup throws out
+// of the initialiser, which leaves the static uninitialised and lets the next call try again.
 static PFN_cuTensorMapEncodeTiled_v12000 get_encode_fn() {
-  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
-  if (!fn) {
+  static const PFN_cuTensorMapEncodeTiled_v12000 fn = [] {
     cudaDriverEntryPointQueryResult qres;
     void* p = nullptr;
     LB2_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres));
     if (!p || qres != cudaDriverEntryPointSuccess) fail(LB2_CUDA_ERROR, "cuTensorMapEncodeTiled not available");
-    fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(p);
-  }
+    return reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(p);
+  }();
   return fn;
 }
 
